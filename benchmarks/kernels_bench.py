@@ -210,6 +210,46 @@ def main():
     group_by_total([small], [(a, "first"), (a, "last")], "group-by i8 key, first/last f64")
     i32.free()
     small.free()
+
+    # ---- equi-join: build-side sort, gathers of its keys, heads + compactions, count (binary search), scan, emit, the takes ----
+    def join_total(lk, rk, how, what, payload=None):
+        def once():
+            li, ri = rdf.join_indices(lk, rk, how)
+            out = [li, ri]
+            if payload is not None:   # DataFrame::join then takes the columns of both sides
+                out += [payload[0].take(li), payload[1].take(ri)]
+            return out
+        res = timed(ctx, once, reps=3)
+        total = sum(v[0] for v in res.values())
+        print(f"{what:44s} {total:8.4f} ms  (" + ", ".join(f"{k} {v[0]:.3f}" for k, v in sorted(res.items())) + ")", flush=True)
+        rows_out.append({"case": what, "config": "join", "kernel": "sort + take + filter + join", "ms": total, "rows": args.rows,
+                         "parts": {k: v[0] for k, v in res.items()}})
+
+    def keys(dtype, n_rows, hi, col_id):   # integer keys uniform in [0, hi)
+        n_lens = [chunk] * (n_rows // chunk) if n_rows >= chunk else [n_rows]
+        f = G(rdf.F64, n_lens, 0, 0.0, float(hi), col_id=col_id)
+        k = f.cast(dtype)
+        f.free()
+        return k
+
+    P = rdf.PrimitiveArray
+    dim = rdf.Column.upload([P.from_numpy(np.random.default_rng(1).permutation(1_000_000).astype(np.int32))])   # unique keys
+    dim_val = G(rdf.F64, [1_000_000], 0, -1.0, 1.0, col_id=40)
+    fact = keys(rdf.I32, args.rows, 1_000_000, 41)
+    join_total([fact], [dim], "left", f"left join {args.rows:.0e} x 1e6 unique i32 keys + takes", (a, dim_val))
+    fact.free()
+    l64, r64 = keys(rdf.I64, 10_000_000, 1_000_000, 42), keys(rdf.I64, 10_000_000, 1_000_000, 43)
+    join_total([l64], [r64], "inner", "inner join 1e7 x 1e7 i64, ~10 matches per row")
+    l64.free(); r64.free()
+    la, lb = keys(rdf.I32, 10_000_000, 1000, 44), keys(rdf.I8, 10_000_000, 100, 45)
+    ra, rb = keys(rdf.I32, 1_000_000, 1000, 46), keys(rdf.I8, 1_000_000, 100, 47)
+    join_total([la, lb], [ra, rb], "inner", "inner join 1e7 x 1e6 on (i32, i8), ~10 matches")
+    for col in (la, lb, ra, rb, dim, dim_val):
+        col.free()
+    hot_l = rdf.Column.upload([P.from_numpy(np.zeros(100_000, np.int64))])
+    hot_r = rdf.Column.upload([P.from_numpy(np.zeros(1_000, np.int64))])
+    join_total([hot_l], [hot_r], "inner", "hot key: 1e5 x 1e3 rows of one key (1e8 out)")
+    hot_l.free(); hot_r.free()
     if args.json:
         with open(args.json, "w") as f:
             json.dump({"rows": args.rows, "peak_GBs": pk, "peak_source": pk_src, "results": rows_out}, f, indent=1)

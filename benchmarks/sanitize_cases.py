@@ -68,6 +68,13 @@ for dtype in (rdf.I8, rdf.I16, rdf.I32, rdf.I64, rdf.U8, rdf.U16, rdf.U32, rdf.U
     keys, res = rdf.group_by([k2, k1], [(v, f) for f in fns])
     for c in keys + res:
         c.download()
+    # equi-join: every join type (count, scan, emit; full: the unmatched rows), two criteria over ragged, sliced chunks
+    jl, jr = col(True), col(False)[2:]
+    lk2 = rdf.Column.upload([P.from_numpy(rng.integers(0, 3, sum(c.length for c in jl)).astype(np.int16))])
+    rk2 = rdf.Column.upload([P.from_numpy(rng.integers(0, 3, sum(c.length for c in jr)).astype(np.int16), rng.random(sum(c.length for c in jr)) > 0.1)])
+    for how in rdf.native.JOIN_TYPES:
+        li, ri = rdf.join_indices([rdf.Column.upload(jl), lk2], [rdf.Column.upload(jr), rk2], how)
+        li.download(); ri.download()
 # round 2: the fleet code path on one GPU, and a single-rank communicator (pack -> combine -> unpack on the stream)
 fleet = rdf.Context.multi(1)
 fa = [P.from_numpy(rng.integers(-100, 100, n).astype(np.int64), rng.random(n) > 0.3) for n in (1000, 0, 77)]

@@ -317,6 +317,35 @@ typedef struct { const bdf_col* column; int32_t function; } bdf_group_agg;
 int  bdf_group_by_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_col* const* keys, int32_t n_aggs, const bdf_group_agg* aggs,
                       bdf_col** out_keys /* n_keys */, bdf_col** out /* n_aggs */, int64_t* n_groups);
 
+/* ---- equi-join (Transformation::Join -> DataFrame::join, src/dataframe.rs:626-719; the body of calc_equijoin_indices,
+ * src/functions/join.rs:19-137) ------------------------------------------------------------------------------------------------
+ * Criterion k is the pair (left_keys[k], right_keys[k]), 1..16 of them, numeric.  The result is two UInt32 columns of n_rows rows,
+ * one chunk each: row numbers that count through the chunks of each side, NULL = no partner.  They feed bdf_take_dev directly, the
+ * way DataFrame::join feeds Column::take.
+ * Match.  A left row and a right row match when, for every criterion, both slots are valid and their values are equal.  Equality is
+ *   the key equality of sort and group-by: all NaNs are equal, -0.0 == 0.0.  A row with a null in any criterion matches nothing.
+ * Order (fixed, so the result is deterministic):
+ *   INNER, LEFT  left rows in row order; each left row's matches in ascending right row order.  LEFT: a left row without a match
+ *                appears once, in its place, with a NULL right index (null-key rows count as having no match).
+ *   RIGHT        exactly LEFT with the sides swapped, and the two output columns swapped back: right rows in row order.
+ *   FULL         the LEFT output, then every right row no left row matched, in right row order, with a NULL left index.
+ * Departures from the reference, on purpose:
+ *   1. pair order: as above, instead of HashMap iteration order;
+ *   2. null keys: the reference hashes a null-key row under its truncated key bytes, so null rows can match each other, and also
+ *      appends the row again as unmatched (a LEFT join can list it twice); here a null-key row never matches and appears once;
+ *   3. FULL: the reference's FullJoin arm (join.rs:109-133) emits only the matched pairs and the null-key rows, dropping every
+ *      unmatched row whose key is valid; here FULL is the SQL full outer join;
+ *   4. float keys: the reference compares raw bytes (-0.0 != 0.0); here floats follow the key equality above (Postgres's too);
+ *   5. zero criteria: in the reference every row then matches every row (a cross join); here it is refused.
+ * Errors (nothing is returned and nothing leaks): n_keys outside 1..16 ("Join criteria cannot be empty" for 0) or a null pointer
+ *   -> BDF_INVALID; an unknown join type or a non-numeric key -> BDF_UNSUPPORTED; a criterion whose two columns have different
+ *   dtypes -> BDF_UNSUPPORTED "Join columns must have compatible types" (the text of try_join); key columns of one side with
+ *   different lengths -> BDF_LENGTH_MISMATCH; a side of more than 2^32-1 rows -> the sort's BDF_UNSUPPORTED; a multi-GPU context
+ *   -> BDF_UNSUPPORTED (as sort / take / filter / group-by); an output that does not fit in device memory -> BDF_OOM. */
+typedef enum { BDF_JOIN_LEFT = 0, BDF_JOIN_RIGHT, BDF_JOIN_INNER, BDF_JOIN_FULL } bdf_join_type;   /* JoinType order */
+int  bdf_join_indices_dev(bdf_ctx* ctx, int32_t join_type, int32_t n_keys, const bdf_col* const* left_keys, const bdf_col* const* right_keys,
+                          bdf_col** left_indices, bdf_col** right_indices, int64_t* n_rows);
+
 /* ---- N4: Arrow IPC files either side of the path ---------------------------------------------------------------
  * DataFrame::from_arrow (src/dataframe.rs:391-407: arrow::ipc::reader::FileReader, every RecordBatch -> one chunk per
  * column) and DataFrame::to_arrow (:515-525: arrow::ipc::writer::FileWriter).  The file is mapped and its footer, schema
@@ -353,7 +382,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

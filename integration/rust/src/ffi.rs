@@ -113,6 +113,10 @@ extern "C" {
     // group-by over 1..16 key columns with a flat list of (column, function) pairs; every returned column is the caller's to free
     pub fn bdf_group_by_dev(ctx: *mut BdfCtx, n_keys: i32, keys: *const *const BdfCol, n_aggs: i32, aggs: *const BdfGroupAgg,
                             out_keys: *mut *mut BdfCol, out: *mut *mut BdfCol, n_groups: *mut i64) -> c_int;
+    // equi-join (calc_equijoin_indices): join_type in JoinType order (LeftJoin, RightJoin, InnerJoin, FullJoin); two UInt32 index
+    // columns, NULL = no partner, to take every column of each side with
+    pub fn bdf_join_indices_dev(ctx: *mut BdfCtx, join_type: i32, n_keys: i32, left_keys: *const *const BdfCol, right_keys: *const *const BdfCol,
+                                left_indices: *mut *mut BdfCol, right_indices: *mut *mut BdfCol, n_rows: *mut i64) -> c_int;
     // Arrow IPC files (DataFrame::from_arrow / to_arrow)
     pub fn bdf_ipc_open(path: *const c_char, out: *mut *mut BdfIpc) -> c_int;
     pub fn bdf_ipc_close(file: *mut BdfIpc);

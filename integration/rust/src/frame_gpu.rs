@@ -165,6 +165,28 @@ pub fn group_by_device(frame: &DeviceColumns, keys: &[usize], aggr: &[(usize, Gr
     Ok(res)
 }
 
+/// `DataFrame::join` (src/dataframe.rs:626-719) with the body of `calc_equijoin_indices` as one call.  `criteria`: (left column,
+/// right column) pairs; `join_type`: JoinType's discriminant (Left, Right, Inner, Full -- bdf_join_type).  Output = every column of
+/// `left`, then every column of `right`, taken by the index pairs (NULL index -> NULL slot); a name present on both sides becomes
+/// `a.<name>` / `b.<name>`, the schema `Dataset::try_join` plans.  Pair order and the departures from the reference: include/b200df.h.
+pub fn join_device(left: &DeviceColumns, right: &DeviceColumns, criteria: &[(usize, usize)], join_type: i32) -> Result<DeviceColumns, String> {
+    let lk: Vec<*const BdfCol> = criteria.iter().map(|(l, _)| left.cols[*l] as *const BdfCol).collect();
+    let rk: Vec<*const BdfCol> = criteria.iter().map(|(_, r)| right.cols[*r] as *const BdfCol).collect();
+    let (mut li, mut ri, mut n_rows) = (std::ptr::null_mut(), std::ptr::null_mut(), 0i64);
+    check(unsafe { bdf_join_indices_dev(dev(), join_type, lk.len() as i32, lk.as_ptr(), rk.as_ptr(), &mut li, &mut ri, &mut n_rows) })?;
+    let idx = DeviceColumns { names: vec![], cols: vec![li, ri] };   // freed when this function returns, early or not
+    let mut out = DeviceColumns { names: vec![], cols: vec![] };
+    for (side, other, prefix, indices) in [(left, right, "a", idx.cols[0]), (right, left, "b", idx.cols[1])] {
+        for (name, col) in side.names.iter().zip(&side.cols) {
+            let mut taken: *mut BdfCol = std::ptr::null_mut();
+            check(unsafe { bdf_take_dev(dev(), *col, indices, &mut taken) })?;
+            out.names.push(if other.names.contains(name) { format!("{}.{}", prefix, name) } else { name.clone() });
+            out.cols.push(taken);
+        }
+    }
+    Ok(out)
+}
+
 /// A run of Float64 Calculations whose intermediates are not kept (config 2: h = sin(((a+b)*c)/d)) as one pass.
 /// `inputs` are column indices; node k writes slot inputs.len() + k (see include/b200df.h, bdf_eval_expr_dev).
 pub fn fused_chain(frame: &DeviceColumns, inputs: &[usize], nodes: &[BdfExprNode]) -> Result<*mut BdfCol, String> {

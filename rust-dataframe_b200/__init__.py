@@ -13,11 +13,11 @@ from .arrays import (BooleanArray, DTYPE_NAMES, F32, F64, I8, I16, I32, I64, NP_
                      width_of)
 from .ipc import IpcFile, write_ipc, write_ipc_host
 from . import frame
-from .frame import DeviceFrame, plan_aggregate, plan_fusion
-from .functions import AggFuture, AggregateFunctions, Column, ScalarFunctions, cast, eval_expr, eval_expr_agg, group_aggregate, group_by, sort_columns, sort_indices
+from .frame import DeviceFrame, plan_aggregate, plan_fusion, plan_join
+from .functions import AggFuture, AggregateFunctions, Column, ScalarFunctions, cast, eval_expr, eval_expr_agg, group_aggregate, group_by, join_indices, sort_columns, sort_indices
 
 __all__ = [
     "native", "ArrowError", "ComputeError", "Context", "DivideByZero", "ReferencePanic", "UnsupportedType",
-    "default_context", "PrimitiveArray", "BooleanArray", "ScalarFunctions", "AggregateFunctions", "Column", "AggFuture", "cast", "eval_expr", "eval_expr_agg", "group_aggregate", "group_by", "sort_indices", "sort_columns", "IpcFile", "write_ipc", "write_ipc_host", "frame", "DeviceFrame", "plan_aggregate", "plan_fusion",
+    "default_context", "PrimitiveArray", "BooleanArray", "ScalarFunctions", "AggregateFunctions", "Column", "AggFuture", "cast", "eval_expr", "eval_expr_agg", "group_aggregate", "group_by", "join_indices", "sort_indices", "sort_columns", "IpcFile", "write_ipc", "write_ipc_host", "frame", "DeviceFrame", "plan_aggregate", "plan_fusion", "plan_join",
     "I8", "I16", "I32", "I64", "U8", "U16", "U32", "U64", "F32", "F64", "NP_DTYPES", "DTYPE_NAMES", "dtype_of", "width_of",
 ]

@@ -20,8 +20,8 @@ ADD, SUB, MUL, DIV, ATAN2, HYPOT, LOG = range(7)
 SUM, MIN, MAX, COUNT = range(4)
 OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID = range(9)
 ASYNC = 1
-K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP = range(12)
-KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group"]
+K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN = range(13)
+KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -30,6 +30,9 @@ BOOL = 10
 GROUP_SUM, GROUP_MAX, GROUP_MIN, GROUP_AVG, GROUP_COUNT, GROUP_COUNT_DISTINCT, GROUP_FIRST, GROUP_LAST = range(8)
 GROUP_FNS = {"sum": GROUP_SUM, "max": GROUP_MAX, "min": GROUP_MIN, "avg": GROUP_AVG, "count": GROUP_COUNT,
              "count_distinct": GROUP_COUNT_DISTINCT, "first": GROUP_FIRST, "last": GROUP_LAST}
+# bdf_join_type (JoinType order)
+JOIN_LEFT, JOIN_RIGHT, JOIN_INNER, JOIN_FULL = range(4)
+JOIN_TYPES = {"left": JOIN_LEFT, "right": JOIN_RIGHT, "inner": JOIN_INNER, "full": JOIN_FULL}
 
 
 class View(C.Structure):
@@ -153,6 +156,7 @@ def lib() -> C.CDLL:
         "bdf_take_dev": ([vp, vp, vp, P(vp)], C.c_int),
         "bdf_group_aggregate_dev": ([vp, vp, i32, P(vp), P(vp), P(GroupOut), P(i64)], C.c_int),
         "bdf_group_by_dev": ([vp, i32, P(vp), i32, P(GroupAggC), P(vp), P(vp), P(i64)], C.c_int),
+        "bdf_join_indices_dev": ([vp, i32, i32, P(vp), P(vp), P(vp), P(vp), P(i64)], C.c_int),
         "bdf_compare_dev": ([vp, C.c_int, vp, vp, C.c_double, P(vp)], C.c_int),
         "bdf_boolean_dev": ([vp, C.c_int, vp, vp, P(vp)], C.c_int),
         "bdf_filter_dev": ([vp, vp, vp, P(vp)], C.c_int),
@@ -200,7 +204,7 @@ EXPORTED_SYMBOLS = [
     "bdf_host_alloc", "bdf_host_free", "bdf_host_register", "bdf_host_unregister", "bdf_binary", "bdf_unary", "bdf_cast",
     "bdf_aggregate", "bdf_aggregate_all", "bdf_avg", "bdf_upload", "bdf_upload_many", "bdf_col_wait", "bdf_col_describe",
     "bdf_col_chunk_info", "bdf_binary_dev", "bdf_unary_dev", "bdf_cast_dev", "bdf_aggregate_dev",
-    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
+    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_join_indices_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
     "bdf_binary_agg_dev", "bdf_binary_agg_dev_async", "bdf_aggregate_all_dev_async", "bdf_future_wait", "bdf_col_free", "bdf_profile_enable", "bdf_profile_read",
     "bdf_launch_count", "bdf_timer_start", "bdf_timer_stop", "bdf_flush_l2", "bdf_generate",
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",

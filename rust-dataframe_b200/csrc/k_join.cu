@@ -1,0 +1,268 @@
+// k_join.cu -- equi-join indices (Transformation::Join -> DataFrame::join, src/dataframe.rs:626-719 -> calc_equijoin_indices,
+// src/functions/join.rs:19-137), sort-based.
+//
+// The host (runtime.cu join_dev) sorts the build side's keys with the stable radix lexsort of k_sort.cu, gathers them, and
+// compacts the distinct key tuples and the first sorted row of every run with the head kernel and stream compaction of the
+// group-by.  The kernels here:
+//   k_join_count        one thread per probe row, reading the probe side's chunks in place: a binary search of the distinct
+//                       build tuples in the sort's total order (sort_keys.cuh: the very key transform the sort used, null last)
+//                       gives the run of equal build rows; writes the run's first sorted row and the row's output count
+//                       (outer joins: at least 1), marks the run as hit (full join), and the CTA's total.
+//   k_join_scan_blocks  one CTA: exclusive scan of the CTA totals; the grand total lands behind the last row's count.
+//   k_join_scan_rows    the counts of every CTA become 64-bit exclusive output offsets.
+//   k_join_emit         load-balanced by OUTPUT position: every CTA owns kJoinTile output rows, finds the probe rows that produce
+//                       them with a binary search of the offsets, and writes (probe row, perm[run start + j]) and both validity
+//                       bitmaps as whole words.  A hot key with 10^5 x 10^3 partners is spread over the whole GPU.  Rows past
+//                       the probe part are the unmatched build rows a full join appends (null probe index).
+//   k_join_unmatched    full join: every sorted build row of a run nobody hit sets its ORIGINAL row's bit in a mask; the mask
+//                       then compacts an iota (k_filter.cu), which lists the unmatched rows in ascending row order.
+#include "sort_keys.cuh"
+
+#include <algorithm>
+
+namespace bdf {
+
+constexpr int kMaxJoinKeys = 16;
+constexpr int kJoinItems = 8;
+constexpr int kJoinTile = kThreads * kJoinItems;   // rows per CTA of the count, scan and emit kernels
+constexpr uint32_t kNoMatch = 0xffffffffu;         // match start of a probe row without partners (build rows are < 2^32 - 1)
+
+struct JoinKey {
+    const SortChunk* probe;        // chunk table of the probe column (the concatenated row space)
+    const void* build;             // the distinct build keys of this criterion, in sort order (one chunk)
+    const uint32_t* build_valid;   // its validity (bit offset 0), or null
+    int n_chunks;
+    int dtype;
+};
+struct JoinKeys { JoinKey k[kMaxJoinKeys]; int n; };
+
+// Build run r against the probe tuple (every probe key valid): <0, 0, >0 as run r sorts before, equal to, after the probe.
+__device__ __forceinline__ int join_cmp_run(const JoinKeys& keys, const unsigned long long (&pk)[kMaxJoinKeys], long long r) {
+#pragma unroll
+    for (int k = 0; k < kMaxJoinKeys; k++) {
+        if (k >= keys.n) break;
+        const JoinKey& K = keys.k[k];
+        if (K.build_valid && !((__ldg(K.build_valid + (r >> 5)) >> (r & 31)) & 1u)) return 1;   // null sorts after every value
+        const unsigned long long b = sort_key_at(K.dtype, K.build, r);
+        if (b != pk[k]) return b < pk[k] ? -1 : 1;
+    }
+    return 0;
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_join_count(const __grid_constant__ JoinKeys keys, long long n_probe, const uint32_t* __restrict__ run_starts, long long n_runs, long long n_build,
+             int outer, unsigned long long* __restrict__ counts, uint32_t* __restrict__ match_start, unsigned char* __restrict__ hit,
+             unsigned long long* __restrict__ block_sums) {
+    __shared__ unsigned long long s_warp[kWarpsPerCta];
+    unsigned long long total = 0;
+    for (int it = 0; it < kJoinItems; it++) {
+        const long long i = (long long)blockIdx.x * kJoinTile + it * kThreads + threadIdx.x;
+        if (i >= n_probe) break;
+        unsigned long long pk[kMaxJoinKeys];
+        bool valid = true;
+#pragma unroll
+        for (int k = 0; k < kMaxJoinKeys; k++) {
+            pk[k] = 0;
+            if (k < keys.n && valid) {
+                const JoinKey& K = keys.k[k];
+                const SortChunk ch = K.probe[K.n_chunks == 1 ? 0 : chunk_of(K.probe, K.n_chunks, i)];
+                const long long local = i - ch.start;
+                valid = ch.validity ? chunk_bit(ch.validity, ch.bit_off + local) : true;
+                if (valid) pk[k] = sort_key_at(K.dtype, ch.values, local);
+            }
+        }
+        unsigned long long cnt = 0;
+        uint32_t start = kNoMatch;
+        if (valid && n_runs > 0) {   // a null in any criterion matches nothing
+            long long lo = 0, hi = n_runs;
+            while (lo < hi) {
+                const long long mid = (lo + hi) >> 1;
+                if (join_cmp_run(keys, pk, mid) < 0) lo = mid + 1;
+                else hi = mid;
+            }
+            if (lo < n_runs && join_cmp_run(keys, pk, lo) == 0) {
+                start = run_starts[lo];
+                cnt = (unsigned long long)((lo + 1 < n_runs ? (long long)run_starts[lo + 1] : n_build) - (long long)start);
+                if (hit) hit[lo] = 1;
+            }
+        }
+        if (outer && cnt == 0) cnt = 1;
+        counts[i] = cnt;
+        match_start[i] = start;
+        total += cnt;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = total;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long t = 0;
+#pragma unroll
+        for (int w = 0; w < kWarpsPerCta; w++) t += s_warp[w];
+        block_sums[blockIdx.x] = t;
+    }
+}
+
+// Exclusive scan of the CTA totals in place (one CTA of 1024 threads, each owning a contiguous run); *total = the sum.
+__global__ void __launch_bounds__(1024) k_join_scan_blocks(unsigned long long* __restrict__ data, long long count, unsigned long long* __restrict__ total) {
+    __shared__ unsigned long long s_warp[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long per = (count + 1023) / 1024;
+    const long long begin = min(count, (long long)threadIdx.x * per), end = min(count, begin + per);
+    unsigned long long sum = 0;
+    for (long long i = begin; i < end; i++) sum += data[i];
+    unsigned long long x = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        unsigned long long w = s_warp[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
+        s_warp[lane] = w;   // inclusive over warps
+    }
+    __syncthreads();
+    unsigned long long run = (warp ? s_warp[warp - 1] : 0ull) + x - sum;
+    for (long long i = begin; i < end; i++) { const unsigned long long v = data[i]; data[i] = run; run += v; }
+    if (threadIdx.x == 1023) *total = run;
+}
+
+// The counts of CTA b (rows [b * kJoinTile, ...), thread t owning kJoinItems consecutive rows) -> exclusive offsets.
+__global__ void __launch_bounds__(kThreads)
+k_join_scan_rows(unsigned long long* __restrict__ counts, long long n, const unsigned long long* __restrict__ block_offsets) {
+    __shared__ unsigned long long s_warp[kWarpsPerCta];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long base = (long long)blockIdx.x * kJoinTile + (long long)threadIdx.x * kJoinItems;
+    unsigned long long v[kJoinItems], sum = 0;
+#pragma unroll
+    for (int k = 0; k < kJoinItems; k++) { v[k] = base + k < n ? counts[base + k] : 0ull; sum += v[k]; }
+    unsigned long long x = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    unsigned long long run = block_offsets[blockIdx.x] + x - sum;
+#pragma unroll
+    for (int w = 0; w < kWarpsPerCta; w++) run += w < warp ? s_warp[w] : 0ull;
+#pragma unroll
+    for (int k = 0; k < kJoinItems; k++) {
+        if (base + k < n) counts[base + k] = run;
+        run += v[k];
+    }
+}
+
+// The last probe row i in [lo, hi] with offs[i] <= o (offs is non-decreasing; probe rows of an inner join may produce nothing).
+__device__ __forceinline__ long long join_row_of(const unsigned long long* __restrict__ offs, long long lo, long long hi, unsigned long long o) {
+    while (lo < hi) {
+        const long long mid = (lo + hi + 1) >> 1;
+        if (offs[mid] <= o) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_join_emit(const unsigned long long* __restrict__ offs, long long n_probe, const uint32_t* __restrict__ match_start, const uint32_t* __restrict__ perm,
+            unsigned long long probe_rows, const uint32_t* __restrict__ unmatched, unsigned long long n_out, uint32_t* __restrict__ probe_out,
+            uint32_t* __restrict__ probe_valid, uint32_t* __restrict__ build_out, uint32_t* __restrict__ build_valid) {
+    __shared__ long long s_range[2];
+    const unsigned long long o0 = (unsigned long long)blockIdx.x * kJoinTile;
+    if (threadIdx.x < 2) {   // the probe rows behind this CTA's first and last output row of the probe part
+        long long r = 0;
+        if (o0 < probe_rows) {
+            const unsigned long long o = threadIdx.x == 0 ? o0 : min(o0 + kJoinTile, probe_rows) - 1;
+            r = join_row_of(offs, 0, n_probe - 1, o);
+        }
+        s_range[threadIdx.x] = r;
+    }
+    __syncthreads();
+    const long long lo = s_range[0], hi = s_range[1];
+    for (int it = 0; it < kJoinItems; it++) {
+        const unsigned long long o = o0 + (unsigned long long)(it * kThreads + threadIdx.x);
+        bool pv = false, bv = false;
+        uint32_t p = 0, b = 0;
+        if (o < probe_rows) {
+            const long long i = join_row_of(offs, lo, hi, o);
+            p = (uint32_t)i;
+            pv = true;
+            const uint32_t s = match_start[i];
+            if (s != kNoMatch) { b = __ldg(perm + (unsigned long long)s + (o - offs[i])); bv = true; }
+        } else if (o < n_out) {
+            b = unmatched[o - probe_rows];
+            bv = true;
+        }
+        if (o < n_out) { probe_out[o] = p; build_out[o] = b; }
+        const unsigned pw = __ballot_sync(0xffffffffu, pv), bw = __ballot_sync(0xffffffffu, bv);
+        if ((threadIdx.x & 31) == 0 && o < n_out) {
+            if (probe_valid) probe_valid[o >> 5] = pw;
+            if (build_valid) build_valid[o >> 5] = bw;
+        }
+    }
+}
+
+// Sorted build row s belongs to the last run whose start is <= s; an unhit run's rows are unmatched: bit perm[s] of the mask.
+__global__ void __launch_bounds__(kThreads)
+k_join_unmatched(const uint32_t* __restrict__ perm, long long n_build, const uint32_t* __restrict__ run_starts, long long n_runs,
+                 const unsigned char* __restrict__ hit, uint32_t* __restrict__ mask) {
+    for (long long s = (long long)blockIdx.x * kThreads + threadIdx.x; s < n_build; s += (long long)gridDim.x * kThreads) {
+        long long lo = 0, hi = n_runs - 1;
+        while (lo < hi) {
+            const long long mid = (lo + hi + 1) >> 1;
+            if ((long long)run_starts[mid] <= s) lo = mid; else hi = mid - 1;
+        }
+        if (!hit[lo]) {
+            const uint32_t r = perm[s];
+            atomicOr(mask + (r >> 5), 1u << (r & 31));
+        }
+    }
+}
+
+// ---- launchers ------------------------------------------------------------------------------------------------------
+int join_tile_rows() { return kJoinTile; }
+
+// Criterion k: dtype, the probe column's chunk table (sort_table) and chunk count, the distinct build keys and their validity.
+cudaError_t launch_join_count(int n_keys, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,
+                              const uint32_t* const* build_valid, long long n_probe, const uint32_t* run_starts, long long n_runs, long long n_build,
+                              int outer, unsigned long long* counts, uint32_t* match_start, unsigned char* hit, unsigned long long* block_sums,
+                              cudaStream_t s) {
+    if (n_probe <= 0) return cudaSuccess;
+    if (n_keys < 1 || n_keys > kMaxJoinKeys) return cudaErrorInvalidValue;
+    JoinKeys jk{};
+    for (int k = 0; k < n_keys; k++)
+        jk.k[k] = JoinKey{(const SortChunk*)probe_tables[k], build_keys[k], build_valid[k], probe_chunks[k], dtypes[k]};
+    jk.n = n_keys;
+    const long long blocks = (n_probe + kJoinTile - 1) / kJoinTile;
+    k_join_count<<<(unsigned)blocks, kThreads, 0, s>>>(jk, n_probe, run_starts, n_runs, n_build, outer, counts, match_start, hit, block_sums);
+    return cudaGetLastError();
+}
+
+// counts: n_probe + 1 entries; afterwards counts[i] = the first output row of probe row i, counts[n_probe] = the total.
+cudaError_t launch_join_scan(unsigned long long* counts, long long n_probe, unsigned long long* block_sums, cudaStream_t s) {
+    if (n_probe <= 0) return cudaMemsetAsync(counts, 0, sizeof(unsigned long long), s);
+    const long long blocks = (n_probe + kJoinTile - 1) / kJoinTile;
+    k_join_scan_blocks<<<1, 1024, 0, s>>>(block_sums, blocks, counts + n_probe);
+    k_join_scan_rows<<<(unsigned)blocks, kThreads, 0, s>>>(counts, n_probe, block_sums);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_join_emit(const unsigned long long* offs, long long n_probe, const uint32_t* match_start, const uint32_t* perm, unsigned long long probe_rows,
+                             const uint32_t* unmatched, unsigned long long n_out, uint32_t* probe_out, uint32_t* probe_valid, uint32_t* build_out,
+                             uint32_t* build_valid, cudaStream_t s) {
+    if (n_out == 0) return cudaSuccess;
+    const unsigned long long blocks = (n_out + kJoinTile - 1) / kJoinTile;
+    if (blocks > 0x7fffffffull) return cudaErrorInvalidConfiguration;
+    k_join_emit<<<(unsigned)blocks, kThreads, 0, s>>>(offs, n_probe, match_start, perm, probe_rows, unmatched, n_out, probe_out, probe_valid, build_out,
+                                                      build_valid);
+    return cudaGetLastError();
+}
+
+// mask: ceil(n_build / 32) zeroed words.
+cudaError_t launch_join_unmatched(const uint32_t* perm, long long n_build, const uint32_t* run_starts, long long n_runs, const unsigned char* hit,
+                                  uint32_t* mask, int sm_count, cudaStream_t s) {
+    if (n_build <= 0) return cudaSuccess;
+    const long long want = (n_build + kThreads - 1) / kThreads;
+    k_join_unmatched<<<(unsigned)std::min<long long>(want, (long long)sm_count * 8), kThreads, 0, s>>>(perm, n_build, run_starts, n_runs, hit, mask);
+    return cudaGetLastError();
+}
+
+}  // namespace bdf

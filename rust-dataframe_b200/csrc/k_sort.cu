@@ -16,7 +16,7 @@
 // k_sort_keys also folds the OR and the AND of the keys it builds.
 // HBM traffic per executed pass: 8 (hist) + 12 + 12 B/row with 64-bit keys, 4 + 8 + 8 with 32-bit keys (criteria of at most
 // 4 bytes); a Float64/Int64 criterion = 8 value passes (+1 if nullable), Int32/Float32 = 4 (+1).
-#include "common.cuh"
+#include "sort_keys.cuh"
 
 #include <algorithm>
 
@@ -27,60 +27,6 @@ constexpr int kSortThreads = 512;                      // scatter CTA: 16 warps
 constexpr int kSortWarps = kSortThreads / 32;
 constexpr int kSortTile = kSortThreads * kSortItems;   // 4096 keys per tile: a digit's run in a tile averages 16 keys (128 B of keys,
                                                        // 64 B of indices) on a uniformly distributed byte; 2048-key tiles were slower
-
-template <typename To, typename From> __device__ __forceinline__ To bit_cast_to(From f) {
-    static_assert(sizeof(To) == sizeof(From), "bit_cast_to: sizes differ");
-    To t;
-    memcpy(&t, &f, sizeof(To));
-    return t;
-}
-
-struct SortChunk {          // one chunk of a column in the concatenated row space
-    const void* values;
-    const uint32_t* validity;
-    int64_t start;          // first global row of the chunk
-    int32_t bit_off;        // residual bit offset of the validity bitmap
-    int32_t val_bit_off;    // boolean columns: residual bit offset of the values bitmap
-};
-
-__device__ __forceinline__ int chunk_of(const SortChunk* __restrict__ t, int n, int64_t row) {
-    int lo = 0, hi = n - 1;
-    while (lo < hi) {   // last chunk whose start <= row (empty chunks share their start with the next one)
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(&t[mid].start) <= row) lo = mid; else hi = mid - 1;
-    }
-    return lo;
-}
-__device__ __forceinline__ bool chunk_bit(const uint32_t* __restrict__ bits, int64_t bit) {
-    return (__ldg(bits + (bit >> 5)) >> (bit & 31)) & 1u;
-}
-
-// ---- order-preserving keys --------------------------------------------------------------------------------------
-template <typename T> struct SortKey;
-template <> struct SortKey<int8_t>   { static __device__ __forceinline__ unsigned long long of(int8_t x)   { return (uint8_t)x ^ 0x80u; } };
-template <> struct SortKey<int16_t>  { static __device__ __forceinline__ unsigned long long of(int16_t x)  { return (uint16_t)x ^ 0x8000u; } };
-template <> struct SortKey<int32_t>  { static __device__ __forceinline__ unsigned long long of(int32_t x)  { return (uint32_t)x ^ 0x80000000u; } };
-template <> struct SortKey<int64_t>  { static __device__ __forceinline__ unsigned long long of(int64_t x)  { return (unsigned long long)x ^ (1ull << 63); } };
-template <> struct SortKey<uint8_t>  { static __device__ __forceinline__ unsigned long long of(uint8_t x)  { return x; } };
-template <> struct SortKey<uint16_t> { static __device__ __forceinline__ unsigned long long of(uint16_t x) { return x; } };
-template <> struct SortKey<uint32_t> { static __device__ __forceinline__ unsigned long long of(uint32_t x) { return x; } };
-template <> struct SortKey<uint64_t> { static __device__ __forceinline__ unsigned long long of(uint64_t x) { return x; } };
-template <> struct SortKey<float> {
-    static __device__ __forceinline__ unsigned long long of(float x) {
-        if (x != x) return 0xffffffffull;            // every NaN is the same, greatest key
-        if (x == 0.0f) x = 0.0f;                     // -0.0 == 0.0
-        const uint32_t b = __float_as_uint(x);
-        return (b >> 31) ? (uint32_t)~b : (b | 0x80000000u);
-    }
-};
-template <> struct SortKey<double> {
-    static __device__ __forceinline__ unsigned long long of(double x) {
-        if (x != x) return ~0ull;
-        if (x == 0.0) x = 0.0;
-        const unsigned long long b = (unsigned long long)__double_as_longlong(x);
-        return (b >> 63) ? ~b : (b | (1ull << 63));
-    }
-};
 
 // keys[i] = key of row idx[i] (idx == nullptr: row i) of the chunked column; mode 1: the null flag instead.
 // Also folds the bitwise OR and AND of every key written into agree[0], agree[1]: a byte on which OR == AND is the

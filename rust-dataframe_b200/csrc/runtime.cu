@@ -2078,6 +2078,180 @@ static int group_aggregate_dev(bdf_ctx* c, const bdf_col* key, int n_values, con
 }
 
 // ---------------------------------------------------------------------------------------------------
+// equi-join (k_join.cu): the build side (the right side; the left side for RIGHT) is sorted, gathered and cut into runs of equal
+// key tuples exactly as group_by_dev does it; every probe row binary-searches the distinct tuples, the counts are scanned into
+// output offsets (one host wait for the total), and the emit writes the index pairs by output position.  FULL appends the build
+// rows of the runs no probe row hit, listed in row order by a compaction of an iota.
+
+namespace bdf {
+int join_tile_rows();
+cudaError_t launch_join_count(int n_keys, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,
+                              const uint32_t* const* build_valid, long long n_probe, const uint32_t* run_starts, long long n_runs, long long n_build,
+                              int outer, unsigned long long* counts, uint32_t* match_start, unsigned char* hit, unsigned long long* block_sums,
+                              cudaStream_t s);
+cudaError_t launch_join_scan(unsigned long long* counts, long long n_probe, unsigned long long* block_sums, cudaStream_t s);
+cudaError_t launch_join_emit(const unsigned long long* offs, long long n_probe, const uint32_t* match_start, const uint32_t* perm, unsigned long long probe_rows,
+                             const uint32_t* unmatched, unsigned long long n_out, uint32_t* probe_out, uint32_t* probe_valid, uint32_t* build_out,
+                             uint32_t* build_valid, cudaStream_t s);
+cudaError_t launch_join_unmatched(const uint32_t* perm, long long n_build, const uint32_t* run_starts, long long n_runs, const unsigned char* hit,
+                                  uint32_t* mask, int sm_count, cudaStream_t s);
+}  // namespace bdf
+
+static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, const bdf_col* const* rk, bdf_col** out_l, bdf_col** out_r,
+                    int64_t* n_rows_out) {
+    if (n_keys == 0) return fail(BDF_INVALID, "Join criteria cannot be empty");
+    if (n_keys < 0 || n_keys > 16) return fail(BDF_INVALID, "1..16 join criteria");
+    if (!lk || !rk) return fail(BDF_INVALID, "null argument");
+    for (int k = 0; k < n_keys; k++)
+        if (!lk[k] || !rk[k]) return fail(BDF_INVALID, "null join column");
+    if (how < BDF_JOIN_LEFT || how > BDF_JOIN_FULL) return fail(BDF_UNSUPPORTED, "unknown join type %d", how);
+    for (int k = 0; k < n_keys; k++)
+        if (lk[k]->dtype < 0 || lk[k]->dtype >= BDF_NTYPES || rk[k]->dtype < 0 || rk[k]->dtype >= BDF_NTYPES)
+            return fail(BDF_UNSUPPORTED, "join columns must be numeric");
+    for (int k = 0; k < n_keys; k++)
+        if (lk[k]->dtype != rk[k]->dtype) return fail(BDF_UNSUPPORTED, "Join columns must have compatible types");
+    for (int k = 0; k < n_keys; k++)
+        if (lk[k]->total_len != lk[0]->total_len || rk[k]->total_len != rk[0]->total_len)
+            return fail(BDF_LENGTH_MISMATCH, "join columns of one side have different lengths");
+    if (lk[0]->total_len > 0xffffffffLL || rk[0]->total_len > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
+    const bool swap = how == BDF_JOIN_RIGHT, full = how == BDF_JOIN_FULL, outer = how != BDF_JOIN_INNER;
+    const bdf_col* const* probe = swap ? rk : lk;
+    const bdf_col* const* build = swap ? lk : rk;
+    const int64_t np = probe[0]->total_len, nb = build[0]->total_len;
+    std::vector<bdf_col*> tmp;   // everything made on the way; released at the end whatever happens
+    int st = BDF_OK;
+    cudaError_t e = cudaSuccess;
+
+    // the build side: sorted row numbers, the distinct key tuples, the first sorted row of every run
+    std::vector<bdf_sort_key> sk((size_t)n_keys);
+    for (int k = 0; k < n_keys; k++) sk[k] = bdf_sort_key{build[k], 0};
+    bdf_col *perm = nullptr, *head = nullptr, *iota = nullptr, *starts = nullptr, *mask = nullptr, *unm = nullptr, *pidx = nullptr, *bidx = nullptr;
+    std::vector<const bdf_col*> skeys;
+    std::vector<bdf_col*> ukeys((size_t)n_keys, nullptr);
+    st = sort_indices_dev(c, n_keys, sk.data(), &perm);
+    if (st == BDF_OK) tmp.push_back(perm);
+    for (int k = 0; k < n_keys && st == BDF_OK; k++) {
+        bdf_col* s = nullptr;
+        st = take_dev(c, build[k], perm, &s);
+        if (st == BDF_OK) { tmp.push_back(s); skeys.push_back(s); }
+    }
+    if (st == BDF_OK) st = group_heads(c, skeys, false, nb, &head);
+    if (st == BDF_OK) tmp.push_back(head);
+    for (int k = 0; k < n_keys && st == BDF_OK; k++) {
+        st = filter_dev(c, skeys[k], head, &ukeys[k]);
+        if (st == BDF_OK) tmp.push_back(ukeys[k]);
+    }
+    if (st == BDF_OK) st = col_alloc(c, BDF_U32, {ChunkPlan{nb, false}}, nullptr, 0, &iota);
+    if (st == BDF_OK) {
+        tmp.push_back(iota);
+        c->launches++;
+        e = nb > 0 ? launch_iota((uint32_t*)iota->chunks[0].values, nb, c->sm_count, c->s_compute) : cudaSuccess;
+        if (e == cudaSuccess) e = finish_single_group(c, iota);
+        if (e != cudaSuccess) st = fail_cuda(e, "join iota");
+    }
+    if (st == BDF_OK) st = filter_dev(c, iota, head, &starts);
+    int64_t n_runs = 0;
+    if (st == BDF_OK) { tmp.push_back(starts); n_runs = starts->chunks[0].len; }
+
+    // the probe side is read in place, through the chunk tables of its key columns
+    std::vector<const void*> ptables((size_t)n_keys), bkeys((size_t)n_keys);
+    std::vector<const uint32_t*> bvalid((size_t)n_keys);
+    std::vector<int> pchunks((size_t)n_keys), dtypes((size_t)n_keys);
+    int64_t key_bytes = 0;
+    for (int k = 0; k < n_keys && st == BDF_OK; k++) {
+        void* t = nullptr;
+        st = sort_table(c, probe[k], &t, &pchunks[k], nullptr);
+        ptables[k] = t;
+        bkeys[k] = ukeys[k]->chunks[0].values;
+        bvalid[k] = ukeys[k]->chunks[0].validity;
+        dtypes[k] = probe[k]->dtype;
+        key_bytes += dtype_width(probe[k]->dtype);
+    }
+    const int64_t blocks = (np + join_tile_rows() - 1) / join_tile_rows();
+    unsigned long long *counts = nullptr, *block_sums = nullptr;
+    uint32_t* mstart = nullptr;
+    unsigned char* hit = nullptr;
+    if (st == BDF_OK) {
+        e = cudaMallocAsync((void**)&counts, (size_t)(np + 1) * sizeof(unsigned long long), c->s_compute);
+        if (e == cudaSuccess) e = cudaMallocAsync((void**)&mstart, (size_t)std::max<int64_t>(np, 1) * sizeof(uint32_t), c->s_compute);
+        if (e == cudaSuccess) e = cudaMallocAsync((void**)&block_sums, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long), c->s_compute);
+        if (e == cudaSuccess && full) e = cudaMallocAsync((void**)&hit, (size_t)std::max<int64_t>(n_runs, 1), c->s_compute);
+        if (e == cudaSuccess && full) e = cudaMemsetAsync(hit, 0, (size_t)std::max<int64_t>(n_runs, 1), c->s_compute);
+        if (e != cudaSuccess) st = fail_cuda(e, "join scratch allocation");
+    }
+    unsigned long long total = 0;   // output rows of the probe part
+    if (st == BDF_OK) {
+        {
+            LaunchTimer t(c, BDF_K_JOIN, BDF_U32, np, np * (key_bytes + 8 + 4));
+            e = launch_join_count(n_keys, dtypes.data(), ptables.data(), pchunks.data(), bkeys.data(), bvalid.data(), np, (const uint32_t*)starts->chunks[0].values,
+                                  n_runs, nb, outer ? 1 : 0, counts, mstart, hit, block_sums, c->s_compute);
+        }
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_JOIN, BDF_U64, np, np * 16 + blocks * 16);
+            c->launches++;   // two kernels: the CTA totals, then the rows
+            e = launch_join_scan(counts, np, block_sums, c->s_compute);
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&total, counts + np, sizeof(total), cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // the output length sizes the result
+        if (e != cudaSuccess) st = fail_cuda(e, "join count");
+    }
+
+    // FULL: the build rows of runs nobody hit, in row order
+    int64_t n_unm = 0;
+    if (st == BDF_OK && full) {
+        st = col_alloc(c, kBool, {ChunkPlan{nb, false}}, nullptr, 0, &mask);
+        if (st == BDF_OK) {
+            tmp.push_back(mask);
+            e = nb > 0 ? cudaMemsetAsync(mask->chunks[0].values, 0, (size_t)(nb + 31) / 32 * 4, c->s_compute) : cudaSuccess;
+            if (e == cudaSuccess) {
+                LaunchTimer t(c, BDF_K_JOIN, kBool, nb, nb * 8 + n_runs * 5);
+                e = launch_join_unmatched((const uint32_t*)perm->chunks[0].values, nb, (const uint32_t*)starts->chunks[0].values, n_runs, hit,
+                                          (uint32_t*)mask->chunks[0].values, c->sm_count, c->s_compute);
+            }
+            if (e == cudaSuccess) e = finish_single_group(c, mask);
+            if (e != cudaSuccess) st = fail_cuda(e, "join unmatched rows");
+        }
+        if (st == BDF_OK) st = filter_dev(c, iota, mask, &unm);
+        if (st == BDF_OK) { tmp.push_back(unm); n_unm = unm->chunks[0].len; }
+    }
+
+    const unsigned long long n_out = total + (unsigned long long)n_unm;
+    if (st == BDF_OK && (long double)n_out * 8.25L > (long double)c->hbm_bytes)   // two UInt32 columns and their bitmaps
+        st = fail(BDF_OOM, "a join output of %llu rows does not fit in device memory", n_out);
+    if (st == BDF_OK) st = col_alloc(c, BDF_U32, {ChunkPlan{(int64_t)n_out, full}}, nullptr, 0, &pidx);
+    if (st == BDF_OK) st = col_alloc(c, BDF_U32, {ChunkPlan{(int64_t)n_out, outer}}, nullptr, 0, &bidx);
+    if (st == BDF_OK) {
+        {
+            LaunchTimer t(c, BDF_K_JOIN, BDF_U32, (int64_t)n_out, (int64_t)n_out * 12 + (int64_t)bitmap_bytes((int64_t)n_out) * 2);
+            e = launch_join_emit(counts, np, mstart, (const uint32_t*)perm->chunks[0].values, total, unm ? (const uint32_t*)unm->chunks[0].values : nullptr, n_out,
+                                 (uint32_t*)pidx->chunks[0].values, pidx->chunks[0].validity, (uint32_t*)bidx->chunks[0].values, bidx->chunks[0].validity,
+                                 c->s_compute);
+        }
+        if (e == cudaSuccess) e = finish_single_group(c, pidx);
+        if (e == cudaSuccess) e = finish_single_group(c, bidx);
+        if (e != cudaSuccess) st = fail_cuda(e, "join emit");
+    }
+    for (void* p : {(void*)counts, (void*)mstart, (void*)block_sums, (void*)hit})
+        if (p) cudaFreeAsync(p, c->s_compute);
+    if (st != BDF_OK) {
+        const std::string keep = g_err;
+        cudaGetLastError();
+        for (bdf_col* t : tmp) col_release(c, t);
+        col_release(c, pidx);
+        col_release(c, bidx);
+        g_err = keep;
+        return st;
+    }
+    for (bdf_col* t : tmp) col_release(c, t);
+    pidx->null_counts[0] = full ? n_unm : 0;
+    bidx->null_counts[0] = outer ? -1 : 0;   // the probe rows without a partner: counted on demand
+    *out_l = swap ? bidx : pidx;
+    *out_r = swap ? pidx : bidx;
+    if (n_rows_out) *n_rows_out = (int64_t)n_out;
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Multi-GPU context (bdf_init_multi): ONE process, every GPU of the box.  The library owns the sharding that the
 // reference leaves to rayon (par_iter over chunks, src/functions/scalar.rs:28-31,99-102): the rows of a call are cut into
 // one contiguous range per GPU (cuts on 64-row boundaries inside a chunk, so a piece is a zero-copy Arrow slice whose
@@ -3264,6 +3438,14 @@ int bdf_group_by_dev(bdf_ctx* c, int32_t n_keys, const bdf_col* const* keys, int
     if (!keys || !out_keys || (n_aggs && (!aggs || !out))) return fail(BDF_INVALID, "null argument");
     if (n_aggs < 0 || n_aggs > 64) return fail(BDF_INVALID, "0..64 aggregations");
     return group_by_dev(c, n_keys, keys, n_aggs, aggs, out_keys, out, n_groups);
+}
+
+int bdf_join_indices_dev(bdf_ctx* c, int32_t join_type, int32_t n_keys, const bdf_col* const* left_keys, const bdf_col* const* right_keys,
+                         bdf_col** left_indices, bdf_col** right_indices, int64_t* n_rows) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "a join moves rows between chunks: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    if (!left_indices || !right_indices) return fail(BDF_INVALID, "null argument");
+    return join_dev(c, join_type, n_keys, left_keys, right_keys, left_indices, right_indices, n_rows);
 }
 
 int bdf_take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, bdf_col** out) {

@@ -17,9 +17,11 @@ The planner is plain host logic (tested without a GPU); everything that touches 
 Kept as the reference has it: select/drop keep frame order (:258-330), with_column replaces an existing name by
 drop + append (:97-113), arithmetic Calculations exist for the 8 types of calculate's match (Int8/UInt8 panic with
 "Unsupported operation"), trig for floats only, GroupAggregate panics.  Different on purpose: ``limit`` gathers the
-first rows into one chunk (the reference slices chunks zero-copy), Join is not mirrored (src/functions/join.rs emits
-its pairs in HashMap iteration order and hashes null rows with truncated keys -- there is no single right answer
-to be identical to).
+first rows into one chunk (the reference slices chunks zero-copy).  Join (``DeviceFrame.join``, the ``("join", (other,
+criteria, how))`` step) plans the schema ``Dataset::try_join`` plans and takes every column by the index pairs of
+``bdf_join_indices_dev``, whose order is defined where the reference's is not (src/functions/join.rs emits its pairs in
+HashMap iteration order): left rows in row order, each one's partners in right row order; a null key matches nothing, and
+FULL is the SQL full outer join (include/b200df.h lists the five departures).
 """
 from __future__ import annotations
 
@@ -129,6 +131,34 @@ def plan_aggregate(schema: Dict[str, int], groups: Sequence[str], aggregations: 
     return out
 
 
+def join(other: "DeviceFrame", criteria: Sequence[Tuple[str, str]], how: str):
+    """Transformation::Join against `other`: criteria [(column of this frame, column of other)], how in left | right | inner | full."""
+    return ("join", (other, [(a, b) for a, b in criteria], how))
+
+
+def plan_join(schema_a: Dict[str, int], schema_b: Dict[str, int], criteria: Sequence[Tuple[str, str]]) -> List[Tuple[str, int]]:
+    """The joined schema `Dataset::try_join` (expression.rs:223-287) plans for `criteria` ([(column of a, column of b)]), as
+    [(name, dtype)]: a's columns, then b's; a name present on both sides becomes `a.<name>` / `b.<name>`.  Its checks in its
+    order, per criterion: both missing, a missing, b missing, different types -- ComputeError with its texts.  Then what the
+    device path adds: non-numeric keys are UnsupportedType, and zero criteria (a cross join in the reference) are refused."""
+    for a, b in criteria:
+        if a not in schema_a and b not in schema_b:
+            raise N.ComputeError("Join columns do not exist in tables")
+        if a not in schema_a:
+            raise N.ComputeError("Join column does not exist in table A")
+        if b not in schema_b:
+            raise N.ComputeError("Join column does not exist in table B")
+        if schema_a[a] != schema_b[b]:
+            raise N.ComputeError("Join columns must have compatible types")
+    for a, _ in criteria:
+        if schema_a[a] == BOOL or not 0 <= schema_a[a] <= F64:
+            raise N.UnsupportedType(f"join column {a!r} is not numeric: join keys must be")
+    if not criteria:
+        raise N.ComputeError("Join criteria cannot be empty")
+    out = [(f"a.{n}" if n in schema_b else n, t) for n, t in schema_a.items()]
+    return out + [(f"b.{n}" if n in schema_a else n, t) for n, t in schema_b.items()]
+
+
 # ---- BooleanFilter (expression.rs:752-763) as nested tuples: ("col", name) | ("scalar", v) | ("not", x) | ("and", a, b) | ("gt", a, b) ...
 def col(name: str):
     return ("col", name)
@@ -203,6 +233,11 @@ def _schema_walk(schema: "OrderedDict[str, int]", transformations: Sequence[tupl
                 t = arg.dtype if arg.function == "cast" else cur.get(arg.inputs[0], F64)
                 cur.pop(arg.output, None)
                 cur[arg.output] = t
+        elif kind == "join":
+            try:
+                cur = OrderedDict(plan_join(cur, arg[0].schema, arg[1]))
+            except N.ArrowError:       # the step itself raises when it is evaluated; nothing after it is fused
+                cur = OrderedDict()
     out.append(cur)
     return out
 
@@ -223,6 +258,10 @@ def plan_fusion(schema: "OrderedDict[str, int]", transformations: Sequence[tuple
     steps = list(transformations)
     schemas = _schema_walk(schema, steps)
     needed = _needed_after(steps, list(schemas[-1].keys()))
+    for i, (kind, _) in enumerate(steps):
+        if kind == "join":   # every column of the frame reaches the joined frame (perhaps renamed): all are observable
+            for j in range(i):
+                needed[j] |= set(schemas[i])
     out: List[tuple] = []
     i = 0
     while i < len(steps):
@@ -413,6 +452,20 @@ class DeviceFrame:
                 cols[f"{fn}({x})"] = r
         return DeviceFrame(OrderedDict((name, cols[name]) for name, _ in plan))
 
+    def join(self, other: "DeviceFrame", criteria: Sequence[Tuple[str, str]], how: str) -> "DeviceFrame":
+        """DataFrame::join (src/dataframe.rs:626-719): the schema of `plan_join`, every column of both sides taken by the index
+        pairs of `join_indices` (one chunk each; a NULL index gives a NULL slot)."""
+        from .functions import join_indices
+
+        plan = plan_join(self.schema, other.schema, criteria)
+        li, ri = join_indices([self.column(a) for a, _ in criteria], [other.column(b) for _, b in criteria], how)
+        try:
+            cols = [c.take(li) for c in self.columns.values()] + [c.take(ri) for c in other.columns.values()]
+        finally:
+            li.free()
+            ri.free()
+        return DeviceFrame(OrderedDict((name, c) for (name, _), c in zip(plan, cols)))
+
     def limit(self, count: int) -> "DeviceFrame":
         if not self.columns:
             return self
@@ -487,6 +540,8 @@ class DeviceFrame:
                 frame = frame.limit(arg)
             elif kind == "sort":
                 frame = frame.sort(arg)
+            elif kind == "join":
+                frame = frame.join(*arg)
             elif kind == "group_aggregate":
                 raise N.ReferencePanic("aggregations not supported")       # evaluation.rs:73
             else:

@@ -514,6 +514,27 @@ def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
     return [Column(ctx, C.c_void_p(hk[k])) for k in range(nk)], [Column(ctx, C.c_void_p(out[j])) for j in range(na)]
 
 
+def join_indices(left_keys: Sequence["Column"], right_keys: Sequence["Column"], how: str):
+    """calc_equijoin_indices (src/functions/join.rs:19-137) on the device (bdf_join_indices_dev): criterion k is
+    ``(left_keys[k], right_keys[k])``; ``how`` is "left", "right", "inner" or "full".  Returns ``(left_idx, right_idx)``, two
+    one-chunk UInt32 Columns of row numbers (NULL = no partner) to ``take`` each side's columns with.  The order of the pairs is
+    fixed (left rows in row order, each one's partners in right row order; see include/b200df.h), a null key matches nothing,
+    NaN == NaN and -0.0 == 0.0."""
+    if how not in N.JOIN_TYPES:
+        raise N.UnsupportedType(f"join type {how!r} is not one of {sorted(N.JOIN_TYPES)}")
+    if len(left_keys) != len(right_keys):
+        raise N.ComputeError("every join criterion needs a left and a right column")
+    if not left_keys:
+        raise N.ComputeError("Join criteria cannot be empty")
+    ctx = left_keys[0].ctx
+    n = len(left_keys)
+    lk = (C.c_void_p * n)(*[k.handle for k in left_keys])
+    rk = (C.c_void_p * n)(*[k.handle for k in right_keys])
+    hl, hr, rows = C.c_void_p(), C.c_void_p(), C.c_int64(0)
+    N.raise_for_status(N.lib().bdf_join_indices_dev(ctx.handle, N.JOIN_TYPES[how], n, lk, rk, C.byref(hl), C.byref(hr), C.byref(rows)))
+    return Column(ctx, hl), Column(ctx, hr)
+
+
 def _expr_nodes(nodes: Sequence[tuple]):
     arr = (N.ExprNode * len(nodes))()
     for k, nd in enumerate(nodes):
