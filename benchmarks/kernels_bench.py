@@ -4,6 +4,7 @@ the library's compute stream via its launch records).  Not the headline benchmar
 is the evidence that every kernel of the path, not only f64 add, runs near the HBM roofline.
 
     python benchmarks/kernels_bench.py [--rows 100000000] [--json kernels.json]
+    python benchmarks/kernels_bench.py --csv [--csv-rows 50000000] [--json csv.json]   # the CSV reader rows instead (a 2.55 GB temporary file)
 """
 from __future__ import annotations
 
@@ -11,6 +12,8 @@ import argparse
 import json
 import os
 import sys
+import tempfile
+import time
 
 import numpy as np
 
@@ -47,12 +50,101 @@ def timed(ctx, fn, reps=12):
     return {k: (float(np.median([r["ms"] for r in v])), v[0]["bytes"], v[0]["rows"]) for k, v in by.items()}
 
 
+def _digits(v, width):
+    """uint8 [len(v), width]: the non-negative integers v as zero-padded ASCII."""
+    p = 10 ** np.arange(width - 1, -1, -1, dtype=np.int64)
+    return ((v[:, None] // p[None, :]) % 10 + 48).astype(np.uint8)
+
+
+def write_csv(path, rows, seed=11, block=5_000_000):
+    """rows x (Int64 id, lat and lng with 6 decimals, Boolean, a quoted city with a comma): 51 bytes per row, fixed width."""
+    rng = np.random.default_rng(seed)
+    with open(path, "wb") as f:
+        f.write(b"id,lat,lng,flag,city\n")
+        for r0 in range(0, rows, block):
+            n = min(block, rows - r0)
+            m = np.empty((n, 51), np.uint8)
+            m[:, 0:10] = _digits(np.arange(r0, r0 + n, dtype=np.int64) * 7 % 10 ** 10, 10)
+            lat, lng = rng.integers(-90_000_000, 90_000_000, n), rng.integers(-180_000_000, 180_000_000, n)
+            m[:, 10] = 44
+            m[:, 11] = np.where(lat < 0, 45, 43)
+            d = _digits(np.abs(lat), 8)
+            m[:, 12:14], m[:, 14], m[:, 15:21] = d[:, :2], 46, d[:, 2:]
+            m[:, 21] = 44
+            m[:, 22] = np.where(lng < 0, 45, 43)
+            d = _digits(np.abs(lng), 9)
+            m[:, 23:26], m[:, 26], m[:, 27:33] = d[:, :3], 46, d[:, 3:]
+            m[:, 33] = 44
+            flag = rng.random(n) < 0.5
+            m[:, 34:50] = np.where(flag[:, None], np.frombuffer(b'true,"Leeds, UK"', np.uint8), np.frombuffer(b'false,"Leed, UK"', np.uint8))
+            m[:, 50] = 10
+            f.write(m.tobytes())
+
+
+def csv_bench(ctx, rows, rows_out, reps=3):
+    """File -> device columns: the upload, the tokenizer and parse kernels (launch records), end to end; Arrow C++ on the host."""
+    with tempfile.TemporaryDirectory() as td:
+        path = os.path.join(td, "bench.csv")
+        write_csv(path, rows)
+        nbytes = os.path.getsize(path)
+        schema = [rdf.I64, rdf.F64, rdf.F64, N.BOOL, N.UTF8]
+        e2e, up, tok, parse = [], [], [], []
+        for _ in range(reps + 1):
+            ctx.synchronize()
+            ctx.profile_read()
+            ctx.profile_enable(True)
+            t0 = time.perf_counter()
+            with rdf.CsvFile(path, schema=schema, ctx=ctx) as f:
+                cols = f.read(["id", "lat", "lng", "flag"])
+                ctx.synchronize()
+                t1 = time.perf_counter()
+                st = f.stats()
+            ctx.profile_enable(False)
+            recs = [r for r in ctx.profile_read() if r["kernel"] == "csv"]
+            for c in cols.values():
+                c.free()
+            e2e.append((t1 - t0) * 1e3)
+            up.append(st["upload_ms"])
+            tok.append(sum(r["ms"] for r in recs[:3]))   # tokenize (4 kernels), field index, record check
+            parse.append(sum(r["ms"] for r in recs[3:]))
+        med = lambda v: float(np.median(v[1:]))   # the first run warms up
+        for name, ms in (("csv upload (page cache -> HBM)", med(up)), ("csv tokenize + index + check", med(tok)),
+                         ("csv parse 4 columns", med(parse)), ("csv file -> device columns, end to end", med(e2e))):
+            gbs = nbytes / ms / 1e6
+            rows_out.append({"case": name, "config": "csv", "kernel": "csv", "ms": ms, "rows": rows, "file_bytes": nbytes, "GBs_of_file": gbs})
+            print(f"{name:44s} {ms:9.2f} ms  {gbs:7.2f} GB/s of file bytes ({nbytes / 1e9:.2f} GB, {rows:.1e} rows)", flush=True)
+        try:
+            import pyarrow as pa
+            import pyarrow.csv as pacsv
+        except ImportError:
+            return
+        types = {"id": pa.int64(), "lat": pa.float64(), "lng": pa.float64(), "flag": pa.bool_(), "city": pa.string()}
+        ts = []
+        for _ in range(2):
+            t0 = time.perf_counter()
+            pacsv.read_csv(path, convert_options=pacsv.ConvertOptions(column_types=types))
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ms = min(ts)
+        name = f"Arrow C++ (not the reference) read_csv, {os.cpu_count()} cores"
+        rows_out.append({"case": name, "config": "csv", "kernel": "host", "ms": ms, "rows": rows, "file_bytes": nbytes, "GBs_of_file": nbytes / ms / 1e6})
+        print(f"{name:44s} {ms:9.2f} ms  {nbytes / ms / 1e6:7.2f} GB/s of file bytes", flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--csv-rows", type=int, default=50_000_000)
+    ap.add_argument("--csv", action="store_true", help="run the CSV reader rows instead of the kernel table")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.csv:
+        rows_out = []
+        csv_bench(ctx, args.csv_rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"results": rows_out}, f, indent=1)
+        return
     chunk = 4_000_000
     lens = [chunk] * (args.rows // chunk)
     G = rdf.Column.generate

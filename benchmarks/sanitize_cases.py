@@ -75,6 +75,20 @@ for dtype in (rdf.I8, rdf.I16, rdf.I32, rdf.I64, rdf.U8, rdf.U16, rdf.U32, rdf.U
     for how in rdf.native.JOIN_TYPES:
         li, ri = rdf.join_indices([rdf.Column.upload(jl), lk2], [rdf.Column.upload(jr), rk2], how)
         li.download(); ri.download()
+# CSV reader: tokenizer scan, field index, record check, inference, parse of every type (exact fallback included), scatter
+import tempfile
+with tempfile.TemporaryDirectory() as td:
+    path = os.path.join(td, "s.csv")
+    with open(path, "w") as fh:
+        fh.write("a,b,c,d,e\n")
+        for r in range(20000):
+            fh.write(f'{r},"x, ""{r}""",{"" if r % 7 == 0 else r * 0.25},{"true" if r % 2 else "False"},1.00000000000000011102230246251565404236316680908203125\n')
+    with rdf.CsvFile(path, batch_size=1000) as f:
+        for c in f.read().values():
+            c.download()
+    with rdf.CsvFile(path, batch_size=7, schema=[rdf.U16, -1, rdf.F32, 10, rdf.F32]) as f:
+        for c in f.read().values():
+            c.download()
 # round 2: the fleet code path on one GPU, and a single-rank communicator (pack -> combine -> unpack on the stream)
 fleet = rdf.Context.multi(1)
 fa = [P.from_numpy(rng.integers(-100, 100, n).astype(np.int64), rng.random(n) > 0.3) for n in (1000, 0, 77)]

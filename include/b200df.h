@@ -32,6 +32,7 @@
  *                          max on floats: T::Native: Float / Ord)
  *   BDF_WOULD_PANIC     -> the reference panics here (max/min .unwrap() on an all-null or empty chunk,
  *                          aggregate.rs:19,29); the binding turns it back into a panic
+ *   BDF_PARSE           -> ArrowError::ParseError(bdf_last_error()) (the CSV reader)
  *   BDF_CUDA / BDF_OOM / BDF_INVALID -> ArrowError::ComputeError(bdf_last_error())
  * There is NO CPU fallback: without a usable CUDA device bdf_init fails with BDF_CUDA.
  *
@@ -77,7 +78,8 @@ typedef enum { BDF_AND = 0, BDF_OR, BDF_NOT } bdf_boolop;
 
 typedef enum {
     BDF_OK = 0, BDF_LENGTH_MISMATCH = 1, BDF_DIVIDE_BY_ZERO = 2, BDF_UNSUPPORTED = 3, BDF_CUDA = 4,
-    BDF_NCCL = 5 /* the communicator (bdf_comm_*) or a collective failed */, BDF_OOM = 6, BDF_WOULD_PANIC = 7, BDF_INVALID = 8
+    BDF_NCCL = 5 /* the communicator (bdf_comm_*) or a collective failed */, BDF_OOM = 6, BDF_WOULD_PANIC = 7, BDF_INVALID = 8,
+    BDF_PARSE = 9 /* a CSV value does not parse as its column's type: ArrowError::ParseError(bdf_last_error()) */
 } bdf_status;
 
 /* One chunk = one PrimitiveArray<T> in Arrow memory layout (ArrayData: buffers[0], null bitmap, len, offset). */
@@ -373,6 +375,60 @@ int  bdf_ipc_write_host(const char* path, int32_t n_cols, const char* const* nam
                         const bdf_view* const* cols /* [n_cols][n_batches] */);
 int  bdf_ipc_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols);
 
+/* ---- CSV files straight to the device (DataFrame::from_csv, src/dataframe.rs:349-389; LazyFrame::read(Csv), src/evaluation.rs:328) ----
+ * The reference reads with arrow-rs's csv::Reader (ReaderBuilder::infer_schema(max_records).has_header(..).with_batch_size(1024)) over
+ * the csv / csv-core crates.  Those crates are not restated from source: the rules below are RECALLED, parity unpinned, except the
+ * uk_cities reads the reference tests pin (3 columns, 37 rows, the lat/lng values).
+ * Records (csv-core, default configuration): a DFA over bytes with states StartRecord, StartField, InField, InQuoted, QuoteInQuoted.
+ *   '"' opens a quoted field only at the start of a field (elsewhere in an unquoted field it is a literal byte); inside quotes ""
+ *   is one '"' and a lone '"' closes the quotes; bytes after the close up to the next delimiter / terminator are appended
+ *   literally ("ab"cd -> abcd); the delimiter, '\r' and '\n' are literal inside quotes.  A record ends at '\r', '\n' or "\r\n";
+ *   runs of terminators are skipped (blank lines make no record).  End of file ends the last record; an unterminated quote at
+ *   end of file simply ends the field (csv-core's end-of-input from InQuoted ends the field and the record).  A leading UTF-8
+ *   BOM (EF BB BF) is skipped (the csv crate strips it).  Every record must have as many fields as the first one (the reader is
+ *   not flexible), else BDF_INVALID "CSV error: record R (line: L, byte: B): found record with N fields, but the previous record
+ *   has M fields" (R counts records from 0, the header included; L is 1 + the '\n' bytes before the record; B its byte offset).
+ *   With has_header the first record gives the names, else they are column_1, column_2, ...
+ * Inference (infer_file_schema) over the first max_records data records (all when max_records < 0): an empty field (unquoted or
+ *   "") is a null and adds no type; otherwise, in order: the unquoted value starts with '"' -> Utf8; (?i)^(true)$|^(false)$ ->
+ *   Boolean; ^-?(\d+\.\d+)$ -> Float64; ^-?(\d+)$ -> Int64; else Utf8.  Per column: one type -> it; {Int64, Float64} -> Float64;
+ *   anything else, a column without any type included -> Utf8.  nullable = an empty field was seen there.  So 1e5, .5, +1 and inf
+ *   infer as Utf8.  Departure: \d is ASCII 0-9 here; Rust's regex \d also matches other Unicode digits.
+ * Values: an empty field is NULL; otherwise Rust's FromStr of the column type on the unquoted value.  Integers [+-]?[0-9]+, unsigned
+ *   types refuse '-' (even -0), overflow is an error.  Floats: [+-]? then digits with an optional '.' and optional [eE][+-]?digits
+ *   (1. and .5 parse, . and 1e do not), or inf / infinity / nan in any case; CORRECTLY ROUNDED to the column type (Float32 straight
+ *   from the decimal, never through Float64); -nan is NaN with the sign bit.  Boolean: to_lowercase() == "true" / "false".
+ *   A failure: BDF_PARSE "Error while parsing value {s} for column {c} at line {l}", s the unquoted value, c the column's index in
+ *   the file, l the data record's index from 0 plus 1 with a header (records, not physical lines).  The reported field is the
+ *   first the reference would meet: by RecordBatch, then by column in the requested order, then by row.
+ * Types: the ten numeric types and Boolean are read; Utf8 (and anything else) is not on the device path: bdf_csv_column reports it
+ *   with dtype -1 and bdf_csv_read refuses it (read such columns on the CPU, e.g. arrow's reader with a projection of just them).
+ *   An explicit schema gives one dtype per column: 0..9, BDF_BOOL, or BDF_UTF8 / -1 (skipped); any other value -> BDF_UNSUPPORTED.
+ * Output: one chunk of batch_size rows per RecordBatch (the last one shorter), null counts set, no validity bitmap in a chunk
+ *   without nulls.
+ * Departures from the reference, on purpose: (1) from_csv truncates the frame at the first batch that fails to parse (Err(e) =>
+ *   has_next = false); here the read fails with BDF_PARSE.  (2) unequal field counts: inside the inferred records the reference
+ *   panics (build(..).unwrap()), after them it truncates; here both give BDF_INVALID.  (3) a file without data records (a header
+ *   only, or empty) makes the reference panic at batches[0]: BDF_WOULD_PANIC.  (4) ASCII digits, above.
+ * Memory: bdf_csv_open keeps the file's bytes and the field index (8 B per field) in HBM until bdf_csv_close and needs about 0.25 B
+ *   per file byte more while tokenizing; a read needs its outputs and, when it reads a float column, a list for the float fields
+ *   the fast path cannot round, allocated up front: max(65536, float fields / 64) entries of 40 B (at least 2.6 MB, about 0.63 B
+ *   per float field).  What does not fit gives BDF_OOM; a failed call leaks nothing.  A multi-GPU context -> BDF_UNSUPPORTED.
+ *   Float fields whose rounding the device cannot decide (more than 19 significant digits where the truncation is ambiguous, or an
+ *   ambiguous 128-bit product) are rounded exactly on the host (strtod / strtof in the C locale) and written back; bdf_csv_stats
+ *   counts them.  More of them than max(65536, float fields / 64) in one read -> BDF_UNSUPPORTED. */
+#define BDF_UTF8 11   /* schema entry only: a string column (not read on the device) */
+typedef struct { int32_t has_header; uint8_t delimiter; int64_t max_records /* <0: all */; int64_t batch_size; } bdf_csv_options;
+typedef struct bdf_csv bdf_csv;
+int  bdf_csv_open(bdf_ctx* ctx, const char* path, const bdf_csv_options* options, int32_t n_schema, const int32_t* schema_dtypes /* NULL: infer */,
+                  bdf_csv** out);
+int  bdf_csv_describe(const bdf_csv* file, int32_t* n_columns, int64_t* n_batches, int64_t* n_rows);
+int  bdf_csv_column(const bdf_csv* file, int32_t col, const char** name, int32_t* dtype /* -1 off the path */, int32_t* nullable);
+int  bdf_csv_read(bdf_ctx* ctx, const bdf_csv* file, int32_t n_cols, const int32_t* cols, bdf_col** out /* n_cols */);   /* projection */
+/* fields in the file; float fields the last read rounded on the host; host time of the file's upload in bdf_csv_open */
+int  bdf_csv_stats(const bdf_csv* file, int64_t* n_fields, int64_t* exact_fields, double* upload_ms);
+void bdf_csv_close(bdf_ctx* ctx, bdf_csv* file);   /* the context that opened it */
+
 /* ---- measurement support ------------------------------------------------------------------------ */
 /* Per-launch CUDA-event timing on the library's compute stream (the stream the kernels run on). */
 typedef struct {
@@ -382,7 +438,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

@@ -27,6 +27,11 @@ pub struct BdfOut {
 pub enum BdfCtx {}
 pub enum BdfCol {}   // a column resident in HBM (one chunk per RecordBatch)
 pub enum BdfIpc {}   // a mapped Arrow IPC file
+pub enum BdfCsv {}
+pub const BDF_PARSE: i32 = 9;   // -> ArrowError::ParseError(last_error())
+pub const BDF_UTF8: i32 = 11;   // CSV schema entry: a string column the device skips
+#[repr(C)]
+pub struct BdfCsvOptions { pub has_header: i32, pub delimiter: u8, pub max_records: i64 /* <0: all */, pub batch_size: i64 }
 
 #[repr(C)]
 pub struct BdfExprNode { pub op: i32, pub a: i32, pub b: i32 }   // op: bdf_binop, or BDF_EXPR_UNARY + bdf_unop
@@ -117,6 +122,14 @@ extern "C" {
     // columns, NULL = no partner, to take every column of each side with
     pub fn bdf_join_indices_dev(ctx: *mut BdfCtx, join_type: i32, n_keys: i32, left_keys: *const *const BdfCol, right_keys: *const *const BdfCol,
                                 left_indices: *mut *mut BdfCol, right_indices: *mut *mut BdfCol, n_rows: *mut i64) -> c_int;
+    // CSV files straight to the device (DataFrame::from_csv): rules, departures and memory in include/b200df.h
+    pub fn bdf_csv_open(ctx: *mut BdfCtx, path: *const c_char, options: *const BdfCsvOptions, n_schema: i32, schema_dtypes: *const i32,
+                        out: *mut *mut BdfCsv) -> c_int;
+    pub fn bdf_csv_describe(file: *const BdfCsv, n_columns: *mut i32, n_batches: *mut i64, n_rows: *mut i64) -> c_int;
+    pub fn bdf_csv_column(file: *const BdfCsv, col: i32, name: *mut *const c_char, dtype: *mut i32, nullable: *mut i32) -> c_int;
+    pub fn bdf_csv_read(ctx: *mut BdfCtx, file: *const BdfCsv, n_cols: i32, cols: *const i32, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_csv_stats(file: *const BdfCsv, n_fields: *mut i64, exact_fields: *mut i64, upload_ms: *mut f64) -> c_int;
+    pub fn bdf_csv_close(ctx: *mut BdfCtx, file: *mut BdfCsv);
     // Arrow IPC files (DataFrame::from_arrow / to_arrow)
     pub fn bdf_ipc_open(path: *const c_char, out: *mut *mut BdfIpc) -> c_int;
     pub fn bdf_ipc_close(file: *mut BdfIpc);

@@ -187,6 +187,36 @@ pub fn join_device(left: &DeviceColumns, right: &DeviceColumns, criteria: &[(usi
     Ok(out)
 }
 
+/// `DataFrame::from_csv(path, None)` on the device: a header, ',', the schema inferred from every record, 1024 rows per
+/// RecordBatch (`schema`: one dtype per column instead, BDF_UTF8 for a string column).  Utf8 columns are not on the device path and
+/// are left out; a caller that needs them reads just those with arrow's CPU reader and a projection
+/// (`csv::Reader::new(file, schema, true, None, 1024, Some(utf8_columns))`).
+pub fn from_csv_device(path: &str, schema: Option<&[i32]>) -> Result<DeviceColumns, String> {
+    let c_path = std::ffi::CString::new(path).map_err(|e| e.to_string())?;
+    let opts = BdfCsvOptions { has_header: 1, delimiter: b',', max_records: -1, batch_size: 1024 };
+    let (n_schema, dtypes) = schema.map_or((0, std::ptr::null()), |s| (s.len() as i32, s.as_ptr()));
+    let mut file: *mut BdfCsv = std::ptr::null_mut();
+    check(unsafe { bdf_csv_open(dev(), c_path.as_ptr(), &opts, n_schema, dtypes, &mut file) })?;
+    let (mut n_cols, mut n_batches, mut n_rows) = (0i32, 0i64, 0i64);
+    let res = (|| {
+        check(unsafe { bdf_csv_describe(file, &mut n_cols, &mut n_batches, &mut n_rows) })?;
+        let (mut names, mut idx) = (vec![], vec![]);
+        for i in 0..n_cols {
+            let (mut name, mut dtype, mut nullable) = (std::ptr::null(), 0i32, 0i32);
+            check(unsafe { bdf_csv_column(file, i, &mut name, &mut dtype, &mut nullable) })?;
+            if dtype >= 0 {
+                names.push(unsafe { std::ffi::CStr::from_ptr(name) }.to_string_lossy().into_owned());
+                idx.push(i);
+            }
+        }
+        let mut cols = vec![std::ptr::null_mut(); idx.len()];
+        check(unsafe { bdf_csv_read(dev(), file, idx.len() as i32, idx.as_ptr(), cols.as_mut_ptr()) })?;
+        Ok(DeviceColumns { names, cols })
+    })();
+    unsafe { bdf_csv_close(dev(), file) };
+    res
+}
+
 /// A run of Float64 Calculations whose intermediates are not kept (config 2: h = sin(((a+b)*c)/d)) as one pass.
 /// `inputs` are column indices; node k writes slot inputs.len() + k (see include/b200df.h, bdf_eval_expr_dev).
 pub fn fused_chain(frame: &DeviceColumns, inputs: &[usize], nodes: &[BdfExprNode]) -> Result<*mut BdfCol, String> {

@@ -18,14 +18,15 @@ ADD, SUB, MUL, DIV, ATAN2, HYPOT, LOG = range(7)
 (ABS, SIN, COS, TAN, ACOS, ASIN, ATAN, CBRT, CEIL, COSH, DEGREES, EXP, EXPM1, FLOOR, LOG10, LOG2, RADIANS, ROUND, SINH,
  SQRT, TANH) = range(21)
 SUM, MIN, MAX, COUNT = range(4)
-OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID = range(9)
+OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID, PARSE = range(10)
 ASYNC = 1
-K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN = range(13)
-KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join"]
+K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV = range(14)
+KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
 BOOL = 10
+UTF8 = 11   # CSV schema entry only: a string column the device skips
 # bdf_group_fn (AggregateFunction order)
 GROUP_SUM, GROUP_MAX, GROUP_MIN, GROUP_AVG, GROUP_COUNT, GROUP_COUNT_DISTINCT, GROUP_FIRST, GROUP_LAST = range(8)
 GROUP_FNS = {"sum": GROUP_SUM, "max": GROUP_MAX, "min": GROUP_MIN, "avg": GROUP_AVG, "count": GROUP_COUNT,
@@ -66,6 +67,10 @@ class GroupAggC(C.Structure):
     _fields_ = [("column", C.c_void_p), ("function", C.c_int32)]
 
 
+class CsvOptions(C.Structure):
+    _fields_ = [("has_header", C.c_int32), ("delimiter", C.c_uint8), ("max_records", C.c_int64), ("batch_size", C.c_int64)]
+
+
 class LaunchRecord(C.Structure):
     _fields_ = [("kernel", C.c_int32), ("dtype", C.c_int32), ("rows", C.c_int64), ("bytes", C.c_int64),
                 ("ms", C.c_float)]
@@ -82,6 +87,10 @@ class ComputeError(ArrowError):
 class DivideByZero(ArrowError):
     def __init__(self, msg="Divide by zero error"):
         super().__init__(msg)
+
+
+class ParseError(ArrowError):
+    """ArrowError::ParseError: a CSV value does not parse as its column's type."""
 
 
 class UnsupportedType(ArrowError):
@@ -184,6 +193,12 @@ def lib() -> C.CDLL:
         "bdf_ipc_read_batches": ([vp, vp, i32, P(i32), i64, P(i64), C.c_int, P(vp)], C.c_int),
         "bdf_ipc_write_host": ([C.c_char_p, i32, P(C.c_char_p), P(i32), i64, P(P(View))], C.c_int),
         "bdf_ipc_write": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp)], C.c_int),
+        "bdf_csv_open": ([vp, C.c_char_p, P(CsvOptions), i32, P(i32), P(vp)], C.c_int),
+        "bdf_csv_describe": ([vp, P(i32), P(i64), P(i64)], C.c_int),
+        "bdf_csv_column": ([vp, i32, P(C.c_char_p), P(i32), P(i32)], C.c_int),
+        "bdf_csv_read": ([vp, vp, i32, P(i32), P(vp)], C.c_int),
+        "bdf_csv_stats": ([vp, P(i64), P(i64), P(C.c_double)], C.c_int),
+        "bdf_csv_close": ([vp, vp], None),
         "bdf_generate": ([vp, C.c_int, C.c_int, C.c_double, C.c_double, u64, u64, i64, P(i64), i64, C.c_uint32, P(vp)],
                          C.c_int),
     }
@@ -209,6 +224,7 @@ EXPORTED_SYMBOLS = [
     "bdf_launch_count", "bdf_timer_start", "bdf_timer_stop", "bdf_flush_l2", "bdf_generate",
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",
     "bdf_ipc_write_host", "bdf_ipc_write",
+    "bdf_csv_open", "bdf_csv_describe", "bdf_csv_column", "bdf_csv_read", "bdf_csv_stats", "bdf_csv_close",
 ]
 
 
@@ -226,6 +242,8 @@ def raise_for_status(st: int) -> None:
         raise ReferencePanic(msg)
     if st == OOM:
         raise MemoryError(msg)
+    if st == PARSE:
+        raise ParseError(msg)
     raise ComputeError(f"[bdf status {st}] {msg}")
 
 

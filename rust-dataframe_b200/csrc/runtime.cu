@@ -7,6 +7,8 @@
 // already on its way back.  When all inputs are already resident an operator is ONE batched launch over
 // every chunk of the column.
 #include <algorithm>
+#include <cerrno>
+#include <chrono>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -19,7 +21,11 @@
 #include <limits>
 #include <functional>
 #include <sched.h>
+#include <fcntl.h>
+#include <locale.h>
 #include <sys/mman.h>
+#include <sys/stat.h>
+#include <unistd.h>
 #include <string>
 #include <thread>
 #include <vector>
@@ -2252,6 +2258,430 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
 }
 
 // ---------------------------------------------------------------------------------------------------
+// CSV reader (k_csv.cu; the rules are in include/b200df.h): the file is mapped and its bytes go to HBM through the pageable staging
+// path; the tokenizer scan builds the field index there, the field counts are checked and the schema inferred on the device.  The
+// bytes and the index stay until bdf_csv_close; a read parses only the requested columns.
+
+namespace bdf {
+int csv_tile_bytes();
+int csv_parse_rows();
+size_t csv_desc_bytes();
+size_t csv_slow_bytes();
+size_t csv_patch_bytes();
+cudaError_t launch_csv_tokenize(const uint8_t* text, long long n, uint8_t delim, uint32_t* agg, uint8_t* start, int* final_state, uint16_t* fe,
+                                uint16_t* re, unsigned long long* block_counts, cudaStream_t s);
+cudaError_t launch_csv_index(const uint16_t* fe, const uint16_t* re, long long n, const unsigned long long* block_offsets, unsigned long long* ends,
+                             unsigned long long* first_rec, cudaStream_t s);
+cudaError_t launch_csv_check(const unsigned long long* ends, long long n_fields, long long k, unsigned long long* bad, int sm_count, cudaStream_t s);
+cudaError_t launch_csv_infer(const uint8_t* text, const unsigned long long* ends, long long f0, long long f1, long long k, unsigned int* col_bits,
+                             int sm_count, cudaStream_t s);
+cudaError_t launch_csv_parse(const uint8_t* text, const unsigned long long* ends, const void* cols, int n_cols, long long f0, long long k, long long n_rows,
+                             long long batch, unsigned long long* err_key, void* slow, unsigned long long* n_slow, long long slow_cap, cudaStream_t s);
+cudaError_t launch_csv_scatter(const void* patches, long long n, cudaStream_t s);
+}  // namespace bdf
+
+struct bdf_csv {
+    int fd = -1;
+    const uint8_t* map = nullptr;   // the whole file
+    size_t size = 0;
+    size_t off = 0;                 // 3 when the file starts with a UTF-8 BOM
+    int64_t n = 0;                  // bytes after the BOM (what the device holds)
+    uint8_t* d_text = nullptr;
+    unsigned long long* d_ends = nullptr;   // per field: end byte | bit 63 when it ends its record
+    int64_t n_fields = 0, k = 0, n_rows = 0, f0 = 0, batch = 1024;
+    int has_header = 1;
+    uint8_t delim = ',';
+    std::vector<std::string> names;
+    std::vector<int32_t> dtypes, nullable;
+    mutable int64_t exact_fields = 0;
+    double upload_ms = 0;
+};
+
+static constexpr unsigned long long kCsvRec = 1ull << 63;
+
+static void csv_free(bdf_ctx* c, bdf_csv* f) {
+    if (!f) return;
+    if (f->d_text) cudaFreeAsync(f->d_text, c->s_compute);
+    if (f->d_ends) cudaFreeAsync(f->d_ends, c->s_compute);
+    if (f->map) munmap((void*)f->map, f->size);
+    if (f->fd >= 0) close(f->fd);
+    delete f;
+}
+
+// The unquoted value of raw field bytes [s, e) of the mapping (the rules of csv_parse.cuh's Unquote).
+static std::string csv_unquote(const uint8_t* s, const uint8_t* e) {
+    std::string out;
+    int st = 0;
+    if (s < e && *s == '"') { st = 1; s++; }
+    for (; s < e; s++) {
+        const uint8_t b = *s;
+        if (st == 0) out += (char)b;
+        else if (st == 1) { if (b == '"') st = 2; else out += (char)b; }
+        else if (b == '"') { st = 1; out += '"'; }
+        else { st = 0; out += (char)b; }
+    }
+    return out;
+}
+
+// Raw span of field f from two entries of the index (prev: the entry of f - 1, or none for f == 0).
+static void csv_span(const bdf_csv* f, bool has_prev, unsigned long long prev, unsigned long long cur, int64_t* s, int64_t* e) {
+    const unsigned long long mask = kCsvRec - 1;
+    *e = (int64_t)(cur & mask);
+    int64_t a = has_prev ? (int64_t)(prev & mask) + 1 : 0;
+    if (!has_prev || (prev & kCsvRec))
+        while (a < *e && (f->map[f->off + a] == '\r' || f->map[f->off + a] == '\n')) a++;
+    *s = a;
+}
+
+static int csv_fetch(bdf_ctx* c, const bdf_csv* f, int64_t first, int64_t count, std::vector<unsigned long long>& out) {
+    out.resize((size_t)std::max<int64_t>(count, 1));
+    if (count > 0) {
+        CK(cudaMemcpyAsync(out.data(), f->d_ends + first, (size_t)count * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->s_compute));
+        CK(cudaStreamSynchronize(c->s_compute));
+    }
+    return BDF_OK;
+}
+
+// The field at index `bad` disagrees with the first record's field count: the csv crate's UnequalLengths text.
+static int csv_unequal(bdf_ctx* c, bdf_csv* f, int64_t bad) {
+    const int64_t r = bad / f->k, first = r * f->k;
+    std::vector<unsigned long long> v;
+    TRY(csv_fetch(c, f, first, bad - first + 1, v));
+    int64_t n_found = bad - first + 1;
+    if (!(v[(size_t)(bad - first)] & kCsvRec)) {   // more fields than the first record: find this record's end
+        for (int64_t i = bad + 1; i < f->n_fields; i += 65536) {
+            std::vector<unsigned long long> w;
+            const int64_t cnt = std::min<int64_t>(65536, f->n_fields - i);
+            TRY(csv_fetch(c, f, i, cnt, w));
+            int64_t j = 0;
+            while (j < cnt && !(w[(size_t)j] & kCsvRec)) j++;
+            if (j < cnt) { n_found = i + j - first + 1; break; }
+        }
+    }
+    unsigned long long prev = 0;
+    std::vector<unsigned long long> p;
+    if (first > 0) { TRY(csv_fetch(c, f, first - 1, 1, p)); prev = p[0]; }
+    int64_t s, e;
+    csv_span(f, first > 0, prev, v[0], &s, &e);
+    const int64_t byte = (int64_t)f->off + s;
+    int64_t line = 1;
+    for (int64_t i = 0; i < byte; i++) line += f->map[i] == '\n';
+    return fail(BDF_INVALID, "CSV error: record %lld (line: %lld, byte: %lld): found record with %lld fields, but the previous record has %lld fields",
+                (long long)r, (long long)line, (long long)byte, (long long)n_found, (long long)f->k);
+}
+
+static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int n_schema, const int32_t* schema, bdf_csv** out) {
+    if (!path || !o || !out) return fail(BDF_INVALID, "null argument");
+    if (o->batch_size < 1) return fail(BDF_INVALID, "batch_size must be at least 1");
+    if (o->delimiter == '"' || o->delimiter == '\r' || o->delimiter == '\n') return fail(BDF_INVALID, "the delimiter cannot be a quote or a line terminator");
+    if (schema) {
+        if (n_schema < 1) return fail(BDF_INVALID, "an explicit schema needs at least one column");
+        for (int i = 0; i < n_schema; i++)
+            if (!((schema[i] >= 0 && schema[i] <= kBool) || schema[i] == BDF_UTF8 || schema[i] == -1))
+                return fail(BDF_UNSUPPORTED, "schema column %d: type %d is not read from CSV (numeric, Boolean or Utf8)", i, schema[i]);
+    }
+    bdf_csv* f = new (std::nothrow) bdf_csv();
+    if (!f) return fail(BDF_OOM, "host allocation failed");
+    f->has_header = o->has_header ? 1 : 0;
+    f->delim = o->delimiter;
+    f->batch = o->batch_size;
+    f->fd = open(path, O_RDONLY | O_CLOEXEC);
+    struct stat sb;
+    if (f->fd < 0 || fstat(f->fd, &sb) != 0) { const int err = errno; csv_free(c, f); return fail(BDF_INVALID, "cannot open %s: %s", path, strerror(err)); }
+    f->size = (size_t)sb.st_size;
+    if (f->size) {
+        void* m = mmap(nullptr, f->size, PROT_READ, MAP_PRIVATE, f->fd, 0);
+        if (m == MAP_FAILED) { const int err = errno; csv_free(c, f); return fail(BDF_INVALID, "cannot map %s: %s", path, strerror(err)); }
+        f->map = (const uint8_t*)m;
+    }
+    if (f->size >= 3 && f->map[0] == 0xEF && f->map[1] == 0xBB && f->map[2] == 0xBF) f->off = 3;
+    f->n = (int64_t)(f->size - f->off);
+    const int64_t tile = csv_tile_bytes();
+    const int64_t tiles = std::max<int64_t>((f->n + tile - 1) / tile, 1);
+    if ((long double)tiles * tile * 1.3L > (long double)c->hbm_bytes) { csv_free(c, f); return fail(BDF_OOM, "a CSV file of %lld bytes does not fit in device memory", (long long)f->n); }
+
+    int st = BDF_OK;
+    cudaError_t e = cudaSuccess;
+    uint32_t* agg = nullptr;
+    uint8_t* start = nullptr;
+    uint16_t *fe = nullptr, *re = nullptr;
+    unsigned long long *counts = nullptr, *small = nullptr;   // small: [0] final state, [1] first record end, [2] first bad field
+    unsigned int* bits = nullptr;
+    auto scratch_free = [&]() {
+        for (void* p : {(void*)agg, (void*)start, (void*)fe, (void*)re, (void*)counts, (void*)small, (void*)bits})
+            if (p) cudaFreeAsync(p, c->s_compute);
+        agg = nullptr; start = nullptr; fe = nullptr; re = nullptr; counts = nullptr; small = nullptr; bits = nullptr;
+    };
+    auto bail = [&](int status) {
+        const std::string keep = g_err;
+        cudaGetLastError();
+        scratch_free();
+        cudaStreamSynchronize(c->s_h2d);
+        csv_free(c, f);
+        g_err = keep;
+        return status;
+    };
+
+    // the bytes: page cache -> pinned staging -> HBM
+    e = cudaMallocAsync((void**)&f->d_text, (size_t)(tiles * tile), c->s_compute);
+    if (e == cudaSuccess) e = cudaMemsetAsync(f->d_text + f->n, 0, (size_t)(tiles * tile - f->n), c->s_compute);
+    if (e == cudaSuccess) e = cudaEventRecord(c->ev_tmp, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->s_h2d, c->ev_tmp, 0);
+    const auto t0 = std::chrono::steady_clock::now();
+    if (e == cudaSuccess && f->n) e = h2d_copy(c, f->d_text, f->map + f->off, (size_t)f->n);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_h2d);
+    f->upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (e != cudaSuccess) { fail_cuda(e, "CSV upload"); return bail(cuda_status(e)); }
+
+    // tokenize: the state at every CTA, the field / record end masks, the field count
+    e = cudaMallocAsync((void**)&agg, (size_t)tiles * 4, c->s_compute);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&start, (size_t)tiles, c->s_compute);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&fe, (size_t)tiles * kThreads * 2, c->s_compute);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&re, (size_t)tiles * kThreads * 2, c->s_compute);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&counts, (size_t)(tiles + 1) * 8, c->s_compute);
+    if (e == cudaSuccess) e = cudaMallocAsync((void**)&small, 4 * 8, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemsetAsync(small, 0xff, 4 * 8, c->s_compute);
+    if (e != cudaSuccess) { fail_cuda(e, "CSV tokenizer scratch allocation"); return bail(cuda_status(e)); }
+    {
+        LaunchTimer t(c, BDF_K_CSV, kBool, f->n, f->n * 2 + tiles * kThreads * 4);
+        c->launches += 3;   // reduce, CTA-state scan, mark, count scan
+        e = launch_csv_tokenize(f->d_text, f->n, f->delim, agg, start, (int*)small, fe, re, counts, c->s_compute);
+    }
+    unsigned long long host_small[4] = {0, 0, 0, 0}, total = 0;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&total, counts + tiles, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(host_small, small, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e != cudaSuccess) { fail_cuda(e, "CSV tokenizer"); return bail(cuda_status(e)); }
+    const int final_state = (int)(host_small[0] & 0xffffffffu);
+    const bool eof_field = final_state != 0;   // the last record has no terminator: end of file ends it
+    f->n_fields = (int64_t)total + (eof_field ? 1 : 0);
+    if (f->n_fields == 0) { fail(BDF_WOULD_PANIC, "the CSV file has no records: the reference panics at batches[0]"); return bail(BDF_WOULD_PANIC); }
+
+    // the field index
+    e = cudaMallocAsync((void**)&f->d_ends, (size_t)f->n_fields * 8, c->s_compute);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_CSV, BDF_U64, f->n, tiles * kThreads * 4 + (int64_t)total * 8);
+        e = launch_csv_index(fe, re, f->n, counts, f->d_ends, small + 1, c->s_compute);
+    }
+    unsigned long long eof_entry = (unsigned long long)f->n | kCsvRec;
+    if (e == cudaSuccess && eof_field) e = cudaMemcpyAsync(f->d_ends + total, &eof_entry, 8, cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(host_small, small, 4 * 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e != cudaSuccess) { fail_cuda(e, "CSV field index"); return bail(cuda_status(e)); }
+    const unsigned long long first_rec = std::min<unsigned long long>(host_small[1], eof_field ? total : ~0ull);
+    f->k = (int64_t)first_rec + 1;
+
+    // every record has the first record's field count
+    {
+        LaunchTimer t(c, BDF_K_CSV, BDF_U64, f->n_fields, f->n_fields * 8);
+        e = launch_csv_check(f->d_ends, f->n_fields, f->k, small + 2, c->sm_count, c->s_compute);
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(host_small, small, 4 * 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e != cudaSuccess) { fail_cuda(e, "CSV record check"); return bail(cuda_status(e)); }
+    if (host_small[2] != ~0ull) return bail(csv_unequal(c, f, (int64_t)host_small[2]));
+    const int64_t n_records = f->n_fields / f->k;
+    f->f0 = f->has_header ? f->k : 0;
+    f->n_rows = n_records - f->has_header;
+    if (f->k > 0x7fffffffLL) { fail(BDF_UNSUPPORTED, "more than 2^31-1 columns"); return bail(BDF_UNSUPPORTED); }
+    const int k = (int)f->k;
+
+    // names
+    if (f->has_header) {
+        std::vector<unsigned long long> h;
+        st = csv_fetch(c, f, 0, f->k, h);
+        if (st != BDF_OK) return bail(st);
+        for (int i = 0; i < k; i++) {
+            int64_t s, en;
+            csv_span(f, i > 0, i > 0 ? h[(size_t)i - 1] : 0, h[(size_t)i], &s, &en);
+            f->names.push_back(csv_unquote(f->map + f->off + s, f->map + f->off + en));
+        }
+    } else {
+        for (int i = 0; i < k; i++) f->names.push_back("column_" + std::to_string(i + 1));
+    }
+    if (f->n_rows == 0) { fail(BDF_WOULD_PANIC, "the CSV file has no data records: the reference panics at batches[0]"); return bail(BDF_WOULD_PANIC); }
+
+    // schema
+    if (schema) {
+        if (n_schema != k) { fail(BDF_INVALID, "the schema has %d columns, the file %d", n_schema, k); return bail(BDF_INVALID); }
+        for (int i = 0; i < k; i++) {
+            f->dtypes.push_back(schema[i] == BDF_UTF8 ? -1 : schema[i]);
+            f->nullable.push_back(1);
+        }
+    } else {
+        const int64_t rows = o->max_records < 0 ? f->n_rows : std::min<int64_t>(o->max_records, f->n_rows);
+        std::vector<unsigned int> hb((size_t)k, 0u);
+        e = cudaMallocAsync((void**)&bits, (size_t)k * 4, c->s_compute);
+        if (e == cudaSuccess) e = cudaMemsetAsync(bits, 0, (size_t)k * 4, c->s_compute);
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_CSV, BDF_U32, rows * f->k, rows * f->k * 16);
+            e = launch_csv_infer(f->d_text, f->d_ends, f->f0, f->f0 + rows * f->k, f->k, bits, c->sm_count, c->s_compute);
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(hb.data(), bits, (size_t)k * 4, cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+        if (e != cudaSuccess) { fail_cuda(e, "CSV schema inference"); return bail(cuda_status(e)); }
+        for (int i = 0; i < k; i++) {
+            const unsigned int types = hb[(size_t)i] & ~1u;   // bit 0: an empty field (a null)
+            int dt = -1;                                       // Utf8: other, a mix, or no type at all
+            if (types == 2u) dt = kBool;
+            else if (types == 4u) dt = BDF_I64;
+            else if (types == 8u || types == 12u) dt = BDF_F64;
+            f->dtypes.push_back(dt);
+            f->nullable.push_back((hb[(size_t)i] & 1u) ? 1 : 0);
+        }
+    }
+    scratch_free();
+    *out = f;
+    return BDF_OK;
+}
+
+static int csv_read(bdf_ctx* c, const bdf_csv* f, int n_cols, const int32_t* cols, bdf_col** out) {
+    if (!f || !out || (n_cols > 0 && !cols)) return fail(BDF_INVALID, "null argument");
+    if (n_cols < 0 || n_cols > 65535) return fail(BDF_INVALID, "0..65535 columns");
+    for (int i = 0; i < n_cols; i++) {
+        if (cols[i] < 0 || cols[i] >= (int)f->k) return fail(BDF_INVALID, "column %d out of range (the file has %lld)", cols[i], (long long)f->k);
+        if (f->dtypes[(size_t)cols[i]] < 0)
+            return fail(BDF_UNSUPPORTED, "column %d (%s) is Utf8: not on the device path", cols[i], f->names[(size_t)cols[i]].c_str());
+    }
+    const int64_t batch = f->batch, n_chunks = (f->n_rows + batch - 1) / batch;
+    const int rows_per_tile = csv_parse_rows();
+    std::vector<ChunkPlan> plan((size_t)n_chunks);
+    for (int64_t i = 0; i < n_chunks; i++) plan[(size_t)i] = ChunkPlan{std::min(batch, f->n_rows - i * batch), true};
+    std::vector<bdf_col*> res((size_t)n_cols, nullptr);
+    int st = BDF_OK;
+    cudaError_t e = cudaSuccess;
+    char* descs = nullptr;
+    unsigned long long* small = nullptr;   // [0] first failing field key, [1] slow-path fields
+    void* slow = nullptr;
+    void* patches = nullptr;
+    const size_t dsz = csv_desc_bytes();
+    std::vector<char> hdesc((size_t)std::max(n_cols, 1) * dsz, 0);
+    int64_t float_fields = 0, out_bytes = 0;
+    for (int i = 0; i < n_cols && st == BDF_OK; i++) {
+        const int dt = f->dtypes[(size_t)cols[i]];
+        st = col_alloc(c, dt, plan, nullptr, rows_per_tile, &res[(size_t)i]);
+        if (st != BDF_OK) break;
+        bdf_col* col = res[(size_t)i];
+        const DevChunk& c0 = col->chunks[0];
+        const long long vs = n_chunks > 1 ? (long long)(col->chunks[1].values - c0.values) : 0;
+        const long long bs = n_chunks > 1 ? (long long)((char*)col->chunks[1].validity - (char*)c0.validity) : 0;
+        const DevChunk& cl = col->chunks[(size_t)n_chunks - 1];
+        if (cl.values != c0.values + vs * (n_chunks - 1) || (char*)cl.validity != (char*)c0.validity + bs * (n_chunks - 1)) {
+            st = fail(BDF_INVALID, "internal: CSV output chunks are not evenly spaced");
+            break;
+        }
+        struct Desc { char* values; long long vstride; uint32_t* validity; long long bstride; uint32_t* warp_counts; int dtype; int file_col; } d{
+            c0.values, vs, c0.validity, bs, col->d_warp_counts, dt, cols[i]};
+        static_assert(sizeof(Desc) == 48, "CsvColDesc layout");
+        memcpy(hdesc.data() + (size_t)i * dsz, &d, sizeof d);
+        if (dt == BDF_F32 || dt == BDF_F64) float_fields += f->n_rows;
+        out_bytes += (int64_t)value_bytes(dt, f->n_rows, 0) + bitmap_bytes(f->n_rows);
+    }
+    const long long slow_cap = std::max<long long>(65536, float_fields / 64);
+    if (st == BDF_OK) {
+        e = cudaMallocAsync((void**)&descs, hdesc.size(), c->s_compute);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(descs, hdesc.data(), hdesc.size(), cudaMemcpyHostToDevice, c->s_compute);
+        if (e == cudaSuccess) e = cudaMallocAsync((void**)&small, 16, c->s_compute);
+        if (e == cudaSuccess) e = cudaMemsetAsync(small, 0xff, 8, c->s_compute);
+        if (e == cudaSuccess) e = cudaMemsetAsync(small + 1, 0, 8, c->s_compute);
+        if (e == cudaSuccess && float_fields) e = cudaMallocAsync(&slow, (size_t)slow_cap * csv_slow_bytes(), c->s_compute);
+        if (e != cudaSuccess) st = fail_cuda(e, "CSV read scratch allocation");
+    }
+    unsigned long long hs[2] = {~0ull, 0};
+    if (st == BDF_OK) {
+        {
+            const int64_t fields = f->n_rows * n_cols;
+            LaunchTimer t(c, BDF_K_CSV, n_cols == 1 ? f->dtypes[(size_t)cols[0]] : -1, fields,
+                          f->n * n_cols / std::max<int64_t>(f->k, 1) + fields * 16 + out_bytes);
+            e = launch_csv_parse(f->d_text, f->d_ends, descs, n_cols, f->f0, f->k, f->n_rows, batch, small, slow, small + 1, slow_cap, c->s_compute);
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(hs, small, 16, cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+        if (e != cudaSuccess) st = fail_cuda(e, "CSV parse");
+    }
+    if (st == BDF_OK && hs[0] != ~0ull) {   // the first failing field: (batch, column in the request, row)
+        const unsigned long long key = hs[0];
+        const int64_t row = (int64_t)(key % (unsigned long long)batch), rest = (int64_t)(key / (unsigned long long)batch);
+        const int p = (int)(rest % n_cols);
+        const int64_t chunk = rest / n_cols, r = chunk * batch + row, fld = f->f0 + r * f->k + cols[p];
+        std::vector<unsigned long long> v;
+        st = csv_fetch(c, f, fld > 0 ? fld - 1 : 0, fld > 0 ? 2 : 1, v);
+        if (st == BDF_OK) {
+            int64_t s, en;
+            csv_span(f, fld > 0, fld > 0 ? v[0] : 0, fld > 0 ? v[1] : v[0], &s, &en);
+            g_err = "Error while parsing value " + csv_unquote(f->map + f->off + s, f->map + f->off + en) + " for column " + std::to_string(cols[p]) +
+                    " at line " + std::to_string(r + f->has_header);
+            st = BDF_PARSE;
+        }
+    }
+    int64_t n_slow = (int64_t)hs[1];
+    if (st == BDF_OK && n_slow > slow_cap)
+        st = fail(BDF_UNSUPPORTED, "%lld float fields need exact rounding, more than the %lld one read resolves", (long long)n_slow, slow_cap);
+    if (st == BDF_OK && n_slow > 0) {   // exact rounding on the host, in the C locale, written back by one scatter
+        struct Slow { long long start, end; int col, pad; long long chunk, row; };
+        struct Patch { unsigned long long dst, bits; int width, pad; };
+        std::vector<Slow> sl((size_t)n_slow);
+        e = cudaMemcpyAsync(sl.data(), slow, (size_t)n_slow * sizeof(Slow), cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+        if (e != cudaSuccess) st = fail_cuda(e, "CSV exact rounding");
+        static locale_t cloc = newlocale(LC_ALL_MASK, "C", (locale_t)0);
+        std::vector<Patch> hp;
+        for (size_t i = 0; i < sl.size() && st == BDF_OK; i++) {
+            const Slow& x = sl[i];
+            const std::string v = csv_unquote(f->map + f->off + x.start, f->map + f->off + x.end);
+            const bdf_col* col = res[(size_t)x.col];
+            Patch pt{};
+            if (col->dtype == BDF_F64) {
+                const double d = strtod_l(v.c_str(), nullptr, cloc);
+                memcpy(&pt.bits, &d, 8);
+                pt.width = 8;
+            } else {
+                const float fl = strtof_l(v.c_str(), nullptr, cloc);
+                uint32_t b;
+                memcpy(&b, &fl, 4);
+                pt.bits = b;
+                pt.width = 4;
+            }
+            pt.dst = (unsigned long long)(uintptr_t)(col->chunks[(size_t)x.chunk].values + x.row * pt.width);
+            hp.push_back(pt);
+        }
+        static_assert(sizeof(Patch) == 24, "CsvPatch layout");
+        if (st == BDF_OK) {
+            e = cudaMallocAsync(&patches, hp.size() * sizeof(Patch), c->s_compute);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(patches, hp.data(), hp.size() * sizeof(Patch), cudaMemcpyHostToDevice, c->s_compute);
+            if (e == cudaSuccess) {
+                LaunchTimer t(c, BDF_K_CSV, -1, (int64_t)hp.size(), (int64_t)hp.size() * 32);
+                e = launch_csv_scatter(patches, (long long)hp.size(), c->s_compute);
+            }
+            if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // hp is read by the copy
+            if (e != cudaSuccess) st = fail_cuda(e, "CSV exact rounding");
+        }
+    }
+    for (int i = 0; i < n_cols && st == BDF_OK; i++) {
+        bdf_col* col = res[(size_t)i];
+        col->counts_on_device = true;
+        st = fetch_counts(c, col);
+        if (st != BDF_OK) break;
+        for (size_t j = 0; j < col->chunks.size(); j++)
+            if (col->null_counts[j] == 0) col->chunks[j].validity = nullptr;   // no bitmap in a chunk without nulls
+        e = finish_single_group(c, col);
+        if (e != cudaSuccess) st = fail_cuda(e, "CSV read");
+    }
+    for (void* p : {(void*)descs, (void*)small, slow, patches})
+        if (p) cudaFreeAsync(p, c->s_compute);
+    if (st != BDF_OK) {
+        const std::string keep = g_err;
+        cudaGetLastError();
+        for (bdf_col* col : res) col_release(c, col);
+        g_err = keep;
+        return st;
+    }
+    f->exact_fields = n_slow;
+    for (int i = 0; i < n_cols; i++) out[i] = res[(size_t)i];
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Multi-GPU context (bdf_init_multi): ONE process, every GPU of the box.  The library owns the sharding that the
 // reference leaves to rayon (par_iter over chunks, src/functions/scalar.rs:28-31,99-102): the rows of a call are cut into
 // one contiguous range per GPU (cuts on 64-row boundaries inside a chunk, so a piece is a zero-copy Arrow slice whose
@@ -3446,6 +3876,50 @@ int bdf_join_indices_dev(bdf_ctx* c, int32_t join_type, int32_t n_keys, const bd
     ENTER(c);
     if (!left_indices || !right_indices) return fail(BDF_INVALID, "null argument");
     return join_dev(c, join_type, n_keys, left_keys, right_keys, left_indices, right_indices, n_rows);
+}
+
+int bdf_csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* options, int32_t n_schema, const int32_t* schema_dtypes, bdf_csv** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the CSV reader reads into one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return csv_open(c, path, options, n_schema, schema_dtypes, out);
+}
+
+int bdf_csv_describe(const bdf_csv* f, int32_t* n_columns, int64_t* n_batches, int64_t* n_rows) {
+    if (!f) return fail(BDF_INVALID, "null file");
+    if (n_columns) *n_columns = (int32_t)f->k;
+    if (n_batches) *n_batches = (f->n_rows + f->batch - 1) / f->batch;
+    if (n_rows) *n_rows = f->n_rows;
+    return BDF_OK;
+}
+
+int bdf_csv_column(const bdf_csv* f, int32_t col, const char** name, int32_t* dtype, int32_t* nullable) {
+    if (!f) return fail(BDF_INVALID, "null file");
+    if (col < 0 || col >= (int32_t)f->k) return fail(BDF_INVALID, "column %d out of range", col);
+    if (name) *name = f->names[(size_t)col].c_str();
+    if (dtype) *dtype = f->dtypes[(size_t)col];
+    if (nullable) *nullable = f->nullable[(size_t)col];
+    return BDF_OK;
+}
+
+int bdf_csv_read(bdf_ctx* c, const bdf_csv* f, int32_t n_cols, const int32_t* cols, bdf_col** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the CSV reader reads into one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return csv_read(c, f, n_cols, cols, out);
+}
+
+int bdf_csv_stats(const bdf_csv* f, int64_t* n_fields, int64_t* exact_fields, double* upload_ms) {
+    if (!f) return fail(BDF_INVALID, "null file");
+    if (n_fields) *n_fields = f->n_fields;
+    if (exact_fields) *exact_fields = f->exact_fields;
+    if (upload_ms) *upload_ms = f->upload_ms;
+    return BDF_OK;
+}
+
+void bdf_csv_close(bdf_ctx* c, bdf_csv* f) {
+    if (!c || !f || c->fleet) return;
+    std::lock_guard<std::mutex> lock(c->mu);
+    cudaSetDevice(c->device);
+    csv_free(c, f);
 }
 
 int bdf_take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, bdf_col** out) {

@@ -35,6 +35,7 @@ import numpy as np
 from . import _native as N
 from .arrays import F32, F64, I8, I64, U8, U32, U64, PrimitiveArray, is_float
 from .functions import Column, _expr_nodes, eval_expr, sort_indices
+from .csv_reader import CsvFile
 from .ipc import BOOL, IpcFile, write_ipc
 
 ARITH = {"add": N.ADD, "subtract": N.SUB, "multiply": N.MUL, "divide": N.DIV}
@@ -341,6 +342,18 @@ class DeviceFrame:
         with IpcFile(path) as f:
             names = [n for n, dt, _ in f.schema if dt >= 0 and (columns is None or n in columns)]
             cols = f.read(names, ctx=ctx)
+        return cls(OrderedDict((n, cols[n]) for n in names))
+
+    @classmethod
+    def from_csv(cls, path: str, has_header: bool = True, delimiter: str = ",", max_records: Optional[int] = None, batch_size: int = 1024,
+                 schema: Optional[Sequence[int]] = None, columns: Optional[Sequence[str]] = None,
+                 ctx: Optional[N.Context] = None) -> "DeviceFrame":
+        """DataFrame::from_csv(path, None) with the defaults: a header, ',' and a schema inferred from every record, 1024 rows per
+        RecordBatch.  Utf8 columns are not on the device path and are left out (read them on the CPU)."""
+        with CsvFile(path, has_header=has_header, delimiter=delimiter, max_records=max_records, batch_size=batch_size, schema=schema,
+                     ctx=ctx) as f:
+            names = [n for n, dt, _ in f.schema if dt >= 0 and (columns is None or n in columns)]
+            cols = f.read(names)
         return cls(OrderedDict((n, cols[n]) for n in names))
 
     @classmethod
