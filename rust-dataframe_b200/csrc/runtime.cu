@@ -63,7 +63,9 @@ static int cuda_status(cudaError_t e) { return e == cudaErrorMemoryAllocation ? 
 // Set by the communicator layer (comm.cu reports NCCL failures as text + cudaErrorUnknown): turns the next
 // fail_cuda into BDF_NCCL.
 static thread_local std::string g_nccl_err;
+// Reports a failed CUDA call and clears the runtime's last error, so that the next call does not see it again.
 static int fail_cuda(cudaError_t e, const char* what) {
+    cudaGetLastError();
     if (!g_nccl_err.empty()) {
         const std::string m = g_nccl_err;
         g_nccl_err.clear();
@@ -75,8 +77,10 @@ static int fail_cuda(cudaError_t e, const char* what) {
 #define CK(call)                                                                                       \
     do {                                                                                               \
         cudaError_t _e = (call);                                                                       \
-        if (_e != cudaSuccess)                                                                         \
+        if (_e != cudaSuccess) {                                                                       \
+            cudaGetLastError();                                                                        \
             return fail(cuda_status(_e), "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
+        }                                                                                              \
     } while (0)
 
 #define TRY(expr)                  \
@@ -360,6 +364,61 @@ static void col_release(bdf_ctx* c, bdf_col* col) {
     col_destroy_host(c, col);
 }
 
+// What an owner does with an object it still holds.  No drop writes g_err, so after a failure the caller reads the error of
+// the step that failed.
+static void drop(bdf_ctx* c, bdf_col* col) { col_release(c, col); }
+static void drop(bdf_ctx* c, bdf_future* f) {   // its event goes back to the pool
+    ev_put(c, f->ev);
+    delete f;
+}
+
+// Owns what an operator body made until the body hands it to its caller with release(); every other exit drops it.
+template <class T>
+class Owned {
+  public:
+    explicit Owned(bdf_ctx* c, T* p = nullptr) : c_(c), p_(p) {}
+    Owned(Owned&& o) noexcept : c_(o.c_), p_(o.release()) {}
+    Owned& operator=(Owned&& o) noexcept {
+        if (this != &o) {
+            if (p_) drop(c_, p_);
+            c_ = o.c_;
+            p_ = o.release();
+        }
+        return *this;
+    }
+    ~Owned() { if (p_) drop(c_, p_); }
+    T* get() const { return p_; }
+    T* operator->() const { return p_; }
+    T** out() { return &p_; }   // where a maker writes the object: only on an empty owner
+    T* release() { T* p = p_; p_ = nullptr; return p; }
+
+  private:
+    bdf_ctx* c_;
+    T* p_;
+};
+using ColOwner = Owned<bdf_col>;
+using FutOwner = Owned<bdf_future>;
+
+// One stream-ordered allocation on the compute stream, freed in the same stream order when the scope ends.
+template <class T>
+class Scratch {
+  public:
+    Scratch() = default;
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    ~Scratch() { if (p_) cudaFreeAsync(p_, c_->s_compute); }
+    cudaError_t alloc(bdf_ctx* c, size_t bytes) {
+        c_ = c;
+        return cudaMallocAsync((void**)&p_, bytes, c->s_compute);
+    }
+    T* get() const { return p_; }
+    operator T*() const { return p_; }
+
+  private:
+    bdf_ctx* c_ = nullptr;
+    T* p_ = nullptr;
+};
+
 struct ChunkPlan {
     int64_t len;
     bool has_validity;
@@ -636,22 +695,21 @@ struct UploadSpec {
 
 // Upload K columns with their chunks interleaved (a0,b0,a1,b1,...) so that a binary operator can start on
 // chunk i as soon as BOTH of its inputs have landed.
-static int upload_many(bdf_ctx* c, const std::vector<UploadSpec>& specs, bool async, std::vector<bdf_col*>& cols) {
-    cols.assign(specs.size(), nullptr);
+static int upload_many(bdf_ctx* c, const std::vector<UploadSpec>& specs, bool async, std::vector<bdf_col*>& out) {
     int64_t max_n = 0;
-    auto cleanup = [&]() { for (auto*& col : cols) { col_release(c, col); col = nullptr; } };
+    std::vector<ColOwner> cols;
     for (size_t k = 0; k < specs.size(); k++) {
         const UploadSpec& s = specs[k];
         std::vector<ChunkPlan> plan((size_t)s.n);
         std::vector<int32_t> offs((size_t)s.n);
         for (int64_t i = 0; i < s.n; i++) {
             const bdf_view& v = s.views[i];
-            if (v.len < 0 || v.offset < 0 || (v.len > 0 && !v.values)) { cleanup(); return fail(BDF_INVALID, "bad view %lld", (long long)i); }
+            if (v.len < 0 || v.offset < 0 || (v.len > 0 && !v.values)) return fail(BDF_INVALID, "bad view %lld", (long long)i);
             plan[i] = {v.len, v.validity != nullptr};
             offs[i] = (int32_t)(v.offset & 7);
         }
-        int st = col_alloc(c, s.dtype, plan, &offs, 0, &cols[k]);
-        if (st != BDF_OK) { cleanup(); return st; }
+        cols.emplace_back(c);
+        TRY(col_alloc(c, s.dtype, plan, &offs, 0, cols[k].out()));
         for (int64_t i = 0; i < s.n; i++)
             cols[k]->null_counts[i] = s.views[i].validity ? (s.views[i].null_count >= 0 ? s.views[i].null_count : -1) : 0;
         max_n = std::max(max_n, s.n);
@@ -692,11 +750,12 @@ static int upload_many(bdf_ctx* c, const std::vector<UploadSpec>& specs, bool as
     }
     if (e == cudaSuccess && !async) e = cudaStreamSynchronize(c->s_h2d);
     if (e != cudaSuccess) {
-        cudaGetLastError();
-        cudaStreamSynchronize(c->s_h2d);
-        cleanup();
-        return fail(cuda_status(e), "upload failed: %s", cudaGetErrorString(e));
+        const int st = fail_cuda(e, "upload");
+        cudaStreamSynchronize(c->s_h2d);   // no copy may still write into the columns when they are freed
+        return st;
     }
+    out.clear();
+    for (ColOwner& col : cols) out.push_back(col.release());
     return BDF_OK;
 }
 
@@ -708,11 +767,10 @@ static int download_enqueue(bdf_ctx* c, bdf_col* col, bdf_out* out) {
     bool misaligned = false;
     for (auto& ch : col->chunks) misaligned = misaligned || (ch.validity && ch.bit_off != 0) || ch.val_bit_off != 0;
     if (misaligned) {  // an uploaded slice downloaded as-is: shift its bitmap to offset 0 first
-        bdf_col* tmp = nullptr;
-        TRY(realign(c, col, &tmp));
-        int st = download_enqueue(c, tmp, out);
-        if (st != BDF_OK) { col_release(c, tmp); return st; }
-        col->dl_tmp = tmp;
+        ColOwner tmp(c);
+        TRY(realign(c, col, tmp.out()));
+        TRY(download_enqueue(c, tmp.get(), out));
+        col->dl_tmp = tmp.release();
         return BDF_OK;
     }
     const int w = dtype_width(col->dtype);
@@ -832,31 +890,29 @@ static int binary_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bd
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++)
         plan[i] = {l->chunks[i].len, op > BDF_DIV || l->chunks[i].validity || r->chunks[i].validity};
-    bdf_col* o = nullptr;
+    ColOwner o(c);
     const int tile = elems_per_tile_binary(op, dtype);
-    TRY(col_alloc(c, dtype, plan, nullptr, tile, &o));
+    TRY(col_alloc(c, dtype, plan, nullptr, tile, o.out()));
     o->counts_on_device = o->d_warp_counts != nullptr;
 
     const int w = dtype_width(dtype);
     void *hp = nullptr, *dp = nullptr;
-    int st = ring_alloc(c, (size_t)n * sizeof(BinDesc), &hp, &dp);
+    TRY(ring_alloc(c, (size_t)n * sizeof(BinDesc), &hp, &dp));
     BinDesc* dd = (BinDesc*)dp;
     cudaError_t e = cudaSuccess;
     // K5: aggregate of the output fused into the same pass -> one partial per tile, folded by k_finish
     AggDev* partials = nullptr;
     bdf_ctx::PartBuf* pb = nullptr;
     int64_t total_tiles = 0, tile_base = 0;
-    bdf_future* f = nullptr;
-    if (fut && st == BDF_OK) {
-        if (op > BDF_DIV) { col_release(c, o); return fail(BDF_UNSUPPORTED, "fused aggregate is available for add/subtract/multiply/divide"); }
+    FutOwner f(c);
+    if (fut) {
+        if (op > BDF_DIV) return fail(BDF_UNSUPPORTED, "fused aggregate is available for add/subtract/multiply/divide");
         for (int64_t i = 0; i < n; i++) total_tiles += (l->chunks[i].len + tile - 1) / tile;
-        st = future_new(c, dtype, 1, o->total_len, &f);
-        if (st == BDF_OK) {
-            e = part_acquire(c, total_tiles, &pb);
-            partials = pb->p;
-        }
+        TRY(future_new(c, dtype, 1, o->total_len, f.out()));
+        e = part_acquire(c, total_tiles, &pb);
+        partials = pb->p;
     }
-    if (st == BDF_OK && e == cudaSuccess) {
+    if (e == cudaSuccess) {
         BinDesc* hd = (BinDesc*)hp;
         const std::vector<int64_t> ends = plan_groups(n, {l, r});
         if (op == BDF_DIV) e = cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute);
@@ -889,15 +945,15 @@ static int binary_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bd
             begin = end;
             tile_base += tiles;
         }
-        if (e == cudaSuccess && f) {
+        if (e == cudaSuccess && f.get()) {
             // fold the per-tile partials on the finish stream: the next operator on the compute stream does not wait
             c->launches++;
             for (auto& g : o->groups) cudaStreamWaitEvent(c->s_fin, g.ev, 0);
-            e = launch_finish(dtype_is_float(dtype), partials, total_tiles, c->sm_count, c->d_stage, c->d_ticket + 1, future_target(c, f, 0), c->s_fin);
+            e = launch_finish(dtype_is_float(dtype), partials, total_tiles, c->sm_count, c->d_stage, c->d_ticket + 1, future_target(c, f.get(), 0), c->s_fin);
             if (e == cudaSuccess) e = cudaEventRecord(pb->done, c->s_fin);
             pb->used = true;
             f->chunks[0] = (uint32_t)n;
-            if (e == cudaSuccess) e = future_combine(c, f, c->s_fin);   // ranks of a communicator: one grouped NCCL reduction
+            if (e == cudaSuccess) e = future_combine(c, f.get(), c->s_fin);   // ranks of a communicator: one grouped NCCL reduction
             if (e == cudaSuccess) e = cudaEventRecord(f->ev, c->s_fin);
         }
         if (e == cudaSuccess && op == BDF_DIV) {
@@ -905,21 +961,12 @@ static int binary_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bd
             if (is_global(c)) e = flag_allreduce(c);
             if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
             if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-            if (e == cudaSuccess && *c->h_flag) {
-                col_release(c, o);
-                if (f) { ev_put(c, f->ev); delete f; }
-                return fail(BDF_DIVIDE_BY_ZERO, "Divide by zero error");
-            }
+            if (e == cudaSuccess && *c->h_flag) return fail(BDF_DIVIDE_BY_ZERO, "Divide by zero error");
         }
     }
-    if (st != BDF_OK || e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        if (f) { ev_put(c, f->ev); delete f; }
-        return st != BDF_OK ? st : fail_cuda(e, "binary op");
-    }
-    *out = o;
-    if (fut) *fut = f;
+    if (e != cudaSuccess) return fail_cuda(e, "binary op");
+    *out = o.release();
+    if (fut) *fut = f.release();
     return BDF_OK;
 }
 
@@ -944,54 +991,48 @@ static int map_dev(bdf_ctx* c, bool is_cast, int op_or_to, const bdf_col* in, bd
     const bool fallible = is_cast && cast_is_fallible(from, to);
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++) plan[i] = {in->chunks[i].len, in->chunks[i].validity != nullptr || fallible};
-    bdf_col* o = nullptr;
+    ColOwner o(c);
     const int tile = is_cast ? elems_per_tile_cast(from, to) : elems_per_tile_unary(op_or_to, from);
-    TRY(col_alloc(c, to, plan, nullptr, tile, &o));
+    TRY(col_alloc(c, to, plan, nullptr, tile, o.out()));
     o->counts_on_device = o->d_warp_counts != nullptr;
 
     const int wf = dtype_width(from), wt = dtype_width(to);
     void *hp = nullptr, *dp = nullptr;
-    int st = ring_alloc(c, (size_t)n * sizeof(UnDesc), &hp, &dp);
+    TRY(ring_alloc(c, (size_t)n * sizeof(UnDesc), &hp, &dp));
     UnDesc* dd = (UnDesc*)dp;
     cudaError_t e = cudaSuccess;
-    if (st == BDF_OK) {
-        UnDesc* hd = (UnDesc*)hp;
-        const std::vector<int64_t> ends = plan_groups(n, {in});
-        int64_t begin = 0;
-        for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
-            const int64_t end = ends[gi];
-            int64_t tiles = 0, rows = 0, bytes = 0;
-            for (int64_t i = begin; i < end; i++) {
-                const DevChunk &a = in->chunks[i], &oc = o->chunks[i];
-                hd[i] = UnDesc{a.values, oc.values, a.validity, oc.validity, a.len, tiles, a.bit_off, 0};
-                tiles += (a.len + tile - 1) / tile;
-                rows += a.len;
-                bytes += a.len * (wf + wt) + ((a.validity ? 1 : 0) + (oc.validity ? 1 : 0)) * bitmap_bytes(a.len);
-            }
-            wait_groups(c->s_compute, in, begin, end);
-            if (end > begin) {
-                e = desc_upload(c, dd + begin, hd + begin, (size_t)(end - begin) * sizeof(UnDesc));
-                if (e == cudaSuccess) {
-                    LaunchTimer t(c, is_cast ? BDF_K_CAST : BDF_K_UNARY, to, rows, bytes);
-                    e = is_cast ? launch_cast(from, to, dd + begin, (int)(end - begin), tiles, o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute)
-                                : launch_unary(op_or_to, from, dd + begin, (int)(end - begin), tiles, o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute);
-                }
-            }
-            if (e == cudaSuccess) {
-                Group g{begin, end, nullptr};
-                e = ev_get(c, &g.ev);
-                if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
-                o->groups.push_back(g);
-            }
-            begin = end;
+    UnDesc* hd = (UnDesc*)hp;
+    const std::vector<int64_t> ends = plan_groups(n, {in});
+    int64_t begin = 0;
+    for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
+        const int64_t end = ends[gi];
+        int64_t tiles = 0, rows = 0, bytes = 0;
+        for (int64_t i = begin; i < end; i++) {
+            const DevChunk &a = in->chunks[i], &oc = o->chunks[i];
+            hd[i] = UnDesc{a.values, oc.values, a.validity, oc.validity, a.len, tiles, a.bit_off, 0};
+            tiles += (a.len + tile - 1) / tile;
+            rows += a.len;
+            bytes += a.len * (wf + wt) + ((a.validity ? 1 : 0) + (oc.validity ? 1 : 0)) * bitmap_bytes(a.len);
         }
+        wait_groups(c->s_compute, in, begin, end);
+        if (end > begin) {
+            e = desc_upload(c, dd + begin, hd + begin, (size_t)(end - begin) * sizeof(UnDesc));
+            if (e == cudaSuccess) {
+                LaunchTimer t(c, is_cast ? BDF_K_CAST : BDF_K_UNARY, to, rows, bytes);
+                e = is_cast ? launch_cast(from, to, dd + begin, (int)(end - begin), tiles, o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute)
+                            : launch_unary(op_or_to, from, dd + begin, (int)(end - begin), tiles, o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute);
+            }
+        }
+        if (e == cudaSuccess) {
+            Group g{begin, end, nullptr};
+            e = ev_get(c, &g.ev);
+            if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
+            o->groups.push_back(g);
+        }
+        begin = end;
     }
-    if (st != BDF_OK || e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        return st != BDF_OK ? st : fail(cuda_status(e), "%s failed: %s", is_cast ? "cast" : "unary op", cudaGetErrorString(e));
-    }
-    *out = o;
+    if (e != cudaSuccess) return fail_cuda(e, is_cast ? "cast" : "unary op");
+    *out = o.release();
     return BDF_OK;
 }
 
@@ -1020,7 +1061,7 @@ static int future_new(bdf_ctx* c, int dtype, int fused, int64_t rows, bdf_future
         c->local_next += n;
     }
     cudaError_t e = ev_get(c, &f->ev);
-    if (e != cudaSuccess) { delete f; return fail(cuda_status(e), "event creation failed: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) { delete f; return fail_cuda(e, "event creation"); }
     *out = f;
     return BDF_OK;
 }
@@ -1160,25 +1201,20 @@ static int aggregate_many_dev_async(bdf_ctx* c, int n_cols, bdf_col* const* cols
     std::vector<uint32_t> panics((size_t)n_cols, 0u);
     if (need_counts)
         for (int k = 0; k < n_cols; k++) TRY(count_panic_chunks(c, cols[k], &panics[k]));
-    bdf_future* f = nullptr;
-    TRY(future_new(c, cols[0]->dtype, 2, 0, &f, n_cols));
-    int st = BDF_OK;
+    FutOwner f(c);
+    TRY(future_new(c, cols[0]->dtype, 2, 0, f.out(), n_cols));
     for (int k = 0; k < n_cols; k++) {
         bdf_col* col = cols[k];
         const int64_t n = (int64_t)col->chunks.size();
         f->dtypes[k] = col->dtype; f->rows[k] = col->total_len; f->panics[k] = panics[k]; f->chunks[k] = (uint32_t)n;
         wait_groups(c->s_compute, col, 0, n);
     }
-    if (n_cols == 1) st = reduce_range(c, cols[0], 0, (int64_t)cols[0]->chunks.size(), future_target(c, f, 0));
-    else st = reduce_columns(c, n_cols, cols, f);
-    cudaError_t e = cudaSuccess;
-    if (st == BDF_OK) e = future_combine(c, f, c->s_compute);
-    if (st == BDF_OK && e == cudaSuccess) e = cudaEventRecord(f->ev, c->s_compute);
-    if (st != BDF_OK || e != cudaSuccess) {
-        ev_put(c, f->ev); delete f;
-        return st != BDF_OK ? st : fail_cuda(e, "aggregate");
-    }
-    *fut = f;
+    if (n_cols == 1) TRY(reduce_range(c, cols[0], 0, (int64_t)cols[0]->chunks.size(), future_target(c, f.get(), 0)));
+    else TRY(reduce_columns(c, n_cols, cols, f.get()));
+    cudaError_t e = future_combine(c, f.get(), c->s_compute);
+    if (e == cudaSuccess) e = cudaEventRecord(f->ev, c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "aggregate");
+    *fut = f.release();
     return BDF_OK;
 }
 
@@ -1202,8 +1238,7 @@ static int future_wait(bdf_ctx* c, bdf_future* f, bdf_agg4* out) {
                 out[i].n_chunks = (int64_t)f->chunks[i];
             }
         }
-    ev_put(c, f->ev);
-    delete f;
+    drop(c, f);
     if (e != cudaSuccess) return fail(cuda_status(e), "waiting for an aggregate failed: %s", cudaGetErrorString(e));
     return BDF_OK;
 }
@@ -1333,54 +1368,45 @@ static cudaError_t finish_single_group(bdf_ctx* c, bdf_col* o) {
     return e;
 }
 
-// BooleanFilter::{Gt,..,Le}: cast both sides to Float64 (as the reference does, expression.rs:820-845), compare.
+// BooleanFilter::{Gt,..,Le}: cast both sides to Float64 (as the reference does, expression.rs:820-845), compare.  The casts are
+// fused into the kernel's loads.
 static int compare_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, double scalar, bdf_col** out) {
     if (op < 0 || op > 5) return fail(BDF_INVALID, "invalid comparison op %d", op);
     if (l->dtype == kBool || (r && r->dtype == kBool)) return fail(BDF_UNSUPPORTED, "comparison of boolean columns is not part of this path");
-    auto cleanup = [] {};  // (the Float64 casts of the reference are fused into the kernel's loads)
     const int64_t n = r ? std::min<int64_t>((int64_t)l->chunks.size(), (int64_t)r->chunks.size()) : (int64_t)l->chunks.size();
     for (int64_t i = 0; r && i < n; i++)
-        if (l->chunks[i].len != r->chunks[i].len) { cleanup(); return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length"); }
+        if (l->chunks[i].len != r->chunks[i].len) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++) plan[i] = {l->chunks[i].len, l->chunks[i].validity != nullptr || (r && r->chunks[i].validity != nullptr)};
     const int tile = compare_tile_elems();
-    bdf_col* o = nullptr;
-    int st = col_alloc(c, kBool, plan, nullptr, tile, &o);
-    if (st != BDF_OK) { cleanup(); return st; }
+    ColOwner o(c);
+    TRY(col_alloc(c, kBool, plan, nullptr, tile, o.out()));
     o->counts_on_device = o->d_warp_counts != nullptr;
     void *hp = nullptr, *dp = nullptr;
-    st = ring_alloc(c, (size_t)n * sizeof(BinDesc), &hp, &dp);
-    cudaError_t e = cudaSuccess;
-    if (st == BDF_OK) {
-        BinDesc* hd = (BinDesc*)hp;
-        int64_t tiles = 0, rows = 0, bytes = 0;
-        for (int64_t i = 0; i < n; i++) {
-            const DevChunk& a = l->chunks[i];
-            const DevChunk* b = r ? &r->chunks[i] : nullptr;
-            const DevChunk& oc = o->chunks[i];
-            hd[i] = BinDesc{a.values, b ? b->values : nullptr, oc.values, a.validity, b ? b->validity : nullptr, oc.validity, a.len, tiles,
-                            a.bit_off, b ? b->bit_off : 0};
-            tiles += (a.len + tile - 1) / tile;
-            rows += a.len;
-            bytes += (dtype_width(l->dtype) + (b ? dtype_width(r->dtype) : 0)) * a.len +
-                     bitmap_bytes(a.len) * (1 + (a.validity ? 1 : 0) + (b && b->validity ? 1 : 0) + (oc.validity ? 1 : 0));
-        }
-        wait_groups(c->s_compute, l, 0, n);
-        if (r) wait_groups(c->s_compute, r, 0, n);
-        e = desc_upload(c, dp, hd, (size_t)n * sizeof(BinDesc));
-        if (e == cudaSuccess) {
-            LaunchTimer t(c, BDF_K_COMPARE, kBool, rows, bytes);
-            e = launch_compare(op, (const BinDesc*)dp, (int)n, tiles, l->dtype, r ? r->dtype : BDF_F64, r == nullptr, scalar, o->d_warp_counts, c->s_compute);
-        }
-        if (e == cudaSuccess) e = finish_single_group(c, o);
+    TRY(ring_alloc(c, (size_t)n * sizeof(BinDesc), &hp, &dp));
+    BinDesc* hd = (BinDesc*)hp;
+    int64_t tiles = 0, rows = 0, bytes = 0;
+    for (int64_t i = 0; i < n; i++) {
+        const DevChunk& a = l->chunks[i];
+        const DevChunk* b = r ? &r->chunks[i] : nullptr;
+        const DevChunk& oc = o->chunks[i];
+        hd[i] = BinDesc{a.values, b ? b->values : nullptr, oc.values, a.validity, b ? b->validity : nullptr, oc.validity, a.len, tiles,
+                        a.bit_off, b ? b->bit_off : 0};
+        tiles += (a.len + tile - 1) / tile;
+        rows += a.len;
+        bytes += (dtype_width(l->dtype) + (b ? dtype_width(r->dtype) : 0)) * a.len +
+                 bitmap_bytes(a.len) * (1 + (a.validity ? 1 : 0) + (b && b->validity ? 1 : 0) + (oc.validity ? 1 : 0));
     }
-    cleanup();
-    if (st != BDF_OK || e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        return st != BDF_OK ? st : fail(cuda_status(e), "compare failed: %s", cudaGetErrorString(e));
+    wait_groups(c->s_compute, l, 0, n);
+    if (r) wait_groups(c->s_compute, r, 0, n);
+    cudaError_t e = desc_upload(c, dp, hd, (size_t)n * sizeof(BinDesc));
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_COMPARE, kBool, rows, bytes);
+        e = launch_compare(op, (const BinDesc*)dp, (int)n, tiles, l->dtype, r ? r->dtype : BDF_F64, r == nullptr, scalar, o->d_warp_counts, c->s_compute);
     }
-    *out = o;
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "compare");
+    *out = o.release();
     return BDF_OK;
 }
 
@@ -1394,38 +1420,31 @@ static int boolean_dev(bdf_ctx* c, int op, const bdf_col* a, const bdf_col* b, b
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++) plan[i] = {a->chunks[i].len, a->chunks[i].validity != nullptr || (b && b->chunks[i].validity != nullptr)};
     const int tile = bool_tile_elems();
-    bdf_col* o = nullptr;
-    TRY(col_alloc(c, kBool, plan, nullptr, tile, &o));
+    ColOwner o(c);
+    TRY(col_alloc(c, kBool, plan, nullptr, tile, o.out()));
     o->counts_on_device = o->d_warp_counts != nullptr;
     void *hp = nullptr, *dp = nullptr;
-    int st = ring_alloc(c, (size_t)n * bool_desc_size(), &hp, &dp);
-    cudaError_t e = cudaSuccess;
-    if (st == BDF_OK) {
-        int64_t tiles = 0, rows = 0;
-        for (int64_t i = 0; i < n; i++) {
-            const DevChunk& x = a->chunks[i];
-            const DevChunk* y = b ? &b->chunks[i] : nullptr;
-            const DevChunk& oc = o->chunks[i];
-            fill_bool_desc(hp, i, (const uint32_t*)x.values, y ? (const uint32_t*)y->values : nullptr, (uint32_t*)oc.values, x.validity,
-                           y ? y->validity : nullptr, oc.validity, x.len, tiles, x.val_bit_off, y ? y->val_bit_off : 0, x.bit_off, y ? y->bit_off : 0);
-            tiles += (x.len + tile - 1) / tile;
-            rows += x.len;
-        }
-        wait_groups(c->s_compute, a, 0, n);
-        if (b) wait_groups(c->s_compute, b, 0, n);
-        e = desc_upload(c, dp, hp, (size_t)n * bool_desc_size());
-        if (e == cudaSuccess) {
-            LaunchTimer t(c, BDF_K_COMPARE, kBool, rows, rows / 8 * (b ? 3 : 2));
-            e = launch_boolean(op, dp, (int)n, tiles, o->d_warp_counts, c->s_compute);
-        }
-        if (e == cudaSuccess) e = finish_single_group(c, o);
+    TRY(ring_alloc(c, (size_t)n * bool_desc_size(), &hp, &dp));
+    int64_t tiles = 0, rows = 0;
+    for (int64_t i = 0; i < n; i++) {
+        const DevChunk& x = a->chunks[i];
+        const DevChunk* y = b ? &b->chunks[i] : nullptr;
+        const DevChunk& oc = o->chunks[i];
+        fill_bool_desc(hp, i, (const uint32_t*)x.values, y ? (const uint32_t*)y->values : nullptr, (uint32_t*)oc.values, x.validity,
+                       y ? y->validity : nullptr, oc.validity, x.len, tiles, x.val_bit_off, y ? y->val_bit_off : 0, x.bit_off, y ? y->bit_off : 0);
+        tiles += (x.len + tile - 1) / tile;
+        rows += x.len;
     }
-    if (st != BDF_OK || e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        return st != BDF_OK ? st : fail(cuda_status(e), "boolean op failed: %s", cudaGetErrorString(e));
+    wait_groups(c->s_compute, a, 0, n);
+    if (b) wait_groups(c->s_compute, b, 0, n);
+    cudaError_t e = desc_upload(c, dp, hp, (size_t)n * bool_desc_size());
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_COMPARE, kBool, rows, rows / 8 * (b ? 3 : 2));
+        e = launch_boolean(op, dp, (int)n, tiles, o->d_warp_counts, c->s_compute);
     }
-    *out = o;
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "boolean op");
+    *out = o.release();
     return BDF_OK;
 }
 
@@ -1444,22 +1463,12 @@ static int filter_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* mask, bd
     for (int64_t i = 0; i < n; i++) { tile0[i] = tiles; tiles += (values->chunks[i].len + tile - 1) / tile; rows += values->chunks[i].len; }
     void *hp = nullptr, *dp = nullptr;
     TRY(ring_alloc(c, (size_t)n * filter_desc_size(), &hp, &dp));
-    unsigned int* d_counts = nullptr; long long *d_offsets = nullptr, *d_totals = nullptr;
-    auto free_scratch = [&]() {
-        if (d_counts) cudaFreeAsync(d_counts, c->s_compute);
-        if (d_offsets) cudaFreeAsync(d_offsets, c->s_compute);
-        if (d_totals) cudaFreeAsync(d_totals, c->s_compute);
-    };
-    {   // three scratch arrays; a failure part-way frees what was already obtained
-        cudaError_t ea = cudaMallocAsync((void**)&d_counts, std::max<size_t>(1, (size_t)tiles) * sizeof(unsigned int), c->s_compute);
-        if (ea == cudaSuccess) ea = cudaMallocAsync((void**)&d_offsets, std::max<size_t>(1, (size_t)tiles) * sizeof(long long), c->s_compute);
-        if (ea == cudaSuccess) ea = cudaMallocAsync((void**)&d_totals, std::max<size_t>(1, (size_t)n) * sizeof(long long), c->s_compute);
-        if (ea != cudaSuccess) {
-            cudaGetLastError();
-            free_scratch();
-            return fail(cuda_status(ea), "filter scratch allocation failed: %s", cudaGetErrorString(ea));
-        }
-    }
+    Scratch<unsigned int> d_counts;
+    Scratch<long long> d_offsets, d_totals;
+    cudaError_t e = d_counts.alloc(c, std::max<size_t>(1, (size_t)tiles) * sizeof(unsigned int));
+    if (e == cudaSuccess) e = d_offsets.alloc(c, std::max<size_t>(1, (size_t)tiles) * sizeof(long long));
+    if (e == cudaSuccess) e = d_totals.alloc(c, std::max<size_t>(1, (size_t)n) * sizeof(long long));
+    if (e != cudaSuccess) return fail_cuda(e, "filter scratch allocation");
     // pass 1: counts + scan (output pointers are not needed yet)
     for (int64_t i = 0; i < n; i++) {
         const DevChunk &v = values->chunks[i], &m = mask->chunks[i];
@@ -1467,7 +1476,7 @@ static int filter_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* mask, bd
     }
     wait_groups(c->s_compute, values, 0, n);
     wait_groups(c->s_compute, mask, 0, n);
-    cudaError_t e = desc_upload(c, dp, hp, (size_t)n * filter_desc_size());
+    e = desc_upload(c, dp, hp, (size_t)n * filter_desc_size());
     std::vector<long long> totals((size_t)std::max<int64_t>(n, 1), 0);
     if (e == cudaSuccess) {
         LaunchTimer t(c, BDF_K_FILTER, dtype, rows, rows / 4);
@@ -1476,37 +1485,29 @@ static int filter_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* mask, bd
     }
     if (e == cudaSuccess && n) e = cudaMemcpyAsync(totals.data(), d_totals, (size_t)n * sizeof(long long), cudaMemcpyDeviceToHost, c->s_compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);  // output lengths are needed to size the result
-    if (e != cudaSuccess) { cudaGetLastError(); free_scratch(); return fail(cuda_status(e), "filter (count) failed: %s", cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail_cuda(e, "filter (count)");
     std::vector<ChunkPlan> plan((size_t)n);
     int64_t kept = 0;
     for (int64_t i = 0; i < n; i++) { plan[i] = {(int64_t)totals[i], values->chunks[i].validity != nullptr}; kept += totals[i]; }
-    bdf_col* o = nullptr;
-    int st = col_alloc(c, dtype, plan, nullptr, 0, &o);
-    if (st != BDF_OK) { free_scratch(); return st; }
+    ColOwner o(c);
+    TRY(col_alloc(c, dtype, plan, nullptr, 0, o.out()));
     for (int64_t i = 0; i < n; i++) o->null_counts[i] = o->chunks[i].validity ? -1 : 0;  // counted on demand
     // pass 2: scatter
     void *hp2 = nullptr, *dp2 = nullptr;
-    st = ring_alloc(c, (size_t)n * filter_desc_size(), &hp2, &dp2);
-    if (st == BDF_OK) {
-        for (int64_t i = 0; i < n; i++) {
-            const DevChunk &v = values->chunks[i], &m = mask->chunks[i], &oc = o->chunks[i];
-            fill_filter_desc(hp2, i, v.values, oc.values, v.validity, oc.validity, (const uint32_t*)m.values, m.validity, v.len, tile0[i], v.bit_off, m.val_bit_off, m.bit_off);
-        }
-        e = desc_upload(c, dp2, hp2, (size_t)n * filter_desc_size());
-        if (e == cudaSuccess) {
-            const int w = dtype_width(dtype);
-            LaunchTimer t(c, BDF_K_FILTER, dtype, rows, rows * w + kept * w + rows / 4);
-            e = launch_filter_scatter(dtype, dp2, (int)n, tiles, d_offsets, c->s_compute);
-        }
-        if (e == cudaSuccess) e = finish_single_group(c, o);
+    TRY(ring_alloc(c, (size_t)n * filter_desc_size(), &hp2, &dp2));
+    for (int64_t i = 0; i < n; i++) {
+        const DevChunk &v = values->chunks[i], &m = mask->chunks[i], &oc = o->chunks[i];
+        fill_filter_desc(hp2, i, v.values, oc.values, v.validity, oc.validity, (const uint32_t*)m.values, m.validity, v.len, tile0[i], v.bit_off, m.val_bit_off, m.bit_off);
     }
-    free_scratch();
-    if (st != BDF_OK || e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        return st != BDF_OK ? st : fail(cuda_status(e), "filter (scatter) failed: %s", cudaGetErrorString(e));
+    e = desc_upload(c, dp2, hp2, (size_t)n * filter_desc_size());
+    if (e == cudaSuccess) {
+        const int w = dtype_width(dtype);
+        LaunchTimer t(c, BDF_K_FILTER, dtype, rows, rows * w + kept * w + rows / 4);
+        e = launch_filter_scatter(dtype, dp2, (int)n, tiles, d_offsets, c->s_compute);
     }
-    *out = o;
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "filter (scatter)");
+    *out = o.release();
     return BDF_OK;
 }
 
@@ -1583,24 +1584,24 @@ static int expr_dev(bdf_ctx* c, int n_inputs, const bdf_col* const* inputs, int 
         plan[ch] = {inputs[0]->chunks[ch].len, hv};
     }
     const int tile = expr_tile_elems();
-    bdf_col* o = nullptr;
+    ColOwner o(c);
     if (out) {
-        TRY(col_alloc(c, BDF_F64, plan, nullptr, tile, &o));
+        TRY(col_alloc(c, BDF_F64, plan, nullptr, tile, o.out()));
         o->counts_on_device = o->d_warp_counts != nullptr;
     }
     int64_t total_tiles = 0, total_rows = 0;
     for (int64_t ch = 0; ch < n; ch++) { total_tiles += (plan[ch].len + tile - 1) / tile; total_rows += plan[ch].len; }
     void *hp = nullptr, *dp = nullptr;
-    int st = ring_alloc(c, (size_t)n * expr_desc_size(), &hp, &dp);
+    TRY(ring_alloc(c, (size_t)n * expr_desc_size(), &hp, &dp));
     cudaError_t e = cudaSuccess;
-    bdf_future* f = nullptr;
+    FutOwner f(c);
     bdf_ctx::PartBuf* pb = nullptr;
-    if (fut && st == BDF_OK) {
-        st = future_new(c, BDF_F64, 1, total_rows, &f);
-        if (st == BDF_OK) e = part_acquire(c, total_tiles, &pb);
+    if (fut) {
+        TRY(future_new(c, BDF_F64, 1, total_rows, f.out()));
+        e = part_acquire(c, total_tiles, &pb);
     }
     cudaEvent_t ev_done = nullptr;   // the launch's completion on the compute stream, for the finish stream
-    if (st == BDF_OK && e == cudaSuccess) {
+    if (e == cudaSuccess) {
         int64_t tiles = 0, bytes = 0;
         for (int64_t ch = 0; ch < n; ch++) {
             const void* in[8]; const uint32_t* vin[8]; int32_t off[8];
@@ -1611,31 +1612,31 @@ static int expr_dev(bdf_ctx* c, int n_inputs, const bdf_col* const* inputs, int 
                 if ((uintptr_t)x.values & 15) e = cudaErrorMisalignedAddress;
                 bytes += (int64_t)dtype_width(inputs[i]->dtype) * x.len + (x.validity ? bitmap_bytes(x.len) : 0);
             }
-            double* po = o ? (double*)o->chunks[ch].values : nullptr;
-            uint32_t* vo = o ? o->chunks[ch].validity : nullptr;
+            double* po = o.get() ? (double*)o->chunks[ch].values : nullptr;
+            uint32_t* vo = o.get() ? o->chunks[ch].validity : nullptr;
             fill_expr_desc(hp, ch, n_inputs, in, vin, off, po, vo, len, tiles);
             tiles += (len + tile - 1) / tile;
-            if (o) bytes += 8 * len + (vo ? bitmap_bytes(len) : 0);
+            if (o.get()) bytes += 8 * len + (vo ? bitmap_bytes(len) : 0);
         }
         for (int i = 0; i < n_inputs; i++) wait_groups(c->s_compute, inputs[i], 0, n);
         if (e == cudaSuccess) e = desc_upload(c, dp, hp, (size_t)n * expr_desc_size());
         if (e == cudaSuccess && has_div) e = cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute);
         if (e == cudaSuccess) {
             LaunchTimer t(c, BDF_K_EXPR, BDF_F64, total_rows, bytes);
-            e = launch_expr(dp, (int)n, total_tiles, prog, o ? o->d_warp_counts : nullptr, c->d_flag, pb ? pb->p : nullptr, c->s_compute);
+            e = launch_expr(dp, (int)n, total_tiles, prog, o.get() ? o->d_warp_counts : nullptr, c->d_flag, pb ? pb->p : nullptr, c->s_compute);
         }
-        if (e == cudaSuccess && o) e = finish_single_group(c, o);
-        if (e == cudaSuccess && f) {
+        if (e == cudaSuccess && o.get()) e = finish_single_group(c, o.get());
+        if (e == cudaSuccess && f.get()) {
             // fold the per-tile partials on the finish stream, like K5
             c->launches++;
             e = ev_get(c, &ev_done);
             if (e == cudaSuccess) e = cudaEventRecord(ev_done, c->s_compute);
             if (e == cudaSuccess) e = cudaStreamWaitEvent(c->s_fin, ev_done, 0);
-            if (e == cudaSuccess) e = launch_finish(true, pb->p, total_tiles, c->sm_count, c->d_stage, c->d_ticket + 1, future_target(c, f, 0), c->s_fin);
+            if (e == cudaSuccess) e = launch_finish(true, pb->p, total_tiles, c->sm_count, c->d_stage, c->d_ticket + 1, future_target(c, f.get(), 0), c->s_fin);
             if (e == cudaSuccess) e = cudaEventRecord(pb->done, c->s_fin);
             pb->used = true;
             f->chunks[0] = (uint32_t)n;
-            if (e == cudaSuccess) e = future_combine(c, f, c->s_fin);
+            if (e == cudaSuccess) e = future_combine(c, f.get(), c->s_fin);
             if (e == cudaSuccess) e = cudaEventRecord(f->ev, c->s_fin);
             if (ev_done) ev_put(c, ev_done);
         }
@@ -1643,21 +1644,12 @@ static int expr_dev(bdf_ctx* c, int n_inputs, const bdf_col* const* inputs, int 
             if (is_global(c)) e = flag_allreduce(c);
             if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
             if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-            if (e == cudaSuccess && *c->h_flag) {
-                if (o) col_release(c, o);
-                if (f) { ev_put(c, f->ev); delete f; }
-                return fail(BDF_DIVIDE_BY_ZERO, "Divide by zero error");
-            }
+            if (e == cudaSuccess && *c->h_flag) return fail(BDF_DIVIDE_BY_ZERO, "Divide by zero error");
         }
     }
-    if (st != BDF_OK || e != cudaSuccess) {
-        cudaGetLastError();
-        if (o) col_release(c, o);
-        if (f) { ev_put(c, f->ev); delete f; }
-        return st != BDF_OK ? st : fail_cuda(e, "fused expression");
-    }
-    if (out) *out = o;
-    if (fut) *fut = f;
+    if (e != cudaSuccess) return fail_cuda(e, "fused expression");
+    if (out) *out = o.release();
+    if (fut) *fut = f.release();
     return BDF_OK;
 }
 
@@ -1696,7 +1688,7 @@ static int sort_table(bdf_ctx* c, const bdf_col* col, void** dev, int* n_chunks,
     if (n == 0) fill_sort_chunk(hp, 0, nullptr, nullptr, 0, 0, 0);
     wait_groups(c->s_compute, col, 0, n);
     cudaError_t e = desc_upload(c, *dev, hp, (size_t)std::max<int64_t>(n, 1) * sort_chunk_size());
-    if (e != cudaSuccess) return fail(cuda_status(e), "descriptor upload failed: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail_cuda(e, "descriptor upload");
     *n_chunks = (int)std::max<int64_t>(n, 1);
     if (nullable) *nullable = any;
     return BDF_OK;
@@ -1712,22 +1704,22 @@ static int sort_indices_dev(bdf_ctx* c, int n_keys, const bdf_sort_key* keys, bd
     }
     const int64_t n = keys[0].column->total_len;
     if (n > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
-    bdf_col* o = nullptr;
-    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, sort_tile_elems(), &o));
+    ColOwner o(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, sort_tile_elems(), o.out()));
     cudaError_t e = cudaSuccess;
     int st = BDF_OK;
-    unsigned long long* kbuf[2] = {nullptr, nullptr};
-    uint32_t* ibuf[2] = {nullptr, nullptr};
-    unsigned int* block_hist = nullptr;
-    unsigned long long* agree = nullptr;   // [0] OR, [1] AND of the keys of the current criterion
     if (n > 0) {
+        Scratch<unsigned long long> kbuf[2];
+        Scratch<uint32_t> ibuf[2];
+        Scratch<unsigned int> block_hist;
+        Scratch<unsigned long long> agree;   // [0] OR, [1] AND of the keys of the current criterion
         if (!c->h_sort_agree) e = cudaHostAlloc((void**)&c->h_sort_agree, 2 * sizeof(unsigned long long), cudaHostAllocDefault);
         for (int b = 0; b < 2 && e == cudaSuccess; b++) {
-            e = cudaMallocAsync((void**)&kbuf[b], (size_t)n * 8, c->s_compute);
-            if (e == cudaSuccess) e = cudaMallocAsync((void**)&ibuf[b], (size_t)n * 4, c->s_compute);
+            e = kbuf[b].alloc(c, (size_t)n * 8);
+            if (e == cudaSuccess) e = ibuf[b].alloc(c, (size_t)n * 4);
         }
-        if (e == cudaSuccess) e = cudaMallocAsync((void**)&block_hist, (size_t)256 * sort_pass_ctas(n, c->sm_count) * sizeof(unsigned int), c->s_compute);
-        if (e == cudaSuccess) e = cudaMallocAsync((void**)&agree, 2 * sizeof(unsigned long long), c->s_compute);
+        if (e == cudaSuccess) e = block_hist.alloc(c, (size_t)256 * sort_pass_ctas(n, c->sm_count) * sizeof(unsigned int));
+        if (e == cudaSuccess) e = agree.alloc(c, 2 * sizeof(unsigned long long));
         int cur = 0;
         int64_t passes = 0, pass_bytes = 0;
         if (e == cudaSuccess) {
@@ -1760,17 +1752,11 @@ static int sort_indices_dev(bdf_ctx* c, int n_keys, const bdf_sort_key* keys, bd
             c->last_sort_passes = passes;
         }
         if (c->profiling && !c->prof.empty() && c->prof.back().rec.kernel == BDF_K_SORT) c->prof.back().rec.bytes = 8 * n + pass_bytes + 4 * n;
-        for (int b = 0; b < 2; b++) { if (kbuf[b]) cudaFreeAsync(kbuf[b], c->s_compute); if (ibuf[b]) cudaFreeAsync(ibuf[b], c->s_compute); }
-        if (block_hist) cudaFreeAsync(block_hist, c->s_compute);
-        if (agree) cudaFreeAsync(agree, c->s_compute);
     }
-    if (e == cudaSuccess && st == BDF_OK) e = finish_single_group(c, o);
-    if (st != BDF_OK || e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        return st != BDF_OK ? st : fail(cuda_status(e), "sort failed: %s", cudaGetErrorString(e));
-    }
-    *out = o;
+    TRY(st);
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "sort");
+    *out = o.release();
     return BDF_OK;
 }
 
@@ -1782,8 +1768,8 @@ static int take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, b
     bool vnull = false, inull = false;
     TRY(sort_table(c, values, &vt, &nv, &vnull));
     TRY(sort_table(c, indices, &it, &ni, &inull));
-    bdf_col* o = nullptr;
-    TRY(col_alloc(c, values->dtype, {ChunkPlan{n, vnull || inull}}, nullptr, take_tile_elems(), &o));
+    ColOwner o(c);
+    TRY(col_alloc(c, values->dtype, {ChunkPlan{n, vnull || inull}}, nullptr, take_tile_elems(), o.out()));
     o->counts_on_device = o->d_warp_counts != nullptr;
     cudaError_t e = cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute);
     if (e == cudaSuccess) {
@@ -1791,16 +1777,12 @@ static int take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, b
         LaunchTimer t(c, BDF_K_TAKE, values->dtype, n, n * (4 + 2 * (int64_t)w));
         e = launch_take(values->dtype, vt, nv, it, ni, n, values->total_len, o->chunks[0].values, o->chunks[0].validity, o->d_warp_counts, c->d_flag, c->s_compute);
     }
-    if (e == cudaSuccess) e = finish_single_group(c, o);
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
     if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-    if (e == cudaSuccess && *c->h_flag) { col_release(c, o); return fail(BDF_INVALID, "take: index out of bounds"); }
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        return fail(cuda_status(e), "take failed: %s", cudaGetErrorString(e));
-    }
-    *out = o;
+    if (e == cudaSuccess && *c->h_flag) return fail(BDF_INVALID, "take: index out of bounds");
+    if (e != cudaSuccess) return fail_cuda(e, "take");
+    *out = o.release();
     return BDF_OK;
 }
 
@@ -1823,8 +1805,8 @@ size_t group_big_scratch_bytes(long long n_rows);
 
 // Head bitmap (a boolean column of n rows) over one-chunk columns in sorted order.
 static int group_heads(bdf_ctx* c, const std::vector<const bdf_col*>& cols, bool and_last_valid, int64_t n, bdf_col** out) {
-    bdf_col* head = nullptr;
-    TRY(col_alloc(c, kBool, {ChunkPlan{n, false}}, nullptr, 0, &head));
+    ColOwner head(c);
+    TRY(col_alloc(c, kBool, {ChunkPlan{n, false}}, nullptr, 0, head.out()));
     std::vector<const void*> vals(cols.size());
     std::vector<const uint32_t*> valid(cols.size());
     std::vector<int> widths(cols.size()), is_float(cols.size());
@@ -1838,33 +1820,65 @@ static int group_heads(bdf_ctx* c, const std::vector<const bdf_col*>& cols, bool
     c->launches++;
     cudaError_t e = launch_group_heads((int)cols.size(), vals.data(), valid.data(), widths.data(), is_float.data(), and_last_valid ? 1 : 0, n,
                                        (uint32_t*)head->chunks[0].values, c->s_compute);
-    if (e == cudaSuccess) e = finish_single_group(c, head);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, head);
-        return fail_cuda(e, "group heads");
-    }
-    *out = head;
+    if (e == cudaSuccess) e = finish_single_group(c, head.get());
+    if (e != cudaSuccess) return fail_cuda(e, "group heads");
+    *out = head.release();
     return BDF_OK;
 }
 
 // A copy of a one-chunk column made on the compute stream (the same aggregate requested twice gets two columns).
 static int group_clone(bdf_ctx* c, const bdf_col* src, bdf_col** out) {
     const DevChunk& s = src->chunks[0];
-    bdf_col* o = nullptr;
-    TRY(col_alloc(c, src->dtype, {ChunkPlan{s.len, s.validity != nullptr}}, nullptr, 0, &o));
+    ColOwner o(c);
+    TRY(col_alloc(c, src->dtype, {ChunkPlan{s.len, s.validity != nullptr}}, nullptr, 0, o.out()));
     cudaError_t e = cudaSuccess;
     if (s.len) e = cudaMemcpyAsync(o->chunks[0].values, s.values, (size_t)s.len * dtype_width(src->dtype), cudaMemcpyDeviceToDevice, c->s_compute);
     if (e == cudaSuccess && s.len && s.validity)
         e = cudaMemcpyAsync(o->chunks[0].validity, s.validity, (size_t)bitmap_bytes(s.len), cudaMemcpyDeviceToDevice, c->s_compute);
-    if (e == cudaSuccess) e = finish_single_group(c, o);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        return fail_cuda(e, "group result copy");
-    }
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "group result copy");
     o->null_counts[0] = src->null_counts[0];
-    *out = o;
+    *out = o.release();
+    return BDF_OK;
+}
+
+// The runs of equal key tuples in sorted order: group-by's groups, and the join's build side.
+struct SortedRuns {
+    explicit SortedRuns(bdf_ctx* c) : perm(c), head(c), iota(c), starts(c) {}
+    ColOwner perm;                   // the stable sort permutation (sorted position -> row)
+    std::vector<ColOwner> sorted;    // the key columns in sorted order
+    ColOwner head;                   // bit i: sorted row i starts a run
+    std::vector<ColOwner> distinct;  // the key tuple of every run
+    ColOwner iota;                   // 0, 1, .., n-1
+    ColOwner starts;                 // the first sorted row of every run
+    int64_t n_runs = 0;
+};
+
+// Sort the keys, gather them in sorted order, mark the heads, compact the distinct key tuples and the run starts.  `what` names
+// the caller's iota in a CUDA failure.
+static int sorted_runs(bdf_ctx* c, int n_keys, const bdf_col* const* keys, const char* what, SortedRuns* r) {
+    const int64_t n = keys[0]->total_len;
+    std::vector<bdf_sort_key> sk((size_t)n_keys);
+    for (int k = 0; k < n_keys; k++) sk[k] = bdf_sort_key{keys[k], 0};
+    TRY(sort_indices_dev(c, n_keys, sk.data(), r->perm.out()));
+    std::vector<const bdf_col*> sorted;
+    for (int k = 0; k < n_keys; k++) {
+        r->sorted.emplace_back(c);
+        TRY(take_dev(c, keys[k], r->perm.get(), r->sorted[k].out()));
+        sorted.push_back(r->sorted[k].get());
+    }
+    TRY(group_heads(c, sorted, false, n, r->head.out()));
+    for (int k = 0; k < n_keys; k++) {
+        r->distinct.emplace_back(c);
+        TRY(filter_dev(c, sorted[k], r->head.get(), r->distinct[k].out()));
+    }
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, r->iota.out()));
+    c->launches++;
+    cudaError_t e = n > 0 ? launch_iota((uint32_t*)r->iota->chunks[0].values, n, c->sm_count, c->s_compute) : cudaSuccess;
+    if (e == cudaSuccess) e = finish_single_group(c, r->iota.get());
+    if (e != cudaSuccess) return fail_cuda(e, what);
+    TRY(filter_dev(c, r->iota.get(), r->head.get(), r->starts.out()));
+    r->n_runs = r->starts->chunks.empty() ? 0 : r->starts->chunks[0].len;
     return BDF_OK;
 }
 
@@ -1885,41 +1899,18 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
         if (v->total_len != keys[0]->total_len) return fail(BDF_LENGTH_MISMATCH, "key and value columns have different lengths");
     }
     const int64_t n = keys[0]->total_len;
-    std::vector<bdf_col*> tmp;                       // everything made on the way; released at the end whatever happens
-    std::vector<bdf_col*> ukeys((size_t)n_keys, nullptr), res((size_t)n_aggs, nullptr);   // the results (released only on failure)
-    auto release_all = [&](std::vector<bdf_col*>& v) { for (bdf_col*& t : v) { if (t) col_release(c, t); t = nullptr; } };
-    int st = BDF_OK;
+    SortedRuns runs(c);
+    TRY(sorted_runs(c, n_keys, keys, "group iota", &runs));
+    const bdf_col* idx = runs.perm.get();
+    const int64_t n_groups = runs.n_runs;
+    const uint32_t* d_starts = (const uint32_t*)runs.starts->chunks[0].values;
+    std::vector<ColOwner> res;
+    for (int j = 0; j < n_aggs; j++) res.emplace_back(c);
     cudaError_t e = cudaSuccess;
-    std::vector<bdf_sort_key> sk((size_t)n_keys);
-    for (int k = 0; k < n_keys; k++) sk[k] = bdf_sort_key{keys[k], 0};
-    bdf_col *idx = nullptr, *head = nullptr, *iota = nullptr, *starts = nullptr;
-    std::vector<const bdf_col*> skeys;
-    st = sort_indices_dev(c, n_keys, sk.data(), &idx);
-    if (st == BDF_OK) tmp.push_back(idx);
-    for (int k = 0; k < n_keys && st == BDF_OK; k++) {
-        bdf_col* s = nullptr;
-        st = take_dev(c, keys[k], idx, &s);
-        if (st == BDF_OK) { tmp.push_back(s); skeys.push_back(s); }
-    }
-    if (st == BDF_OK) st = group_heads(c, skeys, false, n, &head);
-    if (st == BDF_OK) tmp.push_back(head);
-    for (int k = 0; k < n_keys && st == BDF_OK; k++) st = filter_dev(c, skeys[k], head, &ukeys[k]);   // the distinct key tuples, in sort order
-    if (st == BDF_OK) st = col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, &iota);
-    if (st == BDF_OK) {
-        tmp.push_back(iota);
-        c->launches++;
-        e = n > 0 ? launch_iota((uint32_t*)iota->chunks[0].values, n, c->sm_count, c->s_compute) : cudaSuccess;
-        if (e == cudaSuccess) e = finish_single_group(c, iota);
-        if (e != cudaSuccess) st = fail_cuda(e, "group iota");
-    }
-    if (st == BDF_OK) st = filter_dev(c, iota, head, &starts);                     // first sorted row of every group
-    int64_t n_groups = 0;
-    if (st == BDF_OK) { tmp.push_back(starts); n_groups = starts->chunks.empty() ? 0 : starts->chunks[0].len; }
-    const uint32_t* d_starts = st == BDF_OK ? (const uint32_t*)starts->chunks[0].values : nullptr;
 
     // sum / count / min / max / avg: every distinct value column is gathered once and folded once
     std::vector<bool> done((size_t)n_aggs, false);
-    for (int j0 = 0; j0 < n_aggs && st == BDF_OK; j0++) {
+    for (int j0 = 0; j0 < n_aggs; j0++) {
         const int f0 = aggs[j0].function;
         if (done[j0] || f0 == BDF_GROUP_COUNT_DISTINCT || f0 == BDF_GROUP_FIRST || f0 == BDF_GROUP_LAST) continue;
         const bdf_col* v = aggs[j0].column;
@@ -1931,54 +1922,49 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
         const bool mm = want[BDF_GROUP_MAX] || want[BDF_GROUP_MIN];
         // the accumulators the single-key entry never needed: only EXTRA folds write avg, and a float column's min / max
         const bool extra = want[BDF_GROUP_AVG] || (is_float && mm);
-        bdf_col *sval = nullptr, *csum = nullptr, *ccnt = nullptr, *cmin = nullptr, *cmax = nullptr, *cavg = nullptr;
-        std::vector<bdf_col*> cols;   // made for this column; what nobody asked for is released with tmp
-        st = take_dev(c, v, idx, &sval);
-        if (st == BDF_OK) { tmp.push_back(sval); st = col_alloc(c, dt, {ChunkPlan{n_groups, false}}, nullptr, 0, &csum); }
-        if (st == BDF_OK) { cols.push_back(csum); st = col_alloc(c, BDF_I64, {ChunkPlan{n_groups, false}}, nullptr, 0, &ccnt); }
-        if (st == BDF_OK) cols.push_back(ccnt);
+        ColOwner sval(c), csum(c), ccnt(c), cmin(c), cmax(c), cavg(c);   // what nobody asks for is dropped with the owner
+        TRY(take_dev(c, v, idx, sval.out()));
+        TRY(col_alloc(c, dt, {ChunkPlan{n_groups, false}}, nullptr, 0, csum.out()));
+        TRY(col_alloc(c, BDF_I64, {ChunkPlan{n_groups, false}}, nullptr, 0, ccnt.out()));
         // integers without extra: the kernel writes min and max together
-        if (st == BDF_OK && (want[BDF_GROUP_MIN] || (mm && !is_float))) { st = col_alloc(c, dt, {ChunkPlan{n_groups, true}}, nullptr, 0, &cmin); if (st == BDF_OK) cols.push_back(cmin); }
-        if (st == BDF_OK && (want[BDF_GROUP_MAX] || (mm && !is_float))) { st = col_alloc(c, dt, {ChunkPlan{n_groups, true}}, nullptr, 0, &cmax); if (st == BDF_OK) cols.push_back(cmax); }
-        if (st == BDF_OK && want[BDF_GROUP_AVG]) { st = col_alloc(c, BDF_F64, {ChunkPlan{n_groups, true}}, nullptr, 0, &cavg); if (st == BDF_OK) cols.push_back(cavg); }
-        for (bdf_col* r : cols) tmp.push_back(r);
-        if (st != BDF_OK) break;
-        bdf_col* const validity_of[3] = {cmin, cmax, cavg};
+        if (want[BDF_GROUP_MIN] || (mm && !is_float)) TRY(col_alloc(c, dt, {ChunkPlan{n_groups, true}}, nullptr, 0, cmin.out()));
+        if (want[BDF_GROUP_MAX] || (mm && !is_float)) TRY(col_alloc(c, dt, {ChunkPlan{n_groups, true}}, nullptr, 0, cmax.out()));
+        if (want[BDF_GROUP_AVG]) TRY(col_alloc(c, BDF_F64, {ChunkPlan{n_groups, true}}, nullptr, 0, cavg.out()));
+        bdf_col* const validity_of[3] = {cmin.get(), cmax.get(), cavg.get()};
         bdf_col* nonempty = nullptr;   // the kernel sets this bitmap; the others get a copy
         for (bdf_col* r : validity_of) if (r && !nonempty) nonempty = r;
-        wait_groups(c->s_compute, sval, 0, 1);
-        wait_groups(c->s_compute, starts, 0, 1);
+        wait_groups(c->s_compute, sval.get(), 0, 1);
+        wait_groups(c->s_compute, runs.starts.get(), 0, 1);
         {
             const int w = dtype_width(dt);
-            const int outs = 1 + (cmin ? 1 : 0) + (cmax ? 1 : 0);
-            LaunchTimer t(c, BDF_K_GROUP, dt, n, n * w + (sval->chunks[0].validity ? bitmap_bytes(n) : 0) + n_groups * (4 + outs * w + 8 + (cavg ? 8 : 0)));
-            void* scratch = nullptr;
-            e = cudaMallocAsync(&scratch, group_big_scratch_bytes(n), c->s_compute);
+            const int outs = 1 + (cmin.get() ? 1 : 0) + (cmax.get() ? 1 : 0);
+            LaunchTimer t(c, BDF_K_GROUP, dt, n, n * w + (sval->chunks[0].validity ? bitmap_bytes(n) : 0) + n_groups * (4 + outs * w + 8 + (cavg.get() ? 8 : 0)));
+            Scratch<void> scratch;
+            e = scratch.alloc(c, group_big_scratch_bytes(n));
             c->launches += 3;   // long groups among short ones: k_group_medium; hot keys: k_group_big + k_group_big_finish
             if (e == cudaSuccess)
                 e = launch_group_reduce(dt, extra, sval->chunks[0].values, sval->chunks[0].validity, d_starts, n_groups, n, csum->chunks[0].values,
-                                        (long long*)ccnt->chunks[0].values, cmin ? cmin->chunks[0].values : nullptr, cmax ? cmax->chunks[0].values : nullptr,
-                                        cavg ? (double*)cavg->chunks[0].values : nullptr, nonempty ? nonempty->chunks[0].validity : nullptr, scratch,
+                                        (long long*)ccnt->chunks[0].values, cmin.get() ? cmin->chunks[0].values : nullptr, cmax.get() ? cmax->chunks[0].values : nullptr,
+                                        cavg.get() ? (double*)cavg->chunks[0].values : nullptr, nonempty ? nonempty->chunks[0].validity : nullptr, scratch,
                                         c->sm_count, c->s_compute);
-            if (scratch) cudaFreeAsync(scratch, c->s_compute);
         }
         // min / max / avg share one validity pattern: copy the bitmap rather than set it several times with atomics
         for (bdf_col* r : validity_of)
             if (e == cudaSuccess && r && r != nonempty && n_groups)
                 e = cudaMemcpyAsync(r->chunks[0].validity, nonempty->chunks[0].validity, (size_t)bitmap_bytes(n_groups), cudaMemcpyDeviceToDevice, c->s_compute);
-        for (bdf_col* r : cols)
-            if (e == cudaSuccess) {
+        for (bdf_col* r : {csum.get(), ccnt.get(), cmin.get(), cmax.get(), cavg.get()})
+            if (r && e == cudaSuccess) {
                 e = finish_single_group(c, r);
                 if (r->chunks[0].validity) r->null_counts[0] = -1;   // learnt on demand (ensure_null_counts)
             }
-        if (e != cudaSuccess) { st = fail_cuda(e, "group aggregate"); break; }
-        bdf_col* const by_fn[5] = {csum, cmax, cmin, cavg, ccnt};
-        for (int j = j0; j < n_aggs && st == BDF_OK; j++) {
-            if (aggs[j].column != v || aggs[j].function > BDF_GROUP_COUNT) continue;
-            bdf_col* r = by_fn[aggs[j].function];
-            auto it = std::find(tmp.begin(), tmp.end(), r);
-            if (it != tmp.end()) { tmp.erase(it); res[j] = r; }   // first request: the column itself
-            else st = group_clone(c, r, &res[j]);               // the same aggregate again: a copy
+        if (e != cudaSuccess) return fail_cuda(e, "group aggregate");
+        ColOwner* const by_fn[5] = {&csum, &cmax, &cmin, &cavg, &ccnt};
+        bdf_col* const made[5] = {csum.get(), cmax.get(), cmin.get(), cavg.get(), ccnt.get()};
+        for (int j = j0; j < n_aggs; j++) {
+            const int fn = aggs[j].function;
+            if (aggs[j].column != v || fn > BDF_GROUP_COUNT) continue;
+            if (by_fn[fn]->get()) res[j] = std::move(*by_fn[fn]);   // first request: the column itself
+            else TRY(group_clone(c, made[fn], res[j].out()));       // the same aggregate again: a copy
             done[j] = true;
         }
     }
@@ -1986,66 +1972,51 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
     // first / last: the original row of every group's first / last sorted row, then a take of the original column
     bool need_first = false, need_last = false;
     for (int j = 0; j < n_aggs; j++) { need_first |= aggs[j].function == BDF_GROUP_FIRST; need_last |= aggs[j].function == BDF_GROUP_LAST; }
-    bdf_col *first_rows = nullptr, *last_rows = nullptr;
-    if (st == BDF_OK && need_first) { st = col_alloc(c, BDF_U32, {ChunkPlan{n_groups, false}}, nullptr, 0, &first_rows); if (st == BDF_OK) tmp.push_back(first_rows); }
-    if (st == BDF_OK && need_last) { st = col_alloc(c, BDF_U32, {ChunkPlan{n_groups, false}}, nullptr, 0, &last_rows); if (st == BDF_OK) tmp.push_back(last_rows); }
-    if (st == BDF_OK && (need_first || need_last)) {
+    ColOwner first_rows(c), last_rows(c);
+    if (need_first) TRY(col_alloc(c, BDF_U32, {ChunkPlan{n_groups, false}}, nullptr, 0, first_rows.out()));
+    if (need_last) TRY(col_alloc(c, BDF_U32, {ChunkPlan{n_groups, false}}, nullptr, 0, last_rows.out()));
+    if (need_first || need_last) {
         wait_groups(c->s_compute, idx, 0, 1);
         c->launches++;
-        e = launch_group_bounds((const uint32_t*)idx->chunks[0].values, d_starts, n_groups, n, first_rows ? (uint32_t*)first_rows->chunks[0].values : nullptr,
-                                last_rows ? (uint32_t*)last_rows->chunks[0].values : nullptr, c->s_compute);
-        for (bdf_col* r : {first_rows, last_rows})
+        e = launch_group_bounds((const uint32_t*)idx->chunks[0].values, d_starts, n_groups, n, first_rows.get() ? (uint32_t*)first_rows->chunks[0].values : nullptr,
+                                last_rows.get() ? (uint32_t*)last_rows->chunks[0].values : nullptr, c->s_compute);
+        for (bdf_col* r : {first_rows.get(), last_rows.get()})
             if (r && e == cudaSuccess) e = finish_single_group(c, r);
-        if (e != cudaSuccess) st = fail_cuda(e, "group bounds");
+        if (e != cudaSuccess) return fail_cuda(e, "group bounds");
     }
-    for (int j = 0; j < n_aggs && st == BDF_OK; j++)
+    for (int j = 0; j < n_aggs; j++)
         if (aggs[j].function == BDF_GROUP_FIRST || aggs[j].function == BDF_GROUP_LAST)
-            st = take_dev(c, aggs[j].column, aggs[j].function == BDF_GROUP_FIRST ? first_rows : last_rows, &res[j]);
+            TRY(take_dev(c, aggs[j].column, aggs[j].function == BDF_GROUP_FIRST ? first_rows.get() : last_rows.get(), res[j].out()));
 
     // count_distinct: a second stable lexsort over (keys..., value); a head of (keys..., value) on a valid value starts a
     // distinct value of its group (the groups occupy the same row ranges in both sort orders)
-    for (int j = 0; j < n_aggs && st == BDF_OK; j++) {
+    for (int j = 0; j < n_aggs; j++) {
         if (aggs[j].function != BDF_GROUP_COUNT_DISTINCT) continue;
-        std::vector<bdf_col*> local;
-        std::vector<bdf_sort_key> sk2 = sk;
+        std::vector<bdf_sort_key> sk2((size_t)n_keys);
+        for (int k = 0; k < n_keys; k++) sk2[k] = bdf_sort_key{keys[k], 0};
         sk2.push_back(bdf_sort_key{aggs[j].column, 0});
-        bdf_col *idx2 = nullptr, *sval = nullptr, *dhead = nullptr, *pos = nullptr, *cd = nullptr;
-        st = sort_indices_dev(c, n_keys + 1, sk2.data(), &idx2);
-        if (st == BDF_OK) { local.push_back(idx2); st = take_dev(c, aggs[j].column, idx2, &sval); }
-        if (st == BDF_OK) {
-            local.push_back(sval);
-            std::vector<const bdf_col*> cols = skeys;
-            cols.push_back(sval);
-            st = group_heads(c, cols, true, n, &dhead);
+        ColOwner idx2(c), sval(c), dhead(c), pos(c);
+        TRY(sort_indices_dev(c, n_keys + 1, sk2.data(), idx2.out()));
+        TRY(take_dev(c, aggs[j].column, idx2.get(), sval.out()));
+        std::vector<const bdf_col*> cols;
+        for (const ColOwner& s : runs.sorted) cols.push_back(s.get());
+        cols.push_back(sval.get());
+        TRY(group_heads(c, cols, true, n, dhead.out()));
+        TRY(filter_dev(c, runs.iota.get(), dhead.get(), pos.out()));
+        TRY(col_alloc(c, BDF_I64, {ChunkPlan{n_groups, false}}, nullptr, 0, res[j].out()));
+        bdf_col* cd = res[j].get();
+        wait_groups(c->s_compute, pos.get(), 0, 1);
+        c->launches++;
+        {
+            LaunchTimer t(c, BDF_K_GROUP, BDF_I64, n_groups, n_groups * 16);
+            e = launch_group_distinct((const uint32_t*)pos->chunks[0].values, pos->chunks[0].len, d_starts, n_groups, n, (long long*)cd->chunks[0].values,
+                                      c->s_compute);
         }
-        if (st == BDF_OK) { local.push_back(dhead); st = filter_dev(c, iota, dhead, &pos); }
-        if (st == BDF_OK) { local.push_back(pos); st = col_alloc(c, BDF_I64, {ChunkPlan{n_groups, false}}, nullptr, 0, &cd); }
-        if (st == BDF_OK) {
-            wait_groups(c->s_compute, pos, 0, 1);
-            c->launches++;
-            {
-                LaunchTimer t(c, BDF_K_GROUP, BDF_I64, n_groups, n_groups * 16);
-                e = launch_group_distinct((const uint32_t*)pos->chunks[0].values, pos->chunks[0].len, d_starts, n_groups, n, (long long*)cd->chunks[0].values,
-                                          c->s_compute);
-            }
-            if (e == cudaSuccess) e = finish_single_group(c, cd);
-            if (e != cudaSuccess) { col_release(c, cd); st = fail_cuda(e, "group distinct count"); }
-            else res[j] = cd;
-        }
-        for (bdf_col* t : local) col_release(c, t);
+        if (e == cudaSuccess) e = finish_single_group(c, cd);
+        if (e != cudaSuccess) return fail_cuda(e, "group distinct count");
     }
-    if (st != BDF_OK) {
-        const std::string keep = g_err;
-        cudaGetLastError();
-        release_all(tmp);
-        release_all(ukeys);
-        release_all(res);
-        g_err = keep;
-        return st;
-    }
-    release_all(tmp);
-    for (int k = 0; k < n_keys; k++) out_keys[k] = ukeys[k];
-    for (int j = 0; j < n_aggs; j++) out[j] = res[j];
+    for (int k = 0; k < n_keys; k++) out_keys[k] = runs.distinct[k].release();
+    for (int j = 0; j < n_aggs; j++) out[j] = res[j].release();
     if (n_groups_out) *n_groups_out = n_groups;
     return BDF_OK;
 }
@@ -2085,7 +2056,7 @@ static int group_aggregate_dev(bdf_ctx* c, const bdf_col* key, int n_values, con
 
 // ---------------------------------------------------------------------------------------------------
 // equi-join (k_join.cu): the build side (the right side; the left side for RIGHT) is sorted, gathered and cut into runs of equal
-// key tuples exactly as group_by_dev does it; every probe row binary-searches the distinct tuples, the counts are scanned into
+// key tuples by sorted_runs, as group-by's groups are; every probe row binary-searches the distinct tuples, the counts are scanned into
 // output offsets (one host wait for the total), and the emit writes the index pairs by output position.  FULL appends the build
 // rows of the runs no probe row hit, listed in row order by a compaction of an iota.
 
@@ -2124,135 +2095,90 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
     const bdf_col* const* probe = swap ? rk : lk;
     const bdf_col* const* build = swap ? lk : rk;
     const int64_t np = probe[0]->total_len, nb = build[0]->total_len;
-    std::vector<bdf_col*> tmp;   // everything made on the way; released at the end whatever happens
-    int st = BDF_OK;
-    cudaError_t e = cudaSuccess;
 
     // the build side: sorted row numbers, the distinct key tuples, the first sorted row of every run
-    std::vector<bdf_sort_key> sk((size_t)n_keys);
-    for (int k = 0; k < n_keys; k++) sk[k] = bdf_sort_key{build[k], 0};
-    bdf_col *perm = nullptr, *head = nullptr, *iota = nullptr, *starts = nullptr, *mask = nullptr, *unm = nullptr, *pidx = nullptr, *bidx = nullptr;
-    std::vector<const bdf_col*> skeys;
-    std::vector<bdf_col*> ukeys((size_t)n_keys, nullptr);
-    st = sort_indices_dev(c, n_keys, sk.data(), &perm);
-    if (st == BDF_OK) tmp.push_back(perm);
-    for (int k = 0; k < n_keys && st == BDF_OK; k++) {
-        bdf_col* s = nullptr;
-        st = take_dev(c, build[k], perm, &s);
-        if (st == BDF_OK) { tmp.push_back(s); skeys.push_back(s); }
-    }
-    if (st == BDF_OK) st = group_heads(c, skeys, false, nb, &head);
-    if (st == BDF_OK) tmp.push_back(head);
-    for (int k = 0; k < n_keys && st == BDF_OK; k++) {
-        st = filter_dev(c, skeys[k], head, &ukeys[k]);
-        if (st == BDF_OK) tmp.push_back(ukeys[k]);
-    }
-    if (st == BDF_OK) st = col_alloc(c, BDF_U32, {ChunkPlan{nb, false}}, nullptr, 0, &iota);
-    if (st == BDF_OK) {
-        tmp.push_back(iota);
-        c->launches++;
-        e = nb > 0 ? launch_iota((uint32_t*)iota->chunks[0].values, nb, c->sm_count, c->s_compute) : cudaSuccess;
-        if (e == cudaSuccess) e = finish_single_group(c, iota);
-        if (e != cudaSuccess) st = fail_cuda(e, "join iota");
-    }
-    if (st == BDF_OK) st = filter_dev(c, iota, head, &starts);
-    int64_t n_runs = 0;
-    if (st == BDF_OK) { tmp.push_back(starts); n_runs = starts->chunks[0].len; }
+    SortedRuns runs(c);
+    TRY(sorted_runs(c, n_keys, build, "join iota", &runs));
+    const int64_t n_runs = runs.n_runs;
+    const uint32_t* perm = (const uint32_t*)runs.perm->chunks[0].values;
+    const uint32_t* starts = (const uint32_t*)runs.starts->chunks[0].values;
 
     // the probe side is read in place, through the chunk tables of its key columns
     std::vector<const void*> ptables((size_t)n_keys), bkeys((size_t)n_keys);
     std::vector<const uint32_t*> bvalid((size_t)n_keys);
     std::vector<int> pchunks((size_t)n_keys), dtypes((size_t)n_keys);
     int64_t key_bytes = 0;
-    for (int k = 0; k < n_keys && st == BDF_OK; k++) {
+    for (int k = 0; k < n_keys; k++) {
         void* t = nullptr;
-        st = sort_table(c, probe[k], &t, &pchunks[k], nullptr);
+        TRY(sort_table(c, probe[k], &t, &pchunks[k], nullptr));
         ptables[k] = t;
-        bkeys[k] = ukeys[k]->chunks[0].values;
-        bvalid[k] = ukeys[k]->chunks[0].validity;
+        bkeys[k] = runs.distinct[k]->chunks[0].values;
+        bvalid[k] = runs.distinct[k]->chunks[0].validity;
         dtypes[k] = probe[k]->dtype;
         key_bytes += dtype_width(probe[k]->dtype);
     }
     const int64_t blocks = (np + join_tile_rows() - 1) / join_tile_rows();
-    unsigned long long *counts = nullptr, *block_sums = nullptr;
-    uint32_t* mstart = nullptr;
-    unsigned char* hit = nullptr;
-    if (st == BDF_OK) {
-        e = cudaMallocAsync((void**)&counts, (size_t)(np + 1) * sizeof(unsigned long long), c->s_compute);
-        if (e == cudaSuccess) e = cudaMallocAsync((void**)&mstart, (size_t)std::max<int64_t>(np, 1) * sizeof(uint32_t), c->s_compute);
-        if (e == cudaSuccess) e = cudaMallocAsync((void**)&block_sums, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long), c->s_compute);
-        if (e == cudaSuccess && full) e = cudaMallocAsync((void**)&hit, (size_t)std::max<int64_t>(n_runs, 1), c->s_compute);
-        if (e == cudaSuccess && full) e = cudaMemsetAsync(hit, 0, (size_t)std::max<int64_t>(n_runs, 1), c->s_compute);
-        if (e != cudaSuccess) st = fail_cuda(e, "join scratch allocation");
-    }
+    Scratch<unsigned long long> counts, block_sums;
+    Scratch<uint32_t> mstart;
+    Scratch<unsigned char> hit;
+    cudaError_t e = counts.alloc(c, (size_t)(np + 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = mstart.alloc(c, (size_t)std::max<int64_t>(np, 1) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess && full) e = hit.alloc(c, (size_t)std::max<int64_t>(n_runs, 1));
+    if (e == cudaSuccess && full) e = cudaMemsetAsync(hit, 0, (size_t)std::max<int64_t>(n_runs, 1), c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "join scratch allocation");
     unsigned long long total = 0;   // output rows of the probe part
-    if (st == BDF_OK) {
-        {
-            LaunchTimer t(c, BDF_K_JOIN, BDF_U32, np, np * (key_bytes + 8 + 4));
-            e = launch_join_count(n_keys, dtypes.data(), ptables.data(), pchunks.data(), bkeys.data(), bvalid.data(), np, (const uint32_t*)starts->chunks[0].values,
-                                  n_runs, nb, outer ? 1 : 0, counts, mstart, hit, block_sums, c->s_compute);
-        }
-        if (e == cudaSuccess) {
-            LaunchTimer t(c, BDF_K_JOIN, BDF_U64, np, np * 16 + blocks * 16);
-            c->launches++;   // two kernels: the CTA totals, then the rows
-            e = launch_join_scan(counts, np, block_sums, c->s_compute);
-        }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&total, counts + np, sizeof(total), cudaMemcpyDeviceToHost, c->s_compute);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // the output length sizes the result
-        if (e != cudaSuccess) st = fail_cuda(e, "join count");
+    {
+        LaunchTimer t(c, BDF_K_JOIN, BDF_U32, np, np * (key_bytes + 8 + 4));
+        e = launch_join_count(n_keys, dtypes.data(), ptables.data(), pchunks.data(), bkeys.data(), bvalid.data(), np, starts, n_runs, nb, outer ? 1 : 0,
+                              counts, mstart, hit, block_sums, c->s_compute);
     }
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_JOIN, BDF_U64, np, np * 16 + blocks * 16);
+        c->launches++;   // two kernels: the CTA totals, then the rows
+        e = launch_join_scan(counts, np, block_sums, c->s_compute);
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&total, counts + np, sizeof(total), cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // the output length sizes the result
+    if (e != cudaSuccess) return fail_cuda(e, "join count");
 
     // FULL: the build rows of runs nobody hit, in row order
+    ColOwner mask(c), unm(c);
     int64_t n_unm = 0;
-    if (st == BDF_OK && full) {
-        st = col_alloc(c, kBool, {ChunkPlan{nb, false}}, nullptr, 0, &mask);
-        if (st == BDF_OK) {
-            tmp.push_back(mask);
-            e = nb > 0 ? cudaMemsetAsync(mask->chunks[0].values, 0, (size_t)(nb + 31) / 32 * 4, c->s_compute) : cudaSuccess;
-            if (e == cudaSuccess) {
-                LaunchTimer t(c, BDF_K_JOIN, kBool, nb, nb * 8 + n_runs * 5);
-                e = launch_join_unmatched((const uint32_t*)perm->chunks[0].values, nb, (const uint32_t*)starts->chunks[0].values, n_runs, hit,
-                                          (uint32_t*)mask->chunks[0].values, c->sm_count, c->s_compute);
-            }
-            if (e == cudaSuccess) e = finish_single_group(c, mask);
-            if (e != cudaSuccess) st = fail_cuda(e, "join unmatched rows");
+    if (full) {
+        TRY(col_alloc(c, kBool, {ChunkPlan{nb, false}}, nullptr, 0, mask.out()));
+        e = nb > 0 ? cudaMemsetAsync(mask->chunks[0].values, 0, (size_t)(nb + 31) / 32 * 4, c->s_compute) : cudaSuccess;
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_JOIN, kBool, nb, nb * 8 + n_runs * 5);
+            e = launch_join_unmatched(perm, nb, starts, n_runs, hit, (uint32_t*)mask->chunks[0].values, c->sm_count, c->s_compute);
         }
-        if (st == BDF_OK) st = filter_dev(c, iota, mask, &unm);
-        if (st == BDF_OK) { tmp.push_back(unm); n_unm = unm->chunks[0].len; }
+        if (e == cudaSuccess) e = finish_single_group(c, mask.get());
+        if (e != cudaSuccess) return fail_cuda(e, "join unmatched rows");
+        TRY(filter_dev(c, runs.iota.get(), mask.get(), unm.out()));
+        n_unm = unm->chunks[0].len;
     }
 
     const unsigned long long n_out = total + (unsigned long long)n_unm;
-    if (st == BDF_OK && (long double)n_out * 8.25L > (long double)c->hbm_bytes)   // two UInt32 columns and their bitmaps
-        st = fail(BDF_OOM, "a join output of %llu rows does not fit in device memory", n_out);
-    if (st == BDF_OK) st = col_alloc(c, BDF_U32, {ChunkPlan{(int64_t)n_out, full}}, nullptr, 0, &pidx);
-    if (st == BDF_OK) st = col_alloc(c, BDF_U32, {ChunkPlan{(int64_t)n_out, outer}}, nullptr, 0, &bidx);
-    if (st == BDF_OK) {
-        {
-            LaunchTimer t(c, BDF_K_JOIN, BDF_U32, (int64_t)n_out, (int64_t)n_out * 12 + (int64_t)bitmap_bytes((int64_t)n_out) * 2);
-            e = launch_join_emit(counts, np, mstart, (const uint32_t*)perm->chunks[0].values, total, unm ? (const uint32_t*)unm->chunks[0].values : nullptr, n_out,
-                                 (uint32_t*)pidx->chunks[0].values, pidx->chunks[0].validity, (uint32_t*)bidx->chunks[0].values, bidx->chunks[0].validity,
-                                 c->s_compute);
-        }
-        if (e == cudaSuccess) e = finish_single_group(c, pidx);
-        if (e == cudaSuccess) e = finish_single_group(c, bidx);
-        if (e != cudaSuccess) st = fail_cuda(e, "join emit");
+    if ((long double)n_out * 8.25L > (long double)c->hbm_bytes)   // two UInt32 columns and their bitmaps
+        return fail(BDF_OOM, "a join output of %llu rows does not fit in device memory", n_out);
+    ColOwner pidx(c), bidx(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{(int64_t)n_out, full}}, nullptr, 0, pidx.out()));
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{(int64_t)n_out, outer}}, nullptr, 0, bidx.out()));
+    {
+        LaunchTimer t(c, BDF_K_JOIN, BDF_U32, (int64_t)n_out, (int64_t)n_out * 12 + (int64_t)bitmap_bytes((int64_t)n_out) * 2);
+        e = launch_join_emit(counts, np, mstart, perm, total, unm.get() ? (const uint32_t*)unm->chunks[0].values : nullptr, n_out,
+                             (uint32_t*)pidx->chunks[0].values, pidx->chunks[0].validity, (uint32_t*)bidx->chunks[0].values, bidx->chunks[0].validity,
+                             c->s_compute);
     }
-    for (void* p : {(void*)counts, (void*)mstart, (void*)block_sums, (void*)hit})
-        if (p) cudaFreeAsync(p, c->s_compute);
-    if (st != BDF_OK) {
-        const std::string keep = g_err;
-        cudaGetLastError();
-        for (bdf_col* t : tmp) col_release(c, t);
-        col_release(c, pidx);
-        col_release(c, bidx);
-        g_err = keep;
-        return st;
-    }
-    for (bdf_col* t : tmp) col_release(c, t);
+    if (e == cudaSuccess) e = finish_single_group(c, pidx.get());
+    if (e == cudaSuccess) e = finish_single_group(c, bidx.get());
+    if (e != cudaSuccess) return fail_cuda(e, "join emit");
     pidx->null_counts[0] = full ? n_unm : 0;
     bidx->null_counts[0] = outer ? -1 : 0;   // the probe rows without a partner: counted on demand
-    *out_l = swap ? bidx : pidx;
-    *out_r = swap ? pidx : bidx;
+    bdf_col* p = pidx.release();
+    bdf_col* b = bidx.release();
+    *out_l = swap ? b : p;
+    *out_r = swap ? p : b;
     if (n_rows_out) *n_rows_out = (int64_t)n_out;
     return BDF_OK;
 }
@@ -2307,6 +2233,7 @@ static void csv_free(bdf_ctx* c, bdf_csv* f) {
     if (f->fd >= 0) close(f->fd);
     delete f;
 }
+static void drop(bdf_ctx* c, bdf_csv* f) { csv_free(c, f); }
 
 // The unquoted value of raw field bytes [s, e) of the mapping (the rules of csv_parse.cuh's Unquote).
 static std::string csv_unquote(const uint8_t* s, const uint8_t* e) {
@@ -2380,50 +2307,34 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
             if (!((schema[i] >= 0 && schema[i] <= kBool) || schema[i] == BDF_UTF8 || schema[i] == -1))
                 return fail(BDF_UNSUPPORTED, "schema column %d: type %d is not read from CSV (numeric, Boolean or Utf8)", i, schema[i]);
     }
-    bdf_csv* f = new (std::nothrow) bdf_csv();
-    if (!f) return fail(BDF_OOM, "host allocation failed");
+    Owned<bdf_csv> f(c, new (std::nothrow) bdf_csv());
+    if (!f.get()) return fail(BDF_OOM, "host allocation failed");
     f->has_header = o->has_header ? 1 : 0;
     f->delim = o->delimiter;
     f->batch = o->batch_size;
     f->fd = open(path, O_RDONLY | O_CLOEXEC);
     struct stat sb;
-    if (f->fd < 0 || fstat(f->fd, &sb) != 0) { const int err = errno; csv_free(c, f); return fail(BDF_INVALID, "cannot open %s: %s", path, strerror(err)); }
+    if (f->fd < 0 || fstat(f->fd, &sb) != 0) return fail(BDF_INVALID, "cannot open %s: %s", path, strerror(errno));
     f->size = (size_t)sb.st_size;
     if (f->size) {
         void* m = mmap(nullptr, f->size, PROT_READ, MAP_PRIVATE, f->fd, 0);
-        if (m == MAP_FAILED) { const int err = errno; csv_free(c, f); return fail(BDF_INVALID, "cannot map %s: %s", path, strerror(err)); }
+        if (m == MAP_FAILED) return fail(BDF_INVALID, "cannot map %s: %s", path, strerror(errno));
         f->map = (const uint8_t*)m;
     }
     if (f->size >= 3 && f->map[0] == 0xEF && f->map[1] == 0xBB && f->map[2] == 0xBF) f->off = 3;
     f->n = (int64_t)(f->size - f->off);
     const int64_t tile = csv_tile_bytes();
     const int64_t tiles = std::max<int64_t>((f->n + tile - 1) / tile, 1);
-    if ((long double)tiles * tile * 1.3L > (long double)c->hbm_bytes) { csv_free(c, f); return fail(BDF_OOM, "a CSV file of %lld bytes does not fit in device memory", (long long)f->n); }
+    if ((long double)tiles * tile * 1.3L > (long double)c->hbm_bytes) return fail(BDF_OOM, "a CSV file of %lld bytes does not fit in device memory", (long long)f->n);
 
-    int st = BDF_OK;
-    cudaError_t e = cudaSuccess;
-    uint32_t* agg = nullptr;
-    uint8_t* start = nullptr;
-    uint16_t *fe = nullptr, *re = nullptr;
-    unsigned long long *counts = nullptr, *small = nullptr;   // small: [0] final state, [1] first record end, [2] first bad field
-    unsigned int* bits = nullptr;
-    auto scratch_free = [&]() {
-        for (void* p : {(void*)agg, (void*)start, (void*)fe, (void*)re, (void*)counts, (void*)small, (void*)bits})
-            if (p) cudaFreeAsync(p, c->s_compute);
-        agg = nullptr; start = nullptr; fe = nullptr; re = nullptr; counts = nullptr; small = nullptr; bits = nullptr;
-    };
-    auto bail = [&](int status) {
-        const std::string keep = g_err;
-        cudaGetLastError();
-        scratch_free();
-        cudaStreamSynchronize(c->s_h2d);
-        csv_free(c, f);
-        g_err = keep;
-        return status;
-    };
+    Scratch<uint32_t> agg;
+    Scratch<uint8_t> start;
+    Scratch<uint16_t> fe, re;
+    Scratch<unsigned long long> counts, small;   // small: [0] final state, [1] first record end, [2] first bad field
+    Scratch<unsigned int> bits;
 
     // the bytes: page cache -> pinned staging -> HBM
-    e = cudaMallocAsync((void**)&f->d_text, (size_t)(tiles * tile), c->s_compute);
+    cudaError_t e = cudaMallocAsync((void**)&f->d_text, (size_t)(tiles * tile), c->s_compute);
     if (e == cudaSuccess) e = cudaMemsetAsync(f->d_text + f->n, 0, (size_t)(tiles * tile - f->n), c->s_compute);
     if (e == cudaSuccess) e = cudaEventRecord(c->ev_tmp, c->s_compute);
     if (e == cudaSuccess) e = cudaStreamWaitEvent(c->s_h2d, c->ev_tmp, 0);
@@ -2431,31 +2342,35 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
     if (e == cudaSuccess && f->n) e = h2d_copy(c, f->d_text, f->map + f->off, (size_t)f->n);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_h2d);
     f->upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    if (e != cudaSuccess) { fail_cuda(e, "CSV upload"); return bail(cuda_status(e)); }
+    if (e != cudaSuccess) {
+        const int st = fail_cuda(e, "CSV upload");
+        cudaStreamSynchronize(c->s_h2d);   // no copy may still read the mapping when it is unmapped
+        return st;
+    }
 
     // tokenize: the state at every CTA, the field / record end masks, the field count
-    e = cudaMallocAsync((void**)&agg, (size_t)tiles * 4, c->s_compute);
-    if (e == cudaSuccess) e = cudaMallocAsync((void**)&start, (size_t)tiles, c->s_compute);
-    if (e == cudaSuccess) e = cudaMallocAsync((void**)&fe, (size_t)tiles * kThreads * 2, c->s_compute);
-    if (e == cudaSuccess) e = cudaMallocAsync((void**)&re, (size_t)tiles * kThreads * 2, c->s_compute);
-    if (e == cudaSuccess) e = cudaMallocAsync((void**)&counts, (size_t)(tiles + 1) * 8, c->s_compute);
-    if (e == cudaSuccess) e = cudaMallocAsync((void**)&small, 4 * 8, c->s_compute);
+    e = agg.alloc(c, (size_t)tiles * 4);
+    if (e == cudaSuccess) e = start.alloc(c, (size_t)tiles);
+    if (e == cudaSuccess) e = fe.alloc(c, (size_t)tiles * kThreads * 2);
+    if (e == cudaSuccess) e = re.alloc(c, (size_t)tiles * kThreads * 2);
+    if (e == cudaSuccess) e = counts.alloc(c, (size_t)(tiles + 1) * 8);
+    if (e == cudaSuccess) e = small.alloc(c, 4 * 8);
     if (e == cudaSuccess) e = cudaMemsetAsync(small, 0xff, 4 * 8, c->s_compute);
-    if (e != cudaSuccess) { fail_cuda(e, "CSV tokenizer scratch allocation"); return bail(cuda_status(e)); }
+    if (e != cudaSuccess) return fail_cuda(e, "CSV tokenizer scratch allocation");
     {
         LaunchTimer t(c, BDF_K_CSV, kBool, f->n, f->n * 2 + tiles * kThreads * 4);
         c->launches += 3;   // reduce, CTA-state scan, mark, count scan
-        e = launch_csv_tokenize(f->d_text, f->n, f->delim, agg, start, (int*)small, fe, re, counts, c->s_compute);
+        e = launch_csv_tokenize(f->d_text, f->n, f->delim, agg, start, (int*)small.get(), fe, re, counts, c->s_compute);
     }
     unsigned long long host_small[4] = {0, 0, 0, 0}, total = 0;
     if (e == cudaSuccess) e = cudaMemcpyAsync(&total, counts + tiles, 8, cudaMemcpyDeviceToHost, c->s_compute);
     if (e == cudaSuccess) e = cudaMemcpyAsync(host_small, small, 8, cudaMemcpyDeviceToHost, c->s_compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-    if (e != cudaSuccess) { fail_cuda(e, "CSV tokenizer"); return bail(cuda_status(e)); }
+    if (e != cudaSuccess) return fail_cuda(e, "CSV tokenizer");
     const int final_state = (int)(host_small[0] & 0xffffffffu);
     const bool eof_field = final_state != 0;   // the last record has no terminator: end of file ends it
     f->n_fields = (int64_t)total + (eof_field ? 1 : 0);
-    if (f->n_fields == 0) { fail(BDF_WOULD_PANIC, "the CSV file has no records: the reference panics at batches[0]"); return bail(BDF_WOULD_PANIC); }
+    if (f->n_fields == 0) return fail(BDF_WOULD_PANIC, "the CSV file has no records: the reference panics at batches[0]");
 
     // the field index
     e = cudaMallocAsync((void**)&f->d_ends, (size_t)f->n_fields * 8, c->s_compute);
@@ -2467,7 +2382,7 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
     if (e == cudaSuccess && eof_field) e = cudaMemcpyAsync(f->d_ends + total, &eof_entry, 8, cudaMemcpyHostToDevice, c->s_compute);
     if (e == cudaSuccess) e = cudaMemcpyAsync(host_small, small, 4 * 8, cudaMemcpyDeviceToHost, c->s_compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-    if (e != cudaSuccess) { fail_cuda(e, "CSV field index"); return bail(cuda_status(e)); }
+    if (e != cudaSuccess) return fail_cuda(e, "CSV field index");
     const unsigned long long first_rec = std::min<unsigned long long>(host_small[1], eof_field ? total : ~0ull);
     f->k = (int64_t)first_rec + 1;
 
@@ -2478,32 +2393,31 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(host_small, small, 4 * 8, cudaMemcpyDeviceToHost, c->s_compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-    if (e != cudaSuccess) { fail_cuda(e, "CSV record check"); return bail(cuda_status(e)); }
-    if (host_small[2] != ~0ull) return bail(csv_unequal(c, f, (int64_t)host_small[2]));
+    if (e != cudaSuccess) return fail_cuda(e, "CSV record check");
+    if (host_small[2] != ~0ull) return csv_unequal(c, f.get(), (int64_t)host_small[2]);
     const int64_t n_records = f->n_fields / f->k;
     f->f0 = f->has_header ? f->k : 0;
     f->n_rows = n_records - f->has_header;
-    if (f->k > 0x7fffffffLL) { fail(BDF_UNSUPPORTED, "more than 2^31-1 columns"); return bail(BDF_UNSUPPORTED); }
+    if (f->k > 0x7fffffffLL) return fail(BDF_UNSUPPORTED, "more than 2^31-1 columns");
     const int k = (int)f->k;
 
     // names
     if (f->has_header) {
         std::vector<unsigned long long> h;
-        st = csv_fetch(c, f, 0, f->k, h);
-        if (st != BDF_OK) return bail(st);
+        TRY(csv_fetch(c, f.get(), 0, f->k, h));
         for (int i = 0; i < k; i++) {
             int64_t s, en;
-            csv_span(f, i > 0, i > 0 ? h[(size_t)i - 1] : 0, h[(size_t)i], &s, &en);
+            csv_span(f.get(), i > 0, i > 0 ? h[(size_t)i - 1] : 0, h[(size_t)i], &s, &en);
             f->names.push_back(csv_unquote(f->map + f->off + s, f->map + f->off + en));
         }
     } else {
         for (int i = 0; i < k; i++) f->names.push_back("column_" + std::to_string(i + 1));
     }
-    if (f->n_rows == 0) { fail(BDF_WOULD_PANIC, "the CSV file has no data records: the reference panics at batches[0]"); return bail(BDF_WOULD_PANIC); }
+    if (f->n_rows == 0) return fail(BDF_WOULD_PANIC, "the CSV file has no data records: the reference panics at batches[0]");
 
     // schema
     if (schema) {
-        if (n_schema != k) { fail(BDF_INVALID, "the schema has %d columns, the file %d", n_schema, k); return bail(BDF_INVALID); }
+        if (n_schema != k) return fail(BDF_INVALID, "the schema has %d columns, the file %d", n_schema, k);
         for (int i = 0; i < k; i++) {
             f->dtypes.push_back(schema[i] == BDF_UTF8 ? -1 : schema[i]);
             f->nullable.push_back(1);
@@ -2511,7 +2425,7 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
     } else {
         const int64_t rows = o->max_records < 0 ? f->n_rows : std::min<int64_t>(o->max_records, f->n_rows);
         std::vector<unsigned int> hb((size_t)k, 0u);
-        e = cudaMallocAsync((void**)&bits, (size_t)k * 4, c->s_compute);
+        e = bits.alloc(c, (size_t)k * 4);
         if (e == cudaSuccess) e = cudaMemsetAsync(bits, 0, (size_t)k * 4, c->s_compute);
         if (e == cudaSuccess) {
             LaunchTimer t(c, BDF_K_CSV, BDF_U32, rows * f->k, rows * f->k * 16);
@@ -2519,7 +2433,7 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
         }
         if (e == cudaSuccess) e = cudaMemcpyAsync(hb.data(), bits, (size_t)k * 4, cudaMemcpyDeviceToHost, c->s_compute);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-        if (e != cudaSuccess) { fail_cuda(e, "CSV schema inference"); return bail(cuda_status(e)); }
+        if (e != cudaSuccess) return fail_cuda(e, "CSV schema inference");
         for (int i = 0; i < k; i++) {
             const unsigned int types = hb[(size_t)i] & ~1u;   // bit 0: an empty field (a null)
             int dt = -1;                                       // Utf8: other, a mix, or no type at all
@@ -2530,8 +2444,7 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
             f->nullable.push_back((hb[(size_t)i] & 1u) ? 1 : 0);
         }
     }
-    scratch_free();
-    *out = f;
+    *out = f.release();
     return BDF_OK;
 }
 
@@ -2547,29 +2460,24 @@ static int csv_read(bdf_ctx* c, const bdf_csv* f, int n_cols, const int32_t* col
     const int rows_per_tile = csv_parse_rows();
     std::vector<ChunkPlan> plan((size_t)n_chunks);
     for (int64_t i = 0; i < n_chunks; i++) plan[(size_t)i] = ChunkPlan{std::min(batch, f->n_rows - i * batch), true};
-    std::vector<bdf_col*> res((size_t)n_cols, nullptr);
-    int st = BDF_OK;
-    cudaError_t e = cudaSuccess;
-    char* descs = nullptr;
-    unsigned long long* small = nullptr;   // [0] first failing field key, [1] slow-path fields
-    void* slow = nullptr;
-    void* patches = nullptr;
+    std::vector<ColOwner> res;
+    Scratch<char> descs;
+    Scratch<unsigned long long> small;   // [0] first failing field key, [1] slow-path fields
+    Scratch<void> slow, patches;
     const size_t dsz = csv_desc_bytes();
     std::vector<char> hdesc((size_t)std::max(n_cols, 1) * dsz, 0);
     int64_t float_fields = 0, out_bytes = 0;
-    for (int i = 0; i < n_cols && st == BDF_OK; i++) {
+    for (int i = 0; i < n_cols; i++) {
         const int dt = f->dtypes[(size_t)cols[i]];
-        st = col_alloc(c, dt, plan, nullptr, rows_per_tile, &res[(size_t)i]);
-        if (st != BDF_OK) break;
-        bdf_col* col = res[(size_t)i];
+        res.emplace_back(c);
+        TRY(col_alloc(c, dt, plan, nullptr, rows_per_tile, res[(size_t)i].out()));
+        bdf_col* col = res[(size_t)i].get();
         const DevChunk& c0 = col->chunks[0];
         const long long vs = n_chunks > 1 ? (long long)(col->chunks[1].values - c0.values) : 0;
         const long long bs = n_chunks > 1 ? (long long)((char*)col->chunks[1].validity - (char*)c0.validity) : 0;
         const DevChunk& cl = col->chunks[(size_t)n_chunks - 1];
-        if (cl.values != c0.values + vs * (n_chunks - 1) || (char*)cl.validity != (char*)c0.validity + bs * (n_chunks - 1)) {
-            st = fail(BDF_INVALID, "internal: CSV output chunks are not evenly spaced");
-            break;
-        }
+        if (cl.values != c0.values + vs * (n_chunks - 1) || (char*)cl.validity != (char*)c0.validity + bs * (n_chunks - 1))
+            return fail(BDF_INVALID, "internal: CSV output chunks are not evenly spaced");
         struct Desc { char* values; long long vstride; uint32_t* validity; long long bstride; uint32_t* warp_counts; int dtype; int file_col; } d{
             c0.values, vs, c0.validity, bs, col->d_warp_counts, dt, cols[i]};
         static_assert(sizeof(Desc) == 48, "CsvColDesc layout");
@@ -2578,58 +2486,52 @@ static int csv_read(bdf_ctx* c, const bdf_csv* f, int n_cols, const int32_t* col
         out_bytes += (int64_t)value_bytes(dt, f->n_rows, 0) + bitmap_bytes(f->n_rows);
     }
     const long long slow_cap = std::max<long long>(65536, float_fields / 64);
-    if (st == BDF_OK) {
-        e = cudaMallocAsync((void**)&descs, hdesc.size(), c->s_compute);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(descs, hdesc.data(), hdesc.size(), cudaMemcpyHostToDevice, c->s_compute);
-        if (e == cudaSuccess) e = cudaMallocAsync((void**)&small, 16, c->s_compute);
-        if (e == cudaSuccess) e = cudaMemsetAsync(small, 0xff, 8, c->s_compute);
-        if (e == cudaSuccess) e = cudaMemsetAsync(small + 1, 0, 8, c->s_compute);
-        if (e == cudaSuccess && float_fields) e = cudaMallocAsync(&slow, (size_t)slow_cap * csv_slow_bytes(), c->s_compute);
-        if (e != cudaSuccess) st = fail_cuda(e, "CSV read scratch allocation");
-    }
+    cudaError_t e = descs.alloc(c, hdesc.size());
+    if (e == cudaSuccess) e = cudaMemcpyAsync(descs, hdesc.data(), hdesc.size(), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess) e = small.alloc(c, 16);
+    if (e == cudaSuccess) e = cudaMemsetAsync(small, 0xff, 8, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemsetAsync(small + 1, 0, 8, c->s_compute);
+    if (e == cudaSuccess && float_fields) e = slow.alloc(c, (size_t)slow_cap * csv_slow_bytes());
+    if (e != cudaSuccess) return fail_cuda(e, "CSV read scratch allocation");
     unsigned long long hs[2] = {~0ull, 0};
-    if (st == BDF_OK) {
-        {
-            const int64_t fields = f->n_rows * n_cols;
-            LaunchTimer t(c, BDF_K_CSV, n_cols == 1 ? f->dtypes[(size_t)cols[0]] : -1, fields,
-                          f->n * n_cols / std::max<int64_t>(f->k, 1) + fields * 16 + out_bytes);
-            e = launch_csv_parse(f->d_text, f->d_ends, descs, n_cols, f->f0, f->k, f->n_rows, batch, small, slow, small + 1, slow_cap, c->s_compute);
-        }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(hs, small, 16, cudaMemcpyDeviceToHost, c->s_compute);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-        if (e != cudaSuccess) st = fail_cuda(e, "CSV parse");
+    {
+        const int64_t fields = f->n_rows * n_cols;
+        LaunchTimer t(c, BDF_K_CSV, n_cols == 1 ? f->dtypes[(size_t)cols[0]] : -1, fields,
+                      f->n * n_cols / std::max<int64_t>(f->k, 1) + fields * 16 + out_bytes);
+        e = launch_csv_parse(f->d_text, f->d_ends, descs, n_cols, f->f0, f->k, f->n_rows, batch, small, slow, small + 1, slow_cap, c->s_compute);
     }
-    if (st == BDF_OK && hs[0] != ~0ull) {   // the first failing field: (batch, column in the request, row)
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hs, small, 16, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "CSV parse");
+    if (hs[0] != ~0ull) {   // the first failing field: (batch, column in the request, row)
         const unsigned long long key = hs[0];
         const int64_t row = (int64_t)(key % (unsigned long long)batch), rest = (int64_t)(key / (unsigned long long)batch);
         const int p = (int)(rest % n_cols);
         const int64_t chunk = rest / n_cols, r = chunk * batch + row, fld = f->f0 + r * f->k + cols[p];
         std::vector<unsigned long long> v;
-        st = csv_fetch(c, f, fld > 0 ? fld - 1 : 0, fld > 0 ? 2 : 1, v);
-        if (st == BDF_OK) {
-            int64_t s, en;
-            csv_span(f, fld > 0, fld > 0 ? v[0] : 0, fld > 0 ? v[1] : v[0], &s, &en);
-            g_err = "Error while parsing value " + csv_unquote(f->map + f->off + s, f->map + f->off + en) + " for column " + std::to_string(cols[p]) +
-                    " at line " + std::to_string(r + f->has_header);
-            st = BDF_PARSE;
-        }
+        TRY(csv_fetch(c, f, fld > 0 ? fld - 1 : 0, fld > 0 ? 2 : 1, v));
+        int64_t s, en;
+        csv_span(f, fld > 0, fld > 0 ? v[0] : 0, fld > 0 ? v[1] : v[0], &s, &en);
+        g_err = "Error while parsing value " + csv_unquote(f->map + f->off + s, f->map + f->off + en) + " for column " + std::to_string(cols[p]) +
+                " at line " + std::to_string(r + f->has_header);
+        return BDF_PARSE;
     }
     int64_t n_slow = (int64_t)hs[1];
-    if (st == BDF_OK && n_slow > slow_cap)
-        st = fail(BDF_UNSUPPORTED, "%lld float fields need exact rounding, more than the %lld one read resolves", (long long)n_slow, slow_cap);
-    if (st == BDF_OK && n_slow > 0) {   // exact rounding on the host, in the C locale, written back by one scatter
+    if (n_slow > slow_cap)
+        return fail(BDF_UNSUPPORTED, "%lld float fields need exact rounding, more than the %lld one read resolves", (long long)n_slow, slow_cap);
+    if (n_slow > 0) {   // exact rounding on the host, in the C locale, written back by one scatter
         struct Slow { long long start, end; int col, pad; long long chunk, row; };
         struct Patch { unsigned long long dst, bits; int width, pad; };
         std::vector<Slow> sl((size_t)n_slow);
         e = cudaMemcpyAsync(sl.data(), slow, (size_t)n_slow * sizeof(Slow), cudaMemcpyDeviceToHost, c->s_compute);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-        if (e != cudaSuccess) st = fail_cuda(e, "CSV exact rounding");
+        if (e != cudaSuccess) return fail_cuda(e, "CSV exact rounding");
         static locale_t cloc = newlocale(LC_ALL_MASK, "C", (locale_t)0);
         std::vector<Patch> hp;
-        for (size_t i = 0; i < sl.size() && st == BDF_OK; i++) {
+        for (size_t i = 0; i < sl.size(); i++) {
             const Slow& x = sl[i];
             const std::string v = csv_unquote(f->map + f->off + x.start, f->map + f->off + x.end);
-            const bdf_col* col = res[(size_t)x.col];
+            const bdf_col* col = res[(size_t)x.col].get();
             Patch pt{};
             if (col->dtype == BDF_F64) {
                 const double d = strtod_l(v.c_str(), nullptr, cloc);
@@ -2646,38 +2548,26 @@ static int csv_read(bdf_ctx* c, const bdf_csv* f, int n_cols, const int32_t* col
             hp.push_back(pt);
         }
         static_assert(sizeof(Patch) == 24, "CsvPatch layout");
-        if (st == BDF_OK) {
-            e = cudaMallocAsync(&patches, hp.size() * sizeof(Patch), c->s_compute);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(patches, hp.data(), hp.size() * sizeof(Patch), cudaMemcpyHostToDevice, c->s_compute);
-            if (e == cudaSuccess) {
-                LaunchTimer t(c, BDF_K_CSV, -1, (int64_t)hp.size(), (int64_t)hp.size() * 32);
-                e = launch_csv_scatter(patches, (long long)hp.size(), c->s_compute);
-            }
-            if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // hp is read by the copy
-            if (e != cudaSuccess) st = fail_cuda(e, "CSV exact rounding");
+        e = patches.alloc(c, hp.size() * sizeof(Patch));
+        if (e == cudaSuccess) e = cudaMemcpyAsync(patches, hp.data(), hp.size() * sizeof(Patch), cudaMemcpyHostToDevice, c->s_compute);
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_CSV, -1, (int64_t)hp.size(), (int64_t)hp.size() * 32);
+            e = launch_csv_scatter(patches, (long long)hp.size(), c->s_compute);
         }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // hp is read by the copy
+        if (e != cudaSuccess) return fail_cuda(e, "CSV exact rounding");
     }
-    for (int i = 0; i < n_cols && st == BDF_OK; i++) {
-        bdf_col* col = res[(size_t)i];
+    for (int i = 0; i < n_cols; i++) {
+        bdf_col* col = res[(size_t)i].get();
         col->counts_on_device = true;
-        st = fetch_counts(c, col);
-        if (st != BDF_OK) break;
+        TRY(fetch_counts(c, col));
         for (size_t j = 0; j < col->chunks.size(); j++)
             if (col->null_counts[j] == 0) col->chunks[j].validity = nullptr;   // no bitmap in a chunk without nulls
         e = finish_single_group(c, col);
-        if (e != cudaSuccess) st = fail_cuda(e, "CSV read");
-    }
-    for (void* p : {(void*)descs, (void*)small, slow, patches})
-        if (p) cudaFreeAsync(p, c->s_compute);
-    if (st != BDF_OK) {
-        const std::string keep = g_err;
-        cudaGetLastError();
-        for (bdf_col* col : res) col_release(c, col);
-        g_err = keep;
-        return st;
+        if (e != cudaSuccess) return fail_cuda(e, "CSV read");
     }
     f->exact_fields = n_slow;
-    for (int i = 0; i < n_cols; i++) out[i] = res[(size_t)i];
+    for (int i = 0; i < n_cols; i++) out[i] = res[(size_t)i].release();
     return BDF_OK;
 }
 

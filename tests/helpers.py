@@ -1,7 +1,19 @@
 """Shared comparison helpers for the parity tests."""
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
+
+
+def pool_used(ctx) -> int:
+    """Bytes of the device's default memory pool (every stream-ordered allocation of the library) now in use."""
+    cu = C.CDLL("libcuda.so.1")
+    dev, pool, used = C.c_int(), C.c_void_p(), C.c_uint64()
+    assert cu.cuInit(0) == 0 and cu.cuDeviceGet(C.byref(dev), ctx.device) == 0
+    assert cu.cuDeviceGetDefaultMemPool(C.byref(pool), dev) == 0
+    assert cu.cuMemPoolGetAttribute(pool, 7, C.byref(used)) == 0   # CU_MEMPOOL_ATTR_USED_MEM_CURRENT
+    return used.value
 
 
 def ulp_distance(a: np.ndarray, b: np.ndarray) -> np.ndarray:

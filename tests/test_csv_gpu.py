@@ -1,5 +1,4 @@
 """DataFrame::from_csv on the device against tests/csv_oracle.py: every value bit for bit, and the same null slots."""
-import ctypes as C
 import json
 import os
 import struct
@@ -8,6 +7,7 @@ import numpy as np
 import pytest
 
 import csv_oracle as co
+from helpers import pool_used
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 UK = os.path.join(HERE, "golden", "uk_cities_with_headers.csv")
@@ -228,15 +228,6 @@ def test_ten_million_rows_and_repeatability(rdf, ctx, tmp_path):
         assert len(lens) == (n + 1023) // 1024
 
 
-def _pool_used(ctx):
-    cu = C.CDLL("libcuda.so.1")
-    dev, pool, used = C.c_int(), C.c_void_p(), C.c_uint64()
-    assert cu.cuCtxGetDevice(C.byref(dev)) == 0
-    assert cu.cuDeviceGetDefaultMemPool(C.byref(pool), dev) == 0
-    assert cu.cuMemPoolGetAttribute(pool, 7, C.byref(used)) == 0   # CU_MEMPOOL_ATTR_USED_MEM_CURRENT
-    return used.value
-
-
 @pytest.mark.gpu
 def test_errors_leak_nothing(rdf, ctx, tmp_path):
     N = rdf.native
@@ -247,7 +238,7 @@ def test_errors_leak_nothing(rdf, ctx, tmp_path):
         return str(p)
 
     ctx.synchronize()
-    before = _pool_used(ctx)
+    before = pool_used(ctx)
     with pytest.raises(rdf.ComputeError, match=r"CSV error: record 2 \(line: 3, byte: 8\): found record with 3 fields, but the previous record has 2 fields"):
         rdf.CsvFile(write("u.csv", b"a,b\n1,2\n3,4,5\n6,7\n"), ctx=ctx)
     with pytest.raises(rdf.ComputeError, match="found record with 1 fields, but the previous record has 2 fields"):
@@ -268,7 +259,7 @@ def test_errors_leak_nothing(rdf, ctx, tmp_path):
         with pytest.raises(rdf.ComputeError):
             f.read([5])
     ctx.synchronize()
-    assert _pool_used(ctx) == before
+    assert pool_used(ctx) == before
     fleet = rdf.Context.multi(0)
     try:
         with pytest.raises(rdf.UnsupportedType):

@@ -7,7 +7,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 
-from helpers import assert_same_array, random_mask
+from helpers import assert_same_array, pool_used, random_mask
 
 pytestmark = pytest.mark.gpu
 
@@ -135,9 +135,15 @@ def test_divide_by_zero_follows_the_materialised_chain(rdf, ctx, oracle):
         assert st == oracle.OK
         for g, w in zip(got, want):
             assert_same_array(g, w, what="masked zero divisors", check_payload=False)
-    # a zero that only appears in an INTERMEDIATE (a - a) is found too
+    # a zero that only appears in an INTERMEDIATE (a - a) is found too; the refused calls drop their output columns
+    ctx.synchronize()
+    before = pool_used(ctx)
     with pytest.raises(rdf.DivideByZero):
         rdf.eval_expr([ca], [(N.SUB, 0, 0), (N.DIV, 0, 1)])
+    with pytest.raises(rdf.DivideByZero):
+        rdf.eval_expr([ca, cz], [(N.ADD, 0, 0), (N.DIV, 2, 1)])
+    ctx.synchronize()
+    assert pool_used(ctx) == before
 
 
 def test_argument_validation(rdf, ctx):

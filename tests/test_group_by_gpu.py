@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import group_by_oracle as gbo
+from helpers import pool_used
 
 FNS = ["sum", "max", "min", "avg", "count", "count_distinct", "first", "last"]
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -238,6 +239,9 @@ def test_group_by_errors(rdf, ctx):
     b = rdf.Column.upload([P.from_numpy(np.arange(11, dtype=np.int64))], ctx=ctx)
     f = rdf.Column.upload([P.from_numpy(np.arange(10, dtype=np.float64))], ctx=ctx)
     flag = rdf.Column.upload([rdf.BooleanArray.from_numpy(np.arange(10) % 2 == 0)], ctx=ctx)
+    rdf.group_by([a], [(f, fn) for fn in ("sum", "count_distinct", "first")])
+    ctx.synchronize()
+    before = pool_used(ctx)
     with pytest.raises(rdf.ComputeError):
         rdf.group_by([], [(a, "sum")])                                   # no key: BDF_INVALID
     with pytest.raises(rdf.ComputeError):
@@ -264,6 +268,8 @@ def test_group_by_errors(rdf, ctx):
     out_k, out = (C.c_void_p * 1)(), (C.c_void_p * 1)()
     assert N.lib().bdf_group_by_dev(ctx.handle, 1, keys, 1, aggs, out_k, out, None) == N.UNSUPPORTED
     assert N.lib().bdf_group_by_dev(ctx.handle, 1, None, 0, None, out_k, out, None) == N.INVALID
+    ctx.synchronize()
+    assert pool_used(ctx) == before
     fleet = rdf.Context.multi(0)
     try:
         fk = rdf.Column.upload([P.from_numpy(np.arange(10, dtype=np.int64))], ctx=fleet)

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import join_oracle as jo
+from helpers import pool_used
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DTYPES = ["int8", "int16", "int32", "int64", "uint8", "uint16", "uint32", "uint64", "float32", "float64"]
@@ -157,16 +158,6 @@ def test_join_same_bits_on_a_second_run(rdf, ctx):
         assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
 
 
-def _pool_used(ctx):
-    """Bytes of the device's default memory pool (every stream-ordered allocation of the library) now in use."""
-    cu = C.CDLL("libcuda.so.1")
-    dev, pool, used = C.c_int(), C.c_void_p(), C.c_uint64()
-    assert cu.cuInit(0) == 0 and cu.cuDeviceGet(C.byref(dev), ctx.device) == 0
-    assert cu.cuDeviceGetDefaultMemPool(C.byref(pool), dev) == 0
-    assert cu.cuMemPoolGetAttribute(pool, 7, C.byref(used)) == 0   # CU_MEMPOOL_ATTR_USED_MEM_CURRENT
-    return used.value
-
-
 @pytest.mark.gpu
 def test_join_errors_leak_nothing(rdf, ctx):
     P, N = rdf.PrimitiveArray, rdf.native
@@ -188,7 +179,7 @@ def test_join_errors_leak_nothing(rdf, ctx):
         return st, (N.lib().bdf_last_error() or b"").decode()
 
     ctx.synchronize()
-    before = _pool_used(ctx)
+    before = pool_used(ctx)
     assert call(N.JOIN_INNER, [], []) == (N.INVALID, "Join criteria cannot be empty")
     assert call(N.JOIN_INNER, [a] * 17, [a] * 17)[0] == N.INVALID
     hl, hr = C.c_void_p(), C.c_void_p()
@@ -207,7 +198,7 @@ def test_join_errors_leak_nothing(rdf, ctx):
     with pytest.raises(rdf.ComputeError, match="Join criteria cannot be empty"):
         rdf.join_indices([], [], "inner")
     ctx.synchronize()
-    assert _pool_used(ctx) == before
+    assert pool_used(ctx) == before
     fleet = rdf.Context.multi(0)
     try:
         fk = rdf.Column.upload([P.from_numpy(np.arange(10, dtype=np.int64))], ctx=fleet)

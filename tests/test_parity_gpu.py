@@ -15,7 +15,7 @@ import os
 import numpy as np
 import pytest
 
-from helpers import assert_same_array, random_mask, ulp_distance
+from helpers import assert_same_array, pool_used, random_mask, ulp_distance
 
 pytestmark = pytest.mark.gpu
 
@@ -115,6 +115,19 @@ def test_divide_by_zero_and_errors(rdf, ctx, oracle):
     ok = P.from_numpy(np.ones(5, dtype=np.int64))
     with pytest.raises(rdf.DivideByZero):
         rdf.ScalarFunctions.divide([ok, P.from_numpy(big)], [ok, P.from_numpy(big)])
+    # on device columns DivideByZero comes after the output column (and the fused aggregate's future) was made: nothing leaks
+    ca = rdf.Column.upload([P.from_pylist(rdf.F64, [6.0, 8.0, 10.0])], ctx=ctx)
+    cz = rdf.Column.upload([P.from_pylist(rdf.F64, [2.0, 0.0, 5.0])], ctx=ctx)
+    ca.divide(ca).free()
+    ca.binary_agg(rdf.native.DIV, ca)[0].free()
+    ctx.synchronize()
+    before = pool_used(ctx)
+    with pytest.raises(rdf.DivideByZero):
+        ca.divide(cz)
+    with pytest.raises(rdf.DivideByZero):
+        ca.binary_agg(rdf.native.DIV, cz)
+    ctx.synchronize()
+    assert pool_used(ctx) == before
     # length mismatch: same message as the reference (src/functions/scalar.rs:508-511)
     with pytest.raises(rdf.ComputeError, match="Cannot perform math operation on arrays of different length"):
         rdf.ScalarFunctions.add([P.from_pylist(rdf.I64, [1, 2, 3])], [P.from_pylist(rdf.I64, [1, 2])])
@@ -133,6 +146,27 @@ def test_divide_by_zero_and_errors(rdf, ctx, oracle):
         rdf.ScalarFunctions.abs([P.from_pylist(rdf.U32, [1])])
     with pytest.raises(rdf.UnsupportedType):
         rdf.AggregateFunctions.max([P.from_pylist(rdf.F64, [1.0])])
+
+
+def test_upload_many_bad_view_leaks_nothing(rdf, ctx):
+    """A bad view in the second column is found after the first column's arenas were allocated."""
+    import ctypes as C
+    N = rdf.native
+    good = [rdf.PrimitiveArray.from_numpy(np.arange(1000, dtype=np.int64))]
+    for col in rdf.Column.upload_many([good, good], ctx=ctx):
+        col.free()
+    views = [N.make_views(good), N.make_views(good)]
+    views[1][0].values = None   # 1000 rows without a values buffer
+    dtypes, counts = (C.c_int32 * 2)(rdf.I64, rdf.I64), (C.c_int64 * 2)(1, 1)
+    ptrs = (C.POINTER(N.View) * 2)(*[C.cast(v, C.POINTER(N.View)) for v in views])
+    outs = (C.c_void_p * 2)()
+    ctx.synchronize()
+    before = pool_used(ctx)
+    assert N.lib().bdf_upload_many(ctx.handle, 2, dtypes, counts, ptrs, 0, outs) == N.INVALID
+    assert N.lib().bdf_last_error() == b"bad view 0"
+    assert outs[0] is None and outs[1] is None
+    ctx.synchronize()
+    assert pool_used(ctx) == before
 
 
 def test_reference_goldens_on_gpu(rdf, ctx, oracle):
@@ -606,8 +640,13 @@ def test_fused_aggregate_is_deterministic_and_rejects_math_ops(rdf, ctx):
         sums.add(float(agg["sum"]).hex())
         col.free()
     assert len(sums) == 1
-    with pytest.raises(rdf.UnsupportedType):
-        a.binary_agg(rdf.native.ATAN2, b)
+    ctx.synchronize()
+    before = pool_used(ctx)
+    for op in (rdf.native.ATAN2, rdf.native.HYPOT, rdf.native.LOG):   # refused after the output column was made
+        with pytest.raises(rdf.UnsupportedType):
+            a.binary_agg(op, b)
+    ctx.synchronize()
+    assert pool_used(ctx) == before
 
 
 def test_split_download_overlaps_and_matches(rdf, ctx, oracle):

@@ -5,7 +5,7 @@ for EQUALITY, taken columns bit for bit."""
 import numpy as np
 import pytest
 
-from helpers import assert_same_array, random_mask
+from helpers import assert_same_array, pool_used, random_mask
 
 pytestmark = pytest.mark.gpu
 
@@ -113,8 +113,15 @@ def test_take_rules(rdf, ctx, oracle):
     dense = [rdf.PrimitiveArray.from_numpy(np.arange(1000, dtype=np.int64))]
     out = rdf.Column.upload(dense).take(rdf.Column.upload([rdf.PrimitiveArray.from_numpy(np.array([999, 0, 5], np.uint32))])).download()[0]
     assert out.validity is None and out.value_slice().tolist() == [999, 0, 5]
-    with pytest.raises(rdf.ArrowError):      # index past the end
-        rdf.Column.upload(dense).take(rdf.Column.upload([rdf.PrimitiveArray.from_numpy(np.array([1000], np.uint32))]))
+    # index past the end: found by the kernel, after the output column was made, which is dropped again
+    cd = rdf.Column.upload(dense)
+    past_end = rdf.Column.upload([rdf.PrimitiveArray.from_numpy(np.array([1000], np.uint32))])
+    ctx.synchronize()
+    before = pool_used(ctx)
+    with pytest.raises(rdf.ArrowError, match="take: index out of bounds$"):
+        cd.take(past_end)
+    ctx.synchronize()
+    assert pool_used(ctx) == before
     with pytest.raises(rdf.UnsupportedType):  # indices must be UInt32
         cv.take(rdf.Column.upload(dense))
     with pytest.raises(rdf.UnsupportedType):  # boolean sort criterion
