@@ -225,7 +225,7 @@ struct bdf_ctx {
     size_t hbm_bytes = 0;
     cudaStream_t s_compute = nullptr, s_h2d = nullptr, s_d2h = nullptr;
     cudaStream_t s_desc = nullptr;  // descriptor copies: run ahead of the compute stream, off its critical path
-    cudaStream_t s_fin = nullptr;   // k_finish of fused aggregates: overlaps the next operator
+    cudaStream_t s_fin = nullptr;   // k_finish of fused aggregates: overlaps the next operator (highest priority)
     std::mutex mu;
     // pinned staging: descriptor ring + small result area
     char* ring = nullptr;           // pinned host side of the descriptor ring
@@ -482,9 +482,13 @@ static bool col_complete(const bdf_col* col) {
     return true;
 }
 
+// A group whose event has already fired adds no wait to the stream.
 static void wait_groups(cudaStream_t s, const bdf_col* col, int64_t begin, int64_t end) {
     for (auto& g : col->groups)
-        if (g.begin < end && g.end > begin) cudaStreamWaitEvent(s, g.ev, 0);
+        if (g.begin < end && g.end > begin && cudaEventQuery(g.ev) != cudaSuccess) {
+            cudaGetLastError();   // NotReady must not reach a later launch check
+            cudaStreamWaitEvent(s, g.ev, 0);
+        }
 }
 
 // Group boundaries for an operator over `n` chunks: a single group when the inputs are resident, else
@@ -872,7 +876,13 @@ static cudaError_t part_acquire(bdf_ctx* c, int64_t total_tiles, bdf_ctx::PartBu
         if (e == cudaSuccess) pb->cap = need;
     }
     if (e == cudaSuccess && !pb->done) e = cudaEventCreateWithFlags(&pb->done, cudaEventDisableTiming);
-    if (e == cudaSuccess && pb->used) e = cudaStreamWaitEvent(c->s_compute, pb->done, 0);  // its previous k_finish has read it
+    if (e == cudaSuccess && pb->used) {  // its previous k_finish has read it: wait on the device only while that is still pending
+        e = cudaEventQuery(pb->done);
+        if (e == cudaErrorNotReady) {
+            cudaGetLastError();   // NotReady must not reach a later launch check
+            e = cudaStreamWaitEvent(c->s_compute, pb->done, 0);
+        }
+    }
     *out = pb;
     return e;
 }
@@ -3223,7 +3233,11 @@ static int init_impl(bdf_ctx* c, int device) {
     CK(cudaStreamCreateWithFlags(&c->s_h2d, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&c->s_d2h, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&c->s_desc, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&c->s_fin, cudaStreamNonBlocking));
+    // The finish stream's few CTAs are scheduled ahead of the CTAs still queued from the next operator's grid: at the default
+    // priority a k_finish waited for the whole next K5 grid to be dispatched, so the host saw the step's result one step late.
+    int prio_least = 0, prio_greatest = 0;
+    CK(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
+    CK(cudaStreamCreateWithPriority(&c->s_fin, cudaStreamNonBlocking, prio_greatest));
     cudaMemPool_t pool;
     CK(cudaDeviceGetDefaultMemPool(&pool, device));
     uint64_t keep = ~0ull;  // keep freed arenas cached: operators allocate their outputs per call
