@@ -5,6 +5,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
 
     python benchmarks/kernels_bench.py [--rows 100000000] [--json kernels.json]
     python benchmarks/kernels_bench.py --csv [--csv-rows 50000000] [--json csv.json]   # the CSV reader rows instead (a 2.55 GB temporary file)
+    python benchmarks/kernels_bench.py --window [--rows 100000000]                      # only the window-function rows
 """
 from __future__ import annotations
 
@@ -130,14 +131,99 @@ def csv_bench(ctx, rows, rows_out, reps=3):
         print(f"{name:44s} {ms:9.2f} ms  {nbytes / ms / 1e6:7.2f} GB/s of file bytes", flush=True)
 
 
+def window_parts(recs, value_calls):
+    """Label the launch records of ONE bdf_window_dev call by step, in launch order: the sort, the gathers of the sorted keys, the
+    head bitmaps (k_group_heads, the boolean OR), the runs (popcount scan and run-start compactions), the ranks, then per value call
+    (``value_calls``: "shift" or "scan" in call order) the gather of x in sorted order, the kernel itself and the gather back to row
+    order."""
+    parts, k, seen_rank, back = {}, 0, False, False
+    for r in recs:
+        kind = r["kernel"]
+        if kind == "sort":
+            label = "sort"
+        elif kind == "compare" or (kind == "window" and r["dtype"] == N.BOOL):
+            label = "heads"
+        elif kind == "filter" or (kind == "window" and r["dtype"] == rdf.U64):
+            label = "runs"
+        elif kind == "window" and r["dtype"] == rdf.U32 and not seen_rank:
+            label, seen_rank = "rank", True
+        elif kind == "window":
+            label, k, back = value_calls[k], k + 1, True
+        elif kind == "take":
+            label = "key gathers" if not seen_rank else "return gathers" if back else "value gathers"
+            back = False if seen_rank else back
+        else:
+            label = kind
+        parts[label] = parts.get(label, 0.0) + r["ms"]
+    return parts
+
+
+def window_bench(ctx, rows, lens, rows_out, reps=3):
+    """Window functions over 1e8 rows (bdf_window_dev): every row prints its total and its parts."""
+    G = rdf.Column.generate
+
+    def run(what, part, order, calls, value_calls):
+        for _ in range(2):   # warm-up
+            for c in rdf.window(part, order, calls):
+                c.free()
+        ctx.synchronize()
+        ctx.profile_read()
+        totals, per_run = [], []
+        for _ in range(reps):
+            ctx.profile_enable(True)
+            out = rdf.window(part, order, calls)
+            ctx.profile_enable(False)
+            recs = ctx.profile_read()
+            for c in out:
+                c.free()
+            p = window_parts(recs, value_calls)
+            per_run.append(p)
+            totals.append(sum(p.values()))
+        med = int(np.argsort(totals)[len(totals) // 2])
+        parts = per_run[med]
+        print(f"{what:60s} {totals[med]:8.3f} ms  (" + ", ".join(f"{k} {v:.3f}" for k, v in parts.items()) + ")", flush=True)
+        rows_out.append({"case": what, "config": "window", "ms": totals[med], "runs_ms": totals, "rows": rows, "parts": parts})
+        return parts
+
+    x = G(rdf.F64, lens, 0, -1e3, 1e3, col_id=60)
+    p = run(f"running sum f64 over {rows:.0e} rows (no keys: the scan alone)", [], [], [("sum", x, "rows")], ["scan"])
+    pk, pk_src = configs_bench._peak()
+    scan_bytes = rows * 16   # 8 B read + 8 B written per row
+    print(f"{'':60s} scan: {scan_bytes / p['scan'] / 1e6:8.1f} GB/s algorithmic = {scan_bytes / p['scan'] / 1e6 / pk:5.3f} of the "
+          f"{pk:.0f} GB/s ceiling ({pk_src})", flush=True)
+    kf = G(rdf.F64, lens, 0, 0.0, rows / 100.0, col_id=61)
+    key = kf.cast(rdf.I32)                                  # ~1e6 partitions of ~100 rows
+    kf.free()
+    run("partition i32 (~1e6) order f64 desc: row_number, rank, lag, sum RANGE", [key], [(x, True)],
+        [("row_number",), ("rank",), ("lag", x, 1), ("sum", x, "range")], ["shift", "scan"])
+    key.free()
+    o = G(rdf.I64, lens, 3, col_id=62)
+    run("one partition, order i64: rank, cume_dist (hot partition)", [], [(o, False)], [("rank",), ("cume_dist",)], [])
+    o.free()
+    kf = G(rdf.F64, lens, 0, -100.0, 100.0, col_id=63)
+    small = kf.cast(rdf.I8)                                 # 200 partitions, no order
+    kf.free()
+    run("partition i8 (200), no order: sum PARTITION (totals on every row)", [small], [], [("sum", x, "partition")], ["scan"])
+    small.free()
+    x.free()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
     ap.add_argument("--json", default=None)
     ap.add_argument("--csv-rows", type=int, default=50_000_000)
     ap.add_argument("--csv", action="store_true", help="run the CSV reader rows instead of the kernel table")
+    ap.add_argument("--window", action="store_true", help="run only the window-function rows")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.window:
+        rows_out = []
+        window_bench(ctx, args.rows, [4_000_000] * (args.rows // 4_000_000), rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"results": rows_out}, f, indent=1)
+        return
     if args.csv:
         rows_out = []
         csv_bench(ctx, args.csv_rows, rows_out)
@@ -342,6 +428,8 @@ def main():
     hot_r = rdf.Column.upload([P.from_numpy(np.zeros(1_000, np.int64))])
     join_total([hot_l], [hot_r], "inner", "hot key: 1e5 x 1e3 rows of one key (1e8 out)")
     hot_l.free(); hot_r.free()
+    # ---- window functions: sort, key gathers, heads, runs, ranks, the value gather, shift / scan, the gathers back to row order ----
+    window_bench(ctx, args.rows, lens, rows_out)
     if args.json:
         with open(args.json, "w") as f:
             json.dump({"rows": args.rows, "peak_GBs": pk, "peak_source": pk_src, "results": rows_out}, f, indent=1)

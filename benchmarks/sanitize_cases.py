@@ -75,6 +75,15 @@ for dtype in (rdf.I8, rdf.I16, rdf.I32, rdf.I64, rdf.U8, rdf.U16, rdf.U32, rdf.U
     for how in rdf.native.JOIN_TYPES:
         li, ri = rdf.join_indices([rdf.Column.upload(jl), lk2], [rdf.Column.upload(jr), rk2], how)
         li.download(); ri.download()
+    # window functions over the ragged, sliced chunks: heads, runs, ranks, shifts and the three-kernel scan, with and without keys
+    wx = rdf.Column.upload(jl)
+    wk = rdf.Column.upload([P.from_numpy(rng.integers(0, 4, len(wx)).astype(np.int8), rng.random(len(wx)) > 0.1)])
+    wo = rdf.Column.upload([P.from_numpy(rng.integers(0, 9, len(wx)).astype(np.int32))])
+    wcalls = [("row_number",), ("rank",), ("dense_rank",), ("percent_rank",), ("cume_dist",), ("lag", wx, 2), ("lead", wx, 1, 0)] + \
+             [(f, wx, fr) for f in ("sum", "count", "min", "max") for fr in ("rows", "range", "partition")]
+    for part, order in (([wk], [(wo, True)]), ([], []), ([wk], []), ([], [(wo, False)])):
+        for c in rdf.window(part, order, wcalls):
+            c.download()
 # CSV reader: tokenizer scan, field index, record check, inference, parse of every type (exact fallback included), scatter
 import tempfile
 with tempfile.TemporaryDirectory() as td:

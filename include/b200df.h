@@ -348,6 +348,58 @@ typedef enum { BDF_JOIN_LEFT = 0, BDF_JOIN_RIGHT, BDF_JOIN_INNER, BDF_JOIN_FULL 
 int  bdf_join_indices_dev(bdf_ctx* ctx, int32_t join_type, int32_t n_keys, const bdf_col* const* left_keys, const bdf_col* const* right_keys,
                           bdf_col** left_indices, bdf_col** right_indices, int64_t* n_rows);
 
+/* ---- window functions (WindowFunctions, src/functions/window.rs:1-11; WindowSpec, src/window.rs:8-22: stubs in the reference) ----
+ * One call computes n_calls window columns that share one specification, so the rows are sorted once.
+ * Rows and order.  Partitions are the runs of equal tuples of the 0..16 numeric partition_by columns; within a partition rows are
+ *   ordered by the 0..16 numeric order_by columns, each ascending or descending.  Both use the key rules of sort, group-by and join:
+ *   nulls are one value and come last in both directions (as DataFrame::sort puts them), all NaNs are one value greater than every
+ *   number, -0.0 == 0.0.  Peers are rows of a partition with equal order tuples.  Ties are broken by the caller's row order (chunk
+ *   order, then row), which the stable sort keeps, so ROW_NUMBER, LAG / LEAD and the ROWS frame are deterministic where SQL leaves
+ *   them unspecified.
+ * Output.  One chunk per call, in the caller's row order: row r of every output belongs to input row r (a window adds columns to a
+ *   frame, it does not reorder it).  Every output is a new column the caller frees.
+ * Ranking functions (column == NULL; never NULL):
+ *   ROW_NUMBER    UInt32: the 1-based position in the partition.
+ *   RANK          UInt32: 1 + the number of rows of the partition before the first peer.
+ *   DENSE_RANK    UInt32: 1 + the number of distinct peer groups of the partition before this one.
+ *   PERCENT_RANK  Float64: (double)(rank - 1) / (double)(partition rows - 1); 0 for a one-row partition.
+ *   CUME_DIST     Float64: (double)(rows of the partition up to and including the last peer) / (double)(partition rows).
+ *   Both Float64 functions are one IEEE division, so their results are bit-exact.
+ * LAG / LEAD (column x of any numeric type, offset k >= 0): x at the row k positions before / after this row in the partition, in the
+ *   dtype of x.  A row outside the partition gives the default (default_bits: T::Native of x in the low bytes, as bdf_agg4) when
+ *   has_default, else NULL; a row inside whose x is null gives NULL (RESPECT NULLS).  k = 0 is x itself.
+ * Aggregates of x over a frame: ROWS = the first row of the partition through the current row; RANGE = through the current row's last
+ *   peer (SQL's default frame with an ORDER BY); PARTITION = the whole partition (SQL's default without one; also writes a group total
+ *   back onto every row).  Types and null rules are those of bdf_group_by_dev:
+ *   SUM    dtype of x; integers wrap, floats accumulate in double and are rounded once.  Never NULL: a frame without a valid value sums
+ *          to 0, like AggregateFunctions::sum (SQL would give NULL).
+ *   COUNT  Int64: the valid slots of the frame.
+ *   MIN / MAX  dtype of x; NULL without a valid value; floats by the totalOrder rule of bdf_group_by_dev.
+ *   AVG    Float64: the double sum over the count; NULL when the count is 0; Int64 / UInt64 refused.
+ * Degenerate specifications: without order columns every row of a partition is a peer (rank 1; ROWS follows row order); without
+ *   partition columns the whole column is one partition; with neither, nothing is sorted or gathered for ROWS: the aggregates are
+ *   row-order running aggregates over the caller's chunks read in place.
+ * Deterministic: the same inputs give the same bits, float sums included (a segmented scan over a fixed tile decomposition; no atomics
+ *   on values).
+ * Errors (nothing is returned and nothing leaks): n_partition or n_order outside 0..16, n_calls outside 0..64, a null pointer, a
+ *   negative offset, a ranking call with a column, a LAG / LEAD / aggregate call without one, or a call without any column at all (no
+ *   keys and only ranking functions: no rows to number) -> BDF_INVALID; an unknown function or frame, a non-numeric column, AVG of
+ *   Int64 / UInt64 ("avg needs f64: From<T::Native>"), more than 2^32-1 rows (the sort's message), a multi-GPU context ->
+ *   BDF_UNSUPPORTED; columns of different lengths -> BDF_LENGTH_MISMATCH. */
+typedef enum { BDF_WIN_ROW_NUMBER = 0, BDF_WIN_RANK, BDF_WIN_DENSE_RANK, BDF_WIN_PERCENT_RANK, BDF_WIN_CUME_DIST,
+               BDF_WIN_LAG, BDF_WIN_LEAD, BDF_WIN_SUM, BDF_WIN_COUNT, BDF_WIN_MIN, BDF_WIN_MAX, BDF_WIN_AVG } bdf_window_fn;
+typedef enum { BDF_FRAME_ROWS = 0, BDF_FRAME_RANGE, BDF_FRAME_PARTITION } bdf_window_frame;
+typedef struct {
+    int32_t function;        /* bdf_window_fn */
+    int32_t frame;           /* bdf_window_frame; aggregates only */
+    const bdf_col* column;   /* LAG / LEAD / aggregates; NULL for the five ranking functions */
+    int64_t offset;          /* LAG / LEAD, >= 0 */
+    uint64_t default_bits;   /* LAG / LEAD: T::Native of `column` in the low bytes (as bdf_agg4) */
+    int32_t has_default;
+} bdf_window_call;
+int  bdf_window_dev(bdf_ctx* ctx, int32_t n_partition, const bdf_col* const* partition_by, int32_t n_order, const bdf_sort_key* order_by,
+                    int32_t n_calls, const bdf_window_call* calls, bdf_col** out /* n_calls */);
+
 /* ---- N4: Arrow IPC files either side of the path ---------------------------------------------------------------
  * DataFrame::from_arrow (src/dataframe.rs:391-407: arrow::ipc::reader::FileReader, every RecordBatch -> one chunk per
  * column) and DataFrame::to_arrow (:515-525: arrow::ipc::writer::FileWriter).  The file is mapped and its footer, schema
@@ -438,7 +490,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

@@ -62,6 +62,28 @@ pub const BDF_GROUP_LAST: i32 = 7;
 
 #[repr(C)]
 pub struct BdfSortKey { pub column: *const BdfCol, pub descending: i32 }
+/// bdf_window_call (include/b200df.h): one window function over the shared WindowSpec.  `column` is null for the five ranking
+/// functions; `offset` / `default_bits` / `has_default` are LAG / LEAD's, `frame` (bdf_window_frame) the aggregates'.
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct BdfWindowCall { pub function: i32, pub frame: i32, pub column: *const BdfCol, pub offset: i64, pub default_bits: u64, pub has_default: i32 }
+/// bdf_window_fn, in WindowFunctions order, then the aggregates.
+pub const BDF_WIN_ROW_NUMBER: i32 = 0;
+pub const BDF_WIN_RANK: i32 = 1;
+pub const BDF_WIN_DENSE_RANK: i32 = 2;
+pub const BDF_WIN_PERCENT_RANK: i32 = 3;
+pub const BDF_WIN_CUME_DIST: i32 = 4;
+pub const BDF_WIN_LAG: i32 = 5;
+pub const BDF_WIN_LEAD: i32 = 6;
+pub const BDF_WIN_SUM: i32 = 7;
+pub const BDF_WIN_COUNT: i32 = 8;
+pub const BDF_WIN_MIN: i32 = 9;
+pub const BDF_WIN_MAX: i32 = 10;
+pub const BDF_WIN_AVG: i32 = 11;
+/// bdf_window_frame: ROWS = partition start .. current row, RANGE = .. the current row's last peer, PARTITION = the whole partition.
+pub const BDF_FRAME_ROWS: i32 = 0;
+pub const BDF_FRAME_RANGE: i32 = 1;
+pub const BDF_FRAME_PARTITION: i32 = 2;
 pub const BDF_ASYNC: c_int = 1;
 
 /// All four aggregates of one pass (include/b200df.h `bdf_agg4`, ABI version 2: `n_chunks` added).
@@ -122,6 +144,10 @@ extern "C" {
     // columns, NULL = no partner, to take every column of each side with
     pub fn bdf_join_indices_dev(ctx: *mut BdfCtx, join_type: i32, n_keys: i32, left_keys: *const *const BdfCol, right_keys: *const *const BdfCol,
                                 left_indices: *mut *mut BdfCol, right_indices: *mut *mut BdfCol, n_rows: *mut i64) -> c_int;
+    // window functions over one WindowSpec (src/window.rs:8-22; WindowFunctions, src/functions/window.rs:1-11): n_calls one-chunk columns
+    // in the caller's row order, every one the caller's to free
+    pub fn bdf_window_dev(ctx: *mut BdfCtx, n_partition: i32, partition_by: *const *const BdfCol, n_order: i32, order_by: *const BdfSortKey,
+                          n_calls: i32, calls: *const BdfWindowCall, out: *mut *mut BdfCol) -> c_int;
     // CSV files straight to the device (DataFrame::from_csv): rules, departures and memory in include/b200df.h
     pub fn bdf_csv_open(ctx: *mut BdfCtx, path: *const c_char, options: *const BdfCsvOptions, n_schema: i32, schema_dtypes: *const i32,
                         out: *mut *mut BdfCsv) -> c_int;

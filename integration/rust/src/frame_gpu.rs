@@ -187,6 +187,21 @@ pub fn join_device(left: &DeviceColumns, right: &DeviceColumns, criteria: &[(usi
     Ok(out)
 }
 
+/// Window functions over one `WindowSpec` (src/window.rs:8-22, not in lib.rs; `WindowFunctions`, src/functions/window.rs:1-11, empty
+/// bodies): `partition` are column indices of `frame`, `order` (column index, descending) pairs, `calls` (output name, call) with
+/// `call.column` a column pointer of `frame` or null for a ranking function.  The rows are sorted once for all calls.  Returns the new
+/// columns only, one chunk each in the frame's row order, named by `calls`; the caller appends them as `DataFrame::with_column` does
+/// (an existing name is replaced), so the frame's own columns are never copied.  Rules and departures: include/b200df.h.
+pub fn window_device(frame: &DeviceColumns, partition: &[usize], order: &[(usize, bool)], calls: &[(String, BdfWindowCall)]) -> Result<DeviceColumns, String> {
+    let part: Vec<*const BdfCol> = partition.iter().map(|p| frame.cols[*p] as *const BdfCol).collect();
+    let ord: Vec<BdfSortKey> = order.iter().map(|(c, d)| BdfSortKey { column: frame.cols[*c], descending: *d as i32 }).collect();
+    let spec: Vec<BdfWindowCall> = calls.iter().map(|(_, c)| *c).collect();
+    let mut out = vec![std::ptr::null_mut(); spec.len()];
+    check(unsafe { bdf_window_dev(dev(), part.len() as i32, part.as_ptr(), ord.len() as i32, ord.as_ptr(), spec.len() as i32, spec.as_ptr(),
+                                  out.as_mut_ptr()) })?;
+    Ok(DeviceColumns { names: calls.iter().map(|(n, _)| n.clone()).collect(), cols: out })
+}
+
 /// `DataFrame::from_csv(path, None)` on the device: a header, ',', the schema inferred from every record, 1024 rows per
 /// RecordBatch (`schema`: one dtype per column instead, BDF_UTF8 for a string column).  Utf8 columns are not on the device path and
 /// are left out; a caller that needs them reads just those with arrow's CPU reader and a projection

@@ -20,8 +20,9 @@ ADD, SUB, MUL, DIV, ATAN2, HYPOT, LOG = range(7)
 SUM, MIN, MAX, COUNT = range(4)
 OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID, PARSE = range(10)
 ASYNC = 1
-K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV = range(14)
-KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv"]
+K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW = range(15)
+KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
+                "window"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -34,6 +35,14 @@ GROUP_FNS = {"sum": GROUP_SUM, "max": GROUP_MAX, "min": GROUP_MIN, "avg": GROUP_
 # bdf_join_type (JoinType order)
 JOIN_LEFT, JOIN_RIGHT, JOIN_INNER, JOIN_FULL = range(4)
 JOIN_TYPES = {"left": JOIN_LEFT, "right": JOIN_RIGHT, "inner": JOIN_INNER, "full": JOIN_FULL}
+# bdf_window_fn / bdf_window_frame
+(WIN_ROW_NUMBER, WIN_RANK, WIN_DENSE_RANK, WIN_PERCENT_RANK, WIN_CUME_DIST, WIN_LAG, WIN_LEAD, WIN_SUM, WIN_COUNT, WIN_MIN, WIN_MAX,
+ WIN_AVG) = range(12)
+WINDOW_FNS = {"row_number": WIN_ROW_NUMBER, "rank": WIN_RANK, "dense_rank": WIN_DENSE_RANK, "percent_rank": WIN_PERCENT_RANK,
+              "cume_dist": WIN_CUME_DIST, "lag": WIN_LAG, "lead": WIN_LEAD, "sum": WIN_SUM, "count": WIN_COUNT, "min": WIN_MIN,
+              "max": WIN_MAX, "avg": WIN_AVG}
+FRAME_ROWS, FRAME_RANGE, FRAME_PARTITION = range(3)
+WINDOW_FRAMES = {"rows": FRAME_ROWS, "range": FRAME_RANGE, "partition": FRAME_PARTITION}
 
 
 class View(C.Structure):
@@ -65,6 +74,11 @@ class GroupOut(C.Structure):
 
 class GroupAggC(C.Structure):
     _fields_ = [("column", C.c_void_p), ("function", C.c_int32)]
+
+
+class WindowCall(C.Structure):
+    _fields_ = [("function", C.c_int32), ("frame", C.c_int32), ("column", C.c_void_p), ("offset", C.c_int64), ("default_bits", C.c_uint64),
+                ("has_default", C.c_int32)]
 
 
 class CsvOptions(C.Structure):
@@ -166,6 +180,7 @@ def lib() -> C.CDLL:
         "bdf_group_aggregate_dev": ([vp, vp, i32, P(vp), P(vp), P(GroupOut), P(i64)], C.c_int),
         "bdf_group_by_dev": ([vp, i32, P(vp), i32, P(GroupAggC), P(vp), P(vp), P(i64)], C.c_int),
         "bdf_join_indices_dev": ([vp, i32, i32, P(vp), P(vp), P(vp), P(vp), P(i64)], C.c_int),
+        "bdf_window_dev": ([vp, i32, P(vp), i32, P(SortKeyC), i32, P(WindowCall), P(vp)], C.c_int),
         "bdf_compare_dev": ([vp, C.c_int, vp, vp, C.c_double, P(vp)], C.c_int),
         "bdf_boolean_dev": ([vp, C.c_int, vp, vp, P(vp)], C.c_int),
         "bdf_filter_dev": ([vp, vp, vp, P(vp)], C.c_int),
@@ -219,7 +234,7 @@ EXPORTED_SYMBOLS = [
     "bdf_host_alloc", "bdf_host_free", "bdf_host_register", "bdf_host_unregister", "bdf_binary", "bdf_unary", "bdf_cast",
     "bdf_aggregate", "bdf_aggregate_all", "bdf_avg", "bdf_upload", "bdf_upload_many", "bdf_col_wait", "bdf_col_describe",
     "bdf_col_chunk_info", "bdf_binary_dev", "bdf_unary_dev", "bdf_cast_dev", "bdf_aggregate_dev",
-    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_join_indices_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
+    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_join_indices_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
     "bdf_binary_agg_dev", "bdf_binary_agg_dev_async", "bdf_aggregate_all_dev_async", "bdf_future_wait", "bdf_col_free", "bdf_profile_enable", "bdf_profile_read",
     "bdf_launch_count", "bdf_timer_start", "bdf_timer_stop", "bdf_flush_l2", "bdf_generate",
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",

@@ -16,14 +16,14 @@
 //                   work list and k_group_big folds it one CTA per 64 Ki-row segment (thread-strided fold + fixed block
 //                   tree), k_group_big_finish then folds a group's segment partials in segment order -- still deterministic,
 //                   and a single hot key is spread over the whole GPU instead of one warp.  The EXTRA instantiations carry
-//                   what only bdf_group_by_dev asks for (GroupAggX below); the others fold exactly what they always did.
+//                   what only bdf_group_by_dev asks for (GroupAggX, group_acc.cuh); the others fold exactly what they always did.
 //                   In a 1- or 8-lane launch a group longer than kLaneRows rows per lane goes to a second list instead, and
 //                   k_group_medium folds each of those with a warp (the 32-lane order and tree), so a few long groups among
 //                   many one-row groups do not leave single threads walking tens of thousands of rows.
 //   k_group_bounds  the original row number of every group's first and last row (first / last: a take of those rows).
 //   k_group_distinct  one thread per group: the number of distinct-value heads inside the group's row range, by two
 //                   binary searches over their compacted positions -- O(log n) per group, a hot key needs nothing special.
-#include "common.cuh"
+#include "group_acc.cuh"
 
 namespace bdf {
 
@@ -70,55 +70,6 @@ k_group_heads(const __grid_constant__ HeadKeys keys, long long n, uint32_t* __re
 }
 
 // ---- (b) per-group fold -------------------------------------------------------------------------------------------------
-// The accumulator of the EXTRA instantiations (FusedAgg<T> itself stays as K4/K5 use it).  Integers: FusedAgg's wrapping sum
-// and min/max keys plus a double sum for avg.  Floats: FusedAgg's double sum (which is also avg's numerator) plus min/max
-// over order-preserving unsigned keys of the IEEE totalOrder with every NaN made the positive quiet NaN.
-template <typename T> struct FloatKey;
-template <> struct FloatKey<float> {
-    static __device__ __forceinline__ unsigned long long key(float x) {
-        const unsigned int u = x != x ? 0x7fc00000u : __float_as_uint(x);
-        return (unsigned long long)((u & 0x80000000u) ? ~u : (u | 0x80000000u));
-    }
-    static __device__ __forceinline__ float value(unsigned long long k) {
-        const unsigned int u = (unsigned int)k;
-        return __uint_as_float((u & 0x80000000u) ? (u ^ 0x80000000u) : ~u);
-    }
-};
-template <> struct FloatKey<double> {
-    static __device__ __forceinline__ unsigned long long key(double x) {
-        const unsigned long long u = x != x ? 0x7ff8000000000000ull : (unsigned long long)__double_as_longlong(x);
-        return (u >> 63) ? ~u : (u | (1ull << 63));
-    }
-    static __device__ __forceinline__ double value(unsigned long long k) {
-        return __longlong_as_double((long long)((k >> 63) ? (k ^ (1ull << 63)) : ~k));
-    }
-};
-
-template <typename T, bool F = IsFloat<T>::value> struct GroupAggX;
-template <typename T> struct GroupAggX<T, false> {
-    FusedAgg<T> a;
-    double dsum;
-    __device__ __forceinline__ void init() { a.init(); dsum = 0.0; }
-    __device__ __forceinline__ void add(T x, bool valid, unsigned long long flip) { a.add(x, valid, flip); dsum = __dadd_rn(dsum, valid ? (double)x : 0.0); }
-    __device__ __forceinline__ void merge_shfl(int o) { a.merge_shfl(o); dsum = __dadd_rn(dsum, __shfl_xor_sync(0xffffffffu, dsum, o)); }
-    __device__ __forceinline__ void merge(const GroupAggX& o) { a.merge(o.a); dsum = __dadd_rn(dsum, o.dsum); }
-};
-template <typename T> struct GroupAggX<T, true> {
-    double sum;
-    unsigned long long kmin, kmax;
-    __device__ __forceinline__ void init() { sum = 0.0; kmin = ~0ull; kmax = 0; }
-    __device__ __forceinline__ void add(T x, bool valid, unsigned long long) {
-        sum = __dadd_rn(sum, valid ? (double)x : 0.0);
-        if (valid) { const unsigned long long k = FloatKey<T>::key(x); kmin = k < kmin ? k : kmin; kmax = k > kmax ? k : kmax; }
-    }
-    __device__ __forceinline__ void merge_shfl(int o) {
-        const double s2 = __shfl_xor_sync(0xffffffffu, sum, o);
-        const unsigned long long a2 = __shfl_xor_sync(0xffffffffu, kmin, o), b2 = __shfl_xor_sync(0xffffffffu, kmax, o);
-        sum = __dadd_rn(sum, s2); kmin = a2 < kmin ? a2 : kmin; kmax = b2 > kmax ? b2 : kmax;
-    }
-    __device__ __forceinline__ void merge(const GroupAggX& o) { sum = __dadd_rn(sum, o.sum); kmin = o.kmin < kmin ? o.kmin : kmin; kmax = o.kmax > kmax ? o.kmax : kmax; }
-};
-
 template <typename T, bool EXTRA> struct GroupAcc { using type = FusedAgg<T>; };
 template <typename T> struct GroupAcc<T, true> { using type = GroupAggX<T>; };
 
@@ -134,10 +85,6 @@ struct BigWork { unsigned int n_groups, n_segments, n_medium; BigGroup list[1]; 
 // thread must not walk tens of thousands of rows while its neighbours are done after one.
 constexpr long long kLaneRows = 512;
 static_assert(sizeof(GroupAggX<long long>) <= kPartBytes && sizeof(GroupAggX<double>) <= kPartBytes && sizeof(FusedAgg<long long>) <= kPartBytes, "partials");
-
-template <typename T> struct GroupFlip {
-    static constexpr unsigned long long value = IsFloat<T>::value ? 0ull : (((T)-1 < (T)0) ? (1ull << (8 * sizeof(T) - 1)) : 0ull);
-};
 
 template <typename T, bool EXTRA>
 __device__ __forceinline__ void group_write(const typename GroupAcc<T, EXTRA>::type& acc, unsigned long long cnt, long long g, const GroupOuts<T>& o,

@@ -1813,23 +1813,31 @@ cudaError_t launch_group_distinct(const uint32_t* pos, long long n_pos, const ui
 size_t group_big_scratch_bytes(long long n_rows);
 }  // namespace bdf
 
-// Head bitmap (a boolean column of n rows) over one-chunk columns in sorted order.
-static int group_heads(bdf_ctx* c, const std::vector<const bdf_col*>& cols, bool and_last_valid, int64_t n, bdf_col** out) {
+// Head bitmap (a boolean column of n rows) over one-chunk columns in sorted order.  kernel >= 0: the launch gets a launch record
+// under that bdf_kernel_id (the window's heads); group-by and join keep theirs unrecorded.
+static int group_heads(bdf_ctx* c, const std::vector<const bdf_col*>& cols, bool and_last_valid, int64_t n, bdf_col** out, int kernel = -1) {
     ColOwner head(c);
     TRY(col_alloc(c, kBool, {ChunkPlan{n, false}}, nullptr, 0, head.out()));
     std::vector<const void*> vals(cols.size());
     std::vector<const uint32_t*> valid(cols.size());
     std::vector<int> widths(cols.size()), is_float(cols.size());
+    int64_t key_bytes = 0;
     for (size_t k = 0; k < cols.size(); k++) {
         wait_groups(c->s_compute, cols[k], 0, 1);
         vals[k] = cols[k]->chunks[0].values;
         valid[k] = cols[k]->chunks[0].validity;
         widths[k] = dtype_width(cols[k]->dtype);
         is_float[k] = dtype_is_float(cols[k]->dtype) ? 1 : 0;
+        key_bytes += widths[k];
     }
-    c->launches++;
-    cudaError_t e = launch_group_heads((int)cols.size(), vals.data(), valid.data(), widths.data(), is_float.data(), and_last_valid ? 1 : 0, n,
-                                       (uint32_t*)head->chunks[0].values, c->s_compute);
+    cudaError_t e;
+    {
+        std::unique_ptr<LaunchTimer> t;
+        if (kernel >= 0) t.reset(new LaunchTimer(c, kernel, kBool, n, n * key_bytes + bitmap_bytes(n)));
+        else c->launches++;
+        e = launch_group_heads((int)cols.size(), vals.data(), valid.data(), widths.data(), is_float.data(), and_last_valid ? 1 : 0, n,
+                               (uint32_t*)head->chunks[0].values, c->s_compute);
+    }
     if (e == cudaSuccess) e = finish_single_group(c, head.get());
     if (e != cudaSuccess) return fail_cuda(e, "group heads");
     *out = head.release();
@@ -2190,6 +2198,258 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
     *out_l = swap ? b : p;
     *out_r = swap ? p : b;
     if (n_rows_out) *n_rows_out = (int64_t)n_out;
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// window functions (k_window.cu): the rows are sorted by (partition keys, order keys) once for all calls; the partition heads (P) and
+// the peer heads (Q = P OR the order keys' heads) are marked with k_group_heads, and each gets a per-word prefix of its runs and the
+// compacted run starts, so a position finds its partition and peer bounds in O(1).  Ranking functions are written straight to row
+// order through the permutation; lag / lead and the scans work in sorted order and come back through one take each, whose index
+// is the frame's last sorted position of every row.  Without any key nothing is sorted: the kernels read the caller's chunks in place.
+
+namespace bdf {
+int window_count_tile();
+cudaError_t launch_window_count(const uint32_t* words, long long n_words, unsigned long long* counts, unsigned long long* block_sums, cudaStream_t s);
+cudaError_t launch_window_rank(const void* const* p, long long n_p, const void* const* q, long long n_q, long long n, const uint32_t* perm,
+                               void* const* outs, cudaStream_t s);
+cudaError_t launch_window_shift(int dtype, const void* const* p, long long n_p, long long n, const void* x, int nx, long long k, int lead,
+                                unsigned long long def_bits, int has_def, void* out, uint32_t* vout, cudaStream_t s);
+size_t window_scan_scratch_bytes(long long n);
+cudaError_t launch_window_scan(int dtype, int fn, const void* x, int nx, const uint32_t* heads, long long n, void* scratch, void* out, uint32_t* vout,
+                               cudaStream_t s);
+}  // namespace bdf
+
+// One head bitmap and what k_window needs to find the run of a position in O(1).
+struct WinHeadsHost {
+    explicit WinHeadsHost(bdf_ctx* c) : bits(c), starts(c) {}
+    ColOwner bits;                        // bit i: sorted position i starts a run
+    Scratch<unsigned long long> prefix;   // per head word: the runs that start before it
+    ColOwner starts;                      // the first position of every run
+    int64_t n_runs = 0;
+    const void* arrays[3] = {nullptr, nullptr, nullptr};   // {words, prefix, starts} as the kernels take them
+};
+
+static int window_runs(bdf_ctx* c, const bdf_col* iota, int64_t n, WinHeadsHost* h) {
+    const int64_t words = (n + 31) / 32;
+    const int64_t blocks = (words + window_count_tile() - 1) / window_count_tile();
+    Scratch<unsigned long long> block_sums;
+    cudaError_t e = h->prefix.alloc(c, (size_t)(words + 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_WINDOW, BDF_U64, n, words * (4 + 8 + 16));   // popcounts written, then read and written by the scan
+        c->launches += 2;                                                       // the scan's two kernels
+        e = launch_window_count((const uint32_t*)h->bits->chunks[0].values, words, h->prefix, block_sums, c->s_compute);
+        if (e == cudaSuccess) e = launch_join_scan(h->prefix, words, block_sums, c->s_compute);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "window run prefix");
+    TRY(filter_dev(c, iota, h->bits.get(), h->starts.out()));
+    h->n_runs = h->starts->chunks[0].len;
+    h->arrays[0] = h->bits->chunks[0].values;
+    h->arrays[1] = h->prefix.get();
+    h->arrays[2] = h->starts->chunks[0].values;
+    return BDF_OK;
+}
+
+static bool win_is_rank(int f) { return f >= BDF_WIN_ROW_NUMBER && f <= BDF_WIN_CUME_DIST; }
+static bool win_is_shift(int f) { return f == BDF_WIN_LAG || f == BDF_WIN_LEAD; }
+
+static int win_out_dtype(const bdf_window_call& k) {
+    switch (k.function) {
+        case BDF_WIN_ROW_NUMBER: case BDF_WIN_RANK: case BDF_WIN_DENSE_RANK: return BDF_U32;
+        case BDF_WIN_PERCENT_RANK: case BDF_WIN_CUME_DIST: case BDF_WIN_AVG: return BDF_F64;
+        case BDF_WIN_COUNT: return BDF_I64;
+        default: return k.column->dtype;
+    }
+}
+
+static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_order, const bdf_sort_key* order, int n_calls,
+                      const bdf_window_call* calls, bdf_col** out) {
+    if (n_part < 0 || n_part > 16 || n_order < 0 || n_order > 16) return fail(BDF_INVALID, "0..16 partition and 0..16 order columns");
+    if (n_calls < 0 || n_calls > 64) return fail(BDF_INVALID, "0..64 window calls");
+    if ((n_part && !part) || (n_order && !order) || (n_calls && (!calls || !out))) return fail(BDF_INVALID, "null argument");
+    std::vector<const bdf_col*> cols;   // every column of the call, for the type and length checks
+    for (int k = 0; k < n_part; k++) cols.push_back(part[k]);
+    for (int k = 0; k < n_order; k++) cols.push_back(order[k].column);
+    for (const bdf_col* x : cols)
+        if (!x) return fail(BDF_INVALID, "null partition or order column");
+    for (int j = 0; j < n_calls; j++) {
+        const bdf_window_call& k = calls[j];
+        if (k.function < BDF_WIN_ROW_NUMBER || k.function > BDF_WIN_AVG) return fail(BDF_UNSUPPORTED, "unknown window function %d", k.function);
+        if (win_is_rank(k.function) && k.column) return fail(BDF_INVALID, "a ranking function takes no column");
+        if (!win_is_rank(k.function) && !k.column) return fail(BDF_INVALID, "lag, lead and the aggregates need a column");
+        if (win_is_shift(k.function) && k.offset < 0) return fail(BDF_INVALID, "lag / lead offset must be >= 0");
+        if (!win_is_rank(k.function) && !win_is_shift(k.function) && (k.frame < BDF_FRAME_ROWS || k.frame > BDF_FRAME_PARTITION))
+            return fail(BDF_UNSUPPORTED, "unknown window frame %d", k.frame);
+        if (k.column) cols.push_back(k.column);
+    }
+    for (const bdf_col* x : cols)
+        if (x->dtype < 0 || x->dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "window columns must be numeric");
+    for (int j = 0; j < n_calls; j++)
+        if (calls[j].function == BDF_WIN_AVG && (calls[j].column->dtype == BDF_I64 || calls[j].column->dtype == BDF_U64))
+            return fail(BDF_UNSUPPORTED, "avg needs f64: From<T::Native>");
+    if (cols.empty()) {
+        if (n_calls == 0) return BDF_OK;
+        return fail(BDF_INVALID, "a window without partition, order or value columns has no rows to number");
+    }
+    for (const bdf_col* x : cols)
+        if (x->total_len != cols[0]->total_len) return fail(BDF_LENGTH_MISMATCH, "window columns have different lengths");
+    const int64_t n = cols[0]->total_len;
+    if (n > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
+    if (n_calls == 0) return BDF_OK;
+
+    std::vector<ColOwner> res;
+    for (int j = 0; j < n_calls; j++) res.emplace_back(c);
+    cudaError_t e = cudaSuccess;
+    if (n == 0) {
+        for (int j = 0; j < n_calls; j++) {
+            TRY(col_alloc(c, win_out_dtype(calls[j]), {ChunkPlan{0, false}}, nullptr, 0, res[j].out()));
+            e = finish_single_group(c, res[j].get());
+            if (e != cudaSuccess) return fail_cuda(e, "window");
+        }
+        for (int j = 0; j < n_calls; j++) out[j] = res[j].release();
+        return BDF_OK;
+    }
+
+    // what the calls need: peer bounds, and the gather index of each frame
+    const bool sorted = n_part + n_order > 0;
+    bool need_q = false, need_inv = false, need_range = false, need_part = false;
+    for (int j = 0; j < n_calls; j++) {
+        const int f = calls[j].function;
+        if (f == BDF_WIN_RANK || f == BDF_WIN_DENSE_RANK || f == BDF_WIN_PERCENT_RANK || f == BDF_WIN_CUME_DIST) need_q = true;
+        else if (win_is_shift(f)) need_inv = need_inv || sorted;
+        else if (!win_is_rank(f)) {
+            const int fr = calls[j].frame;
+            if (fr == BDF_FRAME_ROWS) need_inv = need_inv || sorted;
+            else if (fr == BDF_FRAME_RANGE && sorted) { need_q = true; need_range = true; }
+            else need_part = true;   // PARTITION, and RANGE without keys: every row is a peer
+        }
+    }
+    const bool has_p = n_part > 0, has_q = need_q && n_order > 0;
+
+    ColOwner perm(c), iota(c);
+    WinHeadsHost P(c), Q(c);
+    if (sorted) {
+        std::vector<bdf_sort_key> sk;
+        for (int k = 0; k < n_part; k++) sk.push_back(bdf_sort_key{part[k], 0});
+        for (int k = 0; k < n_order; k++) sk.push_back(order[k]);
+        TRY(sort_indices_dev(c, (int)sk.size(), sk.data(), perm.out()));
+        TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, iota.out()));
+        c->launches++;
+        e = launch_iota((uint32_t*)iota->chunks[0].values, n, c->sm_count, c->s_compute);
+        if (e == cudaSuccess) e = finish_single_group(c, iota.get());
+        if (e != cudaSuccess) return fail_cuda(e, "window iota");
+        // the two bitmaps take two launches: 16 + 16 keys exceed what one k_group_heads compares
+        auto heads_of = [&](int k0, int k1, bdf_col** h) -> int {
+            std::vector<ColOwner> keys;
+            std::vector<const bdf_col*> sorted_keys;
+            for (int k = k0; k < k1; k++) {
+                keys.emplace_back(c);
+                TRY(take_dev(c, sk[k].column, perm.get(), keys.back().out()));
+                sorted_keys.push_back(keys.back().get());
+            }
+            return group_heads(c, sorted_keys, false, n, h, BDF_K_WINDOW);
+        };
+        if (has_p) {
+            TRY(heads_of(0, n_part, P.bits.out()));
+            TRY(window_runs(c, iota.get(), n, &P));
+        }
+        if (has_q) {
+            ColOwner oh(c);
+            TRY(heads_of(n_part, n_part + n_order, oh.out()));
+            if (has_p) TRY(boolean_dev(c, BDF_OR, P.bits.get(), oh.get(), Q.bits.out()));
+            else Q.bits = std::move(oh);
+            TRY(window_runs(c, iota.get(), n, &Q));
+        }
+    }
+    const void* const* p_arrays = has_p ? P.arrays : nullptr;
+    const uint32_t* perm_d = sorted ? (const uint32_t*)perm->chunks[0].values : nullptr;
+
+    // ranking functions (the first call of each; a repeated call gets a copy) and the gather indices, in one pass
+    int first_of[5] = {-1, -1, -1, -1, -1};
+    void* rank_outs[8] = {};
+    ColOwner inv(c), range_end(c), part_end(c);
+    int64_t u32_outs = 0, f64_outs = 0;
+    for (int j = 0; j < n_calls; j++) {
+        const int f = calls[j].function;
+        if (!win_is_rank(f) || first_of[f] >= 0) continue;
+        first_of[f] = j;
+        TRY(col_alloc(c, win_out_dtype(calls[j]), {ChunkPlan{n, false}}, nullptr, 0, res[j].out()));
+        rank_outs[f] = res[j]->chunks[0].values;
+        (win_out_dtype(calls[j]) == BDF_F64 ? f64_outs : u32_outs)++;
+    }
+    ColOwner* const index_cols[3] = {&inv, &range_end, &part_end};
+    const bool need_index[3] = {need_inv, need_range, need_part};
+    for (int k = 0; k < 3; k++)
+        if (need_index[k]) {
+            TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, index_cols[k]->out()));
+            rank_outs[5 + k] = (*index_cols[k])->chunks[0].values;
+            u32_outs++;
+        }
+    if (u32_outs + f64_outs) {
+        LaunchTimer t(c, BDF_K_WINDOW, BDF_U32, n, n * ((sorted ? 4 : 0) + (has_p ? 8 : 0) + (has_q ? 16 : 0) + 4 * u32_outs + 8 * f64_outs));
+        e = launch_window_rank(p_arrays, P.n_runs, has_q ? Q.arrays : nullptr, Q.n_runs, n, perm_d, rank_outs, c->s_compute);
+    }
+    for (int j = 0; j < n_calls && e == cudaSuccess; j++)
+        if (res[j].get()) e = finish_single_group(c, res[j].get());
+    for (int k = 0; k < 3 && e == cudaSuccess; k++)
+        if (index_cols[k]->get()) e = finish_single_group(c, index_cols[k]->get());
+    if (e != cudaSuccess) return fail_cuda(e, "window ranks");
+    for (int j = 0; j < n_calls; j++)
+        if (win_is_rank(calls[j].function) && first_of[calls[j].function] != j) TRY(group_clone(c, res[first_of[calls[j].function]].get(), res[j].out()));
+
+    // lag / lead and the scans read x in sorted order: one gather per distinct column
+    std::vector<std::pair<const bdf_col*, ColOwner>> gathered;
+    auto source = [&](const bdf_col* x, const bdf_col** src) -> int {
+        if (!sorted) { *src = x; return BDF_OK; }
+        for (auto& g : gathered)
+            if (g.first == x) { *src = g.second.get(); return BDF_OK; }
+        gathered.emplace_back(x, ColOwner(c));
+        TRY(take_dev(c, x, perm.get(), gathered.back().second.out()));
+        *src = gathered.back().second.get();
+        return BDF_OK;
+    };
+    for (int j = 0; j < n_calls; j++) {
+        const bdf_window_call& k = calls[j];
+        if (win_is_rank(k.function)) continue;
+        const bdf_col* src = nullptr;
+        TRY(source(k.column, &src));
+        void* table = nullptr;
+        int n_chunks = 0;
+        bool nullable = false;
+        TRY(sort_table(c, src, &table, &n_chunks, &nullable));
+        const int dt = k.column->dtype, w = dtype_width(dt);
+        ColOwner tmp(c);
+        const bdf_col* idx = nullptr;   // sorted order back to row order; null: tmp already is in row order
+        if (win_is_shift(k.function)) {
+            TRY(col_alloc(c, dt, {ChunkPlan{n, true}}, nullptr, 0, tmp.out()));
+            LaunchTimer t(c, BDF_K_WINDOW, dt, n, n * (2 * w + (has_p ? 8 : 0)) + (nullable ? bitmap_bytes(n) : 0) + bitmap_bytes(n));
+            e = launch_window_shift(dt, p_arrays, P.n_runs, n, table, n_chunks, k.offset, k.function == BDF_WIN_LEAD ? 1 : 0, k.default_bits,
+                                    k.has_default ? 1 : 0, tmp->chunks[0].values, tmp->chunks[0].validity, c->s_compute);
+            idx = inv.get();
+        } else {
+            const int fn = k.function - BDF_WIN_SUM;   // SUM, COUNT, MIN, MAX, AVG: the order of k_window.cu's scans
+            const int od = win_out_dtype(k);
+            const bool out_nullable = k.function == BDF_WIN_MIN || k.function == BDF_WIN_MAX || k.function == BDF_WIN_AVG;
+            TRY(col_alloc(c, od, {ChunkPlan{n, out_nullable}}, nullptr, 0, tmp.out()));
+            Scratch<void> scratch;
+            e = scratch.alloc(c, window_scan_scratch_bytes(n));
+            if (e == cudaSuccess) {
+                LaunchTimer t(c, BDF_K_WINDOW, od, n, n * (w + dtype_width(od)) + (nullable ? bitmap_bytes(n) : 0) + (has_p ? bitmap_bytes(n) : 0) +
+                                                       (out_nullable ? bitmap_bytes(n) : 0));
+                c->launches += 2;   // tile reduce, carry scan, tile rescan
+                e = launch_window_scan(dt, fn, table, n_chunks, has_p ? (const uint32_t*)P.arrays[0] : nullptr, n, scratch, tmp->chunks[0].values,
+                                       out_nullable ? tmp->chunks[0].validity : nullptr, c->s_compute);
+            }
+            idx = k.frame == BDF_FRAME_ROWS ? inv.get() : (k.frame == BDF_FRAME_RANGE && sorted) ? range_end.get() : part_end.get();
+        }
+        if (e == cudaSuccess) e = finish_single_group(c, tmp.get());
+        if (e != cudaSuccess) return fail_cuda(e, "window");
+        if (tmp->chunks[0].validity) tmp->null_counts[0] = -1;   // learnt on demand (ensure_null_counts)
+        if (idx) TRY(take_dev(c, tmp.get(), idx, res[j].out()));
+        else res[j] = std::move(tmp);
+    }
+    for (int j = 0; j < n_calls; j++) out[j] = res[j].release();
     return BDF_OK;
 }
 
@@ -3780,6 +4040,13 @@ int bdf_join_indices_dev(bdf_ctx* c, int32_t join_type, int32_t n_keys, const bd
     ENTER(c);
     if (!left_indices || !right_indices) return fail(BDF_INVALID, "null argument");
     return join_dev(c, join_type, n_keys, left_keys, right_keys, left_indices, right_indices, n_rows);
+}
+
+int bdf_window_dev(bdf_ctx* c, int32_t n_partition, const bdf_col* const* partition_by, int32_t n_order, const bdf_sort_key* order_by,
+                   int32_t n_calls, const bdf_window_call* calls, bdf_col** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "a window moves rows between chunks: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return window_dev(c, n_partition, partition_by, n_order, order_by, n_calls, calls, out);
 }
 
 int bdf_csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* options, int32_t n_schema, const int32_t* schema_dtypes, bdf_csv** out) {

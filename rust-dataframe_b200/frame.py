@@ -21,7 +21,9 @@ first rows into one chunk (the reference slices chunks zero-copy).  Join (``Devi
 criteria, how))`` step) plans the schema ``Dataset::try_join`` plans and takes every column by the index pairs of
 ``bdf_join_indices_dev``, whose order is defined where the reference's is not (src/functions/join.rs emits its pairs in
 HashMap iteration order): left rows in row order, each one's partners in right row order; a null key matches nothing, and
-FULL is the SQL full outer join (include/b200df.h lists the five departures).
+FULL is the SQL full outer join (include/b200df.h lists the five departures).  Window functions (``DeviceFrame.window``, the
+``("window", (partition_by, order_by, calls))`` step) add one column per call in the frame's row order, as ``with_column`` does; the
+reference declares WindowSpec and WindowFunctions without bodies (src/window.rs:8-22, src/functions/window.rs:1-11).
 """
 from __future__ import annotations
 
@@ -34,7 +36,7 @@ import numpy as np
 
 from . import _native as N
 from .arrays import F32, F64, I8, I64, U8, U32, U64, PrimitiveArray, is_float
-from .functions import Column, _expr_nodes, eval_expr, sort_indices
+from .functions import Column, _expr_nodes, eval_expr, sort_indices, window as _window
 from .csv_reader import CsvFile
 from .ipc import BOOL, IpcFile, write_ipc
 
@@ -160,6 +162,47 @@ def plan_join(schema_a: Dict[str, int], schema_b: Dict[str, int], criteria: Sequ
     return out + [(f"b.{n}" if n in schema_a else n, t) for n, t in schema_b.items()]
 
 
+def window(partition_by: Sequence[str], order_by: Sequence[Tuple[str, bool]], calls: Sequence[tuple]):
+    """Window functions over one WindowSpec: ``calls`` are ``(output, function, *arguments)`` with column arguments by name, e.g.
+    ``("r", "rank")``, ``("prev", "lag", "x", 1, 0.0)`` or ``("s", "sum", "x", "range")`` (see functions.window)."""
+    return ("window", (list(partition_by), [(c, bool(d)) for c, d in order_by], [tuple(c) for c in calls]))
+
+
+WINDOW_RANKING = {"row_number": U32, "rank": U32, "dense_rank": U32, "percent_rank": F64, "cume_dist": F64}
+
+
+def _window_columns(partition_by, order_by, calls) -> List[str]:
+    return list(partition_by) + [c for c, _ in order_by] + [c[2] for c in calls if c[1] not in WINDOW_RANKING and len(c) > 2]
+
+
+def plan_window(schema: Dict[str, int], partition_by: Sequence[str], order_by: Sequence[Tuple[str, bool]], calls: Sequence[tuple]) -> List[Tuple[str, int]]:
+    """The frame after a window step, as [(name, dtype)]: the frame's columns, then every call's output in call order; an output
+    whose name exists replaces that column in place of the old one at the end, as with_column does.  A missing column is a
+    ComputeError; an unknown function, a non-numeric column and avg of Int64 / UInt64 are UnsupportedType.  Output types: UInt32
+    for row_number / rank / dense_rank, Float64 for percent_rank / cume_dist / avg, Int64 for count, the column's type otherwise."""
+    for name in _window_columns(partition_by, order_by, calls):
+        if name not in schema:
+            raise N.ComputeError(f"Window column {json.dumps(name)} does not exist")
+    out = OrderedDict(schema)
+    for call in calls:
+        fn = call[1]
+        if fn not in N.WINDOW_FNS:
+            raise N.UnsupportedType(f"window function {fn!r} is not one of {sorted(N.WINDOW_FNS)}")
+        if fn not in WINDOW_RANKING and len(call) < 3:
+            raise N.ComputeError(f"{fn} needs a column")
+    for name in _window_columns(partition_by, order_by, calls):
+        if schema[name] == BOOL or not 0 <= schema[name] <= F64:
+            raise N.UnsupportedType(f"column {name!r} is not numeric: window keys and values must be")
+    for call in calls:
+        fn = call[1]
+        if fn == "avg" and schema[call[2]] in (I64, U64):
+            raise N.UnsupportedType("avg needs f64: From<T::Native>")
+        t = WINDOW_RANKING.get(fn, F64 if fn == "avg" else I64 if fn == "count" else schema[call[2]] if len(call) > 2 else None)
+        out.pop(call[0], None)
+        out[call[0]] = t
+    return list(out.items())
+
+
 # ---- BooleanFilter (expression.rs:752-763) as nested tuples: ("col", name) | ("scalar", v) | ("not", x) | ("and", a, b) | ("gt", a, b) ...
 def col(name: str):
     return ("col", name)
@@ -193,6 +236,8 @@ def _columns_read(t) -> set:
         return _filter_columns(arg)
     if kind == "sort":
         return {c for c, _ in arg}
+    if kind == "window":
+        return set(_window_columns(*arg))
     return set()
 
 
@@ -212,7 +257,9 @@ def _needed_after(transformations: Sequence[tuple], final_columns: Sequence[str]
                 live = (live - {arg.output}) | {arg.inputs[0]}
             else:
                 live = (live - {arg.output}) | set(arg.inputs)   # a Calculation is kept even when its output is dead:
-        else:                                                   # its DivideByZero panic is observable
+        elif kind == "window":                                  # its DivideByZero panic is observable
+            live = (live - {c[0] for c in arg[2]}) | _columns_read(transformations[i])   # the outputs are new columns
+        else:
             live = live | _columns_read(transformations[i])
     return needed
 
@@ -238,6 +285,11 @@ def _schema_walk(schema: "OrderedDict[str, int]", transformations: Sequence[tupl
             try:
                 cur = OrderedDict(plan_join(cur, arg[0].schema, arg[1]))
             except N.ArrowError:       # the step itself raises when it is evaluated; nothing after it is fused
+                cur = OrderedDict()
+        elif kind == "window":
+            try:
+                cur = OrderedDict(plan_window(cur, *arg))
+            except N.ArrowError:
                 cur = OrderedDict()
     out.append(cur)
     return out
@@ -479,6 +531,22 @@ class DeviceFrame:
             ri.free()
         return DeviceFrame(OrderedDict((name, c) for (name, _), c in zip(plan, cols)))
 
+    def window(self, partition_by: Sequence[str], order_by: Sequence[Tuple[str, bool]], calls: Sequence[tuple]) -> "DeviceFrame":
+        """Window functions over one specification (bdf_window_dev, one sort for all calls): every call ``(output, function,
+        *arguments)`` adds its column as with_column does (an existing name is replaced); the other columns are untouched."""
+        plan_window(self.schema, partition_by, order_by, calls)
+        args = []
+        for call in calls:
+            rest = list(call[2:])
+            if call[1] not in WINDOW_RANKING:
+                rest[0] = self.column(rest[0])
+            args.append((call[1], *rest))
+        res = _window([self.column(p) for p in partition_by], [(self.column(c), d) for c, d in order_by], args)
+        frame = self
+        for call, r in zip(calls, res):
+            frame = frame.with_column(call[0], r)
+        return frame
+
     def limit(self, count: int) -> "DeviceFrame":
         if not self.columns:
             return self
@@ -555,6 +623,8 @@ class DeviceFrame:
                 frame = frame.sort(arg)
             elif kind == "join":
                 frame = frame.join(*arg)
+            elif kind == "window":
+                frame = frame.window(*arg)
             elif kind == "group_aggregate":
                 raise N.ReferencePanic("aggregations not supported")       # evaluation.rs:73
             else:

@@ -535,6 +535,59 @@ def join_indices(left_keys: Sequence["Column"], right_keys: Sequence["Column"], 
     return Column(ctx, hl), Column(ctx, hr)
 
 
+def _window_call(call: tuple, ordered: bool) -> "N.WindowCall":
+    """One call tuple -> bdf_window_call.  ``("row_number",)`` .. ``("cume_dist",)``; ``("lag" | "lead", x, offset=1, default=None)``;
+    ``("sum" | "count" | "min" | "max" | "avg", x, frame=None)`` with frame "rows", "range" or "partition" (None: SQL's default, "range"
+    with an ORDER BY and "partition" without)."""
+    name = call[0]
+    if name not in N.WINDOW_FNS:
+        raise N.UnsupportedType(f"window function {name!r} is not one of {sorted(N.WINDOW_FNS)}")
+    fn = N.WINDOW_FNS[name]
+    k = N.WindowCall()
+    k.function = fn
+    if fn <= N.WIN_CUME_DIST:
+        if len(call) != 1:
+            raise N.ComputeError(f"{name} takes no column")
+        return k
+    if len(call) < 2:
+        raise N.ComputeError(f"{name} needs a column")
+    x = call[1]
+    k.column = x.handle.value if isinstance(x.handle, C.c_void_p) else x.handle
+    if fn in (N.WIN_LAG, N.WIN_LEAD):
+        k.offset = int(call[2]) if len(call) > 2 else 1
+        default = call[3] if len(call) > 3 else None
+        if default is not None:
+            raw = np.array(default, dtype=NP_DTYPES[x.dtype]).tobytes()   # T::Native in the low bytes
+            k.default_bits = int.from_bytes(raw.ljust(8, b"\0"), "little")
+            k.has_default = 1
+        return k
+    frame = call[2] if len(call) > 2 and call[2] is not None else ("range" if ordered else "partition")
+    if frame not in N.WINDOW_FRAMES:
+        raise N.UnsupportedType(f"window frame {frame!r} is not one of {sorted(N.WINDOW_FRAMES)}")
+    k.frame = N.WINDOW_FRAMES[frame]
+    return k
+
+
+def window(partition_by: Sequence["Column"], order_by: Sequence[tuple], calls: Sequence[tuple]) -> List["Column"]:
+    """Window functions over one specification (bdf_window_dev): rows are partitioned by the tuple of ``partition_by`` columns
+    and ordered inside a partition by ``order_by`` (``[(Column, descending)]``; nulls last in both directions, ties in row order).
+    ``calls`` are tuples as ``_window_call`` describes, e.g. ``("row_number",)``, ``("lag", x, 1, 0.0)`` or ``("sum", x, "range")``.
+    Returns one one-chunk Column per call, in the caller's row order: row r of each belongs to input row r."""
+    cols = list(partition_by) + [c for c, _ in order_by] + [c[1] for c in calls if len(c) > 1]
+    ctx = cols[0].ctx if cols else N.default_context()
+    arr = (N.WindowCall * max(len(calls), 1))()
+    for j, call in enumerate(calls):
+        arr[j] = _window_call(call, bool(order_by))
+    handle = lambda c: c.handle.value if isinstance(c.handle, C.c_void_p) else c.handle
+    pk = (C.c_void_p * max(len(partition_by), 1))(*[handle(c) for c in partition_by])
+    ok = (N.SortKeyC * max(len(order_by), 1))()
+    for i, (c, desc) in enumerate(order_by):
+        ok[i].column, ok[i].descending = handle(c), 1 if desc else 0
+    out = (C.c_void_p * max(len(calls), 1))()
+    N.raise_for_status(N.lib().bdf_window_dev(ctx.handle, len(partition_by), pk, len(order_by), ok, len(calls), arr, out))
+    return [Column(ctx, C.c_void_p(out[j])) for j in range(len(calls))]
+
+
 def _expr_nodes(nodes: Sequence[tuple]):
     arr = (N.ExprNode * len(nodes))()
     for k, nd in enumerate(nodes):
