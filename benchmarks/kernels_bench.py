@@ -6,6 +6,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py [--rows 100000000] [--json kernels.json]
     python benchmarks/kernels_bench.py --csv [--csv-rows 50000000] [--json csv.json]   # the CSV reader rows instead (a 2.55 GB temporary file)
     python benchmarks/kernels_bench.py --window [--rows 100000000]                      # only the window-function rows
+    python benchmarks/kernels_bench.py --math [--rows 100000000]                        # only the float-function rows
 """
 from __future__ import annotations
 
@@ -208,6 +209,25 @@ def window_bench(ctx, rows, lens, rows_out, reps=3):
     x.free()
 
 
+def math_bench(ctx, lens, report):
+    """The float function library: trig, the functions with an exact-result step (log2 f64, log10 f32, hypot f64) next to
+    their siblings without one, and the same functions in the fused kernel."""
+    G = rdf.Column.generate
+    x = G(rdf.F64, lens, 0, 1e-3, 1e3, col_id=30)
+    y = G(rdf.F64, lens, 0, 1e-3, 1e3, col_id=31)
+    x32 = G(rdf.F32, lens, 0, 1e-3, 1e3, col_id=32)
+    for name in ("sin", "exp", "log2", "log10"):
+        report(f"{name} f64", "math", timed(ctx, lambda: x.unary(getattr(N, name.upper()))), "unary")
+    for name in ("sin", "log2", "log10"):
+        report(f"{name} f32", "math", timed(ctx, lambda: x32.unary(getattr(N, name.upper()))), "unary")
+    for name in ("atan2", "hypot", "log"):
+        report(f"{name} f64", "math", timed(ctx, lambda: getattr(x, name)(y)), "binary")
+    report("N3 fused log2(a) + b", "math", timed(ctx, lambda: rdf.eval_expr([x, y], [("log2", 0), (N.ADD, 2, 1)])), "expr")
+    report("N3 fused hypot(a, b)", "math", timed(ctx, lambda: rdf.eval_expr([x, y], [(N.HYPOT, 0, 1)])), "expr")
+    for col in (x, y, x32):
+        col.free()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
@@ -215,6 +235,7 @@ def main():
     ap.add_argument("--csv-rows", type=int, default=50_000_000)
     ap.add_argument("--csv", action="store_true", help="run the CSV reader rows instead of the kernel table")
     ap.add_argument("--window", action="store_true", help="run only the window-function rows")
+    ap.add_argument("--math", action="store_true", help="run only the float-function rows (unary, atan2/hypot/log, fused)")
     args = ap.parse_args()
     ctx = rdf.default_context()
     if args.window:
@@ -243,6 +264,13 @@ def main():
         rows_out.append({"case": name, "config": config, "kernel": kind, "ms": ms, "rows": rows, "bytes_per_row": nbytes / rows,
                          "GBs": gbs, "frac_of_peak": gbs / pk, "rows_per_s": rows / ms * 1e3})
         print(f"{name:44s} {ms:8.4f} ms  {nbytes / rows:7.3f} B/row  {gbs:8.1f} GB/s  {gbs / pk:5.3f} of peak  {rows / ms * 1e3:10.3e} rows/s", flush=True)
+
+    if args.math:
+        math_bench(ctx, lens, report)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"results": rows_out}, f, indent=1)
+        return
 
     # ---- config 1/metric: f64 add, sum ----
     a = G(rdf.F64, lens, 0, -1e3, 1e3, col_id=0)

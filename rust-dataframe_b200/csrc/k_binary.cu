@@ -15,6 +15,7 @@
 //
 // Roofline: HBM.  Algorithmic bytes/row = 3*sizeof(T) + (v_in + [v_in>0])/8  (24 B/row for f64, no nulls).
 #include "common.cuh"
+#include "math_exact.cuh"
 
 namespace bdf {
 
@@ -39,7 +40,7 @@ __device__ __forceinline__ T bin_apply(T a, T b, bool valid, bool& divzero) {
                 divzero |= valid && (b == 0.0);
                 return __ddiv_rn(a, valid ? b : 1.0);
             } else if constexpr (OP == OP_ATAN2) return valid ? atan2(a, b) : 0.0;
-            else if constexpr (OP == OP_HYPOT) return valid ? hypot(a, b) : 0.0;
+            else if constexpr (OP == OP_HYPOT) return valid ? hypot_exact(a, b) : 0.0;
             else return valid ? __ddiv_rn(log(a), log(b)) : 0.0;
         } else {
             if constexpr (OP == OP_ADD) return __fadd_rn(a, b);

@@ -12,6 +12,7 @@
 // Execution model: the host compiles the straight-line DAG into an ACCUMULATOR program (expr_compile below): one
 // register accumulator; the input tiles and up to two temporaries staged in shared memory (see k_expr).
 #include "common.cuh"
+#include "math_exact.cuh"
 
 #include <cstdlib>
 #include <vector>
@@ -60,7 +61,7 @@ __device__ __forceinline__ double expr_unary(double x) {
     else if constexpr (F == 12) return expm1(x);
     else if constexpr (F == 13) return floor(x);
     else if constexpr (F == 14) return log10(x);
-    else if constexpr (F == 15) return log2(x);
+    else if constexpr (F == 15) return log2_exact(x);
     else if constexpr (F == 16) return __dmul_rn(x, 3.14159265358979323846264338327950288 / 180.0);
     else if constexpr (F == 17) return round(x);
     else if constexpr (F == 18) return sinh(x);
@@ -163,7 +164,7 @@ __device__ __forceinline__ void expr_binop(Vec<double, 2> (&out)[U], const Vec<d
             else if constexpr (OP == 2) q = __dmul_rn(a, b);
             else if constexpr (OP == 3) { divzero |= v && (b == 0.0); q = __ddiv_rn(a, v ? b : 1.0); }
             else if constexpr (OP == 4) { const double y = atan2(a, b); q = v ? y : 0.0; }
-            else if constexpr (OP == 5) { const double y = hypot(a, b); q = v ? y : 0.0; }
+            else if constexpr (OP == 5) { const double y = hypot_exact(a, b); q = v ? y : 0.0; }
             else { const double y = __ddiv_rn(log(a), log(b)); q = v ? y : 0.0; }
             out[j].e[e] = q;
         }

@@ -6,11 +6,13 @@
 // radians,round,sinh,sqrt,tanh} (scalar.rs:106-457): null -> null with payload 0, else num::Float::f(x)
 // (= platform libm on the CPU).  CUDA's double/float math functions are used at full precision (no
 // fast-math); documented error <= 2 ulp (f64 sin/cos/tan), <= 2/2/4 ulp (f32 sinf/cosf/tanf), so results
-// are compared with glibc under the ulp tolerance stated in tests/test_parity_gpu.py.
+// are compared with glibc under the ulp tolerance stated in tests/test_parity_gpu.py.  log2 (f64) and log10 (f32) go
+// through math_exact.cuh, which returns the exact k at 2^k / 10^k where CUDA's result is 1 ulp off.
 //
 // Roofline: HBM, 2*sizeof(T) + 2*[nullable]/8 bytes/row (16 B/row for f64); f64 trig is close to the FP64
 // pipe limit (see DESIGN.md).
 #include "common.cuh"
+#include "math_exact.cuh"
 
 namespace bdf {
 
@@ -36,7 +38,7 @@ __device__ __forceinline__ double un_apply(double x) {
     else if constexpr (OP == UN_EXPM1) return expm1(x);
     else if constexpr (OP == UN_FLOOR) return floor(x);
     else if constexpr (OP == UN_LOG10) return log10(x);
-    else if constexpr (OP == UN_LOG2) return log2(x);
+    else if constexpr (OP == UN_LOG2) return log2_exact(x);
     else if constexpr (OP == UN_RADIANS) return __dmul_rn(x, 3.14159265358979323846264338327950288 / 180.0);
     else if constexpr (OP == UN_ROUND) return round(x);
     else if constexpr (OP == UN_SINH) return sinh(x);
@@ -60,7 +62,7 @@ __device__ __forceinline__ float un_apply(float x) {
     else if constexpr (OP == UN_EXP) return expf(x);
     else if constexpr (OP == UN_EXPM1) return expm1f(x);
     else if constexpr (OP == UN_FLOOR) return floorf(x);
-    else if constexpr (OP == UN_LOG10) return log10f(x);
+    else if constexpr (OP == UN_LOG10) return log10_exact(x);
     else if constexpr (OP == UN_LOG2) return log2f(x);
     else if constexpr (OP == UN_RADIANS) return __fmul_rn(x, 3.14159265358979323846264338327950288f / 180.0f);
     else if constexpr (OP == UN_ROUND) return roundf(x);
