@@ -7,6 +7,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --csv [--csv-rows 50000000] [--json csv.json]   # the CSV reader rows instead (a 2.55 GB temporary file)
     python benchmarks/kernels_bench.py --window [--rows 100000000]                      # only the window-function rows
     python benchmarks/kernels_bench.py --math [--rows 100000000]                        # only the float-function rows
+    python benchmarks/kernels_bench.py --stats [--rows 100000000]                       # only the statistical-aggregate rows
 """
 from __future__ import annotations
 
@@ -228,6 +229,54 @@ def math_bench(ctx, lens, report):
         col.free()
 
 
+def _card():
+    import subprocess
+
+    try:   # read-only query: the card and its power limit belong beside every number of the run
+        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
+                              timeout=30).stdout.strip().splitlines()[0]
+    except Exception as e:   # noqa: BLE001
+        return f"unknown ({e})"
+
+
+def stats_bench(ctx, lens, report, rows_out):
+    """The statistical aggregates: k_moments against k_reduce on the same columns (old and new rows alternating, the median of
+    three medians), group-by variance against avg (fold part apart from sort and takes), whole-column count_distinct."""
+    G = rdf.Column.generate
+    print("card:", _card(), flush=True)
+    cols = [("f64", G(rdf.F64, lens, 0, -1e3, 1e3, col_id=50)), ("f64 10% nulls", G(rdf.F64, lens, 0, -1e3, 1e3, col_id=51, null_mod=10)),
+            ("i32", G(rdf.I32, lens, 2, col_id=52))]
+    for what, col in cols:
+        old, new = [], []
+        for _ in range(3):
+            old.append(timed(ctx, lambda: col.aggregate_all())["reduce"])
+            new.append(timed(ctx, lambda: col.moments())["moments"])
+        med = lambda runs: (float(np.median([r[0] for r in runs])), runs[0][1], runs[0][2])
+        report(f"aggregate_all {what} (k_reduce)", "stats", {"reduce": med(old)}, "reduce")
+        report(f"moments {what} (k_moments)", "stats", {"moments": med(new)}, "moments")
+        print(f"{'':44s} ratio moments / reduce = {med(new)[0] / med(old)[0]:.3f}", flush=True)
+    a = cols[0][1]
+    i32n = G(rdf.I32, lens, 2, col_id=53, null_mod=10)
+    kf = G(rdf.F64, lens, 0, -100.0, 100.0, col_id=54)
+    small = kf.cast(rdf.I8)
+    kf.free()
+    for fn in ("avg", "variance", "avg", "variance"):
+        res = timed(ctx, lambda: [c.free() for part in rdf.group_by([i32n, small], [(a, fn)]) for c in part] and None, reps=3)
+        total = sum(v[0] for v in res.values())
+        print(f"group-by i32 (nulls) x i8, {fn} f64{'':14s} {total:8.4f} ms  (" + ", ".join(f"{k} {v[0]:.3f}" for k, v in sorted(res.items())) + ")",
+              flush=True)
+        rows_out.append({"case": f"group-by i32 (nulls) x i8 keys, {fn} f64", "config": "stats", "kernel": "sort + take + filter + group",
+                         "ms": total, "parts": {k: v[0] for k, v in res.items()}})
+    res = timed(ctx, lambda: cols[2][1].count_distinct(), reps=3)
+    total = sum(v[0] for v in res.values())
+    print(f"{'count_distinct i32 (whole column)':44s} {total:8.4f} ms  (" + ", ".join(f"{k} {v[0]:.3f}" for k, v in sorted(res.items())) + ")",
+          flush=True)
+    rows_out.append({"case": "count_distinct i32 (whole column)", "config": "stats", "kernel": "sort + take + filter + group", "ms": total,
+                     "parts": {k: v[0] for k, v in res.items()}})
+    for col in [c for _, c in cols] + [i32n, small]:
+        col.free()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
@@ -236,6 +285,7 @@ def main():
     ap.add_argument("--csv", action="store_true", help="run the CSV reader rows instead of the kernel table")
     ap.add_argument("--window", action="store_true", help="run only the window-function rows")
     ap.add_argument("--math", action="store_true", help="run only the float-function rows (unary, atan2/hypot/log, fused)")
+    ap.add_argument("--stats", action="store_true", help="run only the statistical-aggregate rows (moments, group variance, count_distinct)")
     args = ap.parse_args()
     ctx = rdf.default_context()
     if args.window:
@@ -265,8 +315,8 @@ def main():
                          "GBs": gbs, "frac_of_peak": gbs / pk, "rows_per_s": rows / ms * 1e3})
         print(f"{name:44s} {ms:8.4f} ms  {nbytes / rows:7.3f} B/row  {gbs:8.1f} GB/s  {gbs / pk:5.3f} of peak  {rows / ms * 1e3:10.3e} rows/s", flush=True)
 
-    if args.math:
-        math_bench(ctx, lens, report)
+    if args.math or args.stats:
+        (math_bench(ctx, lens, report) if args.math else stats_bench(ctx, lens, report, rows_out))
         if args.json:
             with open(args.json, "w") as f:
                 json.dump({"results": rows_out}, f, indent=1)

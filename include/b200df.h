@@ -313,8 +313,16 @@ int  bdf_group_aggregate_dev(bdf_ctx* ctx, const bdf_col* key, int32_t n_values,
  *   unknown function, avg of Int64 / UInt64 -> BDF_UNSUPPORTED; columns of different lengths -> BDF_LENGTH_MISMATCH; a
  *   multi-GPU context (rows change chunks, as for sort / take / filter) -> BDF_UNSUPPORTED; more than 2^32-1 rows -> the
  *   sort's BDF_UNSUPPORTED.  On failure nothing is returned and nothing leaks. */
+/* The statistical functions (section "statistical aggregates" below) per group:
+ *   KURTOSIS / SKEWNESS / STDDEV / VARIANCE / STDDEV_POP / VAR_POP   Float64: the statistic of the group's moment record, NULL where
+ *                   it is None.  Any numeric x (Int64 / UInt64 included).  The record is folded per group by the fold paths and the
+ *                   fixed order of SUM (a one-value record merged per valid value; moments.cuh), then one kernel derives the statistic.
+ *   SUM_DISTINCT    dtype of x: the sum of the group's distinct valid values (equality as COUNT_DISTINCT), which come out of the same
+ *                   second sort in ascending order and are folded with SUM's fold (integers wrap, floats in double from +0.0, rounded
+ *                   once).  Never NULL: a group without a valid value sums to 0.  A NaN among them makes the sum NaN. */
 typedef enum { BDF_GROUP_SUM = 0, BDF_GROUP_MAX, BDF_GROUP_MIN, BDF_GROUP_AVG, BDF_GROUP_COUNT, BDF_GROUP_COUNT_DISTINCT, BDF_GROUP_FIRST,
-               BDF_GROUP_LAST } bdf_group_fn;   /* AggregateFunction order */
+               BDF_GROUP_LAST, BDF_GROUP_KURTOSIS, BDF_GROUP_SKEWNESS, BDF_GROUP_STDDEV, BDF_GROUP_SUM_DISTINCT, BDF_GROUP_VARIANCE,
+               BDF_GROUP_STDDEV_POP, BDF_GROUP_VAR_POP } bdf_group_fn;   /* AggregateFunction order, then the population forms */
 typedef struct { const bdf_col* column; int32_t function; } bdf_group_agg;
 int  bdf_group_by_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_col* const* keys, int32_t n_aggs, const bdf_group_agg* aggs,
                       bdf_col** out_keys /* n_keys */, bdf_col** out /* n_aggs */, int64_t* n_groups);
@@ -399,6 +407,45 @@ typedef struct {
 } bdf_window_call;
 int  bdf_window_dev(bdf_ctx* ctx, int32_t n_partition, const bdf_col* const* partition_by, int32_t n_order, const bdf_sort_key* order_by,
                     int32_t n_calls, const bdf_window_call* calls, bdf_col** out /* n_calls */);
+
+/* ---- statistical aggregates (AggregateFunctions::{variance, stddev, skewness, kurtosis, count_distinct, sum_distinct}: empty stubs in
+ * the reference, src/functions/aggregate.rs:81,94-102, "TODO population and sample stddevs / variances"; the names follow Spark, and so
+ * do the definitions) -----------------------------------------------------------------------------------------------------------------
+ * Input.  A column of any of the ten numeric types; every valid value is read `as f64` (Int64 / UInt64 beyond 2^53 round to nearest,
+ *   Float32 is exact); nulls are skipped.  Unlike avg, Int64 / UInt64 are accepted: avg's refusal mirrors its declared bound
+ *   f64: From<T::Native>, the stubs declare none, and the CSV reader infers Int64 for every integer column.
+ * The moment record of the valid values x1..xn: count = n, mean, and the central sums m2 = sum (x - mean)^2, m3 = sum (x - mean)^3,
+ *   m4 = sum (x - mean)^4 -- computed in one pass, as accurately as two passes would (never as sum x^2 - n mean^2).  If every valid
+ *   value is equal, mean is exactly that value and m2 = m3 = m4 = 0 exactly.  If any valid value is NaN or +-inf, mean, m2, m3 and m4
+ *   are NaN.  Overflow of an intermediate follows IEEE arithmetic (inf / NaN) and is not an error.
+ * The statistics, each from the record with exactly this operation order (n = (double)count, no FMA contraction, IEEE sqrt):
+ *   VAR_POP = m2 / n                 VARIANCE = m2 / (n - 1)        (sample; Spark's variance)
+ *   STDDEV_POP = sqrt(VAR_POP)       STDDEV = sqrt(VARIANCE)        (sample; Spark's stddev)
+ *   SKEWNESS = (sqrt(n) * m3) / (m2 * sqrt(m2))                     KURTOSIS = (n * m4) / (m2 * m2) - 3   (excess)
+ *   None (is_some = 0; NULL per group): every statistic when count = 0; the sample forms also when count = 1; SKEWNESS and KURTOSIS
+ *   also when m2 = 0 (Spark 3 with null on divide by zero).
+ * Multi-GPU: every GPU computes the record of its rows; the records are combined with bdf_moments_merge in rank order (on a
+ *   communicator they are all-gathered first), so every rank returns the same bits, and a fleet or communicator of one GPU returns
+ *   the one-GPU bits.
+ * count_distinct / sum_distinct use the key equality of sort, group-by and join (all NaNs are one value, -0.0 == 0.0); nulls are not
+ *   counted.  count is Int64; sum has the dtype of x (T::Native bits in the low bytes, zero-padded, as bdf_agg4): integers wrap, floats
+ *   are the distinct values accumulated in double in ascending value order from +0.0 (group-by's SUM fold) and rounded once.  Never
+ *   None: no valid values sum to 0, like AggregateFunctions::sum.  A NaN among the values makes the sum NaN.  The values are sorted
+ *   (the group-by's second sort with the whole column as one group), so both need every row on one GPU: on either kind of multi-GPU
+ *   context they are BDF_UNSUPPORTED.
+ * Deterministic: the same inputs with the same chunking give the same bits (no atomics on values; fold orders depend only on shapes).
+ * Errors (nothing is written, nothing leaks): a null pointer or an unknown bdf_stat -> BDF_INVALID; a non-numeric or Boolean column ->
+ *   BDF_UNSUPPORTED. */
+typedef struct { int64_t count; double mean, m2, m3, m4; } bdf_moment_rec;
+typedef struct { int64_t count; uint64_t sum; /* T::Native bits, as bdf_agg4 */ } bdf_distinct_rec;
+typedef enum { BDF_STAT_VARIANCE = 0, BDF_STAT_VAR_POP, BDF_STAT_STDDEV, BDF_STAT_STDDEV_POP, BDF_STAT_SKEWNESS, BDF_STAT_KURTOSIS } bdf_stat;
+int  bdf_moments(bdf_ctx* ctx, int dtype, int64_t n_chunks, const bdf_view* in, bdf_moment_rec* out);   /* host in */
+int  bdf_moments_dev(bdf_ctx* ctx, const bdf_col* in, bdf_moment_rec* out);
+/* No context, no GPU: the formulas above, and the pairwise merge (Chan / Pebay, moments.cuh) the library itself uses across ranks. */
+int  bdf_moments_stat(const bdf_moment_rec* m, int stat, double* out, int32_t* is_some);
+int  bdf_moments_merge(const bdf_moment_rec* a, const bdf_moment_rec* b, bdf_moment_rec* out);
+int  bdf_distinct(bdf_ctx* ctx, int dtype, int64_t n_chunks, const bdf_view* in, bdf_distinct_rec* out);   /* host in */
+int  bdf_distinct_dev(bdf_ctx* ctx, const bdf_col* in, bdf_distinct_rec* out);
 
 /* ---- N4: Arrow IPC files either side of the path ---------------------------------------------------------------
  * DataFrame::from_arrow (src/dataframe.rs:391-407: arrow::ipc::reader::FileReader, every RecordBatch -> one chunk per
@@ -490,7 +537,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

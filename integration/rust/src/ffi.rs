@@ -58,6 +58,29 @@ pub const BDF_GROUP_AVG: i32 = 3;
 pub const BDF_GROUP_COUNT: i32 = 4;
 pub const BDF_GROUP_COUNT_DISTINCT: i32 = 5;
 pub const BDF_GROUP_FIRST: i32 = 6;
+// (BDF_GROUP_LAST = 7 follows; then the statistical functions, continuing AggregateFunction's order, and the population forms)
+pub const BDF_GROUP_KURTOSIS: i32 = 8;
+pub const BDF_GROUP_SKEWNESS: i32 = 9;
+pub const BDF_GROUP_STDDEV: i32 = 10;
+pub const BDF_GROUP_SUM_DISTINCT: i32 = 11;
+pub const BDF_GROUP_VARIANCE: i32 = 12;
+pub const BDF_GROUP_STDDEV_POP: i32 = 13;
+pub const BDF_GROUP_VAR_POP: i32 = 14;
+/// bdf_moment_rec: count, mean and the central sums m2, m3, m4 of the valid values (read `as f64`).
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct BdfMomentRec { pub count: i64, pub mean: f64, pub m2: f64, pub m3: f64, pub m4: f64 }
+/// bdf_distinct_rec: the number of distinct valid values and their sum (T::Native bits in the low bytes).
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct BdfDistinctRec { pub count: i64, pub sum: u64 }
+/// bdf_stat
+pub const BDF_STAT_VARIANCE: i32 = 0;
+pub const BDF_STAT_VAR_POP: i32 = 1;
+pub const BDF_STAT_STDDEV: i32 = 2;
+pub const BDF_STAT_STDDEV_POP: i32 = 3;
+pub const BDF_STAT_SKEWNESS: i32 = 4;
+pub const BDF_STAT_KURTOSIS: i32 = 5;
 pub const BDF_GROUP_LAST: i32 = 7;
 
 #[repr(C)]
@@ -121,6 +144,11 @@ extern "C" {
     pub fn bdf_aggregate(ctx: *mut BdfCtx, op: c_int, dtype: c_int, n: i64, input: *const BdfView, out_scalar: *mut c_void,
                          is_some: *mut i32) -> c_int;
     pub fn bdf_avg(ctx: *mut BdfCtx, dtype: c_int, n: i64, input: *const BdfView, out: *mut f64, is_some: *mut i32) -> c_int;
+    // statistical aggregates: a context computes the moment record; a pure function derives a statistic from it
+    pub fn bdf_moments(ctx: *mut BdfCtx, dtype: c_int, n: i64, input: *const BdfView, out: *mut BdfMomentRec) -> c_int;
+    pub fn bdf_moments_stat(m: *const BdfMomentRec, stat: c_int, out: *mut f64, is_some: *mut i32) -> c_int;
+    pub fn bdf_moments_merge(a: *const BdfMomentRec, b: *const BdfMomentRec, out: *mut BdfMomentRec) -> c_int;
+    pub fn bdf_distinct(ctx: *mut BdfCtx, dtype: c_int, n: i64, input: *const BdfView, out: *mut BdfDistinctRec) -> c_int;
     // device-resident columns (the lazy evaluator keeps a frame's numeric columns in HBM between Calculations)
     pub fn bdf_upload_many(ctx: *mut BdfCtx, n_cols: i64, dtypes: *const i32, n_chunks: *const i64, input: *const *const BdfView, flags: c_int,
                            out: *mut *mut BdfCol) -> c_int;

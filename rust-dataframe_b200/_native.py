@@ -20,18 +20,26 @@ ADD, SUB, MUL, DIV, ATAN2, HYPOT, LOG = range(7)
 SUM, MIN, MAX, COUNT = range(4)
 OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID, PARSE = range(10)
 ASYNC = 1
-K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW = range(15)
+(K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW,
+ K_MOMENTS) = range(16)
 KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
-                "window"]
+                "window", "moments"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
 BOOL = 10
 UTF8 = 11   # CSV schema entry only: a string column the device skips
 # bdf_group_fn (AggregateFunction order)
-GROUP_SUM, GROUP_MAX, GROUP_MIN, GROUP_AVG, GROUP_COUNT, GROUP_COUNT_DISTINCT, GROUP_FIRST, GROUP_LAST = range(8)
+(GROUP_SUM, GROUP_MAX, GROUP_MIN, GROUP_AVG, GROUP_COUNT, GROUP_COUNT_DISTINCT, GROUP_FIRST, GROUP_LAST, GROUP_KURTOSIS, GROUP_SKEWNESS,
+ GROUP_STDDEV, GROUP_SUM_DISTINCT, GROUP_VARIANCE, GROUP_STDDEV_POP, GROUP_VAR_POP) = range(15)
 GROUP_FNS = {"sum": GROUP_SUM, "max": GROUP_MAX, "min": GROUP_MIN, "avg": GROUP_AVG, "count": GROUP_COUNT,
-             "count_distinct": GROUP_COUNT_DISTINCT, "first": GROUP_FIRST, "last": GROUP_LAST}
+             "count_distinct": GROUP_COUNT_DISTINCT, "first": GROUP_FIRST, "last": GROUP_LAST, "kurtosis": GROUP_KURTOSIS,
+             "skewness": GROUP_SKEWNESS, "stddev": GROUP_STDDEV, "sum_distinct": GROUP_SUM_DISTINCT, "variance": GROUP_VARIANCE,
+             "stddev_pop": GROUP_STDDEV_POP, "var_pop": GROUP_VAR_POP}
+# bdf_stat
+STAT_VARIANCE, STAT_VAR_POP, STAT_STDDEV, STAT_STDDEV_POP, STAT_SKEWNESS, STAT_KURTOSIS = range(6)
+STATS = {"variance": STAT_VARIANCE, "var_pop": STAT_VAR_POP, "stddev": STAT_STDDEV, "stddev_pop": STAT_STDDEV_POP,
+         "skewness": STAT_SKEWNESS, "kurtosis": STAT_KURTOSIS}
 # bdf_join_type (JoinType order)
 JOIN_LEFT, JOIN_RIGHT, JOIN_INNER, JOIN_FULL = range(4)
 JOIN_TYPES = {"left": JOIN_LEFT, "right": JOIN_RIGHT, "inner": JOIN_INNER, "full": JOIN_FULL}
@@ -58,6 +66,14 @@ class Out(C.Structure):
 class Agg4(C.Structure):
     _fields_ = [("sum", C.c_uint64), ("min", C.c_uint64), ("max", C.c_uint64), ("count", C.c_int64),
                 ("rows", C.c_int64), ("any_valid", C.c_int32), ("would_panic", C.c_int32), ("n_chunks", C.c_int64)]
+
+
+class MomentRec(C.Structure):
+    _fields_ = [("count", C.c_int64), ("mean", C.c_double), ("m2", C.c_double), ("m3", C.c_double), ("m4", C.c_double)]
+
+
+class DistinctRec(C.Structure):
+    _fields_ = [("count", C.c_int64), ("sum", C.c_uint64)]
 
 
 class ExprNode(C.Structure):
@@ -171,6 +187,12 @@ def lib() -> C.CDLL:
         "bdf_aggregate_dev": ([vp, C.c_int, vp, vp, P(i32)], C.c_int),
         "bdf_aggregate_all_dev": ([vp, vp, P(Agg4)], C.c_int),
         "bdf_avg_dev": ([vp, vp, P(C.c_double), P(i32)], C.c_int),
+        "bdf_moments": ([vp, C.c_int, i64, P(View), P(MomentRec)], C.c_int),
+        "bdf_moments_dev": ([vp, vp, P(MomentRec)], C.c_int),
+        "bdf_moments_stat": ([P(MomentRec), C.c_int, P(C.c_double), P(i32)], C.c_int),
+        "bdf_moments_merge": ([P(MomentRec), P(MomentRec), P(MomentRec)], C.c_int),
+        "bdf_distinct": ([vp, C.c_int, i64, P(View), P(DistinctRec)], C.c_int),
+        "bdf_distinct_dev": ([vp, vp, P(DistinctRec)], C.c_int),
         "bdf_expr_check": ([i32, P(i32), i32, P(ExprNode), P(i32), P(i32)], C.c_int),
         "bdf_eval_expr_dev": ([vp, i32, P(vp), i32, P(ExprNode), P(vp)], C.c_int),
         "bdf_eval_expr_agg_dev": ([vp, i32, P(vp), i32, P(ExprNode), P(vp), P(Agg4)], C.c_int),
@@ -240,6 +262,7 @@ EXPORTED_SYMBOLS = [
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",
     "bdf_ipc_write_host", "bdf_ipc_write",
     "bdf_csv_open", "bdf_csv_describe", "bdf_csv_column", "bdf_csv_read", "bdf_csv_stats", "bdf_csv_close",
+    "bdf_moments", "bdf_moments_dev", "bdf_moments_stat", "bdf_moments_merge", "bdf_distinct", "bdf_distinct_dev",
 ]
 
 

@@ -4,6 +4,7 @@
 #pragma once
 
 #include "common.cuh"
+#include "moments.cuh"
 
 namespace bdf {
 
@@ -54,6 +55,26 @@ template <typename T> struct GroupAggX<T, true> {
         sum = __dadd_rn(sum, s2); kmin = a2 < kmin ? a2 : kmin; kmax = b2 > kmax ? b2 : kmax;
     }
     __device__ __forceinline__ void merge(const GroupAggX& o) { sum = __dadd_rn(sum, o.sum); kmin = o.kmin < kmin ? o.kmin : kmin; kmax = o.kmax > kmax ? o.kmax : kmax; }
+};
+
+// The moments accumulator (variance, stddev, skewness, kurtosis): every valid value is read `as f64` and merged into the record as
+// a one-value record, in the fold order of the other accumulators (moments.cuh).  It carries its own count.
+template <typename T> struct GroupMoments {
+    Moments m;
+    __device__ __forceinline__ void init() { m = Moments{0, 0.0, 0.0, 0.0, 0.0}; }
+    __device__ __forceinline__ void add(T x, bool valid, unsigned long long) {
+        if (valid) m = moments_merge(m, moments_one((double)x));
+    }
+    __device__ __forceinline__ void merge_shfl(int o) {
+        Moments b;
+        b.count = __shfl_xor_sync(0xffffffffu, m.count, o);
+        b.mean = __shfl_xor_sync(0xffffffffu, m.mean, o);
+        b.m2 = __shfl_xor_sync(0xffffffffu, m.m2, o);
+        b.m3 = __shfl_xor_sync(0xffffffffu, m.m3, o);
+        b.m4 = __shfl_xor_sync(0xffffffffu, m.m4, o);
+        m = moments_merge(m, b);
+    }
+    __device__ __forceinline__ void merge(const GroupMoments& o) { m = moments_merge(m, o.m); }
 };
 
 template <typename T> struct GroupFlip {

@@ -15,8 +15,10 @@
 //                   valid value.  A group of more than kBigGroup rows is not folded by its warp: the warp registers it in a
 //                   work list and k_group_big folds it one CTA per 64 Ki-row segment (thread-strided fold + fixed block
 //                   tree), k_group_big_finish then folds a group's segment partials in segment order -- still deterministic,
-//                   and a single hot key is spread over the whole GPU instead of one warp.  The EXTRA instantiations carry
-//                   what only bdf_group_by_dev asks for (GroupAggX, group_acc.cuh); the others fold exactly what they always did.
+//                   and a single hot key is spread over the whole GPU instead of one warp.  The accumulator is a template
+//                   argument: ACC 0 folds what the single-key entry always folded (FusedAgg), ACC 1 what only bdf_group_by_dev
+//                   asks for (GroupAggX, group_acc.cuh), ACC 2 the moment record of the statistics (GroupMoments) -- the three
+//                   share every fold path, order and tree.
 //                   In a 1- or 8-lane launch a group longer than kLaneRows rows per lane goes to a second list instead, and
 //                   k_group_medium folds each of those with a warp (the 32-lane order and tree), so a few long groups among
 //                   many one-row groups do not leave single threads walking tens of thousands of rows.
@@ -70,28 +72,33 @@ k_group_heads(const __grid_constant__ HeadKeys keys, long long n, uint32_t* __re
 }
 
 // ---- (b) per-group fold -------------------------------------------------------------------------------------------------
-template <typename T, bool EXTRA> struct GroupAcc { using type = FusedAgg<T>; };
-template <typename T> struct GroupAcc<T, true> { using type = GroupAggX<T>; };
+template <typename T, int ACC> struct GroupAcc { using type = FusedAgg<T>; };
+template <typename T> struct GroupAcc<T, 1> { using type = GroupAggX<T>; };
+template <typename T> struct GroupAcc<T, 2> { using type = GroupMoments<T>; };
 
-// Where the results of one value column go.  min / max / avg (and nonempty, their shared validity) may be null.
-template <typename T> struct GroupOuts { T *sum, *min, *max; long long* count; double* avg; uint32_t* nonempty; };
+// Where the results of one value column go.  min / max / avg (and nonempty, their shared validity) may be null; ACC 2 writes only
+// the moment records `mom`.
+template <typename T> struct GroupOuts { T *sum, *min, *max; long long* count; double* avg; uint32_t* nonempty; Moments* mom; };
 
 // Hot keys.  The work list lives in device memory: {counters, list[]} then the segment partials.
 constexpr long long kBigGroup = 65536;   // rows a single warp still folds itself; also the segment length of k_group_big
-constexpr size_t kPartBytes = 32;        // the largest accumulator (GroupAggX of an integer)
+constexpr size_t kPartBytes = 40;        // the largest accumulator (GroupMoments)
 struct BigGroup { unsigned long long g, begin, end; unsigned int seg0, n_seg; };
 struct BigWork { unsigned int n_groups, n_segments, n_medium; BigGroup list[1]; };   // list[capacity] follows
 // A group longer than kLaneRows rows per lane of a 1- or 8-lane launch is folded by a warp of its own (k_group_medium): one
 // thread must not walk tens of thousands of rows while its neighbours are done after one.
 constexpr long long kLaneRows = 512;
-static_assert(sizeof(GroupAggX<long long>) <= kPartBytes && sizeof(GroupAggX<double>) <= kPartBytes && sizeof(FusedAgg<long long>) <= kPartBytes, "partials");
+static_assert(sizeof(GroupAggX<long long>) <= kPartBytes && sizeof(GroupAggX<double>) <= kPartBytes && sizeof(FusedAgg<long long>) <= kPartBytes &&
+              sizeof(GroupMoments<double>) <= kPartBytes, "partials");
 
-template <typename T, bool EXTRA>
-__device__ __forceinline__ void group_write(const typename GroupAcc<T, EXTRA>::type& acc, unsigned long long cnt, long long g, const GroupOuts<T>& o,
+template <typename T, int ACC>
+__device__ __forceinline__ void group_write(const typename GroupAcc<T, ACC>::type& acc, unsigned long long cnt, long long g, const GroupOuts<T>& o,
                                             bool set_valid) {
     constexpr unsigned long long flip = GroupFlip<T>::value;
-    o.count[g] = (long long)cnt;
-    if constexpr (!EXTRA) {
+    if constexpr (ACC == 2) {
+        o.mom[g] = acc.m;   // the statistics are derived in k_group_stats
+    } else if constexpr (ACC == 0) {
+        o.count[g] = (long long)cnt;
         const FusedAgg<T>& a = acc;
         if constexpr (IsFloat<T>::value) {
             o.sum[g] = (T)a.sum;
@@ -105,6 +112,7 @@ __device__ __forceinline__ void group_write(const typename GroupAcc<T, EXTRA>::t
             }
         }
     } else {
+        o.count[g] = (long long)cnt;
         double dsum;
         if constexpr (IsFloat<T>::value) {
             dsum = acc.sum;
@@ -125,11 +133,11 @@ __device__ __forceinline__ void group_write(const typename GroupAcc<T, EXTRA>::t
 
 // One CTA per (hot group, segment): thread t folds rows begin + t, begin + t + 256, ... of the segment, then warp trees, then the
 // warps in order -> partial[seg0 + segment].  The grid is fixed; CTAs walk the work items (the counters are only known on the device).
-template <typename T, bool EXTRA>
+template <typename T, int ACC>
 __global__ void __launch_bounds__(kThreads)
-k_group_big(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, const BigWork* __restrict__ big, typename GroupAcc<T, EXTRA>::type* __restrict__ part,
+k_group_big(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, const BigWork* __restrict__ big, typename GroupAcc<T, ACC>::type* __restrict__ part,
             unsigned long long* __restrict__ part_cnt) {
-    using Acc = typename GroupAcc<T, EXTRA>::type;
+    using Acc = typename GroupAcc<T, ACC>::type;
     __shared__ Acc s_a[kWarpsPerCta];
     __shared__ unsigned long long s_c[kWarpsPerCta];
     const unsigned int n_big = big->n_groups, n_seg = big->n_segments;
@@ -165,21 +173,21 @@ k_group_big(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, cons
 }
 
 // One thread per hot group: its segment partials in segment order.
-template <typename T, bool EXTRA>
-__global__ void k_group_big_finish(const BigWork* __restrict__ big, const typename GroupAcc<T, EXTRA>::type* __restrict__ part,
+template <typename T, int ACC>
+__global__ void k_group_big_finish(const BigWork* __restrict__ big, const typename GroupAcc<T, ACC>::type* __restrict__ part,
                                    const unsigned long long* __restrict__ part_cnt, const GroupOuts<T> out) {
     const unsigned int gi = blockIdx.x * blockDim.x + threadIdx.x;
     if (gi >= big->n_groups) return;
     const BigGroup bg = big->list[gi];
-    typename GroupAcc<T, EXTRA>::type a = part[bg.seg0];
+    typename GroupAcc<T, ACC>::type a = part[bg.seg0];
     unsigned long long cnt = part_cnt[bg.seg0];
     for (unsigned int k = 1; k < bg.n_seg; k++) { a.merge(part[bg.seg0 + k]); cnt += part_cnt[bg.seg0 + k]; }
-    group_write<T, EXTRA>(a, cnt, (long long)bg.g, out, true);
+    group_write<T, ACC>(a, cnt, (long long)bg.g, out, true);
 }
 
 // LANES lanes per group (32, 8 or 1 -- the launcher picks by the average group length, so ~1e8 one-row groups do not spend a
 // warp each).  No lane leaves before the shuffles: a sub-group that is past the end, or defers its group, folds an empty range.
-template <typename T, int LANES, bool EXTRA>
+template <typename T, int LANES, int ACC>
 __global__ void __launch_bounds__(kThreads)
 k_group_reduce(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, const uint32_t* __restrict__ starts, long long n_groups,
                long long n_rows, const GroupOuts<T> out, BigWork* __restrict__ big, unsigned long long* __restrict__ medium) {
@@ -204,7 +212,7 @@ k_group_reduce(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, c
         mine = false;
         e = b;
     }
-    typename GroupAcc<T, EXTRA>::type a;
+    typename GroupAcc<T, ACC>::type a;
     a.init();
     unsigned long long cnt = 0;
     constexpr unsigned long long flip = GroupFlip<T>::value;
@@ -216,8 +224,8 @@ k_group_reduce(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, c
 #pragma unroll
     for (int o = LANES / 2; o > 0; o >>= 1) { a.merge_shfl(o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o); }
     const bool writer = mine && sub == 0;
-    if (writer) group_write<T, EXTRA>(a, cnt, g, out, false);
-    if constexpr (!IsFloat<T>::value || EXTRA) {
+    if (writer) group_write<T, ACC>(a, cnt, g, out, false);
+    if constexpr (!IsFloat<T>::value || ACC != 0) {
         if (out.nonempty) {   // min/max/avg validity: the warp's groups share one bitmap word -> one store (LANES == 1) or one atomic per warp
             const unsigned bal = __ballot_sync(0xffffffffu, writer && cnt != 0);
             if ((threadIdx.x & 31) == 0) {
@@ -242,7 +250,7 @@ __global__ void k_group_avg(const long long* __restrict__ count, long long n_gro
 
 // A warp per group of the medium list, in the order and with the tree of the 32-lane k_group_reduce (grid-stride over the
 // list, whose length is only known on the device).  The validity bit is OR-ed in: the 1-lane launch stores whole words.
-template <typename T, bool EXTRA>
+template <typename T, int ACC>
 __global__ void __launch_bounds__(kThreads)
 k_group_medium(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, const uint32_t* __restrict__ starts, long long n_groups,
                long long n_rows, const BigWork* __restrict__ big, const unsigned long long* __restrict__ medium, const GroupOuts<T> out) {
@@ -252,7 +260,7 @@ k_group_medium(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, c
     for (unsigned int w = blockIdx.x * kWarpsPerCta + (threadIdx.x >> 5); w < n_med; w += gridDim.x * kWarpsPerCta) {
         const long long g = (long long)medium[w];
         const long long b = starts[g], e = g + 1 < n_groups ? (long long)starts[g + 1] : n_rows;
-        typename GroupAcc<T, EXTRA>::type a;
+        typename GroupAcc<T, ACC>::type a;
         a.init();
         unsigned long long cnt = 0;
         for (long long i = b + lane; i < e; i += 32) {
@@ -262,7 +270,7 @@ k_group_medium(const T* __restrict__ val, const uint32_t* __restrict__ vvalid, c
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) { a.merge_shfl(o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o); }
-        if (lane == 0) group_write<T, EXTRA>(a, cnt, g, out, true);
+        if (lane == 0) group_write<T, ACC>(a, cnt, g, out, true);
     }
 }
 
@@ -286,12 +294,16 @@ __device__ __forceinline__ long long lower_bound_u32(const uint32_t* __restrict_
     return lo;
 }
 
+// out: the group's distinct-value count (may be null); first: the index of its first distinct value in the compacted list (may be
+// null), i.e. the group starts of the distinct values themselves (sum_distinct folds them with launch_group_reduce).
 __global__ void k_group_distinct(const uint32_t* __restrict__ pos, long long n_pos, const uint32_t* __restrict__ starts, long long n_groups,
-                                 long long n_rows, long long* __restrict__ out) {
+                                 long long n_rows, long long* __restrict__ out, uint32_t* __restrict__ first) {
     const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= n_groups) return;
     const long long e = g + 1 < n_groups ? (long long)starts[g + 1] : n_rows;
-    out[g] = lower_bound_u32(pos, n_pos, e) - lower_bound_u32(pos, n_pos, (long long)starts[g]);
+    const long long b = lower_bound_u32(pos, n_pos, (long long)starts[g]);
+    if (out) out[g] = lower_bound_u32(pos, n_pos, e) - b;
+    if (first) first[g] = (uint32_t)b;
 }
 
 // ---- launchers ------------------------------------------------------------------------------------------------------
@@ -314,10 +326,10 @@ size_t group_big_scratch_bytes(long long n_rows) {   // work list + segment part
     return 64 + max_groups * sizeof(BigGroup) + max_segs * (kPartBytes + 8) + max_medium * 8 + 256;
 }
 
-template <typename T, bool EXTRA>
+template <typename T, int ACC>
 static cudaError_t reduce_one(const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows, const GroupOuts<T>& out,
                               void* scratch, int sm_count, cudaStream_t s) {
-    using Acc = typename GroupAcc<T, EXTRA>::type;
+    using Acc = typename GroupAcc<T, ACC>::type;
     BigWork* big = (BigWork*)scratch;
     cudaError_t e = cudaMemsetAsync(big, 0, 16, s);   // the three counters
     if (e != cudaSuccess) return e;
@@ -330,14 +342,14 @@ static cudaError_t reduce_one(const void* val, const uint32_t* vvalid, const uin
     const long long avg = n_rows / n_groups;   // lanes per group by the average group length
     const int lanes = avg > 64 ? 32 : avg > 4 ? 8 : 1;
     const unsigned grid = (unsigned)((n_groups * lanes + kThreads - 1) / kThreads);
-    if (lanes == 32) k_group_reduce<T, 32, EXTRA><<<grid, kThreads, 0, s>>>((const T*)val, vvalid, starts, n_groups, n_rows, out, big, medium);
-    else if (lanes == 8) k_group_reduce<T, 8, EXTRA><<<grid, kThreads, 0, s>>>((const T*)val, vvalid, starts, n_groups, n_rows, out, big, medium);
-    else k_group_reduce<T, 1, EXTRA><<<grid, kThreads, 0, s>>>((const T*)val, vvalid, starts, n_groups, n_rows, out, big, medium);
+    if (lanes == 32) k_group_reduce<T, 32, ACC><<<grid, kThreads, 0, s>>>((const T*)val, vvalid, starts, n_groups, n_rows, out, big, medium);
+    else if (lanes == 8) k_group_reduce<T, 8, ACC><<<grid, kThreads, 0, s>>>((const T*)val, vvalid, starts, n_groups, n_rows, out, big, medium);
+    else k_group_reduce<T, 1, ACC><<<grid, kThreads, 0, s>>>((const T*)val, vvalid, starts, n_groups, n_rows, out, big, medium);
     if (lanes < 32 && n_rows > kLaneRows)   // finds nothing to do when no group is long
-        k_group_medium<T, EXTRA><<<(unsigned)(sm_count * 4), kThreads, 0, s>>>((const T*)val, vvalid, starts, n_groups, n_rows, big, medium, out);
+        k_group_medium<T, ACC><<<(unsigned)(sm_count * 4), kThreads, 0, s>>>((const T*)val, vvalid, starts, n_groups, n_rows, big, medium, out);
     if (n_rows > kBigGroup) {   // hot keys are possible: the two follow-up kernels find nothing to do when there are none
-        k_group_big<T, EXTRA><<<(unsigned)(sm_count * 4), kThreads, 0, s>>>((const T*)val, vvalid, big, part, part_cnt);
-        k_group_big_finish<T, EXTRA><<<(unsigned)((max_groups + 127) / 128), 128, 0, s>>>(big, part, part_cnt, out);
+        k_group_big<T, ACC><<<(unsigned)(sm_count * 4), kThreads, 0, s>>>((const T*)val, vvalid, big, part, part_cnt);
+        k_group_big_finish<T, ACC><<<(unsigned)((max_groups + 127) / 128), 128, 0, s>>>(big, part, part_cnt, out);
     }
     if (out.avg) k_group_avg<<<(unsigned)((n_groups + kThreads - 1) / kThreads), kThreads, 0, s>>>(out.count, n_groups, out.avg);
     return cudaGetLastError();
@@ -347,8 +359,56 @@ template <typename T>
 static cudaError_t reduce_typed(bool extra, const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows, void* sum,
                                 long long* count, void* mn, void* mx, double* avg, uint32_t* nonempty, void* scratch, int sm_count, cudaStream_t s) {
     const GroupOuts<T> out{(T*)sum, (T*)mn, (T*)mx, count, avg, nonempty};
-    return extra ? reduce_one<T, true>(val, vvalid, starts, n_groups, n_rows, out, scratch, sm_count, s)
-                 : reduce_one<T, false>(val, vvalid, starts, n_groups, n_rows, out, scratch, sm_count, s);
+    return extra ? reduce_one<T, 1>(val, vvalid, starts, n_groups, n_rows, out, scratch, sm_count, s)
+                 : reduce_one<T, 0>(val, vvalid, starts, n_groups, n_rows, out, scratch, sm_count, s);
+}
+
+template <typename T>
+static cudaError_t moments_typed(const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows, Moments* mom,
+                                 void* scratch, int sm_count, cudaStream_t s) {
+    GroupOuts<T> out{};
+    out.mom = mom;
+    return reduce_one<T, 2>(val, vvalid, starts, n_groups, n_rows, out, scratch, sm_count, s);
+}
+
+// The moment record of every group (the fold paths of launch_group_reduce with the GroupMoments accumulator).
+cudaError_t launch_group_moments(int dtype, const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows,
+                                 Moments* mom, void* scratch, int sm_count, cudaStream_t s) {
+    if (n_groups <= 0) return cudaSuccess;
+    if (n_groups > 0x7fffffffLL * kWarpsPerCta) return cudaErrorInvalidConfiguration;
+#define BDF_MOMENTS(T) moments_typed<T>(val, vvalid, starts, n_groups, n_rows, mom, scratch, sm_count, s)
+    switch (dtype) {
+        case T_I8: return BDF_MOMENTS(int8_t);
+        case T_I16: return BDF_MOMENTS(int16_t);
+        case T_I32: return BDF_MOMENTS(int32_t);
+        case T_I64: return BDF_MOMENTS(int64_t);
+        case T_U8: return BDF_MOMENTS(uint8_t);
+        case T_U16: return BDF_MOMENTS(uint16_t);
+        case T_U32: return BDF_MOMENTS(uint32_t);
+        case T_U64: return BDF_MOMENTS(uint64_t);
+        case T_F32: return BDF_MOMENTS(float);
+        case T_F64: return BDF_MOMENTS(double);
+        default: return cudaErrorInvalidValue;
+    }
+#undef BDF_MOMENTS
+}
+
+// One statistic of every group's record (moments_stat): the value and the validity bit (0 = None).  The divisions live here, out
+// of the fold, as avg's do in k_group_avg; a warp's 32 groups share one bitmap word, which its first lane stores.
+__global__ void __launch_bounds__(kThreads)
+k_group_stats(const Moments* __restrict__ mom, long long n_groups, int stat, double* __restrict__ out, uint32_t* __restrict__ valid) {
+    const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
+    double v = 0.0;
+    const bool some = g < n_groups && moments_stat(mom[g], stat, &v);
+    if (g < n_groups) out[g] = some ? v : 0.0;
+    const unsigned w = __ballot_sync(0xffffffffu, some);
+    if ((threadIdx.x & 31) == 0 && g < n_groups) valid[g >> 5] = w;
+}
+
+cudaError_t launch_group_stats(const Moments* mom, long long n_groups, int stat, double* out, uint32_t* valid, cudaStream_t s) {
+    if (n_groups <= 0) return cudaSuccess;
+    k_group_stats<<<(unsigned)((n_groups + kThreads - 1) / kThreads), kThreads, 0, s>>>(mom, n_groups, stat, out, valid);
+    return cudaGetLastError();
 }
 
 // scratch: group_big_scratch_bytes(n_rows) of device memory.  mn / mx / avg may be null (without extra, integer mn and mx
@@ -383,9 +443,9 @@ cudaError_t launch_group_bounds(const uint32_t* idx, const uint32_t* starts, lon
 }
 
 cudaError_t launch_group_distinct(const uint32_t* pos, long long n_pos, const uint32_t* starts, long long n_groups, long long n_rows, long long* out,
-                                  cudaStream_t s) {
+                                  uint32_t* first, cudaStream_t s) {
     if (n_groups <= 0) return cudaSuccess;
-    k_group_distinct<<<(unsigned)((n_groups + kThreads - 1) / kThreads), kThreads, 0, s>>>(pos, n_pos, starts, n_groups, n_rows, out);
+    k_group_distinct<<<(unsigned)((n_groups + kThreads - 1) / kThreads), kThreads, 0, s>>>(pos, n_pos, starts, n_groups, n_rows, out, first);
     return cudaGetLastError();
 }
 

@@ -33,6 +33,7 @@
 #include "../../include/b200df.h"
 #include "common.cuh"
 #include "comm.cuh"
+#include "moments.cuh"
 
 using namespace bdf;
 
@@ -1809,9 +1810,25 @@ cudaError_t launch_group_reduce(int dtype, bool extra, const void* val, const ui
 cudaError_t launch_group_bounds(const uint32_t* idx, const uint32_t* starts, long long n_groups, long long n_rows, uint32_t* first, uint32_t* last,
                                 cudaStream_t s);
 cudaError_t launch_group_distinct(const uint32_t* pos, long long n_pos, const uint32_t* starts, long long n_groups, long long n_rows, long long* out,
-                                  cudaStream_t s);
+                                  uint32_t* first, cudaStream_t s);
+cudaError_t launch_group_moments(int dtype, const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows,
+                                 Moments* mom, void* scratch, int sm_count, cudaStream_t s);
+cudaError_t launch_group_stats(const Moments* mom, long long n_groups, int stat, double* out, uint32_t* valid, cudaStream_t s);
 size_t group_big_scratch_bytes(long long n_rows);
 }  // namespace bdf
+
+static bool group_is_stat(int fn) { return fn == BDF_GROUP_KURTOSIS || fn == BDF_GROUP_SKEWNESS || fn == BDF_GROUP_STDDEV || fn == BDF_GROUP_VARIANCE ||
+                                           fn == BDF_GROUP_STDDEV_POP || fn == BDF_GROUP_VAR_POP; }
+static int group_stat_of(int fn) {   // bdf_group_fn -> bdf_stat
+    switch (fn) {
+        case BDF_GROUP_KURTOSIS: return BDF_STAT_KURTOSIS;
+        case BDF_GROUP_SKEWNESS: return BDF_STAT_SKEWNESS;
+        case BDF_GROUP_STDDEV: return BDF_STAT_STDDEV;
+        case BDF_GROUP_VARIANCE: return BDF_STAT_VARIANCE;
+        case BDF_GROUP_STDDEV_POP: return BDF_STAT_STDDEV_POP;
+        default: return BDF_STAT_VAR_POP;
+    }
+}
 
 // Head bitmap (a boolean column of n rows) over one-chunk columns in sorted order.  kernel >= 0: the launch gets a launch record
 // under that bdf_kernel_id (the window's heads); group-by and join keep theirs unrecorded.
@@ -1900,6 +1917,58 @@ static int sorted_runs(bdf_ctx* c, int n_keys, const bdf_col* const* keys, const
     return BDF_OK;
 }
 
+// The distinct valid values of x inside every group: a second stable lexsort over (keys..., x) -- the groups occupy the same row
+// ranges in both sort orders -- and the heads of (keys..., x) on a valid x, each of which starts a distinct value of its group.
+// n_keys == 0: the whole column is one group.  sval: x in that order; pos: the sorted rows of the heads (ascending value order
+// inside every group).
+struct DistinctRuns {
+    explicit DistinctRuns(bdf_ctx* c) : sval(c), dhead(c), pos(c) {}
+    ColOwner sval, dhead, pos;
+};
+
+static int distinct_runs(bdf_ctx* c, int n_keys, const bdf_col* const* keys, const std::vector<const bdf_col*>& sorted_keys, const bdf_col* x,
+                         const bdf_col* iota, int64_t n, DistinctRuns* r) {
+    std::vector<bdf_sort_key> sk2((size_t)n_keys);
+    for (int k = 0; k < n_keys; k++) sk2[k] = bdf_sort_key{keys[k], 0};
+    sk2.push_back(bdf_sort_key{x, 0});
+    ColOwner idx2(c);
+    TRY(sort_indices_dev(c, n_keys + 1, sk2.data(), idx2.out()));
+    TRY(take_dev(c, x, idx2.get(), r->sval.out()));
+    std::vector<const bdf_col*> cols = sorted_keys;
+    cols.push_back(r->sval.get());
+    TRY(group_heads(c, cols, true, n, r->dhead.out()));
+    TRY(filter_dev(c, iota, r->dhead.get(), r->pos.out()));
+    return BDF_OK;
+}
+
+// sum_distinct: the distinct values (the head values, in ascending order inside every group) folded per group by the SUM fold of
+// launch_group_reduce; d_first: the first distinct value of every group (launch_group_distinct's `first`).
+static int distinct_sum(bdf_ctx* c, const DistinctRuns& dr, const uint32_t* d_first, int64_t n_groups, bdf_col** out) {
+    const int dt = dr.sval->dtype;
+    const int w = dtype_width(dt);
+    ColOwner dvals(c), sum(c), cnt(c);
+    TRY(filter_dev(c, dr.sval.get(), dr.dhead.get(), dvals.out()));
+    const int64_t nd = dvals->chunks.empty() ? 0 : dvals->chunks[0].len;
+    TRY(col_alloc(c, dt, {ChunkPlan{n_groups, false}}, nullptr, 0, sum.out()));
+    TRY(col_alloc(c, BDF_I64, {ChunkPlan{n_groups, false}}, nullptr, 0, cnt.out()));
+    if (nd) wait_groups(c->s_compute, dvals.get(), 0, 1);
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_GROUP, dt, nd, nd * w + n_groups * (4 + w + 8));
+        Scratch<void> scratch;
+        e = scratch.alloc(c, group_big_scratch_bytes(nd));
+        c->launches += 3;
+        if (e == cudaSuccess)
+            e = launch_group_reduce(dt, false, nd ? dvals->chunks[0].values : nullptr, nd ? dvals->chunks[0].validity : nullptr, d_first, n_groups, nd,
+                                    sum->chunks[0].values, (long long*)cnt->chunks[0].values, nullptr, nullptr, nullptr, nullptr, scratch, c->sm_count,
+                                    c->s_compute);
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, sum.get());
+    if (e != cudaSuccess) return fail_cuda(e, "distinct sum");
+    *out = sum.release();
+    return BDF_OK;
+}
+
 static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int n_aggs, const bdf_group_agg* aggs, bdf_col** out_keys, bdf_col** out,
                         int64_t* n_groups_out) {
     if (n_keys < 1 || n_keys > 16) return fail(BDF_INVALID, "1..16 group key columns");
@@ -1912,7 +1981,7 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
         const bdf_col* v = aggs[j].column;
         if (!v) return fail(BDF_INVALID, "null value column");
         if (v->dtype < 0 || v->dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "aggregated columns must be numeric");
-        if (aggs[j].function < BDF_GROUP_SUM || aggs[j].function > BDF_GROUP_LAST) return fail(BDF_UNSUPPORTED, "unknown group function %d", aggs[j].function);
+        if (aggs[j].function < BDF_GROUP_SUM || aggs[j].function > BDF_GROUP_VAR_POP) return fail(BDF_UNSUPPORTED, "unknown group function %d", aggs[j].function);
         if (aggs[j].function == BDF_GROUP_AVG && (v->dtype == BDF_I64 || v->dtype == BDF_U64)) return fail(BDF_UNSUPPORTED, "avg needs f64: From<T::Native>");
         if (v->total_len != keys[0]->total_len) return fail(BDF_LENGTH_MISMATCH, "key and value columns have different lengths");
     }
@@ -1930,7 +1999,7 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
     std::vector<bool> done((size_t)n_aggs, false);
     for (int j0 = 0; j0 < n_aggs; j0++) {
         const int f0 = aggs[j0].function;
-        if (done[j0] || f0 == BDF_GROUP_COUNT_DISTINCT || f0 == BDF_GROUP_FIRST || f0 == BDF_GROUP_LAST) continue;
+        if (done[j0] || f0 == BDF_GROUP_COUNT_DISTINCT || f0 == BDF_GROUP_FIRST || f0 == BDF_GROUP_LAST || f0 > BDF_GROUP_LAST) continue;
         const bdf_col* v = aggs[j0].column;
         bool want[5] = {false, false, false, false, false};   // sum, max, min, avg, count (bdf_group_fn order)
         for (int j = j0; j < n_aggs; j++)
@@ -2006,32 +2075,79 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
         if (aggs[j].function == BDF_GROUP_FIRST || aggs[j].function == BDF_GROUP_LAST)
             TRY(take_dev(c, aggs[j].column, aggs[j].function == BDF_GROUP_FIRST ? first_rows.get() : last_rows.get(), res[j].out()));
 
-    // count_distinct: a second stable lexsort over (keys..., value); a head of (keys..., value) on a valid value starts a
-    // distinct value of its group (the groups occupy the same row ranges in both sort orders)
-    for (int j = 0; j < n_aggs; j++) {
-        if (aggs[j].function != BDF_GROUP_COUNT_DISTINCT) continue;
-        std::vector<bdf_sort_key> sk2((size_t)n_keys);
-        for (int k = 0; k < n_keys; k++) sk2[k] = bdf_sort_key{keys[k], 0};
-        sk2.push_back(bdf_sort_key{aggs[j].column, 0});
-        ColOwner idx2(c), sval(c), dhead(c), pos(c);
-        TRY(sort_indices_dev(c, n_keys + 1, sk2.data(), idx2.out()));
-        TRY(take_dev(c, aggs[j].column, idx2.get(), sval.out()));
-        std::vector<const bdf_col*> cols;
-        for (const ColOwner& s : runs.sorted) cols.push_back(s.get());
-        cols.push_back(sval.get());
-        TRY(group_heads(c, cols, true, n, dhead.out()));
-        TRY(filter_dev(c, runs.iota.get(), dhead.get(), pos.out()));
-        TRY(col_alloc(c, BDF_I64, {ChunkPlan{n_groups, false}}, nullptr, 0, res[j].out()));
-        bdf_col* cd = res[j].get();
-        wait_groups(c->s_compute, pos.get(), 0, 1);
-        c->launches++;
+    // variance / stddev / skewness / kurtosis (and the population forms): every value column is gathered once and folded once into
+    // a moment record per group; every requested statistic is then one small kernel over the records
+    std::vector<bool> stat_done((size_t)n_aggs, false);
+    for (int j0 = 0; j0 < n_aggs; j0++) {
+        if (stat_done[j0] || !group_is_stat(aggs[j0].function)) continue;
+        const bdf_col* v = aggs[j0].column;
+        ColOwner sval(c);
+        TRY(take_dev(c, v, idx, sval.out()));
+        for (int j = j0; j < n_aggs; j++)
+            if (aggs[j].column == v && group_is_stat(aggs[j].function)) TRY(col_alloc(c, BDF_F64, {ChunkPlan{n_groups, true}}, nullptr, 0, res[j].out()));
+        wait_groups(c->s_compute, sval.get(), 0, 1);
+        wait_groups(c->s_compute, runs.starts.get(), 0, 1);
+        Scratch<void> scratch;
+        Scratch<Moments> mom;
         {
-            LaunchTimer t(c, BDF_K_GROUP, BDF_I64, n_groups, n_groups * 16);
-            e = launch_group_distinct((const uint32_t*)pos->chunks[0].values, pos->chunks[0].len, d_starts, n_groups, n, (long long*)cd->chunks[0].values,
-                                      c->s_compute);
+            const int w = dtype_width(v->dtype);
+            LaunchTimer t(c, BDF_K_GROUP, v->dtype, n, n * w + (sval->chunks[0].validity ? bitmap_bytes(n) : 0) + n_groups * (4 + (int64_t)sizeof(Moments)));
+            e = scratch.alloc(c, group_big_scratch_bytes(n));
+            if (e == cudaSuccess) e = mom.alloc(c, (size_t)std::max<int64_t>(n_groups, 1) * sizeof(Moments));
+            c->launches += 3;   // as for the other folds: k_group_medium, k_group_big, k_group_big_finish
+            if (e == cudaSuccess)
+                e = launch_group_moments(v->dtype, sval->chunks[0].values, sval->chunks[0].validity, d_starts, n_groups, n, mom, scratch, c->sm_count,
+                                         c->s_compute);
         }
-        if (e == cudaSuccess) e = finish_single_group(c, cd);
-        if (e != cudaSuccess) return fail_cuda(e, "group distinct count");
+        for (int j = j0; j < n_aggs && e == cudaSuccess; j++) {
+            if (aggs[j].column != v || !group_is_stat(aggs[j].function)) continue;
+            bdf_col* r = res[j].get();
+            {
+                LaunchTimer t(c, BDF_K_GROUP, BDF_F64, n_groups, n_groups * ((int64_t)sizeof(Moments) + 8) + bitmap_bytes(n_groups));
+                e = launch_group_stats(mom, n_groups, group_stat_of(aggs[j].function), (double*)r->chunks[0].values, r->chunks[0].validity, c->s_compute);
+            }
+            if (e == cudaSuccess) e = finish_single_group(c, r);
+            r->null_counts[0] = -1;   // learnt on demand (ensure_null_counts)
+            stat_done[j] = true;
+        }
+        if (e != cudaSuccess) return fail_cuda(e, "group statistics");
+    }
+
+    // count_distinct / sum_distinct: the distinct valid values of every group (distinct_runs); count_distinct counts them, sum_distinct
+    // folds them -- in ascending order, with the SUM fold of launch_group_reduce over their own group starts
+    for (int j = 0; j < n_aggs; j++) {
+        const int fn = aggs[j].function;
+        if (fn != BDF_GROUP_COUNT_DISTINCT && fn != BDF_GROUP_SUM_DISTINCT) continue;
+        std::vector<const bdf_col*> sorted_keys;
+        for (const ColOwner& s : runs.sorted) sorted_keys.push_back(s.get());
+        DistinctRuns dr(c);
+        TRY(distinct_runs(c, n_keys, keys, sorted_keys, aggs[j].column, runs.iota.get(), n, &dr));
+        if (fn == BDF_GROUP_COUNT_DISTINCT) {
+            TRY(col_alloc(c, BDF_I64, {ChunkPlan{n_groups, false}}, nullptr, 0, res[j].out()));
+            bdf_col* cd = res[j].get();
+            wait_groups(c->s_compute, dr.pos.get(), 0, 1);
+            c->launches++;
+            {
+                LaunchTimer t(c, BDF_K_GROUP, BDF_I64, n_groups, n_groups * 16);
+                e = launch_group_distinct((const uint32_t*)dr.pos->chunks[0].values, dr.pos->chunks[0].len, d_starts, n_groups, n,
+                                          (long long*)cd->chunks[0].values, nullptr, c->s_compute);
+            }
+            if (e == cudaSuccess) e = finish_single_group(c, cd);
+            if (e != cudaSuccess) return fail_cuda(e, "group distinct count");
+        } else {
+            ColOwner dstarts(c);
+            TRY(col_alloc(c, BDF_U32, {ChunkPlan{n_groups, false}}, nullptr, 0, dstarts.out()));
+            wait_groups(c->s_compute, dr.pos.get(), 0, 1);
+            c->launches++;
+            {
+                LaunchTimer t(c, BDF_K_GROUP, BDF_U32, n_groups, n_groups * 12);
+                e = launch_group_distinct((const uint32_t*)dr.pos->chunks[0].values, dr.pos->chunks[0].len, d_starts, n_groups, n, nullptr,
+                                          (uint32_t*)dstarts->chunks[0].values, c->s_compute);
+            }
+            if (e == cudaSuccess) e = finish_single_group(c, dstarts.get());
+            if (e != cudaSuccess) return fail_cuda(e, "group distinct starts");
+            TRY(distinct_sum(c, dr, (const uint32_t*)dstarts->chunks[0].values, n_groups, res[j].out()));
+        }
     }
     for (int k = 0; k < n_keys; k++) out_keys[k] = runs.distinct[k].release();
     for (int j = 0; j < n_aggs; j++) out[j] = res[j].release();
@@ -2069,6 +2185,85 @@ static int group_aggregate_dev(bdf_ctx* c, const bdf_col* key, int n_values, con
         outs[j].min = is_int ? res[r++] : nullptr;
         outs[j].max = is_int ? res[r++] : nullptr;
     }
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// statistical aggregates (k_moments.cu, moments.cuh): the moment record of a whole column, and its distinct values
+
+namespace bdf {
+cudaError_t launch_moments(int dtype, const RedDesc* d, int n, int64_t tiles, Moments* partials, Moments* result, cudaStream_t s);
+int64_t moments_partials(int64_t tiles);
+}  // namespace bdf
+
+static_assert(sizeof(Moments) == sizeof(bdf_moment_rec) && offsetof(bdf_moment_rec, m4) == offsetof(Moments, m4), "bdf_moment_rec layout");
+
+// One launch of k_moments over every chunk and its finish; on a rank of a communicator the records of all ranks are all-gathered
+// and merged in rank order, so every rank returns the same bits.
+static int moments_dev(bdf_ctx* c, const bdf_col* col, Moments* out) {
+    if (col->dtype < 0 || col->dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "the statistics need a numeric column");
+    const int64_t n = (int64_t)col->chunks.size();
+    wait_groups(c->s_compute, col, 0, n);
+    const int tile = elems_per_tile(col->dtype);
+    void *hp = nullptr, *dp = nullptr;
+    TRY(ring_alloc(c, (size_t)std::max<int64_t>(n, 1) * sizeof(RedDesc), &hp, &dp));
+    RedDesc* hd = (RedDesc*)hp;
+    int64_t tiles = 0, rows = 0;
+    for (int64_t i = 0; i < n; i++) {
+        const DevChunk& ch = col->chunks[i];
+        hd[i].in = ch.values; hd[i].vin = ch.validity; hd[i].len = ch.len; hd[i].tile0 = tiles; hd[i].off = ch.bit_off; hd[i].pad = 0;
+        tiles += (ch.len + tile - 1) / tile;
+        rows += ch.len;
+    }
+    CK(desc_upload(c, dp, hd, (size_t)n * sizeof(RedDesc)));
+    Scratch<Moments> parts;
+    Moments* result = (Moments*)c->h_agg_dev;   // device-mapped pinned memory: the finish writes the record straight to the host
+    {
+        LaunchTimer t(c, BDF_K_MOMENTS, col->dtype, rows, reduce_bytes(col, 0, n));   // k_moments + k_moments_finish
+        CK(parts.alloc(c, (size_t)std::max<int64_t>(moments_partials(tiles), 1) * sizeof(Moments)));
+        CK(launch_moments(col->dtype, (const RedDesc*)dp, (int)n, tiles, parts, result, c->s_compute));
+        c->launches++;
+    }
+    CK(cudaStreamSynchronize(c->s_compute));
+    Moments mine;
+    memcpy(&mine, (const void*)c->h_agg, sizeof mine);
+    if (is_global(c)) {
+        std::vector<Moments> all((size_t)comm_world(c->comm));
+        std::string err;
+        c->collectives++;
+        cudaError_t e = comm_host_allgather(c->comm, &mine, all.data(), sizeof(Moments), c->s_compute, &err);
+        if (e != cudaSuccess) { g_nccl_err = err; return fail_cuda(e, "moments"); }
+        mine = Moments{0, 0.0, 0.0, 0.0, 0.0};
+        for (const Moments& m : all) mine = moments_merge(mine, m);
+    }
+    *out = mine;
+    return BDF_OK;
+}
+
+// count_distinct / sum_distinct of a whole column: the group-by's distinct machinery with the column as one group.
+static int distinct_dev(bdf_ctx* c, const bdf_col* x, bdf_distinct_rec* out) {
+    if (x->dtype < 0 || x->dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "count_distinct / sum_distinct need a numeric column");
+    if (is_global(c))
+        return fail(BDF_UNSUPPORTED, "distinct values need every row of the column on one GPU (as sort / group-by / join): use a one-GPU context");
+    const int64_t n = x->total_len;
+    if (n == 0) { *out = bdf_distinct_rec{0, 0}; return BDF_OK; }
+    ColOwner iota(c), first(c), sum(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, iota.out()));
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{1, false}}, nullptr, 0, first.out()));
+    c->launches++;
+    cudaError_t e = launch_iota((uint32_t*)iota->chunks[0].values, n, c->sm_count, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemsetAsync(first->chunks[0].values, 0, sizeof(uint32_t), c->s_compute);   // the one group starts at 0
+    if (e == cudaSuccess) e = finish_single_group(c, iota.get());
+    if (e == cudaSuccess) e = finish_single_group(c, first.get());
+    if (e != cudaSuccess) return fail_cuda(e, "distinct iota");
+    DistinctRuns dr(c);
+    TRY(distinct_runs(c, 0, nullptr, {}, x, iota.get(), n, &dr));
+    const int64_t count = dr.pos->chunks.empty() ? 0 : dr.pos->chunks[0].len;
+    TRY(distinct_sum(c, dr, (const uint32_t*)first->chunks[0].values, 1, sum.out()));
+    uint64_t bits = 0;
+    CK(cudaMemcpyAsync(&bits, sum->chunks[0].values, (size_t)dtype_width(x->dtype), cudaMemcpyDeviceToHost, c->s_compute));
+    CK(cudaStreamSynchronize(c->s_compute));
+    *out = bdf_distinct_rec{count, bits};
     return BDF_OK;
 }
 
@@ -3253,6 +3448,32 @@ static int fleet_avg_dev(bdf_ctx* c, const bdf_col* col, double* out, int32_t* i
     return BDF_OK;
 }
 
+// Every GPU computes the record of its row ranges; the kids of a fleet of several GPUs are the ranks of one communicator, so each
+// of them all-gathers the records and merges them in rank order (moments_dev) and returns the same bits.  A fleet of one GPU is the
+// one-GPU context's call.
+static int fleet_moments_dev(bdf_ctx* c, const bdf_col* col, bdf_moment_rec* out) {
+    Fleet* f = c->fleet;
+    if (!is_fleet_col(col)) return fail(BDF_INVALID, "a column of a one-GPU context was passed to a multi-GPU context");
+    std::vector<bdf_moment_rec> rec(f->kids.size());
+    TRY(fleet_run(f, [&](int k) { return bdf_moments_dev(f->kids[k], col->fparts[k], &rec[k]); }));
+    *out = rec[0];
+    return BDF_OK;
+}
+
+static int fleet_moments_host(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_moment_rec* out) {
+    bdf_col* col = nullptr;
+    const int32_t dt = dtype;
+    const bdf_view* ptr = in;
+    TRY(fleet_upload_many(c, 1, &dt, &n, &ptr, BDF_ASYNC, &col));
+    const int st = fleet_moments_dev(c, col, out);
+    const std::string keep = g_err;
+    Fleet* f = c->fleet;
+    fleet_run(f, [&](int k) { return bdf_col_wait(f->kids[k], col->fparts[k]); });   // host inputs must not be touched after return
+    fleet_col_free(f, col);
+    g_err = keep;
+    return st;
+}
+
 // Fused operator + aggregate: every kid runs the one-GPU entry on its parts; the future yields the global records.
 static int fleet_with_future(bdf_ctx* c, int out_dtype, std::initializer_list<const bdf_col*> inputs, bool want_col, bdf_col** out, bdf_future** fut,
                              const std::function<int(int, bdf_col**, bdf_future**)>& call) {
@@ -3901,6 +4122,45 @@ int bdf_avg_dev(bdf_ctx* c, const bdf_col* in, double* out, int32_t* is_some) {
     return avg_dev(c, const_cast<bdf_col*>(in), out, is_some);
 }
 
+int bdf_moments_dev(bdf_ctx* c, const bdf_col* in, bdf_moment_rec* out) {
+    if (c && c->fleet) { if (!in || !out) return fail(BDF_INVALID, "null argument"); return fleet_moments_dev(c, in, out); }
+    ENTER(c);
+    if (!in || !out) return fail(BDF_INVALID, "null argument");
+    Moments m;
+    TRY(moments_dev(c, in, &m));
+    memcpy(out, &m, sizeof m);
+    return BDF_OK;
+}
+
+int bdf_distinct_dev(bdf_ctx* c, const bdf_col* in, bdf_distinct_rec* out) {
+    if (c && c->fleet)
+        return fail(BDF_UNSUPPORTED, "distinct values need every row of the column on one GPU (as sort / group-by / join): use a one-GPU context");
+    ENTER(c);
+    if (!in || !out) return fail(BDF_INVALID, "null argument");
+    return distinct_dev(c, in, out);
+}
+
+int bdf_moments_stat(const bdf_moment_rec* m, int stat, double* out, int32_t* is_some) {
+    if (!m || !out || !is_some) return fail(BDF_INVALID, "null argument");
+    if (stat < BDF_STAT_VARIANCE || stat > BDF_STAT_KURTOSIS) return fail(BDF_INVALID, "unknown statistic %d", stat);
+    Moments r;
+    memcpy(&r, m, sizeof r);
+    double v = 0.0;
+    *is_some = moments_stat(r, stat, &v) ? 1 : 0;
+    *out = v;
+    return BDF_OK;
+}
+
+int bdf_moments_merge(const bdf_moment_rec* a, const bdf_moment_rec* b, bdf_moment_rec* out) {
+    if (!a || !b || !out) return fail(BDF_INVALID, "null argument");
+    Moments x, y;
+    memcpy(&x, a, sizeof x);
+    memcpy(&y, b, sizeof y);
+    const Moments r = moments_merge(x, y);
+    memcpy(out, &r, sizeof r);
+    return BDF_OK;
+}
+
 int bdf_binary_agg_dev_async(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bdf_col** out, bdf_future** fut) {
     if (c && c->fleet) {
         if (!l || !r || !out || !fut) return fail(BDF_INVALID, "null argument");
@@ -4256,6 +4516,51 @@ int bdf_avg(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, double* out, i
     std::vector<bdf_col*> cols;
     TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
     int st = avg_dev(c, cols[0], out, is_some);
+    std::string keep = g_err;
+    cudaStreamSynchronize(c->s_h2d);
+    col_release(c, cols[0]);
+    g_err = keep;
+    return st;
+}
+
+// Host-in entries of the statistics: a Boolean column is a type the operators do not take (BDF_UNSUPPORTED), not a bad dtype.
+static int check_stat_dtype(int dtype) {
+    if (dtype == kBool) return fail(BDF_UNSUPPORTED, "the statistics need a numeric column");
+    return check_dtype(dtype);
+}
+
+int bdf_moments(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_moment_rec* out) {
+    if (c && c->fleet) {
+        TRY(check_stat_dtype(dtype));
+        if (n < 0 || (n && !in) || !out) return fail(BDF_INVALID, "bad arguments");
+        return fleet_moments_host(c, dtype, n, in, out);
+    }
+    ENTER(c);
+    TRY(check_stat_dtype(dtype));
+    if (n < 0 || (n && !in) || !out) return fail(BDF_INVALID, "bad arguments");
+    std::vector<bdf_col*> cols;
+    TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
+    Moments m;
+    int st = moments_dev(c, cols[0], &m);
+    std::string keep = g_err;
+    cudaStreamSynchronize(c->s_h2d);
+    col_release(c, cols[0]);
+    g_err = keep;
+    if (st == BDF_OK) memcpy(out, &m, sizeof m);
+    return st;
+}
+
+int bdf_distinct(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_distinct_rec* out) {
+    if (c && c->fleet)
+        return fail(BDF_UNSUPPORTED, "distinct values need every row of the column on one GPU (as sort / group-by / join): use a one-GPU context");
+    ENTER(c);
+    TRY(check_stat_dtype(dtype));
+    if (n < 0 || (n && !in) || !out) return fail(BDF_INVALID, "bad arguments");
+    if (is_global(c))
+        return fail(BDF_UNSUPPORTED, "distinct values need every row of the column on one GPU (as sort / group-by / join): use a one-GPU context");
+    std::vector<bdf_col*> cols;
+    TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
+    int st = distinct_dev(c, cols[0], out);
     std::string keep = g_err;
     cudaStreamSynchronize(c->s_h2d);
     col_release(c, cols[0]);

@@ -191,8 +191,90 @@ class AggregateFunctions:
         N.raise_for_status(N.lib().bdf_aggregate_all(ctx.handle, dtype, len(arrays), N.make_views(arrays), C.byref(a)))
         return _agg4_to_dict(dtype, a)
 
+    # -- statistical aggregates (include/b200df.h "statistical aggregates"): the stubs of aggregate.rs:81,94-102 --
+    @staticmethod
+    def moments(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> dict:
+        """The moment record {count, mean, m2, m3, m4} of the valid values, every numeric type read ``as f64``."""
+        ctx = ctx or N.default_context()
+        if dtype is None:
+            dtype = _dtype_of(arrays) if len(arrays) else N_I64_FALLBACK
+        r = N.MomentRec()
+        N.raise_for_status(N.lib().bdf_moments(ctx.handle, dtype, len(arrays), N.make_views(arrays), C.byref(r)))
+        return _moments_to_dict(r)
+
+    @staticmethod
+    def variance(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> Optional[float]:
+        """Sample variance m2 / (n - 1), as Spark's variance."""
+        return moments_stat(AggregateFunctions.moments(arrays, dtype, ctx), "variance")
+
+    @staticmethod
+    def variance_pop(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> Optional[float]:
+        return moments_stat(AggregateFunctions.moments(arrays, dtype, ctx), "var_pop")
+
+    @staticmethod
+    def stddev(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> Optional[float]:
+        """Sample standard deviation sqrt(m2 / (n - 1)), as Spark's stddev."""
+        return moments_stat(AggregateFunctions.moments(arrays, dtype, ctx), "stddev")
+
+    @staticmethod
+    def stddev_pop(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> Optional[float]:
+        return moments_stat(AggregateFunctions.moments(arrays, dtype, ctx), "stddev_pop")
+
+    @staticmethod
+    def skewness(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> Optional[float]:
+        return moments_stat(AggregateFunctions.moments(arrays, dtype, ctx), "skewness")
+
+    @staticmethod
+    def kurtosis(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> Optional[float]:
+        """Excess kurtosis n m4 / m2^2 - 3."""
+        return moments_stat(AggregateFunctions.moments(arrays, dtype, ctx), "kurtosis")
+
+    @staticmethod
+    def _distinct(arrays: Chunks, dtype: Optional[int], ctx):
+        ctx = ctx or N.default_context()
+        if dtype is None:
+            dtype = _dtype_of(arrays) if len(arrays) else N_I64_FALLBACK
+        r = N.DistinctRec()
+        N.raise_for_status(N.lib().bdf_distinct(ctx.handle, dtype, len(arrays), N.make_views(arrays), C.byref(r)))
+        return dtype, r
+
+    @staticmethod
+    def count_distinct(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> int:
+        """The number of distinct valid values (all NaNs are one value, -0.0 == 0.0)."""
+        return int(AggregateFunctions._distinct(arrays, dtype, ctx)[1].count)
+
+    @staticmethod
+    def sum_distinct(arrays: Chunks, dtype: Optional[int] = None, ctx=None):
+        """The sum of the distinct valid values in the dtype of the column (0 when there is none, like ``sum``)."""
+        dtype, r = AggregateFunctions._distinct(arrays, dtype, ctx)
+        return _scalar_from_bits(dtype, r.sum)
+
 
 N_I64_FALLBACK = 3  # Int64: only used to type an empty Vec (results do not depend on it)
+
+
+def _moments_to_dict(r: "N.MomentRec") -> dict:
+    return {"count": int(r.count), "mean": float(r.mean), "m2": float(r.m2), "m3": float(r.m3), "m4": float(r.m4)}
+
+
+def moments_stat(rec: dict, stat: str) -> Optional[float]:
+    """bdf_moments_stat: one of "variance", "var_pop", "stddev", "stddev_pop", "skewness", "kurtosis" from a moment record (no
+    context and no GPU needed); ``None`` is Rust's None."""
+    if stat not in N.STATS:
+        raise N.ComputeError(f"unknown statistic {stat!r}")
+    r = N.MomentRec(rec["count"], rec["mean"], rec["m2"], rec["m3"], rec["m4"])
+    out, some = C.c_double(0), C.c_int32(0)
+    N.raise_for_status(N.lib().bdf_moments_stat(C.byref(r), N.STATS[stat], C.byref(out), C.byref(some)))
+    return out.value if some.value else None
+
+
+def moments_merge(a: dict, b: dict) -> dict:
+    """bdf_moments_merge: the record of the union of two sets of values (the merge the library uses across GPUs)."""
+    ra = N.MomentRec(a["count"], a["mean"], a["m2"], a["m3"], a["m4"])
+    rb = N.MomentRec(b["count"], b["mean"], b["m2"], b["m3"], b["m4"])
+    out = N.MomentRec()
+    N.raise_for_status(N.lib().bdf_moments_merge(C.byref(ra), C.byref(rb), C.byref(out)))
+    return _moments_to_dict(out)
 
 
 def _agg4_to_dict(dtype: int, a: "N.Agg4") -> dict:
@@ -398,6 +480,26 @@ class Column:
         N.raise_for_status(N.lib().bdf_avg_dev(self.ctx.handle, self.handle, C.byref(out), C.byref(some)))
         return out.value if some.value else None
 
+    def moments(self) -> dict:
+        r = N.MomentRec()
+        N.raise_for_status(N.lib().bdf_moments_dev(self.ctx.handle, self.handle, C.byref(r)))
+        return _moments_to_dict(r)
+
+    def variance(self): return moments_stat(self.moments(), "variance")
+    def variance_pop(self): return moments_stat(self.moments(), "var_pop")
+    def stddev(self): return moments_stat(self.moments(), "stddev")
+    def stddev_pop(self): return moments_stat(self.moments(), "stddev_pop")
+    def skewness(self): return moments_stat(self.moments(), "skewness")
+    def kurtosis(self): return moments_stat(self.moments(), "kurtosis")
+
+    def _distinct(self):
+        r = N.DistinctRec()
+        N.raise_for_status(N.lib().bdf_distinct_dev(self.ctx.handle, self.handle, C.byref(r)))
+        return r
+
+    def count_distinct(self) -> int: return int(self._distinct().count)
+    def sum_distinct(self): return _scalar_from_bits(self.dtype, self._distinct().sum)
+
     @staticmethod
     def aggregate_all_many(columns: Sequence["Column"], asynchronous: bool = False):
         """sum/min/max/count of several columns in ONE call: one reduction per column, one host wait and (on a rank of
@@ -493,9 +595,10 @@ def group_aggregate(key: "Column", values: Sequence["Column"]):
 
 def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
     """Group-by over 1..16 key columns (bdf_group_by_dev).  ``aggregations``: ``[(Column, function)]`` with function one of
-    "sum", "max", "min", "avg", "count", "count_distinct", "first", "last".  Returns ``([key Column per key],
-    [result Column per aggregation])``; groups in the order DataFrame::sort gives (ascending, nulls last per key).  Counts are
-    Int64, avg is Float64, everything else has the value column's type; see include/b200df.h for the NULL rules."""
+    "sum", "max", "min", "avg", "count", "count_distinct", "first", "last", "kurtosis", "skewness", "stddev", "sum_distinct",
+    "variance", "stddev_pop", "var_pop".  Returns ``([key Column per key], [result Column per aggregation])``; groups in the order
+    DataFrame::sort gives (ascending, nulls last per key).  Counts are Int64, avg and the statistics are Float64, everything else
+    has the value column's type; see include/b200df.h for the NULL rules."""
     fns = []
     for _, fn in aggregations:
         if fn not in N.GROUP_FNS:

@@ -9,6 +9,7 @@
 #pragma once
 
 #include <algorithm>
+#include <cstring>
 #include <optional>
 #include <string>
 #include <utility>
@@ -177,8 +178,37 @@ struct AggregateFunctions {
         check(bdf_avg(context(), ArrowType<T>::id, (int64_t)v.size(), v.data(), &out, &some));
         return some ? std::optional<double>(out) : std::nullopt;
     }
+    // The stubs of aggregate.rs:81,94-102 (include/b200df.h "statistical aggregates"): sample variance / stddev as Spark's, the
+    // population forms, skewness, excess kurtosis; any numeric T, read as f64.
+    template <typename T> static std::optional<double> variance(const Arrays<T>& a) { return stat<T>(BDF_STAT_VARIANCE, a); }
+    template <typename T> static std::optional<double> variance_pop(const Arrays<T>& a) { return stat<T>(BDF_STAT_VAR_POP, a); }
+    template <typename T> static std::optional<double> stddev(const Arrays<T>& a) { return stat<T>(BDF_STAT_STDDEV, a); }
+    template <typename T> static std::optional<double> stddev_pop(const Arrays<T>& a) { return stat<T>(BDF_STAT_STDDEV_POP, a); }
+    template <typename T> static std::optional<double> skewness(const Arrays<T>& a) { return stat<T>(BDF_STAT_SKEWNESS, a); }
+    template <typename T> static std::optional<double> kurtosis(const Arrays<T>& a) { return stat<T>(BDF_STAT_KURTOSIS, a); }
+    template <typename T> static int64_t count_distinct(const Arrays<T>& a) { return distinct<T>(a).count; }
+    template <typename T> static T sum_distinct(const Arrays<T>& a) {   // 0 without a valid value, like sum
+        const bdf_distinct_rec r = distinct<T>(a);
+        T out{};
+        std::memcpy(&out, &r.sum, sizeof(T));
+        return out;
+    }
 
    private:
+    template <typename T> static std::optional<double> stat(int which, const Arrays<T>& a) {
+        auto v = detail::views(a);
+        bdf_moment_rec m{};
+        check(bdf_moments(context(), ArrowType<T>::id, (int64_t)v.size(), v.data(), &m));
+        double out = 0; int32_t some = 0;
+        check(bdf_moments_stat(&m, which, &out, &some));
+        return some ? std::optional<double>(out) : std::nullopt;
+    }
+    template <typename T> static bdf_distinct_rec distinct(const Arrays<T>& a) {
+        auto v = detail::views(a);
+        bdf_distinct_rec r{};
+        check(bdf_distinct(context(), ArrowType<T>::id, (int64_t)v.size(), v.data(), &r));
+        return r;
+    }
     static void check(int st) {
         if (st == BDF_WOULD_PANIC) throw ReferencePanic(bdf_last_error());
         if (st == BDF_UNSUPPORTED) throw std::logic_error(std::string("trait bound not satisfied: ") + bdf_last_error());
