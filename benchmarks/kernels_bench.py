@@ -8,6 +8,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --window [--rows 100000000]                      # only the window-function rows
     python benchmarks/kernels_bench.py --math [--rows 100000000]                        # only the float-function rows
     python benchmarks/kernels_bench.py --stats [--rows 100000000]                       # only the statistical-aggregate rows
+    python benchmarks/kernels_bench.py --csv-write [--csv-rows 50000000]                # the CSV writer rows (the reader's table written back)
 """
 from __future__ import annotations
 
@@ -131,6 +132,62 @@ def csv_bench(ctx, rows, rows_out, reps=3):
         name = f"Arrow C++ (not the reference) read_csv, {os.cpu_count()} cores"
         rows_out.append({"case": name, "config": "csv", "kernel": "host", "ms": ms, "rows": rows, "file_bytes": nbytes, "GBs_of_file": nbytes / ms / 1e6})
         print(f"{name:44s} {ms:9.2f} ms  {nbytes / ms / 1e6:7.2f} GB/s of file bytes", flush=True)
+
+
+def csv_write_bench(ctx, rows, rows_out, reps=3):
+    """The reader benchmark's table (Int64, two Float64, Boolean) read onto the device, then written back: the measure + scan and
+    emit kernels (launch records) in GB/s of text, end to end to /dev/null (D2H and the pipeline without a file system) and to a file;
+    pyarrow's write_csv on the host cores.  Medians of `reps` runs after a warm-up."""
+    print("card:", _card(), flush=True)
+    with tempfile.TemporaryDirectory() as td:
+        src = os.path.join(td, "bench.csv")
+        write_csv(src, rows)
+        with rdf.CsvFile(src, schema=[rdf.I64, rdf.F64, rdf.F64, N.BOOL, N.UTF8], batch_size=1 << 20, ctx=ctx) as f:
+            cols = f.read(["id", "lat", "lng", "flag"])
+        os.unlink(src)
+        out = os.path.join(td, "out.csv")
+        rdf.write_csv(out, cols)
+        text = os.path.getsize(out)
+        res = {"measure + scan": [], "emit": [], "end to end, /dev/null": [], "end to end, file": []}
+        for i in range(reps + 1):
+            for target, key in (("/dev/null", "end to end, /dev/null"), (out, "end to end, file")):
+                ctx.synchronize()
+                ctx.profile_read()
+                ctx.profile_enable(True)
+                t0 = time.perf_counter()
+                rdf.write_csv(target, cols)
+                t1 = time.perf_counter()
+                ctx.profile_enable(False)
+                recs = [r for r in ctx.profile_read() if r["kernel"] == "csv_write"]
+                if i == 0:
+                    continue
+                res[key].append((t1 - t0) * 1e3)
+                if target == "/dev/null":
+                    res["measure + scan"].append(sum(r["ms"] for r in recs if r["dtype"] == rdf.U64))
+                    res["emit"].append(sum(r["ms"] for r in recs if r["dtype"] == rdf.U8))
+        for key, v in res.items():
+            ms = float(np.median(v))
+            rows_out.append({"case": f"csv write {key}", "config": "csv-write", "kernel": "csv_write", "ms": ms, "rows": rows, "text_bytes": text,
+                             "GBs_of_text": text / ms / 1e6})
+            print(f"{'csv write ' + key:44s} {ms:9.2f} ms  {text / ms / 1e6:7.2f} GB/s of text ({text / 1e9:.2f} GB, {rows:.1e} rows)", flush=True)
+        try:
+            import pyarrow as pa
+            import pyarrow.csv as pacsv
+        except ImportError:
+            return
+        host = {n: np.concatenate([a.value_bits() if n == "flag" else a.value_slice() for a in c.download()]) for n, c in cols.items()}
+        table = pa.table(host)
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            pacsv.write_csv(table, out)
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ms = float(np.median(ts))
+        name = f"pyarrow write_csv (not the reference), {os.cpu_count()} cores"
+        rows_out.append({"case": name, "config": "csv-write", "kernel": "host", "ms": ms, "rows": rows, "text_bytes": os.path.getsize(out)})
+        print(f"{name:44s} {ms:9.2f} ms  {os.path.getsize(out) / ms / 1e6:7.2f} GB/s of its text", flush=True)
+        for c in cols.values():
+            c.free()
 
 
 def window_parts(recs, value_calls):
@@ -286,8 +343,16 @@ def main():
     ap.add_argument("--window", action="store_true", help="run only the window-function rows")
     ap.add_argument("--math", action="store_true", help="run only the float-function rows (unary, atan2/hypot/log, fused)")
     ap.add_argument("--stats", action="store_true", help="run only the statistical-aggregate rows (moments, group variance, count_distinct)")
+    ap.add_argument("--csv-write", action="store_true", help="run only the CSV writer rows")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.csv_write:
+        rows_out = []
+        csv_write_bench(ctx, args.csv_rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"results": rows_out}, f, indent=1)
+        return
     if args.window:
         rows_out = []
         window_bench(ctx, args.rows, [4_000_000] * (args.rows // 4_000_000), rows_out)

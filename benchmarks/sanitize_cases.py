@@ -98,6 +98,23 @@ with tempfile.TemporaryDirectory() as td:
     with rdf.CsvFile(path, batch_size=7, schema=[rdf.U16, -1, rdf.F32, 10, rdf.F32]) as f:
         for c in f.read().values():
             c.download()
+    # CSV writer: measure, scan and emit over ragged sliced chunks with an empty one; one nullable column (""); rows too long for the
+    # emit window (direct stores)
+    def wcol(dtype, scale=1.0):
+        out = []
+        for k, n in enumerate(lens):
+            v = (rng.uniform(-1, 1, n + 9) * scale).astype(rdf.NP_DTYPES[dtype])
+            a = P.from_numpy(v, rng.random(n + 9) > 0.2)
+            a.null_count = -1
+            out.append(a.slice(3 + k, n))
+        return rdf.Column.upload(out)
+    bits = [rdf.BooleanArray.from_numpy(rng.random(n + 5) > 0.5).slice(5, n) for n in lens]
+    for b in bits:
+        b.null_count = 0
+    rdf.write_csv(os.path.join(td, "w.csv"), {"d": wcol(rdf.F64), "f": wcol(rdf.F32), "i": wcol(rdf.I16, 3e4), "b": rdf.Column.upload(bits)},
+                  delimiter="|")
+    rdf.write_csv(os.path.join(td, "w1.csv"), {"d": wcol(rdf.F64)})
+    rdf.write_csv(os.path.join(td, "w2.csv"), {f"t{j}": wcol(rdf.F64, 1e-300) for j in range(8)})
 # round 2: the fleet code path on one GPU, and a single-rank communicator (pack -> combine -> unpack on the stream)
 fleet = rdf.Context.multi(1)
 fa = [P.from_numpy(rng.integers(-100, 100, n).astype(np.int64), rng.random(n) > 0.3) for n in (1000, 0, 77)]

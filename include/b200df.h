@@ -528,6 +528,46 @@ int  bdf_csv_read(bdf_ctx* ctx, const bdf_csv* file, int32_t n_cols, const int32
 int  bdf_csv_stats(const bdf_csv* file, int64_t* n_fields, int64_t* exact_fields, double* upload_ms);
 void bdf_csv_close(bdf_ctx* ctx, bdf_csv* file);   /* the context that opened it */
 
+/* ---- CSV files straight from the device (DataFrame::to_csv, src/dataframe.rs:527-543; Evaluate::write(Csv(path, options)),
+ * src/evaluation.rs:343) ------------------------------------------------------------------------------------------------------------
+ * The reference writes with arrow-rs's csv::Writer over the csv crate.  Neither is restated from source: the rules below are RECALLED,
+ * parity unpinned (the reference's own tests only check that the write succeeds).
+ * Layout.  A header record with the column names unless has_header = 0, then one record per row in row order (chunk order, then
+ *   row); fields separated by the delimiter; every record ends with "\n" (the csv crate's default terminator), the last one too.  A
+ *   frame without rows is the header alone (an empty file without one).
+ * NULL.  An empty field.  A record of exactly one field that is empty (a one-column frame, a NULL row) is written "" as the csv crate
+ *   does -- and as the round trip needs: the reader skips blank lines.
+ * Values (Rust's ToString / Display of the native value):
+ *   integers (the 8 types)  plain decimal, '-' for negatives (-9223372036854775808, 18446744073709551615);
+ *   Boolean                 true / false;
+ *   Float32 / Float64       the SHORTEST digit string that reads back to the same value in that type (Float32 as an f32, never via
+ *                           f64), the one closest to the exact value when several do; written positionally, never with an exponent:
+ *                           1 (not 1.0), 0.1, 100000000000000000000 for 1e20, 0.0000001 for 1e-7, 340282350000000000000000000000000000000
+ *                           for f32::MAX; the longest field is 327 bytes (the negative smallest f64 subnormal).  NaN whatever its sign
+ *                           or payload, inf, -inf.  -0.0 is written -0: a decision (Rust before 1.53 printed 0), so that the value
+ *                           survives a round trip.  Later arrow versions format floats with lexical_core instead (1.0, exponent
+ *                           forms); which form the reference's pinned branch used is not known.
+ * Header names are quoted as the csv crate's QuoteStyle::Necessary does: a name containing the delimiter, '"', '\r' or '\n' (or the
+ *   only, empty, name) is put in quotes with every '"' doubled.  Values never need quotes: the delimiter may not occur in them.
+ * Options.  options == NULL: a header and ','.  The reference's plan carries CsvWriteOptions { has_headers, delimiter }
+ *   (src/expression.rs:380-384) but Evaluate::write ignores them; here they are honoured (a departure).  Allowed delimiters are bytes
+ *   that cannot occur in a formatted value: not NUL, a digit, '-', '.', '"', '\r', '\n' or a letter of NaN / inf / true / false
+ *   (N a i n f t r u e l s); any other -> BDF_INVALID.
+ * Types.  The ten numeric types and Boolean.  A frame with a Utf8 column is written on the CPU (arrow's writer), as for reading.
+ * Reading it back.  With Display an all-integral Float64 column (1, 2) is inferred as Int64 by the reader (the reference behaves the
+ *   same); exact round trips need an explicit schema.  With one, every value reads back bit for bit (NaN as a NaN: Display drops its
+ *   sign and payload).
+ * Input.  As bdf_ipc_write: chunk b of every column has the same length; any other chunk structure -> BDF_LENGTH_MISMATCH.  Any number
+ *   of columns.
+ * Memory.  The rows go in blocks whose text surely fits a device buffer: two 64 MiB text buffers, the byte offsets of up to 2^21 rows
+ *   (16 MiB) and 32 B per (chunk, column) of the column table in HBM; the context's pinned staging slots (6 x 8 MiB, shared with
+ *   uploads) carry the text to the file, written with pwrite by the staging threads.  Neither grows with the file.
+ * Errors (nothing leaks): a null pointer, n_cols <= 0 or a refused delimiter -> BDF_INVALID; a path that cannot be created or written
+ *   -> BDF_INVALID with the OS error text (the file is then incomplete); a multi-GPU context -> BDF_UNSUPPORTED (as the reader). */
+typedef struct { int32_t has_header; uint8_t delimiter; } bdf_csv_write_options;
+int  bdf_csv_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
+                   const bdf_csv_write_options* options /* NULL: a header and ',' */);
+
 /* ---- measurement support ------------------------------------------------------------------------ */
 /* Per-launch CUDA-event timing on the library's compute stream (the stream the kernels run on). */
 typedef struct {
@@ -537,7 +577,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

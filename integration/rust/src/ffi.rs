@@ -32,6 +32,9 @@ pub const BDF_PARSE: i32 = 9;   // -> ArrowError::ParseError(last_error())
 pub const BDF_UTF8: i32 = 11;   // CSV schema entry: a string column the device skips
 #[repr(C)]
 pub struct BdfCsvOptions { pub has_header: i32, pub delimiter: u8, pub max_records: i64 /* <0: all */, pub batch_size: i64 }
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct BdfCsvWriteOptions { pub has_header: i32, pub delimiter: u8 }
 
 #[repr(C)]
 pub struct BdfExprNode { pub op: i32, pub a: i32, pub b: i32 }   // op: bdf_binop, or BDF_EXPR_UNARY + bdf_unop
@@ -184,6 +187,9 @@ extern "C" {
     pub fn bdf_csv_read(ctx: *mut BdfCtx, file: *const BdfCsv, n_cols: i32, cols: *const i32, out: *mut *mut BdfCol) -> c_int;
     pub fn bdf_csv_stats(file: *const BdfCsv, n_fields: *mut i64, exact_fields: *mut i64, upload_ms: *mut f64) -> c_int;
     pub fn bdf_csv_close(ctx: *mut BdfCtx, file: *mut BdfCsv);
+    // CSV files straight from the device (DataFrame::to_csv): chunk b of every column = RecordBatch b; options NULL: a header and ','
+    pub fn bdf_csv_write(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol,
+                         options: *const BdfCsvWriteOptions) -> c_int;
     // Arrow IPC files (DataFrame::from_arrow / to_arrow)
     pub fn bdf_ipc_open(path: *const c_char, out: *mut *mut BdfIpc) -> c_int;
     pub fn bdf_ipc_close(file: *mut BdfIpc);

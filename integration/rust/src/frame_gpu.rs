@@ -232,6 +232,19 @@ pub fn from_csv_device(path: &str, schema: Option<&[i32]>) -> Result<DeviceColum
     res
 }
 
+/// `DataFrame::to_csv(path)` / `Evaluate::write(Csv(path, options))` on the device: every column of the frame is formatted on the GPU
+/// (floats in their shortest round-trip digits, as Display prints them) and streamed to the file.  `options`: `CsvWriteOptions
+/// { has_headers, delimiter }`, which the reference carries but ignores; None is a header and ','.
+pub fn to_csv_device(frame: &DeviceColumns, path: &str, options: Option<(bool, u8)>) -> Result<(), String> {
+    let c_path = CString::new(path).map_err(|e| e.to_string())?;
+    let names: Vec<CString> = frame.names.iter().map(|n| CString::new(n.as_str())).collect::<Result<_, _>>().map_err(|e| e.to_string())?;
+    let name_ptrs: Vec<*const c_char> = names.iter().map(|n| n.as_ptr()).collect();
+    let cols: Vec<*const BdfCol> = frame.cols.iter().map(|c| *c as *const BdfCol).collect();
+    let opts = options.map(|(h, d)| BdfCsvWriteOptions { has_header: h as i32, delimiter: d });
+    let p = opts.as_ref().map_or(std::ptr::null(), |o| o as *const BdfCsvWriteOptions);
+    check(unsafe { bdf_csv_write(dev(), c_path.as_ptr(), cols.len() as i32, name_ptrs.as_ptr(), cols.as_ptr(), p) })
+}
+
 /// A run of Float64 Calculations whose intermediates are not kept (config 2: h = sin(((a+b)*c)/d)) as one pass.
 /// `inputs` are column indices; node k writes slot inputs.len() + k (see include/b200df.h, bdf_eval_expr_dev).
 pub fn fused_chain(frame: &DeviceColumns, inputs: &[usize], nodes: &[BdfExprNode]) -> Result<*mut BdfCol, String> {

@@ -21,9 +21,9 @@ SUM, MIN, MAX, COUNT = range(4)
 OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID, PARSE = range(10)
 ASYNC = 1
 (K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW,
- K_MOMENTS) = range(16)
+ K_MOMENTS, K_CSV_WRITE) = range(17)
 KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
-                "window", "moments"]
+                "window", "moments", "csv_write"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -99,6 +99,10 @@ class WindowCall(C.Structure):
 
 class CsvOptions(C.Structure):
     _fields_ = [("has_header", C.c_int32), ("delimiter", C.c_uint8), ("max_records", C.c_int64), ("batch_size", C.c_int64)]
+
+
+class CsvWriteOptions(C.Structure):
+    _fields_ = [("has_header", C.c_int32), ("delimiter", C.c_uint8)]
 
 
 class LaunchRecord(C.Structure):
@@ -236,6 +240,7 @@ def lib() -> C.CDLL:
         "bdf_csv_read": ([vp, vp, i32, P(i32), P(vp)], C.c_int),
         "bdf_csv_stats": ([vp, P(i64), P(i64), P(C.c_double)], C.c_int),
         "bdf_csv_close": ([vp, vp], None),
+        "bdf_csv_write": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(CsvWriteOptions)], C.c_int),
         "bdf_generate": ([vp, C.c_int, C.c_int, C.c_double, C.c_double, u64, u64, i64, P(i64), i64, C.c_uint32, P(vp)],
                          C.c_int),
     }
@@ -261,7 +266,7 @@ EXPORTED_SYMBOLS = [
     "bdf_launch_count", "bdf_timer_start", "bdf_timer_stop", "bdf_flush_l2", "bdf_generate",
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",
     "bdf_ipc_write_host", "bdf_ipc_write",
-    "bdf_csv_open", "bdf_csv_describe", "bdf_csv_column", "bdf_csv_read", "bdf_csv_stats", "bdf_csv_close",
+    "bdf_csv_open", "bdf_csv_describe", "bdf_csv_column", "bdf_csv_read", "bdf_csv_stats", "bdf_csv_close", "bdf_csv_write",
     "bdf_moments", "bdf_moments_dev", "bdf_moments_stat", "bdf_moments_merge", "bdf_distinct", "bdf_distinct_dev",
 ]
 

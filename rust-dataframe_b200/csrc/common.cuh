@@ -223,6 +223,13 @@ struct GenDesc {
     void* out; uint32_t* vout;
     int64_t len; int64_t tile0; int64_t row0;
 };
+// CSV writer (k_csv_write.cu): one per (chunk, column), chunk-major.
+struct CsvwDesc {
+    const void* values; const uint32_t* validity;
+    int32_t bit_off;       // validity bit offset
+    int32_t val_bit_off;   // Boolean values bit offset
+    int32_t dtype; int32_t pad;
+};
 
 // Partial / final aggregate as the kernels produce it.
 struct AggDev {

@@ -7,6 +7,7 @@
 // already on its way back.  When all inputs are already resident an operator is ONE batched launch over
 // every chunk of the column.
 #include <algorithm>
+#include <atomic>
 #include <cerrno>
 #include <chrono>
 #include <cstdarg>
@@ -179,35 +180,36 @@ class CopyPool {
     void copy(char* dst, const char* src, size_t n, bool populate = false) {
         constexpr size_t kJob = (size_t)512 << 10;
         if (th_.empty() || n < 2 * kJob) { job_copy(dst, src, n, populate); return; }
+        run((n + kJob - 1) / kJob, [=](size_t j) { job_copy(dst + j * kJob, src + j * kJob, std::min(kJob, n - j * kJob), populate); });
+    }
+    // fn(0) .. fn(jobs - 1) on the workers and the calling thread; returns when all have finished.
+    void run(size_t jobs, const std::function<void(size_t)>& fn) {
         std::unique_lock<std::mutex> lk(m_);
-        populate_ = populate;
-        dst_ = dst; src_ = src; n_ = n; next_ = 0; jobs_ = (n + kJob - 1) / kJob; done_ = 0;
+        fn_ = &fn; next_ = 0; jobs_ = jobs; done_ = 0;
         lk.unlock();
         cv_work_.notify_all();
         lk.lock();
         while (next_ < jobs_) {   // the caller works too
             const size_t j = next_++;
             lk.unlock();
-            job_copy(dst + j * kJob, src + j * kJob, std::min(kJob, n - j * kJob), populate);
+            fn(j);
             lk.lock();
             done_++;
         }
         cv_done_.wait(lk, [this] { return done_ == jobs_; });
-        jobs_ = 0; next_ = 0; done_ = 0;
+        jobs_ = 0; next_ = 0; done_ = 0; fn_ = nullptr;
     }
 
   private:
     void work() {
-        constexpr size_t kJob = (size_t)512 << 10;
         std::unique_lock<std::mutex> lk(m_);
         for (;;) {
             cv_work_.wait(lk, [this] { return stop_ || next_ < jobs_; });
             if (stop_) return;
             const size_t j = next_++;
-            char* d = dst_; const char* s = src_; const size_t n = n_;
-            const bool pop = populate_;
+            const std::function<void(size_t)>* fn = fn_;
             lk.unlock();
-            job_copy(d + j * kJob, s + j * kJob, std::min(kJob, n - j * kJob), pop);
+            (*fn)(j);
             lk.lock();
             if (++done_ == jobs_) cv_done_.notify_all();
         }
@@ -215,9 +217,9 @@ class CopyPool {
     std::mutex m_;
     std::condition_variable cv_work_, cv_done_;
     std::vector<std::thread> th_;
-    char* dst_ = nullptr; const char* src_ = nullptr;
-    size_t n_ = 0, next_ = 0, jobs_ = 0, done_ = 0;
-    bool stop_ = false, populate_ = false;
+    const std::function<void(size_t)>* fn_ = nullptr;
+    size_t next_ = 0, jobs_ = 0, done_ = 0;
+    bool stop_ = false;
 };
 
 struct bdf_ctx {
@@ -3037,6 +3039,201 @@ static int csv_read(bdf_ctx* c, const bdf_csv* f, int n_cols, const int32_t* col
 }
 
 // ---------------------------------------------------------------------------------------------------
+// CSV writer (k_csv_write.cu; DataFrame::to_csv, src/dataframe.rs:527-543).  The rows go in blocks whose text surely fits one of two
+// fixed device buffers: while block k is measured, scanned and formatted, block k-1 crosses PCIe through the pinned staging slots
+// and the CopyPool threads pwrite every slot at its offset in the file (known from the scan), so neither HBM nor pinned memory
+// grows with the file.
+
+namespace bdf {
+int csvw_tile();
+cudaError_t launch_csvw_measure(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows,
+                                unsigned long long* lens, unsigned long long* block_sums, cudaStream_t s);
+cudaError_t launch_csvw_emit(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows, int delim,
+                             const unsigned long long* offs, char* out, cudaStream_t s);
+}  // namespace bdf
+
+static constexpr size_t kCsvwText = (size_t)64 << 20;        // bytes of each of the two device text buffers
+static constexpr int64_t kCsvwMaxRows = (int64_t)1 << 21;    // rows per block at most (their lengths and offsets: 16 MiB)
+// The longest field of each dtype (BDF_I8 .. BDF_F64, BDF_BOOL).  A positional float whose last digit sits at 10^e (e < 0) is 2 - e
+// bytes plus its sign, and the shortest digits never need e below the rounding interval's width (2^-1074 > 10^-324, 2^-149 > 10^-45):
+// at most 327 bytes for Float64 (-0.000...0005, the negative smallest subnormal) and 48 for Float32; above 1, 310 and 40.
+static const int kCsvwMaxField[11] = {4, 6, 11, 20, 3, 5, 10, 20, 48, 327, 5};
+
+// The delimiter must not occur in any value's text, so that no value needs quotes.
+static bool csvw_delim_ok(int d) {
+    return !((d >= '0' && d <= '9') || strchr("-.\"\r\nNaintruefls", d) || d == 0);
+}
+
+// The header record, quoted as the csv crate's QuoteStyle::Necessary quotes.
+static std::string csvw_header(int n_cols, const char* const* names, char delim) {
+    std::string h;
+    for (int j = 0; j < n_cols; j++) {
+        if (j) h += delim;
+        const char* s = names[j];
+        const bool quote = (n_cols == 1 && !*s) || strpbrk(s, "\"\r\n") || strchr(s, delim);
+        if (!quote) { h += s; continue; }
+        h += '"';
+        for (; *s; s++) { if (*s == '"') h += '"'; h += *s; }
+        h += '"';
+    }
+    return h + '\n';
+}
+
+static int pwrite_all(int fd, const char* p, size_t n, off_t off) {   // 0 or an errno
+    while (n) {
+        const ssize_t w = pwrite(fd, p, n, off);
+        if (w < 0) { if (errno == EINTR) continue; return errno; }
+        if (w == 0) return EIO;
+        p += w; n -= (size_t)w; off += w;
+    }
+    return 0;
+}
+
+static int csv_write(bdf_ctx* c, const char* path, int n_cols, const char* const* names, const bdf_col* const* cols, const bdf_csv_write_options* opt) {
+    if (!path || !names || !cols) return fail(BDF_INVALID, "null argument");
+    if (n_cols <= 0) return fail(BDF_INVALID, "no columns to write");
+    const int delim = opt ? opt->delimiter : ',';
+    if (!csvw_delim_ok(delim)) return fail(BDF_INVALID, "delimiter 0x%02x can occur in a formatted value", delim);
+    int64_t n_chunks = -1, max_row = n_cols + 2;
+    for (int j = 0; j < n_cols; j++) {
+        const bdf_col* col = cols[j];
+        if (!col || !names[j]) return fail(BDF_INVALID, "null column or name");
+        if (!col->fparts.empty()) return fail(BDF_INVALID, "a column of a multi-GPU context was passed to a one-GPU context");
+        if (!((col->dtype >= 0 && col->dtype < BDF_NTYPES) || col->dtype == kBool)) return fail(BDF_UNSUPPORTED, "column '%s': dtype %d", names[j], col->dtype);
+        const int64_t nc = (int64_t)col->chunks.size();
+        if (n_chunks < 0) n_chunks = nc;
+        if (nc != n_chunks)
+            return fail(BDF_LENGTH_MISMATCH, "columns have different numbers of chunks (%lld, %lld)", (long long)nc, (long long)n_chunks);
+        for (int64_t b = 0; b < nc; b++)
+            if (col->chunks[b].len != cols[0]->chunks[b].len)
+                return fail(BDF_LENGTH_MISMATCH, "chunk %lld: column '%s' has %lld rows, column '%s' has %lld", (long long)b, names[j],
+                            (long long)col->chunks[b].len, names[0], (long long)cols[0]->chunks[b].len);
+        max_row += kCsvwMaxField[col->dtype];
+    }
+    std::vector<long long> starts((size_t)n_chunks + 1, 0);
+    std::vector<CsvwDesc> descs((size_t)n_chunks * n_cols);
+    for (int64_t b = 0; b < n_chunks; b++) {
+        starts[b + 1] = starts[b] + cols[0]->chunks[b].len;
+        for (int j = 0; j < n_cols; j++) {
+            const DevChunk& ch = cols[j]->chunks[b];
+            descs[b * n_cols + j] = CsvwDesc{ch.values, ch.validity, ch.bit_off, ch.val_bit_off, cols[j]->dtype, 0};
+        }
+    }
+    const int64_t rows = starts[n_chunks];
+    const size_t text_cap = std::max<size_t>(kCsvwText, (size_t)max_row);
+    const int64_t block_rows = std::max<int64_t>(1, std::min<int64_t>(kCsvwMaxRows, (int64_t)(text_cap / (size_t)max_row)));
+
+    const int fd = open(path, O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0644);
+    if (fd < 0) return fail(BDF_INVALID, "cannot create %s: %s", path, strerror(errno));
+    struct FdGuard { int fd; ~FdGuard() { if (fd >= 0) close(fd); } } fdg{fd};
+    off_t file_off = 0;
+    if (!opt || opt->has_header) {
+        const std::string h = csvw_header(n_cols, names, (char)delim);
+        const int we = pwrite_all(fd, h.data(), h.size(), 0);
+        if (we) return fail(BDF_INVALID, "writing %s failed: %s", path, strerror(we));
+        file_off = (off_t)h.size();
+    }
+    auto finish = [&]() {
+        const int fdv = fdg.fd;
+        fdg.fd = -1;
+        if (close(fdv) != 0) return fail(BDF_INVALID, "closing %s failed: %s", path, strerror(errno));
+        return (int)BDF_OK;
+    };
+    if (rows == 0) return finish();
+
+    for (int j = 0; j < n_cols; j++) wait_groups(c->s_compute, cols[j], 0, n_chunks);
+    TRY(ensure_stage(c));
+    Scratch<CsvwDesc> d_desc;
+    Scratch<long long> d_starts;
+    Scratch<char> text[2];
+    Scratch<unsigned long long> lens, sums;
+    const int64_t max_tiles = (block_rows + csvw_tile() - 1) / csvw_tile();
+    cudaError_t e = d_desc.alloc(c, descs.size() * sizeof(CsvwDesc));
+    if (e == cudaSuccess) e = d_starts.alloc(c, starts.size() * sizeof(long long));
+    if (e == cudaSuccess) e = text[0].alloc(c, text_cap);
+    if (e == cudaSuccess) e = text[1].alloc(c, text_cap);
+    if (e == cudaSuccess) e = lens.alloc(c, (size_t)(block_rows + 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = sums.alloc(c, (size_t)max_tiles * sizeof(unsigned long long));
+    // pageable sources: the copies have read them when they return
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_desc, descs.data(), descs.size() * sizeof(CsvwDesc), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_starts, starts.data(), starts.size() * sizeof(long long), cudaMemcpyHostToDevice, c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "CSV write setup");
+    struct Pinned { unsigned long long* p = nullptr; ~Pinned() { if (p) cudaFreeHost(p); } } tot;
+    struct Events { bdf_ctx* c; cudaEvent_t ev[4] = {}; ~Events() { for (auto x : ev) ev_put(c, x); } } evs{c};
+    CK(cudaHostAlloc((void**)&tot.p, 2 * sizeof(unsigned long long), cudaHostAllocDefault));
+    for (auto& x : evs.ev) CK(ev_get(c, &x));
+    cudaEvent_t* ev_emit = evs.ev;       // block k's text is complete in text[k & 1]
+    cudaEvent_t* ev_d2h = evs.ev + 2;    // block k's text has left text[k & 1]
+    // Declared after the buffers, so it runs first on every exit: no copy may still read a text buffer when it is freed.
+    struct DrainD2H { cudaStream_t s; ~DrainD2H() { cudaStreamSynchronize(s); } } drain_guard{c->s_d2h};
+
+    const int64_t n_blocks = (rows + block_rows - 1) / block_rows;
+    size_t emit_rec[2] = {0, 0};
+    auto enqueue = [&](int64_t k) -> int {
+        const int b = (int)(k & 1);
+        const int64_t row0 = k * block_rows, n = std::min(block_rows, rows - row0);
+        cudaError_t e2 = k >= 2 ? cudaStreamWaitEvent(c->s_compute, ev_d2h[b], 0) : cudaSuccess;
+        if (e2 == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_CSV_WRITE, BDF_U64, n, n * (8 + 16));   // lengths written, then read and written by the scan
+            c->launches += 2;                                                // the scan's two kernels
+            e2 = launch_csvw_measure(d_desc, d_starts, n_cols, (int)n_chunks, row0, n, lens, sums, c->s_compute);
+            if (e2 == cudaSuccess) e2 = launch_join_scan(lens, n, sums, c->s_compute);
+        }
+        if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(tot.p + b, lens + n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->s_compute);
+        if (e2 == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_CSV_WRITE, BDF_U8, n, n * 8);   // + the text, once the block's size is known
+            e2 = launch_csvw_emit(d_desc, d_starts, n_cols, (int)n_chunks, row0, n, delim, lens, text[b], c->s_compute);
+        }
+        if (c->profiling) emit_rec[b] = c->prof.size() - 1;
+        if (e2 == cudaSuccess) e2 = cudaEventRecord(ev_emit[b], c->s_compute);
+        return e2 == cudaSuccess ? BDF_OK : fail_cuda(e2, "CSV write kernels");
+    };
+    struct Pending { bdf_ctx::StageSlot* sl; off_t off; size_t n; };
+    std::deque<Pending> pending;
+    auto retire = [&]() -> int {
+        const Pending p = pending.front();
+        pending.pop_front();
+        CK(cudaEventSynchronize(p.sl->ev));
+        p.sl->busy = false;
+        constexpr size_t kJob = (size_t)512 << 10;
+        std::atomic<int> werr{0};
+        c->pool->run((p.n + kJob - 1) / kJob, [&](size_t j) {
+            const int we = pwrite_all(fd, p.sl->p + j * kJob, std::min(kJob, p.n - j * kJob), p.off + (off_t)(j * kJob));
+            if (we) werr = we;
+        });
+        if (werr) return fail(BDF_INVALID, "writing %s failed: %s", path, strerror(werr));
+        return BDF_OK;
+    };
+    auto drain = [&](int64_t k) -> int {
+        const int b = (int)(k & 1);
+        CK(cudaEventSynchronize(ev_emit[b]));
+        const size_t bytes = (size_t)tot.p[b];
+        if (c->profiling) c->prof[emit_rec[b]].rec.bytes += (int64_t)bytes;
+        CK(cudaStreamWaitEvent(c->s_d2h, ev_emit[b], 0));
+        for (size_t off = 0; off < bytes; off += kStageBytes) {
+            const size_t n = std::min(kStageBytes, bytes - off);
+            if ((int)pending.size() >= kStageSlots - 1) TRY(retire());
+            bdf_ctx::StageSlot& sl = c->stage[c->stage_next++ % kStageSlots];
+            if (sl.busy) CK(cudaEventSynchronize(sl.ev));   // an upload's slot
+            CK(cudaMemcpyAsync(sl.p, text[b] + off, n, cudaMemcpyDeviceToHost, c->s_d2h));
+            CK(cudaEventRecord(sl.ev, c->s_d2h));
+            sl.busy = true;
+            pending.push_back(Pending{&sl, file_off + (off_t)off, n});
+        }
+        CK(cudaEventRecord(ev_d2h[b], c->s_d2h));
+        file_off += (off_t)bytes;
+        return BDF_OK;
+    };
+    TRY(enqueue(0));
+    for (int64_t k = 0; k < n_blocks; k++) {
+        if (k + 1 < n_blocks) TRY(enqueue(k + 1));
+        TRY(drain(k));
+    }
+    while (!pending.empty()) TRY(retire());
+    return finish();
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Multi-GPU context (bdf_init_multi): ONE process, every GPU of the box.  The library owns the sharding that the
 // reference leaves to rayon (par_iter over chunks, src/functions/scalar.rs:28-31,99-102): the rows of a call are cut into
 // one contiguous range per GPU (cuts on 64-row boundaries inside a chunk, so a piece is a zero-copy Arrow slice whose
@@ -4351,6 +4548,13 @@ void bdf_csv_close(bdf_ctx* c, bdf_csv* f) {
     std::lock_guard<std::mutex> lock(c->mu);
     cudaSetDevice(c->device);
     csv_free(c, f);
+}
+
+int bdf_csv_write(bdf_ctx* c, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
+                  const bdf_csv_write_options* options) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the CSV writer writes from one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return csv_write(c, path, n_cols, names, cols, options);
 }
 
 int bdf_take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, bdf_col** out) {

@@ -1,4 +1,5 @@
-"""CSV files straight to the GPU: DataFrame::from_csv (src/dataframe.rs:349-389) and LazyFrame::read(Csv) (src/evaluation.rs:328).
+"""CSV files straight to and from the GPU: DataFrame::from_csv (src/dataframe.rs:349-389), LazyFrame::read(Csv) (src/evaluation.rs:328)
+and DataFrame::to_csv (src/dataframe.rs:527-543).
 
 The library maps the file, uploads its bytes, tokenizes them with csv-core's record DFA run as a scan, checks the field counts,
 infers the schema and parses the requested columns on the device (csrc/k_csv.cu; the rules are in include/b200df.h):
@@ -6,11 +7,12 @@ infers the schema and parses the requested columns on the device (csrc/k_csv.cu;
     with CsvFile(path) as f:                 # arrow's defaults: header, ',', infer from every record, 1024 rows per batch
         f.schema                             # [(name, dtype or -1, nullable)]; Utf8 columns are -1 (not on the device path)
         cols = f.read(["lat", "lng"])        # -> {name: Column}, one chunk per RecordBatch
+    write_csv("out.csv", cols)               # a header, ',', floats in their shortest round-trip digits (csrc/k_csv_write.cu)
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional, Sequence, Union
+from typing import Dict, Mapping, Optional, Sequence, Union
 
 from . import _native as N
 
@@ -91,3 +93,19 @@ class CsvFile:
         outs = (C.c_void_p * max(k, 1))()
         N.raise_for_status(N.lib().bdf_csv_read(self.ctx.handle, self.handle, k, arr, outs))
         return {self.schema[i][0]: Column(self.ctx, C.c_void_p(outs[j])) for j, i in enumerate(idx)}
+
+
+def write_csv(path: str, columns: Mapping[str, "object"], has_header: bool = True, delimiter: str = ",") -> None:
+    """Device Columns (chunk b of every column has the same length) -> a CSV file, formatted on the device (bdf_csv_write; the rules
+    are in include/b200df.h).  ``delimiter`` may not be a byte that occurs in a value (a digit, '-', '.', quotes, line ends, letters
+    of NaN / inf / true / false)."""
+    d = delimiter.encode() if isinstance(delimiter, str) else bytes(delimiter)
+    if len(d) != 1:
+        raise ValueError("the delimiter is one byte")
+    names = list(columns)
+    k = len(names)
+    ctx = columns[names[0]].ctx if k else N.default_context()
+    cnames = (C.c_char_p * max(k, 1))(*[s.encode() for s in names])
+    handles = (C.c_void_p * max(k, 1))(*[columns[s].handle for s in names])
+    opts = N.CsvWriteOptions(1 if has_header else 0, d[0])
+    N.raise_for_status(N.lib().bdf_csv_write(ctx.handle, str(path).encode(), k, cnames, handles, C.byref(opts)))

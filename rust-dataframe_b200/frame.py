@@ -37,7 +37,7 @@ import numpy as np
 from . import _native as N
 from .arrays import F32, F64, I8, I64, U8, U32, U64, PrimitiveArray, is_float
 from .functions import Column, _expr_nodes, eval_expr, sort_indices, window as _window
-from .csv_reader import CsvFile
+from .csv_reader import CsvFile, write_csv
 from .ipc import BOOL, IpcFile, write_ipc
 
 ARITH = {"add": N.ADD, "subtract": N.SUB, "multiply": N.MUL, "divide": N.DIV}
@@ -416,6 +416,10 @@ class DeviceFrame:
 
     def to_arrow(self, path: str) -> None:
         write_ipc(path, dict(self.columns))
+
+    def to_csv(self, path: str, has_header: bool = True, delimiter: str = ",") -> None:
+        """DataFrame::to_csv: the frame's text is formatted on the device and streamed to the file (write_csv)."""
+        write_csv(path, self.columns, has_header=has_header, delimiter=delimiter)
 
     def to_host(self) -> Dict[str, list]:
         return {n: c.download() for n, c in self.columns.items()}
