@@ -9,6 +9,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --math [--rows 100000000]                        # only the float-function rows
     python benchmarks/kernels_bench.py --stats [--rows 100000000]                       # only the statistical-aggregate rows
     python benchmarks/kernels_bench.py --csv-write [--csv-rows 50000000]                # the CSV writer rows (the reader's table written back)
+    python benchmarks/kernels_bench.py --lists [--rows 100000000]                       # the list-function rows (ArrayFunctions)
 """
 from __future__ import annotations
 
@@ -334,6 +335,98 @@ def stats_bench(ctx, lens, report, rows_out):
         col.free()
 
 
+def _stream_read_rate(rows):
+    """The read-only HBM rate of benchmarks/tune_stream.cu (best read-only sum), built into a temporary directory and run here."""
+    import re
+    import subprocess
+
+    src = os.path.join(ROOT, "benchmarks", "tune_stream.cu")
+    with tempfile.TemporaryDirectory() as td:
+        exe = os.path.join(td, "tune_stream")
+        nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+        subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", src, "-o", exe], check=True, capture_output=True)
+        out = subprocess.run([exe, str(rows)], check=True, capture_output=True, text=True).stdout
+    m = re.search(r"CEILING read-only ([0-9.]+) GB/s", out)
+    return float(m.group(1))
+
+
+def _card():
+    import subprocess
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+    return q.strip().splitlines()[0] if q.strip() else "unknown"
+
+
+def _timed_calls(ctx, fn, reps=3):
+    """Median over `reps` calls (after one warm-up) of the sum of the library's per-launch CUDA-event records of one call."""
+    out = fn()
+    del out
+    ctx.synchronize()
+    ctx.profile_read()
+    sums = []
+    for _ in range(reps):
+        ctx.profile_enable(True)
+        out = fn()
+        ctx.profile_enable(False)
+        sums.append(sum(r["ms"] for r in ctx.profile_read()))
+        last = out
+        del out
+    return float(np.median(sums)), last
+
+
+def lists_bench(ctx, rows, rows_out):
+    """ArrayFunctions over rows elements of Int64 and Float64 in 25 chunks at mean list lengths 4, 32 and 1000 (lengths uniform in
+    [1, 2 * mean - 1]: no empty list, so max / min are defined), plus one hot list of rows / 10 elements among about rows one-element lists.
+    Algorithmic bytes: offsets and elements read once, plus what is written."""
+    card = _card()
+    stream = _stream_read_rate(rows)
+    print(f"card: {card}; tune_stream read-only rate {stream:.1f} GB/s", flush=True)
+    rows_out.append({"case": "tune_stream read-only", "GBs": stream, "card": card})
+    rng = np.random.default_rng(20261015)
+    n_chunks = 25
+    per = rows // n_chunks
+    for dt in (rdf.I64, rdf.F64):
+        npdt = rdf.NP_DTYPES[dt]
+        w = npdt.itemsize
+        shapes = [("mean 4", 4), ("mean 32", 32), ("mean 1000", 1000), ("hot list", 0)]
+        for label, mean in shapes:
+            chunks = []
+            for k in range(n_chunks):
+                if mean:
+                    lens = rng.integers(1, 2 * mean, max(per // mean, 1))
+                else:   # chunk 0 is one list of rows / 10 elements, every other element is a one-element list
+                    lens = np.ones(per, dtype=np.int64) if k else np.array([rows // 10], dtype=np.int64)
+                off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
+                vals = rng.integers(0, 1 << 20, int(off[-1])).astype(npdt)
+                chunks.append(rdf.ListArray(dt, off, None, 0, len(lens), 0, rdf.PrimitiveArray.from_numpy(vals)))
+            c = rdf.ListColumn.upload(chunks, ctx)
+            E = sum(len(ch.values) for ch in chunks)
+            N_ = sum(len(ch) for ch in chunks)
+            del chunks
+            off_b = 4 * (N_ + n_chunks)
+            cases = [("array_contains", lambda: c.array_contains(5), lambda o: E * w + off_b + N_ / 8, True),
+                     ("array_position", lambda: c.array_position(5), lambda o: E * w + off_b + 4 * N_, True),
+                     ("array_max", lambda: c.array_max(), lambda o: E * w + off_b + N_ * w + N_ / 8, True),
+                     ("array_min", lambda: c.array_min(), lambda o: E * w + off_b + N_ * w + N_ / 8, True),
+                     ("size", lambda: c.size(), lambda o: off_b + 4 * N_, True),
+                     ("array_sort (lexsort path)", lambda: c.array_sort(), lambda o: 2 * (E * w + off_b), False),
+                     ("array_distinct", lambda: c.array_distinct(), lambda o: E * w + off_b + len(o.values()) * w + 4 * (N_ + 1), False),
+                     ("array_remove", lambda: c.array_remove(5), lambda o: E * w + off_b + len(o.values()) * w + 4 * (N_ + 1), False),
+                     ("array_repeat(2)", lambda: c.array_repeat(2), lambda o: E * w + off_b + 2 * E * w + 4 * (N_ + 1), False),
+                     ("array_union(self)", lambda: c.array_union(c), lambda o: 2 * (E * w + off_b) + len(o.values()) * w + 4 * (N_ + 1), False),
+                     ("explode", lambda: c.explode(), lambda o: E * w + off_b + E * (w + 4), False)]
+            for name, fn, nbytes, single in cases:
+                ms, out = _timed_calls(ctx, fn)
+                b = nbytes(out)
+                gbs = b / ms / 1e6
+                rows_out.append({"case": f"{name} {rdf.DTYPE_NAMES[dt]} {label}", "ms": ms, "elements": E, "lists": N_, "bytes": b, "GBs": gbs,
+                                 "frac_of_stream_read": gbs / stream if single else None, "card": card})
+                frac = f"  {gbs / stream:5.3f} of read rate" if single else ""
+                print(f"{name:28s} {rdf.DTYPE_NAMES[dt]:8s} {label:10s} {ms:9.3f} ms {gbs:8.1f} GB/s{frac}", flush=True)
+                del out
+            c.free()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
@@ -344,8 +437,16 @@ def main():
     ap.add_argument("--math", action="store_true", help="run only the float-function rows (unary, atan2/hypot/log, fused)")
     ap.add_argument("--stats", action="store_true", help="run only the statistical-aggregate rows (moments, group variance, count_distinct)")
     ap.add_argument("--csv-write", action="store_true", help="run only the CSV writer rows")
+    ap.add_argument("--lists", action="store_true", help="run only the list-function rows (ArrayFunctions)")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.lists:
+        rows_out = []
+        lists_bench(ctx, args.rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"results": rows_out}, f, indent=1)
+        return
     if args.csv_write:
         rows_out = []
         csv_write_bench(ctx, args.csv_rows, rows_out)

@@ -115,6 +115,30 @@ with tempfile.TemporaryDirectory() as td:
                   delimiter="|")
     rdf.write_csv(os.path.join(td, "w1.csv"), {"d": wcol(rdf.F64)})
     rdf.write_csv(os.path.join(td, "w2.csv"), {f"t{j}": wcol(rdf.F64, 1e-300) for j in range(8)})
+# list functions: ragged list chunks (null lists spanning elements, empty lists, null elements, a sliced list array and a sliced child),
+# lists past the lane rounds of the search (the long-list work list and its grid-stride pass), every function once
+for dtype in (rdf.I8, rdf.U16, rdf.I64, rdf.F32, rdf.F64):
+    npdt = rdf.NP_DTYPES[dtype]
+    def lchunk(n, long_every=0):
+        lens = rng.integers(0, 9, n)
+        if long_every:
+            lens[::long_every] = 20000
+        off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32) + 3
+        m = int(off[-1]) + 5
+        child = P.from_numpy(rng.integers(0, 6, m).astype(npdt), rng.random(m) > 0.2).slice(2, m - 2)
+        child.null_count = -1
+        valid = rng.random(n + 2) > 0.1
+        return rdf.ListArray(dtype, np.concatenate([[0], off]).astype(np.int32), rdf.arrays.pack_validity(valid), 1, n, int((~valid[1:n + 1]).sum()), child)
+    la = rdf.ListColumn.upload([lchunk(n) for n in (0, 1, 33, 2049)] + [lchunk(300, 7)])
+    lb = rdf.ListColumn.upload([lchunk(n) for n in (0, 1, 33, 2049)] + [lchunk(300, 11)])
+    for col in (la.array_contains(3), la.array_position(3), la.size()):
+        col.download()
+    for res in (la.array_remove(3), la.array_sort(), la.array_distinct(), la.array_repeat(2), la.array_except(lb), la.array_intersect(lb), la.array_union(lb)):
+        res.download()
+    for col in la.explode():
+        col.download()
+    nonempty = rdf.ListColumn.upload([rdf.ListArray.from_pylist(dtype, [[1, None], [None], None, [k % 100 for k in range(70000)]])])
+    nonempty.array_max().download(); nonempty.array_min().download()
 # round 2: the fleet code path on one GPU, and a single-rank communicator (pack -> combine -> unpack on the stream)
 fleet = rdf.Context.multi(1)
 fa = [P.from_numpy(rng.integers(-100, 100, n).astype(np.int64), rng.random(n) > 0.3) for n in (1000, 0, 77)]

@@ -53,7 +53,7 @@ extern "C" {
 #pragma GCC visibility push(default) /* the library is built with -fvisibility=hidden; these are its exports */
 #endif
 
-#define BDF_ABI_VERSION 2
+#define BDF_ABI_VERSION 3
 
 /* Arrow primitive types, in arrow::datatypes::DataType order. */
 typedef enum {
@@ -568,6 +568,92 @@ typedef struct { int32_t has_header; uint8_t delimiter; } bdf_csv_write_options;
 int  bdf_csv_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
                    const bdf_csv_write_options* options /* NULL: a header and ',' */);
 
+/* ---- list columns and ArrayFunctions (src/functions/array.rs; size / explode: ScalarFunctions stubs, scalar.rs:237,414) ----------
+ * Layout.  Arrow List<T> with 32-bit offsets, T one of the ten numeric types, one chunk per RecordBatch.  A bdf_list holds per chunk the
+ *   list validity, len + 1 Int32 offsets rebased to start at 0, and the elements as an ordinary bdf_col whose chunk i holds exactly the
+ *   elements [offsets[0], offsets[len]) of list chunk i (bdf_list_values lends it out: every column operator works on the elements).
+ *   LargeList, nested lists, FixedSizeList and Boolean / Utf8 children are not on the device path (BDF_UNSUPPORTED).
+ * bdf_list_view.  The list's offset applies to offsets and validity; `values` is the child array, whose own offset and validity apply
+ *   (offsets index the child from values.offset).  Only the elements the lists reference cross PCIe.  A null list whose offsets span
+ *   elements is uploaded as it is; every function below ignores those elements.
+ * Limits.  Elements per chunk below 2^31 (Int32 offsets), elements per call below 2^32 (the sort's UInt32 row numbers): beyond either,
+ *   BDF_UNSUPPORTED.  A list-returning function gives ONE chunk (as take and sort do), so its elements must also stay below 2^31.
+ *   A multi-GPU context -> BDF_UNSUPPORTED for every list entry (as sort / take).
+ * Rules shared by every function:
+ *   Equality is the key equality of sort, group-by, join and count_distinct: integers exact, all NaNs one value, -0.0 == 0.0 (a
+ *     deliberate departure from the reference's PartialEq, for NaN only).
+ *   The search value is T::Native bits in the low bytes of a uint64_t (as bdf_window_call.default_bits).
+ *   A null list gives a valid EMPTY list in every list-returning function (the reference's ListBuilder::append(true) on a.is_null(i)).
+ *   Deterministic: the same bits on every run, no atomics on values.
+ * Per function ("pinned" = one of the reference's six array tests covers it; "unpinned" = follows Spark 2.4 where the reference is
+ *   silent or its body is private and broken):
+ *   CONTAINS (array.rs:15)   Boolean, chunks of the input.  Null list -> NULL; otherwise true iff a VALID element equals v (a null slot
+ *                            never matches, so a valid list never gives NULL).  Pinned.
+ *   POSITION (:233)          Int32, chunks of the input, never NULL: the 1-based index of the first valid element equal to v (null slots
+ *                            count as positions), 0 without one; a null list -> 0 (as the reference appends).  Pinned.
+ *   MAX / MIN (:182, :206)   T, chunks of the input.  Null elements are skipped; a list whose elements are all null -> NULL; a null list
+ *                            -> NULL; a valid EMPTY list -> BDF_WOULD_PANIC (.max().unwrap()).  Floats (an extension) use group-by's
+ *                            float rule: IEEE totalOrder keys, -0.0 < +0.0, NaN greatest, returned as the positive quiet NaN.
+ *   SIZE (scalar.rs:414)     Int32, chunks of the input: the slot count; a null list -> -1 (Spark 2.4).
+ *   REMOVE (:262)            Elements equal to v removed, order kept; null elements are kept as null.  Pinned (offsets, value count).
+ *   SORT (:328)              Ascending in DataFrame::sort's order (NaN greatest, -0.0 == 0.0, ties in input order), nulls last.  Pinned.
+ *   DISTINCT (:39)           The first occurrence of each value in input order; at most one null, at the first null's place.  Unpinned.
+ *   REPEAT (:294)            The list concatenated `count` times; 0 -> empty; count < 0 -> BDF_INVALID (the reference casts it to usize);
+ *                            nulls repeat as nulls.  Unpinned.
+ *   EXCEPT / INTERSECT / UNION (:66, :110, :356)  Distinct results in the order of first appearance: except = in a, not in b;
+ *                            intersect = in a and in b; union = a then b.  Null elements are one value.  A null a -> a valid empty list;
+ *                            a null b counts as empty.  Different list counts per chunk -> BDF_LENGTH_MISMATCH ("Expected array a and b
+ *                            to have the same length").  Unpinned.
+ *   EXPLODE (scalar.rs:237)  Two one-chunk columns: UInt32 parent row numbers (counted through the chunks) and the T values, one row
+ *                            per element of every valid list, in order; null and empty lists give no row (Spark); null elements give
+ *                            null values.  Other columns follow with bdf_take_dev(col, rows).
+ * Errors (nothing is returned and nothing leaks): a null pointer or an unknown function -> BDF_INVALID; a non-numeric child, the limits
+ *   above, a multi-GPU context -> BDF_UNSUPPORTED; children of different dtypes in a set function -> BDF_UNSUPPORTED. */
+#define BDF_LIST_BASE 32   /* bdf_ipc_list_column reports a List<T> column as BDF_LIST_BASE + T */
+typedef struct bdf_list bdf_list;
+typedef struct {
+    const int32_t* offsets;   /* base of the offsets buffer, NOT offset-adjusted: entries offset .. offset + len are read    */
+    const uint8_t* validity;  /* list validity, LSB-first, 1 = valid; NULL when every list is valid                          */
+    int64_t        len;       /* lists                                                                                      */
+    int64_t        offset;    /* list offset (sliced ListArray)                                                             */
+    int64_t        null_count;
+    bdf_view       values;    /* the child array                                                                            */
+} bdf_list_view;
+/* One downloaded list chunk.  offsets >= len + 1 Int32, validity >= ceil(len / 8) bytes (may be NULL if the chunk has no null list),
+ * values >= elements x width bytes, value_validity >= ceil(elements / 8) bytes (may be NULL if no element is null); sizes come from
+ * bdf_list_chunk_info.  Bitmaps are written at bit 0. */
+typedef struct {
+    int32_t* offsets;
+    uint8_t* validity;
+    void*    values;
+    uint8_t* value_validity;
+    int64_t  null_count, value_null_count;   /* OUT */
+    int32_t  has_validity, has_value_validity; /* OUT */
+} bdf_list_out;
+typedef enum { BDF_LIST_CONTAINS = 0, BDF_LIST_POSITION } bdf_list_find_fn;
+typedef enum { BDF_LIST_MAX = 0, BDF_LIST_MIN, BDF_LIST_SIZE } bdf_list_reduce_fn;
+typedef enum { BDF_LIST_REMOVE = 0, BDF_LIST_SORT, BDF_LIST_DISTINCT, BDF_LIST_REPEAT } bdf_list_transform_fn;
+typedef enum { BDF_LIST_EXCEPT = 0, BDF_LIST_INTERSECT, BDF_LIST_UNION } bdf_list_set_fn;
+int  bdf_list_upload(bdf_ctx* ctx, int child_dtype, int64_t n_chunks, const bdf_list_view* in, int flags, bdf_list** out);
+int  bdf_list_describe(const bdf_list* list, int32_t* child_dtype, int64_t* n_chunks, int64_t* total_len);
+int  bdf_list_chunk_info(bdf_ctx* ctx, const bdf_list* list, int64_t chunk, int64_t* len, int64_t* null_count, int64_t* n_elements);
+int  bdf_list_download(bdf_ctx* ctx, const bdf_list* list, bdf_list_out* out /* n_chunks */);
+const bdf_col* bdf_list_values(const bdf_list* list);   /* owned by the list */
+void bdf_list_free(bdf_ctx* ctx, bdf_list* list);
+int  bdf_list_find_dev(bdf_ctx* ctx, int fn, const bdf_list* list, uint64_t value_bits, bdf_col** out);
+int  bdf_list_reduce_dev(bdf_ctx* ctx, int fn, const bdf_list* list, bdf_col** out);
+int  bdf_list_transform_dev(bdf_ctx* ctx, int fn, const bdf_list* list, uint64_t value_bits /* REMOVE */, int64_t count /* REPEAT */,
+                            bdf_list** out);
+int  bdf_list_set_dev(bdf_ctx* ctx, int fn, const bdf_list* a, const bdf_list* b, bdf_list** out);
+int  bdf_list_explode_dev(bdf_ctx* ctx, const bdf_list* list, bdf_col** rows, bdf_col** values);
+/* List<T> columns of an IPC file.  bdf_ipc_column keeps reporting them with dtype -1 (outside the column path: bdf_ipc_read and
+ * bdf_ipc_view refuse them, and readers that take every column of dtype >= 0 are unaffected); bdf_ipc_list_column gives
+ * BDF_LIST_BASE + T for a List of one numeric T and -1 for every other column (LargeList, nested lists, List<bool> ...);
+ * bdf_ipc_read_list uploads one, one chunk per RecordBatch, offsets and child buffers taken from the mapping (no context needed for
+ * the first, none of the three needs a GPU except the read). */
+int  bdf_ipc_list_column(const bdf_ipc* file, int32_t col, int32_t* dtype);
+int  bdf_ipc_read_list(bdf_ctx* ctx, const bdf_ipc* file, int32_t col, int flags, bdf_list** out);
+
 /* ---- measurement support ------------------------------------------------------------------------ */
 /* Per-launch CUDA-event timing on the library's compute stream (the stream the kernels run on). */
 typedef struct {
@@ -577,7 +663,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

@@ -37,6 +37,27 @@ pub struct BdfCsvOptions { pub has_header: i32, pub delimiter: u8, pub max_recor
 pub struct BdfCsvWriteOptions { pub has_header: i32, pub delimiter: u8 }
 
 #[repr(C)]
+pub struct BdfListView { pub offsets: *const i32, pub validity: *const u8, pub len: i64, pub offset: i64, pub null_count: i64, pub values: BdfView }
+#[repr(C)]
+pub struct BdfListOut {
+    pub offsets: *mut i32, pub validity: *mut u8, pub values: *mut c_void, pub value_validity: *mut u8,
+    pub null_count: i64, pub value_null_count: i64, pub has_validity: i32, pub has_value_validity: i32,
+}
+pub enum BdfList {}
+pub const BDF_LIST_BASE: i32 = 32;   // bdf_ipc_list_column: BDF_LIST_BASE + T
+pub const BDF_LIST_CONTAINS: i32 = 0;
+pub const BDF_LIST_POSITION: i32 = 1;
+pub const BDF_LIST_MAX: i32 = 0;
+pub const BDF_LIST_MIN: i32 = 1;
+pub const BDF_LIST_SIZE: i32 = 2;
+pub const BDF_LIST_REMOVE: i32 = 0;
+pub const BDF_LIST_SORT: i32 = 1;
+pub const BDF_LIST_DISTINCT: i32 = 2;
+pub const BDF_LIST_REPEAT: i32 = 3;
+pub const BDF_LIST_EXCEPT: i32 = 0;
+pub const BDF_LIST_INTERSECT: i32 = 1;
+pub const BDF_LIST_UNION: i32 = 2;
+#[repr(C)]
 pub struct BdfExprNode { pub op: i32, pub a: i32, pub b: i32 }   // op: bdf_binop, or BDF_EXPR_UNARY + bdf_unop
 pub const BDF_EXPR_UNARY: i32 = 100;
 /// bdf_group_out: per value column; `min` / `max` are NULL for Float columns (T::Native: Ord).
@@ -198,6 +219,20 @@ extern "C" {
     pub fn bdf_ipc_read(ctx: *mut BdfCtx, file: *const BdfIpc, n_cols: i32, cols: *const i32, flags: c_int, out: *mut *mut BdfCol) -> c_int;
     pub fn bdf_ipc_read_batches(ctx: *mut BdfCtx, file: *const BdfIpc, n_cols: i32, cols: *const i32, n_batches: i64, batches: *const i64,
                                 flags: c_int, out: *mut *mut BdfCol) -> c_int;
+    // List<T> columns and ArrayFunctions (src/functions/array.rs): rules, departures and limits in include/b200df.h
+    pub fn bdf_list_upload(ctx: *mut BdfCtx, child_dtype: c_int, n_chunks: i64, lists: *const BdfListView, flags: c_int, out: *mut *mut BdfList) -> c_int;
+    pub fn bdf_list_describe(list: *const BdfList, child_dtype: *mut i32, n_chunks: *mut i64, total_len: *mut i64) -> c_int;
+    pub fn bdf_list_chunk_info(ctx: *mut BdfCtx, list: *const BdfList, chunk: i64, len: *mut i64, null_count: *mut i64, n_elements: *mut i64) -> c_int;
+    pub fn bdf_list_download(ctx: *mut BdfCtx, list: *const BdfList, out: *mut BdfListOut) -> c_int;
+    pub fn bdf_list_values(list: *const BdfList) -> *const BdfCol;
+    pub fn bdf_list_free(ctx: *mut BdfCtx, list: *mut BdfList);
+    pub fn bdf_list_find_dev(ctx: *mut BdfCtx, func: c_int, list: *const BdfList, value_bits: u64, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_list_reduce_dev(ctx: *mut BdfCtx, func: c_int, list: *const BdfList, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_list_transform_dev(ctx: *mut BdfCtx, func: c_int, list: *const BdfList, value_bits: u64, count: i64, out: *mut *mut BdfList) -> c_int;
+    pub fn bdf_list_set_dev(ctx: *mut BdfCtx, func: c_int, a: *const BdfList, b: *const BdfList, out: *mut *mut BdfList) -> c_int;
+    pub fn bdf_list_explode_dev(ctx: *mut BdfCtx, list: *const BdfList, rows: *mut *mut BdfCol, values: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_ipc_list_column(file: *const BdfIpc, col: i32, dtype: *mut i32) -> c_int;
+    pub fn bdf_ipc_read_list(ctx: *mut BdfCtx, file: *const BdfIpc, col: i32, flags: c_int, out: *mut *mut BdfList) -> c_int;
     pub fn bdf_ipc_write(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol) -> c_int;
 }
 

@@ -21,9 +21,9 @@ SUM, MIN, MAX, COUNT = range(4)
 OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID, PARSE = range(10)
 ASYNC = 1
 (K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW,
- K_MOMENTS, K_CSV_WRITE) = range(17)
+ K_MOMENTS, K_CSV_WRITE, K_LIST) = range(18)
 KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
-                "window", "moments", "csv_write"]
+                "window", "moments", "csv_write", "list"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -51,6 +51,12 @@ WINDOW_FNS = {"row_number": WIN_ROW_NUMBER, "rank": WIN_RANK, "dense_rank": WIN_
               "max": WIN_MAX, "avg": WIN_AVG}
 FRAME_ROWS, FRAME_RANGE, FRAME_PARTITION = range(3)
 WINDOW_FRAMES = {"rows": FRAME_ROWS, "range": FRAME_RANGE, "partition": FRAME_PARTITION}
+# list columns (bdf_list_*)
+LIST_BASE = 32
+LIST_CONTAINS, LIST_POSITION = range(2)
+LIST_MAX, LIST_MIN, LIST_SIZE = range(3)
+LIST_REMOVE, LIST_SORT, LIST_DISTINCT, LIST_REPEAT = range(4)
+LIST_EXCEPT, LIST_INTERSECT, LIST_UNION = range(3)
 
 
 class View(C.Structure):
@@ -95,6 +101,16 @@ class GroupAggC(C.Structure):
 class WindowCall(C.Structure):
     _fields_ = [("function", C.c_int32), ("frame", C.c_int32), ("column", C.c_void_p), ("offset", C.c_int64), ("default_bits", C.c_uint64),
                 ("has_default", C.c_int32)]
+
+
+class ListView(C.Structure):
+    _fields_ = [("offsets", C.c_void_p), ("validity", C.c_void_p), ("len", C.c_int64), ("offset", C.c_int64), ("null_count", C.c_int64),
+                ("values", View)]
+
+
+class ListOut(C.Structure):
+    _fields_ = [("offsets", C.c_void_p), ("validity", C.c_void_p), ("values", C.c_void_p), ("value_validity", C.c_void_p),
+                ("null_count", C.c_int64), ("value_null_count", C.c_int64), ("has_validity", C.c_int32), ("has_value_validity", C.c_int32)]
 
 
 class CsvOptions(C.Structure):
@@ -243,12 +259,25 @@ def lib() -> C.CDLL:
         "bdf_csv_write": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(CsvWriteOptions)], C.c_int),
         "bdf_generate": ([vp, C.c_int, C.c_int, C.c_double, C.c_double, u64, u64, i64, P(i64), i64, C.c_uint32, P(vp)],
                          C.c_int),
+        "bdf_list_upload": ([vp, C.c_int, i64, P(ListView), C.c_int, P(vp)], C.c_int),
+        "bdf_list_describe": ([vp, P(i32), P(i64), P(i64)], C.c_int),
+        "bdf_list_chunk_info": ([vp, vp, i64, P(i64), P(i64), P(i64)], C.c_int),
+        "bdf_list_download": ([vp, vp, P(ListOut)], C.c_int),
+        "bdf_list_values": ([vp], vp),
+        "bdf_list_free": ([vp, vp], None),
+        "bdf_list_find_dev": ([vp, C.c_int, vp, u64, P(vp)], C.c_int),
+        "bdf_list_reduce_dev": ([vp, C.c_int, vp, P(vp)], C.c_int),
+        "bdf_list_transform_dev": ([vp, C.c_int, vp, u64, i64, P(vp)], C.c_int),
+        "bdf_list_set_dev": ([vp, C.c_int, vp, vp, P(vp)], C.c_int),
+        "bdf_list_explode_dev": ([vp, vp, P(vp), P(vp)], C.c_int),
+        "bdf_ipc_list_column": ([vp, i32, P(i32)], C.c_int),
+        "bdf_ipc_read_list": ([vp, vp, i32, C.c_int, P(vp)], C.c_int),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError if the library does not export a declared symbol
         fn.argtypes = args
         fn.restype = res
-    if L.bdf_abi_version() != 2:
+    if L.bdf_abi_version() != 3:
         raise RuntimeError("libb200df.so ABI version mismatch")
     _lib = L
     return L
@@ -268,6 +297,9 @@ EXPORTED_SYMBOLS = [
     "bdf_ipc_write_host", "bdf_ipc_write",
     "bdf_csv_open", "bdf_csv_describe", "bdf_csv_column", "bdf_csv_read", "bdf_csv_stats", "bdf_csv_close", "bdf_csv_write",
     "bdf_moments", "bdf_moments_dev", "bdf_moments_stat", "bdf_moments_merge", "bdf_distinct", "bdf_distinct_dev",
+    "bdf_list_upload", "bdf_list_describe", "bdf_list_chunk_info", "bdf_list_download", "bdf_list_values", "bdf_list_free",
+    "bdf_list_find_dev", "bdf_list_reduce_dev", "bdf_list_transform_dev", "bdf_list_set_dev", "bdf_list_explode_dev",
+    "bdf_ipc_list_column", "bdf_ipc_read_list",
 ]
 
 

@@ -197,3 +197,76 @@ class BooleanArray:
 
 def chunk_lengths(chunks: Sequence[PrimitiveArray]) -> List[int]:
     return [c.length for c in chunks]
+
+
+class ListArray:
+    """One chunk of an Arrow ``List<T>`` column (32-bit offsets, T one of the ten numeric types): the memory contract of
+    ``bdf_list_view`` -- Int32 offsets and an optional list validity bitmap, both starting at ``offset``, over a child
+    ``PrimitiveArray`` that the offsets index (from the child's own offset)."""
+
+    __slots__ = ("dtype", "offsets", "validity", "offset", "length", "null_count", "values", "_keepalive")
+
+    def __init__(self, dtype: int, offsets: np.ndarray, validity: Optional[np.ndarray], offset: int, length: int, null_count: int,
+                 values: PrimitiveArray, keepalive=None):
+        self.dtype = dtype
+        self.offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+        self.validity = None if validity is None else np.ascontiguousarray(validity, dtype=np.uint8)
+        self.offset = int(offset)
+        self.length = int(length)
+        if self.offsets.shape[0] < self.offset + self.length + 1:
+            raise ValueError("offsets buffer too short")
+        self.null_count = 0 if self.validity is None else int(null_count)
+        self.values = values
+        self._keepalive = keepalive
+
+    @classmethod
+    def from_pylist(cls, dtype: int, items: Iterable) -> "ListArray":
+        """[[1, 2], None, [], [None, 3]]: None lists are null (spanning no element), None elements are null elements."""
+        items = list(items)
+        offsets = [0]
+        flat: list = []
+        for x in items:
+            if x is not None:
+                flat.extend(x)
+            offsets.append(len(flat))
+        mask = np.array([x is not None for x in items], dtype=bool)
+        validity = None if mask.all() else pack_validity(mask)
+        return cls(dtype, np.array(offsets, dtype=np.int32), validity, 0, len(items), int((~mask).sum()),
+                   PrimitiveArray.from_pylist(dtype, flat))
+
+    @classmethod
+    def from_arrow(cls, arr) -> "ListArray":
+        """Zero-copy view of a pyarrow ListArray (list offset, child offset and both validities preserved)."""
+        import pyarrow as pa
+
+        if not pa.types.is_list(arr.type):
+            raise TypeError(f"{arr.type} is not a List with 32-bit offsets")
+        child = PrimitiveArray.from_arrow(arr.values)
+        bufs = arr.buffers()
+        n_off = arr.offset + len(arr) + 1
+        offsets = np.frombuffer(bufs[1], dtype=np.int32, count=n_off) if bufs[1] is not None else np.zeros(n_off, np.int32)
+        validity = np.frombuffer(bufs[0], dtype=np.uint8) if bufs[0] is not None else None
+        return cls(child.dtype, offsets, validity, arr.offset, len(arr), arr.null_count, child, keepalive=arr)
+
+    def __len__(self) -> int:
+        return self.length
+
+    def valid_mask(self) -> np.ndarray:
+        if self.validity is None:
+            return np.ones(self.length, dtype=bool)
+        bits = np.unpackbits(self.validity, bitorder="little")
+        return bits[self.offset:self.offset + self.length].astype(bool)
+
+    def to_pylist(self) -> list:
+        """None for a null list; elements as numpy scalars of the child type, None for a null element."""
+        vm = self.valid_mask()
+        cm = self.values.valid_mask()
+        vals = self.values.values[self.values.offset:self.values.offset + self.values.length]
+        out = []
+        for k in range(self.length):
+            if not vm[k]:
+                out.append(None)
+                continue
+            b, e = int(self.offsets[self.offset + k]), int(self.offsets[self.offset + k + 1])
+            out.append([vals[i] if cm[i] else None for i in range(b, e)])
+        return out

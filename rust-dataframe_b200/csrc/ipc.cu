@@ -105,6 +105,7 @@ enum { T_NONE = 0, T_Null, T_Int, T_FloatingPoint, T_Binary, T_Utf8, T_Bool, T_D
 struct IpcField {
     std::string name;
     int dtype = -1;       // bdf_dtype, BDF_BOOL, or -1: a type outside the path
+    int list_child = -1;  // a List<T> of one numeric T (dtype stays -1: bdf_ipc_list_column / bdf_ipc_read_list): T
     bool nullable = false;
     int64_t n_nodes = 0, n_buffers = 0;   // what the field (with its children) occupies in every RecordBatch
 };
@@ -164,13 +165,21 @@ bool parse_field(const FbTable& f, IpcField* out, int depth, int64_t* budget, st
             if (!parse_field(ch, &c, depth + 1, budget, why)) return false;
             out->n_nodes += c.n_nodes;
             out->n_buffers += c.n_buffers;
+            // List<T> of one numeric child T: the list path (bdf_ipc_read_list); every other nested type stays outside
+            if (tt == T_List && cnt == 1 && c.dtype >= BDF_I8 && c.dtype <= BDF_F64) out->list_child = c.dtype;
         }
     }
     return true;
 }
 
 struct IpcBuf { int64_t off = 0, len = 0; };
-struct IpcColChunk { int64_t len = 0, null_count = 0; IpcBuf validity, values; };
+struct IpcColChunk {
+    int64_t len = 0, null_count = 0;
+    IpcBuf validity, values;            // a List<T> column: values = its Int32 offsets
+    int64_t child_len = 0, child_nulls = 0;
+    IpcBuf child_validity, child_values;
+    bool list_ok = true;                // a List column: its buffers fit the batch (checked by bdf_ipc_read_list)
+};
 struct IpcBatch {
     int64_t rows = 0;
     size_t body = 0;          // file offset of the body
@@ -284,21 +293,33 @@ int bdf_ipc_open(const char* path, bdf_ipc** out) {
         size_t ni = 0, bi = 0;
         for (size_t c = 0; c < f->fields.size(); c++) {
             const IpcField& fld = f->fields[c];
-            if (fld.dtype >= 0) {
+            if (fld.dtype >= 0 || fld.list_child >= 0) {
                 IpcColChunk& cc = b.cols[c];
                 mb.rd(nfirst + 16 * ni, &cc.len); mb.rd(nfirst + 16 * ni + 8, &cc.null_count);
                 mb.rd(bufirst + 16 * bi, &cc.validity.off); mb.rd(bufirst + 16 * bi + 8, &cc.validity.len);
                 mb.rd(bufirst + 16 * (bi + 1), &cc.values.off); mb.rd(bufirst + 16 * (bi + 1) + 8, &cc.values.len);
-                int64_t need = 0;
-                dtype_bytes(fld.dtype, cc.len, &need);
+                int64_t need = cc.len > 0 ? (cc.len + 1) * 4 : 0;   // a list's offsets (a list array without lists may have none)
+                if (fld.dtype >= 0) dtype_bytes(fld.dtype, cc.len, &need);
                 const bool has_v = cc.null_count > 0;
                 // offsets and lengths come from the file: compare each with what is left of the body (off + len may wrap)
                 auto fits = [body_len](const IpcBuf& bf, int64_t min_len) {
                     return bf.off >= 0 && bf.len >= min_len && bf.off <= body_len && bf.len <= body_len - bf.off;
                 };
-                if (cc.len != b.rows || cc.null_count < 0 || cc.null_count > cc.len || !fits(cc.values, need) ||
-                    (has_v && !fits(cc.validity, (cc.len + 7) / 8)))
+                const bool ok = cc.len == b.rows && cc.null_count >= 0 && cc.null_count <= cc.len && fits(cc.values, need) &&
+                                (!has_v || fits(cc.validity, (cc.len + 7) / 8));
+                // a List column is only checked for bdf_ipc_read_list: a file whose list column that reader cannot use still opens
+                if (!ok && fld.list_child < 0)
                     return ipc_fail(BDF_INVALID, "record batch %u, column '%s': buffers do not fit the batch", k, fld.name.c_str());
+                cc.list_ok = ok;
+                if (fld.list_child >= 0 && ok) {   // the child's node and buffers follow the list's
+                    mb.rd(nfirst + 16 * (ni + 1), &cc.child_len); mb.rd(nfirst + 16 * (ni + 1) + 8, &cc.child_nulls);
+                    mb.rd(bufirst + 16 * (bi + 2), &cc.child_validity.off); mb.rd(bufirst + 16 * (bi + 2) + 8, &cc.child_validity.len);
+                    mb.rd(bufirst + 16 * (bi + 3), &cc.child_values.off); mb.rd(bufirst + 16 * (bi + 3) + 8, &cc.child_values.len);
+                    int64_t cneed = 0;
+                    dtype_bytes(fld.list_child, cc.child_len, &cneed);
+                    cc.list_ok = cc.child_len >= 0 && cc.child_nulls >= 0 && cc.child_nulls <= cc.child_len && fits(cc.child_values, cneed) &&
+                                 (cc.child_nulls == 0 || fits(cc.child_validity, (cc.child_len + 7) / 8));
+                }
             }
             ni += fld.n_nodes;
             bi += fld.n_buffers;
@@ -365,6 +386,33 @@ int bdf_ipc_read_batches(bdf_ctx* ctx, const bdf_ipc* f, int32_t n_cols, const i
         vp[i] = views[i].data();
     }
     return bdf_upload_many(ctx, n_cols, dtypes.data(), nch.data(), vp.data(), flags, out);
+}
+
+int bdf_ipc_read_list(bdf_ctx* ctx, const bdf_ipc* f, int32_t col, int flags, bdf_list** out) {
+    if (!ctx || !f || !out) return ipc_fail(BDF_INVALID, "null argument");
+    if (col < 0 || (size_t)col >= f->fields.size()) return ipc_fail(BDF_INVALID, "column index out of range");
+    const int dt = f->fields[col].list_child;
+    if (dt < 0) return ipc_fail(BDF_UNSUPPORTED, "column '%s' is not a List of a numeric type", f->fields[col].name.c_str());
+    std::vector<bdf_list_view> views(std::max<size_t>(f->batches.size(), 1));
+    for (size_t b = 0; b < f->batches.size(); b++) {
+        const IpcBatch& bt = f->batches[b];
+        const IpcColChunk& c = bt.cols[col];
+        if (!c.list_ok) return ipc_fail(BDF_INVALID, "record batch %zu, column '%s': list buffers do not fit the batch", b, f->fields[col].name.c_str());
+        const uint8_t* body = f->map + bt.body;
+        views[b].offsets = c.len > 0 ? (const int32_t*)(body + c.values.off) : nullptr;
+        views[b].validity = c.null_count > 0 ? body + c.validity.off : nullptr;
+        views[b].len = c.len;
+        views[b].offset = 0;
+        views[b].null_count = c.null_count;
+        views[b].values = bdf_view{body + c.child_values.off, c.child_nulls > 0 ? body + c.child_validity.off : nullptr, c.child_len, 0, c.child_nulls};
+    }
+    return bdf_list_upload(ctx, dt, (int64_t)f->batches.size(), views.data(), flags, out);
+}
+
+int bdf_ipc_list_column(const bdf_ipc* f, int32_t col, int32_t* dtype) {
+    if (!f || !dtype || col < 0 || (size_t)col >= f->fields.size()) return ipc_fail(BDF_INVALID, "column index out of range");
+    *dtype = f->fields[col].list_child < 0 ? -1 : BDF_LIST_BASE + f->fields[col].list_child;
+    return BDF_OK;
 }
 
 int bdf_ipc_read(bdf_ctx* ctx, const bdf_ipc* f, int32_t n_cols, const int32_t* cols, int flags, bdf_col** out) {

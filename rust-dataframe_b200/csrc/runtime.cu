@@ -3839,6 +3839,506 @@ static void fleet_destroy(bdf_ctx* c) {
 }
 
 // ---------------------------------------------------------------------------------------------------
+// list columns and ArrayFunctions (k_list.cu).  Contains / position / max / min / size work chunk by chunk on the list's own
+// offsets.  The functions that return lists work in the element space of the call (every element of the input lists, counted
+// through the chunks): a parent column (the element's global list number, NULL for an element of a null list) and the stable
+// lexsort over (parent, value) turn them into the existing sort / take / heads / filter steps, and the result's offsets come from
+// the list numbers of the kept elements.  They return one chunk, as take and sort do.
+
+namespace bdf {
+size_t list_find_scratch_bytes(long long n_elem);
+cudaError_t launch_list_find(int dtype, const int32_t* off, const uint32_t* lvalid, long long len, long long n_elem, const void* values,
+                             const uint32_t* vvalid, int vbit_off, uint64_t value_bits, int mode, uint32_t* bits, int32_t* pos, void* scratch,
+                             int sm_count, cudaStream_t s);
+cudaError_t launch_list_parent(const int32_t* off, const uint32_t* lvalid, const uint32_t* and_valid, long long len, long long n_elem, long long list0,
+                               long long elem0, uint32_t* parent, uint32_t* inlist, cudaStream_t s);
+cudaError_t launch_list_remove_mask(int dtype, const void* values, const uint32_t* vvalid, int vbit_off, long long n_elem, long long elem0,
+                                    uint64_t value_bits, const uint32_t* inlist, uint32_t* keep, cudaStream_t s);
+cudaError_t launch_list_mark(const uint32_t* perm, const uint32_t* head, const uint32_t* pvalid, long long n, long long split, int mode, uint32_t* keep,
+                             cudaStream_t s);
+cudaError_t launch_list_offsets(const uint32_t* kp, long long n_kept, long long n_lists, long long mult, int32_t* out, cudaStream_t s);
+cudaError_t launch_list_repeat(const int32_t* base, long long n_lists, long long count, const uint32_t* rows, long long n_out, uint32_t* src, cudaStream_t s);
+cudaError_t launch_list_size(const int32_t* off, const uint32_t* lvalid, long long len, int32_t* out, cudaStream_t s);
+cudaError_t launch_list_minmax_valid(const int32_t* off, const uint32_t* lvalid, const uint32_t* nonempty, long long len, uint32_t* valid, int* empty,
+                                     cudaStream_t s);
+}  // namespace bdf
+
+struct bdf_list {
+    int dtype = 0;
+    bdf_col* values = nullptr;               // chunk i = the elements of list chunk i
+    std::vector<int64_t> lens, null_counts;  // lists and null lists per chunk
+    std::vector<int64_t> valid_elems;        // elements that belong to a valid list, per chunk
+    std::vector<int32_t*> off;               // device: len + 1 offsets from 0
+    std::vector<uint32_t*> valid;            // device: the list validity at bit 0, or nullptr
+    char* arena = nullptr;                   // the offsets and validity of every chunk
+    int64_t total_len = 0;
+};
+
+static void list_release(bdf_ctx* c, bdf_list* l) {
+    if (!l) return;
+    if (l->values) col_release(c, l->values);
+    if (l->arena) cudaFreeAsync(l->arena, c->s_compute);
+    delete l;
+}
+static void drop(bdf_ctx* c, bdf_list* l) { list_release(c, l); }
+using ListOwner = Owned<bdf_list>;
+
+static constexpr int64_t kListMaxChunkElems = 0x7fffffffLL;    // Int32 offsets
+static constexpr int64_t kListMaxCallElems = 0xffffffffLL;     // the sort's UInt32 row numbers
+
+// A list whose offsets (and validity, where has_valid) live in one device arena; the caller fills them and sets `values`.
+static int list_alloc(bdf_ctx* c, int dtype, const std::vector<int64_t>& lens, const std::vector<bool>& has_valid, bdf_list** out) {
+    ListOwner l(c, new (std::nothrow) bdf_list());
+    if (!l.get()) return fail(BDF_OOM, "host allocation failed");
+    l->dtype = dtype;
+    l->lens = lens;
+    const size_t n = lens.size();
+    std::vector<size_t> ooff(n), voff(n);
+    size_t bytes = 0;
+    for (size_t i = 0; i < n; i++) {
+        ooff[i] = bytes;
+        bytes += align_up((size_t)(lens[i] + 1) * 4, 256);
+        voff[i] = bytes;
+        if (has_valid[i]) bytes += align_up((size_t)(lens[i] + 31) / 32 * 4 + 8, 256);
+        l->total_len += lens[i];
+    }
+    cudaError_t e = cudaMallocAsync((void**)&l->arena, std::max<size_t>(bytes, 256), c->s_compute);
+    if (e != cudaSuccess) { cudaGetLastError(); l->arena = nullptr; return fail(cuda_status(e), "list allocation of %zu bytes failed", bytes); }
+    for (size_t i = 0; i < n; i++) {
+        l->off.push_back((int32_t*)(l->arena + ooff[i]));
+        l->valid.push_back(has_valid[i] ? (uint32_t*)(l->arena + voff[i]) : nullptr);
+    }
+    l->null_counts.assign(n, 0);
+    l->valid_elems.assign(n, 0);
+    *out = l.release();
+    return BDF_OK;
+}
+
+static bool host_bit(const uint8_t* bits, int64_t i) { return (bits[i >> 3] >> (i & 7)) & 1u; }
+
+static int list_upload(bdf_ctx* c, int dtype, int64_t n, const bdf_list_view* in, bool async, bdf_list** out) {
+    if (dtype < 0 || dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "list columns on the device have one of the ten numeric child types");
+    std::vector<bdf_view> child((size_t)n);
+    std::vector<std::vector<int32_t>> offs((size_t)n);
+    std::vector<std::vector<uint32_t>> bits((size_t)n);
+    std::vector<int64_t> lens((size_t)n), nulls((size_t)n, 0), valid_elems((size_t)n, 0);
+    std::vector<bool> has_valid((size_t)n);
+    int64_t total = 0;
+    for (int64_t i = 0; i < n; i++) {
+        const bdf_list_view& v = in[i];
+        if (v.len < 0 || v.offset < 0 || (v.len > 0 && !v.offsets) || v.values.len < 0 || v.values.offset < 0)
+            return fail(BDF_INVALID, "bad list view %lld", (long long)i);
+        const int32_t* o = v.offsets ? v.offsets + v.offset : nullptr;
+        const int64_t first = o ? o[0] : 0, last = o ? o[v.len] : 0;
+        if (first < 0 || last > v.values.len) return fail(BDF_INVALID, "list chunk %lld: offsets outside the child array", (long long)i);
+        offs[i].resize((size_t)v.len + 1);
+        offs[i][0] = 0;
+        for (int64_t k = 0; k < v.len; k++) {
+            if (o[k + 1] < o[k]) return fail(BDF_INVALID, "list chunk %lld: offsets decrease at %lld", (long long)i, (long long)k);
+            offs[i][k + 1] = (int32_t)(o[k + 1] - first);
+        }
+        if (last - first >= kListMaxChunkElems) return fail(BDF_UNSUPPORTED, "list chunk %lld: 2^31 or more elements", (long long)i);
+        lens[i] = v.len;
+        has_valid[i] = v.validity != nullptr;
+        if (v.validity) bits[i].assign((size_t)(v.len + 31) / 32 + 2, 0u);
+        for (int64_t k = 0; k < v.len; k++) {
+            const bool ok = !v.validity || host_bit(v.validity, v.offset + k);
+            if (v.validity && ok) bits[i][k >> 5] |= 1u << (k & 31);
+            if (ok) valid_elems[i] += o[k + 1] - o[k];
+            else nulls[i]++;
+        }
+        child[i] = bdf_view{v.values.values, v.values.validity, last - first, v.values.offset + first,
+                            (first == 0 && last == v.values.len) ? v.values.null_count : -1};
+        total += last - first;
+    }
+    if (total >= kListMaxCallElems) return fail(BDF_UNSUPPORTED, "a list call holds 2^32 or more elements (the sort's UInt32 row numbers)");
+    ListOwner l(c);
+    TRY(list_alloc(c, dtype, lens, has_valid, l.out()));
+    l->null_counts = nulls;
+    l->valid_elems = valid_elems;
+    std::vector<bdf_col*> cols;
+    TRY(upload_many(c, {UploadSpec{dtype, n, child.data()}}, async, cols));
+    ColOwner values(c, cols[0]);
+    bool misaligned = false;
+    for (auto& ch : values->chunks) misaligned = misaligned || (ch.validity && ch.bit_off != 0);
+    if (misaligned) {   // the fold of max / min reads validity at bit 0
+        ColOwner re(c);
+        TRY(realign(c, values.get(), re.out()));
+        values = std::move(re);
+    }
+    for (int64_t i = 0; i < n; i++) {
+        CK(cudaMemcpyAsync(l->off[i], offs[i].data(), offs[i].size() * 4, cudaMemcpyHostToDevice, c->s_compute));
+        if (l->valid[i]) CK(cudaMemcpyAsync(l->valid[i], bits[i].data(), bits[i].size() * 4, cudaMemcpyHostToDevice, c->s_compute));
+    }
+    CK(cudaStreamSynchronize(c->s_compute));   // the host vectors go out of scope
+    l->values = values.release();
+    *out = l.release();
+    return BDF_OK;
+}
+
+static int list_download(bdf_ctx* c, const bdf_list* l, bdf_list_out* out) {
+    const int64_t n = (int64_t)l->lens.size();
+    std::vector<bdf_out> vo((size_t)std::max<int64_t>(n, 1));
+    for (int64_t i = 0; i < n; i++) {
+        if (!out[i].offsets) return fail(BDF_INVALID, "list output chunk %lld has no offsets buffer", (long long)i);
+        if (l->valid[i] && l->lens[i] && !out[i].validity) return fail(BDF_INVALID, "list output chunk %lld needs a validity buffer", (long long)i);
+        vo[i] = bdf_out{out[i].values, out[i].value_validity, l->values->chunks[i].len, 0, 0};
+    }
+    TRY(download(c, l->values, vo.data()));
+    // the offsets and validity are written by kernels on the compute stream (k_list_offsets is the last step of every list-returning
+    // function): copy them in that stream's order
+    std::vector<uint32_t> words;
+    for (int64_t i = 0; i < n; i++) {
+        CK(cudaMemcpyAsync(out[i].offsets, l->off[i], (size_t)(l->lens[i] + 1) * 4, cudaMemcpyDeviceToHost, c->s_compute));
+        CK(cudaStreamSynchronize(c->s_compute));
+        out[i].has_validity = l->valid[i] != nullptr;
+        out[i].null_count = l->null_counts[i];
+        if (l->valid[i] && l->lens[i]) {
+            words.resize((size_t)(l->lens[i] + 31) / 32);
+            CK(cudaMemcpyAsync(words.data(), l->valid[i], words.size() * 4, cudaMemcpyDeviceToHost, c->s_compute));
+            CK(cudaStreamSynchronize(c->s_compute));
+            memcpy(out[i].validity, words.data(), (size_t)bitmap_bytes(l->lens[i]));
+        }
+        out[i].has_value_validity = vo[i].has_validity;
+        out[i].value_null_count = vo[i].null_count;
+    }
+    return BDF_OK;
+}
+
+// A column that borrows device memory owned by other columns (no arenas, no events): views for the sort keys and the concatenated
+// children of two lists.  Everything that reads it runs on the compute stream after the owners were produced.
+static int col_borrow(int dtype, const std::vector<DevChunk>& chunks, bdf_col** out) {
+    bdf_col* col = new (std::nothrow) bdf_col();
+    if (!col) return fail(BDF_OOM, "host allocation failed");
+    col->dtype = dtype;
+    col->chunks = chunks;
+    for (auto& ch : chunks) col->total_len += ch.len;
+    col->null_counts.assign(chunks.size(), -1);
+    col->tile0.assign(chunks.size() + 1, 0);
+    *out = col;
+    return BDF_OK;
+}
+
+// The element space of one call over the children of `parts` in order.  and_valid[k]: a list whose validity also gates part k's
+// elements (union: b's elements take part only where a's list is valid), or null.
+struct ListElems {
+    explicit ListElems(bdf_ctx* c) : parent(c), inlist(c), iota(c), keyed(c), child(c) {}
+    ColOwner parent;   // UInt32: the global list number of every element
+    ColOwner inlist;   // Boolean: the element belongs to a valid list
+    ColOwner iota;     // UInt32: 0 .. n-1
+    ColOwner keyed;    // parent with inlist as its validity: the first sort key, elements of null lists sort last
+    ColOwner child;    // the children of the parts, chunk after chunk (borrowed)
+    int64_t n = 0;
+};
+
+static int list_elems(bdf_ctx* c, const std::vector<const bdf_list*>& parts, const std::vector<const bdf_list*>& and_valid, ListElems* x) {
+    std::vector<DevChunk> chunks;
+    for (const bdf_list* l : parts) {
+        wait_groups(c->s_compute, l->values, 0, (int64_t)l->values->chunks.size());
+        for (auto& ch : l->values->chunks) chunks.push_back(ch);
+        x->n += l->values->total_len;
+    }
+    const int64_t n = x->n;
+    TRY(col_borrow(parts[0]->dtype, chunks, x->child.out()));
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, x->parent.out()));
+    TRY(col_alloc(c, kBool, {ChunkPlan{n, false}}, nullptr, 0, x->inlist.out()));
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, x->iota.out()));
+    uint32_t* parent = (uint32_t*)x->parent->chunks[0].values;
+    uint32_t* inlist = (uint32_t*)x->inlist->chunks[0].values;
+    cudaError_t e = n ? cudaMemsetAsync(inlist, 0, align_up((size_t)bitmap_bytes(n), 4), c->s_compute) : cudaSuccess;
+    {
+        LaunchTimer t(c, BDF_K_LIST, BDF_U32, n, 4 * n + n / 8);
+        int64_t elem0 = 0;
+        for (size_t k = 0; k < parts.size() && e == cudaSuccess; k++) {
+            const bdf_list* l = parts[k];
+            int64_t list0 = 0;
+            for (size_t i = 0; i < l->lens.size() && e == cudaSuccess; i++) {
+                const int64_t ne = l->values->chunks[i].len;
+                e = launch_list_parent(l->off[i], l->valid[i], and_valid[k] ? and_valid[k]->valid[i] : nullptr, l->lens[i], ne, list0, elem0, parent,
+                                       inlist, c->s_compute);
+                list0 += l->lens[i];
+                elem0 += ne;
+            }
+        }
+    }
+    c->launches++;
+    if (e == cudaSuccess && n) e = launch_iota((uint32_t*)x->iota->chunks[0].values, n, c->sm_count, c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "list parents");
+    DevChunk kc = x->parent->chunks[0];
+    kc.validity = inlist;
+    TRY(col_borrow(BDF_U32, {kc}, x->keyed.out()));
+    return BDF_OK;
+}
+
+// The one-chunk result list: values = child[rows], offsets from kp (the kept elements' list numbers, ascending), times mult.
+static int list_result(bdf_ctx* c, int dtype, const bdf_col* child, const bdf_col* rows, const bdf_col* kp, int64_t n_lists, int64_t mult,
+                       bdf_list** out) {
+    const int64_t n_kept = kp->total_len;
+    if (n_kept * mult >= kListMaxChunkElems) return fail(BDF_UNSUPPORTED, "a list result of 2^31 or more elements (one chunk of Int32 offsets)");
+    ListOwner l(c);
+    TRY(list_alloc(c, dtype, {n_lists}, {false}, l.out()));
+    l->valid_elems[0] = n_kept * mult;
+    ColOwner values(c);
+    TRY(take_dev(c, child, rows, values.out()));
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_LIST, BDF_I32, n_lists, 4 * (n_lists + 1));
+        e = launch_list_offsets(n_kept ? (const uint32_t*)kp->chunks[0].values : nullptr, n_kept, n_lists, mult, l->off[0], c->s_compute);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "list offsets");
+    l->values = values.release();
+    *out = l.release();
+    return BDF_OK;
+}
+
+static int bool_zeroed(bdf_ctx* c, int64_t n, bdf_col** out) {
+    ColOwner b(c);
+    TRY(col_alloc(c, kBool, {ChunkPlan{n, false}}, nullptr, 0, b.out()));
+    if (n) CK(cudaMemsetAsync(b->chunks[0].values, 0, align_up((size_t)bitmap_bytes(n), 4), c->s_compute));
+    *out = b.release();
+    return BDF_OK;
+}
+
+static int list_find(bdf_ctx* c, int fn, const bdf_list* l, uint64_t bits, bdf_col** out) {
+    if (fn != BDF_LIST_CONTAINS && fn != BDF_LIST_POSITION) return fail(BDF_INVALID, "unknown list find function %d", fn);
+    const bool contains = fn == BDF_LIST_CONTAINS;
+    const size_t n = l->lens.size();
+    std::vector<ChunkPlan> plan(n);
+    int64_t max_elems = 0, rows = 0;
+    for (size_t i = 0; i < n; i++) {
+        plan[i] = {l->lens[i], contains && l->valid[i] != nullptr};
+        max_elems = std::max(max_elems, l->values->chunks[i].len);
+        rows += l->values->chunks[i].len;
+    }
+    ColOwner o(c);
+    TRY(col_alloc(c, contains ? kBool : BDF_I32, plan, nullptr, 0, o.out()));
+    Scratch<void> scratch;
+    CK(scratch.alloc(c, list_find_scratch_bytes(max_elems)));
+    wait_groups(c->s_compute, l->values, 0, (int64_t)n);
+    cudaError_t e = cudaSuccess;
+    {
+        const int64_t w = dtype_width(l->dtype);
+        LaunchTimer t(c, BDF_K_LIST, contains ? kBool : BDF_I32, rows, rows * w + 4 * (l->total_len + (int64_t)n) + (contains ? l->total_len / 4 : 4 * l->total_len));
+        for (size_t i = 0; i < n && e == cudaSuccess; i++) {
+            const DevChunk& ch = l->values->chunks[i];
+            DevChunk& oc = o->chunks[i];
+            if (contains && l->lens[i]) {
+                e = cudaMemsetAsync(oc.values, 0, align_up((size_t)bitmap_bytes(l->lens[i]), 4), c->s_compute);
+                if (e == cudaSuccess && oc.validity)
+                    e = cudaMemcpyAsync(oc.validity, l->valid[i], (size_t)bitmap_bytes(l->lens[i]), cudaMemcpyDeviceToDevice, c->s_compute);
+            }
+            if (e == cudaSuccess)
+                e = launch_list_find(l->dtype, l->off[i], l->valid[i], l->lens[i], ch.len, ch.values, ch.validity, ch.bit_off, bits, contains ? 0 : 1,
+                                     (uint32_t*)oc.values, (int32_t*)oc.values, scratch, c->sm_count, c->s_compute);
+            o->null_counts[i] = oc.validity ? l->null_counts[i] : 0;
+        }
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "list find");
+    *out = o.release();
+    return BDF_OK;
+}
+
+static int list_reduce(bdf_ctx* c, int fn, const bdf_list* l, bdf_col** out) {
+    if (fn < BDF_LIST_MAX || fn > BDF_LIST_SIZE) return fail(BDF_INVALID, "unknown list reduce function %d", fn);
+    const size_t n = l->lens.size();
+    const bool size = fn == BDF_LIST_SIZE;
+    std::vector<ChunkPlan> plan(n);
+    int64_t max_len = 0, max_elems = 0, rows = 0;
+    for (size_t i = 0; i < n; i++) {
+        plan[i] = {l->lens[i], !size};
+        max_len = std::max(max_len, l->lens[i]);
+        max_elems = std::max(max_elems, l->values->chunks[i].len);
+        rows += l->values->chunks[i].len;
+    }
+    const int dt = size ? BDF_I32 : l->dtype;
+    ColOwner o(c);
+    TRY(col_alloc(c, dt, plan, nullptr, 0, o.out()));
+    wait_groups(c->s_compute, l->values, 0, (int64_t)n);
+    cudaError_t e = cudaSuccess;
+    if (size) {
+        LaunchTimer t(c, BDF_K_LIST, BDF_I32, l->total_len, 8 * l->total_len);
+        for (size_t i = 0; i < n && e == cudaSuccess; i++) e = launch_list_size(l->off[i], l->valid[i], l->lens[i], (int32_t*)o->chunks[i].values, c->s_compute);
+    } else {
+        // the group-by fold with the offsets as group starts: sum / count / the other extreme are scratch
+        const int w = dtype_width(l->dtype);
+        Scratch<char> sum, other, big;
+        Scratch<long long> count;
+        Scratch<uint32_t> nonempty;
+        e = sum.alloc(c, (size_t)std::max<int64_t>(max_len, 1) * 8);
+        if (e == cudaSuccess) e = other.alloc(c, (size_t)std::max<int64_t>(max_len, 1) * w);
+        if (e == cudaSuccess) e = count.alloc(c, (size_t)std::max<int64_t>(max_len, 1) * 8);
+        if (e == cudaSuccess) e = nonempty.alloc(c, ((size_t)max_len + 31) / 32 * 4 + 8);
+        if (e == cudaSuccess) e = big.alloc(c, group_big_scratch_bytes(max_elems));
+        if (e == cudaSuccess) e = cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute);
+        {
+            LaunchTimer t(c, BDF_K_LIST, dt, rows, rows * w + 4 * (l->total_len + (int64_t)n) + l->total_len * w + l->total_len / 8);
+            for (size_t i = 0; i < n && e == cudaSuccess; i++) {
+                const DevChunk& ch = l->values->chunks[i];
+                DevChunk& oc = o->chunks[i];
+                const int64_t len = l->lens[i];
+                if (!len) continue;
+                e = cudaMemsetAsync(nonempty, 0, ((size_t)len + 31) / 32 * 4, c->s_compute);
+                void* mn = fn == BDF_LIST_MIN ? oc.values : (void*)other.get();
+                void* mx = fn == BDF_LIST_MAX ? oc.values : (void*)other.get();
+                c->launches += 3;
+                if (e == cudaSuccess)
+                    e = launch_group_reduce(l->dtype, true, ch.values, ch.validity, (const uint32_t*)l->off[i], len, ch.len, sum, count, mn, mx, nullptr, nonempty,
+                                            big, c->sm_count, c->s_compute);
+                if (e == cudaSuccess) e = launch_list_minmax_valid(l->off[i], l->valid[i], nonempty, len, oc.validity, c->d_flag, c->s_compute);
+                o->null_counts[i] = -1;
+            }
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+        if (e == cudaSuccess && *c->h_flag) return fail(BDF_WOULD_PANIC, "array_max / array_min of an empty list: the reference's .max().unwrap() panics");
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "list reduce");
+    *out = o.release();
+    return BDF_OK;
+}
+
+// Keep the elements whose bit is set in `keep` (element space of x), in element order.
+static int list_keep(bdf_ctx* c, const ListElems& x, const bdf_col* keep, int dtype, int64_t n_lists, bdf_list** out) {
+    ColOwner rows(c), kp(c);
+    TRY(filter_dev(c, x.iota.get(), keep, rows.out()));
+    TRY(filter_dev(c, x.parent.get(), keep, kp.out()));
+    return list_result(c, dtype, x.child.get(), rows.get(), kp.get(), n_lists, 1, out);
+}
+
+// The stable (list, value) sort of the element space, its group heads, and the keep bits `mode` of k_list_mark sets from them.
+static int list_mark(bdf_ctx* c, const ListElems& x, int64_t split, int mode, bdf_col** keep) {
+    const bdf_sort_key keys[2] = {{x.keyed.get(), 0}, {x.child.get(), 0}};
+    ColOwner perm(c), sp(c), sv(c), head(c), k(c);
+    TRY(sort_indices_dev(c, 2, keys, perm.out()));
+    TRY(take_dev(c, x.keyed.get(), perm.get(), sp.out()));
+    TRY(take_dev(c, x.child.get(), perm.get(), sv.out()));
+    TRY(group_heads(c, {sv.get(), sp.get()}, false, x.n, head.out()));
+    TRY(bool_zeroed(c, x.n, k.out()));
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_LIST, kBool, x.n, 4 * x.n + x.n / 4);
+        e = launch_list_mark((const uint32_t*)perm->chunks[0].values, (const uint32_t*)head->chunks[0].values, sp->chunks[0].validity, x.n, split, mode,
+                             (uint32_t*)k->chunks[0].values, c->s_compute);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "list mark");
+    *keep = k.release();
+    return BDF_OK;
+}
+
+static int list_transform(bdf_ctx* c, int fn, const bdf_list* l, uint64_t bits, int64_t count, bdf_list** out) {
+    if (fn < BDF_LIST_REMOVE || fn > BDF_LIST_REPEAT) return fail(BDF_INVALID, "unknown list transform function %d", fn);
+    if (fn == BDF_LIST_REPEAT && count < 0) return fail(BDF_INVALID, "array_repeat: count %lld < 0", (long long)count);
+    ListElems x(c);
+    TRY(list_elems(c, {l}, {nullptr}, &x));
+    const int64_t N = l->total_len;
+    if (fn == BDF_LIST_REMOVE) {
+        ColOwner keep(c);
+        TRY(bool_zeroed(c, x.n, keep.out()));
+        cudaError_t e = cudaSuccess;
+        {
+            LaunchTimer t(c, BDF_K_LIST, kBool, x.n, x.n * dtype_width(l->dtype) + x.n / 4);
+            int64_t elem0 = 0;
+            for (size_t i = 0; i < l->lens.size() && e == cudaSuccess; i++) {
+                const DevChunk& ch = l->values->chunks[i];
+                e = launch_list_remove_mask(l->dtype, ch.values, ch.validity, ch.bit_off, ch.len, elem0, bits, (const uint32_t*)x.inlist->chunks[0].values,
+                                            (uint32_t*)keep->chunks[0].values, c->s_compute);
+                elem0 += ch.len;
+            }
+        }
+        if (e != cudaSuccess) return fail_cuda(e, "array_remove");
+        return list_keep(c, x, keep.get(), l->dtype, N, out);
+    }
+    if (fn == BDF_LIST_DISTINCT) {
+        ColOwner keep(c);
+        TRY(list_mark(c, x, 0, 0, keep.out()));
+        return list_keep(c, x, keep.get(), l->dtype, N, out);
+    }
+    if (fn == BDF_LIST_SORT) {
+        // elements of null lists have a null first key and sort after all others: the first K sorted rows are the result
+        int64_t K = 0;
+        for (int64_t v : l->valid_elems) K += v;
+        const bdf_sort_key keys[2] = {{x.keyed.get(), 0}, {x.child.get(), 0}};
+        ColOwner perm(c), head(c), kp(c);
+        TRY(sort_indices_dev(c, 2, keys, perm.out()));
+        DevChunk pc = perm->chunks[0];
+        pc.len = K;
+        TRY(col_borrow(BDF_U32, {pc}, head.out()));
+        TRY(take_dev(c, x.parent.get(), head.get(), kp.out()));
+        return list_result(c, l->dtype, x.child.get(), head.get(), kp.get(), N, 1, out);
+    }
+    // REPEAT
+    ColOwner rows(c), kp(c), src(c);
+    TRY(filter_dev(c, x.iota.get(), x.inlist.get(), rows.out()));
+    TRY(filter_dev(c, x.parent.get(), x.inlist.get(), kp.out()));
+    const int64_t K = rows->total_len;
+    if (K > 0 && count >= kListMaxChunkElems / K)
+        return fail(BDF_UNSUPPORTED, "array_repeat: a result of 2^31 or more elements (one chunk of Int32 offsets)");
+    const int64_t n_out = K * count;
+    Scratch<int32_t> base;
+    CK(base.alloc(c, (size_t)(N + 1) * 4));
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n_out, false}}, nullptr, 0, src.out()));
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_LIST, BDF_U32, n_out, 8 * n_out + 8 * (N + 1));
+        e = launch_list_offsets(K ? (const uint32_t*)kp->chunks[0].values : nullptr, K, N, 1, base, c->s_compute);
+        if (e == cudaSuccess)
+            e = launch_list_repeat(base, N, count, K ? (const uint32_t*)rows->chunks[0].values : nullptr, n_out, (uint32_t*)src->chunks[0].values, c->s_compute);
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, src.get());
+    if (e != cudaSuccess) return fail_cuda(e, "array_repeat");
+    // the offsets of the result are count x those of the kept elements
+    return list_result(c, l->dtype, x.child.get(), src.get(), kp.get(), N, count, out);
+}
+
+static int list_same_shape(const bdf_list* a, const bdf_list* b) {
+    if (a->dtype != b->dtype) return fail(BDF_UNSUPPORTED, "the two lists have different element types");
+    if (a->lens.size() != b->lens.size()) return fail(BDF_LENGTH_MISMATCH, "Expected array a and b to have the same length");
+    for (size_t i = 0; i < a->lens.size(); i++)
+        if (a->lens[i] != b->lens[i]) return fail(BDF_LENGTH_MISMATCH, "Expected array a and b to have the same length");
+    return BDF_OK;
+}
+
+static int list_set(bdf_ctx* c, int fn, const bdf_list* a, const bdf_list* b, bdf_list** out) {
+    if (fn < BDF_LIST_EXCEPT || fn > BDF_LIST_UNION) return fail(BDF_INVALID, "unknown list set function %d", fn);
+    TRY(list_same_shape(a, b));
+    if (a->values->total_len + b->values->total_len >= kListMaxCallElems)
+        return fail(BDF_UNSUPPORTED, "a list call holds 2^32 or more elements (the sort's UInt32 row numbers)");
+    ListElems x(c);
+    ColOwner keep(c);
+    if (fn == BDF_LIST_UNION) {   // a then b: a group's head is its first appearance in a ++ b
+        TRY(list_elems(c, {a, b}, {nullptr, a}, &x));
+        TRY(list_mark(c, x, 0, 0, keep.out()));
+        // kept elements in element order are a's, then b's: a stable sort by list number puts every list's a part before its b part
+        ColOwner rows(c), kp(c), q(c), rows2(c), kp2(c);
+        TRY(filter_dev(c, x.iota.get(), keep.get(), rows.out()));
+        TRY(filter_dev(c, x.parent.get(), keep.get(), kp.out()));
+        const bdf_sort_key key{kp.get(), 0};
+        TRY(sort_indices_dev(c, 1, &key, q.out()));
+        TRY(take_dev(c, rows.get(), q.get(), rows2.out()));
+        TRY(take_dev(c, kp.get(), q.get(), kp2.out()));
+        return list_result(c, a->dtype, x.child.get(), rows2.get(), kp2.get(), a->total_len, 1, out);
+    }
+    // b then a: a group is [b elements][a elements], so its first a element tells whether b has the value
+    TRY(list_elems(c, {b, a}, {nullptr, nullptr}, &x));
+    TRY(list_mark(c, x, b->values->total_len, fn == BDF_LIST_EXCEPT ? 1 : 2, keep.out()));
+    return list_keep(c, x, keep.get(), a->dtype, a->total_len, out);
+}
+
+static int list_explode(bdf_ctx* c, const bdf_list* l, bdf_col** rows_out, bdf_col** values_out) {
+    ListElems x(c);
+    TRY(list_elems(c, {l}, {nullptr}, &x));
+    ColOwner rows(c), pos(c), values(c);
+    TRY(filter_dev(c, x.parent.get(), x.inlist.get(), rows.out()));
+    TRY(filter_dev(c, x.iota.get(), x.inlist.get(), pos.out()));
+    TRY(take_dev(c, x.child.get(), pos.get(), values.out()));
+    *rows_out = rows.release();
+    *values_out = values.release();
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // C ABI
 
 #define ENTER(ctx)                                                   \
@@ -4896,6 +5396,81 @@ int bdf_generate(bdf_ctx* c, int dtype, int kind, double lo, double hi, uint64_t
     }
     *out = o;
     return BDF_OK;
+}
+
+
+// ---- list columns ------------------------------------------------------------------------------
+
+#define LIST_ENTER(ctx)                                                                                                   \
+    if ((ctx) && (ctx)->fleet) return fail(BDF_UNSUPPORTED, "list columns live on one GPU: use a one-GPU context (bdf_init) for them"); \
+    ENTER(ctx)
+
+int bdf_list_upload(bdf_ctx* c, int child_dtype, int64_t n_chunks, const bdf_list_view* in, int flags, bdf_list** out) {
+    LIST_ENTER(c);
+    if (!out || n_chunks < 0 || (n_chunks && !in)) return fail(BDF_INVALID, "bad arguments");
+    return list_upload(c, child_dtype, n_chunks, in, (flags & BDF_ASYNC) != 0, out);
+}
+
+int bdf_list_describe(const bdf_list* l, int32_t* child_dtype, int64_t* n_chunks, int64_t* total_len) {
+    if (!l) return fail(BDF_INVALID, "null list");
+    if (child_dtype) *child_dtype = l->dtype;
+    if (n_chunks) *n_chunks = (int64_t)l->lens.size();
+    if (total_len) *total_len = l->total_len;
+    return BDF_OK;
+}
+
+int bdf_list_chunk_info(bdf_ctx* c, const bdf_list* l, int64_t chunk, int64_t* len, int64_t* null_count, int64_t* n_elements) {
+    LIST_ENTER(c);
+    if (!l || chunk < 0 || chunk >= (int64_t)l->lens.size()) return fail(BDF_INVALID, "bad chunk index");
+    if (len) *len = l->lens[chunk];
+    if (null_count) *null_count = l->null_counts[chunk];
+    if (n_elements) *n_elements = l->values->chunks[chunk].len;
+    return BDF_OK;
+}
+
+int bdf_list_download(bdf_ctx* c, const bdf_list* l, bdf_list_out* out) {
+    LIST_ENTER(c);
+    if (!l || (!out && !l->lens.empty())) return fail(BDF_INVALID, "null argument");
+    return list_download(c, l, out);
+}
+
+const bdf_col* bdf_list_values(const bdf_list* l) { return l ? l->values : nullptr; }
+
+void bdf_list_free(bdf_ctx* c, bdf_list* l) {
+    if (!c || !l || c->fleet) return;
+    std::lock_guard<std::mutex> lock(c->mu);
+    cudaSetDevice(c->device);
+    list_release(c, l);
+}
+
+int bdf_list_find_dev(bdf_ctx* c, int fn, const bdf_list* l, uint64_t value_bits, bdf_col** out) {
+    LIST_ENTER(c);
+    if (!l || !out) return fail(BDF_INVALID, "null argument");
+    return list_find(c, fn, l, value_bits, out);
+}
+
+int bdf_list_reduce_dev(bdf_ctx* c, int fn, const bdf_list* l, bdf_col** out) {
+    LIST_ENTER(c);
+    if (!l || !out) return fail(BDF_INVALID, "null argument");
+    return list_reduce(c, fn, l, out);
+}
+
+int bdf_list_transform_dev(bdf_ctx* c, int fn, const bdf_list* l, uint64_t value_bits, int64_t count, bdf_list** out) {
+    LIST_ENTER(c);
+    if (!l || !out) return fail(BDF_INVALID, "null argument");
+    return list_transform(c, fn, l, value_bits, count, out);
+}
+
+int bdf_list_set_dev(bdf_ctx* c, int fn, const bdf_list* a, const bdf_list* b, bdf_list** out) {
+    LIST_ENTER(c);
+    if (!a || !b || !out) return fail(BDF_INVALID, "null argument");
+    return list_set(c, fn, a, b, out);
+}
+
+int bdf_list_explode_dev(bdf_ctx* c, const bdf_list* l, bdf_col** rows, bdf_col** values) {
+    LIST_ENTER(c);
+    if (!l || !rows || !values) return fail(BDF_INVALID, "null argument");
+    return list_explode(c, l, rows, values);
 }
 
 }  // extern "C"

@@ -760,3 +760,230 @@ class AggFuture:
                 self.handle = None
         except Exception:
             pass
+
+
+# ---------------------------------------------------------------------------------------------------
+# list columns (ArrayFunctions, src/functions/array.rs; rules in include/b200df.h "list columns")
+
+
+def _value_bits(dtype: int, value) -> int:
+    """T::Native of the list's element type in the low bytes of a u64 (bdf_window_call.default_bits)."""
+    return int(np.array([value], dtype=NP_DTYPES[dtype]).view(f"u{width_of(dtype)}")[0])
+
+
+class ListColumn:
+    """A ``List<T>`` column in HBM: per chunk the list validity, rebased Int32 offsets and the elements, which are an ordinary
+    ``Column`` (``values``)."""
+
+    def __init__(self, ctx: N.Context, handle: C.c_void_p):
+        self.ctx = ctx
+        self.handle = handle
+
+    @classmethod
+    def upload(cls, arrays: Sequence, ctx: Optional[N.Context] = None, dtype: Optional[int] = None) -> "ListColumn":
+        ctx = ctx or N.default_context()
+        if dtype is None:
+            if not arrays:
+                raise ValueError("empty list column: the element type cannot be inferred; pass at least one chunk")
+            dtype = arrays[0].dtype
+        views = (N.ListView * max(len(arrays), 1))()
+        for i, a in enumerate(arrays):
+            if a.dtype != dtype:
+                raise N.UnsupportedType("list chunks of different element types")
+            views[i].offsets = a.offsets.ctypes.data
+            views[i].validity = a.validity.ctypes.data if a.validity is not None else None
+            views[i].len = a.length
+            views[i].offset = a.offset
+            views[i].null_count = a.null_count
+            views[i].values = N.make_views([a.values])[0]
+        h = C.c_void_p()
+        N.raise_for_status(N.lib().bdf_list_upload(ctx.handle, dtype, len(arrays), views, 0, C.byref(h)))
+        return cls(ctx, h)
+
+    def describe(self):
+        dt, n, total = C.c_int32(), C.c_int64(), C.c_int64()
+        N.raise_for_status(N.lib().bdf_list_describe(self.handle, C.byref(dt), C.byref(n), C.byref(total)))
+        return dt.value, n.value, total.value
+
+    @property
+    def dtype(self) -> int:
+        return self.describe()[0]
+
+    @property
+    def n_chunks(self) -> int:
+        return self.describe()[1]
+
+    def __len__(self) -> int:
+        return self.describe()[2]
+
+    def chunk_info(self, i: int) -> dict:
+        ln, nc, ne = C.c_int64(), C.c_int64(), C.c_int64()
+        N.raise_for_status(N.lib().bdf_list_chunk_info(self.ctx.handle, self.handle, i, C.byref(ln), C.byref(nc), C.byref(ne)))
+        return {"len": ln.value, "null_count": nc.value, "n_elements": ne.value}
+
+    def values(self) -> "Column":
+        """The elements as a Column (borrowed: valid while this list lives; freeing it does nothing)."""
+        col = _BorrowedColumn(self.ctx, C.c_void_p(N.lib().bdf_list_values(self.handle)))
+        col._owner = self
+        return col
+
+    def download(self) -> List:
+        from .arrays import ListArray
+
+        dtype, n, _ = self.describe()
+        outs = (N.ListOut * max(n, 1))()
+        keep = []
+        for i in range(n):
+            info = self.chunk_info(i)
+            ln, ne = info["len"], info["n_elements"]
+            off = np.zeros(ln + 1, dtype=np.int32)
+            val = np.zeros((ln + 7) // 8 + 1, dtype=np.uint8)
+            vals = np.zeros(ne, dtype=NP_DTYPES[dtype])
+            vval = np.zeros((ne + 7) // 8 + 1, dtype=np.uint8)
+            outs[i].offsets, outs[i].validity = off.ctypes.data, val.ctypes.data
+            outs[i].values = vals.ctypes.data if ne else None
+            outs[i].value_validity = vval.ctypes.data
+            keep.append((off, val, vals, vval))
+        N.raise_for_status(N.lib().bdf_list_download(self.ctx.handle, self.handle, outs))
+        res = []
+        for i, (off, val, vals, vval) in enumerate(keep):
+            child = PrimitiveArray(dtype, vals, vval if outs[i].has_value_validity else None, 0, vals.shape[0],
+                                   int(outs[i].value_null_count))
+            res.append(ListArray(dtype, off, val if outs[i].has_validity else None, 0, off.shape[0] - 1, int(outs[i].null_count), child))
+        return res
+
+    # -- ArrayFunctions on the device --
+    def _col(self, fn, *args) -> "Column":
+        h = C.c_void_p()
+        N.raise_for_status(fn(self.ctx.handle, *args, C.byref(h)))
+        return Column(self.ctx, h)
+
+    def _list(self, fn, *args) -> "ListColumn":
+        h = C.c_void_p()
+        N.raise_for_status(fn(self.ctx.handle, *args, C.byref(h)))
+        return ListColumn(self.ctx, h)
+
+    def array_contains(self, value) -> "Column":
+        return self._col(N.lib().bdf_list_find_dev, N.LIST_CONTAINS, self.handle, _value_bits(self.dtype, value))
+
+    def array_position(self, value) -> "Column":
+        return self._col(N.lib().bdf_list_find_dev, N.LIST_POSITION, self.handle, _value_bits(self.dtype, value))
+
+    def array_max(self) -> "Column":
+        return self._col(N.lib().bdf_list_reduce_dev, N.LIST_MAX, self.handle)
+
+    def array_min(self) -> "Column":
+        return self._col(N.lib().bdf_list_reduce_dev, N.LIST_MIN, self.handle)
+
+    def size(self) -> "Column":
+        return self._col(N.lib().bdf_list_reduce_dev, N.LIST_SIZE, self.handle)
+
+    def array_remove(self, value) -> "ListColumn":
+        return self._list(N.lib().bdf_list_transform_dev, N.LIST_REMOVE, self.handle, _value_bits(self.dtype, value), 0)
+
+    def array_sort(self) -> "ListColumn":
+        return self._list(N.lib().bdf_list_transform_dev, N.LIST_SORT, self.handle, 0, 0)
+
+    def array_distinct(self) -> "ListColumn":
+        return self._list(N.lib().bdf_list_transform_dev, N.LIST_DISTINCT, self.handle, 0, 0)
+
+    def array_repeat(self, count: int) -> "ListColumn":
+        return self._list(N.lib().bdf_list_transform_dev, N.LIST_REPEAT, self.handle, 0, int(count))
+
+    def array_except(self, other: "ListColumn") -> "ListColumn":
+        return self._list(N.lib().bdf_list_set_dev, N.LIST_EXCEPT, self.handle, other.handle)
+
+    def array_intersect(self, other: "ListColumn") -> "ListColumn":
+        return self._list(N.lib().bdf_list_set_dev, N.LIST_INTERSECT, self.handle, other.handle)
+
+    def array_union(self, other: "ListColumn") -> "ListColumn":
+        return self._list(N.lib().bdf_list_set_dev, N.LIST_UNION, self.handle, other.handle)
+
+    def explode(self):
+        """(UInt32 parent row numbers, values): one row per element of every valid list; null and empty lists give none."""
+        rows, vals = C.c_void_p(), C.c_void_p()
+        N.raise_for_status(N.lib().bdf_list_explode_dev(self.ctx.handle, self.handle, C.byref(rows), C.byref(vals)))
+        return Column(self.ctx, rows), Column(self.ctx, vals)
+
+    def free(self):
+        if self.handle is not None and self.ctx.handle:
+            N.lib().bdf_list_free(self.ctx.handle, self.handle)
+        self.handle = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+class _BorrowedColumn(Column):
+    """A Column whose memory belongs to a ListColumn."""
+
+    def free(self):
+        self.handle = None
+
+
+def _as_list_column(x, ctx) -> ListColumn:
+    return x if isinstance(x, ListColumn) else ListColumn.upload(list(x), ctx)
+
+
+class ArrayFunctions:
+    """ArrayFunctions (src/functions/array.rs) plus Spark's size / explode, one device call each.  Arguments are the column's
+    ListArray chunks (or a ListColumn); list results come back as ListArray chunks, the others as PrimitiveArray /
+    BooleanArray chunks."""
+
+    @staticmethod
+    def _run(arrays, ctx, fn):
+        ctx = ctx or N.default_context()
+        lc = _as_list_column(arrays, ctx)
+        out = fn(lc)
+        return out.download()
+
+    @staticmethod
+    def array_contains(arrays, value, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.array_contains(value))
+
+    @staticmethod
+    def array_position(arrays, value, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.array_position(value))
+
+    @staticmethod
+    def array_max(arrays, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.array_max())
+
+    @staticmethod
+    def array_min(arrays, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.array_min())
+
+    @staticmethod
+    def size(arrays, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.size())
+
+    @staticmethod
+    def array_remove(arrays, value, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.array_remove(value))
+
+    @staticmethod
+    def array_sort(arrays, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.array_sort())
+
+    @staticmethod
+    def array_distinct(arrays, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.array_distinct())
+
+    @staticmethod
+    def array_repeat(arrays, count: int, ctx=None): return ArrayFunctions._run(arrays, ctx, lambda l: l.array_repeat(count))
+
+    @staticmethod
+    def _set(a, b, ctx, name):
+        ctx = ctx or N.default_context()
+        la, lb = _as_list_column(a, ctx), _as_list_column(b, ctx)
+        return getattr(la, name)(lb).download()
+
+    @staticmethod
+    def array_except(a, b, ctx=None): return ArrayFunctions._set(a, b, ctx, "array_except")
+
+    @staticmethod
+    def array_intersect(a, b, ctx=None): return ArrayFunctions._set(a, b, ctx, "array_intersect")
+
+    @staticmethod
+    def array_union(a, b, ctx=None): return ArrayFunctions._set(a, b, ctx, "array_union")
+
+    @staticmethod
+    def explode(arrays, ctx=None):
+        ctx = ctx or N.default_context()
+        rows, vals = _as_list_column(arrays, ctx).explode()
+        return rows.download()[0], vals.download()[0]

@@ -33,6 +33,13 @@ class IpcFile:
             name, dt, nl = C.c_char_p(), C.c_int32(), C.c_int32()
             N.raise_for_status(N.lib().bdf_ipc_column(self.handle, i, C.byref(name), C.byref(dt), C.byref(nl)))
             self.schema.append((name.value.decode("utf-8", "replace"), dt.value, bool(nl.value)))
+        # List<T> columns keep dtype -1 in `schema` (outside the column path); their BDF_LIST_BASE + T codes are here
+        self.list_columns = {}
+        for i in range(self.num_columns):
+            ld = C.c_int32()
+            N.raise_for_status(N.lib().bdf_ipc_list_column(self.handle, i, C.byref(ld)))
+            if ld.value >= 0:
+                self.list_columns[self.schema[i][0]] = ld.value
 
     # -- lifetime --
     def close(self) -> None:
@@ -93,12 +100,23 @@ class IpcFile:
              batches: Optional[Sequence[int]] = None) -> Dict[str, "object"]:
         """The chosen columns (default: every column of a type on the path) as device Columns, one chunk per RecordBatch.
         ``batches`` restricts the read to those RecordBatches (one rank's share: ``parallel.shard_indices``)."""
-        from .functions import Column
+        from .functions import Column, ListColumn
 
         if columns is None:
             idx = [i for i, (_, dt, _) in enumerate(self.schema) if dt >= 0]
         else:
             idx = [self.column_index(c) for c in columns]
+            lists = [i for i in idx if self.schema[i][0] in self.list_columns]
+            if lists:   # List<T> columns come back as ListColumns, one chunk per RecordBatch
+                if batches is not None:
+                    raise N.UnsupportedType("list columns are read whole (every RecordBatch)")
+                ctx = ctx or N.default_context()
+                res = self.read([i for i in idx if i not in lists], ctx, asynchronous) if len(lists) < len(idx) else {}
+                for i in lists:
+                    h = C.c_void_p()
+                    N.raise_for_status(N.lib().bdf_ipc_read_list(ctx.handle, self.handle, i, 0, C.byref(h)))
+                    res[self.schema[i][0]] = ListColumn(ctx, h)
+                return {self.schema[i][0]: res[self.schema[i][0]] for i in idx}
         if not idx:   # no column of a type on the path: an empty frame, not BDF_INVALID from the C side
             return {}
         ctx = ctx or N.default_context()
