@@ -10,6 +10,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --stats [--rows 100000000]                       # only the statistical-aggregate rows
     python benchmarks/kernels_bench.py --csv-write [--csv-rows 50000000]                # the CSV writer rows (the reader's table written back)
     python benchmarks/kernels_bench.py --lists [--rows 100000000]                       # the list-function rows (ArrayFunctions)
+    python benchmarks/kernels_bench.py --temporal [--rows 100000000]                    # the date / timestamp function rows
 """
 from __future__ import annotations
 
@@ -335,8 +336,9 @@ def stats_bench(ctx, lens, report, rows_out):
         col.free()
 
 
-def _stream_read_rate(rows):
-    """The read-only HBM rate of benchmarks/tune_stream.cu (best read-only sum), built into a temporary directory and run here."""
+def _stream_rates(rows):
+    """The HBM rates of benchmarks/tune_stream.cu (best of each class), built into a temporary directory and run here:
+    {"read": read-only sum, "copy": copy 1 read + 1 write} in GB/s."""
     import re
     import subprocess
 
@@ -346,8 +348,8 @@ def _stream_read_rate(rows):
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
         subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", src, "-o", exe], check=True, capture_output=True)
         out = subprocess.run([exe, str(rows)], check=True, capture_output=True, text=True).stdout
-    m = re.search(r"CEILING read-only ([0-9.]+) GB/s", out)
-    return float(m.group(1))
+    m = re.search(r"CEILING read-only ([0-9.]+) GB/s, copy 1R1W ([0-9.]+) GB/s", out)
+    return {"read": float(m.group(1)), "copy": float(m.group(2))}
 
 
 def _card():
@@ -379,7 +381,7 @@ def lists_bench(ctx, rows, rows_out):
     [1, 2 * mean - 1]: no empty list, so max / min are defined), plus one hot list of rows / 10 elements among about rows one-element lists.
     Algorithmic bytes: offsets and elements read once, plus what is written."""
     card = _card()
-    stream = _stream_read_rate(rows)
+    stream = _stream_rates(rows)["read"]
     print(f"card: {card}; tune_stream read-only rate {stream:.1f} GB/s", flush=True)
     rows_out.append({"case": "tune_stream read-only", "GBs": stream, "card": card})
     rng = np.random.default_rng(20261015)
@@ -427,6 +429,51 @@ def lists_bench(ctx, rows, rows_out):
             c.free()
 
 
+def temporal_bench(ctx, rows, rows_out):
+    """Date / timestamp functions over rows values in 25 chunks: Timestamp(us) spread over 1900..2100 with 10 % nulls, and Date32 (the
+    to_date of it).  Each row: the median of three calls (after a warm-up) of the summed per-launch CUDA-event records, its GB/s at the
+    algorithmic bytes (values in + values out + the bitmaps read and written) and the fraction of tune_stream's copy rate."""
+    card = _card()
+    copy = _stream_rates(rows)["copy"]
+    print(f"card: {card}; tune_stream copy (1R1W) rate {copy:.1f} GB/s", flush=True)
+    rows_out.append({"case": "tune_stream copy 1R1W", "GBs": copy, "card": card})
+    n_chunks = 25
+    per = rows // n_chunks
+    lo, hi = -2208988800 * 10 ** 6, 4102444800 * 10 ** 6   # 1900-01-01 .. 2100-01-01 in microseconds
+    rng = np.random.default_rng(20261016)
+    chunks = []
+    for _ in range(n_chunks):
+        v = rng.integers(lo, hi, per)
+        chunks.append(rdf.PrimitiveArray.from_numpy(v, rng.random(per) >= 0.1))
+    T = rdf.TemporalType
+    ts = rdf.Column.upload(chunks, ctx).with_temporal(T.timestamp("us"))
+    del chunks
+    d32 = ts.to_date()
+    # distinct second operands for the two-column rows (a column paired with itself would read its second side from cache)
+    ts2 = ts.date_trunc("hour")   # Timestamp(us)
+    d32b = ts2.add_months(1)      # Date32
+    assert ts2.dtype == rdf.I64 and ts2.temporal == T.timestamp("us") and d32b.dtype == rdf.I32 and d32b.temporal == T.date32()
+    N_ = len(ts)
+    bm = N_ / 8
+    cases = [("year Timestamp(us) -> Int32", lambda: ts.year(), N_ * (8 + 4) + 2 * bm),
+             ("day_of_week Timestamp(us) -> Int32", lambda: ts.day_of_week(), N_ * (8 + 4) + 2 * bm),
+             ("hour Timestamp(us) -> Int32", lambda: ts.hour(), N_ * (8 + 4) + 2 * bm),
+             ("date_trunc(day) Timestamp(us)", lambda: ts.date_trunc("day"), N_ * (8 + 8) + 2 * bm),
+             ("to_date Timestamp(us) -> Date32", lambda: ts.to_date(), N_ * (8 + 4) + 2 * bm),
+             ("add_months(1) Timestamp(us) -> Date32", lambda: ts.add_months(1), N_ * (8 + 4) + 2 * bm),
+             ("year Date32 -> Int32", lambda: d32.year(), N_ * (4 + 4) + 2 * bm),
+             ("day_of_week Date32 -> Int32", lambda: d32.day_of_week(), N_ * (4 + 4) + 2 * bm),
+             ("add_months(1) Date32", lambda: d32.add_months(1), N_ * (4 + 4) + 2 * bm),
+             ("months_between(Timestamp(us), Timestamp(us))", lambda: ts.months_between(ts2), N_ * (8 + 8 + 8) + 3 * bm),
+             ("months_between(Date32, Date32)", lambda: d32.months_between(d32b), N_ * (4 + 4 + 8) + 3 * bm)]
+    for name, fn, b in cases:
+        ms, out = _timed_calls(ctx, fn)
+        gbs = b / ms / 1e6
+        rows_out.append({"case": name, "ms": ms, "rows": N_, "bytes": b, "GBs": gbs, "frac_of_copy": gbs / copy, "card": card})
+        print(f"{name:48s} {ms:9.3f} ms {gbs:8.1f} GB/s  {gbs / copy:5.3f} of copy rate", flush=True)
+        del out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
@@ -438,8 +485,16 @@ def main():
     ap.add_argument("--stats", action="store_true", help="run only the statistical-aggregate rows (moments, group variance, count_distinct)")
     ap.add_argument("--csv-write", action="store_true", help="run only the CSV writer rows")
     ap.add_argument("--lists", action="store_true", help="run only the list-function rows (ArrayFunctions)")
+    ap.add_argument("--temporal", action="store_true", help="run only the date / timestamp function rows")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.temporal:
+        rows_out = []
+        temporal_bench(ctx, args.rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"results": rows_out}, f, indent=1)
+        return
     if args.lists:
         rows_out = []
         lists_bench(ctx, args.rows, rows_out)

@@ -654,6 +654,99 @@ int  bdf_list_explode_dev(bdf_ctx* ctx, const bdf_list* list, bdf_col** rows, bd
 int  bdf_ipc_list_column(const bdf_ipc* file, int32_t col, int32_t* dtype);
 int  bdf_ipc_read_list(bdf_ctx* ctx, const bdf_ipc* file, int32_t col, int flags, bdf_list** out);
 
+/* ---- dates and timestamps (ScalarFunctions::hour, src/functions/scalar.rs:267-273 -> arrow compute::hour; the Spark date functions
+ * that are empty stubs in the same file: add_months, date_add, date_sub, date_trunc, date_diff, day_of_month, day_of_week, day_of_year,
+ * last_day, minute, month, months_between, next_day, quarter, second, to_date, unix_timestamp, year ...) ----------------------------------
+ * Types.  A temporal column is an ORDINARY bdf_col of its physical dtype; a bdf_temporal_type travels beside it (no new bdf_dtype), so
+ *   sort, group-by, join, window, take, filter and min / max work on temporal columns unchanged:
+ *     Date32     BDF_I32  days since 1970-01-01 (unit ignored)      Date64     BDF_I64  milliseconds (unit BDF_MILLISECOND)
+ *     Timestamp  BDF_I64  in its unit (any), tz optional             Time32     BDF_I32  time of day, s or ms
+ *     Time64     BDF_I64  time of day, us or ns
+ *   Any other (kind, unit), or a column whose physical dtype does not match its type -> BDF_INVALID.  "Date kinds" below = Date32,
+ *   Date64 and Timestamp; "time kinds" = Time32 and Time64.
+ * Calendar.  Proleptic Gregorian, no leap seconds.  A value v of a date kind is split by FLOOR division into days = floor(v / units_per_day)
+ *   and a time of day 0 <= tod < units_per_day (so -1 us is 1969-12-31T23:59:59.999999).  Definition, not parity: old arrow versions
+ *   truncated toward zero here (recalled).  Civil fields come from days by Hinnant's civil_from_days (PAPERS.md).
+ * Range.  The dates of chrono's NaiveDate, years -262144 ..= 262143 (days -96465658 ..= 95026601), where arrow's value_as_datetime gives
+ *   None.  A date outside it gives NULL: the date a function reads (the local date for the civil functions, the UTC date for
+ *   UNIX_TIMESTAMP and TO_TIMESTAMP) and a computed result date alike.  A result that does not fit its output type is NULL too (a
+ *   Timestamp(s) in year 3000 converted to ns; date_trunc(year) of a ns value in 1677 whose year start is below i64::MIN).  A Time32 /
+ *   Time64 value outside [0, one day) gives NULL for HOUR / MINUTE / SECOND.  Otherwise a result slot is valid iff its input slot is (the
+ *   two-column functions: iff both are).  Every result carries a validity bitmap (its null count may be 0).
+ * Time zones.  Values are UTC instants.  The functions that read civil fields apply a Timestamp's tz when it is NULL, "UTC", "Z" or
+ *   "+00:00" (no shift) or a fixed offset "+HH:MM" / "-HH:MM" (HH 00..23, MM 00..59): local time = instant + offset, and DATE_TRUNC turns
+ *   the truncated local time back into an instant (local - offset).  Any other tz string -- a named zone such as "Europe/Paris" --
+ *   gives BDF_UNSUPPORTED there: there is no tz database on the device, and UTC fields would be silently wrong.  UNIX_TIMESTAMP and
+ *   TO_TIMESTAMP keep instants and accept any tz.  (Departure: the arrow of the reference's era ignored tz.)
+ * Functions (bdf_temporal_fn; "arg" is the int64_t argument, ignored where the table has none):
+ *   YEAR, QUARTER (1..4), MONTH (1..12), DAY_OF_MONTH, DAY_OF_YEAR (1..366)   date kinds -> Int32: the civil fields.
+ *   DAY_OF_WEEK      date kinds -> Int32, Spark's numbering: 1 = Sunday .. 7 = Saturday.
+ *   HOUR, MINUTE, SECOND   date and time kinds -> Int32 of the (local) time of day; Date32 gives 0 (arrow's hour goes through midnight);
+ *                    SECOND has no fraction.
+ *   TO_DATE          date kinds -> Date32: the civil date.
+ *   DATE_ADD / DATE_SUB   date kinds, arg = days in Int32 range -> Date32: to_date(x) + arg / - arg.
+ *   ADD_MONTHS       date kinds, arg = months in Int32 range -> Date32, SPARK 2.4's rule: the target month is (year, month) + arg; if the
+ *                    start day is the last day of its month, or lies past the end of the target month, the result is the target month's
+ *                    last day, else the same day.  So 2019-02-28 + 1 = 2019-03-31 and 2016-08-31 + 1 = 2016-09-30.  Spark 3 dropped the
+ *                    first half of this rule (2019-02-28 + 1 = 2019-03-28 there).
+ *   LAST_DAY         date kinds -> Date32: the last day of the month.
+ *   NEXT_DAY         date kinds, arg = day of week 1..7 (Spark numbering) -> Date32: the first date strictly after to_date(x) with that
+ *                    weekday.  arg outside 1..7 -> BDF_INVALID (a constant here, not Spark's per-row string that gives NULL).
+ *   DATE_TRUNC       date kinds, arg = bdf_trunc_unit -> the input's type (Timestamp: unit and tz kept): floor in local time to the start
+ *                    of the year / quarter / month / week (Monday) / day / hour / minute / second.  Date32 with a unit below DAY returns
+ *                    x.  Time kinds -> BDF_UNSUPPORTED.
+ *   UNIX_TIMESTAMP   date kinds -> Int64: floor seconds since the epoch (Date32: days x 86400).
+ *   TO_TIMESTAMP     date kinds, arg = target bdf_time_unit -> Timestamp(arg, tz of a Timestamp input, else NULL): the same instant,
+ *                    floor-divided when the target unit is coarser.
+ *   A time kind with any function but HOUR / MINUTE / SECOND -> BDF_UNSUPPORTED.
+ * Two-column functions (bdf_temporal_binary_fn): a and b may be different date kinds; each side's tz rules apply.
+ *   DATE_DIFF(end = a, start = b)  -> Int32: days(to_date(a)) - days(to_date(b)), Spark's datediff.
+ *   MONTHS_BETWEEN(t1 = a, t2 = b) -> Float64, Spark 2.4 with roundOff = true, in exactly this IEEE double sequence (no FMA):
+ *                    monthDiff = (double)((y1 * 12 + m1) - (y2 * 12 + m2)); if d1 == d2 or both are the last day of their month: monthDiff;
+ *                    else secDiff = (double)((d1 - d2) * 86400 + (s1 - s2)) with s the whole seconds of the local time of day (0 for
+ *                    Date32), diff = monthDiff + secDiff / 2678400.0, t = diff * 1e8, k = floor(t), k += 1 if t - k >= 0.5 (Java 8's
+ *                    Math.round, ties toward +inf), result k / 1e8.  ('1997-02-28 10:30:00', '1996-10-30') = 3.94959677.
+ * Results are deterministic and bit-exact: integer arithmetic, plus the one double sequence above.
+ * Comparison.  bdf_compare_dev goes through Float64: exact for Date32 / Time32 values (and for to_date / unix_timestamp results within
+ *   +-2^53), not for Date64 / Timestamp / Time64 instants.  The Python layer therefore refuses compare on a column tagged with a 64-bit
+ *   temporal type (a departure from refusing every tagged column: a date-range filter on to_date() needs it).
+ * Parity unpinned: the reference pins none of this (no test of hour; the stubs have no body).  arrow's and chrono's behaviour and Spark
+ *   2.4's rules and documentation examples are RECALLED.
+ * Chunks.  bdf_temporal / bdf_temporal_dev keep the input's chunks (as bdf_unary); bdf_temporal_binary_dev zips chunks as bdf_binary_dev
+ *   (BDF_LENGTH_MISMATCH on unequal chunk lengths).  All three accept a multi-GPU context and return the one-GPU bits.
+ * Errors (nothing is returned and nothing leaks): a null pointer, an unknown function, an invalid type, a wrong physical dtype or a bad arg
+ *   -> BDF_INVALID; a function the kind does not have or a named tz -> BDF_UNSUPPORTED. */
+typedef enum { BDF_TEMPORAL_NONE = 0, BDF_DATE32, BDF_DATE64, BDF_TIMESTAMP, BDF_TIME32, BDF_TIME64 } bdf_temporal_kind;
+typedef enum { BDF_SECOND = 0, BDF_MILLISECOND, BDF_MICROSECOND, BDF_NANOSECOND } bdf_time_unit;   /* arrow TimeUnit order */
+typedef struct { int32_t kind; int32_t unit; const char* tz; /* Timestamp only; NULL = none */ } bdf_temporal_type;
+typedef enum {
+    BDF_TEMPORAL_YEAR = 0, BDF_TEMPORAL_QUARTER, BDF_TEMPORAL_MONTH, BDF_TEMPORAL_DAY_OF_MONTH, BDF_TEMPORAL_DAY_OF_YEAR, BDF_TEMPORAL_DAY_OF_WEEK,
+    BDF_TEMPORAL_HOUR, BDF_TEMPORAL_MINUTE, BDF_TEMPORAL_SECOND, BDF_TEMPORAL_TO_DATE, BDF_TEMPORAL_DATE_ADD, BDF_TEMPORAL_DATE_SUB,
+    BDF_TEMPORAL_ADD_MONTHS, BDF_TEMPORAL_LAST_DAY, BDF_TEMPORAL_NEXT_DAY, BDF_TEMPORAL_DATE_TRUNC, BDF_TEMPORAL_UNIX_TIMESTAMP,
+    BDF_TEMPORAL_TO_TIMESTAMP, BDF_NTEMPORAL
+} bdf_temporal_fn;
+typedef enum { BDF_TEMPORAL_DATE_DIFF = 0, BDF_TEMPORAL_MONTHS_BETWEEN } bdf_temporal_binary_fn;
+typedef enum { BDF_TRUNC_YEAR = 0, BDF_TRUNC_QUARTER, BDF_TRUNC_MONTH, BDF_TRUNC_WEEK, BDF_TRUNC_DAY, BDF_TRUNC_HOUR, BDF_TRUNC_MINUTE,
+               BDF_TRUNC_SECOND } bdf_trunc_unit;
+/* host in / host out: the drop-in body of ScalarFunctions::hour<T>(Vec<&PrimitiveArray<T>>) -> Vec<Int32Array> and of the stubs.  `out`
+ * holds the result's dtype (bdf_temporal_result). */
+int  bdf_temporal(bdf_ctx* ctx, int fn, const bdf_temporal_type* type, int64_t arg, int64_t n_chunks, const bdf_view* in, bdf_out* out);
+int  bdf_temporal_dev(bdf_ctx* ctx, int fn, const bdf_temporal_type* type, int64_t arg, const bdf_col* in, bdf_col** out);
+int  bdf_temporal_binary_dev(bdf_ctx* ctx, int fn, const bdf_temporal_type* ta, const bdf_col* a, const bdf_temporal_type* tb, const bdf_col* b,
+                             bdf_col** out);
+/* No context, no GPU: validates (fn, type, arg) exactly as the entries do and reports the result's dtype and temporal type (kind 0 for a
+ * plain Int32 / Int64 result; out_type->tz points at type->tz). */
+int  bdf_temporal_result(int fn, const bdf_temporal_type* type, int64_t arg, int32_t* out_dtype, bdf_temporal_type* out_type);
+/* Temporal columns of an IPC file.  bdf_ipc_column keeps reporting Date / Time / Timestamp columns with dtype -1 (as List columns);
+ * bdf_ipc_temporal_column gives the type (kind 0 for any other column, or for a Date / Time field whose unit and width do not form a
+ * valid type); tz points into the open file.  bdf_ipc_read_temporal uploads one such column, one chunk per RecordBatch, its buffers
+ * checked at read time.  bdf_ipc_write_typed is bdf_ipc_write with a type per column (kind 0: as the column's dtype; types == NULL:
+ * all kind 0); it writes the Date / Time / Timestamp field types, tz included.  Duration, Interval and Decimal stay outside the path. */
+int  bdf_ipc_temporal_column(const bdf_ipc* file, int32_t col, bdf_temporal_type* out);
+int  bdf_ipc_read_temporal(bdf_ctx* ctx, const bdf_ipc* file, int32_t col, int flags, bdf_col** out);
+int  bdf_ipc_write_typed(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
+                         const bdf_temporal_type* types /* n_cols entries, or NULL */);
+
 /* ---- measurement support ------------------------------------------------------------------------ */
 /* Per-launch CUDA-event timing on the library's compute stream (the stream the kernels run on). */
 typedef struct {
@@ -663,7 +756,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

@@ -234,6 +234,38 @@ extern "C" {
     pub fn bdf_ipc_list_column(file: *const BdfIpc, col: i32, dtype: *mut i32) -> c_int;
     pub fn bdf_ipc_read_list(ctx: *mut BdfCtx, file: *const BdfIpc, col: i32, flags: c_int, out: *mut *mut BdfList) -> c_int;
     pub fn bdf_ipc_write(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol) -> c_int;
+    // dates and timestamps (include/b200df.h "dates and timestamps")
+    pub fn bdf_temporal(ctx: *mut BdfCtx, func: c_int, ty: *const BdfTemporalType, arg: i64, n: i64, input: *const BdfView, out: *mut BdfOut) -> c_int;
+    pub fn bdf_temporal_dev(ctx: *mut BdfCtx, func: c_int, ty: *const BdfTemporalType, arg: i64, input: *const BdfCol, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_temporal_binary_dev(ctx: *mut BdfCtx, func: c_int, ta: *const BdfTemporalType, a: *const BdfCol, tb: *const BdfTemporalType,
+                                   b: *const BdfCol, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_temporal_result(func: c_int, ty: *const BdfTemporalType, arg: i64, out_dtype: *mut i32, out_type: *mut BdfTemporalType) -> c_int;
+    pub fn bdf_ipc_temporal_column(file: *const BdfIpc, col: i32, out: *mut BdfTemporalType) -> c_int;
+    pub fn bdf_ipc_read_temporal(ctx: *mut BdfCtx, file: *const BdfIpc, col: i32, flags: c_int, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_ipc_write_typed(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol,
+                               types: *const BdfTemporalType) -> c_int;
+}
+
+/// bdf_temporal_type: kind (0 none, 1 Date32, 2 Date64, 3 Timestamp, 4 Time32, 5 Time64), unit (arrow TimeUnit order), tz (Timestamp).
+#[repr(C)]
+pub struct BdfTemporalType { pub kind: i32, pub unit: i32, pub tz: *const c_char }
+
+/// The bdf_temporal_type of an arrow DataType (None for a non-temporal type).  The tz string must outlive the call: the caller keeps
+/// the CString.
+pub fn temporal_type(t: &DataType, tz_keep: &mut Option<std::ffi::CString>) -> Option<BdfTemporalType> {
+    use arrow::datatypes::{DateUnit, TimeUnit};
+    let unit = |u: &TimeUnit| match u { TimeUnit::Second => 0, TimeUnit::Millisecond => 1, TimeUnit::Microsecond => 2, TimeUnit::Nanosecond => 3 };
+    match t {
+        DataType::Date32(DateUnit::Day) => Some(BdfTemporalType { kind: 1, unit: 0, tz: std::ptr::null() }),
+        DataType::Date64(DateUnit::Millisecond) => Some(BdfTemporalType { kind: 2, unit: 1, tz: std::ptr::null() }),
+        DataType::Timestamp(u, tz) => {
+            *tz_keep = tz.as_ref().map(|s| std::ffi::CString::new(s.as_str()).unwrap());
+            Some(BdfTemporalType { kind: 3, unit: unit(u), tz: tz_keep.as_ref().map_or(std::ptr::null(), |c| c.as_ptr()) })
+        }
+        DataType::Time32(u) => Some(BdfTemporalType { kind: 4, unit: unit(u), tz: std::ptr::null() }),
+        DataType::Time64(u) => Some(BdfTemporalType { kind: 5, unit: unit(u), tz: std::ptr::null() }),
+        _ => None,
+    }
 }
 
 /// Process-wide context.  A plain process gets ONE context over every GPU of the box (`bdf_init_multi(0, ..)`: the library

@@ -4,7 +4,7 @@ use std::sync::Arc;
 
 use arrow::array::{Array, ArrayData, PrimitiveArray};
 use arrow::buffer::MutableBuffer;
-use arrow::datatypes::ArrowNumericType;
+use arrow::datatypes::{ArrowNumericType, ArrowPrimitiveType, DataType, DateUnit, TimeUnit};
 use arrow::error::ArrowError;
 
 use crate::ffi::*;
@@ -34,7 +34,7 @@ pub fn gpu_unary<T: ArrowNumericType>(op: c_int, array: Vec<&PrimitiveArray<T>>)
     Ok(finish::<T>(vals, bits, &outs))
 }
 
-fn alloc_outputs<T: ArrowNumericType>(lens: &[usize]) -> (Vec<MutableBuffer>, Vec<MutableBuffer>, Vec<BdfOut>) {
+fn alloc_outputs<T: ArrowPrimitiveType>(lens: &[usize]) -> (Vec<MutableBuffer>, Vec<MutableBuffer>, Vec<BdfOut>) {
     let width = std::mem::size_of::<T::Native>();
     // Both buffers get their FINAL length before the call (zero-filled once, as arrow's own kernels do with `with_bitset`): the
     // library then writes into initialised memory of the right size and nothing has to be resized afterwards -- on arrow
@@ -56,9 +56,80 @@ fn finish<T: ArrowNumericType>(vals: Vec<MutableBuffer>, bits: Vec<MutableBuffer
     }).collect()
 }
 
+/// Dates and timestamps: the temporal function `func` (bdf_temporal_fn: 0 year .. 6 hour .. 17 to_timestamp) over every chunk of a column
+/// whose DataType is Date32 / Date64 / Timestamp / Time32 / Time64; R is the result type bdf_temporal_result reports: Int32Type for the
+/// fields, Date32Type for to_date .. next_day, T for date_trunc, Int64Type for unix_timestamp, the Timestamp*Type of the target unit for
+/// to_timestamp.  The chunks keep their layout: T::Native and R::Native are the physical i32 / i64.  The arrays carry the DataType the
+/// library reports, so a to_timestamp result keeps the input's tz.
+pub fn gpu_temporal<T: ArrowPrimitiveType, R: ArrowPrimitiveType>(func: c_int, arg: i64, array: Vec<&PrimitiveArray<T>>)
+    -> Result<Vec<PrimitiveArray<R>>, ArrowError>
+{
+    let mut tz = None;
+    let ty = temporal_type(&T::get_data_type(), &mut tz)
+        .ok_or_else(|| ArrowError::ComputeError(format!("{:?} is not a date, time or timestamp type", T::get_data_type())))?;
+    let mut dt: i32 = -1;
+    let mut out_ty = BdfTemporalType { kind: 0, unit: 0, tz: std::ptr::null() };
+    let st = unsafe { bdf_temporal_result(func, &ty, arg, &mut dt, &mut out_ty) };
+    if st != BDF_OK { return Err(to_arrow_error(st)); }
+    let result_type = temporal_data_type(&out_ty).unwrap_or_else(R::get_data_type);
+    // R must have the reported physical width and, for a temporal result, the reported kind and unit (the tz comes from the library)
+    let mut keep = None;
+    let same_kind = match (temporal_type(&R::get_data_type(), &mut keep), out_ty.kind) {
+        (None, 0) => true,
+        (Some(r), k) => r.kind == k && r.unit == out_ty.unit,
+        _ => false,
+    };
+    if dt != physical_id(&R::get_data_type()) || !same_kind {
+        return Err(ArrowError::ComputeError(format!("{:?} is not the result type of temporal function {}: {:?}", R::get_data_type(), func, result_type)));
+    }
+    let v: Vec<BdfView> = array.iter().map(|a| view(*a)).collect();
+    let (vals, bits, mut outs) = alloc_outputs::<R>(&array.iter().map(|a| a.len()).collect::<Vec<_>>());
+    let st = unsafe { bdf_temporal(ctx(), func, &ty, arg, v.len() as i64, v.as_ptr(), outs.as_mut_ptr()) };
+    if st != BDF_OK { return Err(to_arrow_error(st)); }
+    Ok(finish_as::<R>(vals, bits, &outs, &result_type))
+}
+
+/// The bdf_dtype of a primitive DataType: numeric types by dtype_id, temporal types by their physical width (Date32 / Time32: Int32).
+fn physical_id(t: &DataType) -> c_int {
+    let mut keep = None;
+    match temporal_type(t, &mut keep) {
+        Some(tt) => if tt.kind == 1 || tt.kind == 4 { 2 } else { 3 },
+        None => dtype_id(t),
+    }
+}
+
+/// The arrow DataType of a bdf_temporal_type (None for kind 0).
+fn temporal_data_type(t: &BdfTemporalType) -> Option<DataType> {
+    let unit = match t.unit { 0 => TimeUnit::Second, 1 => TimeUnit::Millisecond, 2 => TimeUnit::Microsecond, _ => TimeUnit::Nanosecond };
+    match t.kind {
+        1 => Some(DataType::Date32(DateUnit::Day)),
+        2 => Some(DataType::Date64(DateUnit::Millisecond)),
+        3 => {
+            let tz = if t.tz.is_null() { None } else { Some(unsafe { std::ffi::CStr::from_ptr(t.tz) }.to_string_lossy().into_owned()) };
+            Some(DataType::Timestamp(unit, tz.map(Arc::new)))
+        }
+        4 => Some(DataType::Time32(unit)),
+        5 => Some(DataType::Time64(unit)),
+        _ => None,
+    }
+}
+
+fn finish_as<R: ArrowPrimitiveType>(vals: Vec<MutableBuffer>, bits: Vec<MutableBuffer>, outs: &[BdfOut], data_type: &DataType) -> Vec<PrimitiveArray<R>> {
+    outs.iter().zip(vals.into_iter().zip(bits.into_iter())).map(|(o, (v, b))| {
+        let nulls = if o.has_validity != 0 { Some(b.freeze()) } else { None };
+        let data = ArrayData::new(data_type.clone(), o.len as usize, Some(o.null_count as usize), nulls, 0, vec![v.freeze()], vec![]);
+        PrimitiveArray::<R>::from(Arc::new(data))
+    }).collect()
+}
+
 // In src/functions/scalar.rs the bodies become:
 //   pub fn add<T>(left, right)          -> gpu_binary(0, left, right)     // was: left.par_iter().zip(..).map(compute::add)   (scalar.rs:16-32)
 //   pub fn subtract<T>(left, right)     -> gpu_binary(1, left, right)     // (scalar.rs:34-50)
 //   pub fn divide<T>(left, right)       -> gpu_binary(3, left, right)     // Err(ArrowError::DivideByZero) preserved (scalar.rs:51-68)
 //   pub fn multiply / par_multiply<T>   -> gpu_binary(2, left, right)     // (scalar.rs:69-103)
 //   pub fn abs/sin/cos/tan/acos/...<T>  -> gpu_unary(op, array)           // was: scalar_op(a, |a| Ok(num::Float::sin(a)))      (scalar.rs:106-457)
+//   pub fn hour<T>(array) -> Result<Vec<Int32Array>>  -> gpu_temporal::<T, Int32Type>(6, 0, array)   // was: compute::hour per chunk (scalar.rs:267-273)
+//   the stubs: year 0, quarter 1, month 2, day_of_month 3, day_of_year 4, day_of_week 5, minute 7, second 8  -> gpu_temporal::<T, Int32Type>
+//              to_date 9, date_add 10 (arg days), date_sub 11, add_months 12 (arg months), last_day 13, next_day 14 (arg 1..7)
+//                                                                   -> gpu_temporal::<T, Date32Type>
+//              date_trunc 15 (arg bdf_trunc_unit) -> gpu_temporal::<T, T>; unix_timestamp 16 -> Int64Type; to_timestamp 17 -> Timestamp*Type

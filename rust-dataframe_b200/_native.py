@@ -21,9 +21,9 @@ SUM, MIN, MAX, COUNT = range(4)
 OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID, PARSE = range(10)
 ASYNC = 1
 (K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW,
- K_MOMENTS, K_CSV_WRITE, K_LIST) = range(18)
+ K_MOMENTS, K_CSV_WRITE, K_LIST, K_TEMPORAL) = range(19)
 KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
-                "window", "moments", "csv_write", "list"]
+                "window", "moments", "csv_write", "list", "temporal"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -57,6 +57,18 @@ LIST_CONTAINS, LIST_POSITION = range(2)
 LIST_MAX, LIST_MIN, LIST_SIZE = range(3)
 LIST_REMOVE, LIST_SORT, LIST_DISTINCT, LIST_REPEAT = range(4)
 LIST_EXCEPT, LIST_INTERSECT, LIST_UNION = range(3)
+# dates and timestamps (bdf_temporal_*)
+TEMPORAL_NONE, DATE32, DATE64, TIMESTAMP, TIME32, TIME64 = range(6)
+SECOND, MILLISECOND, MICROSECOND, NANOSECOND = range(4)
+(T_YEAR, T_QUARTER, T_MONTH, T_DAY_OF_MONTH, T_DAY_OF_YEAR, T_DAY_OF_WEEK, T_HOUR, T_MINUTE, T_SECOND, T_TO_DATE, T_DATE_ADD, T_DATE_SUB,
+ T_ADD_MONTHS, T_LAST_DAY, T_NEXT_DAY, T_DATE_TRUNC, T_UNIX_TIMESTAMP, T_TO_TIMESTAMP) = range(18)
+TEMPORAL_FNS = {"year": T_YEAR, "quarter": T_QUARTER, "month": T_MONTH, "day_of_month": T_DAY_OF_MONTH, "day_of_year": T_DAY_OF_YEAR,
+                "day_of_week": T_DAY_OF_WEEK, "hour": T_HOUR, "minute": T_MINUTE, "second": T_SECOND, "to_date": T_TO_DATE,
+                "date_add": T_DATE_ADD, "date_sub": T_DATE_SUB, "add_months": T_ADD_MONTHS, "last_day": T_LAST_DAY, "next_day": T_NEXT_DAY,
+                "date_trunc": T_DATE_TRUNC, "unix_timestamp": T_UNIX_TIMESTAMP, "to_timestamp": T_TO_TIMESTAMP}
+T_DATE_DIFF, T_MONTHS_BETWEEN = range(2)
+TRUNC_UNITS = {"year": 0, "quarter": 1, "month": 2, "week": 3, "day": 4, "hour": 5, "minute": 6, "second": 7}
+TIME_UNITS = {"s": SECOND, "ms": MILLISECOND, "us": MICROSECOND, "ns": NANOSECOND}
 
 
 class View(C.Structure):
@@ -101,6 +113,10 @@ class GroupAggC(C.Structure):
 class WindowCall(C.Structure):
     _fields_ = [("function", C.c_int32), ("frame", C.c_int32), ("column", C.c_void_p), ("offset", C.c_int64), ("default_bits", C.c_uint64),
                 ("has_default", C.c_int32)]
+
+
+class TemporalTypeC(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("unit", C.c_int32), ("tz", C.c_char_p)]
 
 
 class ListView(C.Structure):
@@ -272,6 +288,13 @@ def lib() -> C.CDLL:
         "bdf_list_explode_dev": ([vp, vp, P(vp), P(vp)], C.c_int),
         "bdf_ipc_list_column": ([vp, i32, P(i32)], C.c_int),
         "bdf_ipc_read_list": ([vp, vp, i32, C.c_int, P(vp)], C.c_int),
+        "bdf_temporal": ([vp, C.c_int, P(TemporalTypeC), i64, i64, P(View), P(Out)], C.c_int),
+        "bdf_temporal_dev": ([vp, C.c_int, P(TemporalTypeC), i64, vp, P(vp)], C.c_int),
+        "bdf_temporal_binary_dev": ([vp, C.c_int, P(TemporalTypeC), vp, P(TemporalTypeC), vp, P(vp)], C.c_int),
+        "bdf_temporal_result": ([C.c_int, P(TemporalTypeC), i64, P(i32), P(TemporalTypeC)], C.c_int),
+        "bdf_ipc_temporal_column": ([vp, i32, P(TemporalTypeC)], C.c_int),
+        "bdf_ipc_read_temporal": ([vp, vp, i32, C.c_int, P(vp)], C.c_int),
+        "bdf_ipc_write_typed": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(TemporalTypeC)], C.c_int),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError if the library does not export a declared symbol
@@ -300,6 +323,8 @@ EXPORTED_SYMBOLS = [
     "bdf_list_upload", "bdf_list_describe", "bdf_list_chunk_info", "bdf_list_download", "bdf_list_values", "bdf_list_free",
     "bdf_list_find_dev", "bdf_list_reduce_dev", "bdf_list_transform_dev", "bdf_list_set_dev", "bdf_list_explode_dev",
     "bdf_ipc_list_column", "bdf_ipc_read_list",
+    "bdf_temporal", "bdf_temporal_dev", "bdf_temporal_binary_dev", "bdf_temporal_result", "bdf_ipc_temporal_column", "bdf_ipc_read_temporal",
+    "bdf_ipc_write_typed",
 ]
 
 

@@ -36,10 +36,93 @@ def pack_validity(mask: np.ndarray) -> np.ndarray:
     return np.packbits(np.asarray(mask, dtype=bool), bitorder="little")
 
 
-class PrimitiveArray:
-    """One chunk of a column: Arrow layout over numpy buffers."""
+DATE32, DATE64, TIMESTAMP, TIME32, TIME64 = range(1, 6)   # bdf_temporal_kind
+_UNITS = {"s": 0, "ms": 1, "us": 2, "ns": 3}
+_UNIT_NAMES = ["s", "ms", "us", "ns"]
+_KIND_NAMES = {DATE32: "date32", DATE64: "date64", TIMESTAMP: "timestamp", TIME32: "time32", TIME64: "time64"}
 
-    __slots__ = ("dtype", "values", "validity", "offset", "length", "null_count", "_keepalive")
+
+class TemporalType:
+    """bdf_temporal_type: the Arrow temporal type a column of physical Int32 / Int64 values carries (include/b200df.h "dates and
+    timestamps").  ``unit`` is an arrow TimeUnit (0 = s .. 3 = ns, or "s" / "ms" / "us" / "ns"); ``tz`` only for timestamps."""
+
+    __slots__ = ("kind", "unit", "tz")
+
+    def __init__(self, kind: int, unit=0, tz: Optional[str] = None):
+        self.kind = int(kind)
+        self.unit = _UNITS[unit] if isinstance(unit, str) else int(unit)
+        self.tz = tz
+
+    @classmethod
+    def date32(cls): return cls(DATE32)
+
+    @classmethod
+    def date64(cls): return cls(DATE64, "ms")
+
+    @classmethod
+    def timestamp(cls, unit="us", tz: Optional[str] = None): return cls(TIMESTAMP, unit, tz)
+
+    @classmethod
+    def time32(cls, unit="s"): return cls(TIME32, unit)
+
+    @classmethod
+    def time64(cls, unit="us"): return cls(TIME64, unit)
+
+    @property
+    def dtype(self) -> int:
+        """The physical dtype of the values (Int32 for Date32 / Time32, else Int64)."""
+        return I32 if self.kind in (DATE32, TIME32) else I64
+
+    def to_arrow(self):
+        import pyarrow as pa
+
+        u = _UNIT_NAMES[self.unit] if 0 <= self.unit < 4 else "s"
+        if self.kind == DATE32:
+            return pa.date32()
+        if self.kind == DATE64:
+            return pa.date64()
+        if self.kind == TIMESTAMP:
+            return pa.timestamp(u, tz=self.tz)
+        if self.kind == TIME32:
+            return pa.time32(u)
+        return pa.time64(u)
+
+    @classmethod
+    def from_arrow(cls, typ) -> Optional["TemporalType"]:
+        """The TemporalType of a pyarrow DataType, or None for a type that is not Date / Time / Timestamp."""
+        import pyarrow as pa
+
+        if pa.types.is_date32(typ):
+            return cls(DATE32)
+        if pa.types.is_date64(typ):
+            return cls(DATE64, "ms")
+        if pa.types.is_timestamp(typ):
+            return cls(TIMESTAMP, typ.unit, typ.tz)
+        if pa.types.is_time32(typ):
+            return cls(TIME32, typ.unit)
+        if pa.types.is_time64(typ):
+            return cls(TIME64, typ.unit)
+        return None
+
+    def __eq__(self, other) -> bool:
+        return isinstance(other, TemporalType) and (self.kind, self.unit, self.tz) == (other.kind, other.unit, other.tz)
+
+    def __hash__(self) -> int:
+        return hash((self.kind, self.unit, self.tz))
+
+    def __repr__(self) -> str:
+        name = _KIND_NAMES.get(self.kind, str(self.kind))
+        if self.kind == DATE32:
+            return "TemporalType(date32)"
+        tz = f", tz={self.tz!r}" if self.tz is not None else ""
+        return f"TemporalType({name}, {_UNIT_NAMES[self.unit] if 0 <= self.unit < 4 else self.unit}{tz})"
+
+
+class PrimitiveArray:
+    """One chunk of a column: Arrow layout over numpy buffers.  ``temporal`` (a TemporalType or None) says that the Int32 / Int64
+    values are dates, times or timestamps."""
+
+    __slots__ = ("dtype", "values", "validity", "offset", "length", "null_count", "_keepalive", "temporal")
 
     def __init__(self, dtype: int, values: np.ndarray, validity: Optional[np.ndarray] = None, offset: int = 0,
                  length: Optional[int] = None, null_count: int = -1, keepalive=None):
@@ -59,6 +142,7 @@ class PrimitiveArray:
             raise ValueError("validity bitmap too short")
         self.null_count = 0 if self.validity is None else int(null_count)
         self._keepalive = keepalive
+        self.temporal = None
 
     # ---- constructors ------------------------------------------------------------------------------
     @classmethod
@@ -86,20 +170,22 @@ class PrimitiveArray:
         """Zero-copy view of a pyarrow primitive array (offset and validity preserved)."""
         import pyarrow as pa
 
-        np_dt = np.dtype(arr.type.to_pandas_dtype())
+        temporal = TemporalType.from_arrow(arr.type)
+        np_dt = NP_DTYPES[temporal.dtype] if temporal is not None else np.dtype(arr.type.to_pandas_dtype())
         dtype = dtype_of(np_dt)
         vbuf, dbuf = arr.buffers()
         n_total = arr.offset + len(arr)
         values = (np.frombuffer(dbuf, dtype=np_dt, count=n_total) if dbuf is not None and n_total
                   else np.zeros(n_total, dtype=np_dt))
         validity = np.frombuffer(vbuf, dtype=np.uint8) if vbuf is not None else None
-        return cls(dtype, values, validity, arr.offset, len(arr), arr.null_count if vbuf is not None else 0,
-                   keepalive=arr)
+        out = cls(dtype, values, validity, arr.offset, len(arr), arr.null_count if vbuf is not None else 0, keepalive=arr)
+        out.temporal = temporal
+        return out
 
     def to_arrow(self):
         import pyarrow as pa
 
-        typ = pa.from_numpy_dtype(NP_DTYPES[self.dtype])
+        typ = self.temporal.to_arrow() if self.temporal is not None else pa.from_numpy_dtype(NP_DTYPES[self.dtype])
         vbuf = pa.py_buffer(self.validity) if self.validity is not None else None
         return pa.Array.from_buffers(typ, self.length, [vbuf, pa.py_buffer(self.values)],
                                      null_count=self.null_count if self.validity is not None else 0,
@@ -144,8 +230,9 @@ class PrimitiveArray:
         """Zero-copy slice (ArrayData::slice): shares buffers, moves the offset."""
         if offset < 0 or length < 0 or offset + length > self.length:
             raise ValueError("slice out of bounds")
-        return PrimitiveArray(self.dtype, self.values, self.validity, self.offset + offset, length, -1,
-                              keepalive=self._keepalive)
+        out = PrimitiveArray(self.dtype, self.values, self.validity, self.offset + offset, length, -1, keepalive=self._keepalive)
+        out.temporal = self.temporal
+        return out
 
     def to_pylist(self) -> List:
         m = self.valid_mask()

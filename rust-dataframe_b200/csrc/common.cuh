@@ -313,4 +313,28 @@ cudaError_t launch_generate(int dtype, int kind, double lo, double hi, uint64_t 
                             uint32_t* d_warp_counts, cudaStream_t s);
 cudaError_t launch_fill(void* p, size_t bytes, int sm_count, cudaStream_t s);
 
+// Dates and timestamps (k_temporal.cu).  Storage unit of a temporal input: days (Date32) or seconds .. nanoseconds.
+enum : int { TC_DAYS = 0, TC_S, TC_MS, TC_US, TC_NS };
+struct TemporalParams {
+    int32_t fn;          // bdf_temporal_fn
+    int32_t aux;         // DATE_TRUNC: bdf_trunc_unit; NEXT_DAY: weekday 1..7 (Spark numbering)
+    int32_t time_kind;   // the input is Time32 / Time64 (a time of day)
+    int32_t pad;
+    int64_t arg;         // DATE_ADD / DATE_SUB days, ADD_MONTHS months
+    int64_t off;         // fixed tz offset in input units (civil functions), |off| < one day
+    int64_t mul, div;    // TO_TIMESTAMP: v * mul (overflow -> NULL) when div == 1, else floor(v / div)
+};
+struct TemporalParams2 {
+    int32_t fn;          // bdf_temporal_binary_fn
+    int32_t cfg_a, cfg_b;
+    int32_t pad;
+    int64_t off_a, off_b;
+};
+int elems_per_tile_temporal(int in_dtype, int out_dtype);
+int elems_per_tile_temporal2(int a_dtype, int b_dtype, int out_dtype);
+cudaError_t launch_temporal(int cfg, int in_dtype, int out_dtype, const TemporalParams& p, const UnDesc* d_descs, int n_chunks,
+                            int64_t total_tiles, uint32_t* d_warp_counts, cudaStream_t s);
+cudaError_t launch_temporal2(int a_dtype, int b_dtype, int out_dtype, const TemporalParams2& p, const BinDesc* d_descs, int n_chunks,
+                             int64_t total_tiles, uint32_t* d_warp_counts, cudaStream_t s);
+
 }  // namespace bdf

@@ -106,6 +106,11 @@ struct IpcField {
     std::string name;
     int dtype = -1;       // bdf_dtype, BDF_BOOL, or -1: a type outside the path
     int list_child = -1;  // a List<T> of one numeric T (dtype stays -1: bdf_ipc_list_column / bdf_ipc_read_list): T
+    // a Date / Time / Timestamp field that forms a valid bdf_temporal_type (dtype stays -1: bdf_ipc_temporal_column /
+    // bdf_ipc_read_temporal): its kind, unit, tz and physical dtype
+    int temporal_kind = 0, temporal_unit = 0, temporal_dtype = -1;
+    bool has_tz = false;
+    std::string tz;
     bool nullable = false;
     int64_t n_nodes = 0, n_buffers = 0;   // what the field (with its children) occupies in every RecordBatch
 };
@@ -147,7 +152,35 @@ bool parse_field(const FbTable& f, IpcField* out, int depth, int64_t* budget, st
             break;
         }
         case T_Bool: own = 2; out->dtype = BDF_BOOL; break;
-        case T_Decimal: case T_Date: case T_Time: case T_Timestamp: case T_Interval: case T_FixedSizeBinary: case T_Duration: own = 2; break;
+        case T_Date: {   // Schema.fbs: Date { unit: DateUnit = MILLISECOND }, DAY = 0
+            own = 2;
+            const int unit = has_ty ? ty.scalar<int16_t>(0, 1) : 1;
+            if (unit == 0) { out->temporal_kind = BDF_DATE32; out->temporal_dtype = BDF_I32; }
+            if (unit == 1) { out->temporal_kind = BDF_DATE64; out->temporal_unit = BDF_MILLISECOND; out->temporal_dtype = BDF_I64; }
+            break;
+        }
+        case T_Time: {   // Time { unit: TimeUnit = MILLISECOND; bitWidth: int = 32 }
+            own = 2;
+            const int unit = has_ty ? ty.scalar<int16_t>(0, 1) : 1;
+            const int bw = has_ty ? ty.scalar<int32_t>(1, 32) : 32;
+            if (bw == 32 && (unit == BDF_SECOND || unit == BDF_MILLISECOND)) { out->temporal_kind = BDF_TIME32; out->temporal_dtype = BDF_I32; }
+            if (bw == 64 && (unit == BDF_MICROSECOND || unit == BDF_NANOSECOND)) { out->temporal_kind = BDF_TIME64; out->temporal_dtype = BDF_I64; }
+            out->temporal_unit = out->temporal_kind ? unit : 0;
+            break;
+        }
+        case T_Timestamp: {   // Timestamp { unit: TimeUnit; timezone: string }
+            own = 2;
+            const int unit = has_ty ? ty.scalar<int16_t>(0, 0) : 0;
+            // a timezone string that does not decode leaves the field stepped over (kind 0): the file still opens, as it did before
+            // temporal columns were read
+            const bool tz_ok = !(has_ty && ty.field(1)) || ty.str(1, &out->tz);
+            if (unit >= BDF_SECOND && unit <= BDF_NANOSECOND && tz_ok) {
+                out->temporal_kind = BDF_TIMESTAMP; out->temporal_unit = unit; out->temporal_dtype = BDF_I64;
+                out->has_tz = has_ty && ty.field(1) != 0;
+            }
+            break;
+        }
+        case T_Decimal: case T_Interval: case T_FixedSizeBinary: case T_Duration: own = 2; break;
         case T_Binary: case T_Utf8: case T_LargeBinary: case T_LargeUtf8: own = 3; break;
         case T_List: case T_LargeList: case T_Map: own = 2; nested = true; break;
         case T_Struct: case T_FixedSizeList: own = 1; nested = true; break;
@@ -293,13 +326,14 @@ int bdf_ipc_open(const char* path, bdf_ipc** out) {
         size_t ni = 0, bi = 0;
         for (size_t c = 0; c < f->fields.size(); c++) {
             const IpcField& fld = f->fields[c];
-            if (fld.dtype >= 0 || fld.list_child >= 0) {
+            if (fld.dtype >= 0 || fld.list_child >= 0 || fld.temporal_kind) {
                 IpcColChunk& cc = b.cols[c];
                 mb.rd(nfirst + 16 * ni, &cc.len); mb.rd(nfirst + 16 * ni + 8, &cc.null_count);
                 mb.rd(bufirst + 16 * bi, &cc.validity.off); mb.rd(bufirst + 16 * bi + 8, &cc.validity.len);
                 mb.rd(bufirst + 16 * (bi + 1), &cc.values.off); mb.rd(bufirst + 16 * (bi + 1) + 8, &cc.values.len);
                 int64_t need = cc.len > 0 ? (cc.len + 1) * 4 : 0;   // a list's offsets (a list array without lists may have none)
                 if (fld.dtype >= 0) dtype_bytes(fld.dtype, cc.len, &need);
+                if (fld.temporal_kind) dtype_bytes(fld.temporal_dtype, cc.len, &need);
                 const bool has_v = cc.null_count > 0;
                 // offsets and lengths come from the file: compare each with what is left of the body (off + len may wrap)
                 auto fits = [body_len](const IpcBuf& bf, int64_t min_len) {
@@ -307,8 +341,8 @@ int bdf_ipc_open(const char* path, bdf_ipc** out) {
                 };
                 const bool ok = cc.len == b.rows && cc.null_count >= 0 && cc.null_count <= cc.len && fits(cc.values, need) &&
                                 (!has_v || fits(cc.validity, (cc.len + 7) / 8));
-                // a List column is only checked for bdf_ipc_read_list: a file whose list column that reader cannot use still opens
-                if (!ok && fld.list_child < 0)
+                // a List or temporal column is only checked when it is read: a file whose such column that reader cannot use still opens
+                if (!ok && fld.dtype >= 0)
                     return ipc_fail(BDF_INVALID, "record batch %u, column '%s': buffers do not fit the batch", k, fld.name.c_str());
                 cc.list_ok = ok;
                 if (fld.list_child >= 0 && ok) {   // the child's node and buffers follow the list's
@@ -415,6 +449,31 @@ int bdf_ipc_list_column(const bdf_ipc* f, int32_t col, int32_t* dtype) {
     return BDF_OK;
 }
 
+int bdf_ipc_temporal_column(const bdf_ipc* f, int32_t col, bdf_temporal_type* out) {
+    if (!f || !out || col < 0 || (size_t)col >= f->fields.size()) return ipc_fail(BDF_INVALID, "column index out of range");
+    const IpcField& fld = f->fields[col];
+    *out = bdf_temporal_type{fld.temporal_kind, fld.temporal_unit, fld.has_tz ? fld.tz.c_str() : nullptr};
+    return BDF_OK;
+}
+
+int bdf_ipc_read_temporal(bdf_ctx* ctx, const bdf_ipc* f, int32_t col, int flags, bdf_col** out) {
+    if (!ctx || !f || !out) return ipc_fail(BDF_INVALID, "null argument");
+    if (col < 0 || (size_t)col >= f->fields.size()) return ipc_fail(BDF_INVALID, "column index out of range");
+    const IpcField& fld = f->fields[col];
+    if (!fld.temporal_kind) return ipc_fail(BDF_UNSUPPORTED, "column '%s' is not a Date, Time or Timestamp column", fld.name.c_str());
+    std::vector<bdf_view> views(std::max<size_t>(f->batches.size(), 1));
+    for (size_t b = 0; b < f->batches.size(); b++) {
+        const IpcBatch& bt = f->batches[b];
+        const IpcColChunk& c = bt.cols[col];
+        if (!c.list_ok) return ipc_fail(BDF_INVALID, "record batch %zu, column '%s': buffers do not fit the batch", b, fld.name.c_str());
+        views[b] = bdf_view{f->map + bt.body + c.values.off, c.null_count > 0 ? f->map + bt.body + c.validity.off : nullptr, c.len, 0, c.null_count};
+    }
+    const int32_t dt = fld.temporal_dtype;
+    const int64_t nch = (int64_t)f->batches.size();
+    const bdf_view* vp = views.data();
+    return bdf_upload_many(ctx, 1, &dt, &nch, &vp, flags, out);
+}
+
 int bdf_ipc_read(bdf_ctx* ctx, const bdf_ipc* f, int32_t n_cols, const int32_t* cols, int flags, bdf_col** out) {
     if (!f) return ipc_fail(BDF_INVALID, "null argument");
     std::vector<int64_t> all(f->batches.size());
@@ -488,7 +547,7 @@ size_t fb_struct_vec(FbOut& o, const void* data, uint32_t count, size_t elem) { 
 }
 
 // Schema table (fields of primitive / boolean type) at the current end of `o`; returns its position.
-size_t fb_schema(FbOut& o, int n_cols, const char* const* names, const int32_t* dtypes) {
+size_t fb_schema(FbOut& o, int n_cols, const char* const* names, const int32_t* dtypes, const bdf_temporal_type* types) {
     std::vector<size_t> refs;
     const size_t schema = fb_table(o, {{1, 0, 0}}, &refs);
     o.pad_to(4);
@@ -499,7 +558,11 @@ size_t fb_schema(FbOut& o, int n_cols, const char* const* names, const int32_t* 
     o.b.resize(slots + 4 * (size_t)n_cols, 0);
     for (int c = 0; c < n_cols; c++) {
         const int dt = dtypes[c];
-        const uint8_t tt = dt == BDF_BOOL ? T_Bool : (dt == BDF_F32 || dt == BDF_F64) ? T_FloatingPoint : T_Int;
+        const int kind = types ? types[c].kind : 0;
+        uint8_t tt = dt == BDF_BOOL ? T_Bool : (dt == BDF_F32 || dt == BDF_F64) ? T_FloatingPoint : T_Int;
+        if (kind == BDF_DATE32 || kind == BDF_DATE64) tt = T_Date;
+        if (kind == BDF_TIME32 || kind == BDF_TIME64) tt = T_Time;
+        if (kind == BDF_TIMESTAMP) tt = T_Timestamp;
         std::vector<size_t> fr;
         // Field: name(0) nullable(1) type_type(2) type(3) children(5)
         const size_t field = fb_table(o, {{0, 0, 0}, {1, 1, 1}, {2, 1, tt}, {3, 0, 0}, {5, 0, 0}}, &fr);
@@ -507,6 +570,15 @@ size_t fb_schema(FbOut& o, int n_cols, const char* const* names, const int32_t* 
         o.link(fr[0], fb_string(o, names[c]));
         size_t ty;
         if (tt == T_Bool) ty = fb_table(o, {}, nullptr);
+        else if (tt == T_Date) ty = fb_table(o, {{0, 2, (uint64_t)(kind == BDF_DATE32 ? 0 : 1)}}, nullptr);
+        else if (tt == T_Time) ty = fb_table(o, {{0, 2, (uint64_t)types[c].unit}, {1, 4, (uint64_t)(kind == BDF_TIME32 ? 32 : 64)}}, nullptr);
+        else if (tt == T_Timestamp) {
+            std::vector<size_t> tr;
+            if (types[c].tz) {
+                ty = fb_table(o, {{0, 2, (uint64_t)types[c].unit}, {1, 0, 0}}, &tr);
+                o.link(tr[0], fb_string(o, types[c].tz));
+            } else ty = fb_table(o, {{0, 2, (uint64_t)types[c].unit}}, nullptr);
+        }
         else if (tt == T_FloatingPoint) ty = fb_table(o, {{0, 2, (uint64_t)(dt == BDF_F32 ? 1 : 2)}}, nullptr);
         else {
             static const int bw[8] = {8, 16, 32, 64, 8, 16, 32, 64};
@@ -571,8 +643,8 @@ void frame_message(FilePlan* plan, int64_t* pos, const FbOut& fb, int32_t* meta_
     *pos = after;
 }
 
-void plan_file(int n_cols, const char* const* names, const int32_t* dtypes, int64_t n_batches, std::vector<std::vector<ChunkSpec>>& spec,
-               FilePlan* plan) {
+void plan_file(int n_cols, const char* const* names, const int32_t* dtypes, const bdf_temporal_type* types, int64_t n_batches,
+               std::vector<std::vector<ChunkSpec>>& spec, FilePlan* plan) {
     int64_t pos = 0;
     plan->meta.push_back({0, {'A', 'R', 'R', 'O', 'W', '1', 0, 0}});
     pos = 8;
@@ -582,7 +654,7 @@ void plan_file(int n_cols, const char* const* names, const int32_t* dtypes, int6
         std::vector<size_t> refs;
         const size_t msg = fb_table(fb, {{0, 2, 4 /* MetadataVersion::V5 */}, {1, 1, 1 /* Schema */}, {2, 0, 0}, {3, 8, 0}}, &refs);
         fb.link(0, msg);
-        fb.link(refs[0], fb_schema(fb, n_cols, names, dtypes));
+        fb.link(refs[0], fb_schema(fb, n_cols, names, dtypes, types));
         fb.pad_to(8);
         int32_t ml;
         frame_message(plan, &pos, fb, &ml);
@@ -629,7 +701,7 @@ void plan_file(int n_cols, const char* const* names, const int32_t* dtypes, int6
     std::vector<size_t> fr;
     const size_t footer = fb_table(fb, {{0, 2, 4}, {1, 0, 0}, {2, 0, 0}, {3, 0, 0}}, &fr);   // version, schema, dictionaries, recordBatches
     fb.link(0, footer);
-    fb.link(fr[0], fb_schema(fb, n_cols, names, dtypes));
+    fb.link(fr[0], fb_schema(fb, n_cols, names, dtypes, types));
     fb.link(fr[1], fb_struct_vec(fb, nullptr, 0, 24));
     fb.link(fr[2], fb_struct_vec(fb, blocks.data(), (uint32_t)blocks.size(), 24));
     fb.pad_to(8);
@@ -710,7 +782,7 @@ int bdf_ipc_write_host(const char* path, int32_t n_cols, const char* const* name
         }
     }
     FilePlan plan;
-    plan_file(n_cols, names, dtypes, n_batches, spec, &plan);
+    plan_file(n_cols, names, dtypes, nullptr, n_batches, spec, &plan);
     OutFile of;
     const int st = of.open_planned(path, plan);
     if (st != BDF_OK) return st;
@@ -728,6 +800,11 @@ int bdf_ipc_write_host(const char* path, int32_t n_cols, const char* const* name
 }
 
 int bdf_ipc_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols) {
+    return bdf_ipc_write_typed(ctx, path, n_cols, names, cols, nullptr);
+}
+
+int bdf_ipc_write_typed(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
+                        const bdf_temporal_type* types) {
     if (!ctx || !path || !names || !cols || n_cols <= 0) return ipc_fail(BDF_INVALID, "null argument");
     std::vector<int32_t> dtypes((size_t)n_cols);
     std::vector<std::vector<ChunkSpec>> spec((size_t)n_cols);
@@ -737,6 +814,14 @@ int bdf_ipc_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* co
         if (!cols[c] || !names[c]) return ipc_fail(BDF_INVALID, "null column or name");
         int st = bdf_col_describe(cols[c], &dtypes[c], &nch, &total);
         if (st != BDF_OK) return st;
+        if (types && types[c].kind) {   // the same validation as the temporal functions' (bdf_temporal_result)
+            int32_t rd = 0;
+            st = bdf_temporal_result(BDF_TEMPORAL_UNIX_TIMESTAMP, &types[c], 0, &rd, nullptr);
+            if (st == BDF_UNSUPPORTED) st = bdf_temporal_result(BDF_TEMPORAL_HOUR, &types[c], 0, &rd, nullptr);   // time kinds
+            if (st != BDF_OK) return st;
+            const int phys = (types[c].kind == BDF_DATE32 || types[c].kind == BDF_TIME32) ? BDF_I32 : BDF_I64;
+            if (dtypes[c] != phys) return ipc_fail(BDF_INVALID, "column '%s' of dtype %d does not hold temporal kind %d", names[c], dtypes[c], types[c].kind);
+        }
         if (n_batches < 0) n_batches = nch;
         if (nch != n_batches) return ipc_fail(BDF_LENGTH_MISMATCH, "columns have different numbers of chunks (%lld, %lld)", (long long)nch, (long long)n_batches);
         spec[c].resize((size_t)nch);
@@ -751,7 +836,7 @@ int bdf_ipc_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* co
         }
     }
     FilePlan plan;
-    plan_file(n_cols, names, dtypes.data(), n_batches, spec, &plan);
+    plan_file(n_cols, names, dtypes.data(), types, n_batches, spec, &plan);
     OutFile of;
     int st = of.open_planned(path, plan);
     if (st != BDF_OK) return st;

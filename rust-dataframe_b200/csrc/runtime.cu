@@ -1049,6 +1049,210 @@ static int map_dev(bdf_ctx* c, bool is_cast, int op_or_to, const bdf_col* in, bd
     return BDF_OK;
 }
 
+// ---- dates and timestamps (k_temporal.cu; the rules are stated in include/b200df.h) ----------------------------------------------
+
+static int64_t temporal_per_sec(int cfg) { return cfg == TC_MS ? 1000LL : cfg == TC_US ? 1000000LL : cfg == TC_NS ? 1000000000LL : 1LL; }
+
+// A valid (kind, unit) -> its physical dtype and storage unit; anything else is BDF_INVALID.
+static int temporal_storage(const bdf_temporal_type* t, int* dtype, int* cfg) {
+    const int u = t->unit;
+    switch (t->kind) {
+        case BDF_DATE32: *dtype = BDF_I32; *cfg = TC_DAYS; return BDF_OK;
+        case BDF_DATE64: if (u == BDF_MILLISECOND) { *dtype = BDF_I64; *cfg = TC_MS; return BDF_OK; } break;
+        case BDF_TIMESTAMP: if (u >= BDF_SECOND && u <= BDF_NANOSECOND) { *dtype = BDF_I64; *cfg = TC_S + u; return BDF_OK; } break;
+        case BDF_TIME32: if (u == BDF_SECOND || u == BDF_MILLISECOND) { *dtype = BDF_I32; *cfg = TC_S + u; return BDF_OK; } break;
+        case BDF_TIME64: if (u == BDF_MICROSECOND || u == BDF_NANOSECOND) { *dtype = BDF_I64; *cfg = TC_S + u; return BDF_OK; } break;
+        default: return fail(BDF_INVALID, "unknown temporal kind %d", t->kind);
+    }
+    return fail(BDF_INVALID, "temporal kind %d does not take time unit %d", t->kind, u);
+}
+
+// The fixed offset of a Timestamp's tz in seconds; false for a tz the device cannot apply (a named zone).
+static bool temporal_tz_offset(const char* tz, int64_t* sec) {
+    *sec = 0;
+    if (!tz || !strcmp(tz, "UTC") || !strcmp(tz, "Z")) return true;
+    const auto dig = [](char ch) { return ch >= '0' && ch <= '9'; };
+    if (strlen(tz) != 6 || (tz[0] != '+' && tz[0] != '-') || !dig(tz[1]) || !dig(tz[2]) || tz[3] != ':' || !dig(tz[4]) || !dig(tz[5])) return false;
+    const int hh = (tz[1] - '0') * 10 + (tz[2] - '0'), mm = (tz[4] - '0') * 10 + (tz[5] - '0');
+    if (hh > 23 || mm > 59) return false;
+    *sec = (tz[0] == '-' ? -1 : 1) * (int64_t)(hh * 3600 + mm * 60);
+    return true;
+}
+
+struct TemporalPlan {
+    int in_dtype = 0, cfg = 0, out_dtype = 0;
+    bdf_temporal_type out_type{};
+    TemporalParams p{};
+};
+
+// Validates (fn, type, arg) and plans the launch: what bdf_temporal_result reports and every entry checks first.
+static int temporal_plan(int fn, const bdf_temporal_type* t, int64_t arg, TemporalPlan* pl) {
+    if (!t) return fail(BDF_INVALID, "null temporal type");
+    if (fn < 0 || fn >= BDF_NTEMPORAL) return fail(BDF_INVALID, "unknown temporal function %d", fn);
+    TRY(temporal_storage(t, &pl->in_dtype, &pl->cfg));
+    const bool time_kind = t->kind == BDF_TIME32 || t->kind == BDF_TIME64;
+    const bool field_of_day = fn == BDF_TEMPORAL_HOUR || fn == BDF_TEMPORAL_MINUTE || fn == BDF_TEMPORAL_SECOND;
+    if (time_kind && !field_of_day) return fail(BDF_UNSUPPORTED, "temporal function %d needs a date or a timestamp, not a time of day", fn);
+    const bool int32_arg = fn == BDF_TEMPORAL_DATE_ADD || fn == BDF_TEMPORAL_DATE_SUB || fn == BDF_TEMPORAL_ADD_MONTHS;
+    if (int32_arg && (arg < INT32_MIN || arg > INT32_MAX)) return fail(BDF_INVALID, "the argument %lld is outside the Int32 range", (long long)arg);
+    if (fn == BDF_TEMPORAL_NEXT_DAY && (arg < 1 || arg > 7)) return fail(BDF_INVALID, "next_day takes a day of week 1..7 (1 = Sunday), not %lld", (long long)arg);
+    if (fn == BDF_TEMPORAL_DATE_TRUNC && (arg < BDF_TRUNC_YEAR || arg > BDF_TRUNC_SECOND)) return fail(BDF_INVALID, "unknown date_trunc unit %lld", (long long)arg);
+    if (fn == BDF_TEMPORAL_TO_TIMESTAMP && (arg < BDF_SECOND || arg > BDF_NANOSECOND)) return fail(BDF_INVALID, "unknown time unit %lld", (long long)arg);
+    const bool instant = fn == BDF_TEMPORAL_UNIX_TIMESTAMP || fn == BDF_TEMPORAL_TO_TIMESTAMP;
+    int64_t off_sec = 0;
+    if (t->kind == BDF_TIMESTAMP && !instant && !temporal_tz_offset(t->tz, &off_sec))
+        return fail(BDF_UNSUPPORTED, "time zone '%s' is not a fixed offset: named zones need a tz database the device does not have", t->tz);
+    TemporalParams& p = pl->p;
+    p.fn = fn;
+    p.time_kind = time_kind ? 1 : 0;
+    p.arg = int32_arg ? arg : 0;
+    p.aux = (fn == BDF_TEMPORAL_NEXT_DAY || fn == BDF_TEMPORAL_DATE_TRUNC) ? (int32_t)arg : 0;
+    p.off = off_sec * temporal_per_sec(pl->cfg);
+    p.mul = 1; p.div = 1;
+    pl->out_type = bdf_temporal_type{BDF_TEMPORAL_NONE, 0, nullptr};
+    switch (fn) {
+        case BDF_TEMPORAL_TO_DATE: case BDF_TEMPORAL_DATE_ADD: case BDF_TEMPORAL_DATE_SUB: case BDF_TEMPORAL_ADD_MONTHS:
+        case BDF_TEMPORAL_LAST_DAY: case BDF_TEMPORAL_NEXT_DAY:
+            pl->out_dtype = BDF_I32; pl->out_type = bdf_temporal_type{BDF_DATE32, 0, nullptr}; break;
+        case BDF_TEMPORAL_DATE_TRUNC: pl->out_dtype = pl->in_dtype; pl->out_type = *t; break;
+        case BDF_TEMPORAL_UNIX_TIMESTAMP: pl->out_dtype = BDF_I64; break;
+        case BDF_TEMPORAL_TO_TIMESTAMP: {
+            pl->out_dtype = BDF_I64;
+            pl->out_type = bdf_temporal_type{BDF_TIMESTAMP, (int32_t)arg, t->kind == BDF_TIMESTAMP ? t->tz : nullptr};
+            const int64_t dst = temporal_per_sec(TC_S + (int)arg);
+            if (pl->cfg == TC_DAYS) p.mul = 86400 * dst;
+            else {
+                const int64_t src = temporal_per_sec(pl->cfg);
+                if (dst >= src) p.mul = dst / src; else p.div = src / dst;
+            }
+            break;
+        }
+        default: pl->out_dtype = BDF_I32; break;   // the Int32 fields
+    }
+    return BDF_OK;
+}
+
+static int temporal_dev(bdf_ctx* c, const TemporalPlan& pl, const bdf_col* in, bdf_col** out) {
+    if (in->dtype != pl.in_dtype) return fail(BDF_INVALID, "a column of dtype %d does not hold this temporal type (dtype %d)", in->dtype, pl.in_dtype);
+    const int64_t n = (int64_t)in->chunks.size();
+    std::vector<ChunkPlan> plan((size_t)n);
+    for (int64_t i = 0; i < n; i++) plan[i] = {in->chunks[i].len, true};   // range rules can turn any slot NULL
+    ColOwner o(c);
+    const int tile = elems_per_tile_temporal(pl.in_dtype, pl.out_dtype);
+    TRY(col_alloc(c, pl.out_dtype, plan, nullptr, tile, o.out()));
+    o->counts_on_device = o->d_warp_counts != nullptr;
+    const int wi = dtype_width(pl.in_dtype), wo = dtype_width(pl.out_dtype);
+    void *hp = nullptr, *dp = nullptr;
+    TRY(ring_alloc(c, (size_t)n * sizeof(UnDesc), &hp, &dp));
+    UnDesc* dd = (UnDesc*)dp;
+    UnDesc* hd = (UnDesc*)hp;
+    cudaError_t e = cudaSuccess;
+    const std::vector<int64_t> ends = plan_groups(n, {in});
+    int64_t begin = 0;
+    for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
+        const int64_t end = ends[gi];
+        int64_t tiles = 0, rows = 0, bytes = 0;
+        for (int64_t i = begin; i < end; i++) {
+            const DevChunk &a = in->chunks[i], &oc = o->chunks[i];
+            hd[i] = UnDesc{a.values, oc.values, a.validity, oc.validity, a.len, tiles, a.bit_off, 0};
+            tiles += (a.len + tile - 1) / tile;
+            rows += a.len;
+            bytes += a.len * (wi + wo) + ((a.validity ? 1 : 0) + 1) * bitmap_bytes(a.len);
+        }
+        wait_groups(c->s_compute, in, begin, end);
+        if (end > begin) {
+            e = desc_upload(c, dd + begin, hd + begin, (size_t)(end - begin) * sizeof(UnDesc));
+            if (e == cudaSuccess) {
+                LaunchTimer t(c, BDF_K_TEMPORAL, pl.out_dtype, rows, bytes);
+                e = launch_temporal(pl.cfg, pl.in_dtype, pl.out_dtype, pl.p, dd + begin, (int)(end - begin), tiles,
+                                    o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute);
+            }
+        }
+        if (e == cudaSuccess) {
+            Group g{begin, end, nullptr};
+            e = ev_get(c, &g.ev);
+            if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
+            o->groups.push_back(g);
+        }
+        begin = end;
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "temporal function");
+    *out = o.release();
+    return BDF_OK;
+}
+
+// One side of a two-column temporal function: a date kind, its storage and its fixed offset in its own units.
+static int temporal_side(const bdf_temporal_type* t, const bdf_col* col, int* cfg, int64_t* off) {
+    if (!t || !col) return fail(BDF_INVALID, "null argument");
+    int dtype = 0;
+    TRY(temporal_storage(t, &dtype, cfg));
+    if (t->kind == BDF_TIME32 || t->kind == BDF_TIME64) return fail(BDF_UNSUPPORTED, "date_diff / months_between need dates or timestamps, not times of day");
+    int64_t sec = 0;
+    if (t->kind == BDF_TIMESTAMP && !temporal_tz_offset(t->tz, &sec))
+        return fail(BDF_UNSUPPORTED, "time zone '%s' is not a fixed offset: named zones need a tz database the device does not have", t->tz);
+    if (col->dtype != dtype) return fail(BDF_INVALID, "a column of dtype %d does not hold this temporal type (dtype %d)", col->dtype, dtype);
+    *off = sec * temporal_per_sec(*cfg);
+    return BDF_OK;
+}
+
+static int temporal_binary_dev(bdf_ctx* c, int fn, const bdf_temporal_type* ta, const bdf_col* a, const bdf_temporal_type* tb, const bdf_col* b,
+                               bdf_col** out) {
+    if (fn != BDF_TEMPORAL_DATE_DIFF && fn != BDF_TEMPORAL_MONTHS_BETWEEN) return fail(BDF_INVALID, "unknown two-column temporal function %d", fn);
+    TemporalParams2 p{};
+    p.fn = fn;
+    TRY(temporal_side(ta, a, &p.cfg_a, &p.off_a));
+    TRY(temporal_side(tb, b, &p.cfg_b, &p.off_b));
+    const int out_dtype = fn == BDF_TEMPORAL_DATE_DIFF ? BDF_I32 : BDF_F64;
+    const int64_t n = std::min<int64_t>((int64_t)a->chunks.size(), (int64_t)b->chunks.size());   // zip()
+    for (int64_t i = 0; i < n; i++)
+        if (a->chunks[i].len != b->chunks[i].len) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
+    std::vector<ChunkPlan> plan((size_t)n);
+    for (int64_t i = 0; i < n; i++) plan[i] = {a->chunks[i].len, true};
+    ColOwner o(c);
+    const int tile = elems_per_tile_temporal2(a->dtype, b->dtype, out_dtype);
+    TRY(col_alloc(c, out_dtype, plan, nullptr, tile, o.out()));
+    o->counts_on_device = o->d_warp_counts != nullptr;
+    const int wrow = dtype_width(a->dtype) + dtype_width(b->dtype) + dtype_width(out_dtype);
+    void *hp = nullptr, *dp = nullptr;
+    TRY(ring_alloc(c, (size_t)n * sizeof(BinDesc), &hp, &dp));
+    BinDesc* dd = (BinDesc*)dp;
+    BinDesc* hd = (BinDesc*)hp;
+    cudaError_t e = cudaSuccess;
+    const std::vector<int64_t> ends = plan_groups(n, {a, b});
+    int64_t begin = 0;
+    for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
+        const int64_t end = ends[gi];
+        int64_t tiles = 0, rows = 0, bytes = 0;
+        for (int64_t i = begin; i < end; i++) {
+            const DevChunk &x = a->chunks[i], &y = b->chunks[i], &oc = o->chunks[i];
+            hd[i] = BinDesc{x.values, y.values, oc.values, x.validity, y.validity, oc.validity, x.len, tiles, x.bit_off, y.bit_off};
+            tiles += (x.len + tile - 1) / tile;
+            rows += x.len;
+            bytes += x.len * wrow + ((x.validity ? 1 : 0) + (y.validity ? 1 : 0) + 1) * bitmap_bytes(x.len);
+        }
+        wait_groups(c->s_compute, a, begin, end);
+        wait_groups(c->s_compute, b, begin, end);
+        if (end > begin) {
+            e = desc_upload(c, dd + begin, hd + begin, (size_t)(end - begin) * sizeof(BinDesc));
+            if (e == cudaSuccess) {
+                LaunchTimer t(c, BDF_K_TEMPORAL, out_dtype, rows, bytes);
+                e = launch_temporal2(a->dtype, b->dtype, out_dtype, p, dd + begin, (int)(end - begin), tiles,
+                                     o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute);
+            }
+        }
+        if (e == cudaSuccess) {
+            Group g{begin, end, nullptr};
+            e = ev_get(c, &g.ev);
+            if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
+            o->groups.push_back(g);
+        }
+        begin = end;
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "temporal function");
+    *out = o.release();
+    return BDF_OK;
+}
+
 static int boolean_dev(bdf_ctx* c, int op, const bdf_col* a, const bdf_col* b, bdf_col** out);
 static int realign(bdf_ctx* c, const bdf_col* in, bdf_col** out) {
     if (in->dtype == kBool) return boolean_dev(c, 1 /* OR: x | x = x, validity AND itself */, in, in, out);
@@ -3756,6 +3960,30 @@ static int fleet_map_host(bdf_ctx* c, bool is_cast, int op_or_to, int dtype, int
     return BDF_OK;
 }
 
+// bdf_temporal over every GPU: the views are sharded as for bdf_unary, every kid runs the one-GPU entry on its pieces.
+static int fleet_temporal_host(bdf_ctx* c, int fn, const bdf_temporal_type* type, int64_t arg, int64_t n, const bdf_view* in, bdf_out* out) {
+    Fleet* f = c->fleet;
+    const int nk = (int)f->kids.size();
+    TemporalPlan pl;
+    TRY(temporal_plan(fn, type, arg, &pl));
+    if (n < 0 || (n && (!in || !out))) return fail(BDF_INVALID, "bad arguments");
+    std::vector<int64_t> lens((size_t)n);
+    for (int64_t i = 0; i < n; i++) {
+        if (in[i].len < 0 || in[i].offset < 0) return fail(BDF_INVALID, "bad view %lld", (long long)i);
+        lens[i] = in[i].len;
+    }
+    const auto map = fleet_plan(lens, nk);
+    std::vector<std::vector<bdf_view>> iv((size_t)nk);
+    std::vector<std::vector<bdf_out>> ov((size_t)nk);
+    for (int k = 0; k < nk; k++) { iv[k] = fleet_views(map, nk, k, in); ov[k] = fleet_outs(map, k, pl.out_dtype, out); }
+    TRY(fleet_run(f, [&](int k) {
+        bdf_view dv{}; bdf_out dummy{};
+        return bdf_temporal(f->kids[k], fn, type, arg, (int64_t)iv[k].size(), iv[k].empty() ? &dv : iv[k].data(), ov[k].empty() ? &dummy : ov[k].data());
+    }));
+    fleet_merge_outs(map, ov, lens, out);
+    return BDF_OK;
+}
+
 // Aggregates of a host column: upload the pieces (every GPU its own), reduce, combine; metadata rules over the caller's chunks.
 static int fleet_aggregate_host(bdf_ctx* c, int kind /* 0 one op, 1 all four, 2 avg */, int op, int dtype, int64_t n, const bdf_view* in, void* out_scalar,
                                 int32_t* is_some, bdf_agg4* all, double* avg) {
@@ -4798,6 +5026,46 @@ int bdf_cast_dev(bdf_ctx* c, int to, const bdf_col* in, bdf_col** out) {
     return map_dev(c, true, to, in, out);
 }
 
+int bdf_temporal_result(int fn, const bdf_temporal_type* type, int64_t arg, int32_t* out_dtype, bdf_temporal_type* out_type) {
+    TemporalPlan pl;
+    TRY(temporal_plan(fn, type, arg, &pl));
+    if (out_dtype) *out_dtype = pl.out_dtype;
+    if (out_type) *out_type = pl.out_type;
+    return BDF_OK;
+}
+
+int bdf_temporal_dev(bdf_ctx* c, int fn, const bdf_temporal_type* type, int64_t arg, const bdf_col* in, bdf_col** out) {
+    TemporalPlan pl;
+    TRY(temporal_plan(fn, type, arg, &pl));
+    if (c && c->fleet) {
+        if (!in || !out) return fail(BDF_INVALID, "null argument");
+        if (in->dtype != pl.in_dtype) return fail(BDF_INVALID, "a column of dtype %d does not hold this temporal type (dtype %d)", in->dtype, pl.in_dtype);
+        Fleet* f = c->fleet;
+        return fleet_map(c, pl.out_dtype, {in}, out, [=](int k, bdf_col** o) { return bdf_temporal_dev(f->kids[k], fn, type, arg, in->fparts[k], o); });
+    }
+    ENTER(c);
+    if (!in || !out) return fail(BDF_INVALID, "null argument");
+    return temporal_dev(c, pl, in, out);
+}
+
+int bdf_temporal_binary_dev(bdf_ctx* c, int fn, const bdf_temporal_type* ta, const bdf_col* a, const bdf_temporal_type* tb, const bdf_col* b,
+                            bdf_col** out) {
+    if (c && c->fleet) {
+        if (!a || !b || !out || !ta || !tb) return fail(BDF_INVALID, "null argument");
+        if (fn != BDF_TEMPORAL_DATE_DIFF && fn != BDF_TEMPORAL_MONTHS_BETWEEN) return fail(BDF_INVALID, "unknown two-column temporal function %d", fn);
+        int cfg = 0;
+        int64_t off = 0;
+        TRY(temporal_side(ta, a, &cfg, &off));
+        TRY(temporal_side(tb, b, &cfg, &off));
+        Fleet* f = c->fleet;
+        return fleet_map(c, fn == BDF_TEMPORAL_DATE_DIFF ? BDF_I32 : BDF_F64, {a, b}, out,
+                         [=](int k, bdf_col** o) { return bdf_temporal_binary_dev(f->kids[k], fn, ta, a->fparts[k], tb, b->fparts[k], o); });
+    }
+    ENTER(c);
+    if (!a || !b || !out) return fail(BDF_INVALID, "null argument");
+    return temporal_binary_dev(c, fn, ta, a, tb, b, out);
+}
+
 int bdf_aggregate_dev(bdf_ctx* c, int op, const bdf_col* in, void* out_scalar, int32_t* is_some) {
     if (c && c->fleet) { if (!in || !out_scalar || !is_some) return fail(BDF_INVALID, "null argument"); return fleet_aggregate_dev(c, op, in, out_scalar, is_some); }
     ENTER(c);
@@ -5171,6 +5439,24 @@ int bdf_cast(bdf_ctx* c, int from, int to, int64_t n, const bdf_view* in, bdf_ou
     if (c && c->fleet) { TRY(check_dtype(to)); return fleet_map_host(c, true, to, from, n, in, out); }
     ENTER(c);
     return map_host(c, true, to, from, n, in, out);
+}
+
+int bdf_temporal(bdf_ctx* c, int fn, const bdf_temporal_type* type, int64_t arg, int64_t n, const bdf_view* in, bdf_out* out) {
+    if (c && c->fleet) return fleet_temporal_host(c, fn, type, arg, n, in, out);
+    ENTER(c);
+    TemporalPlan pl;
+    TRY(temporal_plan(fn, type, arg, &pl));
+    if (n < 0 || (n && (!in || !out))) return fail(BDF_INVALID, "bad arguments");
+    std::vector<bdf_col*> cols;
+    TRY(upload_many(c, {UploadSpec{pl.in_dtype, n, in}}, true, cols));
+    bdf_col* o = nullptr;
+    int st = temporal_dev(c, pl, cols[0], &o);
+    if (st == BDF_OK) st = download(c, o, out);
+    std::string keep = g_err;
+    cudaStreamSynchronize(c->s_h2d);   // host inputs must not be touched after return
+    col_release(c, o); col_release(c, cols[0]);
+    g_err = keep;
+    return st;
 }
 
 int bdf_aggregate(bdf_ctx* c, int op, int dtype, int64_t n, const bdf_view* in, void* out_scalar, int32_t* is_some) {

@@ -392,7 +392,8 @@ class DeviceFrame:
     @classmethod
     def from_arrow(cls, path: str, columns: Optional[Sequence[str]] = None, ctx: Optional[N.Context] = None) -> "DeviceFrame":
         with IpcFile(path) as f:
-            names = [n for n, dt, _ in f.schema if dt >= 0 and (columns is None or n in columns)]
+            # Date / Time / Timestamp columns come in tagged when they are named; with no names the frame is what it always was
+            names = [n for n, dt, _ in f.schema if (dt >= 0 or (columns is not None and n in f.temporal_columns)) and (columns is None or n in columns)]
             cols = f.read(names, ctx=ctx)
         return cls(OrderedDict((n, cols[n]) for n in names))
 
@@ -418,7 +419,11 @@ class DeviceFrame:
         write_ipc(path, dict(self.columns))
 
     def to_csv(self, path: str, has_header: bool = True, delimiter: str = ",") -> None:
-        """DataFrame::to_csv: the frame's text is formatted on the device and streamed to the file (write_csv)."""
+        """DataFrame::to_csv: the frame's text is formatted on the device and streamed to the file (write_csv).  A frame with a
+        temporal column is refused: its raw Int32 / Int64 values are not the text a reader would expect."""
+        for n, c in self.columns.items():
+            if getattr(c, "temporal", None) is not None:
+                raise N.UnsupportedType(f"column {n!r} is {c.temporal!r}: temporal text is not written by the CSV writer")
         write_csv(path, self.columns, has_header=has_header, delimiter=delimiter)
 
     def to_host(self) -> Dict[str, list]:
@@ -477,6 +482,8 @@ class DeviceFrame:
                 raise N.ComputeError(f"Aggregating column {cname!r} does not exist")
             if fn not in ("sum", "count", "min", "max"):
                 raise N.UnsupportedType(f"aggregate {fn!r} is not on the path")
+            if fn == "sum" and getattr(self.columns[cname], "temporal", None) is not None:
+                raise N.UnsupportedType(f"sum of {cname!r} ({self.columns[cname].temporal!r}): temporal values are not summed")
         names = list(OrderedDict.fromkeys(c for c, _ in aggregates))
         keys, res = group_aggregate(self.column(groups), [self.column(c) for c in names])
         out: "OrderedDict[str, Column]" = OrderedDict([(groups, keys)])

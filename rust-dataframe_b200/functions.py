@@ -18,7 +18,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 from . import _native as N
-from .arrays import F64, NP_DTYPES, PrimitiveArray, is_float, width_of
+from .arrays import F64, I64, NP_DTYPES, PrimitiveArray, TemporalType, is_float, width_of
 
 Chunks = Sequence[PrimitiveArray]
 
@@ -126,6 +126,118 @@ def cast(arrays: Chunks, to_dtype: int, ctx=None, pinned_out=False) -> List[Prim
     outs, bufs = N.alloc_outputs(to_dtype, [c.length for c in arrays], ctx, pinned_out)
     N.raise_for_status(N.lib().bdf_cast(ctx.handle, from_dtype, to_dtype, len(arrays), N.make_views(arrays), outs))
     return N.collect_outputs(to_dtype, outs, bufs)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# dates and timestamps (include/b200df.h "dates and timestamps")
+
+
+def _temporal_c(t: TemporalType) -> "N.TemporalTypeC":
+    return N.TemporalTypeC(t.kind, t.unit, t.tz.encode() if t.tz is not None else None)
+
+
+def temporal_result(fn, temporal: TemporalType, arg: int = 0):
+    """bdf_temporal_result: ``(result dtype, result TemporalType or None)`` of a temporal function (a name of ``native.TEMPORAL_FNS`` or
+    its number) on a column of type ``temporal``; raises exactly what the function itself would for (fn, type, arg).  No GPU needed."""
+    fn = N.TEMPORAL_FNS[fn] if isinstance(fn, str) else int(fn)
+    tc, dt, ot = _temporal_c(temporal), C.c_int32(0), N.TemporalTypeC()
+    N.raise_for_status(N.lib().bdf_temporal_result(fn, C.byref(tc), int(arg), C.byref(dt), C.byref(ot)))
+    out = None
+    if ot.kind:
+        tz = None if not ot.tz else ot.tz.decode()
+        out = TemporalType(ot.kind, ot.unit, tz)
+    return dt.value, out
+
+
+_WEEKDAYS = {"su": 1, "mo": 2, "tu": 3, "we": 4, "th": 5, "fr": 6, "sa": 7}
+
+
+def _temporal_arg(fn: int, arg) -> int:
+    """Names accepted for the argument: date_trunc units ("day", "month" ...), time units ("s" .. "ns"), weekdays ("tuesday", "tue")."""
+    if isinstance(arg, str):
+        a = arg.lower()
+        if fn == N.T_DATE_TRUNC:
+            return N.TRUNC_UNITS[{"yyyy": "year", "yy": "year", "mm": "month", "mon": "month", "dd": "day"}.get(a, a)]
+        if fn == N.T_TO_TIMESTAMP:
+            return N.TIME_UNITS[a]
+        if fn == N.T_NEXT_DAY and len(a) >= 2 and a[:2] in _WEEKDAYS:
+            return _WEEKDAYS[a[:2]]
+        raise N.ComputeError(f"argument {arg!r} is not understood by temporal function {fn}")
+    return int(arg)
+
+
+def _temporal_of(arrays: Chunks, temporal: Optional[TemporalType]) -> TemporalType:
+    if temporal is None:
+        for c in arrays:
+            temporal = getattr(c, "temporal", None)
+            break
+    if temporal is None:
+        raise N.UnsupportedType("a temporal function needs the column's temporal type (pass temporal=TemporalType...)")
+    return temporal
+
+
+def _temporal_host(fn: int, arrays: Chunks, temporal: Optional[TemporalType], arg, ctx, pinned_out: bool) -> List[PrimitiveArray]:
+    ctx = ctx or N.default_context()
+    t = _temporal_of(arrays, temporal)
+    a = _temporal_arg(fn, arg)
+    out_dtype, out_t = temporal_result(fn, t, a)
+    if len(arrays) == 0:
+        return []
+    _check_same_type(arrays, t.dtype)
+    outs, bufs = N.alloc_outputs(out_dtype, [c.length for c in arrays], ctx, pinned_out)
+    tc = _temporal_c(t)
+    N.raise_for_status(N.lib().bdf_temporal(ctx.handle, fn, C.byref(tc), a, len(arrays), N.make_views(arrays), outs))
+    res = N.collect_outputs(out_dtype, outs, bufs)
+    for r in res:
+        r.temporal = out_t
+    return res
+
+
+def _add_temporal(name: str, fn: int, has_arg: bool) -> None:
+    if has_arg:
+        def f(arrays: Chunks, arg, temporal: Optional[TemporalType] = None, ctx=None, pinned_out=False) -> List[PrimitiveArray]:
+            return _temporal_host(fn, arrays, temporal, arg, ctx, pinned_out)
+    else:
+        def f(arrays: Chunks, temporal: Optional[TemporalType] = None, ctx=None, pinned_out=False) -> List[PrimitiveArray]:
+            return _temporal_host(fn, arrays, temporal, 0, ctx, pinned_out)
+    f.__name__ = name
+    f.__doc__ = (f"ScalarFunctions::{name} over every chunk of a Date32 / Date64 / Timestamp{' / Time' if fn in (N.T_HOUR, N.T_MINUTE, N.T_SECOND) else ''}"
+                 " column (one bdf_temporal call); the chunks' .temporal tag or `temporal` gives the type.")
+    setattr(ScalarFunctions, name, staticmethod(f))
+
+
+for _name, _fn in N.TEMPORAL_FNS.items():
+    _add_temporal(_name, _fn, _fn in (N.T_DATE_ADD, N.T_DATE_SUB, N.T_ADD_MONTHS, N.T_NEXT_DAY, N.T_DATE_TRUNC, N.T_TO_TIMESTAMP))
+
+
+def _temporal_binary_host(fn: int, a: Chunks, b: Chunks, ta, tb, ctx) -> List[PrimitiveArray]:
+    ctx = ctx or N.default_context()
+    ta, tb = _temporal_of(a, ta), _temporal_of(b, tb)
+    ca = Column.upload(a, ctx, dtype=ta.dtype).with_temporal(ta)
+    cb = Column.upload(b, ctx, dtype=tb.dtype).with_temporal(tb)
+    return ca._temporal_binary(fn, cb).download()
+
+
+def _date_diff_host(end: Chunks, start: Chunks, temporal_end=None, temporal_start=None, ctx=None) -> List[PrimitiveArray]:
+    """Spark's datediff(end, start): days(to_date(end)) - days(to_date(start)) as Int32, chunk by chunk."""
+    return _temporal_binary_host(N.T_DATE_DIFF, end, start, temporal_end, temporal_start, ctx)
+
+
+def _months_between_host(a: Chunks, b: Chunks, temporal_a=None, temporal_b=None, ctx=None) -> List[PrimitiveArray]:
+    """Spark 2.4's months_between(a, b) with roundOff = true, Float64, chunk by chunk."""
+    return _temporal_binary_host(N.T_MONTHS_BETWEEN, a, b, temporal_a, temporal_b, ctx)
+
+
+ScalarFunctions.date_diff = staticmethod(_date_diff_host)
+ScalarFunctions.months_between = staticmethod(_months_between_host)
+
+
+def _refuse_temporal(what: str, *cols) -> None:
+    """Operations that would treat dates as numbers (arithmetic, sums, float comparison) refuse tagged columns before any device call."""
+    for c in cols:
+        t = getattr(c, "temporal", None)
+        if t is not None:
+            raise N.UnsupportedType(f"{what} of a {t!r} column: only numeric types are summed or computed on (temporal values are not)")
 
 
 def _scalar_from_bits(dtype: int, bits: int):
@@ -295,9 +407,18 @@ class Column:
     until ``download``.  Mirrors how Evaluate::calculate (src/evaluation.rs:97-323) materialises every
     Calculation as a new column of the frame."""
 
-    def __init__(self, ctx: N.Context, handle: C.c_void_p):
+    def __init__(self, ctx: N.Context, handle: C.c_void_p, temporal: Optional[TemporalType] = None):
         self.ctx = ctx
         self.handle = handle
+        self.temporal = temporal   # a TemporalType when the Int32 / Int64 values are dates, times or timestamps
+
+    def with_temporal(self, t: Optional[TemporalType]) -> "Column":
+        """Tag the column with a temporal type (None removes the tag); the values are not touched.  The tag is set IN PLACE and the
+        column itself is returned: a Column taken from a DeviceFrame is the frame's own object, so the frame's column is retagged too."""
+        if t is not None and t.dtype != self.dtype:
+            raise N.ComputeError(f"a column of dtype {self.dtype} cannot hold {t!r} (physical dtype {t.dtype})")
+        self.temporal = t
+        return self
 
     # -- construction --
     @classmethod
@@ -310,7 +431,8 @@ class Column:
         h = C.c_void_p()
         st = N.lib().bdf_upload(ctx.handle, dtype, len(arrays), N.make_views(arrays), N.ASYNC if asynchronous else 0, C.byref(h))
         N.raise_for_status(st)
-        col = cls(ctx, h)
+        tags = {getattr(a, "temporal", None) for a in arrays}
+        col = cls(ctx, h, tags.pop() if len(tags) == 1 else None)   # chunks that all carry one temporal type tag the column
         col._hold = arrays if asynchronous else None  # keep host buffers alive while copies are in flight
         return col
 
@@ -371,6 +493,7 @@ class Column:
 
     # -- operators --
     def _bin(self, op: int, other: "Column") -> "Column":
+        _refuse_temporal("arithmetic", self, other)
         h = C.c_void_p()
         N.raise_for_status(N.lib().bdf_binary_dev(self.ctx.handle, op, self.handle, other.handle, C.byref(h)))
         return Column(self.ctx, h)
@@ -386,6 +509,7 @@ class Column:
     # -- fused operator + aggregate of the result (one pass; SURVEY K5) --
     def binary_agg(self, op: int, other: "Column"):
         """(self op other) materialised as a Column AND sum/min/max/count of it, from one kernel pass."""
+        _refuse_temporal("arithmetic", self, other)
         h, a = C.c_void_p(), N.Agg4()
         N.raise_for_status(N.lib().bdf_binary_agg_dev(self.ctx.handle, op, self.handle, other.handle, C.byref(h), C.byref(a)))
         return Column(self.ctx, h), _agg4_to_dict(self.dtype, a)
@@ -394,6 +518,7 @@ class Column:
 
     def binary_agg_async(self, op: int, other: "Column"):
         """Like binary_agg but returns (Column, AggFuture) without waiting for the GPU."""
+        _refuse_temporal("arithmetic", self, other)
         h, f = C.c_void_p(), C.c_void_p()
         N.raise_for_status(N.lib().bdf_binary_agg_dev_async(self.ctx.handle, op, self.handle, other.handle, C.byref(h), C.byref(f)))
         return Column(self.ctx, h), AggFuture(self.ctx, f, self.dtype)
@@ -402,9 +527,10 @@ class Column:
         """Column::take (src/table.rs:218-241): values at the UInt32 row numbers, as ONE chunk; null index -> null slot."""
         h = C.c_void_p()
         N.raise_for_status(N.lib().bdf_take_dev(self.ctx.handle, self.handle, indices.handle, C.byref(h)))
-        return Column(self.ctx, h)
+        return Column(self.ctx, h, self.temporal)
 
     def aggregate_all_async(self) -> "AggFuture":
+        _refuse_temporal("sum", self)
         f = C.c_void_p()
         N.raise_for_status(N.lib().bdf_aggregate_all_dev_async(self.ctx.handle, self.handle, C.byref(f)))
         return AggFuture(self.ctx, f, self.dtype)
@@ -412,7 +538,9 @@ class Column:
     # -- N2: BooleanFilter comparisons, boolean kernels, filter (SURVEY 8(f)) --
     def compare(self, op: int, other) -> "Column":
         """BooleanFilter::{Gt,Ge,Eq,Ne,Lt,Le}: both sides cast to Float64, compared; `other` is a Column or a scalar
-        (BooleanInput::Scalar).  Returns a boolean mask column."""
+        (BooleanInput::Scalar).  Returns a boolean mask column.  A Date64 / Timestamp / Time64 column is refused: the Float64 comparison
+        is not exact for 64-bit instants; compare to_date() (Date32, exact in f64) or unix_timestamp() instead."""
+        _refuse_temporal("Float64 comparison", *[c for c in (self, other) if getattr(getattr(c, "temporal", None), "dtype", None) == I64])
         h = C.c_void_p()
         if isinstance(other, Column):
             st = N.lib().bdf_compare_dev(self.ctx.handle, op, self.handle, other.handle, 0.0, C.byref(h))
@@ -441,9 +569,10 @@ class Column:
         """ChunkedArray::filter: keep the slots where the boolean mask column is valid and true."""
         h = C.c_void_p()
         N.raise_for_status(N.lib().bdf_filter_dev(self.ctx.handle, self.handle, mask.handle, C.byref(h)))
-        return Column(self.ctx, h)
+        return Column(self.ctx, h, self.temporal)
 
     def unary(self, op: int) -> "Column":
+        _refuse_temporal("a math function", self)
         h = C.c_void_p()
         N.raise_for_status(N.lib().bdf_unary_dev(self.ctx.handle, op, self.handle, C.byref(h)))
         return Column(self.ctx, h)
@@ -454,11 +583,14 @@ class Column:
     def abs(self): return self.unary(N.ABS)
 
     def cast(self, to_dtype: int) -> "Column":
+        _refuse_temporal("cast", self)
         h = C.c_void_p()
         N.raise_for_status(N.lib().bdf_cast_dev(self.ctx.handle, to_dtype, self.handle, C.byref(h)))
         return Column(self.ctx, h)
 
     def aggregate(self, op: int):
+        if op == N.SUM:
+            _refuse_temporal("sum", self)
         dtype = self.dtype
         out = np.zeros(1, dtype=np.int64 if (op == N.COUNT or dtype == N.BOOL) else NP_DTYPES[dtype])
         some = C.c_int32(0)
@@ -471,16 +603,19 @@ class Column:
     def count(self): return int(self.aggregate(N.COUNT))
 
     def aggregate_all(self) -> dict:
+        _refuse_temporal("sum", self)
         a = N.Agg4()
         N.raise_for_status(N.lib().bdf_aggregate_all_dev(self.ctx.handle, self.handle, C.byref(a)))
         return _agg4_to_dict(self.dtype, a)
 
     def avg(self):
+        _refuse_temporal("avg", self)
         out, some = C.c_double(0), C.c_int32(0)
         N.raise_for_status(N.lib().bdf_avg_dev(self.ctx.handle, self.handle, C.byref(out), C.byref(some)))
         return out.value if some.value else None
 
     def moments(self) -> dict:
+        _refuse_temporal("a statistic", self)
         r = N.MomentRec()
         N.raise_for_status(N.lib().bdf_moments_dev(self.ctx.handle, self.handle, C.byref(r)))
         return _moments_to_dict(r)
@@ -498,7 +633,47 @@ class Column:
         return r
 
     def count_distinct(self) -> int: return int(self._distinct().count)
-    def sum_distinct(self): return _scalar_from_bits(self.dtype, self._distinct().sum)
+    def sum_distinct(self):
+        _refuse_temporal("sum_distinct", self)
+        return _scalar_from_bits(self.dtype, self._distinct().sum)
+
+    # -- dates and timestamps (include/b200df.h "dates and timestamps"); the column must carry a temporal tag --
+    def _temporal_fn(self, fn: int, arg=0) -> "Column":
+        t = _temporal_of([self], None) if self.temporal is None else self.temporal
+        a = _temporal_arg(fn, arg)
+        _, out_t = temporal_result(fn, t, a)
+        tc = _temporal_c(t)
+        h = C.c_void_p()
+        N.raise_for_status(N.lib().bdf_temporal_dev(self.ctx.handle, fn, C.byref(tc), a, self.handle, C.byref(h)))
+        return Column(self.ctx, h, out_t)
+
+    def _temporal_binary(self, fn: int, other: "Column") -> "Column":
+        ta, tb = _temporal_of([self], self.temporal), _temporal_of([other], other.temporal)
+        ca, cb = _temporal_c(ta), _temporal_c(tb)
+        h = C.c_void_p()
+        N.raise_for_status(N.lib().bdf_temporal_binary_dev(self.ctx.handle, fn, C.byref(ca), self.handle, C.byref(cb), other.handle, C.byref(h)))
+        return Column(self.ctx, h)
+
+    def year(self): return self._temporal_fn(N.T_YEAR)
+    def quarter(self): return self._temporal_fn(N.T_QUARTER)
+    def month(self): return self._temporal_fn(N.T_MONTH)
+    def day_of_month(self): return self._temporal_fn(N.T_DAY_OF_MONTH)
+    def day_of_year(self): return self._temporal_fn(N.T_DAY_OF_YEAR)
+    def day_of_week(self): return self._temporal_fn(N.T_DAY_OF_WEEK)
+    def hour(self): return self._temporal_fn(N.T_HOUR)
+    def minute(self): return self._temporal_fn(N.T_MINUTE)
+    def second(self): return self._temporal_fn(N.T_SECOND)
+    def to_date(self): return self._temporal_fn(N.T_TO_DATE)
+    def date_add(self, days: int): return self._temporal_fn(N.T_DATE_ADD, days)
+    def date_sub(self, days: int): return self._temporal_fn(N.T_DATE_SUB, days)
+    def add_months(self, months: int): return self._temporal_fn(N.T_ADD_MONTHS, months)
+    def last_day(self): return self._temporal_fn(N.T_LAST_DAY)
+    def next_day(self, day_of_week): return self._temporal_fn(N.T_NEXT_DAY, day_of_week)
+    def date_trunc(self, unit): return self._temporal_fn(N.T_DATE_TRUNC, unit)
+    def unix_timestamp(self): return self._temporal_fn(N.T_UNIX_TIMESTAMP)
+    def to_timestamp(self, unit="us"): return self._temporal_fn(N.T_TO_TIMESTAMP, unit)
+    def date_diff(self, start: "Column"): return self._temporal_binary(N.T_DATE_DIFF, start)
+    def months_between(self, other: "Column"): return self._temporal_binary(N.T_MONTHS_BETWEEN, other)
 
     @staticmethod
     def aggregate_all_many(columns: Sequence["Column"], asynchronous: bool = False):
@@ -507,6 +682,7 @@ class Column:
         ctx = columns[0].ctx
         k = len(columns)
         cols = (C.c_void_p * k)(*[c.handle for c in columns])
+        _refuse_temporal("sum", *columns)
         dtypes = [c.dtype for c in columns]
         if asynchronous:
             f = C.c_void_p()
@@ -528,7 +704,11 @@ class Column:
             for i in range(n):
                 outs[i].len = bufs[i][0].shape[0]
         N.raise_for_status(N.lib().bdf_download(self.ctx.handle, self.handle, outs))
-        return N.collect_outputs(dtype, outs, bufs)
+        res = N.collect_outputs(dtype, outs, bufs)
+        if self.temporal is not None:
+            for r in res:
+                r.temporal = self.temporal
+        return res
 
     def download_begin(self, into):
         """Enqueue the device->host copies into `into` = alloc_outputs(...); pair with download_end(into)."""
@@ -582,15 +762,24 @@ def sort_columns(criteria: Sequence[tuple], columns: Sequence["Column"]) -> List
 def group_aggregate(key: "Column", values: Sequence["Column"]):
     """Group-by aggregate (`GroupAggregate`, unimplemented in the reference: src/evaluation.rs:73): returns
     ``(keys Column, [ {"sum": Column, "count": Column, "min": Column | None, "max": Column | None} per value column ])``.
-    Groups in ascending key order, the null key last; see include/b200df.h bdf_group_aggregate_dev."""
+    Groups in ascending key order, the null key last; see include/b200df.h bdf_group_aggregate_dev.  For a temporal value column
+    "sum" is None (dates are not summed; the device's sum is freed unread) and min / max carry the column's tag."""
     ctx = key.ctx
     k = len(values)
     cols = (C.c_void_p * max(k, 1))(*[v.handle for v in values])
     outs = (N.GroupOut * max(k, 1))()
     hk, ng = C.c_void_p(), C.c_int64(0)
     N.raise_for_status(N.lib().bdf_group_aggregate_dev(ctx.handle, key.handle, k, cols, C.byref(hk), outs, C.byref(ng)))
-    wrap = lambda p: Column(ctx, C.c_void_p(p)) if p else None
-    return Column(ctx, hk), [{"sum": wrap(outs[j].sum), "count": wrap(outs[j].count), "min": wrap(outs[j].min), "max": wrap(outs[j].max)} for j in range(k)]
+    wrap = lambda p, t=None: Column(ctx, C.c_void_p(p), t) if p else None
+    res = []
+    for j, v in enumerate(values):
+        t = getattr(v, "temporal", None)
+        s = wrap(outs[j].sum)
+        if t is not None and s is not None:
+            s.free()
+            s = None
+        res.append({"sum": s, "count": wrap(outs[j].count), "min": wrap(outs[j].min, t), "max": wrap(outs[j].max, t)})
+    return Column(ctx, hk, key.temporal), res
 
 
 def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
@@ -600,9 +789,11 @@ def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
     DataFrame::sort gives (ascending, nulls last per key).  Counts are Int64, avg and the statistics are Float64, everything else
     has the value column's type; see include/b200df.h for the NULL rules."""
     fns = []
-    for _, fn in aggregations:
+    for col, fn in aggregations:
         if fn not in N.GROUP_FNS:
             raise N.UnsupportedType(f"group function {fn!r} is not on the path")
+        if fn not in _CARRY_GROUP and fn not in ("count", "count_distinct"):
+            _refuse_temporal(fn, col)
         fns.append(N.GROUP_FNS[fn])
     ctx = keys[0].ctx if keys else (aggregations[0][0].ctx if aggregations else N.default_context())
     nk, na = len(keys), len(aggregations)
@@ -614,7 +805,12 @@ def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
     out = (C.c_void_p * max(na, 1))()
     ng = C.c_int64(0)
     N.raise_for_status(N.lib().bdf_group_by_dev(ctx.handle, nk, kcols, na, aggs, hk, out, C.byref(ng)))
-    return [Column(ctx, C.c_void_p(hk[k])) for k in range(nk)], [Column(ctx, C.c_void_p(out[j])) for j in range(na)]
+    carry = lambda col, fn: getattr(col, "temporal", None) if fn in _CARRY_GROUP else None
+    return ([Column(ctx, C.c_void_p(hk[k]), keys[k].temporal) for k in range(nk)],
+            [Column(ctx, C.c_void_p(out[j]), carry(*aggregations[j])) for j in range(na)])
+
+
+_CARRY_GROUP = ("min", "max", "first", "last")   # aggregations whose results are values of the column: a temporal tag carries
 
 
 def join_indices(left_keys: Sequence["Column"], right_keys: Sequence["Column"], how: str):
@@ -655,6 +851,8 @@ def _window_call(call: tuple, ordered: bool) -> "N.WindowCall":
     if len(call) < 2:
         raise N.ComputeError(f"{name} needs a column")
     x = call[1]
+    if name not in ("lag", "lead", "min", "max", "count"):
+        _refuse_temporal(name, x)
     k.column = x.handle.value if isinstance(x.handle, C.c_void_p) else x.handle
     if fn in (N.WIN_LAG, N.WIN_LEAD):
         k.offset = int(call[2]) if len(call) > 2 else 1
@@ -688,7 +886,8 @@ def window(partition_by: Sequence["Column"], order_by: Sequence[tuple], calls: S
         ok[i].column, ok[i].descending = handle(c), 1 if desc else 0
     out = (C.c_void_p * max(len(calls), 1))()
     N.raise_for_status(N.lib().bdf_window_dev(ctx.handle, len(partition_by), pk, len(order_by), ok, len(calls), arr, out))
-    return [Column(ctx, C.c_void_p(out[j])) for j in range(len(calls))]
+    carry = lambda c: getattr(c[1], "temporal", None) if c[0] in ("lag", "lead", "min", "max") else None
+    return [Column(ctx, C.c_void_p(out[j]), carry(calls[j])) for j in range(len(calls))]
 
 
 def _expr_nodes(nodes: Sequence[tuple]):
@@ -710,6 +909,7 @@ def eval_expr(inputs: Sequence["Column"], nodes: Sequence[tuple]) -> "Column":
     ``nodes`` is a straight-line program: slots ``0..len(inputs)-1`` are the input columns, node ``k`` writes slot
     ``len(inputs)+k``.  A node is ``(binop, a, b)`` with ``binop`` in native.ADD..LOG, or ``("sin", a)`` / ``(native.EXPR_UNARY + unop, a)``
     for a unary function.  The last node is the result column; intermediates never touch HBM."""
+    _refuse_temporal("a fused expression", *inputs)
     ctx = inputs[0].ctx
     cols = (C.c_void_p * len(inputs))(*[c.handle for c in inputs])
     h = C.c_void_p()
@@ -720,6 +920,7 @@ def eval_expr(inputs: Sequence["Column"], nodes: Sequence[tuple]) -> "Column":
 def eval_expr_agg(inputs: Sequence["Column"], nodes: Sequence[tuple], materialise: bool = True, asynchronous: bool = False):
     """eval_expr with sum/count of the result folded into the same pass.  Returns ``(Column or None, aggregate)`` where the
     aggregate is a dict (or an AggFuture when ``asynchronous``); ``materialise=False`` never writes the result column."""
+    _refuse_temporal("a fused expression", *inputs)
     ctx = inputs[0].ctx
     cols = (C.c_void_p * len(inputs))(*[c.handle for c in inputs])
     h = C.c_void_p()

@@ -130,6 +130,24 @@ Result<std::vector<PrimitiveArray<T>>> unary(int op, const std::vector<const Pri
     return out.finish();
 }
 
+// Dates and timestamps: T is the column's physical type (int32_t / int64_t), R the result's (bdf_temporal_result says which).
+template <typename T, typename R>
+Result<std::vector<PrimitiveArray<R>>> temporal(int fn, const bdf_temporal_type& type, int64_t arg, const std::vector<const PrimitiveArray<T>*>& array) {
+    int32_t dt = -1;
+    int st = bdf_temporal_result(fn, &type, arg, &dt, nullptr);
+    if (st == BDF_UNSUPPORTED) throw std::logic_error(std::string("temporal function not available: ") + bdf_last_error());
+    if (st != BDF_OK) return to_error(st);
+    if (dt != ArrowType<R>::id) throw std::logic_error("the result type R does not match bdf_temporal_result");
+    std::vector<int64_t> lens;
+    for (auto* a : array) lens.push_back(a->len());
+    Outputs<R> out(lens);
+    auto v = views(array);
+    st = bdf_temporal(context(), fn, &type, arg, (int64_t)v.size(), v.data(), out.outs.data());
+    if (st == BDF_UNSUPPORTED) throw std::logic_error(std::string("temporal function not available: ") + bdf_last_error());
+    if (st != BDF_OK) return to_error(st);
+    return out.finish();
+}
+
 }  // namespace detail
 
 struct ScalarFunctions {
@@ -150,6 +168,28 @@ struct ScalarFunctions {
     RDF_UNARY(floor, BDF_FLOOR) RDF_UNARY(log10, BDF_LOG10) RDF_UNARY(log2, BDF_LOG2) RDF_UNARY(radians, BDF_RADIANS)
     RDF_UNARY(round, BDF_ROUND) RDF_UNARY(sinh, BDF_SINH) RDF_UNARY(sqrt, BDF_SQRT) RDF_UNARY(tanh, BDF_TANH)
 #undef RDF_UNARY
+
+    // Dates and timestamps (include/b200df.h "dates and timestamps"): `type` is the Arrow temporal type of the column of physical T.
+    // ScalarFunctions::hour<T>(Vec<&PrimitiveArray<T>>) -> Vec<Int32Array> (scalar.rs:267-273) and the stubs of the same file.
+#define RDF_TEMPORAL(name, FN, R) \
+    template <typename T> static Out<R> name(const bdf_temporal_type& t, const Arrays<T>& a) { return detail::temporal<T, R>(FN, t, 0, a); }
+#define RDF_TEMPORAL_ARG(name, FN, R) \
+    template <typename T> static Out<R> name(const bdf_temporal_type& t, int64_t arg, const Arrays<T>& a) { return detail::temporal<T, R>(FN, t, arg, a); }
+    RDF_TEMPORAL(year, BDF_TEMPORAL_YEAR, int32_t) RDF_TEMPORAL(quarter, BDF_TEMPORAL_QUARTER, int32_t) RDF_TEMPORAL(month, BDF_TEMPORAL_MONTH, int32_t)
+    RDF_TEMPORAL(day_of_month, BDF_TEMPORAL_DAY_OF_MONTH, int32_t) RDF_TEMPORAL(day_of_year, BDF_TEMPORAL_DAY_OF_YEAR, int32_t)
+    RDF_TEMPORAL(day_of_week, BDF_TEMPORAL_DAY_OF_WEEK, int32_t) RDF_TEMPORAL(hour, BDF_TEMPORAL_HOUR, int32_t)
+    RDF_TEMPORAL(minute, BDF_TEMPORAL_MINUTE, int32_t) RDF_TEMPORAL(second, BDF_TEMPORAL_SECOND, int32_t)
+    RDF_TEMPORAL(to_date, BDF_TEMPORAL_TO_DATE, int32_t) RDF_TEMPORAL(last_day, BDF_TEMPORAL_LAST_DAY, int32_t)
+    RDF_TEMPORAL(unix_timestamp, BDF_TEMPORAL_UNIX_TIMESTAMP, int64_t)
+    RDF_TEMPORAL_ARG(date_add, BDF_TEMPORAL_DATE_ADD, int32_t) RDF_TEMPORAL_ARG(date_sub, BDF_TEMPORAL_DATE_SUB, int32_t)
+    RDF_TEMPORAL_ARG(add_months, BDF_TEMPORAL_ADD_MONTHS, int32_t) RDF_TEMPORAL_ARG(next_day, BDF_TEMPORAL_NEXT_DAY, int32_t)
+    RDF_TEMPORAL_ARG(to_timestamp, BDF_TEMPORAL_TO_TIMESTAMP, int64_t)
+#undef RDF_TEMPORAL
+#undef RDF_TEMPORAL_ARG
+    // date_trunc keeps the input's type: the result has the column's physical type T
+    template <typename T> static Out<T> date_trunc(const bdf_temporal_type& t, int64_t unit, const Arrays<T>& a) {
+        return detail::temporal<T, T>(BDF_TEMPORAL_DATE_TRUNC, t, unit, a);
+    }
 };
 
 // arrow::compute::cast over every chunk of a column (Function::Cast, src/evaluation.rs:296-315)

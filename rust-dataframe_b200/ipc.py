@@ -15,7 +15,7 @@ from typing import Dict, List, Optional, Sequence, Union
 import numpy as np
 
 from . import _native as N
-from .arrays import NP_DTYPES, BooleanArray, PrimitiveArray
+from .arrays import NP_DTYPES, BooleanArray, PrimitiveArray, TemporalType
 
 BOOL = 10
 
@@ -40,6 +40,13 @@ class IpcFile:
             N.raise_for_status(N.lib().bdf_ipc_list_column(self.handle, i, C.byref(ld)))
             if ld.value >= 0:
                 self.list_columns[self.schema[i][0]] = ld.value
+        # Date / Time / Timestamp columns also keep dtype -1 in `schema`; their types are here (read them by name)
+        self.temporal_columns = {}
+        for i in range(self.num_columns):
+            tt = N.TemporalTypeC()
+            N.raise_for_status(N.lib().bdf_ipc_temporal_column(self.handle, i, C.byref(tt)))
+            if tt.kind:
+                self.temporal_columns[self.schema[i][0]] = TemporalType(tt.kind, tt.unit, tt.tz.decode() if tt.tz else None)
 
     # -- lifetime --
     def close(self) -> None:
@@ -106,6 +113,21 @@ class IpcFile:
             idx = [i for i, (_, dt, _) in enumerate(self.schema) if dt >= 0]
         else:
             idx = [self.column_index(c) for c in columns]
+            temporal = [i for i in idx if self.schema[i][0] in self.temporal_columns]
+            if temporal:   # Date / Time / Timestamp columns come back as tagged Columns of their physical dtype
+                if batches is not None:
+                    raise N.UnsupportedType("temporal columns are read whole (every RecordBatch)")
+                ctx = ctx or N.default_context()
+                rest = [i for i in idx if i not in temporal]
+                res = self.read(rest, ctx, asynchronous) if rest else {}
+                for i in temporal:
+                    name = self.schema[i][0]
+                    h = C.c_void_p()
+                    N.raise_for_status(N.lib().bdf_ipc_read_temporal(ctx.handle, self.handle, i, N.ASYNC if asynchronous else 0, C.byref(h)))
+                    col = Column(ctx, h, self.temporal_columns[name])
+                    col._hold = self if asynchronous else None
+                    res[name] = col
+                return {self.schema[i][0]: res[self.schema[i][0]] for i in idx}
             lists = [i for i in idx if self.schema[i][0] in self.list_columns]
             if lists:   # List<T> columns come back as ListColumns, one chunk per RecordBatch
                 if batches is not None:
@@ -153,10 +175,17 @@ def write_ipc_host(path: str, columns: Dict[str, List]) -> None:
 
 
 def write_ipc(path: str, columns: Dict[str, "object"]) -> None:
-    """Device Columns -> IPC file (DataFrame::to_arrow)."""
+    """Device Columns -> IPC file (DataFrame::to_arrow).  Columns tagged with a TemporalType are written as Date / Time / Timestamp
+    fields (bdf_ipc_write_typed)."""
     names = list(columns)
     k = len(names)
     ctx = columns[names[0]].ctx
     cnames = (C.c_char_p * k)(*[s.encode() for s in names])
     handles = (C.c_void_p * k)(*[columns[s].handle for s in names])
+    tags = [getattr(columns[s], "temporal", None) for s in names]
+    if any(t is not None for t in tags):
+        types = (N.TemporalTypeC * k)(*[N.TemporalTypeC(t.kind, t.unit, t.tz.encode() if t.tz is not None else None) if t is not None
+                                         else N.TemporalTypeC(0, 0, None) for t in tags])
+        N.raise_for_status(N.lib().bdf_ipc_write_typed(ctx.handle, str(path).encode(), k, cnames, handles, types))
+        return
     N.raise_for_status(N.lib().bdf_ipc_write(ctx.handle, str(path).encode(), k, cnames, handles))
