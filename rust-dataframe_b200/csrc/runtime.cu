@@ -3711,24 +3711,38 @@ static int fleet_download(bdf_ctx* c, const bdf_col* col, bdf_out* out, int phas
     return BDF_OK;
 }
 
+// The inputs of one elementwise call on a fleet context: fleet columns whose chunks pair up as zip() pairs them, cut by one plan.
+// `*n` is the number of pairs.  Unequal chunk lengths are reported as `mismatch` and unequal chunk counts as `uneven`, because
+// the entries answer them differently (BDF_LENGTH_MISMATCH or BDF_INVALID, BDF_UNSUPPORTED or BDF_INVALID).
+static int fleet_zip(const bdf_col* const* cols, size_t n_cols, int mismatch, int uneven, int64_t* n) {
+    auto differ = [](int st) {
+        if (st == BDF_LENGTH_MISMATCH) return fail(st, "Cannot perform math operation on arrays of different length");
+        if (st == BDF_UNSUPPORTED) return fail(st, "columns with different numbers of chunks on a multi-GPU context");
+        return fail(BDF_INVALID, "the columns are sharded differently over the GPUs (upload them in one bdf_upload_many call)");
+    };
+    const bdf_col* first = cols[0];
+    *n = (int64_t)first->fmap.size();
+    for (size_t j = 0; j < n_cols; j++) {
+        if (!is_fleet_col(cols[j])) return fail(BDF_INVALID, "a column of a one-GPU context was passed to a multi-GPU context");
+        *n = std::min<int64_t>(*n, (int64_t)cols[j]->fmap.size());
+    }
+    for (size_t j = 0; j < n_cols; j++) {
+        for (int64_t i = 0; i < *n; i++)
+            if (cols[j]->flens[i] != first->flens[i]) return differ(mismatch);
+        if (!fleet_same_map(first, cols[j], *n)) return differ(BDF_INVALID);
+        if (cols[j]->fmap.size() != first->fmap.size()) return differ(uneven);
+    }
+    return BDF_OK;
+}
+
 // One elementwise operator over fleet columns: `call(k, parts of the inputs on kid k, &result part)`.
 static int fleet_map(bdf_ctx* c, int out_dtype, std::initializer_list<const bdf_col*> inputs, bdf_col** out,
                      const std::function<int(int, bdf_col**)>& call) {
     Fleet* f = c->fleet;
     const int nk = (int)f->kids.size();
-    const bdf_col* first = *inputs.begin();
-    int64_t n = (int64_t)first->fmap.size();
-    for (const bdf_col* col : inputs) {
-        if (!is_fleet_col(col)) return fail(BDF_INVALID, "a column of a one-GPU context was passed to a multi-GPU context");
-        n = std::min<int64_t>(n, (int64_t)col->fmap.size());   // zip()
-    }
-    for (const bdf_col* col : inputs) {
-        for (int64_t i = 0; i < n; i++)
-            if (col->flens[i] != first->flens[i]) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
-        if (!fleet_same_map(first, col, n)) return fail(BDF_INVALID, "the columns are sharded differently over the GPUs (upload them in one bdf_upload_many call)");
-        if (col->fmap.size() != first->fmap.size()) return fail(BDF_UNSUPPORTED, "columns with different numbers of chunks on a multi-GPU context");
-    }
-    bdf_col* o = fleet_col_like(first, out_dtype, nk, n);
+    int64_t n = 0;
+    TRY(fleet_zip(inputs.begin(), inputs.size(), BDF_LENGTH_MISMATCH, BDF_UNSUPPORTED, &n));
+    bdf_col* o = fleet_col_like(*inputs.begin(), out_dtype, nk, n);
     if (!o) return fail(BDF_OOM, "host allocation failed");
     int st = fleet_run(f, [&](int k) { return call(k, &o->fparts[k]); });
     if (st != BDF_OK) { const std::string keep = g_err; fleet_col_free(f, o); g_err = keep; return st; }
@@ -3861,38 +3875,14 @@ static int fleet_moments_dev(bdf_ctx* c, const bdf_col* col, bdf_moment_rec* out
     return BDF_OK;
 }
 
-static int fleet_moments_host(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_moment_rec* out) {
-    bdf_col* col = nullptr;
-    const int32_t dt = dtype;
-    const bdf_view* ptr = in;
-    TRY(fleet_upload_many(c, 1, &dt, &n, &ptr, BDF_ASYNC, &col));
-    const int st = fleet_moments_dev(c, col, out);
-    const std::string keep = g_err;
-    Fleet* f = c->fleet;
-    fleet_run(f, [&](int k) { return bdf_col_wait(f->kids[k], col->fparts[k]); });   // host inputs must not be touched after return
-    fleet_col_free(f, col);
-    g_err = keep;
-    return st;
-}
-
 // Fused operator + aggregate: every kid runs the one-GPU entry on its parts; the future yields the global records.
 static int fleet_with_future(bdf_ctx* c, int out_dtype, std::initializer_list<const bdf_col*> inputs, bool want_col, bdf_col** out, bdf_future** fut,
                              const std::function<int(int, bdf_col**, bdf_future**)>& call) {
     Fleet* f = c->fleet;
     const int nk = (int)f->kids.size();
-    const bdf_col* first = *inputs.begin();
-    int64_t n = (int64_t)first->fmap.size();
-    for (const bdf_col* col : inputs) {
-        if (!is_fleet_col(col)) return fail(BDF_INVALID, "a column of a one-GPU context was passed to a multi-GPU context");
-        n = std::min<int64_t>(n, (int64_t)col->fmap.size());
-    }
-    for (const bdf_col* col : inputs) {
-        for (int64_t i = 0; i < n; i++)
-            if (col->flens[i] != first->flens[i]) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
-        if (!fleet_same_map(first, col, n) || col->fmap.size() != first->fmap.size())
-            return fail(BDF_INVALID, "the columns are sharded differently over the GPUs (upload them in one bdf_upload_many call)");
-    }
-    bdf_col* o = want_col ? fleet_col_like(first, out_dtype, nk, n) : nullptr;
+    int64_t n = 0;
+    TRY(fleet_zip(inputs.begin(), inputs.size(), BDF_LENGTH_MISMATCH, BDF_INVALID, &n));
+    bdf_col* o = want_col ? fleet_col_like(*inputs.begin(), out_dtype, nk, n) : nullptr;
     bdf_future* fu = fleet_future_new(nk);
     if ((want_col && !o) || !fu) { fleet_col_free(f, o); delete fu; return fail(BDF_OOM, "host allocation failed"); }
     fu->n = 1;
@@ -3909,97 +3899,52 @@ static int fleet_with_future(bdf_ctx* c, int out_dtype, std::initializer_list<co
     return BDF_OK;
 }
 
-// Host in / host out over every GPU: shard the views, run the one-GPU drop-in entry per kid (its own PCIe link), fold the metadata.
-static int fleet_binary_host(bdf_ctx* c, int op, int dtype, int64_t n_left, const bdf_view* left, int64_t n_right, const bdf_view* right, bdf_out* out) {
+// Host in / host out over every GPU: shard the views of the inputs (chunk i of every input has the same length) by one plan,
+// run the one-GPU drop-in entry per kid on its pieces (its own PCIe link), fold the metadata into `out`.
+// `call(kid, pieces, views of every input, outs)`.
+template <class F>
+static int fleet_host_map(bdf_ctx* c, std::initializer_list<const bdf_view*> inputs, int64_t n, int out_dtype, bdf_out* out, F&& call) {
     Fleet* f = c->fleet;
     const int nk = (int)f->kids.size();
-    TRY(check_dtype(dtype));
-    if (n_left < 0 || n_right < 0 || (n_left && !left) || (n_right && !right)) return fail(BDF_INVALID, "bad arguments");
-    const int64_t n = std::min(n_left, n_right);
+    const size_t ni = inputs.size();
+    const bdf_view* first = *inputs.begin();
     std::vector<int64_t> lens((size_t)n);
     for (int64_t i = 0; i < n; i++) {
-        if (left[i].len != right[i].len) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
-        if (left[i].len < 0 || left[i].offset < 0 || right[i].offset < 0) return fail(BDF_INVALID, "bad view %lld", (long long)i);
-        lens[i] = left[i].len;
+        for (const bdf_view* in : inputs)
+            if (in[i].len != first[i].len) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
+        for (const bdf_view* in : inputs)
+            if (in[i].len < 0 || in[i].offset < 0) return fail(BDF_INVALID, "bad view %lld", (long long)i);
+        lens[i] = first[i].len;
     }
     const auto map = fleet_plan(lens, nk);
-    std::vector<std::vector<bdf_view>> lv((size_t)nk), rv((size_t)nk);
+    std::vector<std::vector<bdf_view>> iv((size_t)nk * ni);   // kid k, input j at k * ni + j
     std::vector<std::vector<bdf_out>> ov((size_t)nk);
-    for (int k = 0; k < nk; k++) { lv[k] = fleet_views(map, nk, k, left); rv[k] = fleet_views(map, nk, k, right); ov[k] = fleet_outs(map, k, dtype, out); }
+    for (int k = 0; k < nk; k++) {
+        size_t j = 0;
+        for (const bdf_view* in : inputs) iv[k * ni + j++] = fleet_views(map, nk, k, in);
+        ov[k] = fleet_outs(map, k, out_dtype, out);
+    }
     TRY(fleet_run(f, [&](int k) {
         bdf_view dv{}; bdf_out dummy{};
-        return bdf_binary(f->kids[k], op, dtype, (int64_t)lv[k].size(), lv[k].empty() ? &dv : lv[k].data(), (int64_t)rv[k].size(),
-                          rv[k].empty() ? &dv : rv[k].data(), ov[k].empty() ? &dummy : ov[k].data());
+        std::vector<const bdf_view*> v(ni);
+        for (size_t j = 0; j < ni; j++) v[j] = iv[k * ni + j].empty() ? &dv : iv[k * ni + j].data();
+        return call(f->kids[k], (int64_t)ov[k].size(), v.data(), ov[k].empty() ? &dummy : ov[k].data());
     }));
     fleet_merge_outs(map, ov, lens, out);
     return BDF_OK;
 }
 
-static int fleet_map_host(bdf_ctx* c, bool is_cast, int op_or_to, int dtype, int64_t n, const bdf_view* in, bdf_out* out) {
-    Fleet* f = c->fleet;
-    const int nk = (int)f->kids.size();
-    TRY(check_dtype(dtype));
-    if (n < 0 || (n && !in)) return fail(BDF_INVALID, "bad arguments");
-    std::vector<int64_t> lens((size_t)n);
-    for (int64_t i = 0; i < n; i++) {
-        if (in[i].len < 0 || in[i].offset < 0) return fail(BDF_INVALID, "bad view %lld", (long long)i);
-        lens[i] = in[i].len;
-    }
-    const auto map = fleet_plan(lens, nk);
-    const int out_dtype = is_cast ? op_or_to : dtype;
-    std::vector<std::vector<bdf_view>> iv((size_t)nk);
-    std::vector<std::vector<bdf_out>> ov((size_t)nk);
-    for (int k = 0; k < nk; k++) { iv[k] = fleet_views(map, nk, k, in); ov[k] = fleet_outs(map, k, out_dtype, out); }
-    TRY(fleet_run(f, [&](int k) {
-        bdf_view dv{}; bdf_out dummy{};
-        const bdf_view* vp = iv[k].empty() ? &dv : iv[k].data();
-        bdf_out* op_ = ov[k].empty() ? &dummy : ov[k].data();
-        return is_cast ? bdf_cast(f->kids[k], dtype, op_or_to, (int64_t)iv[k].size(), vp, op_) : bdf_unary(f->kids[k], op_or_to, dtype, (int64_t)iv[k].size(), vp, op_);
-    }));
-    fleet_merge_outs(map, ov, lens, out);
-    return BDF_OK;
-}
-
-// bdf_temporal over every GPU: the views are sharded as for bdf_unary, every kid runs the one-GPU entry on its pieces.
-static int fleet_temporal_host(bdf_ctx* c, int fn, const bdf_temporal_type* type, int64_t arg, int64_t n, const bdf_view* in, bdf_out* out) {
-    Fleet* f = c->fleet;
-    const int nk = (int)f->kids.size();
-    TemporalPlan pl;
-    TRY(temporal_plan(fn, type, arg, &pl));
-    if (n < 0 || (n && (!in || !out))) return fail(BDF_INVALID, "bad arguments");
-    std::vector<int64_t> lens((size_t)n);
-    for (int64_t i = 0; i < n; i++) {
-        if (in[i].len < 0 || in[i].offset < 0) return fail(BDF_INVALID, "bad view %lld", (long long)i);
-        lens[i] = in[i].len;
-    }
-    const auto map = fleet_plan(lens, nk);
-    std::vector<std::vector<bdf_view>> iv((size_t)nk);
-    std::vector<std::vector<bdf_out>> ov((size_t)nk);
-    for (int k = 0; k < nk; k++) { iv[k] = fleet_views(map, nk, k, in); ov[k] = fleet_outs(map, k, pl.out_dtype, out); }
-    TRY(fleet_run(f, [&](int k) {
-        bdf_view dv{}; bdf_out dummy{};
-        return bdf_temporal(f->kids[k], fn, type, arg, (int64_t)iv[k].size(), iv[k].empty() ? &dv : iv[k].data(), ov[k].empty() ? &dummy : ov[k].data());
-    }));
-    fleet_merge_outs(map, ov, lens, out);
-    return BDF_OK;
-}
-
-// Aggregates of a host column: upload the pieces (every GPU its own), reduce, combine; metadata rules over the caller's chunks.
-static int fleet_aggregate_host(bdf_ctx* c, int kind /* 0 one op, 1 all four, 2 avg */, int op, int dtype, int64_t n, const bdf_view* in, void* out_scalar,
-                                int32_t* is_some, bdf_agg4* all, double* avg) {
-    TRY(check_dtype(dtype));
-    if (n < 0 || (n && !in)) return fail(BDF_INVALID, "bad arguments");
+// A reduction of a host column over every GPU: upload the pieces (every GPU its own), run `body(fleet column)`, and wait for the
+// uploads before the column goes: host inputs must not be touched after return.
+template <class F>
+static int fleet_host_reduce(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, F&& body) {
     bdf_col* col = nullptr;
     const int32_t dt = dtype;
-    const bdf_view* ptr = in;
-    TRY(fleet_upload_many(c, 1, &dt, &n, &ptr, BDF_ASYNC, &col));
-    int st;
-    if (kind == 0) st = fleet_aggregate_dev(c, op, col, out_scalar, is_some);
-    else if (kind == 1) { const bdf_col* cc = col; st = fleet_aggregate_all_blocking(c, 1, &cc, all); }
-    else st = fleet_avg_dev(c, col, avg, is_some);
+    TRY(fleet_upload_many(c, 1, &dt, &n, &in, BDF_ASYNC, &col));
+    const int st = body(col);
     const std::string keep = g_err;
     Fleet* f = c->fleet;
-    fleet_run(f, [&](int k) { return bdf_col_wait(f->kids[k], col->fparts[k]); });   // host inputs must not be touched after return
+    fleet_run(f, [&](int k) { return bdf_col_wait(f->kids[k], col->fparts[k]); });
     fleet_col_free(f, col);
     g_err = keep;
     return st;
@@ -4569,10 +4514,30 @@ static int list_explode(bdf_ctx* c, const bdf_list* l, bdf_col** rows_out, bdf_c
 // ---------------------------------------------------------------------------------------------------
 // C ABI
 
+#define NEED_CTX(ctx) \
+    if (!(ctx)) return fail(BDF_INVALID, "null context")
+
+// An entry checks its arguments first (after NEED_CTX where the null context answers first), then hands a multi-GPU context to
+// the fleet, then ENTERs.  ENTER stays after the fleet dispatch: a fleet branch may call back into an entry with the same context,
+// and the context's mutex is not recursive.
 #define ENTER(ctx)                                                   \
-    if (!(ctx)) return fail(BDF_INVALID, "null context");           \
+    NEED_CTX(ctx);                                                   \
     std::lock_guard<std::mutex> _lock((ctx)->mu);                    \
     CK(cudaSetDevice((ctx)->device));
+
+// Host in / host out on one GPU: upload the views (the copies run ahead of the operator), run `body(uploaded columns)`, and wait
+// for the copies before the inputs go: the caller may reuse its host buffers as soon as the call returns.
+template <class F>
+static int host_call(bdf_ctx* c, const std::vector<UploadSpec>& specs, F&& body) {
+    std::vector<bdf_col*> cols;
+    TRY(upload_many(c, specs, true, cols));
+    const int st = body(cols.data());
+    const std::string keep = g_err;
+    cudaStreamSynchronize(c->s_h2d);
+    for (bdf_col* col : cols) col_release(c, col);
+    g_err = keep;
+    return st;
+}
 
 extern "C" {
 
@@ -4899,16 +4864,18 @@ int bdf_comm_barrier(bdf_ctx* c) {
 }
 
 int bdf_aggregate_all_many_dev_async(bdf_ctx* c, int32_t n_cols, const bdf_col* const* cols, bdf_future** fut) {
-    if (c && c->fleet) { if (!cols || !fut) return fail(BDF_INVALID, "null argument"); return fleet_aggregate_many(c, n_cols, cols, fut); }
-    ENTER(c);
+    NEED_CTX(c);
     if (!cols || !fut) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) return fleet_aggregate_many(c, n_cols, cols, fut);
+    ENTER(c);
     return aggregate_many_dev_async(c, n_cols, const_cast<bdf_col* const*>(cols), false, fut);
 }
 
 int bdf_aggregate_all_many_dev(bdf_ctx* c, int32_t n_cols, const bdf_col* const* cols, bdf_agg4* out) {
-    if (c && c->fleet) { if (!cols || !out) return fail(BDF_INVALID, "null argument"); return fleet_aggregate_all_blocking(c, n_cols, cols, out); }
-    ENTER(c);
+    NEED_CTX(c);
     if (!cols || !out) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) return fleet_aggregate_all_blocking(c, n_cols, cols, out);
+    ENTER(c);
     bdf_future* f = nullptr;
     TRY(aggregate_many_dev_async(c, n_cols, const_cast<bdf_col* const*>(cols), true, &f));
     return future_wait(c, f, out);
@@ -4919,15 +4886,14 @@ int bdf_future_count(const bdf_future* fut) { return fut ? fut->n : 0; }
 // ---- device-resident API -----------------------------------------------------------------------
 
 int bdf_upload(bdf_ctx* c, int dtype, int64_t n_chunks, const bdf_view* in, int flags, bdf_col** out) {
-    if (c && c->fleet) {
-        if (dtype != kBool) TRY(check_dtype(dtype));
-        if (!out || n_chunks < 0 || (n_chunks && !in)) return fail(BDF_INVALID, "bad arguments");
+    NEED_CTX(c);
+    if (dtype != kBool) TRY(check_dtype(dtype));
+    if (!out || n_chunks < 0 || (n_chunks && !in)) return fail(BDF_INVALID, "bad arguments");
+    if (c->fleet) {
         const int32_t dt = dtype;
         return fleet_upload_many(c, 1, &dt, &n_chunks, &in, flags, out);
     }
     ENTER(c);
-    if (dtype != kBool) TRY(check_dtype(dtype));
-    if (!out || n_chunks < 0 || (n_chunks && !in)) return fail(BDF_INVALID, "bad arguments");
     std::vector<bdf_col*> cols;
     TRY(upload_many(c, {UploadSpec{dtype, n_chunks, in}}, (flags & BDF_ASYNC) != 0, cols));
     *out = cols[0];
@@ -4936,22 +4902,16 @@ int bdf_upload(bdf_ctx* c, int dtype, int64_t n_chunks, const bdf_view* in, int 
 
 int bdf_upload_many(bdf_ctx* c, int64_t n_cols, const int32_t* dtypes, const int64_t* n_chunks, const bdf_view* const* in,
                     int flags, bdf_col** out) {
-    if (c && c->fleet) {
-        if (n_cols < 0 || (n_cols && (!dtypes || !n_chunks || !in || !out))) return fail(BDF_INVALID, "bad arguments");
-        for (int64_t k = 0; k < n_cols; k++) {
-            if (dtypes[k] != kBool) TRY(check_dtype(dtypes[k]));
-            if (n_chunks[k] < 0 || (n_chunks[k] && !in[k])) return fail(BDF_INVALID, "bad arguments for column %lld", (long long)k);
-        }
-        return fleet_upload_many(c, n_cols, dtypes, n_chunks, in, flags, out);
-    }
-    ENTER(c);
+    NEED_CTX(c);
     if (n_cols < 0 || (n_cols && (!dtypes || !n_chunks || !in || !out))) return fail(BDF_INVALID, "bad arguments");
-    std::vector<UploadSpec> specs;
     for (int64_t k = 0; k < n_cols; k++) {
         if (dtypes[k] != kBool) TRY(check_dtype(dtypes[k]));
         if (n_chunks[k] < 0 || (n_chunks[k] && !in[k])) return fail(BDF_INVALID, "bad arguments for column %lld", (long long)k);
-        specs.push_back(UploadSpec{dtypes[k], n_chunks[k], in[k]});
     }
+    if (c->fleet) return fleet_upload_many(c, n_cols, dtypes, n_chunks, in, flags, out);
+    ENTER(c);
+    std::vector<UploadSpec> specs;
+    for (int64_t k = 0; k < n_cols; k++) specs.push_back(UploadSpec{dtypes[k], n_chunks[k], in[k]});
     std::vector<bdf_col*> cols;
     TRY(upload_many(c, specs, (flags & BDF_ASYNC) != 0, cols));
     for (int64_t k = 0; k < n_cols; k++) out[k] = cols[k];
@@ -4994,35 +4954,29 @@ int bdf_col_chunk_info(bdf_ctx* c, const bdf_col* col, int64_t chunk, int64_t* l
 }
 
 int bdf_binary_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bdf_col** out) {
-    if (c && c->fleet) {
-        if (!l || !r || !out) return fail(BDF_INVALID, "null argument");
-        Fleet* f = c->fleet;
-        return fleet_map(c, l->dtype, {l, r}, out, [=](int k, bdf_col** o) { return bdf_binary_dev(f->kids[k], op, l->fparts[k], r->fparts[k], o); });
-    }
-    ENTER(c);
+    NEED_CTX(c);
     if (!l || !r || !out) return fail(BDF_INVALID, "null argument");
+    if (Fleet* f = c->fleet)
+        return fleet_map(c, l->dtype, {l, r}, out, [=](int k, bdf_col** o) { return bdf_binary_dev(f->kids[k], op, l->fparts[k], r->fparts[k], o); });
+    ENTER(c);
     return binary_dev(c, op, l, r, out);
 }
 
 int bdf_unary_dev(bdf_ctx* c, int op, const bdf_col* in, bdf_col** out) {
-    if (c && c->fleet) {
-        if (!in || !out) return fail(BDF_INVALID, "null argument");
-        Fleet* f = c->fleet;
-        return fleet_map(c, in->dtype, {in}, out, [=](int k, bdf_col** o) { return bdf_unary_dev(f->kids[k], op, in->fparts[k], o); });
-    }
-    ENTER(c);
+    NEED_CTX(c);
     if (!in || !out) return fail(BDF_INVALID, "null argument");
+    if (Fleet* f = c->fleet)
+        return fleet_map(c, in->dtype, {in}, out, [=](int k, bdf_col** o) { return bdf_unary_dev(f->kids[k], op, in->fparts[k], o); });
+    ENTER(c);
     return map_dev(c, false, op, in, out);
 }
 
 int bdf_cast_dev(bdf_ctx* c, int to, const bdf_col* in, bdf_col** out) {
-    if (c && c->fleet) {
-        if (!in || !out) return fail(BDF_INVALID, "null argument");
-        Fleet* f = c->fleet;
-        return fleet_map(c, to, {in}, out, [=](int k, bdf_col** o) { return bdf_cast_dev(f->kids[k], to, in->fparts[k], o); });
-    }
-    ENTER(c);
+    NEED_CTX(c);
     if (!in || !out) return fail(BDF_INVALID, "null argument");
+    if (Fleet* f = c->fleet)
+        return fleet_map(c, to, {in}, out, [=](int k, bdf_col** o) { return bdf_cast_dev(f->kids[k], to, in->fparts[k], o); });
+    ENTER(c);
     return map_dev(c, true, to, in, out);
 }
 
@@ -5037,21 +4991,22 @@ int bdf_temporal_result(int fn, const bdf_temporal_type* type, int64_t arg, int3
 int bdf_temporal_dev(bdf_ctx* c, int fn, const bdf_temporal_type* type, int64_t arg, const bdf_col* in, bdf_col** out) {
     TemporalPlan pl;
     TRY(temporal_plan(fn, type, arg, &pl));
-    if (c && c->fleet) {
-        if (!in || !out) return fail(BDF_INVALID, "null argument");
+    NEED_CTX(c);
+    if (!in || !out) return fail(BDF_INVALID, "null argument");
+    if (Fleet* f = c->fleet) {
         if (in->dtype != pl.in_dtype) return fail(BDF_INVALID, "a column of dtype %d does not hold this temporal type (dtype %d)", in->dtype, pl.in_dtype);
-        Fleet* f = c->fleet;
         return fleet_map(c, pl.out_dtype, {in}, out, [=](int k, bdf_col** o) { return bdf_temporal_dev(f->kids[k], fn, type, arg, in->fparts[k], o); });
     }
     ENTER(c);
-    if (!in || !out) return fail(BDF_INVALID, "null argument");
     return temporal_dev(c, pl, in, out);
 }
 
 int bdf_temporal_binary_dev(bdf_ctx* c, int fn, const bdf_temporal_type* ta, const bdf_col* a, const bdf_temporal_type* tb, const bdf_col* b,
                             bdf_col** out) {
-    if (c && c->fleet) {
-        if (!a || !b || !out || !ta || !tb) return fail(BDF_INVALID, "null argument");
+    NEED_CTX(c);
+    if (!a || !b || !out) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) {
+        if (!ta || !tb) return fail(BDF_INVALID, "null argument");
         if (fn != BDF_TEMPORAL_DATE_DIFF && fn != BDF_TEMPORAL_MONTHS_BETWEEN) return fail(BDF_INVALID, "unknown two-column temporal function %d", fn);
         int cfg = 0;
         int64_t off = 0;
@@ -5062,35 +5017,38 @@ int bdf_temporal_binary_dev(bdf_ctx* c, int fn, const bdf_temporal_type* ta, con
                          [=](int k, bdf_col** o) { return bdf_temporal_binary_dev(f->kids[k], fn, ta, a->fparts[k], tb, b->fparts[k], o); });
     }
     ENTER(c);
-    if (!a || !b || !out) return fail(BDF_INVALID, "null argument");
     return temporal_binary_dev(c, fn, ta, a, tb, b, out);
 }
 
 int bdf_aggregate_dev(bdf_ctx* c, int op, const bdf_col* in, void* out_scalar, int32_t* is_some) {
-    if (c && c->fleet) { if (!in || !out_scalar || !is_some) return fail(BDF_INVALID, "null argument"); return fleet_aggregate_dev(c, op, in, out_scalar, is_some); }
-    ENTER(c);
+    NEED_CTX(c);
     if (!in || !out_scalar || !is_some) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) return fleet_aggregate_dev(c, op, in, out_scalar, is_some);
+    ENTER(c);
     return aggregate_dev(c, op, const_cast<bdf_col*>(in), out_scalar, is_some);
 }
 
 int bdf_aggregate_all_dev(bdf_ctx* c, const bdf_col* in, bdf_agg4* out) {
-    if (c && c->fleet) { if (!in || !out) return fail(BDF_INVALID, "null argument"); return fleet_aggregate_all_blocking(c, 1, &in, out); }
-    ENTER(c);
+    NEED_CTX(c);
     if (!in || !out) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) return fleet_aggregate_all_blocking(c, 1, &in, out);
+    ENTER(c);
     return aggregate_all_dev(c, const_cast<bdf_col*>(in), true, out);
 }
 
 int bdf_avg_dev(bdf_ctx* c, const bdf_col* in, double* out, int32_t* is_some) {
-    if (c && c->fleet) { if (!in || !out || !is_some) return fail(BDF_INVALID, "null argument"); return fleet_avg_dev(c, in, out, is_some); }
-    ENTER(c);
+    NEED_CTX(c);
     if (!in || !out || !is_some) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) return fleet_avg_dev(c, in, out, is_some);
+    ENTER(c);
     return avg_dev(c, const_cast<bdf_col*>(in), out, is_some);
 }
 
 int bdf_moments_dev(bdf_ctx* c, const bdf_col* in, bdf_moment_rec* out) {
-    if (c && c->fleet) { if (!in || !out) return fail(BDF_INVALID, "null argument"); return fleet_moments_dev(c, in, out); }
-    ENTER(c);
+    NEED_CTX(c);
     if (!in || !out) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) return fleet_moments_dev(c, in, out);
+    ENTER(c);
     Moments m;
     TRY(moments_dev(c, in, &m));
     memcpy(out, &m, sizeof m);
@@ -5127,26 +5085,24 @@ int bdf_moments_merge(const bdf_moment_rec* a, const bdf_moment_rec* b, bdf_mome
 }
 
 int bdf_binary_agg_dev_async(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bdf_col** out, bdf_future** fut) {
-    if (c && c->fleet) {
-        if (!l || !r || !out || !fut) return fail(BDF_INVALID, "null argument");
-        Fleet* f = c->fleet;
+    NEED_CTX(c);
+    if (!l || !r || !out || !fut) return fail(BDF_INVALID, "null argument");
+    if (Fleet* f = c->fleet)
         return fleet_with_future(c, l->dtype, {l, r}, true, out, fut,
                                  [=](int k, bdf_col** o, bdf_future** fu) { return bdf_binary_agg_dev_async(f->kids[k], op, l->fparts[k], r->fparts[k], o, fu); });
-    }
     ENTER(c);
-    if (!l || !r || !out || !fut) return fail(BDF_INVALID, "null argument");
     return binary_dev(c, op, l, r, out, fut);
 }
 
 int bdf_binary_agg_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bdf_col** out, bdf_agg4* agg) {
-    if (c && c->fleet) {
-        if (!l || !r || !out || !agg) return fail(BDF_INVALID, "null argument");
+    NEED_CTX(c);
+    if (!l || !r || !out || !agg) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) {
         bdf_future* fu = nullptr;
         TRY(bdf_binary_agg_dev_async(c, op, l, r, out, &fu));
         return fleet_future_wait(c, fu, agg);
     }
     ENTER(c);
-    if (!l || !r || !out || !agg) return fail(BDF_INVALID, "null argument");
     bdf_future* f = nullptr;
     TRY(binary_dev(c, op, l, r, out, &f));
     return future_wait(c, f, agg);
@@ -5154,13 +5110,12 @@ int bdf_binary_agg_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, b
 
 int bdf_eval_expr_agg_dev_async(bdf_ctx* c, int32_t n_inputs, const bdf_col* const* inputs, int32_t n_nodes, const bdf_expr_node* nodes,
                                 bdf_col** out, bdf_future** fut) {
-    if (c && c->fleet) {
+    NEED_CTX(c);
+    if (Fleet* f = c->fleet) {
         if (!inputs || !nodes || !fut || n_inputs < 1 || n_inputs > 8) return fail(BDF_INVALID, "bad arguments");
         for (int i = 0; i < n_inputs; i++) if (!is_fleet_col(inputs[i])) return fail(BDF_INVALID, "null input column");
-        for (int i = 1; i < n_inputs; i++)
-            if (inputs[i]->fmap.size() != inputs[0]->fmap.size() || !fleet_same_map(inputs[0], inputs[i], (int64_t)inputs[0]->fmap.size()))
-                return fail(BDF_INVALID, "the columns are sharded differently over the GPUs (upload them in one bdf_upload_many call)");
-        Fleet* f = c->fleet;
+        int64_t n = 0;
+        TRY(fleet_zip(inputs, (size_t)n_inputs, BDF_INVALID, BDF_INVALID, &n));
         return fleet_with_future(c, BDF_F64, {inputs[0]}, out != nullptr, out, fut, [=](int k, bdf_col** o, bdf_future** fu) {
             const bdf_col* parts[8];
             for (int i = 0; i < n_inputs; i++) parts[i] = inputs[i]->fparts[k];
@@ -5174,30 +5129,33 @@ int bdf_eval_expr_agg_dev_async(bdf_ctx* c, int32_t n_inputs, const bdf_col* con
 
 int bdf_eval_expr_agg_dev(bdf_ctx* c, int32_t n_inputs, const bdf_col* const* inputs, int32_t n_nodes, const bdf_expr_node* nodes, bdf_col** out,
                           bdf_agg4* agg) {
-    if (c && c->fleet) {
-        if (!agg) return fail(BDF_INVALID, "null argument");
+    NEED_CTX(c);
+    if (!agg) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) {
         bdf_future* fu = nullptr;
         TRY(bdf_eval_expr_agg_dev_async(c, n_inputs, inputs, n_nodes, nodes, out, &fu));
         return fleet_future_wait(c, fu, agg);
     }
     ENTER(c);
-    if (!inputs || !nodes || !agg) return fail(BDF_INVALID, "null argument");
+    if (!inputs || !nodes) return fail(BDF_INVALID, "null argument");
     bdf_future* f = nullptr;
     TRY(expr_dev(c, n_inputs, inputs, n_nodes, nodes, out, &f));
     return future_wait(c, f, agg);
 }
 
 int bdf_aggregate_all_dev_async(bdf_ctx* c, const bdf_col* in, bdf_future** fut) {
-    if (c && c->fleet) { if (!in || !fut) return fail(BDF_INVALID, "null argument"); return fleet_aggregate_many(c, 1, &in, fut); }
-    ENTER(c);
+    NEED_CTX(c);
     if (!in || !fut) return fail(BDF_INVALID, "null argument");
+    if (c->fleet) return fleet_aggregate_many(c, 1, &in, fut);
+    ENTER(c);
     return aggregate_all_dev_async(c, const_cast<bdf_col*>(in), fut);
 }
 
 int bdf_future_wait(bdf_ctx* c, bdf_future* fut, bdf_agg4* out) {
-    if (c && c->fleet) { if (!fut) return fail(BDF_INVALID, "null future"); return fleet_future_wait(c, fut, out); }
-    ENTER(c);
+    NEED_CTX(c);
     if (!fut) return fail(BDF_INVALID, "null future");
+    if (c->fleet) return fleet_future_wait(c, fut, out);
+    ENTER(c);
     return future_wait(c, fut, out);
 }
 
@@ -5217,13 +5175,12 @@ int bdf_expr_check(int32_t n_inputs, const int32_t* input_dtypes, int32_t n_node
 }
 
 int bdf_eval_expr_dev(bdf_ctx* c, int32_t n_inputs, const bdf_col* const* inputs, int32_t n_nodes, const bdf_expr_node* nodes, bdf_col** out) {
-    if (c && c->fleet) {
+    NEED_CTX(c);
+    if (Fleet* f = c->fleet) {
         if (!inputs || !nodes || !out || n_inputs < 1 || n_inputs > 8) return fail(BDF_INVALID, "bad arguments");
         for (int i = 0; i < n_inputs; i++) if (!is_fleet_col(inputs[i])) return fail(BDF_INVALID, "null input column");
-        for (int i = 1; i < n_inputs; i++)
-            if (inputs[i]->fmap.size() != inputs[0]->fmap.size() || !fleet_same_map(inputs[0], inputs[i], (int64_t)inputs[0]->fmap.size()))
-                return fail(BDF_INVALID, "the columns are sharded differently over the GPUs (upload them in one bdf_upload_many call)");
-        Fleet* f = c->fleet;
+        int64_t n = 0;
+        TRY(fleet_zip(inputs, (size_t)n_inputs, BDF_INVALID, BDF_INVALID, &n));
         return fleet_map(c, BDF_F64, {inputs[0]}, out, [=](int k, bdf_col** o) {
             const bdf_col* parts[8];
             for (int i = 0; i < n_inputs; i++) parts[i] = inputs[i]->fparts[k];
@@ -5363,26 +5320,22 @@ int bdf_filter_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* mask, bdf_c
     return filter_dev(c, values, mask, out);
 }
 
-int bdf_download_begin(bdf_ctx* c, const bdf_col* col, bdf_out* out) {
-    if (c && c->fleet) { if (!is_fleet_col(col) || (!out && !col->fmap.empty())) return fail(BDF_INVALID, "null argument"); return fleet_download(c, col, out, 1); }
+static int download_entry(bdf_ctx* c, const bdf_col* col, bdf_out* out, int phase /* 0 both, 1 begin, 2 end */) {
+    NEED_CTX(c);
+    if (c->fleet) {
+        if (!is_fleet_col(col) || (!out && !col->fmap.empty())) return fail(BDF_INVALID, "null argument");
+        return fleet_download(c, col, out, phase);
+    }
     ENTER(c);
     if (!col || (!out && !col->chunks.empty())) return fail(BDF_INVALID, "null argument");
-    return download_enqueue(c, const_cast<bdf_col*>(col), out);
-}
-
-int bdf_download_end(bdf_ctx* c, const bdf_col* col, bdf_out* out) {
-    if (c && c->fleet) { if (!is_fleet_col(col) || (!out && !col->fmap.empty())) return fail(BDF_INVALID, "null argument"); return fleet_download(c, col, out, 2); }
-    ENTER(c);
-    if (!col || (!out && !col->chunks.empty())) return fail(BDF_INVALID, "null argument");
-    return download_finish(c, const_cast<bdf_col*>(col), out);
-}
-
-int bdf_download(bdf_ctx* c, const bdf_col* col, bdf_out* out) {
-    if (c && c->fleet) { if (!is_fleet_col(col) || (!out && !col->fmap.empty())) return fail(BDF_INVALID, "null argument"); return fleet_download(c, col, out, 0); }
-    ENTER(c);
-    if (!col || (!out && !col->chunks.empty())) return fail(BDF_INVALID, "null argument");
+    if (phase == 1) return download_enqueue(c, const_cast<bdf_col*>(col), out);
+    if (phase == 2) return download_finish(c, const_cast<bdf_col*>(col), out);
     return download(c, const_cast<bdf_col*>(col), out);
 }
+
+int bdf_download_begin(bdf_ctx* c, const bdf_col* col, bdf_out* out) { return download_entry(c, col, out, 1); }
+int bdf_download_end(bdf_ctx* c, const bdf_col* col, bdf_out* out) { return download_entry(c, col, out, 2); }
+int bdf_download(bdf_ctx* c, const bdf_col* col, bdf_out* out) { return download_entry(c, col, out, 0); }
 
 void bdf_col_free(bdf_ctx* c, bdf_col* col) {
     if (c && c->fleet) { fleet_col_free(c->fleet, col); return; }
@@ -5395,75 +5348,70 @@ void bdf_col_free(bdf_ctx* c, bdf_col* col) {
 // ---- host in / host out ------------------------------------------------------------------------
 
 int bdf_binary(bdf_ctx* c, int op, int dtype, int64_t n_left, const bdf_view* left, int64_t n_right, const bdf_view* right, bdf_out* out) {
-    if (c && c->fleet) { if (!out && std::min(n_left, n_right) > 0) return fail(BDF_INVALID, "bad arguments"); return fleet_binary_host(c, op, dtype, n_left, left, n_right, right, out); }
-    ENTER(c);
+    NEED_CTX(c);
+    if (c->fleet && !out && std::min(n_left, n_right) > 0) return fail(BDF_INVALID, "bad arguments");
     TRY(check_dtype(dtype));
     if (n_left < 0 || n_right < 0 || (n_left && !left) || (n_right && !right)) return fail(BDF_INVALID, "bad arguments");
     const int64_t n = std::min(n_left, n_right);
+    if (c->fleet)
+        return fleet_host_map(c, {left, right}, n, dtype, out, [=](bdf_ctx* kid, int64_t m, const bdf_view* const* v, bdf_out* o) {
+            return bdf_binary(kid, op, dtype, m, v[0], m, v[1], o);
+        });
+    ENTER(c);
     for (int64_t i = 0; i < n; i++)  // reject before moving a byte
         if (left[i].len != right[i].len) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
-    std::vector<bdf_col*> cols;
-    TRY(upload_many(c, {UploadSpec{dtype, n, left}, UploadSpec{dtype, n, right}}, true, cols));
-    bdf_col* o = nullptr;
-    int st = binary_dev(c, op, cols[0], cols[1], &o);
-    if (st == BDF_OK) st = download(c, o, out);
-    std::string keep = g_err;
-    cudaStreamSynchronize(c->s_h2d);  // host inputs must not be touched after return
-    col_release(c, o); col_release(c, cols[0]); col_release(c, cols[1]);
-    g_err = keep;
-    return st;
+    return host_call(c, {UploadSpec{dtype, n, left}, UploadSpec{dtype, n, right}}, [&](bdf_col* const* in) {
+        ColOwner o(c);
+        TRY(binary_dev(c, op, in[0], in[1], o.out()));
+        return download(c, o.get(), out);
+    });
 }
 
 static int map_host(bdf_ctx* c, bool is_cast, int op_or_to, int dtype, int64_t n, const bdf_view* in, bdf_out* out) {
+    NEED_CTX(c);
+    if (c->fleet && is_cast) TRY(check_dtype(op_or_to));
     TRY(check_dtype(dtype));
     if (n < 0 || (n && !in)) return fail(BDF_INVALID, "bad arguments");
-    std::vector<bdf_col*> cols;
-    TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
-    bdf_col* o = nullptr;
-    int st = map_dev(c, is_cast, op_or_to, cols[0], &o);
-    if (st == BDF_OK) st = download(c, o, out);
-    std::string keep = g_err;
-    cudaStreamSynchronize(c->s_h2d);
-    col_release(c, o); col_release(c, cols[0]);
-    g_err = keep;
-    return st;
+    if (c->fleet)
+        return fleet_host_map(c, {in}, n, is_cast ? op_or_to : dtype, out, [=](bdf_ctx* kid, int64_t m, const bdf_view* const* v, bdf_out* o) {
+            return is_cast ? bdf_cast(kid, dtype, op_or_to, m, v[0], o) : bdf_unary(kid, op_or_to, dtype, m, v[0], o);
+        });
+    ENTER(c);
+    return host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) {
+        ColOwner o(c);
+        TRY(map_dev(c, is_cast, op_or_to, cols[0], o.out()));
+        return download(c, o.get(), out);
+    });
 }
 
-int bdf_unary(bdf_ctx* c, int op, int dtype, int64_t n, const bdf_view* in, bdf_out* out) {
-    if (c && c->fleet) return fleet_map_host(c, false, op, dtype, n, in, out);
-    ENTER(c);
-    return map_host(c, false, op, dtype, n, in, out);
-}
+int bdf_unary(bdf_ctx* c, int op, int dtype, int64_t n, const bdf_view* in, bdf_out* out) { return map_host(c, false, op, dtype, n, in, out); }
 
-int bdf_cast(bdf_ctx* c, int from, int to, int64_t n, const bdf_view* in, bdf_out* out) {
-    if (c && c->fleet) { TRY(check_dtype(to)); return fleet_map_host(c, true, to, from, n, in, out); }
-    ENTER(c);
-    return map_host(c, true, to, from, n, in, out);
-}
+int bdf_cast(bdf_ctx* c, int from, int to, int64_t n, const bdf_view* in, bdf_out* out) { return map_host(c, true, to, from, n, in, out); }
 
 int bdf_temporal(bdf_ctx* c, int fn, const bdf_temporal_type* type, int64_t arg, int64_t n, const bdf_view* in, bdf_out* out) {
-    if (c && c->fleet) return fleet_temporal_host(c, fn, type, arg, n, in, out);
-    ENTER(c);
+    NEED_CTX(c);
     TemporalPlan pl;
     TRY(temporal_plan(fn, type, arg, &pl));
     if (n < 0 || (n && (!in || !out))) return fail(BDF_INVALID, "bad arguments");
-    std::vector<bdf_col*> cols;
-    TRY(upload_many(c, {UploadSpec{pl.in_dtype, n, in}}, true, cols));
-    bdf_col* o = nullptr;
-    int st = temporal_dev(c, pl, cols[0], &o);
-    if (st == BDF_OK) st = download(c, o, out);
-    std::string keep = g_err;
-    cudaStreamSynchronize(c->s_h2d);   // host inputs must not be touched after return
-    col_release(c, o); col_release(c, cols[0]);
-    g_err = keep;
-    return st;
+    if (c->fleet)
+        return fleet_host_map(c, {in}, n, pl.out_dtype, out, [=](bdf_ctx* kid, int64_t m, const bdf_view* const* v, bdf_out* o) {
+            return bdf_temporal(kid, fn, type, arg, m, v[0], o);
+        });
+    ENTER(c);
+    return host_call(c, {UploadSpec{pl.in_dtype, n, in}}, [&](bdf_col* const* cols) {
+        ColOwner o(c);
+        TRY(temporal_dev(c, pl, cols[0], o.out()));
+        return download(c, o.get(), out);
+    });
 }
 
 int bdf_aggregate(bdf_ctx* c, int op, int dtype, int64_t n, const bdf_view* in, void* out_scalar, int32_t* is_some) {
-    if (c && c->fleet) { if (!out_scalar || !is_some) return fail(BDF_INVALID, "bad arguments"); return fleet_aggregate_host(c, 0, op, dtype, n, in, out_scalar, is_some, nullptr, nullptr); }
-    ENTER(c);
+    NEED_CTX(c);
+    if (c->fleet && (!out_scalar || !is_some)) return fail(BDF_INVALID, "bad arguments");
     TRY(check_dtype(dtype));
     if (n < 0 || (n && !in) || !out_scalar || !is_some) return fail(BDF_INVALID, "bad arguments");
+    if (c->fleet) return fleet_host_reduce(c, dtype, n, in, [&](const bdf_col* col) { return fleet_aggregate_dev(c, op, col, out_scalar, is_some); });
+    ENTER(c);
     if (op == BDF_COUNT) {  // metadata only when every null_count is known: no bytes move
         bool known = true;
         int64_t total = 0;
@@ -5473,44 +5421,27 @@ int bdf_aggregate(bdf_ctx* c, int op, int dtype, int64_t n, const bdf_view* in, 
         }
         if (known) { TRY(count_global(c, &total)); *(int64_t*)out_scalar = total; *is_some = 1; return BDF_OK; }
     }
-    std::vector<bdf_col*> cols;
-    TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
-    int st = aggregate_dev(c, op, cols[0], out_scalar, is_some);
-    std::string keep = g_err;
-    cudaStreamSynchronize(c->s_h2d);
-    col_release(c, cols[0]);
-    g_err = keep;
-    return st;
+    return host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) { return aggregate_dev(c, op, cols[0], out_scalar, is_some); });
 }
 
 int bdf_aggregate_all(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_agg4* out) {
-    if (c && c->fleet) { if (!out) return fail(BDF_INVALID, "bad arguments"); return fleet_aggregate_host(c, 1, 0, dtype, n, in, nullptr, nullptr, out, nullptr); }
-    ENTER(c);
+    NEED_CTX(c);
+    if (c->fleet && !out) return fail(BDF_INVALID, "bad arguments");
     TRY(check_dtype(dtype));
     if (n < 0 || (n && !in) || !out) return fail(BDF_INVALID, "bad arguments");
-    std::vector<bdf_col*> cols;
-    TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
-    int st = aggregate_all_dev(c, cols[0], true, out);
-    std::string keep = g_err;
-    cudaStreamSynchronize(c->s_h2d);
-    col_release(c, cols[0]);
-    g_err = keep;
-    return st;
+    if (c->fleet) return fleet_host_reduce(c, dtype, n, in, [&](const bdf_col* col) { return fleet_aggregate_all_blocking(c, 1, &col, out); });
+    ENTER(c);
+    return host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) { return aggregate_all_dev(c, cols[0], true, out); });
 }
 
 int bdf_avg(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, double* out, int32_t* is_some) {
-    if (c && c->fleet) { if (!out || !is_some) return fail(BDF_INVALID, "bad arguments"); return fleet_aggregate_host(c, 2, 0, dtype, n, in, nullptr, is_some, nullptr, out); }
-    ENTER(c);
+    NEED_CTX(c);
+    if (c->fleet && (!out || !is_some)) return fail(BDF_INVALID, "bad arguments");
     TRY(check_dtype(dtype));
     if (n < 0 || (n && !in) || !out || !is_some) return fail(BDF_INVALID, "bad arguments");
-    std::vector<bdf_col*> cols;
-    TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
-    int st = avg_dev(c, cols[0], out, is_some);
-    std::string keep = g_err;
-    cudaStreamSynchronize(c->s_h2d);
-    col_release(c, cols[0]);
-    g_err = keep;
-    return st;
+    if (c->fleet) return fleet_host_reduce(c, dtype, n, in, [&](const bdf_col* col) { return fleet_avg_dev(c, col, out, is_some); });
+    ENTER(c);
+    return host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) { return avg_dev(c, cols[0], out, is_some); });
 }
 
 // Host-in entries of the statistics: a Boolean column is a type the operators do not take (BDF_UNSUPPORTED), not a bad dtype.
@@ -5520,24 +5451,17 @@ static int check_stat_dtype(int dtype) {
 }
 
 int bdf_moments(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_moment_rec* out) {
-    if (c && c->fleet) {
-        TRY(check_stat_dtype(dtype));
-        if (n < 0 || (n && !in) || !out) return fail(BDF_INVALID, "bad arguments");
-        return fleet_moments_host(c, dtype, n, in, out);
-    }
-    ENTER(c);
+    NEED_CTX(c);
     TRY(check_stat_dtype(dtype));
     if (n < 0 || (n && !in) || !out) return fail(BDF_INVALID, "bad arguments");
-    std::vector<bdf_col*> cols;
-    TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
-    Moments m;
-    int st = moments_dev(c, cols[0], &m);
-    std::string keep = g_err;
-    cudaStreamSynchronize(c->s_h2d);
-    col_release(c, cols[0]);
-    g_err = keep;
-    if (st == BDF_OK) memcpy(out, &m, sizeof m);
-    return st;
+    if (c->fleet) return fleet_host_reduce(c, dtype, n, in, [&](const bdf_col* col) { return fleet_moments_dev(c, col, out); });
+    ENTER(c);
+    return host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) {
+        Moments m;
+        TRY(moments_dev(c, cols[0], &m));
+        memcpy(out, &m, sizeof m);
+        return (int)BDF_OK;
+    });
 }
 
 int bdf_distinct(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_distinct_rec* out) {
@@ -5548,14 +5472,7 @@ int bdf_distinct(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_disti
     if (n < 0 || (n && !in) || !out) return fail(BDF_INVALID, "bad arguments");
     if (is_global(c))
         return fail(BDF_UNSUPPORTED, "distinct values need every row of the column on one GPU (as sort / group-by / join): use a one-GPU context");
-    std::vector<bdf_col*> cols;
-    TRY(upload_many(c, {UploadSpec{dtype, n, in}}, true, cols));
-    int st = distinct_dev(c, cols[0], out);
-    std::string keep = g_err;
-    cudaStreamSynchronize(c->s_h2d);
-    col_release(c, cols[0]);
-    g_err = keep;
-    return st;
+    return host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) { return distinct_dev(c, cols[0], out); });
 }
 
 // ---- measurement support -------------------------------------------------------------------------
@@ -5634,14 +5551,11 @@ int bdf_flush_l2(bdf_ctx* c, size_t bytes) {
 
 int bdf_generate(bdf_ctx* c, int dtype, int kind, double lo, double hi, uint64_t seed, uint64_t col_id, int64_t n_chunks,
                  const int64_t* chunk_lens, int64_t row0, uint32_t null_mod, bdf_col** out) {
-    if (c && c->fleet) {
-        TRY(check_dtype(dtype));
-        if (!out || n_chunks < 0 || (n_chunks && !chunk_lens) || kind < 0 || kind > 3) return fail(BDF_INVALID, "bad arguments");
-        return fleet_generate(c, dtype, kind, lo, hi, seed, col_id, n_chunks, chunk_lens, row0, null_mod, out);
-    }
-    ENTER(c);
+    NEED_CTX(c);
     TRY(check_dtype(dtype));
     if (!out || n_chunks < 0 || (n_chunks && !chunk_lens) || kind < 0 || kind > 3) return fail(BDF_INVALID, "bad arguments");
+    if (c->fleet) return fleet_generate(c, dtype, kind, lo, hi, seed, col_id, n_chunks, chunk_lens, row0, null_mod, out);
+    ENTER(c);
     std::vector<ChunkPlan> plan((size_t)n_chunks);
     for (int64_t i = 0; i < n_chunks; i++) {
         if (chunk_lens[i] < 0) return fail(BDF_INVALID, "negative chunk length");
