@@ -337,4 +337,133 @@ cudaError_t launch_temporal(int cfg, int in_dtype, int out_dtype, const Temporal
 cudaError_t launch_temporal2(int a_dtype, int b_dtype, int out_dtype, const TemporalParams2& p, const BinDesc* d_descs, int n_chunks,
                              int64_t total_tiles, uint32_t* d_warp_counts, cudaStream_t s);
 
+struct Moments;   // moments.cuh
+
+// Comparisons, and / or / not, filter (k_filter.cu).
+cudaError_t launch_compare(int op, const BinDesc* d, int n, int64_t tiles, int ta, int tb, bool scalar_rhs, double scalar, uint32_t* wc,
+                           cudaStream_t s);
+int compare_tile_elems();
+int bool_tile_elems();
+cudaError_t launch_boolean(int op, const void* d, int n, int64_t tiles, uint32_t* wc, cudaStream_t s);
+cudaError_t launch_filter_count(const void* d, int n, int64_t tiles, int tile_elems, unsigned int* tile_counts, long long* tile_offsets,
+                                long long* chunk_totals, cudaStream_t s);
+cudaError_t launch_filter_scatter(int dtype, const void* d, int n, int64_t tiles, const long long* tile_offsets, cudaStream_t s);
+size_t filter_desc_size();
+size_t bool_desc_size();
+void fill_filter_desc(void* base, int64_t i, const void* in, void* out, const uint32_t* vin, uint32_t* vout, const uint32_t* mval,
+                      const uint32_t* mvalid, int64_t len, int64_t tile0, int off, int moff, int mvoff);
+void fill_bool_desc(void* base, int64_t i, const uint32_t* a, const uint32_t* b, uint32_t* out, const uint32_t* va, const uint32_t* vb,
+                    uint32_t* vout, int64_t len, int64_t tile0, int offa, int offb, int voffa, int voffb);
+
+// A chain of Calculations fused into one pass (k_expr.cu).
+int expr_tile_elems();
+int expr_max_inputs();
+int expr_max_nodes();
+size_t expr_desc_size();
+void fill_expr_desc(void* base, int64_t i, int n_inputs, const void* const* in, const uint32_t* const* vin, const int32_t* off, double* out,
+                    uint32_t* vout, int64_t len, int64_t tile0);
+size_t expr_prog_size();
+void expr_prog_stats(const void* prog, int* n_instructions, int* n_temporaries);
+int expr_compile(int n_inputs, const int* in_dtypes, int n_nodes, const int* op, const int* a, const int* b, void* prog);
+cudaError_t launch_expr(const void* descs, int n_chunks, int64_t tiles, const void* prog, uint32_t* warp_counts, int* flags, AggDev* tile_partials,
+                        cudaStream_t s);
+
+// Sort indices and take (k_sort.cu).
+size_t sort_chunk_size();
+void fill_sort_chunk(void* base, int64_t i, const void* values, const uint32_t* validity, int64_t start, int32_t bit_off, int32_t val_bit_off);
+int sort_tile_elems();
+int take_tile_elems();
+int sort_pass_ctas(int64_t n, int sm_count);
+cudaError_t launch_iota(uint32_t* out, int64_t n, int sm_count, cudaStream_t s);
+int sort_key_bytes(int dtype);
+cudaError_t launch_sort_keys(int dtype, const void* chunks, int n_chunks, const uint32_t* idx, int64_t n, int mode, int descending,
+                             void* keys, unsigned long long* agree, int sm_count, cudaStream_t s);
+cudaError_t launch_radix_pass(int key_bytes, const void* keys_in, const uint32_t* idx_in, int64_t n, int shift, unsigned int* block_hist,
+                              void* keys_out, uint32_t* idx_out, int sm_count, cudaStream_t s);
+cudaError_t launch_take(int dtype, const void* vals, int n_vals, const void* idxs, int n_idxs, int64_t n, int64_t n_rows_values, void* out,
+                        uint32_t* vout, uint32_t* warp_counts, int* flags, cudaStream_t s);
+
+// Group-by (k_group.cu).
+cudaError_t launch_group_heads(int n_keys, const void* const* values, const uint32_t* const* valid, const int* widths, const int* is_float,
+                               int and_last_valid, long long n, uint32_t* words, cudaStream_t s);
+cudaError_t launch_group_reduce(int dtype, bool extra, const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows,
+                                void* sum, long long* count, void* mn, void* mx, double* avg, uint32_t* nonempty, void* scratch, int sm_count, cudaStream_t s);
+cudaError_t launch_group_bounds(const uint32_t* idx, const uint32_t* starts, long long n_groups, long long n_rows, uint32_t* first, uint32_t* last,
+                                cudaStream_t s);
+cudaError_t launch_group_distinct(const uint32_t* pos, long long n_pos, const uint32_t* starts, long long n_groups, long long n_rows, long long* out,
+                                  uint32_t* first, cudaStream_t s);
+cudaError_t launch_group_moments(int dtype, const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows,
+                                 Moments* mom, void* scratch, int sm_count, cudaStream_t s);
+cudaError_t launch_group_stats(const Moments* mom, long long n_groups, int stat, double* out, uint32_t* valid, cudaStream_t s);
+size_t group_big_scratch_bytes(long long n_rows);
+
+// Statistical aggregates (k_moments.cu).
+cudaError_t launch_moments(int dtype, const RedDesc* d, int n, int64_t tiles, Moments* partials, Moments* result, cudaStream_t s);
+int64_t moments_partials(int64_t tiles);
+
+// Joins (k_join.cu).
+int join_tile_rows();
+cudaError_t launch_join_count(int n_keys, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,
+                              const uint32_t* const* build_valid, long long n_probe, const uint32_t* run_starts, long long n_runs, long long n_build,
+                              int outer, unsigned long long* counts, uint32_t* match_start, unsigned char* hit, unsigned long long* block_sums,
+                              cudaStream_t s);
+cudaError_t launch_join_scan(unsigned long long* counts, long long n_probe, unsigned long long* block_sums, cudaStream_t s);
+cudaError_t launch_join_emit(const unsigned long long* offs, long long n_probe, const uint32_t* match_start, const uint32_t* perm, unsigned long long probe_rows,
+                             const uint32_t* unmatched, unsigned long long n_out, uint32_t* probe_out, uint32_t* probe_valid, uint32_t* build_out,
+                             uint32_t* build_valid, cudaStream_t s);
+cudaError_t launch_join_unmatched(const uint32_t* perm, long long n_build, const uint32_t* run_starts, long long n_runs, const unsigned char* hit,
+                                  uint32_t* mask, int sm_count, cudaStream_t s);
+
+// Window functions (k_window.cu).
+int window_count_tile();
+cudaError_t launch_window_count(const uint32_t* words, long long n_words, unsigned long long* counts, unsigned long long* block_sums, cudaStream_t s);
+cudaError_t launch_window_rank(const void* const* p, long long n_p, const void* const* q, long long n_q, long long n, const uint32_t* perm,
+                               void* const* outs, cudaStream_t s);
+cudaError_t launch_window_shift(int dtype, const void* const* p, long long n_p, long long n, const void* x, int nx, long long k, int lead,
+                                unsigned long long def_bits, int has_def, void* out, uint32_t* vout, cudaStream_t s);
+size_t window_scan_scratch_bytes(long long n);
+cudaError_t launch_window_scan(int dtype, int fn, const void* x, int nx, const uint32_t* heads, long long n, void* scratch, void* out, uint32_t* vout,
+                               cudaStream_t s);
+
+// CSV reader (k_csv.cu).
+int csv_tile_bytes();
+int csv_parse_rows();
+size_t csv_desc_bytes();
+size_t csv_slow_bytes();
+size_t csv_patch_bytes();
+cudaError_t launch_csv_tokenize(const uint8_t* text, long long n, uint8_t delim, uint32_t* agg, uint8_t* start, int* final_state, uint16_t* fe,
+                                uint16_t* re, unsigned long long* block_counts, cudaStream_t s);
+cudaError_t launch_csv_index(const uint16_t* fe, const uint16_t* re, long long n, const unsigned long long* block_offsets, unsigned long long* ends,
+                             unsigned long long* first_rec, cudaStream_t s);
+cudaError_t launch_csv_check(const unsigned long long* ends, long long n_fields, long long k, unsigned long long* bad, int sm_count, cudaStream_t s);
+cudaError_t launch_csv_infer(const uint8_t* text, const unsigned long long* ends, long long f0, long long f1, long long k, unsigned int* col_bits,
+                             int sm_count, cudaStream_t s);
+cudaError_t launch_csv_parse(const uint8_t* text, const unsigned long long* ends, const void* cols, int n_cols, long long f0, long long k, long long n_rows,
+                             long long batch, unsigned long long* err_key, void* slow, unsigned long long* n_slow, long long slow_cap, cudaStream_t s);
+cudaError_t launch_csv_scatter(const void* patches, long long n, cudaStream_t s);
+
+// CSV writer (k_csv_write.cu).
+int csvw_tile();
+cudaError_t launch_csvw_measure(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows,
+                                unsigned long long* lens, unsigned long long* block_sums, cudaStream_t s);
+cudaError_t launch_csvw_emit(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows, int delim,
+                             const unsigned long long* offs, char* out, cudaStream_t s);
+
+// List columns (k_list.cu).
+size_t list_find_scratch_bytes(long long n_elem);
+cudaError_t launch_list_find(int dtype, const int32_t* off, const uint32_t* lvalid, long long len, long long n_elem, const void* values,
+                             const uint32_t* vvalid, int vbit_off, uint64_t value_bits, int mode, uint32_t* bits, int32_t* pos, void* scratch,
+                             int sm_count, cudaStream_t s);
+cudaError_t launch_list_parent(const int32_t* off, const uint32_t* lvalid, const uint32_t* and_valid, long long len, long long n_elem, long long list0,
+                               long long elem0, uint32_t* parent, uint32_t* inlist, cudaStream_t s);
+cudaError_t launch_list_remove_mask(int dtype, const void* values, const uint32_t* vvalid, int vbit_off, long long n_elem, long long elem0,
+                                    uint64_t value_bits, const uint32_t* inlist, uint32_t* keep, cudaStream_t s);
+cudaError_t launch_list_mark(const uint32_t* perm, const uint32_t* head, const uint32_t* pvalid, long long n, long long split, int mode, uint32_t* keep,
+                             cudaStream_t s);
+cudaError_t launch_list_offsets(const uint32_t* kp, long long n_kept, long long n_lists, long long mult, int32_t* out, cudaStream_t s);
+cudaError_t launch_list_repeat(const int32_t* base, long long n_lists, long long count, const uint32_t* rows, long long n_out, uint32_t* src, cudaStream_t s);
+cudaError_t launch_list_size(const int32_t* off, const uint32_t* lvalid, long long len, int32_t* out, cudaStream_t s);
+cudaError_t launch_list_minmax_valid(const int32_t* off, const uint32_t* lvalid, const uint32_t* nonempty, long long len, uint32_t* valid, int* empty,
+                                     cudaStream_t s);
+
 }  // namespace bdf

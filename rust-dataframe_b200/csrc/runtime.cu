@@ -314,6 +314,16 @@ static cudaError_t ev_get(bdf_ctx* c, cudaEvent_t* ev) {
 }
 static void ev_put(bdf_ctx* c, cudaEvent_t ev) { if (ev) c->ev_pool.push_back(ev); }
 
+// Chunks [begin, end) of col are complete once the work enqueued on s so far has run: record that as one of its groups.
+static cudaError_t record_group(bdf_ctx* c, bdf_col* col, int64_t begin, int64_t end, cudaStream_t s) {
+    Group g{begin, end, nullptr};
+    cudaError_t e = ev_get(c, &g.ev);
+    if (e == cudaSuccess) e = cudaEventRecord(g.ev, s);
+    col->groups.push_back(g);
+    return e;
+}
+static cudaError_t finish_single_group(bdf_ctx* c, bdf_col* o) { return record_group(c, o, 0, (int64_t)o->chunks.size(), c->s_compute); }
+
 // Copy descriptors host ring -> device ring on the descriptor stream and make the compute stream wait for
 // them: the copy itself runs while the previous kernel is still busy.
 static cudaError_t desc_upload(bdf_ctx* c, void* dev, const void* host, size_t bytes) {
@@ -746,10 +756,7 @@ static int upload_many(bdf_ctx* c, const std::vector<UploadSpec>& specs, bool as
             for (size_t k = 0; k < specs.size() && e == cudaSuccess; k++) {
                 const int64_t b = std::min(group_begin, specs[k].n), en = std::min(i + 1, specs[k].n);
                 if (en <= b) continue;
-                Group g{b, en, nullptr};
-                e = ev_get(c, &g.ev);
-                if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_h2d);
-                cols[k]->groups.push_back(g);
+                e = record_group(c, cols[k].get(), b, en, c->s_h2d);
             }
             pending = 0;
             group_begin = i + 1;
@@ -890,94 +897,133 @@ static cudaError_t part_acquire(bdf_ctx* c, int64_t total_tiles, bdf_ctx::PartBu
     return e;
 }
 
+// zip() of k columns whose paired chunks must have the same length: *n = the number of chunk tuples.
+static int zip_chunks(const bdf_col* const* cols, int k, int64_t* n) {
+    *n = (int64_t)cols[0]->chunks.size();
+    for (int j = 1; j < k; j++) *n = std::min<int64_t>(*n, (int64_t)cols[j]->chunks.size());
+    for (int j = 1; j < k; j++)
+        for (int64_t i = 0; i < *n; i++)
+            if (cols[j]->chunks[i].len != cols[0]->chunks[i].len)
+                return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
+    return BDF_OK;
+}
+
+// Reads back the device flag the kernels raise (DivideByZero, an index out of bounds, an empty list): waits for the compute stream.
+// all_ranks: the max over the ranks of the communicator, so that every rank takes the same exit.
+static cudaError_t flag_read(bdf_ctx* c, bool all_ranks, int* flag) {
+    cudaError_t e = all_ranks ? flag_allreduce(c) : cudaSuccess;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    *flag = e == cudaSuccess ? *c->h_flag : 0;
+    return e;
+}
+
+// Folds the per-tile partials of a fused aggregate (K5, fused expressions) into the future on the finish stream, so that the next
+// operator on the compute stream does not wait for it.  The caller has made the finish stream wait for the launch that wrote them.
+static cudaError_t fused_finish(bdf_ctx* c, bdf_future* f, bdf_ctx::PartBuf* pb, int64_t tiles, int64_t n_chunks) {
+    c->launches++;
+    cudaError_t e = launch_finish(dtype_is_float(f->dtypes[0]), pb->p, tiles, c->sm_count, c->d_stage, c->d_ticket + 1, future_target(c, f, 0), c->s_fin);
+    if (e == cudaSuccess) e = cudaEventRecord(pb->done, c->s_fin);
+    pb->used = true;
+    f->chunks[0] = (uint32_t)n_chunks;
+    if (e == cudaSuccess) e = future_combine(c, f, c->s_fin);   // ranks of a communicator: one grouped NCCL reduction
+    if (e == cudaSuccess) e = cudaEventRecord(f->ev, c->s_fin);
+    return e;
+}
+
+// The launch loop of the element-wise operators.  Allocates the output column (plan, dtype, tile) and, for every chunk group
+// [begin, end) up to each of `ends`: fills the descriptors of its chunks, makes the compute stream wait for the inputs' groups,
+// uploads the descriptors, launches under one LaunchTimer and records the group's event on the output.  A group without chunks
+// launches nothing.
+//   fill(host descriptors, chunk i, tile0 of i within its group, output chunk i) -> the chunk's bytes for the launch record
+//   launch(device descriptors of the group, begin, end, tiles, tile_base = tiles of the groups before, warp counts) -> cudaError_t
+template <class Fill, class Launch>
+static int launch_groups(bdf_ctx* c, std::initializer_list<const bdf_col*> inputs, const std::vector<int64_t>& ends, int dtype,
+                         const std::vector<ChunkPlan>& plan, int tile, size_t desc_bytes, int kernel, const char* what, Fill fill,
+                         Launch launch, bdf_col** out) {
+    ColOwner o(c);
+    TRY(col_alloc(c, dtype, plan, nullptr, tile, o.out()));
+    o->counts_on_device = o->d_warp_counts != nullptr;
+    void *hp = nullptr, *dp = nullptr;
+    TRY(ring_alloc(c, plan.size() * desc_bytes, &hp, &dp));
+    char *hd = (char*)hp, *dd = (char*)dp;
+    cudaError_t e = cudaSuccess;
+    int64_t begin = 0, tile_base = 0;
+    for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
+        const int64_t end = ends[gi];
+        int64_t tiles = 0, rows = 0, bytes = 0;
+        for (int64_t i = begin; i < end; i++) {
+            bytes += fill((void*)hd, i, tiles, o->chunks[i]);
+            tiles += (plan[i].len + tile - 1) / tile;
+            rows += plan[i].len;
+        }
+        for (const bdf_col* in : inputs)
+            if (in) wait_groups(c->s_compute, in, begin, end);
+        if (end > begin) {
+            e = desc_upload(c, dd + begin * desc_bytes, hd + begin * desc_bytes, (size_t)(end - begin) * desc_bytes);
+            if (e == cudaSuccess) {
+                LaunchTimer t(c, kernel, dtype, rows, bytes);
+                e = launch((const void*)(dd + begin * desc_bytes), begin, end, tiles, tile_base,
+                           o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr);
+            }
+        }
+        if (e == cudaSuccess) e = record_group(c, o.get(), begin, end, c->s_compute);
+        begin = end;
+        tile_base += tiles;
+    }
+    if (e != cudaSuccess) return fail_cuda(e, what);
+    *out = o.release();
+    return BDF_OK;
+}
+
 static int binary_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bdf_col** out, bdf_future** fut = nullptr) {
     if (op < 0 || op >= BDF_NBINARY) return fail(BDF_INVALID, "invalid binary op %d", op);
     if (l->dtype != r->dtype) return fail(BDF_INVALID, "binary op on columns of different types (%d, %d)", l->dtype, r->dtype);
     if (l->dtype == kBool) return fail(BDF_UNSUPPORTED, "arithmetic on a boolean column");
     const int dtype = l->dtype;
     if (op > BDF_DIV && !dtype_is_float(dtype)) return fail(BDF_UNSUPPORTED, "atan2/hypot/log need a float column (T::Native: Float)");
-    const int64_t n = std::min<int64_t>((int64_t)l->chunks.size(), (int64_t)r->chunks.size());  // zip()
-    for (int64_t i = 0; i < n; i++)
-        if (l->chunks[i].len != r->chunks[i].len)
-            return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
+    const bdf_col* in[] = {l, r};
+    int64_t n = 0;
+    TRY(zip_chunks(in, 2, &n));
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++)
         plan[i] = {l->chunks[i].len, op > BDF_DIV || l->chunks[i].validity || r->chunks[i].validity};
-    ColOwner o(c);
     const int tile = elems_per_tile_binary(op, dtype);
-    TRY(col_alloc(c, dtype, plan, nullptr, tile, o.out()));
-    o->counts_on_device = o->d_warp_counts != nullptr;
-
     const int w = dtype_width(dtype);
-    void *hp = nullptr, *dp = nullptr;
-    TRY(ring_alloc(c, (size_t)n * sizeof(BinDesc), &hp, &dp));
-    BinDesc* dd = (BinDesc*)dp;
     cudaError_t e = cudaSuccess;
     // K5: aggregate of the output fused into the same pass -> one partial per tile, folded by k_finish
-    AggDev* partials = nullptr;
     bdf_ctx::PartBuf* pb = nullptr;
-    int64_t total_tiles = 0, tile_base = 0;
+    int64_t total_tiles = 0, total_rows = 0;
     FutOwner f(c);
     if (fut) {
         if (op > BDF_DIV) return fail(BDF_UNSUPPORTED, "fused aggregate is available for add/subtract/multiply/divide");
-        for (int64_t i = 0; i < n; i++) total_tiles += (l->chunks[i].len + tile - 1) / tile;
-        TRY(future_new(c, dtype, 1, o->total_len, f.out()));
+        for (int64_t i = 0; i < n; i++) { total_tiles += (plan[i].len + tile - 1) / tile; total_rows += plan[i].len; }
+        TRY(future_new(c, dtype, 1, total_rows, f.out()));
         e = part_acquire(c, total_tiles, &pb);
-        partials = pb->p;
     }
-    if (e == cudaSuccess) {
-        BinDesc* hd = (BinDesc*)hp;
-        const std::vector<int64_t> ends = plan_groups(n, {l, r});
-        if (op == BDF_DIV) e = cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute);
-        int64_t begin = 0;
-        for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
-            const int64_t end = ends[gi];
-            int64_t tiles = 0, rows = 0, bytes = 0;
-            for (int64_t i = begin; i < end; i++) {
-                const DevChunk &a = l->chunks[i], &b = r->chunks[i], &oc = o->chunks[i];
-                hd[i] = BinDesc{a.values, b.values, oc.values, a.validity, b.validity, oc.validity, a.len, tiles, a.bit_off, b.bit_off};
-                tiles += (a.len + tile - 1) / tile;
-                rows += a.len;
-                bytes += 3 * a.len * w + ((a.validity ? 1 : 0) + (b.validity ? 1 : 0) + (oc.validity ? 1 : 0)) * bitmap_bytes(a.len);
-            }
-            wait_groups(c->s_compute, l, begin, end);
-            wait_groups(c->s_compute, r, begin, end);
-            if (end > begin) {
-                e = desc_upload(c, dd + begin, hd + begin, (size_t)(end - begin) * sizeof(BinDesc));
-                if (e == cudaSuccess) {
-                    LaunchTimer t(c, BDF_K_BINARY, dtype, rows, bytes);
-                    e = launch_binary(op, dtype, dd + begin, (int)(end - begin), tiles, o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->d_flag, c->s_compute, partials ? partials + tile_base : nullptr);
-                }
-            }
-            if (e == cudaSuccess) {
-                Group g{begin, end, nullptr};
-                e = ev_get(c, &g.ev);
-                if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
-                o->groups.push_back(g);
-            }
-            begin = end;
-            tile_base += tiles;
-        }
-        if (e == cudaSuccess && f.get()) {
-            // fold the per-tile partials on the finish stream: the next operator on the compute stream does not wait
-            c->launches++;
-            for (auto& g : o->groups) cudaStreamWaitEvent(c->s_fin, g.ev, 0);
-            e = launch_finish(dtype_is_float(dtype), partials, total_tiles, c->sm_count, c->d_stage, c->d_ticket + 1, future_target(c, f.get(), 0), c->s_fin);
-            if (e == cudaSuccess) e = cudaEventRecord(pb->done, c->s_fin);
-            pb->used = true;
-            f->chunks[0] = (uint32_t)n;
-            if (e == cudaSuccess) e = future_combine(c, f.get(), c->s_fin);   // ranks of a communicator: one grouped NCCL reduction
-            if (e == cudaSuccess) e = cudaEventRecord(f->ev, c->s_fin);
-        }
-        if (e == cudaSuccess && op == BDF_DIV) {
-            // DivideByZero must be returned INSTEAD of data: wait for the flag (every rank of a communicator takes the same exit).
-            if (is_global(c)) e = flag_allreduce(c);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-            if (e == cudaSuccess && *c->h_flag) return fail(BDF_DIVIDE_BY_ZERO, "Divide by zero error");
-        }
-    }
+    const std::vector<int64_t> ends = plan_groups(n, {l, r});
+    if (e == cudaSuccess && op == BDF_DIV) e = cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute);
     if (e != cudaSuccess) return fail_cuda(e, "binary op");
+    ColOwner o(c);
+    TRY(launch_groups(c, {l, r}, ends, dtype, plan, tile, sizeof(BinDesc), BDF_K_BINARY, "binary op",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            const DevChunk &a = l->chunks[i], &b = r->chunks[i];
+            ((BinDesc*)hd)[i] = BinDesc{a.values, b.values, oc.values, a.validity, b.validity, oc.validity, a.len, tile0, a.bit_off, b.bit_off};
+            return 3 * a.len * w + ((a.validity ? 1 : 0) + (b.validity ? 1 : 0) + (oc.validity ? 1 : 0)) * bitmap_bytes(a.len);
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t tile_base, uint32_t* wc) {
+            return launch_binary(op, dtype, (const BinDesc*)dd, (int)(end - begin), tiles, wc, c->d_flag, c->s_compute, pb ? pb->p + tile_base : nullptr);
+        },
+        o.out()));
+    if (f.get()) {
+        for (auto& g : o->groups) cudaStreamWaitEvent(c->s_fin, g.ev, 0);
+        e = fused_finish(c, f.get(), pb, total_tiles, n);
+    }
+    // DivideByZero must be returned INSTEAD of data: wait for the flag (every rank of a communicator takes the same exit).
+    int flag = 0;
+    if (e == cudaSuccess && op == BDF_DIV) e = flag_read(c, is_global(c), &flag);
+    if (e != cudaSuccess) return fail_cuda(e, "binary op");
+    if (flag) return fail(BDF_DIVIDE_BY_ZERO, "Divide by zero error");
     *out = o.release();
     if (fut) *fut = f.release();
     return BDF_OK;
@@ -1004,49 +1050,20 @@ static int map_dev(bdf_ctx* c, bool is_cast, int op_or_to, const bdf_col* in, bd
     const bool fallible = is_cast && cast_is_fallible(from, to);
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++) plan[i] = {in->chunks[i].len, in->chunks[i].validity != nullptr || fallible};
-    ColOwner o(c);
     const int tile = is_cast ? elems_per_tile_cast(from, to) : elems_per_tile_unary(op_or_to, from);
-    TRY(col_alloc(c, to, plan, nullptr, tile, o.out()));
-    o->counts_on_device = o->d_warp_counts != nullptr;
-
     const int wf = dtype_width(from), wt = dtype_width(to);
-    void *hp = nullptr, *dp = nullptr;
-    TRY(ring_alloc(c, (size_t)n * sizeof(UnDesc), &hp, &dp));
-    UnDesc* dd = (UnDesc*)dp;
-    cudaError_t e = cudaSuccess;
-    UnDesc* hd = (UnDesc*)hp;
-    const std::vector<int64_t> ends = plan_groups(n, {in});
-    int64_t begin = 0;
-    for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
-        const int64_t end = ends[gi];
-        int64_t tiles = 0, rows = 0, bytes = 0;
-        for (int64_t i = begin; i < end; i++) {
-            const DevChunk &a = in->chunks[i], &oc = o->chunks[i];
-            hd[i] = UnDesc{a.values, oc.values, a.validity, oc.validity, a.len, tiles, a.bit_off, 0};
-            tiles += (a.len + tile - 1) / tile;
-            rows += a.len;
-            bytes += a.len * (wf + wt) + ((a.validity ? 1 : 0) + (oc.validity ? 1 : 0)) * bitmap_bytes(a.len);
-        }
-        wait_groups(c->s_compute, in, begin, end);
-        if (end > begin) {
-            e = desc_upload(c, dd + begin, hd + begin, (size_t)(end - begin) * sizeof(UnDesc));
-            if (e == cudaSuccess) {
-                LaunchTimer t(c, is_cast ? BDF_K_CAST : BDF_K_UNARY, to, rows, bytes);
-                e = is_cast ? launch_cast(from, to, dd + begin, (int)(end - begin), tiles, o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute)
-                            : launch_unary(op_or_to, from, dd + begin, (int)(end - begin), tiles, o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute);
-            }
-        }
-        if (e == cudaSuccess) {
-            Group g{begin, end, nullptr};
-            e = ev_get(c, &g.ev);
-            if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
-            o->groups.push_back(g);
-        }
-        begin = end;
-    }
-    if (e != cudaSuccess) return fail_cuda(e, is_cast ? "cast" : "unary op");
-    *out = o.release();
-    return BDF_OK;
+    return launch_groups(c, {in}, plan_groups(n, {in}), to, plan, tile, sizeof(UnDesc), is_cast ? BDF_K_CAST : BDF_K_UNARY,
+        is_cast ? "cast" : "unary op",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            const DevChunk& a = in->chunks[i];
+            ((UnDesc*)hd)[i] = UnDesc{a.values, oc.values, a.validity, oc.validity, a.len, tile0, a.bit_off, 0};
+            return a.len * (wf + wt) + ((a.validity ? 1 : 0) + (oc.validity ? 1 : 0)) * bitmap_bytes(a.len);
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t* wc) {
+            return is_cast ? launch_cast(from, to, (const UnDesc*)dd, (int)(end - begin), tiles, wc, c->s_compute)
+                           : launch_unary(op_or_to, from, (const UnDesc*)dd, (int)(end - begin), tiles, wc, c->s_compute);
+        },
+        out);
 }
 
 // ---- dates and timestamps (k_temporal.cu; the rules are stated in include/b200df.h) ----------------------------------------------
@@ -1137,48 +1154,18 @@ static int temporal_dev(bdf_ctx* c, const TemporalPlan& pl, const bdf_col* in, b
     const int64_t n = (int64_t)in->chunks.size();
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++) plan[i] = {in->chunks[i].len, true};   // range rules can turn any slot NULL
-    ColOwner o(c);
     const int tile = elems_per_tile_temporal(pl.in_dtype, pl.out_dtype);
-    TRY(col_alloc(c, pl.out_dtype, plan, nullptr, tile, o.out()));
-    o->counts_on_device = o->d_warp_counts != nullptr;
     const int wi = dtype_width(pl.in_dtype), wo = dtype_width(pl.out_dtype);
-    void *hp = nullptr, *dp = nullptr;
-    TRY(ring_alloc(c, (size_t)n * sizeof(UnDesc), &hp, &dp));
-    UnDesc* dd = (UnDesc*)dp;
-    UnDesc* hd = (UnDesc*)hp;
-    cudaError_t e = cudaSuccess;
-    const std::vector<int64_t> ends = plan_groups(n, {in});
-    int64_t begin = 0;
-    for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
-        const int64_t end = ends[gi];
-        int64_t tiles = 0, rows = 0, bytes = 0;
-        for (int64_t i = begin; i < end; i++) {
-            const DevChunk &a = in->chunks[i], &oc = o->chunks[i];
-            hd[i] = UnDesc{a.values, oc.values, a.validity, oc.validity, a.len, tiles, a.bit_off, 0};
-            tiles += (a.len + tile - 1) / tile;
-            rows += a.len;
-            bytes += a.len * (wi + wo) + ((a.validity ? 1 : 0) + 1) * bitmap_bytes(a.len);
-        }
-        wait_groups(c->s_compute, in, begin, end);
-        if (end > begin) {
-            e = desc_upload(c, dd + begin, hd + begin, (size_t)(end - begin) * sizeof(UnDesc));
-            if (e == cudaSuccess) {
-                LaunchTimer t(c, BDF_K_TEMPORAL, pl.out_dtype, rows, bytes);
-                e = launch_temporal(pl.cfg, pl.in_dtype, pl.out_dtype, pl.p, dd + begin, (int)(end - begin), tiles,
-                                    o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute);
-            }
-        }
-        if (e == cudaSuccess) {
-            Group g{begin, end, nullptr};
-            e = ev_get(c, &g.ev);
-            if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
-            o->groups.push_back(g);
-        }
-        begin = end;
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "temporal function");
-    *out = o.release();
-    return BDF_OK;
+    return launch_groups(c, {in}, plan_groups(n, {in}), pl.out_dtype, plan, tile, sizeof(UnDesc), BDF_K_TEMPORAL, "temporal function",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            const DevChunk& a = in->chunks[i];
+            ((UnDesc*)hd)[i] = UnDesc{a.values, oc.values, a.validity, oc.validity, a.len, tile0, a.bit_off, 0};
+            return a.len * (wi + wo) + ((a.validity ? 1 : 0) + 1) * bitmap_bytes(a.len);
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t* wc) {
+            return launch_temporal(pl.cfg, pl.in_dtype, pl.out_dtype, pl.p, (const UnDesc*)dd, (int)(end - begin), tiles, wc, c->s_compute);
+        },
+        out);
 }
 
 // One side of a two-column temporal function: a date kind, its storage and its fixed offset in its own units.
@@ -1203,54 +1190,23 @@ static int temporal_binary_dev(bdf_ctx* c, int fn, const bdf_temporal_type* ta, 
     TRY(temporal_side(ta, a, &p.cfg_a, &p.off_a));
     TRY(temporal_side(tb, b, &p.cfg_b, &p.off_b));
     const int out_dtype = fn == BDF_TEMPORAL_DATE_DIFF ? BDF_I32 : BDF_F64;
-    const int64_t n = std::min<int64_t>((int64_t)a->chunks.size(), (int64_t)b->chunks.size());   // zip()
-    for (int64_t i = 0; i < n; i++)
-        if (a->chunks[i].len != b->chunks[i].len) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
+    const bdf_col* in[] = {a, b};
+    int64_t n = 0;
+    TRY(zip_chunks(in, 2, &n));
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++) plan[i] = {a->chunks[i].len, true};
-    ColOwner o(c);
     const int tile = elems_per_tile_temporal2(a->dtype, b->dtype, out_dtype);
-    TRY(col_alloc(c, out_dtype, plan, nullptr, tile, o.out()));
-    o->counts_on_device = o->d_warp_counts != nullptr;
     const int wrow = dtype_width(a->dtype) + dtype_width(b->dtype) + dtype_width(out_dtype);
-    void *hp = nullptr, *dp = nullptr;
-    TRY(ring_alloc(c, (size_t)n * sizeof(BinDesc), &hp, &dp));
-    BinDesc* dd = (BinDesc*)dp;
-    BinDesc* hd = (BinDesc*)hp;
-    cudaError_t e = cudaSuccess;
-    const std::vector<int64_t> ends = plan_groups(n, {a, b});
-    int64_t begin = 0;
-    for (size_t gi = 0; gi < ends.size() && e == cudaSuccess; gi++) {
-        const int64_t end = ends[gi];
-        int64_t tiles = 0, rows = 0, bytes = 0;
-        for (int64_t i = begin; i < end; i++) {
-            const DevChunk &x = a->chunks[i], &y = b->chunks[i], &oc = o->chunks[i];
-            hd[i] = BinDesc{x.values, y.values, oc.values, x.validity, y.validity, oc.validity, x.len, tiles, x.bit_off, y.bit_off};
-            tiles += (x.len + tile - 1) / tile;
-            rows += x.len;
-            bytes += x.len * wrow + ((x.validity ? 1 : 0) + (y.validity ? 1 : 0) + 1) * bitmap_bytes(x.len);
-        }
-        wait_groups(c->s_compute, a, begin, end);
-        wait_groups(c->s_compute, b, begin, end);
-        if (end > begin) {
-            e = desc_upload(c, dd + begin, hd + begin, (size_t)(end - begin) * sizeof(BinDesc));
-            if (e == cudaSuccess) {
-                LaunchTimer t(c, BDF_K_TEMPORAL, out_dtype, rows, bytes);
-                e = launch_temporal2(a->dtype, b->dtype, out_dtype, p, dd + begin, (int)(end - begin), tiles,
-                                     o->d_warp_counts ? o->d_warp_counts + o->tile0[begin] * kWarpsPerCta : nullptr, c->s_compute);
-            }
-        }
-        if (e == cudaSuccess) {
-            Group g{begin, end, nullptr};
-            e = ev_get(c, &g.ev);
-            if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
-            o->groups.push_back(g);
-        }
-        begin = end;
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "temporal function");
-    *out = o.release();
-    return BDF_OK;
+    return launch_groups(c, {a, b}, plan_groups(n, {a, b}), out_dtype, plan, tile, sizeof(BinDesc), BDF_K_TEMPORAL, "temporal function",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            const DevChunk &x = a->chunks[i], &y = b->chunks[i];
+            ((BinDesc*)hd)[i] = BinDesc{x.values, y.values, oc.values, x.validity, y.validity, oc.validity, x.len, tile0, x.bit_off, y.bit_off};
+            return x.len * wrow + ((x.validity ? 1 : 0) + (y.validity ? 1 : 0) + 1) * bitmap_bytes(x.len);
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t* wc) {
+            return launch_temporal2(a->dtype, b->dtype, out_dtype, p, (const BinDesc*)dd, (int)(end - begin), tiles, wc, c->s_compute);
+        },
+        out);
 }
 
 static int boolean_dev(bdf_ctx* c, int op, const bdf_col* a, const bdf_col* b, bdf_col** out);
@@ -1560,109 +1516,56 @@ static int avg_dev(bdf_ctx* c, bdf_col* col, double* out, int32_t* is_some) {
 // ---------------------------------------------------------------------------------------------------
 // N2: BooleanFilter comparisons, boolean kernels, filter (k_filter.cu)
 
-namespace bdf {
-cudaError_t launch_compare(int op, const BinDesc* d, int n, int64_t tiles, int ta, int tb, bool scalar_rhs, double scalar, uint32_t* wc,
-                           cudaStream_t s);
-int compare_tile_elems();
-int bool_tile_elems();
-cudaError_t launch_boolean(int op, const void* d, int n, int64_t tiles, uint32_t* wc, cudaStream_t s);
-cudaError_t launch_filter_count(const void* d, int n, int64_t tiles, int tile_elems, unsigned int* tile_counts, long long* tile_offsets,
-                                long long* chunk_totals, cudaStream_t s);
-cudaError_t launch_filter_scatter(int dtype, const void* d, int n, int64_t tiles, const long long* tile_offsets, cudaStream_t s);
-size_t filter_desc_size();
-size_t bool_desc_size();
-void fill_filter_desc(void* base, int64_t i, const void* in, void* out, const uint32_t* vin, uint32_t* vout, const uint32_t* mval,
-                      const uint32_t* mvalid, int64_t len, int64_t tile0, int off, int moff, int mvoff);
-void fill_bool_desc(void* base, int64_t i, const uint32_t* a, const uint32_t* b, uint32_t* out, const uint32_t* va, const uint32_t* vb,
-                    uint32_t* vout, int64_t len, int64_t tile0, int offa, int offb, int voffa, int voffb);
-}  // namespace bdf
-
-static cudaError_t finish_single_group(bdf_ctx* c, bdf_col* o) {
-    Group g{0, (int64_t)o->chunks.size(), nullptr};
-    cudaError_t e = ev_get(c, &g.ev);
-    if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
-    o->groups.push_back(g);
-    return e;
-}
-
 // BooleanFilter::{Gt,..,Le}: cast both sides to Float64 (as the reference does, expression.rs:820-845), compare.  The casts are
 // fused into the kernel's loads.
 static int compare_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, double scalar, bdf_col** out) {
     if (op < 0 || op > 5) return fail(BDF_INVALID, "invalid comparison op %d", op);
     if (l->dtype == kBool || (r && r->dtype == kBool)) return fail(BDF_UNSUPPORTED, "comparison of boolean columns is not part of this path");
-    const int64_t n = r ? std::min<int64_t>((int64_t)l->chunks.size(), (int64_t)r->chunks.size()) : (int64_t)l->chunks.size();
-    for (int64_t i = 0; r && i < n; i++)
-        if (l->chunks[i].len != r->chunks[i].len) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
+    const bdf_col* in[] = {l, r};
+    int64_t n = 0;
+    TRY(zip_chunks(in, r ? 2 : 1, &n));
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++) plan[i] = {l->chunks[i].len, l->chunks[i].validity != nullptr || (r && r->chunks[i].validity != nullptr)};
-    const int tile = compare_tile_elems();
-    ColOwner o(c);
-    TRY(col_alloc(c, kBool, plan, nullptr, tile, o.out()));
-    o->counts_on_device = o->d_warp_counts != nullptr;
-    void *hp = nullptr, *dp = nullptr;
-    TRY(ring_alloc(c, (size_t)n * sizeof(BinDesc), &hp, &dp));
-    BinDesc* hd = (BinDesc*)hp;
-    int64_t tiles = 0, rows = 0, bytes = 0;
-    for (int64_t i = 0; i < n; i++) {
-        const DevChunk& a = l->chunks[i];
-        const DevChunk* b = r ? &r->chunks[i] : nullptr;
-        const DevChunk& oc = o->chunks[i];
-        hd[i] = BinDesc{a.values, b ? b->values : nullptr, oc.values, a.validity, b ? b->validity : nullptr, oc.validity, a.len, tiles,
-                        a.bit_off, b ? b->bit_off : 0};
-        tiles += (a.len + tile - 1) / tile;
-        rows += a.len;
-        bytes += (dtype_width(l->dtype) + (b ? dtype_width(r->dtype) : 0)) * a.len +
-                 bitmap_bytes(a.len) * (1 + (a.validity ? 1 : 0) + (b && b->validity ? 1 : 0) + (oc.validity ? 1 : 0));
-    }
-    wait_groups(c->s_compute, l, 0, n);
-    if (r) wait_groups(c->s_compute, r, 0, n);
-    cudaError_t e = desc_upload(c, dp, hd, (size_t)n * sizeof(BinDesc));
-    if (e == cudaSuccess) {
-        LaunchTimer t(c, BDF_K_COMPARE, kBool, rows, bytes);
-        e = launch_compare(op, (const BinDesc*)dp, (int)n, tiles, l->dtype, r ? r->dtype : BDF_F64, r == nullptr, scalar, o->d_warp_counts, c->s_compute);
-    }
-    if (e == cudaSuccess) e = finish_single_group(c, o.get());
-    if (e != cudaSuccess) return fail_cuda(e, "compare");
-    *out = o.release();
-    return BDF_OK;
+    const int wrow = dtype_width(l->dtype) + (r ? dtype_width(r->dtype) : 0);
+    return launch_groups(c, {l, r}, {n}, kBool, plan, compare_tile_elems(), sizeof(BinDesc), BDF_K_COMPARE, "compare",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            const DevChunk& a = l->chunks[i];
+            const DevChunk* b = r ? &r->chunks[i] : nullptr;
+            ((BinDesc*)hd)[i] = BinDesc{a.values, b ? b->values : nullptr, oc.values, a.validity, b ? b->validity : nullptr, oc.validity, a.len, tile0,
+                                        a.bit_off, b ? b->bit_off : 0};
+            return wrow * a.len + bitmap_bytes(a.len) * (1 + (a.validity ? 1 : 0) + (b && b->validity ? 1 : 0) + (oc.validity ? 1 : 0));
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t* wc) {
+            return launch_compare(op, (const BinDesc*)dd, (int)(end - begin), tiles, l->dtype, r ? r->dtype : BDF_F64, r == nullptr, scalar, wc, c->s_compute);
+        },
+        out);
 }
 
 static int boolean_dev(bdf_ctx* c, int op, const bdf_col* a, const bdf_col* b, bdf_col** out) {
     if (op < 0 || op > 2) return fail(BDF_INVALID, "invalid boolean op %d", op);
     if (a->dtype != kBool || (op != 2 && (!b || b->dtype != kBool))) return fail(BDF_UNSUPPORTED, "and/or/not need boolean columns");
     if (op == 2) b = nullptr;
-    const int64_t n = b ? std::min<int64_t>((int64_t)a->chunks.size(), (int64_t)b->chunks.size()) : (int64_t)a->chunks.size();
-    for (int64_t i = 0; b && i < n; i++)
-        if (a->chunks[i].len != b->chunks[i].len) return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
+    const bdf_col* in[] = {a, b};
+    int64_t n = 0;
+    TRY(zip_chunks(in, b ? 2 : 1, &n));
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t i = 0; i < n; i++) plan[i] = {a->chunks[i].len, a->chunks[i].validity != nullptr || (b && b->chunks[i].validity != nullptr)};
-    const int tile = bool_tile_elems();
-    ColOwner o(c);
-    TRY(col_alloc(c, kBool, plan, nullptr, tile, o.out()));
-    o->counts_on_device = o->d_warp_counts != nullptr;
-    void *hp = nullptr, *dp = nullptr;
-    TRY(ring_alloc(c, (size_t)n * bool_desc_size(), &hp, &dp));
-    int64_t tiles = 0, rows = 0;
-    for (int64_t i = 0; i < n; i++) {
-        const DevChunk& x = a->chunks[i];
-        const DevChunk* y = b ? &b->chunks[i] : nullptr;
-        const DevChunk& oc = o->chunks[i];
-        fill_bool_desc(hp, i, (const uint32_t*)x.values, y ? (const uint32_t*)y->values : nullptr, (uint32_t*)oc.values, x.validity,
-                       y ? y->validity : nullptr, oc.validity, x.len, tiles, x.val_bit_off, y ? y->val_bit_off : 0, x.bit_off, y ? y->bit_off : 0);
-        tiles += (x.len + tile - 1) / tile;
-        rows += x.len;
-    }
-    wait_groups(c->s_compute, a, 0, n);
-    if (b) wait_groups(c->s_compute, b, 0, n);
-    cudaError_t e = desc_upload(c, dp, hp, (size_t)n * bool_desc_size());
-    if (e == cudaSuccess) {
-        LaunchTimer t(c, BDF_K_COMPARE, kBool, rows, rows / 8 * (b ? 3 : 2));
-        e = launch_boolean(op, dp, (int)n, tiles, o->d_warp_counts, c->s_compute);
-    }
-    if (e == cudaSuccess) e = finish_single_group(c, o.get());
-    if (e != cudaSuccess) return fail_cuda(e, "boolean op");
-    *out = o.release();
-    return BDF_OK;
+    int64_t rows = 0;
+    return launch_groups(c, {a, b}, {n}, kBool, plan, bool_tile_elems(), bool_desc_size(), BDF_K_COMPARE, "boolean op",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            const DevChunk& x = a->chunks[i];
+            const DevChunk* y = b ? &b->chunks[i] : nullptr;
+            fill_bool_desc(hd, i, (const uint32_t*)x.values, y ? (const uint32_t*)y->values : nullptr, (uint32_t*)oc.values, x.validity,
+                           y ? y->validity : nullptr, oc.validity, x.len, tile0, x.val_bit_off, y ? y->val_bit_off : 0, x.bit_off, y ? y->bit_off : 0);
+            // the record counts (rows / 8) * (2 or 3) bytes for the whole launch: each chunk adds its step of rows / 8
+            const int64_t before = rows / 8;
+            rows += x.len;
+            return (rows / 8 - before) * (b ? 3 : 2);
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t* wc) {
+            return launch_boolean(op, dd, (int)(end - begin), tiles, wc, c->s_compute);
+        },
+        out);
 }
 
 // ChunkedArray::filter: arrow compute::filter(chunk, mask chunk) for every chunk pair (src/table.rs:97-107).
@@ -1731,20 +1634,6 @@ static int filter_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* mask, bd
 // ---------------------------------------------------------------------------------------------------
 // N3: a chain of Calculations fused into one pass (k_expr.cu)
 
-namespace bdf {
-int expr_tile_elems();
-int expr_max_inputs();
-int expr_max_nodes();
-size_t expr_desc_size();
-void fill_expr_desc(void* base, int64_t i, int n_inputs, const void* const* in, const uint32_t* const* vin, const int32_t* off, double* out,
-                    uint32_t* vout, int64_t len, int64_t tile0);
-size_t expr_prog_size();
-void expr_prog_stats(const void* prog, int* n_instructions, int* n_temporaries);
-int expr_compile(int n_inputs, const int* in_dtypes, int n_nodes, const int* op, const int* a, const int* b, void* prog);
-cudaError_t launch_expr(const void* descs, int n_chunks, int64_t tiles, const void* prog, uint32_t* warp_counts, int* flags, AggDev* tile_partials,
-                        cudaStream_t s);
-}  // namespace bdf
-
 // Validation + host compilation of a fused program (shared by the evaluation entry and bdf_expr_check; needs no device).
 static int expr_prepare(int n_inputs, const int* in_dtypes, int n_nodes, const bdf_expr_node* nodes, unsigned char (&prog)[256], bool* has_div) {
     if (n_inputs < 1 || n_inputs > expr_max_inputs()) return fail(BDF_INVALID, "an expression takes 1..%d input columns", expr_max_inputs());
@@ -1786,14 +1675,8 @@ static int expr_dev(bdf_ctx* c, int n_inputs, const bdf_col* const* inputs, int 
     TRY(expr_prepare(n_inputs, in_dtypes, n_nodes, nodes, prog, &has_div));
     for (int i = 0; i < n_inputs; i++)
         if (!inputs[i]) return fail(BDF_INVALID, "null input column");
-    int64_t n = (int64_t)inputs[0]->chunks.size();
-    for (int i = 0; i < n_inputs; i++) {
-        n = std::min<int64_t>(n, (int64_t)inputs[i]->chunks.size());
-    }
-    for (int64_t ch = 0; ch < n; ch++)
-        for (int i = 1; i < n_inputs; i++)
-            if (inputs[i]->chunks[ch].len != inputs[0]->chunks[ch].len)
-                return fail(BDF_LENGTH_MISMATCH, "Cannot perform math operation on arrays of different length");
+    int64_t n = 0;
+    TRY(zip_chunks(inputs, n_inputs, &n));
     std::vector<ChunkPlan> plan((size_t)n);
     for (int64_t ch = 0; ch < n; ch++) {
         bool hv = false;
@@ -1844,27 +1727,17 @@ static int expr_dev(bdf_ctx* c, int n_inputs, const bdf_col* const* inputs, int 
         }
         if (e == cudaSuccess && o.get()) e = finish_single_group(c, o.get());
         if (e == cudaSuccess && f.get()) {
-            // fold the per-tile partials on the finish stream, like K5
-            c->launches++;
             e = ev_get(c, &ev_done);
             if (e == cudaSuccess) e = cudaEventRecord(ev_done, c->s_compute);
             if (e == cudaSuccess) e = cudaStreamWaitEvent(c->s_fin, ev_done, 0);
-            if (e == cudaSuccess) e = launch_finish(true, pb->p, total_tiles, c->sm_count, c->d_stage, c->d_ticket + 1, future_target(c, f.get(), 0), c->s_fin);
-            if (e == cudaSuccess) e = cudaEventRecord(pb->done, c->s_fin);
-            pb->used = true;
-            f->chunks[0] = (uint32_t)n;
-            if (e == cudaSuccess) e = future_combine(c, f.get(), c->s_fin);
-            if (e == cudaSuccess) e = cudaEventRecord(f->ev, c->s_fin);
+            if (e == cudaSuccess) e = fused_finish(c, f.get(), pb, total_tiles, n);
             if (ev_done) ev_put(c, ev_done);
         }
-        if (e == cudaSuccess && has_div) {
-            if (is_global(c)) e = flag_allreduce(c);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
-            if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-            if (e == cudaSuccess && *c->h_flag) return fail(BDF_DIVIDE_BY_ZERO, "Divide by zero error");
-        }
     }
+    int flag = 0;
+    if (e == cudaSuccess && has_div) e = flag_read(c, is_global(c), &flag);
     if (e != cudaSuccess) return fail_cuda(e, "fused expression");
+    if (flag) return fail(BDF_DIVIDE_BY_ZERO, "Divide by zero error");
     if (out) *out = o.release();
     if (fut) *fut = f.release();
     return BDF_OK;
@@ -1872,22 +1745,6 @@ static int expr_dev(bdf_ctx* c, int n_inputs, const bdf_col* const* inputs, int 
 
 // ---------------------------------------------------------------------------------------------------
 // DataFrame::sort = lexsort_to_indices + take (k_sort.cu)
-
-namespace bdf {
-size_t sort_chunk_size();
-void fill_sort_chunk(void* base, int64_t i, const void* values, const uint32_t* validity, int64_t start, int32_t bit_off, int32_t val_bit_off);
-int sort_tile_elems();
-int take_tile_elems();
-int sort_pass_ctas(int64_t n, int sm_count);
-cudaError_t launch_iota(uint32_t* out, int64_t n, int sm_count, cudaStream_t s);
-int sort_key_bytes(int dtype);
-cudaError_t launch_sort_keys(int dtype, const void* chunks, int n_chunks, const uint32_t* idx, int64_t n, int mode, int descending,
-                             void* keys, unsigned long long* agree, int sm_count, cudaStream_t s);
-cudaError_t launch_radix_pass(int key_bytes, const void* keys_in, const uint32_t* idx_in, int64_t n, int shift, unsigned int* block_hist,
-                              void* keys_out, uint32_t* idx_out, int sm_count, cudaStream_t s);
-cudaError_t launch_take(int dtype, const void* vals, int n_vals, const void* idxs, int n_idxs, int64_t n, int64_t n_rows_values, void* out,
-                        uint32_t* vout, uint32_t* warp_counts, int* flags, cudaStream_t s);
-}  // namespace bdf
 
 // The chunk table of a column in the concatenated row space (descriptor ring, uploaded on the descriptor stream).
 static int sort_table(bdf_ctx* c, const bdf_col* col, void** dev, int* n_chunks, bool* nullable) {
@@ -1995,10 +1852,10 @@ static int take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, b
         e = launch_take(values->dtype, vt, nv, it, ni, n, values->total_len, o->chunks[0].values, o->chunks[0].validity, o->d_warp_counts, c->d_flag, c->s_compute);
     }
     if (e == cudaSuccess) e = finish_single_group(c, o.get());
-    if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-    if (e == cudaSuccess && *c->h_flag) return fail(BDF_INVALID, "take: index out of bounds");
+    int flag = 0;
+    if (e == cudaSuccess) e = flag_read(c, false, &flag);
     if (e != cudaSuccess) return fail_cuda(e, "take");
+    if (flag) return fail(BDF_INVALID, "take: index out of bounds");
     *out = o.release();
     return BDF_OK;
 }
@@ -2007,21 +1864,6 @@ static int take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, b
 // group-by (k_group.cu): sort the keys, gather them, mark group heads, compact keys and group starts, fold every requested
 // value column once per group; first / last are a take of each group's first / last original row; count_distinct sorts
 // (keys..., value) once more and counts the distinct-value heads inside every group.
-
-namespace bdf {
-cudaError_t launch_group_heads(int n_keys, const void* const* values, const uint32_t* const* valid, const int* widths, const int* is_float,
-                               int and_last_valid, long long n, uint32_t* words, cudaStream_t s);
-cudaError_t launch_group_reduce(int dtype, bool extra, const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows,
-                                void* sum, long long* count, void* mn, void* mx, double* avg, uint32_t* nonempty, void* scratch, int sm_count, cudaStream_t s);
-cudaError_t launch_group_bounds(const uint32_t* idx, const uint32_t* starts, long long n_groups, long long n_rows, uint32_t* first, uint32_t* last,
-                                cudaStream_t s);
-cudaError_t launch_group_distinct(const uint32_t* pos, long long n_pos, const uint32_t* starts, long long n_groups, long long n_rows, long long* out,
-                                  uint32_t* first, cudaStream_t s);
-cudaError_t launch_group_moments(int dtype, const void* val, const uint32_t* vvalid, const uint32_t* starts, long long n_groups, long long n_rows,
-                                 Moments* mom, void* scratch, int sm_count, cudaStream_t s);
-cudaError_t launch_group_stats(const Moments* mom, long long n_groups, int stat, double* out, uint32_t* valid, cudaStream_t s);
-size_t group_big_scratch_bytes(long long n_rows);
-}  // namespace bdf
 
 static bool group_is_stat(int fn) { return fn == BDF_GROUP_KURTOSIS || fn == BDF_GROUP_SKEWNESS || fn == BDF_GROUP_STDDEV || fn == BDF_GROUP_VARIANCE ||
                                            fn == BDF_GROUP_STDDEV_POP || fn == BDF_GROUP_VAR_POP; }
@@ -2397,11 +2239,6 @@ static int group_aggregate_dev(bdf_ctx* c, const bdf_col* key, int n_values, con
 // ---------------------------------------------------------------------------------------------------
 // statistical aggregates (k_moments.cu, moments.cuh): the moment record of a whole column, and its distinct values
 
-namespace bdf {
-cudaError_t launch_moments(int dtype, const RedDesc* d, int n, int64_t tiles, Moments* partials, Moments* result, cudaStream_t s);
-int64_t moments_partials(int64_t tiles);
-}  // namespace bdf
-
 static_assert(sizeof(Moments) == sizeof(bdf_moment_rec) && offsetof(bdf_moment_rec, m4) == offsetof(Moments, m4), "bdf_moment_rec layout");
 
 // One launch of k_moments over every chunk and its finish; on a rank of a communicator the records of all ranks are all-gathered
@@ -2478,20 +2315,6 @@ static int distinct_dev(bdf_ctx* c, const bdf_col* x, bdf_distinct_rec* out) {
 // key tuples by sorted_runs, as group-by's groups are; every probe row binary-searches the distinct tuples, the counts are scanned into
 // output offsets (one host wait for the total), and the emit writes the index pairs by output position.  FULL appends the build
 // rows of the runs no probe row hit, listed in row order by a compaction of an iota.
-
-namespace bdf {
-int join_tile_rows();
-cudaError_t launch_join_count(int n_keys, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,
-                              const uint32_t* const* build_valid, long long n_probe, const uint32_t* run_starts, long long n_runs, long long n_build,
-                              int outer, unsigned long long* counts, uint32_t* match_start, unsigned char* hit, unsigned long long* block_sums,
-                              cudaStream_t s);
-cudaError_t launch_join_scan(unsigned long long* counts, long long n_probe, unsigned long long* block_sums, cudaStream_t s);
-cudaError_t launch_join_emit(const unsigned long long* offs, long long n_probe, const uint32_t* match_start, const uint32_t* perm, unsigned long long probe_rows,
-                             const uint32_t* unmatched, unsigned long long n_out, uint32_t* probe_out, uint32_t* probe_valid, uint32_t* build_out,
-                             uint32_t* build_valid, cudaStream_t s);
-cudaError_t launch_join_unmatched(const uint32_t* perm, long long n_build, const uint32_t* run_starts, long long n_runs, const unsigned char* hit,
-                                  uint32_t* mask, int sm_count, cudaStream_t s);
-}  // namespace bdf
 
 static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, const bdf_col* const* rk, bdf_col** out_l, bdf_col** out_r,
                     int64_t* n_rows_out) {
@@ -2608,18 +2431,6 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
 // compacted run starts, so a position finds its partition and peer bounds in O(1).  Ranking functions are written straight to row
 // order through the permutation; lag / lead and the scans work in sorted order and come back through one take each, whose index
 // is the frame's last sorted position of every row.  Without any key nothing is sorted: the kernels read the caller's chunks in place.
-
-namespace bdf {
-int window_count_tile();
-cudaError_t launch_window_count(const uint32_t* words, long long n_words, unsigned long long* counts, unsigned long long* block_sums, cudaStream_t s);
-cudaError_t launch_window_rank(const void* const* p, long long n_p, const void* const* q, long long n_q, long long n, const uint32_t* perm,
-                               void* const* outs, cudaStream_t s);
-cudaError_t launch_window_shift(int dtype, const void* const* p, long long n_p, long long n, const void* x, int nx, long long k, int lead,
-                                unsigned long long def_bits, int has_def, void* out, uint32_t* vout, cudaStream_t s);
-size_t window_scan_scratch_bytes(long long n);
-cudaError_t launch_window_scan(int dtype, int fn, const void* x, int nx, const uint32_t* heads, long long n, void* scratch, void* out, uint32_t* vout,
-                               cudaStream_t s);
-}  // namespace bdf
 
 // One head bitmap and what k_window needs to find the run of a position in O(1).
 struct WinHeadsHost {
@@ -2858,24 +2669,6 @@ static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_
 // CSV reader (k_csv.cu; the rules are in include/b200df.h): the file is mapped and its bytes go to HBM through the pageable staging
 // path; the tokenizer scan builds the field index there, the field counts are checked and the schema inferred on the device.  The
 // bytes and the index stay until bdf_csv_close; a read parses only the requested columns.
-
-namespace bdf {
-int csv_tile_bytes();
-int csv_parse_rows();
-size_t csv_desc_bytes();
-size_t csv_slow_bytes();
-size_t csv_patch_bytes();
-cudaError_t launch_csv_tokenize(const uint8_t* text, long long n, uint8_t delim, uint32_t* agg, uint8_t* start, int* final_state, uint16_t* fe,
-                                uint16_t* re, unsigned long long* block_counts, cudaStream_t s);
-cudaError_t launch_csv_index(const uint16_t* fe, const uint16_t* re, long long n, const unsigned long long* block_offsets, unsigned long long* ends,
-                             unsigned long long* first_rec, cudaStream_t s);
-cudaError_t launch_csv_check(const unsigned long long* ends, long long n_fields, long long k, unsigned long long* bad, int sm_count, cudaStream_t s);
-cudaError_t launch_csv_infer(const uint8_t* text, const unsigned long long* ends, long long f0, long long f1, long long k, unsigned int* col_bits,
-                             int sm_count, cudaStream_t s);
-cudaError_t launch_csv_parse(const uint8_t* text, const unsigned long long* ends, const void* cols, int n_cols, long long f0, long long k, long long n_rows,
-                             long long batch, unsigned long long* err_key, void* slow, unsigned long long* n_slow, long long slow_cap, cudaStream_t s);
-cudaError_t launch_csv_scatter(const void* patches, long long n, cudaStream_t s);
-}  // namespace bdf
 
 struct bdf_csv {
     int fd = -1;
@@ -3247,14 +3040,6 @@ static int csv_read(bdf_ctx* c, const bdf_csv* f, int n_cols, const int32_t* col
 // fixed device buffers: while block k is measured, scanned and formatted, block k-1 crosses PCIe through the pinned staging slots
 // and the CopyPool threads pwrite every slot at its offset in the file (known from the scan), so neither HBM nor pinned memory
 // grows with the file.
-
-namespace bdf {
-int csvw_tile();
-cudaError_t launch_csvw_measure(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows,
-                                unsigned long long* lens, unsigned long long* block_sums, cudaStream_t s);
-cudaError_t launch_csvw_emit(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows, int delim,
-                             const unsigned long long* offs, char* out, cudaStream_t s);
-}  // namespace bdf
 
 static constexpr size_t kCsvwText = (size_t)64 << 20;        // bytes of each of the two device text buffers
 static constexpr int64_t kCsvwMaxRows = (int64_t)1 << 21;    // rows per block at most (their lengths and offsets: 16 MiB)
@@ -4018,24 +3803,6 @@ static void fleet_destroy(bdf_ctx* c) {
 // lexsort over (parent, value) turn them into the existing sort / take / heads / filter steps, and the result's offsets come from
 // the list numbers of the kept elements.  They return one chunk, as take and sort do.
 
-namespace bdf {
-size_t list_find_scratch_bytes(long long n_elem);
-cudaError_t launch_list_find(int dtype, const int32_t* off, const uint32_t* lvalid, long long len, long long n_elem, const void* values,
-                             const uint32_t* vvalid, int vbit_off, uint64_t value_bits, int mode, uint32_t* bits, int32_t* pos, void* scratch,
-                             int sm_count, cudaStream_t s);
-cudaError_t launch_list_parent(const int32_t* off, const uint32_t* lvalid, const uint32_t* and_valid, long long len, long long n_elem, long long list0,
-                               long long elem0, uint32_t* parent, uint32_t* inlist, cudaStream_t s);
-cudaError_t launch_list_remove_mask(int dtype, const void* values, const uint32_t* vvalid, int vbit_off, long long n_elem, long long elem0,
-                                    uint64_t value_bits, const uint32_t* inlist, uint32_t* keep, cudaStream_t s);
-cudaError_t launch_list_mark(const uint32_t* perm, const uint32_t* head, const uint32_t* pvalid, long long n, long long split, int mode, uint32_t* keep,
-                             cudaStream_t s);
-cudaError_t launch_list_offsets(const uint32_t* kp, long long n_kept, long long n_lists, long long mult, int32_t* out, cudaStream_t s);
-cudaError_t launch_list_repeat(const int32_t* base, long long n_lists, long long count, const uint32_t* rows, long long n_out, uint32_t* src, cudaStream_t s);
-cudaError_t launch_list_size(const int32_t* off, const uint32_t* lvalid, long long len, int32_t* out, cudaStream_t s);
-cudaError_t launch_list_minmax_valid(const int32_t* off, const uint32_t* lvalid, const uint32_t* nonempty, long long len, uint32_t* valid, int* empty,
-                                     cudaStream_t s);
-}  // namespace bdf
-
 struct bdf_list {
     int dtype = 0;
     bdf_col* values = nullptr;               // chunk i = the elements of list chunk i
@@ -4362,9 +4129,9 @@ static int list_reduce(bdf_ctx* c, int fn, const bdf_list* l, bdf_col** out) {
                 o->null_counts[i] = -1;
             }
         }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(c->h_flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->s_compute);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
-        if (e == cudaSuccess && *c->h_flag) return fail(BDF_WOULD_PANIC, "array_max / array_min of an empty list: the reference's .max().unwrap() panics");
+        int flag = 0;
+        if (e == cudaSuccess) e = flag_read(c, false, &flag);
+        if (e == cudaSuccess && flag) return fail(BDF_WOULD_PANIC, "array_max / array_min of an empty list: the reference's .max().unwrap() panics");
     }
     if (e == cudaSuccess) e = finish_single_group(c, o.get());
     if (e != cudaSuccess) return fail_cuda(e, "list reduce");
@@ -5561,41 +5328,18 @@ int bdf_generate(bdf_ctx* c, int dtype, int kind, double lo, double hi, uint64_t
         if (chunk_lens[i] < 0) return fail(BDF_INVALID, "negative chunk length");
         plan[i] = {chunk_lens[i], null_mod != 0};
     }
-    bdf_col* o = nullptr;
-    const int tile = elems_per_tile(dtype);
-    TRY(col_alloc(c, dtype, plan, nullptr, tile, &o));
-    o->counts_on_device = o->d_warp_counts != nullptr;
-    void *hp = nullptr, *dp = nullptr;
-    int st = ring_alloc(c, (size_t)n_chunks * sizeof(GenDesc), &hp, &dp);
-    cudaError_t e = cudaSuccess;
-    GenDesc* dd = (GenDesc*)dp;
-    if (st == BDF_OK) {
-        GenDesc* hd = (GenDesc*)hp;
-        int64_t tiles = 0, rows = 0;
-        for (int64_t i = 0; i < n_chunks; i++) {
-            hd[i] = GenDesc{o->chunks[i].values, o->chunks[i].validity, chunk_lens[i], tiles, row0 + rows};
-            tiles += (chunk_lens[i] + tile - 1) / tile;
-            rows += chunk_lens[i];
-        }
-        e = desc_upload(c, dd, hd, (size_t)n_chunks * sizeof(GenDesc));
-        if (e == cudaSuccess) {
-            LaunchTimer t(c, BDF_K_GENERATE, dtype, rows, rows * dtype_width(dtype));
-            e = launch_generate(dtype, kind, lo, hi, seed, col_id, null_mod, dd, (int)n_chunks, tiles, o->d_warp_counts, c->s_compute);
-        }
-        if (e == cudaSuccess) {
-            Group g{0, n_chunks, nullptr};
-            e = ev_get(c, &g.ev);
-            if (e == cudaSuccess) e = cudaEventRecord(g.ev, c->s_compute);
-            o->groups.push_back(g);
-        }
-    }
-    if (st != BDF_OK || e != cudaSuccess) {
-        cudaGetLastError();
-        col_release(c, o);
-        return st != BDF_OK ? st : fail(cuda_status(e), "generate failed: %s", cudaGetErrorString(e));
-    }
-    *out = o;
-    return BDF_OK;
+    const int w = dtype_width(dtype);
+    int64_t rows = 0;
+    return launch_groups(c, {}, {n_chunks}, dtype, plan, elems_per_tile(dtype), sizeof(GenDesc), BDF_K_GENERATE, "generate",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            ((GenDesc*)hd)[i] = GenDesc{oc.values, oc.validity, oc.len, tile0, row0 + rows};
+            rows += oc.len;
+            return oc.len * w;
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t* wc) {
+            return launch_generate(dtype, kind, lo, hi, seed, col_id, null_mod, (const GenDesc*)dd, (int)(end - begin), tiles, wc, c->s_compute);
+        },
+        out);
 }
 
 
