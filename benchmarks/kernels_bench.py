@@ -11,6 +11,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --csv-write [--csv-rows 50000000]                # the CSV writer rows (the reader's table written back)
     python benchmarks/kernels_bench.py --lists [--rows 100000000]                       # the list-function rows (ArrayFunctions)
     python benchmarks/kernels_bench.py --temporal [--rows 100000000]                    # the date / timestamp function rows
+    python benchmarks/kernels_bench.py --ndjson [--csv-rows 50000000]                   # the line-delimited JSON reader rows (a 4.85 GB temporary file)
 """
 from __future__ import annotations
 
@@ -133,6 +134,101 @@ def csv_bench(ctx, rows, rows_out, reps=3):
         ms = min(ts)
         name = f"Arrow C++ (not the reference) read_csv, {os.cpu_count()} cores"
         rows_out.append({"case": name, "config": "csv", "kernel": "host", "ms": ms, "rows": rows, "file_bytes": nbytes, "GBs_of_file": nbytes / ms / 1e6})
+        print(f"{name:44s} {ms:9.2f} ms  {nbytes / ms / 1e6:7.2f} GB/s of file bytes", flush=True)
+
+
+def write_ndjson(path, rows, seed=13, block=2_000_000):
+    """rows x {"id": Int64, "a", "b": Float64 with 7 significant digits, "ok": Boolean, "tags": 0..4 two-digit Int32, "s": a string}:
+    97 bytes per line, fixed width (the unused places of a value are JSON whitespace)."""
+    rng = np.random.default_rng(seed)
+    parts = [b'{"id":', 10, b',"a":', 13, b',"b":', 13, b',"ok":', 5, b',"tags":', 14, b',"s":"abc"}\n']
+    width = sum(len(x) if isinstance(x, bytes) else x for x in parts)
+    with open(path, "wb") as f:
+        for r0 in range(0, rows, block):
+            n = min(block, rows - r0)
+            m = np.empty((n, width), np.uint8)
+            at, fields = 0, []
+            for x in parts:
+                if isinstance(x, bytes):
+                    m[:, at:at + len(x)] = np.frombuffer(x, np.uint8)
+                    at += len(x)
+                else:
+                    fields.append((at, x))
+                    at += x
+            (pi, _), (pa_, _), (pb, _), (po, _), (pt, _) = fields
+            m[:, pi:pi + 10] = _digits(1_000_000_000 + np.arange(r0, r0 + n, dtype=np.int64) * 7 % 9_000_000_000, 10)
+            for p in (pa_, pb):   # [-]d.dddddde[+-]dd
+                mant, ex = rng.integers(1_000_000, 10_000_000, n), rng.integers(-30, 31, n)
+                m[:, p] = np.where(rng.random(n) < 0.5, 45, 32)
+                d = _digits(mant, 7)
+                m[:, p + 1], m[:, p + 2], m[:, p + 3:p + 9] = d[:, 0], 46, d[:, 1:]
+                m[:, p + 9], m[:, p + 10] = 101, np.where(ex < 0, 45, 43)
+                m[:, p + 11:p + 13] = _digits(np.abs(ex), 2)
+            ok = rng.random(n) < 0.5
+            m[:, po:po + 5] = np.where(ok[:, None], np.frombuffer(b"true ", np.uint8), np.frombuffer(b"false", np.uint8))
+            k = rng.integers(0, 5, n)
+            m[:, pt:pt + 14] = 32
+            m[:, pt], m[:, pt + 13] = 91, 93
+            for i in range(4):
+                has = k > i
+                d = _digits(rng.integers(10, 100, n), 2)
+                c = pt + 1 + 3 * i
+                m[:, c] = np.where(has & (i > 0), 44, 32)
+                m[:, c + 1] = np.where(has, d[:, 0], 32)
+                m[:, c + 2] = np.where(has, d[:, 1], 32)
+            f.write(m.tobytes())
+
+
+def ndjson_bench(ctx, rows, rows_out, reps=3):
+    """Line-delimited JSON -> device columns: the upload, the record index, key resolution + inference and the conversions (launch
+    records), end to end; pyarrow's read_json on the host for comparison."""
+    with tempfile.TemporaryDirectory() as td:
+        path = os.path.join(td, "bench.json")
+        write_ndjson(path, rows)
+        nbytes = os.path.getsize(path)
+        e2e, up, tok, keys, parse = [], [], [], [], []
+        for _ in range(reps + 1):
+            ctx.synchronize()
+            ctx.profile_read()
+            ctx.profile_enable(True)
+            t0 = time.perf_counter()
+            with rdf.JsonFile(path, ctx=ctx) as f:
+                cols = f.read(["id", "a", "b", "ok"])
+                tags = f.read_list("tags")
+                ctx.synchronize()
+                t1 = time.perf_counter()
+                st = f.stats()
+                schema = f.schema
+            ctx.profile_enable(False)
+            recs = [r for r in ctx.profile_read() if r["kernel"] == "json"]
+            for c in cols.values():
+                c.free()
+            tags.free()
+            e2e.append((t1 - t0) * 1e3)
+            up.append(st["upload_ms"])
+            tok.append(sum(r["ms"] for r in recs[:5]))     # newline count + index, record check, the two scans, the member list
+            keys.append(sum(r["ms"] for r in recs[5:8]))   # key table, resolution, inference
+            parse.append(sum(r["ms"] for r in recs[8:]))   # four scalar columns, the List<Int64> column
+        assert [n for n, _, _ in schema] == ["id", "a", "b", "ok", "tags", "s"], schema
+        med = lambda v: float(np.median(v[1:]))   # the first run warms up
+        for name, ms in (("json upload (page cache -> HBM)", med(up)), ("json tokenize + index", med(tok)),
+                         ("json key resolution + inference", med(keys)), ("json parse 4 columns + 1 list", med(parse)),
+                         ("json file -> device columns, end to end", med(e2e))):
+            gbs = nbytes / ms / 1e6
+            rows_out.append({"case": name, "config": "ndjson", "kernel": "json", "ms": ms, "rows": rows, "file_bytes": nbytes, "GBs_of_file": gbs})
+            print(f"{name:44s} {ms:9.2f} ms  {gbs:7.2f} GB/s of file bytes ({nbytes / 1e9:.2f} GB, {rows:.1e} records)", flush=True)
+        try:
+            import pyarrow.json as pajson
+        except ImportError:
+            return
+        ts = []
+        for _ in range(2):
+            t0 = time.perf_counter()
+            pajson.read_json(path)
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ms = min(ts)
+        name = f"pyarrow read_json (not the reference), {os.cpu_count()} cores"
+        rows_out.append({"case": name, "config": "ndjson", "kernel": "host", "ms": ms, "rows": rows, "file_bytes": nbytes, "GBs_of_file": nbytes / ms / 1e6})
         print(f"{name:44s} {ms:9.2f} ms  {nbytes / ms / 1e6:7.2f} GB/s of file bytes", flush=True)
 
 
@@ -486,8 +582,20 @@ def main():
     ap.add_argument("--csv-write", action="store_true", help="run only the CSV writer rows")
     ap.add_argument("--lists", action="store_true", help="run only the list-function rows (ArrayFunctions)")
     ap.add_argument("--temporal", action="store_true", help="run only the date / timestamp function rows")
+    ap.add_argument("--ndjson", action="store_true", help="run the line-delimited JSON reader rows (--csv-rows records)")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.ndjson:
+        import subprocess
+
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+        print(f"card: {q.strip()}", flush=True)
+        rows_out = []
+        ndjson_bench(ctx, args.csv_rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"card": q.strip(), "results": rows_out}, f, indent=1)
+        return
     if args.temporal:
         rows_out = []
         temporal_bench(ctx, args.rows, rows_out)

@@ -654,6 +654,69 @@ int  bdf_list_explode_dev(bdf_ctx* ctx, const bdf_list* list, bdf_col** rows, bd
 int  bdf_ipc_list_column(const bdf_ipc* file, int32_t col, int32_t* dtype);
 int  bdf_ipc_read_list(bdf_ctx* ctx, const bdf_ipc* file, int32_t col, int flags, bdf_list** out);
 
+/* ---- line-delimited JSON files straight to the device (DataFrame::from_json, src/dataframe.rs; LazyFrame::read(Json),
+ * src/evaluation.rs:329) ----------------------------------------------------------------------------------------------------------
+ * The reference reads with arrow-rs's json::Reader (infer_json_schema over max_records, then batches of batch_size, default 1024)
+ * over serde_json.  Neither is restated from source: every rule marked RECALLED below is recalled, parity unpinned (the reference
+ * has no JSON test); the others are this library's decisions, listed under Departures.
+ * Records.  A record is one line: '\n' ends it, and a '\r' before the '\n' is whitespace (JSON's whitespace is ' ', '\t', '\r',
+ *   '\n').  Lines made only of whitespace are skipped.  A leading UTF-8 BOM is skipped.  End of file ends the last record.  Every
+ *   record is one JSON object (RFC 8259; RECALLED: serde_json's grammar); anything else is BDF_INVALID "JSON error at line L, byte
+ *   B: what": a record that is not an object, malformed JSON, a number outside JSON's grammar (NaN, Infinity, +1, 01, 1., .5), an
+ *   unterminated string, an invalid escape, a raw control byte in a string, unbalanced brackets, trailing bytes after the object,
+ *   or nesting deeper than 128 levels (RECALLED: serde_json's recursion limit).  L counts lines from 1; B is the byte offset of the
+ *   error in the file (the BOM counted).  A raw '\n' cannot occur in a valid string, so records are split without string state.
+ * Keys.  Compared after their escapes are decoded ("\u0061" is the key a; a lone surrogate escape decodes to U+FFFD).  Columns come
+ *   in the order each key is first seen in the file.  A key repeated in one record: the last value wins (RECALLED: serde_json's
+ *   Map).  At most 65536 distinct raw keys per file, else BDF_UNSUPPORTED; two different keys with the same 64-bit hash are detected
+ *   (every key is compared byte for byte) and give BDF_UNSUPPORTED.
+ * Inference (no schema) over the first max_records records (all of them when max_records < 0); the columns are the keys seen
+ *   there.  Each value is put in one class: null adds no type and makes the column nullable; true / false Boolean; an integer
+ *   literal (no fraction, no exponent) in i64 range Int64; any other number Float64; a string Utf8; an object a struct; an array a
+ *   List of its non-null elements' coerced class.  Per key (RECALLED: arrow's coercion): one type -> it; {Int64, Float64} ->
+ *   Float64; List<Int64> with List<Float64> -> List<Float64>; a numeric scalar with a numeric list -> a List of the coerced element
+ *   type (arrow's "scalar and list -> list"); anything involving Utf8, a struct, Boolean mixed with another type, nested lists, a
+ *   list with a non-numeric element, or only lists that never had a typed element (or only nulls) -> off the device path:
+ *   bdf_json_column reports dtype -1, as bdf_csv_column does for Utf8.  A key missing from an inferred record makes its column
+ *   nullable.
+ * Explicit schema.  (name, dtype) pairs: dtype 0..9, BDF_BOOL, BDF_LIST_BASE + T for a numeric T, or BDF_UTF8 / -1 to skip the
+ *   column (reported with dtype -1); any other -> BDF_UNSUPPORTED, a repeated name -> BDF_INVALID.  Keys not in the schema are
+ *   ignored; every schema column is nullable.
+ * Values.  An absent key or null gives NULL.  Integer columns take integer literals in range for the column type (unsigned types
+ *   refuse a '-' sign, even -0).  Float columns take any JSON number, CORRECTLY ROUNDED to the column type (Float32 straight from the
+ *   decimal, never through Float64: the CSV reader's Eisel-Lemire path and its exact host fallback).  Boolean columns take true /
+ *   false.  A List<T> column takes an array: each element converted like a scalar of T, a null (or non-converting) element a null
+ *   element; a bare number is a one-element list; [] a valid empty list.  Anything that does not convert is NULL: a float or an
+ *   out-of-range integer into an integer column, a string, a Boolean into a number column, a number into a Boolean column, an
+ *   object, an array into a scalar column.  (RECALLED: arrow's reader leaves a non-conforming value null.  pyarrow's reader
+ *   instead ERRORS on such a value once the column's type is fixed: departure 4.)
+ * Output.  One chunk of batch_size rows per RecordBatch (the last one shorter), null counts set, no validity bitmap in a chunk
+ *   without nulls.  bdf_json_read reads numeric and Boolean columns (a projection); bdf_json_read_list reads one List<T> column as a
+ *   bdf_list, one chunk per RecordBatch with offsets from 0 in every chunk (no list bitmap in a chunk without null lists, no element
+ *   bitmap in a chunk without null elements).
+ * Departures from the reference, on purpose: (1) from_json stops at the first Err batch and keeps what it has; here the open (or
+ *   the read) fails.  (2) an empty file, or one of blank lines only, makes the reference panic at batches[0]: BDF_WOULD_PANIC.
+ *   (3) field order is first-seen; the recalled arrow reader of that era kept the inferred fields in a HashMap, so its order was
+ *   unstable.  (4) a value that does not convert is NULL here, where pyarrow errors.  (5) bytes are not checked for valid UTF-8
+ *   (serde_json reads from a str, so invalid UTF-8 is an error there).  (6) a '\r' alone does not end a record.
+ * Memory.  bdf_json_open keeps the file's bytes, 32 B per object member and 4 B per (record, column) in HBM until bdf_json_close and
+ *   needs 16 B per line and 8 B per '\n' more while it indexes; the file itself must fit as for CSV, else BDF_OOM before anything
+ *   is uploaded; anything else that does not fit gives BDF_OOM.  A read needs its outputs and, for float columns, a list of at most
+ *   max(65536, floats / 64) entries of 40 B for the values the device cannot round (rounded on the host with strtod / strtof in the
+ *   C locale; bdf_json_stats counts them; more -> BDF_UNSUPPORTED).  A failed call leaks nothing.  A multi-GPU context ->
+ *   BDF_UNSUPPORTED. */
+typedef struct { int64_t max_records /* <0: all */; int64_t batch_size; } bdf_json_options;
+typedef struct bdf_json bdf_json;
+int  bdf_json_open(bdf_ctx* ctx, const char* path, const bdf_json_options* options, int32_t n_schema, const char* const* schema_names,
+                   const int32_t* schema_dtypes /* both NULL: infer */, bdf_json** out);
+int  bdf_json_describe(const bdf_json* file, int32_t* n_columns, int64_t* n_batches, int64_t* n_rows);
+int  bdf_json_column(const bdf_json* file, int32_t col, const char** name, int32_t* dtype /* -1 off the path */, int32_t* nullable);
+int  bdf_json_read(bdf_ctx* ctx, const bdf_json* file, int32_t n_cols, const int32_t* cols, bdf_col** out /* n_cols */);   /* projection */
+int  bdf_json_read_list(bdf_ctx* ctx, const bdf_json* file, int32_t col, bdf_list** out);
+/* object members in the file; float values the last read rounded on the host; host time of the file's upload in bdf_json_open */
+int  bdf_json_stats(const bdf_json* file, int64_t* n_members, int64_t* exact_fields, double* upload_ms);
+void bdf_json_close(bdf_ctx* ctx, bdf_json* file);   /* the context that opened it */
+
 /* ---- dates and timestamps (ScalarFunctions::hour, src/functions/scalar.rs:267-273 -> arrow compute::hour; the Spark date functions
  * that are empty stubs in the same file: add_months, date_add, date_sub, date_trunc, date_diff, day_of_month, day_of_week, day_of_year,
  * last_day, minute, month, months_between, next_day, quarter, second, to_date, unix_timestamp, year ...) ----------------------------------
@@ -756,7 +819,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL, BDF_K_JSON } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

@@ -21,9 +21,9 @@ SUM, MIN, MAX, COUNT = range(4)
 OK, LENGTH_MISMATCH, DIVIDE_BY_ZERO, UNSUPPORTED, CUDA, NCCL, OOM, WOULD_PANIC, INVALID, PARSE = range(10)
 ASYNC = 1
 (K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW,
- K_MOMENTS, K_CSV_WRITE, K_LIST, K_TEMPORAL) = range(19)
+ K_MOMENTS, K_CSV_WRITE, K_LIST, K_TEMPORAL, K_JSON) = range(20)
 KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
-                "window", "moments", "csv_write", "list", "temporal"]
+                "window", "moments", "csv_write", "list", "temporal", "json"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -127,6 +127,10 @@ class ListView(C.Structure):
 class ListOut(C.Structure):
     _fields_ = [("offsets", C.c_void_p), ("validity", C.c_void_p), ("values", C.c_void_p), ("value_validity", C.c_void_p),
                 ("null_count", C.c_int64), ("value_null_count", C.c_int64), ("has_validity", C.c_int32), ("has_value_validity", C.c_int32)]
+
+
+class JsonOptions(C.Structure):
+    _fields_ = [("max_records", C.c_int64), ("batch_size", C.c_int64)]
 
 
 class CsvOptions(C.Structure):
@@ -273,6 +277,13 @@ def lib() -> C.CDLL:
         "bdf_csv_stats": ([vp, P(i64), P(i64), P(C.c_double)], C.c_int),
         "bdf_csv_close": ([vp, vp], None),
         "bdf_csv_write": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(CsvWriteOptions)], C.c_int),
+        "bdf_json_open": ([vp, C.c_char_p, P(JsonOptions), i32, P(C.c_char_p), P(i32), P(vp)], C.c_int),
+        "bdf_json_describe": ([vp, P(i32), P(i64), P(i64)], C.c_int),
+        "bdf_json_column": ([vp, i32, P(C.c_char_p), P(i32), P(i32)], C.c_int),
+        "bdf_json_read": ([vp, vp, i32, P(i32), P(vp)], C.c_int),
+        "bdf_json_read_list": ([vp, vp, i32, P(vp)], C.c_int),
+        "bdf_json_stats": ([vp, P(i64), P(i64), P(C.c_double)], C.c_int),
+        "bdf_json_close": ([vp, vp], None),
         "bdf_generate": ([vp, C.c_int, C.c_int, C.c_double, C.c_double, u64, u64, i64, P(i64), i64, C.c_uint32, P(vp)],
                          C.c_int),
         "bdf_list_upload": ([vp, C.c_int, i64, P(ListView), C.c_int, P(vp)], C.c_int),
@@ -319,6 +330,7 @@ EXPORTED_SYMBOLS = [
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",
     "bdf_ipc_write_host", "bdf_ipc_write",
     "bdf_csv_open", "bdf_csv_describe", "bdf_csv_column", "bdf_csv_read", "bdf_csv_stats", "bdf_csv_close", "bdf_csv_write",
+    "bdf_json_open", "bdf_json_describe", "bdf_json_column", "bdf_json_read", "bdf_json_read_list", "bdf_json_stats", "bdf_json_close",
     "bdf_moments", "bdf_moments_dev", "bdf_moments_stat", "bdf_moments_merge", "bdf_distinct", "bdf_distinct_dev",
     "bdf_list_upload", "bdf_list_describe", "bdf_list_chunk_info", "bdf_list_download", "bdf_list_values", "bdf_list_free",
     "bdf_list_find_dev", "bdf_list_reduce_dev", "bdf_list_transform_dev", "bdf_list_set_dev", "bdf_list_explode_dev",

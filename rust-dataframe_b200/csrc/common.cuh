@@ -442,6 +442,36 @@ cudaError_t launch_csv_parse(const uint8_t* text, const unsigned long long* ends
                              long long batch, unsigned long long* err_key, void* slow, unsigned long long* n_slow, long long slow_cap, cudaStream_t s);
 cudaError_t launch_csv_scatter(const void* patches, long long n, cudaStream_t s);
 
+// line-delimited JSON reader (k_json.cu).
+int json_tile_bytes();
+int json_parse_rows();
+size_t json_member_bytes();
+size_t json_key_bytes();
+size_t json_desc_bytes();
+size_t json_slow_bytes();
+size_t json_list_chunk_bytes();
+long long json_scan_sums(long long n);
+cudaError_t launch_json_nl_count(const uint8_t* text, long long n, unsigned long long* counts, cudaStream_t s);
+cudaError_t launch_json_nl_index(const uint8_t* text, long long n, const unsigned long long* offsets, unsigned long long* nl, cudaStream_t s);
+cudaError_t launch_json_scan(unsigned long long* data, long long n, unsigned long long* sums, cudaStream_t s);
+cudaError_t launch_json_lex(const uint8_t* text, long long n, const unsigned long long* nl, long long n_nl, unsigned long long* members,
+                            unsigned long long* is_rec, unsigned long long* bad, int sm_count, cudaStream_t s);
+cudaError_t launch_json_members(const uint8_t* text, long long n, const unsigned long long* nl, long long n_nl, const unsigned long long* first_member,
+                                const unsigned long long* rec_of, void* members, int sm_count, cudaStream_t s);
+cudaError_t launch_json_keys(const uint8_t* text, const void* members, long long n_members, void* table, unsigned cap, unsigned int* full, int sm_count,
+                             cudaStream_t s);
+cudaError_t launch_json_resolve(const uint8_t* text, const void* members, long long n_members, const void* table, unsigned cap, const int* col_of, int n_cols,
+                                unsigned int* slots, unsigned int* collision, int sm_count, cudaStream_t s);
+cudaError_t launch_json_infer(const void* members, const unsigned int* slots, long long n_slots, int n_cols, unsigned int* col_bits, int sm_count, cudaStream_t s);
+cudaError_t launch_json_parse(const uint8_t* text, const void* members, const unsigned int* slots, int n_file_cols, const void* cols, int n_cols, long long n_rows,
+                              long long batch, void* slow, unsigned long long* n_slow, long long slow_cap, cudaStream_t s);
+cudaError_t launch_json_list_count(const uint8_t* text, const void* members, const unsigned int* slots, int n_file_cols, int file_col, long long n_rows,
+                                   long long batch, unsigned long long* counts, uint32_t* valid_words, unsigned long long* chunk_nulls, cudaStream_t s);
+cudaError_t launch_json_bounds(const unsigned long long* offs, long long n_rows, long long batch, long long n_chunks, unsigned long long* bounds, cudaStream_t s);
+cudaError_t launch_json_list_fill(const uint8_t* text, const void* members, const unsigned int* slots, int n_file_cols, int file_col, int dtype, long long n_rows,
+                                  long long batch, const unsigned long long* offs, const uint32_t* valid_words, const void* out, unsigned long long* elem_nulls,
+                                  void* slow, unsigned long long* n_slow, long long slow_cap, cudaStream_t s);
+
 // CSV writer (k_csv_write.cu).
 int csvw_tile();
 cudaError_t launch_csvw_measure(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows,

@@ -35,6 +35,7 @@
 #include "common.cuh"
 #include "comm.cuh"
 #include "moments.cuh"
+#include "json_parse.cuh"
 
 using namespace bdf;
 
@@ -2670,13 +2671,56 @@ static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_
 // path; the tokenizer scan builds the field index there, the field counts are checked and the schema inferred on the device.  The
 // bytes and the index stay until bdf_csv_close; a read parses only the requested columns.
 
-struct bdf_csv {
+// A text file as the readers hold it: mapped, and its bytes after a leading UTF-8 BOM in HBM (zero-padded to whole tiles).
+struct MappedText {
     int fd = -1;
     const uint8_t* map = nullptr;   // the whole file
     size_t size = 0;
     size_t off = 0;                 // 3 when the file starts with a UTF-8 BOM
     int64_t n = 0;                  // bytes after the BOM (what the device holds)
     uint8_t* d_text = nullptr;
+    double upload_ms = 0;           // host time of the upload
+};
+
+static void text_free(bdf_ctx* c, MappedText* t) {
+    if (t->d_text) cudaFreeAsync(t->d_text, c->s_compute);
+    if (t->map) munmap((void*)t->map, t->size);
+    if (t->fd >= 0) close(t->fd);
+}
+
+// Map `path`, step over a BOM, and upload the rest through the pageable staging path: page cache -> pinned staging -> HBM.  The
+// device buffer is padded with zeros to whole tiles of `tile` bytes.  `what` names the reader in the messages.
+static int text_open(bdf_ctx* c, const char* path, int64_t tile, const char* what, MappedText* f) {
+    f->fd = open(path, O_RDONLY | O_CLOEXEC);
+    struct stat sb;
+    if (f->fd < 0 || fstat(f->fd, &sb) != 0) return fail(BDF_INVALID, "cannot open %s: %s", path, strerror(errno));
+    f->size = (size_t)sb.st_size;
+    if (f->size) {
+        void* m = mmap(nullptr, f->size, PROT_READ, MAP_PRIVATE, f->fd, 0);
+        if (m == MAP_FAILED) return fail(BDF_INVALID, "cannot map %s: %s", path, strerror(errno));
+        f->map = (const uint8_t*)m;
+    }
+    if (f->size >= 3 && f->map[0] == 0xEF && f->map[1] == 0xBB && f->map[2] == 0xBF) f->off = 3;
+    f->n = (int64_t)(f->size - f->off);
+    const int64_t tiles = std::max<int64_t>((f->n + tile - 1) / tile, 1);
+    if ((long double)tiles * tile * 1.3L > (long double)c->hbm_bytes) return fail(BDF_OOM, "a %s file of %lld bytes does not fit in device memory", what, (long long)f->n);
+    cudaError_t e = cudaMallocAsync((void**)&f->d_text, (size_t)(tiles * tile), c->s_compute);
+    if (e == cudaSuccess) e = cudaMemsetAsync(f->d_text + f->n, 0, (size_t)(tiles * tile - f->n), c->s_compute);
+    if (e == cudaSuccess) e = cudaEventRecord(c->ev_tmp, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->s_h2d, c->ev_tmp, 0);
+    const auto t0 = std::chrono::steady_clock::now();
+    if (e == cudaSuccess && f->n) e = h2d_copy(c, f->d_text, f->map + f->off, (size_t)f->n);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_h2d);
+    f->upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (e != cudaSuccess) {
+        const int st = fail_cuda(e, (std::string(what) + " upload").c_str());
+        cudaStreamSynchronize(c->s_h2d);   // no copy may still read the mapping when it is unmapped
+        return st;
+    }
+    return BDF_OK;
+}
+
+struct bdf_csv : MappedText {
     unsigned long long* d_ends = nullptr;   // per field: end byte | bit 63 when it ends its record
     int64_t n_fields = 0, k = 0, n_rows = 0, f0 = 0, batch = 1024;
     int has_header = 1;
@@ -2684,17 +2728,14 @@ struct bdf_csv {
     std::vector<std::string> names;
     std::vector<int32_t> dtypes, nullable;
     mutable int64_t exact_fields = 0;
-    double upload_ms = 0;
 };
 
 static constexpr unsigned long long kCsvRec = 1ull << 63;
 
 static void csv_free(bdf_ctx* c, bdf_csv* f) {
     if (!f) return;
-    if (f->d_text) cudaFreeAsync(f->d_text, c->s_compute);
     if (f->d_ends) cudaFreeAsync(f->d_ends, c->s_compute);
-    if (f->map) munmap((void*)f->map, f->size);
-    if (f->fd >= 0) close(f->fd);
+    text_free(c, f);
     delete f;
 }
 static void drop(bdf_ctx* c, bdf_csv* f) { csv_free(c, f); }
@@ -2776,20 +2817,9 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
     f->has_header = o->has_header ? 1 : 0;
     f->delim = o->delimiter;
     f->batch = o->batch_size;
-    f->fd = open(path, O_RDONLY | O_CLOEXEC);
-    struct stat sb;
-    if (f->fd < 0 || fstat(f->fd, &sb) != 0) return fail(BDF_INVALID, "cannot open %s: %s", path, strerror(errno));
-    f->size = (size_t)sb.st_size;
-    if (f->size) {
-        void* m = mmap(nullptr, f->size, PROT_READ, MAP_PRIVATE, f->fd, 0);
-        if (m == MAP_FAILED) return fail(BDF_INVALID, "cannot map %s: %s", path, strerror(errno));
-        f->map = (const uint8_t*)m;
-    }
-    if (f->size >= 3 && f->map[0] == 0xEF && f->map[1] == 0xBB && f->map[2] == 0xBF) f->off = 3;
-    f->n = (int64_t)(f->size - f->off);
     const int64_t tile = csv_tile_bytes();
+    TRY(text_open(c, path, tile, "CSV", f.get()));
     const int64_t tiles = std::max<int64_t>((f->n + tile - 1) / tile, 1);
-    if ((long double)tiles * tile * 1.3L > (long double)c->hbm_bytes) return fail(BDF_OOM, "a CSV file of %lld bytes does not fit in device memory", (long long)f->n);
 
     Scratch<uint32_t> agg;
     Scratch<uint8_t> start;
@@ -2797,23 +2827,8 @@ static int csv_open(bdf_ctx* c, const char* path, const bdf_csv_options* o, int 
     Scratch<unsigned long long> counts, small;   // small: [0] final state, [1] first record end, [2] first bad field
     Scratch<unsigned int> bits;
 
-    // the bytes: page cache -> pinned staging -> HBM
-    cudaError_t e = cudaMallocAsync((void**)&f->d_text, (size_t)(tiles * tile), c->s_compute);
-    if (e == cudaSuccess) e = cudaMemsetAsync(f->d_text + f->n, 0, (size_t)(tiles * tile - f->n), c->s_compute);
-    if (e == cudaSuccess) e = cudaEventRecord(c->ev_tmp, c->s_compute);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->s_h2d, c->ev_tmp, 0);
-    const auto t0 = std::chrono::steady_clock::now();
-    if (e == cudaSuccess && f->n) e = h2d_copy(c, f->d_text, f->map + f->off, (size_t)f->n);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_h2d);
-    f->upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    if (e != cudaSuccess) {
-        const int st = fail_cuda(e, "CSV upload");
-        cudaStreamSynchronize(c->s_h2d);   // no copy may still read the mapping when it is unmapped
-        return st;
-    }
-
     // tokenize: the state at every CTA, the field / record end masks, the field count
-    e = agg.alloc(c, (size_t)tiles * 4);
+    cudaError_t e = agg.alloc(c, (size_t)tiles * 4);
     if (e == cudaSuccess) e = start.alloc(c, (size_t)tiles);
     if (e == cudaSuccess) e = fe.alloc(c, (size_t)tiles * kThreads * 2);
     if (e == cudaSuccess) e = re.alloc(c, (size_t)tiles * kThreads * 2);
@@ -4279,6 +4294,500 @@ static int list_explode(bdf_ctx* c, const bdf_list* l, bdf_col** rows_out, bdf_c
 }
 
 // ---------------------------------------------------------------------------------------------------
+// line-delimited JSON reader (k_json.cu; the rules are in include/b200df.h): the file goes to HBM as for the CSV reader; the lines
+// are found, checked and walked on the device, which lists every member of every record's object.  The host decodes the distinct
+// keys into the dictionary and applies the inference's coercion table; the members and the (record, column) slots stay on the
+// device until bdf_json_close, and a read converts only the requested columns.
+
+struct bdf_json : MappedText {
+    void* d_members = nullptr;          // JsonMember per member of every record, in file order
+    unsigned int* d_slots = nullptr;    // [record][column]: 1 + the member that gives the value, 0 for none
+    int64_t n_members = 0, n_rows = 0, batch = 1024;
+    std::vector<std::string> names;
+    std::vector<int32_t> dtypes, nullable;
+    mutable int64_t exact_fields = 0;
+};
+
+static void json_free(bdf_ctx* c, bdf_json* f) {
+    if (!f) return;
+    if (f->d_members) cudaFreeAsync(f->d_members, c->s_compute);
+    if (f->d_slots) cudaFreeAsync(f->d_slots, c->s_compute);
+    text_free(c, f);
+    delete f;
+}
+static void drop(bdf_ctx* c, bdf_json* f) { json_free(c, f); }
+
+static constexpr unsigned kJsonKeyCap = 1u << 16;   // distinct raw keys per file
+
+struct JsonKeyH { unsigned long long hash, first, kstart; uint32_t klen, rec; };    // k_json.cu's JsonKey
+struct JsonSlowH { long long start, end; int col, pad; long long chunk, row; };    // k_json.cu's JsonSlow
+
+static void put_utf8(std::string& out, uint32_t cp) {
+    if (cp < 0x80) out += (char)cp;
+    else if (cp < 0x800) { out += (char)(0xC0 | cp >> 6); out += (char)(0x80 | (cp & 0x3F)); }
+    else if (cp < 0x10000) { out += (char)(0xE0 | cp >> 12); out += (char)(0x80 | ((cp >> 6) & 0x3F)); out += (char)(0x80 | (cp & 0x3F)); }
+    else { out += (char)(0xF0 | cp >> 18); out += (char)(0x80 | ((cp >> 12) & 0x3F)); out += (char)(0x80 | ((cp >> 6) & 0x3F)); out += (char)(0x80 | (cp & 0x3F)); }
+}
+
+// The key a string's raw bytes [s, e) (between the quotes, already checked) stand for: escapes decoded, \uXXXX pairs of surrogates
+// joined, and a lone surrogate as U+FFFD.
+static std::string json_unescape(const uint8_t* s, const uint8_t* e) {
+    std::string out;
+    auto hex4 = [](const uint8_t* p) { uint32_t v = 0; for (int k = 0; k < 4; k++) { const int c = p[k]; v = v * 16 + (uint32_t)(c <= '9' ? c - '0' : (c | 32) - 'a' + 10); } return v; };
+    while (s < e) {
+        if (*s != '\\') { out += (char)*s++; continue; }
+        const uint8_t x = s[1];
+        s += 2;
+        switch (x) {
+            case 'b': out += '\b'; break;
+            case 'f': out += '\f'; break;
+            case 'n': out += '\n'; break;
+            case 'r': out += '\r'; break;
+            case 't': out += '\t'; break;
+            case 'u': {
+                uint32_t cp = hex4(s);
+                s += 4;
+                if (cp >= 0xD800 && cp < 0xDC00 && e - s >= 6 && s[0] == '\\' && s[1] == 'u') {
+                    const uint32_t lo = hex4(s + 2);
+                    if (lo >= 0xDC00 && lo < 0xE000) { cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00); s += 6; }
+                }
+                put_utf8(out, cp >= 0xD800 && cp < 0xE000 ? 0xFFFD : cp);
+                break;
+            }
+            default: out += (char)x; break;   // " \ /
+        }
+    }
+    return out;
+}
+
+struct JsonNoMembers {
+    void member(const uint8_t*, const uint8_t*, const uint8_t*, const uint8_t*, int, bool) {}
+};
+
+// Line `line` (from 0) is malformed: walk it on the host with the device's rules to say where and why.
+static int json_bad_line(bdf_ctx* c, const bdf_json* f, const unsigned long long* d_nl, int64_t n_nl, int64_t line) {
+    unsigned long long b[2] = {0, 0};
+    if (line > 0) CK(cudaMemcpyAsync(&b[0], d_nl + line - 1, 8, cudaMemcpyDeviceToHost, c->s_compute));
+    if (line < n_nl) CK(cudaMemcpyAsync(&b[1], d_nl + line, 8, cudaMemcpyDeviceToHost, c->s_compute));
+    CK(cudaStreamSynchronize(c->s_compute));
+    const uint8_t* text = f->map + f->off;
+    const int64_t s = line > 0 ? (int64_t)b[0] + 1 : 0, e = line < n_nl ? (int64_t)b[1] : f->n;
+    json::Cursor cur{text + s, text + e, 0, nullptr};
+    JsonNoMembers v;
+    json::record(cur, v);
+    static const char* const what[] = {"malformed record", "the record is not an object", "expected a key (a string)", "expected ':'",
+                                       "expected a value", "expected ',' or a closing bracket", "unterminated string", "invalid escape",
+                                       "control character in a string", "invalid number", "invalid literal", "trailing characters after the object",
+                                       "nesting deeper than 128 levels"};
+    const int code = cur.err >= 0 && cur.err <= json::eDepth ? cur.err : 0;
+    const long long byte = (long long)f->off + (long long)((cur.at ? cur.at : text + s) - text);
+    return fail(BDF_INVALID, "JSON error at line %lld, byte %lld: %s", (long long)line + 1, byte, what[code]);
+}
+
+// The coercion table over the class bits of one column (json_parse.cuh): its dtype, or -1 off the device path.
+static int json_coerce(unsigned bits) {
+    const unsigned t = bits & ~(unsigned)(json::kNull | json::kMissing);
+    if (t & (json::kStr | json::kObj | json::kListOther)) return -1;
+    if (t & json::kBool) return t == json::kBool ? kBool : -1;
+    const bool list = (t & (json::kListInt | json::kListFloat | json::kListEmpty)) != 0;
+    const bool fl = (t & (json::kFloat | json::kListFloat)) != 0, in = (t & (json::kInt | json::kListInt)) != 0;
+    if (!fl && !in) return -1;   // only nulls, or lists that never had a typed element
+    const int scalar = fl ? BDF_F64 : BDF_I64;
+    return list ? BDF_LIST_BASE + scalar : scalar;
+}
+
+static bool json_dtype_ok(int t) {
+    return (t >= 0 && t <= kBool) || (t >= BDF_LIST_BASE && t < BDF_LIST_BASE + BDF_NTYPES) || t == BDF_UTF8 || t == -1;
+}
+
+static int json_open(bdf_ctx* c, const char* path, const bdf_json_options* o, int n_schema, const char* const* schema_names, const int32_t* schema,
+                     bdf_json** out) {
+    if (!path || !o || !out) return fail(BDF_INVALID, "null argument");
+    if (o->batch_size < 1) return fail(BDF_INVALID, "batch_size must be at least 1");
+    if (schema || schema_names) {
+        if (!schema || !schema_names || n_schema < 1) return fail(BDF_INVALID, "an explicit schema needs at least one (name, dtype) pair");
+        for (int i = 0; i < n_schema; i++) {
+            if (!schema_names[i]) return fail(BDF_INVALID, "schema column %d has no name", i);
+            if (!json_dtype_ok(schema[i]))
+                return fail(BDF_UNSUPPORTED, "schema column %d: type %d is not read from JSON (numeric, Boolean, List of a numeric type or Utf8)", i, schema[i]);
+            for (int j = 0; j < i; j++)
+                if (strcmp(schema_names[i], schema_names[j]) == 0) return fail(BDF_INVALID, "schema name '%s' repeats", schema_names[i]);
+        }
+    }
+    Owned<bdf_json> f(c, new (std::nothrow) bdf_json());
+    if (!f.get()) return fail(BDF_OOM, "host allocation failed");
+    f->batch = o->batch_size;
+    const int64_t tile = json_tile_bytes();
+    TRY(text_open(c, path, tile, "JSON", f.get()));
+    const int64_t tiles = std::max<int64_t>((f->n + tile - 1) / tile, 1);
+
+    Scratch<unsigned long long> counts, nl, members, is_rec, sums, small;   // small: [0] first bad line
+    Scratch<void> table;
+    Scratch<unsigned int> flags, bits;   // flags: [0] the key table is full, [1] a hash collision
+    Scratch<int> col_of;
+
+    // the '\n' positions
+    cudaError_t e = counts.alloc(c, (size_t)(tiles + 1) * 8);
+    if (e == cudaSuccess) e = small.alloc(c, 8);
+    if (e == cudaSuccess) e = cudaMemsetAsync(small, 0xff, 8, c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "JSON line index scratch allocation");
+    unsigned long long n_nl = 0;
+    {
+        LaunchTimer t(c, BDF_K_JSON, BDF_U8, f->n, f->n);
+        c->launches++;   // count, scan
+        e = launch_json_nl_count(f->d_text, f->n, counts, c->s_compute);
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&n_nl, counts + tiles, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e == cudaSuccess) e = nl.alloc(c, (size_t)std::max<unsigned long long>(n_nl, 1) * 8);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_JSON, BDF_U64, f->n, f->n + (int64_t)n_nl * 8);
+        e = launch_json_nl_index(f->d_text, f->n, counts, nl, c->s_compute);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "JSON line index");
+
+    // every line checked; its members, and whether it is a record
+    const int64_t lines = (int64_t)n_nl + 1;
+    e = members.alloc(c, (size_t)(lines + 1) * 8);
+    if (e == cudaSuccess) e = is_rec.alloc(c, (size_t)(lines + 1) * 8);
+    if (e == cudaSuccess) e = sums.alloc(c, (size_t)json_scan_sums(lines) * 8);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_JSON, BDF_U64, lines, f->n + lines * 16);
+        e = launch_json_lex(f->d_text, f->n, nl, (long long)n_nl, members, is_rec, small, c->sm_count, c->s_compute);
+    }
+    unsigned long long bad = ~0ull;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&bad, small, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "JSON record check");
+    if (bad != ~0ull) return json_bad_line(c, f.get(), nl, (int64_t)n_nl, (int64_t)bad);
+    {
+        LaunchTimer t(c, BDF_K_JSON, BDF_U64, lines, lines * 32);
+        c->launches += 5;   // two scans of three kernels each
+        e = launch_json_scan(members, lines, sums, c->s_compute);
+        if (e == cudaSuccess) e = launch_json_scan(is_rec, lines, sums, c->s_compute);
+    }
+    unsigned long long tot[2] = {0, 0};
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&tot[0], members + lines, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&tot[1], is_rec + lines, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "JSON record scan");
+    f->n_members = (int64_t)tot[0];
+    f->n_rows = (int64_t)tot[1];
+    if (f->n_rows == 0) return fail(BDF_WOULD_PANIC, "the JSON file has no records: the reference panics at batches[0]");
+    if (tot[0] >= 0xffffffffull) return fail(BDF_UNSUPPORTED, "2^32 - 1 or more object members in one file");
+
+    // the members, and the distinct keys
+    e = cudaMallocAsync(&f->d_members, (size_t)std::max<int64_t>(f->n_members, 1) * json_member_bytes(), c->s_compute);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_JSON, -1, lines, f->n + f->n_members * (int64_t)json_member_bytes());
+        e = launch_json_members(f->d_text, f->n, nl, (long long)n_nl, members, is_rec, f->d_members, c->sm_count, c->s_compute);
+    }
+    if (e == cudaSuccess) e = table.alloc(c, (size_t)kJsonKeyCap * json_key_bytes());
+    if (e == cudaSuccess) e = cudaMemsetAsync(table, 0xff, (size_t)kJsonKeyCap * json_key_bytes(), c->s_compute);
+    if (e == cudaSuccess) e = flags.alloc(c, 8);
+    if (e == cudaSuccess) e = cudaMemsetAsync(flags, 0, 8, c->s_compute);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_JSON, -1, f->n_members, f->n_members * 32);
+        c->launches++;   // insert, gather
+        e = launch_json_keys(f->d_text, f->d_members, f->n_members, table, kJsonKeyCap, flags, c->sm_count, c->s_compute);
+    }
+    static_assert(sizeof(JsonKeyH) == 32, "JsonKey layout");
+    std::vector<JsonKeyH> keys(kJsonKeyCap);
+    unsigned int hflags[2] = {0, 0};
+    if (e == cudaSuccess) e = cudaMemcpyAsync(keys.data(), table, (size_t)kJsonKeyCap * sizeof(JsonKeyH), cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hflags, flags, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "JSON key table");
+    if (hflags[0]) return fail(BDF_UNSUPPORTED, "more than %u distinct keys in one file", kJsonKeyCap);
+
+    // the dictionary: every raw key decoded (escapes are rare: only those need work); a name's first member over its spellings
+    struct Name { unsigned long long first; uint32_t rec; };
+    std::vector<std::string> names;
+    std::vector<Name> seen;
+    std::vector<int> name_of(kJsonKeyCap, -1);
+    for (unsigned s = 0; s < kJsonKeyCap; s++) {
+        const JsonKeyH& k = keys[s];
+        if (k.hash == ~0ull) continue;
+        const uint8_t* p = f->map + f->off + k.kstart;
+        const std::string name = memchr(p, '\\', k.klen) ? json_unescape(p, p + k.klen) : std::string((const char*)p, k.klen);
+        size_t j = 0;
+        while (j < names.size() && names[j] != name) j++;   // names are few
+        if (j == names.size()) { names.push_back(name); seen.push_back(Name{k.first, k.rec}); }
+        else if (k.first < seen[j].first) seen[j] = Name{k.first, k.rec};
+        name_of[s] = (int)j;
+    }
+    const int64_t n_inf = o->max_records < 0 ? f->n_rows : std::min<int64_t>(o->max_records, f->n_rows);
+    std::vector<int> col_of_name(names.size(), -1);
+    if (schema) {
+        for (int i = 0; i < n_schema; i++) {
+            f->names.push_back(schema_names[i]);
+            f->dtypes.push_back(schema[i] == BDF_UTF8 ? -1 : schema[i]);
+            f->nullable.push_back(1);
+            for (size_t j = 0; j < names.size(); j++)
+                if (names[j] == schema_names[i] && f->dtypes.back() >= 0) col_of_name[j] = i;
+        }
+    } else {   // the keys of the inferred records, in the order they are first seen
+        std::vector<size_t> order;
+        for (size_t j = 0; j < names.size(); j++)
+            if ((int64_t)seen[j].rec < n_inf) order.push_back(j);
+        std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return seen[a].first < seen[b].first; });
+        for (size_t i = 0; i < order.size(); i++) {
+            col_of_name[order[i]] = (int)i;
+            f->names.push_back(names[order[i]]);
+        }
+    }
+    const int n_cols = (int)f->names.size();
+    if (n_cols > 65535) return fail(BDF_UNSUPPORTED, "more than 65535 columns");
+    std::vector<int> hcol(kJsonKeyCap, -1);
+    for (unsigned s = 0; s < kJsonKeyCap; s++)
+        if (name_of[s] >= 0) hcol[s] = col_of_name[(size_t)name_of[s]];
+
+    // the slots: which member gives each (record, column)
+    const size_t slot_bytes = (size_t)f->n_rows * (size_t)n_cols * 4;
+    if (n_cols) {
+        e = cudaMallocAsync((void**)&f->d_slots, slot_bytes, c->s_compute);
+        if (e == cudaSuccess) e = cudaMemsetAsync(f->d_slots, 0, slot_bytes, c->s_compute);
+        if (e == cudaSuccess) e = col_of.alloc(c, (size_t)kJsonKeyCap * 4);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(col_of, hcol.data(), (size_t)kJsonKeyCap * 4, cudaMemcpyHostToDevice, c->s_compute);
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_JSON, BDF_U32, f->n_members, f->n_members * 48);
+            e = launch_json_resolve(f->d_text, f->d_members, f->n_members, table, kJsonKeyCap, col_of, n_cols, f->d_slots, flags + 1, c->sm_count, c->s_compute);
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(hflags, flags, 8, cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // hcol is read by the copy
+        if (e != cudaSuccess) return fail_cuda(e, "JSON key resolution");
+        if (hflags[1]) return fail(BDF_UNSUPPORTED, "two different keys of the file share a 64-bit hash");
+    }
+
+    // inference: the class bits of every column over the first n_inf records
+    if (!schema && n_cols) {
+        std::vector<unsigned int> hb((size_t)n_cols, 0u);
+        e = bits.alloc(c, (size_t)n_cols * 4);
+        if (e == cudaSuccess) e = cudaMemsetAsync(bits, 0, (size_t)n_cols * 4, c->s_compute);
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_JSON, BDF_U32, n_inf * n_cols, n_inf * n_cols * 8);
+            e = launch_json_infer(f->d_members, f->d_slots, n_inf * n_cols, n_cols, bits, c->sm_count, c->s_compute);
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(hb.data(), bits, (size_t)n_cols * 4, cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+        if (e != cudaSuccess) return fail_cuda(e, "JSON schema inference");
+        for (int i = 0; i < n_cols; i++) {
+            f->dtypes.push_back(json_coerce(hb[(size_t)i]));
+            f->nullable.push_back((hb[(size_t)i] & (json::kNull | json::kMissing)) ? 1 : 0);
+        }
+    }
+    *out = f.release();
+    return BDF_OK;
+}
+
+// The floats the device could not round: rounded exactly on the host (C locale) and written back by k_csv_scatter.  Entry x goes
+// to element x.row of chunk x.chunk of cols[x.col].
+static int json_exact(bdf_ctx* c, const bdf_json* f, const void* slow, int64_t n_slow, const std::vector<const bdf_col*>& cols) {
+    struct Patch { unsigned long long dst, bits; int width, pad; };   // k_csv.cu's CsvPatch
+    static_assert(sizeof(Patch) == 24, "CsvPatch layout");
+    std::vector<JsonSlowH> sl((size_t)n_slow);
+    CK(cudaMemcpyAsync(sl.data(), slow, (size_t)n_slow * sizeof(JsonSlowH), cudaMemcpyDeviceToHost, c->s_compute));
+    CK(cudaStreamSynchronize(c->s_compute));
+    static locale_t cloc = newlocale(LC_ALL_MASK, "C", (locale_t)0);
+    std::vector<Patch> hp;
+    for (const JsonSlowH& x : sl) {
+        const std::string v((const char*)f->map + f->off + x.start, (size_t)(x.end - x.start));
+        const bdf_col* col = cols[(size_t)x.col];
+        Patch pt{};
+        if (col->dtype == BDF_F64) {
+            const double d = strtod_l(v.c_str(), nullptr, cloc);
+            memcpy(&pt.bits, &d, 8);
+            pt.width = 8;
+        } else {
+            const float fl = strtof_l(v.c_str(), nullptr, cloc);
+            uint32_t b;
+            memcpy(&b, &fl, 4);
+            pt.bits = b;
+            pt.width = 4;
+        }
+        pt.dst = (unsigned long long)(uintptr_t)(col->chunks[(size_t)x.chunk].values + x.row * pt.width);
+        hp.push_back(pt);
+    }
+    Scratch<void> patches;
+    cudaError_t e = patches.alloc(c, hp.size() * sizeof(Patch));
+    if (e == cudaSuccess) e = cudaMemcpyAsync(patches, hp.data(), hp.size() * sizeof(Patch), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_JSON, -1, (int64_t)hp.size(), (int64_t)hp.size() * 32);
+        e = launch_csv_scatter(patches, (long long)hp.size(), c->s_compute);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // hp is read by the copy
+    if (e != cudaSuccess) return fail_cuda(e, "JSON exact rounding");
+    return BDF_OK;
+}
+
+static int json_check_col(const bdf_json* f, int col) {
+    if (col < 0 || col >= (int)f->names.size()) return fail(BDF_INVALID, "column %d out of range (the file has %zu)", col, f->names.size());
+    if (f->dtypes[(size_t)col] < 0)
+        return fail(BDF_UNSUPPORTED, "column %d (%s) is not on the device path (a string, an object or a mix of kinds)", col, f->names[(size_t)col].c_str());
+    return BDF_OK;
+}
+
+static int json_read(bdf_ctx* c, const bdf_json* f, int n_cols, const int32_t* cols, bdf_col** out) {
+    if (!f || !out || (n_cols > 0 && !cols)) return fail(BDF_INVALID, "null argument");
+    if (n_cols < 0 || n_cols > 65535) return fail(BDF_INVALID, "0..65535 columns");
+    for (int i = 0; i < n_cols; i++) {
+        TRY(json_check_col(f, cols[i]));
+        if (f->dtypes[(size_t)cols[i]] > kBool)
+            return fail(BDF_UNSUPPORTED, "column %d (%s) is a List: read it with bdf_json_read_list", cols[i], f->names[(size_t)cols[i]].c_str());
+    }
+    const int64_t batch = f->batch, n_chunks = (f->n_rows + batch - 1) / batch;
+    std::vector<ChunkPlan> plan((size_t)n_chunks);
+    for (int64_t i = 0; i < n_chunks; i++) plan[(size_t)i] = ChunkPlan{std::min(batch, f->n_rows - i * batch), true};
+    std::vector<ColOwner> res;
+    Scratch<char> descs;
+    Scratch<unsigned long long> small;   // [0] slow-path values
+    Scratch<void> slow;
+    const size_t dsz = json_desc_bytes();
+    std::vector<char> hdesc((size_t)std::max(n_cols, 1) * dsz, 0);
+    int64_t float_fields = 0, out_bytes = 0;
+    for (int i = 0; i < n_cols; i++) {
+        const int dt = f->dtypes[(size_t)cols[i]];
+        res.emplace_back(c);
+        TRY(col_alloc(c, dt, plan, nullptr, json_parse_rows(), res[(size_t)i].out()));
+        bdf_col* col = res[(size_t)i].get();
+        const DevChunk& c0 = col->chunks[0];
+        const long long vs = n_chunks > 1 ? (long long)(col->chunks[1].values - c0.values) : 0;
+        const long long bs = n_chunks > 1 ? (long long)((char*)col->chunks[1].validity - (char*)c0.validity) : 0;
+        const DevChunk& cl = col->chunks[(size_t)n_chunks - 1];
+        if (cl.values != c0.values + vs * (n_chunks - 1) || (char*)cl.validity != (char*)c0.validity + bs * (n_chunks - 1))
+            return fail(BDF_INVALID, "internal: JSON output chunks are not evenly spaced");
+        struct Desc { char* values; long long vstride; uint32_t* validity; long long bstride; uint32_t* warp_counts; int dtype; int file_col; } d{
+            c0.values, vs, c0.validity, bs, col->d_warp_counts, dt, cols[i]};
+        static_assert(sizeof(Desc) == 48, "JsonColDesc layout");
+        memcpy(hdesc.data() + (size_t)i * dsz, &d, sizeof d);
+        if (dt == BDF_F32 || dt == BDF_F64) float_fields += f->n_rows;
+        out_bytes += (int64_t)value_bytes(dt, f->n_rows, 0) + bitmap_bytes(f->n_rows);
+    }
+    const long long slow_cap = std::max<long long>(65536, float_fields / 64);
+    cudaError_t e = descs.alloc(c, hdesc.size());
+    if (e == cudaSuccess) e = cudaMemcpyAsync(descs, hdesc.data(), hdesc.size(), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess) e = small.alloc(c, 8);
+    if (e == cudaSuccess) e = cudaMemsetAsync(small, 0, 8, c->s_compute);
+    if (e == cudaSuccess && float_fields) e = slow.alloc(c, (size_t)slow_cap * json_slow_bytes());
+    if (e != cudaSuccess) return fail_cuda(e, "JSON read scratch allocation");
+    unsigned long long n_slow = 0;
+    {
+        const int64_t cells = f->n_rows * n_cols;
+        LaunchTimer t(c, BDF_K_JSON, n_cols == 1 ? f->dtypes[(size_t)cols[0]] : -1, cells, cells * 48 + out_bytes);
+        e = launch_json_parse(f->d_text, f->d_members, f->d_slots, (int)f->names.size(), descs, n_cols, f->n_rows, batch, slow, small, slow_cap, c->s_compute);
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&n_slow, small, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // hdesc is read by the copy
+    if (e != cudaSuccess) return fail_cuda(e, "JSON parse");
+    if ((long long)n_slow > slow_cap)
+        return fail(BDF_UNSUPPORTED, "%llu float values need exact rounding, more than the %lld one read resolves", n_slow, slow_cap);
+    if (n_slow) {
+        std::vector<const bdf_col*> targets;
+        for (auto& r : res) targets.push_back(r.get());
+        TRY(json_exact(c, f, slow, (int64_t)n_slow, targets));
+    }
+    for (int i = 0; i < n_cols; i++) {
+        bdf_col* col = res[(size_t)i].get();
+        col->counts_on_device = true;
+        TRY(fetch_counts(c, col));
+        for (size_t j = 0; j < col->chunks.size(); j++)
+            if (col->null_counts[j] == 0) col->chunks[j].validity = nullptr;   // no bitmap in a chunk without nulls
+        e = finish_single_group(c, col);
+        if (e != cudaSuccess) return fail_cuda(e, "JSON read");
+    }
+    f->exact_fields = (int64_t)n_slow;
+    for (int i = 0; i < n_cols; i++) out[i] = res[(size_t)i].release();
+    return BDF_OK;
+}
+
+static int json_read_list(bdf_ctx* c, const bdf_json* f, int col, bdf_list** out) {
+    if (!f || !out) return fail(BDF_INVALID, "null argument");
+    TRY(json_check_col(f, col));
+    const int ldt = f->dtypes[(size_t)col];
+    if (ldt < BDF_LIST_BASE) return fail(BDF_UNSUPPORTED, "column %d (%s) is not a List: read it with bdf_json_read", col, f->names[(size_t)col].c_str());
+    const int dt = ldt - BDF_LIST_BASE;
+    const int64_t batch = f->batch, n_rows = f->n_rows, n_chunks = (n_rows + batch - 1) / batch, words = (batch + 31) / 32;
+    const int n_file_cols = (int)f->names.size();
+    Scratch<unsigned long long> counts, sums, bounds, nulls, small;   // nulls: [chunk] null lists, then [chunk] null elements; small: slow values
+    Scratch<uint32_t> vwords;
+    Scratch<void> descs, slow;
+    cudaError_t e = counts.alloc(c, (size_t)(n_rows + 1) * 8);
+    if (e == cudaSuccess) e = sums.alloc(c, (size_t)json_scan_sums(n_rows) * 8);
+    if (e == cudaSuccess) e = bounds.alloc(c, (size_t)(n_chunks + 1) * 8);
+    if (e == cudaSuccess) e = nulls.alloc(c, (size_t)n_chunks * 16);
+    if (e == cudaSuccess) e = cudaMemsetAsync(nulls, 0, (size_t)n_chunks * 16, c->s_compute);
+    if (e == cudaSuccess) e = vwords.alloc(c, (size_t)(n_chunks * words) * 4);
+    if (e != cudaSuccess) return fail_cuda(e, "JSON list scratch allocation");
+    {
+        LaunchTimer t(c, BDF_K_JSON, ldt, n_rows, n_rows * 16);
+        c->launches += 4;   // count, the scan's three kernels, bounds
+        e = launch_json_list_count(f->d_text, f->d_members, f->d_slots, n_file_cols, col, n_rows, batch, counts, vwords, nulls, c->s_compute);
+        if (e == cudaSuccess) e = launch_json_scan(counts, n_rows, sums, c->s_compute);
+        if (e == cudaSuccess) e = launch_json_bounds(counts, n_rows, batch, n_chunks, bounds, c->s_compute);
+    }
+    std::vector<unsigned long long> hb((size_t)n_chunks + 1), hn((size_t)n_chunks * 2);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hb.data(), bounds, hb.size() * 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hn.data(), nulls, (size_t)n_chunks * 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "JSON list count");
+    if (hb[(size_t)n_chunks] >= (unsigned long long)kListMaxCallElems)
+        return fail(BDF_UNSUPPORTED, "a list call holds 2^32 or more elements (the sort's UInt32 row numbers)");
+    std::vector<int64_t> lens((size_t)n_chunks), elems((size_t)n_chunks);
+    std::vector<ChunkPlan> plan((size_t)n_chunks);
+    for (int64_t i = 0; i < n_chunks; i++) {
+        lens[(size_t)i] = std::min(batch, n_rows - i * batch);
+        elems[(size_t)i] = (int64_t)(hb[(size_t)i + 1] - hb[(size_t)i]);
+        if (elems[(size_t)i] >= kListMaxChunkElems) return fail(BDF_UNSUPPORTED, "list chunk %lld: 2^31 or more elements", (long long)i);
+        plan[(size_t)i] = ChunkPlan{elems[(size_t)i], true};
+    }
+    ListOwner l(c);
+    TRY(list_alloc(c, dt, lens, std::vector<bool>((size_t)n_chunks, true), l.out()));
+    ColOwner child(c);
+    TRY(col_alloc(c, dt, plan, nullptr, 0, child.out()));
+    struct Chunk { int32_t* offsets; uint32_t* validity; char* values; uint32_t* value_validity; };
+    static_assert(sizeof(Chunk) == 32, "JsonListChunk layout");
+    std::vector<Chunk> hc((size_t)n_chunks);
+    for (int64_t i = 0; i < n_chunks; i++) {
+        const DevChunk& ch = child->chunks[(size_t)i];
+        hc[(size_t)i] = Chunk{l->off[(size_t)i], l->valid[(size_t)i], ch.values, ch.validity};
+    }
+    const int64_t total = (int64_t)hb[(size_t)n_chunks];
+    const long long slow_cap = std::max<long long>(65536, total / 64);
+    e = descs.alloc(c, hc.size() * sizeof(Chunk));
+    if (e == cudaSuccess) e = cudaMemcpyAsync(descs, hc.data(), hc.size() * sizeof(Chunk), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess) e = small.alloc(c, 8);
+    if (e == cudaSuccess) e = cudaMemsetAsync(small, 0, 8, c->s_compute);
+    if (e == cudaSuccess && dtype_is_float(dt)) e = slow.alloc(c, (size_t)slow_cap * json_slow_bytes());
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_JSON, dt, total, n_rows * 48 + total * (dtype_width(dt) + 16));
+        e = launch_json_list_fill(f->d_text, f->d_members, f->d_slots, n_file_cols, col, dt, n_rows, batch, counts, vwords, descs, nulls + n_chunks, slow,
+                                  small, slow_cap, c->s_compute);
+    }
+    unsigned long long n_slow = 0;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hn.data() + n_chunks, nulls + n_chunks, (size_t)n_chunks * 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&n_slow, small, 8, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // hc is read by the copy
+    if (e != cudaSuccess) return fail_cuda(e, "JSON list fill");
+    if ((long long)n_slow > slow_cap)
+        return fail(BDF_UNSUPPORTED, "%llu float values need exact rounding, more than the %lld one read resolves", n_slow, slow_cap);
+    if (n_slow) TRY(json_exact(c, f, slow, (int64_t)n_slow, {child.get()}));
+    for (int64_t i = 0; i < n_chunks; i++) {
+        const size_t k = (size_t)i;
+        l->null_counts[k] = (int64_t)hn[k];
+        l->valid_elems[k] = elems[k];   // a null list has no elements
+        if (hn[k] == 0) l->valid[k] = nullptr;   // no bitmap in a chunk without null lists
+        child->null_counts[k] = (int64_t)hn[(size_t)n_chunks + k];
+        if (child->null_counts[k] == 0) child->chunks[k].validity = nullptr;
+    }
+    e = finish_single_group(c, child.get());
+    if (e != cudaSuccess) return fail_cuda(e, "JSON list read");
+    f->exact_fields = (int64_t)n_slow;
+    l->values = child.release();
+    *out = l.release();
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // C ABI
 
 #define NEED_CTX(ctx) \
@@ -5040,6 +5549,57 @@ void bdf_csv_close(bdf_ctx* c, bdf_csv* f) {
     std::lock_guard<std::mutex> lock(c->mu);
     cudaSetDevice(c->device);
     csv_free(c, f);
+}
+
+int bdf_json_open(bdf_ctx* c, const char* path, const bdf_json_options* options, int32_t n_schema, const char* const* schema_names,
+                  const int32_t* schema_dtypes, bdf_json** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the JSON reader reads into one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return json_open(c, path, options, n_schema, schema_names, schema_dtypes, out);
+}
+
+int bdf_json_describe(const bdf_json* f, int32_t* n_columns, int64_t* n_batches, int64_t* n_rows) {
+    if (!f) return fail(BDF_INVALID, "null file");
+    if (n_columns) *n_columns = (int32_t)f->names.size();
+    if (n_batches) *n_batches = (f->n_rows + f->batch - 1) / f->batch;
+    if (n_rows) *n_rows = f->n_rows;
+    return BDF_OK;
+}
+
+int bdf_json_column(const bdf_json* f, int32_t col, const char** name, int32_t* dtype, int32_t* nullable) {
+    if (!f) return fail(BDF_INVALID, "null file");
+    if (col < 0 || col >= (int32_t)f->names.size()) return fail(BDF_INVALID, "column %d out of range", col);
+    if (name) *name = f->names[(size_t)col].c_str();
+    if (dtype) *dtype = f->dtypes[(size_t)col];
+    if (nullable) *nullable = f->nullable[(size_t)col];
+    return BDF_OK;
+}
+
+int bdf_json_read(bdf_ctx* c, const bdf_json* f, int32_t n_cols, const int32_t* cols, bdf_col** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the JSON reader reads into one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return json_read(c, f, n_cols, cols, out);
+}
+
+int bdf_json_read_list(bdf_ctx* c, const bdf_json* f, int32_t col, bdf_list** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the JSON reader reads into one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return json_read_list(c, f, col, out);
+}
+
+int bdf_json_stats(const bdf_json* f, int64_t* n_members, int64_t* exact_fields, double* upload_ms) {
+    if (!f) return fail(BDF_INVALID, "null file");
+    if (n_members) *n_members = f->n_members;
+    if (exact_fields) *exact_fields = f->exact_fields;
+    if (upload_ms) *upload_ms = f->upload_ms;
+    return BDF_OK;
+}
+
+void bdf_json_close(bdf_ctx* c, bdf_json* f) {
+    if (!c || !f || c->fleet) return;
+    std::lock_guard<std::mutex> lock(c->mu);
+    cudaSetDevice(c->device);
+    json_free(c, f);
 }
 
 int bdf_csv_write(bdf_ctx* c, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,

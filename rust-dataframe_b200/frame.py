@@ -38,6 +38,7 @@ from . import _native as N
 from .arrays import F32, F64, I8, I64, U8, U32, U64, PrimitiveArray, is_float
 from .functions import Column, _expr_nodes, eval_expr, sort_indices, window as _window
 from .csv_reader import CsvFile, write_csv
+from .json_reader import JsonFile
 from .ipc import BOOL, IpcFile, write_ipc
 
 ARITH = {"add": N.ADD, "subtract": N.SUB, "multiply": N.MUL, "divide": N.DIV}
@@ -406,6 +407,17 @@ class DeviceFrame:
         with CsvFile(path, has_header=has_header, delimiter=delimiter, max_records=max_records, batch_size=batch_size, schema=schema,
                      ctx=ctx) as f:
             names = [n for n, dt, _ in f.schema if dt >= 0 and (columns is None or n in columns)]
+            cols = f.read(names)
+        return cls(OrderedDict((n, cols[n]) for n in names))
+
+    @classmethod
+    def from_json(cls, path: str, schema: Optional[Sequence[Tuple[str, int]]] = None, max_records: Optional[int] = None, batch_size: int = 1024,
+                  ctx: Optional[N.Context] = None) -> "DeviceFrame":
+        """DataFrame::from_json over a line-delimited file: one object per line, the schema inferred from every record (or the given
+        (name, dtype) pairs), 1024 rows per RecordBatch.  The numeric and Boolean columns are taken; List columns (frames do not carry
+        lists yet; read them with JsonFile.read_list) and columns off the device path are left out."""
+        with JsonFile(path, schema=schema, max_records=max_records, batch_size=batch_size, ctx=ctx) as f:
+            names = [n for n, dt, _ in f.schema if 0 <= dt <= N.BOOL]
             cols = f.read(names)
         return cls(OrderedDict((n, cols[n]) for n in names))
 
