@@ -264,6 +264,7 @@ struct bdf_ctx {
     void* flush_buf = nullptr;
     size_t flush_bytes = 0;
     size_t pipeline_bytes = (size_t)32 << 20;
+    bool pipeline_split = false;   // BDF_PIPELINE_SPLIT: split operators at every input group end, landed or not
     bool profiling = false;
     std::vector<ProfEntry> prof;
     std::vector<cudaEvent_t> prof_pool;   // recycled timing events
@@ -506,9 +507,10 @@ static void wait_groups(cudaStream_t s, const bdf_col* col, int64_t begin, int64
 }
 
 // Group boundaries for an operator over `n` chunks: a single group when the inputs are resident, else
-// the union of the inputs' group ends (so work starts as soon as its own inputs have landed).
-static std::vector<int64_t> plan_groups(int64_t n, std::initializer_list<const bdf_col*> inputs) {
-    bool all_done = true;
+// the union of the inputs' group ends (so work starts as soon as its own inputs have landed).  A context made with
+// BDF_PIPELINE_SPLIT=1 always splits at the group ends, so that the grouped launches run whether or not the copies have landed.
+static std::vector<int64_t> plan_groups(const bdf_ctx* c, int64_t n, std::initializer_list<const bdf_col*> inputs) {
+    bool all_done = !c->pipeline_split;
     for (auto* col : inputs) all_done = all_done && col_complete(col);
     std::vector<int64_t> ends;
     if (!all_done)
@@ -1002,7 +1004,7 @@ static int binary_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bd
         TRY(future_new(c, dtype, 1, total_rows, f.out()));
         e = part_acquire(c, total_tiles, &pb);
     }
-    const std::vector<int64_t> ends = plan_groups(n, {l, r});
+    const std::vector<int64_t> ends = plan_groups(c, n, {l, r});
     if (e == cudaSuccess && op == BDF_DIV) e = cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute);
     if (e != cudaSuccess) return fail_cuda(e, "binary op");
     ColOwner o(c);
@@ -1053,7 +1055,7 @@ static int map_dev(bdf_ctx* c, bool is_cast, int op_or_to, const bdf_col* in, bd
     for (int64_t i = 0; i < n; i++) plan[i] = {in->chunks[i].len, in->chunks[i].validity != nullptr || fallible};
     const int tile = is_cast ? elems_per_tile_cast(from, to) : elems_per_tile_unary(op_or_to, from);
     const int wf = dtype_width(from), wt = dtype_width(to);
-    return launch_groups(c, {in}, plan_groups(n, {in}), to, plan, tile, sizeof(UnDesc), is_cast ? BDF_K_CAST : BDF_K_UNARY,
+    return launch_groups(c, {in}, plan_groups(c, n, {in}), to, plan, tile, sizeof(UnDesc), is_cast ? BDF_K_CAST : BDF_K_UNARY,
         is_cast ? "cast" : "unary op",
         [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
             const DevChunk& a = in->chunks[i];
@@ -1157,7 +1159,7 @@ static int temporal_dev(bdf_ctx* c, const TemporalPlan& pl, const bdf_col* in, b
     for (int64_t i = 0; i < n; i++) plan[i] = {in->chunks[i].len, true};   // range rules can turn any slot NULL
     const int tile = elems_per_tile_temporal(pl.in_dtype, pl.out_dtype);
     const int wi = dtype_width(pl.in_dtype), wo = dtype_width(pl.out_dtype);
-    return launch_groups(c, {in}, plan_groups(n, {in}), pl.out_dtype, plan, tile, sizeof(UnDesc), BDF_K_TEMPORAL, "temporal function",
+    return launch_groups(c, {in}, plan_groups(c, n, {in}), pl.out_dtype, plan, tile, sizeof(UnDesc), BDF_K_TEMPORAL, "temporal function",
         [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
             const DevChunk& a = in->chunks[i];
             ((UnDesc*)hd)[i] = UnDesc{a.values, oc.values, a.validity, oc.validity, a.len, tile0, a.bit_off, 0};
@@ -1198,7 +1200,7 @@ static int temporal_binary_dev(bdf_ctx* c, int fn, const bdf_temporal_type* ta, 
     for (int64_t i = 0; i < n; i++) plan[i] = {a->chunks[i].len, true};
     const int tile = elems_per_tile_temporal2(a->dtype, b->dtype, out_dtype);
     const int wrow = dtype_width(a->dtype) + dtype_width(b->dtype) + dtype_width(out_dtype);
-    return launch_groups(c, {a, b}, plan_groups(n, {a, b}), out_dtype, plan, tile, sizeof(BinDesc), BDF_K_TEMPORAL, "temporal function",
+    return launch_groups(c, {a, b}, plan_groups(c, n, {a, b}), out_dtype, plan, tile, sizeof(BinDesc), BDF_K_TEMPORAL, "temporal function",
         [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
             const DevChunk &x = a->chunks[i], &y = b->chunks[i];
             ((BinDesc*)hd)[i] = BinDesc{x.values, y.values, oc.values, x.validity, y.validity, oc.validity, x.len, tile0, x.bit_off, y.bit_off};
@@ -4909,6 +4911,8 @@ static int init_impl(bdf_ctx* c, int device) {
     if (const char* fg = getenv("BDF_L2_FETCH")) { if (atoi(fg) > 0) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)atoi(fg)); cudaGetLastError(); }
     const char* pb = getenv("BDF_PIPELINE_BYTES");
     if (pb && atoll(pb) > 0) c->pipeline_bytes = (size_t)atoll(pb);
+    const char* ps = getenv("BDF_PIPELINE_SPLIT");
+    c->pipeline_split = ps && atoi(ps) > 0;
     return BDF_OK;
 }
 
