@@ -12,6 +12,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --lists [--rows 100000000]                       # the list-function rows (ArrayFunctions)
     python benchmarks/kernels_bench.py --temporal [--rows 100000000]                    # the date / timestamp function rows
     python benchmarks/kernels_bench.py --ndjson [--csv-rows 50000000]                   # the line-delimited JSON reader rows (a 4.85 GB temporary file)
+    python benchmarks/kernels_bench.py --parquet [--csv-rows 50000000]                  # the Parquet reader rows (two temporary files: snappy, none)
 """
 from __future__ import annotations
 
@@ -177,6 +178,80 @@ def write_ndjson(path, rows, seed=13, block=2_000_000):
                 m[:, c + 1] = np.where(has, d[:, 0], 32)
                 m[:, c + 2] = np.where(has, d[:, 1], 32)
             f.write(m.tobytes())
+
+
+def write_parquet_table(path, rows, compression, seed=17, block=5_000_000):
+    """Int64 id, two Float64 (b: 10 % nulls, values on a grid of 1/64 so that it dictionary-encodes), Boolean, Date32, Timestamp(us),
+    written by pyarrow with its defaults (snappy + dictionary) or uncompressed."""
+    import pyarrow as pa
+    import pyarrow.parquet as pq
+
+    rng = np.random.default_rng(seed)
+    schema = pa.schema([("id", pa.int64()), ("a", pa.float64()), ("b", pa.float64()), ("ok", pa.bool_()), ("d", pa.date32()),
+                        ("ts", pa.timestamp("us"))])
+    with pq.ParquetWriter(path, schema, compression=compression) as w:
+        for s in range(0, rows, block):
+            n = min(block, rows - s)
+            w.write_table(pa.table({
+                "id": pa.array(np.arange(s, s + n, dtype=np.int64)),
+                "a": pa.array(rng.standard_normal(n)),
+                "b": pa.array(rng.integers(0, 4096, n) / 64.0, mask=rng.random(n) < 0.1),
+                "ok": pa.array(rng.random(n) < 0.5),
+                "d": pa.array(rng.integers(0, 20000, n).astype(np.int32), pa.date32()),
+                "ts": pa.array(1_600_000_000_000_000 + np.sort(rng.integers(0, 10 ** 13, n)), pa.timestamp("us")),
+            }, schema=schema))
+
+
+def parquet_bench(ctx, rows, rows_out, reps=3):
+    """Parquet -> device columns, for a file written with pyarrow's defaults and one written uncompressed: the upload of the column
+    chunks, snappy, the run walk + levels and the values (launch records), end to end (open + read + synchronise); pyarrow's
+    read_table on the host for comparison."""
+    import pyarrow.parquet as pq
+
+    names = ["id", "a", "b", "ok", "d", "ts"]
+    with tempfile.TemporaryDirectory() as td:
+        for label, comp in (("snappy", "snappy"), ("none", "none")):
+            path = os.path.join(td, f"bench-{label}.parquet")
+            write_parquet_table(path, rows, comp)
+            fbytes = os.path.getsize(path)
+            e2e, up, sn, lv, va, ub, sb, ob = [], [], [], [], [], 0, 0, 0
+            for _ in range(reps + 1):
+                ctx.synchronize()
+                ctx.profile_read()
+                ctx.profile_enable(True)
+                t0 = time.perf_counter()
+                with rdf.ParquetFile(path) as f:
+                    cols = f.read(names, ctx=ctx)
+                    ctx.synchronize()
+                    t1 = time.perf_counter()
+                    st = f.stats()
+                ctx.profile_enable(False)
+                recs = [r for r in ctx.profile_read() if r["kernel"] == "parquet"]
+                assert len(recs) == 4, recs
+                for c in cols.values():
+                    c.free()
+                e2e.append((t1 - t0) * 1e3)
+                up.append(st["upload_ms"])
+                sn.append(recs[0]["ms"]); lv.append(recs[1]["ms"] + recs[2]["ms"]); va.append(recs[3]["ms"])
+                ub, sb, ob = st["uploaded_bytes"], recs[0]["bytes"] - st["uploaded_bytes"], recs[3]["bytes"]
+            med = lambda v: float(np.median(v[1:]))   # the first run warms up
+            for name, ms, nbytes in ((f"parquet[{label}] upload (page cache -> HBM)", med(up), ub),
+                                     (f"parquet[{label}] snappy", med(sn), ub + sb),
+                                     (f"parquet[{label}] runs + levels", med(lv), ub + sb),
+                                     (f"parquet[{label}] values", med(va), ub + sb + ob),
+                                     (f"parquet[{label}] file -> device columns, end to end", med(e2e), fbytes)):
+                rows_out.append({"case": name, "config": "parquet", "kernel": "parquet", "ms": ms, "rows": rows, "bytes": nbytes,
+                                 "file_bytes": fbytes, "uploaded_bytes": ub, "scratch_bytes": sb, "output_bytes": ob})
+                print(f"{name:52s} {ms:9.2f} ms  {nbytes / 1e9:6.2f} GB  {nbytes / ms / 1e6:8.1f} GB/s", flush=True)
+            ts = []
+            for _ in range(2):
+                t0 = time.perf_counter()
+                pq.read_table(path, columns=names)
+                ts.append((time.perf_counter() - t0) * 1e3)
+            ms = min(ts)
+            name = f"parquet[{label}] pyarrow read_table (not the reference), {os.cpu_count()} cores"
+            rows_out.append({"case": name, "config": "parquet", "kernel": "host", "ms": ms, "rows": rows, "file_bytes": fbytes})
+            print(f"{name:52s} {ms:9.2f} ms  {fbytes / 1e9:6.2f} GB of file", flush=True)
 
 
 def ndjson_bench(ctx, rows, rows_out, reps=3):
@@ -583,8 +658,20 @@ def main():
     ap.add_argument("--lists", action="store_true", help="run only the list-function rows (ArrayFunctions)")
     ap.add_argument("--temporal", action="store_true", help="run only the date / timestamp function rows")
     ap.add_argument("--ndjson", action="store_true", help="run the line-delimited JSON reader rows (--csv-rows records)")
+    ap.add_argument("--parquet", action="store_true", help="run the Parquet reader rows (--csv-rows rows, snappy and uncompressed)")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.parquet:
+        import subprocess
+
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+        print(f"card: {q.strip()}", flush=True)
+        rows_out = []
+        parquet_bench(ctx, args.csv_rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"card": q.strip(), "results": rows_out}, f, indent=1)
+        return
     if args.ndjson:
         import subprocess
 

@@ -810,6 +810,70 @@ int  bdf_ipc_read_temporal(bdf_ctx* ctx, const bdf_ipc* file, int32_t col, int f
 int  bdf_ipc_write_typed(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
                          const bdf_temporal_type* types /* n_cols entries, or NULL */);
 
+/* ---- Parquet files straight to the device (DataFrame::from_parquet, src/dataframe.rs) ----------------------------------------------
+ * The reference reads a file, or every file of a directory, with parquet's ParquetFileArrowReader in batches of 1024 rows.  Rules
+ * marked RECALLED are recalled from arrow-rs of that era, parity unpinned; the others are this library's decisions.
+ * Files.  "PAR1" at both ends and a Thrift compact-protocol FileMetaData footer, parsed on the host: every read is bounds-checked,
+ *   nesting is limited to 32 levels and unknown field ids are skipped (so footers with page indexes, bloom filters, size or geo
+ *   statistics parse).  An encrypted file ("PARE") or a ColumnChunk.file_path pointing into another file -> BDF_UNSUPPORTED.
+ * Pages.  DATA_PAGE (V1), DATA_PAGE_V2 (is_compressed = false included) and at most one DICTIONARY_PAGE, first in its chunk;
+ *   INDEX_PAGE is skipped.  Page CRCs are NOT checked.
+ * Codecs.  UNCOMPRESSED and SNAPPY.  Any other (GZIP, BROTLI, LZ4, LZ4_RAW, ZSTD, LZO) -> BDF_UNSUPPORTED naming the codec when that
+ *   column is read (or checked); the file still opens and the other columns still read.
+ * Encodings.  Values: PLAIN; PLAIN_DICTIONARY / RLE_DICTIONARY ids over a PLAIN dictionary page; RLE for Boolean; BYTE_STREAM_SPLIT for
+ *   the fixed-width types.  A chunk may switch from dictionary to PLAIN pages part-way (what a writer does when the dictionary
+ *   outgrows its limit).  Definition levels: the RLE / bit-packed hybrid.  DELTA_*, the deprecated BIT_PACKED levels, and any
+ *   other encoding -> BDF_UNSUPPORTED for that column, naming the encoding.
+ * Types.  Only top-level primitive columns, required or optional (maximum definition level 0 or 1).  A group, a repeated field or any
+ *   other type is one column of dtype -1, stepped over (as the CSV reader steps over Utf8).  Logical types win over converted types:
+ *     BOOLEAN -> Boolean;  FLOAT -> Float32;  DOUBLE -> Float64
+ *     INT32, none / INT(8|16|32, signed) / INT_8, INT_16, INT_32    -> Int32 / Int8, Int16, Int32
+ *     INT32, INT(8|16|32, unsigned) / UINT_8, UINT_16, UINT_32      -> UInt8, UInt16, UInt32
+ *     INT64, none / INT(64, signed) / INT_64; INT(64, unsigned) / UINT_64 -> Int64; UInt64
+ *     INT32 DATE -> Date32;  INT32 TIME(MILLIS) / TIME_MILLIS -> Time32(ms);  INT64 TIME(MICROS | NANOS) / TIME_MICROS -> Time64(us | ns)
+ *     INT64 TIMESTAMP(unit, isAdjustedToUTC) -> Timestamp(unit, "UTC" if adjusted, else no tz); TIMESTAMP_MILLIS / _MICROS (converted
+ *       only, which the format defines as adjusted to UTC) -> Timestamp(ms | us, "UTC")
+ *     INT96, DECIMAL, FLOAT16, BYTE_ARRAY, FIXED_LEN_BYTE_ARRAY, anything else -> dtype -1
+ *   Temporal columns report their physical dtype (BDF_I32 / BDF_I64) from bdf_parquet_column; bdf_parquet_temporal_column gives the tag.
+ *   Narrow integers: an INT(8|16) value stored in INT32 that does not fit its type is TRUNCATED to its low bits.
+ *   Timestamp tz: when the footer holds an ARROW:schema entry (an Arrow IPC schema message, base64) whose top-level field at the same
+ *   position has the same name and is a Timestamp of the same unit, the tz is that field's (as pyarrow restores a "+01:00" or
+ *   "Europe/Paris" column).  A malformed entry is ignored.  The unit is always Parquet's: departure (1), pyarrow restores a
+ *   Timestamp(s) column from Arrow's metadata; here it reads as Timestamp(ms), and a Date64 column (stored as DATE) as Date32.
+ *   Because the units then differ, such a Timestamp(s, tz) column also loses a named tz: it reads as Timestamp(ms, "UTC") (the
+ *   Parquet type's isAdjustedToUTC), where pyarrow restores Timestamp(s, tz).
+ * Output.  One chunk of batch_size rows (default 1024) per RecordBatch: the batches run across the row groups of one file, and each
+ *   file starts a new chunk (RECALLED; parity unpinned).  Null counts are set; a chunk without nulls has no validity bitmap; a required
+ *   column is not nullable.  A null slot holds 0.
+ * Directories.  The regular files of the directory in byte order of their names (departure (2): the reference takes read_dir's
+ *   unspecified order); names starting with '.' or '_' (_SUCCESS) are skipped (departure (3): the reference fails on them); files
+ *   with zero row groups are skipped.  The first file left gives the schema; every other file must have the same column names, dtypes
+ *   and temporal types (tz included), else BDF_INVALID naming the file and column; nullable is the OR over the files.  No file left
+ *   -> BDF_WOULD_PANIC (the reference's schema.unwrap()).
+ * Errors.  Found on the host: BDF_INVALID "Parquet error in FILE[, row group G][, column C][, page P]: what" -- bad magic, a footer or
+ *   column chunk outside the file, a page header or page running past its chunk, data-page num_values not adding up to the row
+ *   group's rows, more than one dictionary page, dictionary ids without a dictionary.  A bad footer fails bdf_parquet_open; a bad
+ *   chunk fails bdf_parquet_check and a read of its column.  Found on the device (a per-page error word, read back once at the end
+ *   of the read): the same status and message shape -- a corrupt snappy stream, a decompressed size that differs from the page
+ *   header, a dictionary index outside the dictionary, a level, index or value stream that ends early.
+ * Memory.  A read uploads the projected column chunks only, still compressed (bdf_parquet_stats counts their bytes), and needs
+ *   the decompressed size of its snappy pages, run tables of 8 B per entry (per level or index stream, at most min(values, stream
+ *   bytes) + 1 entries), and its outputs; what does not fit gives
+ *   BDF_OOM before anything is uploaded.  A failed call leaks nothing.  The open needs no context and no GPU; a read on a multi-GPU
+ *   context -> BDF_UNSUPPORTED. */
+typedef struct { int64_t batch_size; } bdf_parquet_options;
+typedef struct bdf_parquet bdf_parquet;
+int  bdf_parquet_open(const char* path /* a file or a directory */, const bdf_parquet_options* options /* NULL: defaults */, bdf_parquet** out);
+int  bdf_parquet_describe(const bdf_parquet* file, int32_t* n_columns, int64_t* n_batches, int64_t* n_rows);
+int  bdf_parquet_column(const bdf_parquet* file, int32_t col, const char** name, int32_t* dtype /* physical; -1 off the path */, int32_t* nullable);
+int  bdf_parquet_temporal_column(const bdf_parquet* file, int32_t col, bdf_temporal_type* out);   /* kind 0: not temporal */
+/* No GPU: the status a read of col would give for every cause the host can detect (off the path, codec, encoding, a bad chunk). */
+int  bdf_parquet_check(const bdf_parquet* file, int32_t col);
+int  bdf_parquet_read(bdf_ctx* ctx, const bdf_parquet* file, int32_t n_cols, const int32_t* cols, bdf_col** out /* n_cols */);   /* projection */
+/* of the last read: data and dictionary pages decoded, compressed bytes uploaded, host time of the upload */
+int  bdf_parquet_stats(const bdf_parquet* file, int64_t* n_pages, int64_t* uploaded_bytes, double* upload_ms);
+void bdf_parquet_close(bdf_parquet* file);
+
 /* ---- measurement support ------------------------------------------------------------------------ */
 /* Per-launch CUDA-event timing on the library's compute stream (the stream the kernels run on). */
 typedef struct {
@@ -819,7 +883,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL, BDF_K_JSON } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL, BDF_K_JSON, BDF_K_PARQUET } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

@@ -27,11 +27,15 @@ pub struct BdfOut {
 pub enum BdfCtx {}
 pub enum BdfCol {}   // a column resident in HBM (one chunk per RecordBatch)
 pub enum BdfIpc {}   // a mapped Arrow IPC file
+pub enum BdfParquet {}   // the mapped files of a Parquet read, footers and page headers parsed
 pub enum BdfCsv {}
 pub const BDF_PARSE: i32 = 9;   // -> ArrowError::ParseError(last_error())
 pub const BDF_UTF8: i32 = 11;   // CSV schema entry: a string column the device skips
 #[repr(C)]
 pub struct BdfCsvOptions { pub has_header: i32, pub delimiter: u8, pub max_records: i64 /* <0: all */, pub batch_size: i64 }
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct BdfParquetOptions { pub batch_size: i64 }
 #[repr(C)]
 #[derive(Clone, Copy)]
 pub struct BdfCsvWriteOptions { pub has_header: i32, pub delimiter: u8 }
@@ -244,6 +248,15 @@ extern "C" {
     pub fn bdf_ipc_read_temporal(ctx: *mut BdfCtx, file: *const BdfIpc, col: i32, flags: c_int, out: *mut *mut BdfCol) -> c_int;
     pub fn bdf_ipc_write_typed(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol,
                                types: *const BdfTemporalType) -> c_int;
+    // Parquet files straight to the device (include/b200df.h "Parquet files straight to the device")
+    pub fn bdf_parquet_open(path: *const c_char, options: *const BdfParquetOptions, out: *mut *mut BdfParquet) -> c_int;
+    pub fn bdf_parquet_describe(file: *const BdfParquet, n_columns: *mut i32, n_batches: *mut i64, n_rows: *mut i64) -> c_int;
+    pub fn bdf_parquet_column(file: *const BdfParquet, col: i32, name: *mut *const c_char, dtype: *mut i32, nullable: *mut i32) -> c_int;
+    pub fn bdf_parquet_temporal_column(file: *const BdfParquet, col: i32, out: *mut BdfTemporalType) -> c_int;
+    pub fn bdf_parquet_check(file: *const BdfParquet, col: i32) -> c_int;
+    pub fn bdf_parquet_read(ctx: *mut BdfCtx, file: *const BdfParquet, n_cols: i32, cols: *const i32, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_parquet_stats(file: *const BdfParquet, n_pages: *mut i64, uploaded_bytes: *mut i64, upload_ms: *mut f64) -> c_int;
+    pub fn bdf_parquet_close(file: *mut BdfParquet);
 }
 
 /// bdf_temporal_type: kind (0 none, 1 Date32, 2 Date64, 3 Timestamp, 4 Time32, 5 Time64), unit (arrow TimeUnit order), tz (Timestamp).

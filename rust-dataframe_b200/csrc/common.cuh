@@ -442,6 +442,20 @@ cudaError_t launch_csv_parse(const uint8_t* text, const unsigned long long* ends
                              long long batch, unsigned long long* err_key, void* slow, unsigned long long* n_slow, long long slow_cap, cudaStream_t s);
 cudaError_t launch_csv_scatter(const void* patches, long long n, cudaStream_t s);
 
+// Parquet reader (k_parquet.cu; the page, tile, output and run records are parquet_decode.cuh's pq::Page, Tile, Out and Run).
+size_t pq_page_bytes();
+size_t pq_tile_bytes();
+size_t pq_out_bytes();
+size_t pq_run_bytes();
+cudaError_t launch_pq_snappy(const void* pages, int n_pages, const uint8_t* upload, uint8_t* scratch, int* err, int sm_count, cudaStream_t s);
+cudaError_t launch_pq_runs(const void* pages, int n_pages, const uint8_t* upload, const uint8_t* scratch, void* runs, void* meta, int* err,
+                           cudaStream_t s);
+cudaError_t launch_pq_levels(const void* pages, const void* tiles, int n_tiles, const uint8_t* upload, const uint8_t* scratch, const void* runs,
+                             const void* meta, const void* outs, long long batch, int* tile_valid, unsigned long long* nulls, int* err,
+                             cudaStream_t s);
+cudaError_t launch_pq_values(const void* pages, const void* tiles, int n_tiles, const uint8_t* upload, const uint8_t* scratch, const void* runs,
+                             const void* meta, const void* outs, long long batch, const int* tile_valid, int* err, cudaStream_t s);
+
 // line-delimited JSON reader (k_json.cu).
 int json_tile_bytes();
 int json_parse_rows();

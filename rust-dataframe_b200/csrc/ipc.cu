@@ -13,6 +13,7 @@
 // with or without the 0xFFFFFFFF continuation marker).  Checked against pyarrow in tests/test_ipc.py (both directions).
 // Everything here goes through the public C ABI of the library (bdf_upload_many, bdf_download ...).
 #include "../../include/b200df.h"
+#include "ipc_schema.cuh"
 
 #include <fcntl.h>
 #include <sys/mman.h>
@@ -229,6 +230,35 @@ int dtype_bytes(int dtype, int64_t len, int64_t* out) {
 }
 
 }  // namespace
+
+namespace bdf {
+bool arrow_schema_fields(const uint8_t* p, size_t n, std::vector<ArrowField>* out) {
+    if (n < 8) return false;
+    size_t at = 0;
+    int32_t word;
+    memcpy(&word, p, 4);
+    if (word == -1) { at = 4; memcpy(&word, p + 4, 4); }
+    at += 4;
+    if (word <= 0 || (size_t)word > n - at) return false;
+    const FbBuf mb{p + at, (size_t)word};
+    uint32_t root;
+    FbTable msg, schema;
+    if (!mb.rd(0, &root) || !msg.init(&mb, root) || msg.scalar<uint8_t>(1, 0) != 1 || !msg.table(2, &schema)) return false;
+    size_t first; uint32_t cnt;
+    if (!schema.vec(1, &first, &cnt, 4)) return false;
+    int64_t budget = (int64_t)word / 8 + 16;
+    for (uint32_t i = 0; i < cnt; i++) {
+        uint32_t o;
+        FbTable ft;
+        if (!mb.rd(first + 4 * i, &o) || !ft.init(&mb, first + 4 * i + o)) return false;
+        IpcField fld;
+        std::string why;
+        if (!parse_field(ft, &fld, 0, &budget, &why)) return false;
+        out->push_back(ArrowField{fld.name, fld.temporal_kind, fld.temporal_unit, fld.has_tz, fld.tz});
+    }
+    return true;
+}
+}  // namespace bdf
 
 struct bdf_ipc {
     int fd = -1;

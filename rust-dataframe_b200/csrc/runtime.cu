@@ -36,6 +36,8 @@
 #include "comm.cuh"
 #include "moments.cuh"
 #include "json_parse.cuh"
+#define PQ_HOST_PLAN
+#include "parquet_decode.cuh"
 
 using namespace bdf;
 
@@ -4790,6 +4792,122 @@ static int json_read_list(bdf_ctx* c, const bdf_json* f, int col, bdf_list** out
 }
 
 // ---------------------------------------------------------------------------------------------------
+// Parquet reader (parquet.cu reads the footers and page headers and plans the read; k_parquet.cu decodes; the rules are in
+// include/b200df.h): the projected column chunks go to HBM still compressed, through the pageable staging path, with the page and
+// tile tables; four launches over the whole page table decompress, walk the runs, write the validity and write the values straight
+// into the output chunks.  The per-page error words and per-chunk null counts come back in one copy at the end.
+
+static int parquet_read(bdf_ctx* c, const bdf_parquet* f, int n_cols, const int32_t* cols, bdf_col** out) {
+    if (!f || !out || (n_cols > 0 && !cols)) return fail(BDF_INVALID, "null argument");
+    if (n_cols < 0 || n_cols > 65535) return fail(BDF_INVALID, "0..65535 columns");
+    pq::Plan P;
+    TRY(pq::plan(f, n_cols, cols, &P));
+    const int64_t n_chunks = (int64_t)P.chunk_lens.size(), n_out = n_chunks * n_cols;
+    const int n_pages = (int)P.pages.size(), n_tiles = (int)P.tiles.size();
+    std::vector<int32_t> dtypes((size_t)n_cols), nullable((size_t)n_cols);
+    int64_t out_bytes = 0, rows = 0;
+    for (int i = 0; i < n_cols; i++) {
+        TRY(bdf_parquet_column(f, cols[i], nullptr, &dtypes[(size_t)i], &nullable[(size_t)i]));
+        for (int64_t len : P.chunk_lens) out_bytes += (int64_t)align_up(value_bytes(dtypes[(size_t)i], len, 0) + 8, 256) + (nullable[(size_t)i] ? (int64_t)align_up((size_t)len / 8 + 9, 256) : 0);
+    }
+    for (int64_t len : P.chunk_lens) rows += len;
+    const size_t err_bytes = align_up((size_t)std::max(n_pages, 1) * 4, 8);
+    const size_t small_bytes = err_bytes + (size_t)std::max<int64_t>(n_out, 1) * 8;
+    const long double need = (long double)out_bytes + P.upload_bytes + P.scratch_bytes + (long double)P.run_entries * pq_run_bytes() +
+                             (long double)n_pages * (pq_page_bytes() + 16) + (long double)n_tiles * (pq_tile_bytes() + 4) +
+                             (long double)n_out * pq_out_bytes() + small_bytes;
+    if (need * 1.1L > (long double)c->hbm_bytes)
+        return fail(BDF_OOM, "a Parquet read of %.0Lf bytes (compressed chunks, scratch and outputs) does not fit in device memory", need);
+
+    std::vector<ColOwner> res;
+    std::vector<pq::Out> houts((size_t)std::max<int64_t>(n_out, 1));
+    for (int i = 0; i < n_cols; i++) {
+        std::vector<ChunkPlan> plan((size_t)n_chunks);
+        for (int64_t j = 0; j < n_chunks; j++) plan[(size_t)j] = ChunkPlan{P.chunk_lens[(size_t)j], nullable[(size_t)i] != 0};
+        res.emplace_back(c);
+        TRY(col_alloc(c, dtypes[(size_t)i], plan, nullptr, 0, res[(size_t)i].out()));
+        bdf_col* col = res[(size_t)i].get();
+        if (dtypes[(size_t)i] == kBool && col->arena_values) {   // Boolean values are OR-ed in bit by bit
+            size_t vb = 0;
+            for (int64_t len : P.chunk_lens) vb += align_up(value_bytes(kBool, len, 0) + 8, 256);
+            CK(cudaMemsetAsync(col->arena_values, 0, vb, c->s_compute));
+        }
+        for (int64_t j = 0; j < n_chunks; j++)
+            houts[(size_t)(i * n_chunks + j)] = pq::Out{col->chunks[(size_t)j].values, col->chunks[(size_t)j].validity};
+    }
+    Scratch<uint8_t> upload, scratch, small;
+    Scratch<char> pages, tiles, outs, runs, meta;
+    Scratch<int> tile_valid;
+    cudaError_t e = upload.alloc(c, (size_t)std::max<long long>(P.upload_bytes, 16));
+    if (e == cudaSuccess) e = scratch.alloc(c, (size_t)std::max<long long>(P.scratch_bytes, 16));
+    if (e == cudaSuccess) e = runs.alloc(c, (size_t)std::max<long long>(P.run_entries, 1) * pq_run_bytes());
+    if (e == cudaSuccess) e = meta.alloc(c, (size_t)std::max(n_pages, 1) * 16);
+    if (e == cudaSuccess) e = pages.alloc(c, (size_t)std::max(n_pages, 1) * pq_page_bytes());
+    if (e == cudaSuccess) e = tiles.alloc(c, (size_t)std::max(n_tiles, 1) * pq_tile_bytes());
+    if (e == cudaSuccess) e = tile_valid.alloc(c, (size_t)std::max(n_tiles, 1) * 4);
+    if (e == cudaSuccess) e = outs.alloc(c, houts.size() * pq_out_bytes());
+    if (e == cudaSuccess) e = small.alloc(c, small_bytes);
+    if (e == cudaSuccess) e = cudaMemsetAsync(small, 0, small_bytes, c->s_compute);
+    if (e == cudaSuccess && n_pages) e = cudaMemcpyAsync(pages, P.pages.data(), (size_t)n_pages * pq_page_bytes(), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess && n_tiles) e = cudaMemcpyAsync(tiles, P.tiles.data(), (size_t)n_tiles * pq_tile_bytes(), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(outs, houts.data(), houts.size() * pq_out_bytes(), cudaMemcpyHostToDevice, c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "Parquet read allocation");
+    // the compressed chunks: page cache -> pinned staging -> HBM on the copy stream, after the allocations
+    e = cudaEventRecord(c->ev_tmp, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(c->s_h2d, c->ev_tmp, 0);
+    const auto t0 = std::chrono::steady_clock::now();
+    for (size_t s = 0; s < P.segs.size() && e == cudaSuccess; s++)
+        if (P.segs[s].len) e = h2d_copy(c, upload.get() + P.segs[s].dst, P.segs[s].src, (size_t)P.segs[s].len);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_h2d);
+    const double upload_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (e != cudaSuccess) {
+        const int st = fail_cuda(e, "Parquet upload");
+        cudaStreamSynchronize(c->s_h2d);   // no copy may still write into the buffers when they are freed
+        return st;
+    }
+    int* err = (int*)small.get();
+    unsigned long long* nulls = (unsigned long long*)(small.get() + err_bytes);
+    int64_t comp_bytes = 0;
+    for (const auto& sg : P.segs) comp_bytes += sg.len;
+    {
+        LaunchTimer t(c, BDF_K_PARQUET, BDF_U8, n_pages, comp_bytes + P.scratch_bytes);
+        e = launch_pq_snappy(pages, n_pages, upload, scratch, err, c->sm_count, c->s_compute);
+    }
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_PARQUET, BDF_U32, n_pages, P.run_entries * (int64_t)pq_run_bytes());
+        e = launch_pq_runs(pages, n_pages, upload, scratch, runs, meta, err, c->s_compute);
+    }
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_PARQUET, kBool, rows * n_cols, rows * n_cols / 8);
+        e = launch_pq_levels(pages, tiles, n_tiles, upload, scratch, runs, meta, outs, P.batch, tile_valid, nulls, err, c->s_compute);
+    }
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_PARQUET, n_cols == 1 ? dtypes[0] : -1, rows * n_cols, out_bytes);
+        e = launch_pq_values(pages, tiles, n_tiles, upload, scratch, runs, meta, outs, P.batch, tile_valid, err, c->s_compute);
+    }
+    std::vector<char> hs(small_bytes);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hs.data(), small, small_bytes, cudaMemcpyDeviceToHost, c->s_compute);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // the host tables are read by the copies
+    if (e != cudaSuccess) return fail_cuda(e, "Parquet decode");
+    const int* herr = (const int*)hs.data();
+    for (int p = 0; p < n_pages; p++)
+        if (herr[p]) return pq::page_error(f, P, p, herr[p]);
+    const unsigned long long* hn = (const unsigned long long*)(hs.data() + err_bytes);
+    for (int i = 0; i < n_cols; i++) {
+        bdf_col* col = res[(size_t)i].get();
+        for (int64_t j = 0; j < n_chunks; j++) {
+            col->null_counts[(size_t)j] = (int64_t)hn[i * n_chunks + j];
+            if (col->null_counts[(size_t)j] == 0) col->chunks[(size_t)j].validity = nullptr;   // no bitmap in a chunk without nulls
+        }
+        e = finish_single_group(c, col);
+        if (e != cudaSuccess) return fail_cuda(e, "Parquet read");
+    }
+    pq::set_stats(f, n_pages, comp_bytes, upload_ms);
+    for (int i = 0; i < n_cols; i++) out[i] = res[(size_t)i].release();
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // C ABI
 
 #define NEED_CTX(ctx) \
@@ -5604,6 +5722,12 @@ void bdf_json_close(bdf_ctx* c, bdf_json* f) {
     std::lock_guard<std::mutex> lock(c->mu);
     cudaSetDevice(c->device);
     json_free(c, f);
+}
+
+int bdf_parquet_read(bdf_ctx* c, const bdf_parquet* f, int32_t n_cols, const int32_t* cols, bdf_col** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the Parquet reader reads into one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return parquet_read(c, f, n_cols, cols, out);
 }
 
 int bdf_csv_write(bdf_ctx* c, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,

@@ -39,6 +39,7 @@ from .arrays import F32, F64, I8, I64, U8, U32, U64, PrimitiveArray, is_float
 from .functions import Column, _expr_nodes, eval_expr, sort_indices, window as _window
 from .csv_reader import CsvFile, write_csv
 from .json_reader import JsonFile
+from .parquet_reader import ParquetFile
 from .ipc import BOOL, IpcFile, write_ipc
 
 ARITH = {"add": N.ADD, "subtract": N.SUB, "multiply": N.MUL, "divide": N.DIV}
@@ -419,6 +420,17 @@ class DeviceFrame:
         with JsonFile(path, schema=schema, max_records=max_records, batch_size=batch_size, ctx=ctx) as f:
             names = [n for n, dt, _ in f.schema if 0 <= dt <= N.BOOL]
             cols = f.read(names)
+        return cls(OrderedDict((n, cols[n]) for n in names))
+
+    @classmethod
+    def from_parquet(cls, path: str, columns: Optional[Sequence[str]] = None, batch_size: int = 1024,
+                     ctx: Optional[N.Context] = None) -> "DeviceFrame":
+        """DataFrame::from_parquet over a file or a directory of files: the columns on the device path (numeric, Boolean and
+        temporal, the last tagged), or the named ones, one chunk per RecordBatch of batch_size rows.  String, nested and other
+        columns are left out."""
+        with ParquetFile(path, batch_size=batch_size) as f:
+            names = [n for n, dt, _ in f.schema if dt >= 0 and (columns is None or n in columns)]
+            cols = f.read(names, ctx=ctx)
         return cls(OrderedDict((n, cols[n]) for n in names))
 
     @classmethod
