@@ -13,6 +13,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --temporal [--rows 100000000]                    # the date / timestamp function rows
     python benchmarks/kernels_bench.py --ndjson [--csv-rows 50000000]                   # the line-delimited JSON reader rows (a 4.85 GB temporary file)
     python benchmarks/kernels_bench.py --parquet [--csv-rows 50000000]                  # the Parquet reader rows (two temporary files: snappy, none)
+    python benchmarks/kernels_bench.py --parquet-write [--csv-rows 50000000]            # the Parquet writer rows (none/PLAIN, none/dictionary, snappy/dictionary)
 """
 from __future__ import annotations
 
@@ -252,6 +253,84 @@ def parquet_bench(ctx, rows, rows_out, reps=3):
             name = f"parquet[{label}] pyarrow read_table (not the reference), {os.cpu_count()} cores"
             rows_out.append({"case": name, "config": "parquet", "kernel": "host", "ms": ms, "rows": rows, "file_bytes": fbytes})
             print(f"{name:52s} {ms:9.2f} ms  {fbytes / 1e9:6.2f} GB of file", flush=True)
+
+
+def parquet_write_bench(ctx, rows, rows_out, reps=3):
+    """The reader benchmark's table on the device in 2^20-row chunks, written back with bdf_parquet_write three ways (none / PLAIN,
+    none / dictionary, snappy / dictionary): the dictionary step (the sorted_runs kernels and the id scatter), the encode and the snappy
+    steps from the launch records, end to end to /dev/null and to a file; a D2H copy of one column for the link's rate; pyarrow's
+    write_table with the same options on the host for comparison.  Medians of `reps` runs after a warm-up."""
+    import pyarrow as pa
+    import pyarrow.parquet as pq
+
+    names = ["id", "a", "b", "ok", "d", "ts"]
+    with tempfile.TemporaryDirectory() as td:
+        src = os.path.join(td, "src.parquet")
+        write_parquet_table(src, rows, "none")
+        with rdf.ParquetFile(src, batch_size=1 << 20) as f:
+            cols = f.read(names, ctx=ctx)
+        host = pq.read_table(src)
+        os.unlink(src)
+        import torch   # the link's device -> pinned host rate, for the end-to-end rows to be read against
+
+        dev = torch.empty(rows * 8, dtype=torch.uint8, device="cuda")
+        pin = torch.empty(rows * 8, dtype=torch.uint8, pin_memory=True)
+        d2h = []
+        for _ in range(reps + 1):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            pin.copy_(dev)
+            torch.cuda.synchronize()
+            d2h.append((time.perf_counter() - t0) * 1e3)
+        del dev, pin
+        d2h_ms = float(np.median(d2h[1:]))
+        name = f"parquet write: D2H into pinned memory ({rows * 8 / 1e9:.2f} GB)"
+        rows_out.append({"case": name, "config": "parquet-write", "kernel": "d2h", "ms": d2h_ms, "rows": rows, "GBs": rows * 8 / d2h_ms / 1e6})
+        print(f"{name:58s} {d2h_ms:9.2f} ms  {rows * 8 / d2h_ms / 1e6:7.2f} GB/s", flush=True)
+        out = os.path.join(td, "out.parquet")
+        for label, kw in (("none/PLAIN", {"dictionary": False}), ("none/dictionary", {}), ("snappy/dictionary", {"compression": "snappy"})):
+            rdf.write_parquet(out, cols, **kw)
+            fbytes = os.path.getsize(out)
+            res = {"dictionary": [], "encode": [], "snappy": [], "end to end, /dev/null": [], "end to end, file": []}
+            for i in range(reps + 1):
+                for target, key in (("/dev/null", "end to end, /dev/null"), (out, "end to end, file")):
+                    ctx.synchronize()
+                    ctx.profile_read()
+                    ctx.profile_enable(True)
+                    t0 = time.perf_counter()
+                    rdf.write_parquet(target, cols, **kw)
+                    t1 = time.perf_counter()
+                    ctx.profile_enable(False)
+                    recs = ctx.profile_read()
+                    if i == 0:
+                        continue
+                    res[key].append((t1 - t0) * 1e3)
+                    if target == "/dev/null":
+                        pw = [r for r in recs if r["kernel"] == "parquet_write"]
+                        res["encode"].append(sum(r["ms"] for r in pw if r["dtype"] == -1))
+                        res["snappy"].append(sum(r["ms"] for r in pw if r["dtype"] == rdf.U8))
+                        res["dictionary"].append(sum(r["ms"] for r in recs if not (r["kernel"] == "parquet_write" and r["dtype"] in (-1, rdf.U8))))
+            for key, v in res.items():
+                ms = float(np.median(v))
+                if (key == "snappy" and "snappy" not in label) or (key == "dictionary" and "PLAIN" in label):
+                    continue
+                name = f"parquet write [{label}] {key}"
+                rows_out.append({"case": name, "config": "parquet-write", "kernel": "parquet_write", "ms": ms, "rows": rows, "file_bytes": fbytes,
+                                 "Mrows_per_s": rows / ms / 1e3, "GBs_of_file": fbytes / ms / 1e6})
+                print(f"{name:58s} {ms:9.2f} ms  {rows / ms / 1e3:9.1f} Mrows/s  {fbytes / ms / 1e6:7.2f} GB/s of file ({fbytes / 1e9:.2f} GB)",
+                      flush=True)
+            ts = []
+            for _ in range(2):
+                t0 = time.perf_counter()
+                pq.write_table(host, out, compression="snappy" if "snappy" in label else "none", use_dictionary="PLAIN" not in label,
+                               data_page_version="1.0", row_group_size=1 << 20)
+                ts.append((time.perf_counter() - t0) * 1e3)
+            ms = min(ts)
+            name = f"parquet write [{label}] pyarrow write_table (not the reference), {os.cpu_count()} cores"
+            rows_out.append({"case": name, "config": "parquet-write", "kernel": "host", "ms": ms, "rows": rows, "file_bytes": os.path.getsize(out)})
+            print(f"{name:58s} {ms:9.2f} ms  {rows / ms / 1e3:9.1f} Mrows/s", flush=True)
+        for c in cols.values():
+            c.free()
 
 
 def ndjson_bench(ctx, rows, rows_out, reps=3):
@@ -659,8 +738,20 @@ def main():
     ap.add_argument("--temporal", action="store_true", help="run only the date / timestamp function rows")
     ap.add_argument("--ndjson", action="store_true", help="run the line-delimited JSON reader rows (--csv-rows records)")
     ap.add_argument("--parquet", action="store_true", help="run the Parquet reader rows (--csv-rows rows, snappy and uncompressed)")
+    ap.add_argument("--parquet-write", action="store_true", help="run the Parquet writer rows (--csv-rows rows, three encodings)")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.parquet_write:
+        import subprocess
+
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
+        print(f"card: {q.strip()}", flush=True)
+        rows_out = []
+        parquet_write_bench(ctx, args.csv_rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"card": q.strip(), "results": rows_out}, f, indent=1)
+        return
     if args.parquet:
         import subprocess
 

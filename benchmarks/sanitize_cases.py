@@ -139,6 +139,17 @@ for dtype in (rdf.I8, rdf.U16, rdf.I64, rdf.F32, rdf.F64):
         col.download()
     nonempty = rdf.ListColumn.upload([rdf.ListArray.from_pylist(dtype, [[1, None], [None], None, [k % 100 for k in range(70000)]])])
     nonempty.array_max().download(); nonempty.array_min().download()
+# the Parquet writer: ragged and offset chunks, nulls, every encoding path (PLAIN, dictionary, Boolean bits), snappy fragments, row
+# groups cut across chunks, and a frame without rows
+import tempfile
+with tempfile.TemporaryDirectory() as td:
+    pw = {"i8": rdf.Column.upload([P.from_numpy(rng.integers(-100, 100, n + 5).astype(np.int8), rng.random(n + 5) > 0.2).slice(3, n) for n in lens]),
+          "f64": rdf.Column.upload([P.from_numpy(rng.integers(0, 40, n + 5) / 4.0, rng.random(n + 5) > 0.1).slice(1, n) for n in lens]),
+          "u64": rdf.Column.upload([P.from_numpy(rng.integers(0, 2 ** 63, n, dtype=np.uint64)) for n in lens]),
+          "ok": rdf.Column.upload([rdf.BooleanArray.from_numpy(rng.random(n) < 0.5, rng.random(n) > 0.3) for n in lens], dtype=10)}
+    for kw in ({}, {"compression": "snappy"}, {"dictionary": False}, {"row_group_rows": 700, "compression": "snappy"}):
+        rdf.write_parquet(os.path.join(td, "w.parquet"), pw, **kw)
+    rdf.write_parquet(os.path.join(td, "e.parquet"), {"x": rdf.Column.upload([P.from_numpy(np.zeros(0, dtype=np.int32))])})
 # round 2: the fleet code path on one GPU, and a single-rank communicator (pack -> combine -> unpack on the stream)
 fleet = rdf.Context.multi(1)
 fa = [P.from_numpy(rng.integers(-100, 100, n).astype(np.int64), rng.random(n) > 0.3) for n in (1000, 0, 77)]

@@ -874,6 +874,74 @@ int  bdf_parquet_read(bdf_ctx* ctx, const bdf_parquet* file, int32_t n_cols, con
 int  bdf_parquet_stats(const bdf_parquet* file, int64_t* n_pages, int64_t* uploaded_bytes, double* upload_ms);
 void bdf_parquet_close(bdf_parquet* file);
 
+/* ---- Parquet files straight from the device (DataFrame::to_parquet, src/dataframe.rs:545-560) ----------------------------------------
+ * The reference writes with parquet's ArrowWriter, one write(batch) per RecordBatch.  Rules marked RECALLED are recalled from parquet-rs
+ * of that era (WriterProperties defaults, the early ArrowWriter), parity unpinned; the others are this library's decisions.
+ * Defaults (options == NULL, RECALLED).  UNCOMPRESSED, dictionary on, statistics on, writer version 1.0 (DATA_PAGE V1 pages), one row
+ *   group per RecordBatch, which here is one per chunk; an empty chunk is skipped.  Snappy and row_group_rows are options, as
+ *   bdf_csv_write_options are: row_group_rows = N > 0 cuts row groups of N rows across the chunks.
+ * Schema.  Every column is OPTIONAL (maximum definition level 1), as bdf_ipc_write marks every field nullable.  Types are the inverse of
+ *   the reader's table:
+ *     Int8 / Int16 / Int32 -> INT32 INT(8|16|32, signed);  UInt8 / UInt16 / UInt32 -> INT32 INT(8|16|32, unsigned), widened on the device
+ *     Int64 / UInt64 -> INT64 INT(64, signed / unsigned);  Float32 -> FLOAT;  Float64 -> DOUBLE;  Boolean -> BOOLEAN
+ *     Date32 -> INT32 DATE;  Date64 -> INT32 DATE, floor(ms / 86 400 000)
+ *     Time32(s | ms) -> INT32 TIME(MILLIS), seconds x 1000;  Time64(us | ns) -> INT64 TIME(MICROS | NANOS)
+ *     Timestamp(s) -> INT64 TIMESTAMP(MILLIS), x 1000;  Timestamp(ms | us | ns, tz) -> INT64 TIMESTAMP(unit, isAdjustedToUTC = tz != NULL)
+ *   The converted types are written too where the format has them (INT_8 .. UINT_64, DATE, TIME_MILLIS, TIME_MICROS, and
+ *   TIMESTAMP_MILLIS / _MICROS for a Timestamp with a tz: the format defines those as adjusted to UTC).  An ARROW:schema key-value
+ *   entry holds the base64 of the IPC Schema message bdf_ipc_write_typed writes (every Arrow type, tz included).  pyarrow reads such a
+ *   file exactly as it reads its own file of the same table: the time zone, fixed or named, comes back from the entry, while Date64,
+ *   Time32(s) and Timestamp(s) come back in Parquet's units (Date32 days, milliseconds), as for pyarrow's own files.
+ * Pages.  2^17 rows per data page, the last page of a row group fewer; a page never crosses a row group.  Definition levels: a 4-byte
+ *   length, then the RLE / bit-packed hybrid in bit width 1 -- one RLE run for a page without nulls or with only nulls, else one
+ *   bit-packed run copied from the validity bits.  Values: PLAIN (Boolean bit-packed) or dictionary ids.  Page CRCs are not written.
+ * Dictionary (not for Boolean).  A column chunk's dictionary is its distinct values by raw bit pattern (so -0.0 and 0.0, and NaNs with
+ *   different payloads, are separate entries and round-trip bit for bit), in ascending order of the bits read as unsigned integers: a
+ *   decision, parquet-rs uses first-seen order.  Date64 values of one day are separate entries with the same stored date.  RECALLED
+ *   v1.0 encodings: the dictionary page is PLAIN_DICTIONARY and the data pages PLAIN_DICTIONARY ids: one byte of bit width,
+ *   max(1, ceil(log2 entries)), then one bit-packed run per page.  A chunk whose dictionary would exceed 1 MiB (entries x physical width,
+ *   parquet-rs's default limit) is written PLAIN as a whole, without a dictionary page: a departure, parquet-rs falls back part-way
+ *   through a chunk.  So is a chunk without a valid value.
+ * Snappy.  Each page body (levels and values; a dictionary page's values) is one snappy stream, built from independently compressed
+ *   64 KiB fragments, as the format allows.  Every page of a SNAPPY chunk is compressed, even when that makes it larger.
+ * Statistics.  Per column chunk: null_count, min_value, max_value (the deprecated min / max are not written), and column_orders =
+ *   TYPE_DEFINED_ORDER for every column.  Signed or unsigned order as the logical type says, false < true, over the stored physical
+ *   values (after the x 1000 and Date64 conversions).  Floats skip NaN; a zero minimum is written -0.0 and a zero maximum +0.0.  A chunk
+ *   without a valid non-NaN value has no min / max.
+ * File.  "PAR1", per row group and column the dictionary page and the data pages, the Thrift compact-protocol FileMetaData (version 1,
+ *   root schema element and leaves, row groups with total_byte_size and num_rows, created_by "b200df parquet writer", the ARROW:schema
+ *   entry and the column orders), its length, "PAR1".  A frame without rows is a file with zero row groups (RECALLED: what an
+ *   ArrowWriter closed without a write leaves); pyarrow reads it as an empty table, and bdf_parquet_open gives BDF_WOULD_PANIC for it,
+ *   as the reference's from_parquet would (schema.unwrap()).  The same frame and options give the same bytes, call after call.
+ * Input.  As bdf_csv_write: chunk b of every column has the same length, else BDF_LENGTH_MISMATCH.  The ten numeric types and Boolean;
+ *   types[j] (NULL: none) tags Int32 / Int64 columns as Date, Time or Timestamp (kind 0: none).  A tag is checked as
+ *   bdf_ipc_write_typed checks it (bdf_temporal_result's validation of kind and unit, then the physical dtype): a bad tag, or a column
+ *   that cannot hold it (a Boolean column included) -> BDF_INVALID.  Any other column type -> BDF_UNSUPPORTED.  At most 2^32 - 1 rows
+ *   and at most 2^20 column chunks (row groups x columns) per file, else BDF_INVALID.
+ * Memory.  The pages go in blocks of consecutive pages, in file order, through two fixed 64 MiB device buffers (and an 80 MiB fragment
+ *   buffer for snappy); the context's pinned staging slots (shared with uploads) carry headers and bodies to the file, written with
+ *   pwrite by the staging threads.  Neither grows with the file.  What does, beside the frame itself:
+ *     - the page and tile tables: about 40 B per 2048 rows and column, on the device and the host;
+ *     - while the dictionary of one column is found (one column at a time): one sort of that column and its sorted copies
+ *       (sorted_runs, as group-by) and the row-group ids, about 50 B per row for an 8-byte column, plus 4 B of id per row;
+ *     - kept until the write ends, for each chunk written with a dictionary: 4 B of id per row of the chunk and its entries (at most
+ *       1 MiB).  A column whose chunks all fall back to PLAIN keeps nothing.
+ * Errors (nothing leaks): a null pointer, n_cols <= 0, compression not 0 / 1, dictionary not 0 / 1 or row_group_rows < 0 ->
+ *   BDF_INVALID; a multi-GPU context -> BDF_UNSUPPORTED; BDF_OOM before the file is created.  Every refusal above happens before the
+ *   file is created, so an existing file at the path is left as it was.  The file is written in place, as the CSV writer writes (no
+ *   temporary file and rename: writing to /dev/null stays possible); a path that cannot be created or written -> BDF_INVALID with the
+ *   OS text, and a failed call leaves a file without its trailing magic, which every reader rejects.
+ * Launch records (BDF_K_PARQUET_WRITE): dtype BDF_U32 for the dictionary steps, -1 for the encode of a block (count, layout, encode),
+ *   BDF_U8 for its snappy fragments and compaction. */
+typedef struct {
+    int32_t compression;      /* 0 UNCOMPRESSED, 1 SNAPPY */
+    int32_t dictionary;       /* 0 off, 1 on */
+    int64_t row_group_rows;   /* 0: one row group per chunk; N > 0: N rows per row group, cut across chunks */
+} bdf_parquet_write_options;
+int  bdf_parquet_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
+                       const bdf_temporal_type* types /* n_cols entries or NULL, as bdf_ipc_write_typed */,
+                       const bdf_parquet_write_options* options /* NULL: the defaults above */);
+
 /* ---- measurement support ------------------------------------------------------------------------ */
 /* Per-launch CUDA-event timing on the library's compute stream (the stream the kernels run on). */
 typedef struct {
@@ -883,7 +951,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL, BDF_K_JSON, BDF_K_PARQUET } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL, BDF_K_JSON, BDF_K_PARQUET, BDF_K_PARQUET_WRITE } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

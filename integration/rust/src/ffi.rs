@@ -39,6 +39,9 @@ pub struct BdfParquetOptions { pub batch_size: i64 }
 #[repr(C)]
 #[derive(Clone, Copy)]
 pub struct BdfCsvWriteOptions { pub has_header: i32, pub delimiter: u8 }
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct BdfParquetWriteOptions { pub compression: i32, pub dictionary: i32, pub row_group_rows: i64 }
 
 #[repr(C)]
 pub struct BdfListView { pub offsets: *const i32, pub validity: *const u8, pub len: i64, pub offset: i64, pub null_count: i64, pub values: BdfView }
@@ -257,6 +260,10 @@ extern "C" {
     pub fn bdf_parquet_read(ctx: *mut BdfCtx, file: *const BdfParquet, n_cols: i32, cols: *const i32, out: *mut *mut BdfCol) -> c_int;
     pub fn bdf_parquet_stats(file: *const BdfParquet, n_pages: *mut i64, uploaded_bytes: *mut i64, upload_ms: *mut f64) -> c_int;
     pub fn bdf_parquet_close(file: *mut BdfParquet);
+    // Parquet files straight from the device (DataFrame::to_parquet): types NULL or one per column (kind 0: none); options NULL: the
+    // defaults (uncompressed, dictionary on, one row group per chunk)
+    pub fn bdf_parquet_write(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol,
+                             types: *const BdfTemporalType, options: *const BdfParquetWriteOptions) -> c_int;
 }
 
 /// bdf_temporal_type: kind (0 none, 1 Date32, 2 Date64, 3 Timestamp, 4 Time32, 5 Time64), unit (arrow TimeUnit order), tz (Timestamp).

@@ -245,6 +245,22 @@ pub fn to_csv_device(frame: &DeviceColumns, path: &str, options: Option<(bool, u
     check(unsafe { bdf_csv_write(dev(), c_path.as_ptr(), cols.len() as i32, name_ptrs.as_ptr(), cols.as_ptr(), p) })
 }
 
+/// DataFrame::to_parquet on the device: every column's pages encoded (and snappy-compressed) on the GPU and streamed to the file.
+/// `types`: one per column (kind 0 for a plain column) or None; `options`: None for the defaults.
+pub fn to_parquet_device(frame: &DeviceColumns, path: &str, types: Option<&[BdfTemporalType]>,
+                         options: Option<BdfParquetWriteOptions>) -> Result<(), String> {
+    let c_path = CString::new(path).map_err(|e| e.to_string())?;
+    let names: Vec<CString> = frame.names.iter().map(|n| CString::new(n.as_str())).collect::<Result<_, _>>().map_err(|e| e.to_string())?;
+    let name_ptrs: Vec<*const c_char> = names.iter().map(|n| n.as_ptr()).collect();
+    let cols: Vec<*const BdfCol> = frame.cols.iter().map(|c| *c as *const BdfCol).collect();
+    if let Some(t) = types {
+        if t.len() != cols.len() { return Err("one temporal type per column".to_string()); }
+    }
+    let t = types.map_or(std::ptr::null(), |t| t.as_ptr());
+    let p = options.as_ref().map_or(std::ptr::null(), |o| o as *const BdfParquetWriteOptions);
+    check(unsafe { bdf_parquet_write(dev(), c_path.as_ptr(), cols.len() as i32, name_ptrs.as_ptr(), cols.as_ptr(), t, p) })
+}
+
 /// A run of Float64 Calculations whose intermediates are not kept (config 2: h = sin(((a+b)*c)/d)) as one pass.
 /// `inputs` are column indices; node k writes slot inputs.len() + k (see include/b200df.h, bdf_eval_expr_dev).
 pub fn fused_chain(frame: &DeviceColumns, inputs: &[usize], nodes: &[BdfExprNode]) -> Result<*mut BdfCol, String> {

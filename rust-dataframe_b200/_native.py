@@ -23,7 +23,7 @@ ASYNC = 1
 (K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW,
  K_MOMENTS, K_CSV_WRITE, K_LIST, K_TEMPORAL, K_JSON, K_PARQUET) = range(21)
 KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
-                "window", "moments", "csv_write", "list", "temporal", "json", "parquet"]
+                "window", "moments", "csv_write", "list", "temporal", "json", "parquet", "parquet_write"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -135,6 +135,10 @@ class JsonOptions(C.Structure):
 
 class ParquetOptions(C.Structure):
     _fields_ = [("batch_size", C.c_int64)]
+
+
+class ParquetWriteOptions(C.Structure):
+    _fields_ = [("compression", C.c_int32), ("dictionary", C.c_int32), ("row_group_rows", C.c_int64)]
 
 
 class CsvOptions(C.Structure):
@@ -296,6 +300,7 @@ def lib() -> C.CDLL:
         "bdf_parquet_read": ([vp, vp, i32, P(i32), P(vp)], C.c_int),
         "bdf_parquet_stats": ([vp, P(i64), P(i64), P(C.c_double)], C.c_int),
         "bdf_parquet_close": ([vp], None),
+        "bdf_parquet_write": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(TemporalTypeC), P(ParquetWriteOptions)], C.c_int),
         "bdf_generate": ([vp, C.c_int, C.c_int, C.c_double, C.c_double, u64, u64, i64, P(i64), i64, C.c_uint32, P(vp)],
                          C.c_int),
         "bdf_list_upload": ([vp, C.c_int, i64, P(ListView), C.c_int, P(vp)], C.c_int),
@@ -350,7 +355,7 @@ EXPORTED_SYMBOLS = [
     "bdf_temporal", "bdf_temporal_dev", "bdf_temporal_binary_dev", "bdf_temporal_result", "bdf_ipc_temporal_column", "bdf_ipc_read_temporal",
     "bdf_ipc_write_typed",
     "bdf_parquet_open", "bdf_parquet_describe", "bdf_parquet_column", "bdf_parquet_temporal_column", "bdf_parquet_check", "bdf_parquet_read",
-    "bdf_parquet_stats", "bdf_parquet_close",
+    "bdf_parquet_stats", "bdf_parquet_close", "bdf_parquet_write",
 ]
 
 

@@ -493,6 +493,18 @@ cudaError_t launch_csvw_measure(const CsvwDesc* cols, const long long* chunk_sta
 cudaError_t launch_csvw_emit(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows, int delim,
                              const unsigned long long* offs, char* out, cudaStream_t s);
 
+// Parquet writer (k_parquet_write.cu; the page, tile and page-result records are parquet_encode.cuh's pq::WPage, WTile and WPageOut).
+size_t pqw_page_bytes();
+size_t pqw_tile_bytes();
+size_t pqw_out_bytes();
+cudaError_t launch_pqw_rgid(const long long* rg_start, int n_rg, long long n, uint32_t* out, int sm_count, cudaStream_t s);
+cudaError_t launch_pqw_dict(const uint32_t* run_rg, const uint32_t* run_valid, long long n_runs, const uint32_t* head, const unsigned long long* prefix,
+                            const uint32_t* perm, long long n, unsigned int* count, unsigned int* first, uint32_t* ids, int sm_count, cudaStream_t s);
+cudaError_t launch_pqw_encode(const void* pages, int n_pages, const void* tiles, int n_tiles, unsigned int* tile_valid, unsigned int* tile_base, void* lay,
+                              uint8_t* raw, void* out, cudaStream_t s);
+cudaError_t launch_pqw_snappy(const void* pages, const int* frag_page, int n_frags, uint8_t* raw, void* out, uint8_t* frag, unsigned int* frag_len,
+                              cudaStream_t s);
+
 // List columns (k_list.cu).
 size_t list_find_scratch_bytes(long long n_elem);
 cudaError_t launch_list_find(int dtype, const int32_t* off, const uint32_t* lvalid, long long len, long long n_elem, const void* values,

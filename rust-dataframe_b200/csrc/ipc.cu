@@ -673,21 +673,26 @@ void frame_message(FilePlan* plan, int64_t* pos, const FbOut& fb, int32_t* meta_
     *pos = after;
 }
 
+// The Schema message flatbuffer (before framing).
+FbOut schema_message(int n_cols, const char* const* names, const int32_t* dtypes, const bdf_temporal_type* types) {
+    FbOut fb;
+    fb.put<uint32_t>(0);
+    std::vector<size_t> refs;
+    const size_t msg = fb_table(fb, {{0, 2, 4 /* MetadataVersion::V5 */}, {1, 1, 1 /* Schema */}, {2, 0, 0}, {3, 8, 0}}, &refs);
+    fb.link(0, msg);
+    fb.link(refs[0], fb_schema(fb, n_cols, names, dtypes, types));
+    fb.pad_to(8);
+    return fb;
+}
+
 void plan_file(int n_cols, const char* const* names, const int32_t* dtypes, const bdf_temporal_type* types, int64_t n_batches,
                std::vector<std::vector<ChunkSpec>>& spec, FilePlan* plan) {
     int64_t pos = 0;
     plan->meta.push_back({0, {'A', 'R', 'R', 'O', 'W', '1', 0, 0}});
     pos = 8;
     {   // schema message
-        FbOut fb;
-        fb.put<uint32_t>(0);
-        std::vector<size_t> refs;
-        const size_t msg = fb_table(fb, {{0, 2, 4 /* MetadataVersion::V5 */}, {1, 1, 1 /* Schema */}, {2, 0, 0}, {3, 8, 0}}, &refs);
-        fb.link(0, msg);
-        fb.link(refs[0], fb_schema(fb, n_cols, names, dtypes, types));
-        fb.pad_to(8);
         int32_t ml;
-        frame_message(plan, &pos, fb, &ml);
+        frame_message(plan, &pos, schema_message(n_cols, names, dtypes, types), &ml);
     }
     std::vector<Block> blocks;
     for (int64_t b = 0; b < n_batches; b++) {
@@ -788,6 +793,19 @@ struct OutFile {
 };
 
 }  // namespace
+
+namespace bdf {
+std::string arrow_schema_message(int n_cols, const char* const* names, const int32_t* dtypes, const bdf_temporal_type* types) {
+    FilePlan plan;
+    int64_t pos = 0;
+    int32_t ml;
+    frame_message(&plan, &pos, schema_message(n_cols, names, dtypes, types), &ml);
+    const std::vector<uint8_t>& b = plan.meta[0].bytes;
+    std::string s(b.begin(), b.end());
+    s.resize((size_t)pos, '\0');   // the framing pads the message to a multiple of 64 bytes
+    return s;
+}
+}  // namespace bdf
 
 #pragma GCC visibility push(default)
 extern "C" {

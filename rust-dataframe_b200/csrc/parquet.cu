@@ -1,6 +1,7 @@
 // parquet.cu -- the host half of the Parquet reader: files and directories, the Thrift compact-protocol footer, the column types,
 // and the page-header walk of every on-path column chunk; bdf_parquet_open / _describe / _column / _temporal_column / _check /
 // _stats / _close, and the read plan runtime.cu's bdf_parquet_read uploads and decodes (k_parquet.cu).  No GPU is needed here.
+// At the end, the writer's half: the page headers and the footer bdf_parquet_write (runtime.cu) serialises.
 // The rules are in include/b200df.h ("Parquet files straight to the device").
 #include <algorithm>
 #include <cerrno>
@@ -19,6 +20,8 @@
 #include "../../include/b200df.h"
 #define PQ_HOST_PLAN
 #include "parquet_decode.cuh"
+#define PQ_HOST_WRITE
+#include "parquet_encode.cuh"
 
 #include "ipc_schema.cuh"
 
@@ -816,4 +819,172 @@ void set_stats(const bdf_parquet* f, long long n_pages, long long uploaded, doub
     f->uploaded = uploaded;
     f->upload_ms = upload_ms;
 }
+}  // namespace pq
+
+// ---- the writer's footer and page headers (Thrift compact protocol; runtime.cu's bdf_parquet_write) ------------------------------------
+namespace {
+
+struct ThriftOut {
+    std::string b;
+    std::vector<int16_t> stack;
+    int16_t last = 0;
+    void varint(uint64_t v) {
+        while (v >= 0x80) { b.push_back((char)(v | 0x80)); v >>= 7; }
+        b.push_back((char)v);
+    }
+    static uint64_t zz(int64_t v) { return ((uint64_t)v << 1) ^ (uint64_t)(v >> 63); }
+    void field(int16_t id, int type) {
+        const int d = id - last;
+        if (d > 0 && d <= 15) b.push_back((char)((d << 4) | type));
+        else { b.push_back((char)type); varint(zz(id)); }
+        last = id;
+    }
+    void i32(int16_t id, int32_t v) { field(id, TC_I32); varint(zz(v)); }
+    void i64(int16_t id, int64_t v) { field(id, TC_I64); varint(zz(v)); }
+    void binary(int16_t id, const std::string& s) { field(id, TC_BINARY); varint(s.size()); b += s; }
+    void boolean(int16_t id, bool v) { field(id, v ? TC_TRUE : TC_FALSE); }
+    void byte(int16_t id, int8_t v) { field(id, TC_BYTE); b.push_back((char)v); }
+    void begin(int16_t id) { field(id, TC_STRUCT); elem(); }
+    void elem() { stack.push_back(last); last = 0; }   // a struct that is a list element
+    void end() { b.push_back(0); last = stack.back(); stack.pop_back(); }
+    void list(int16_t id, int type, uint32_t n) {
+        field(id, TC_LIST);
+        if (n < 15) b.push_back((char)((n << 4) | type));
+        else { b.push_back((char)(0xf0 | type)); varint(n); }
+    }
+};
+
+}  // namespace
+
+namespace pq {
+
+std::string page_header(int kind, int raw_len, int comp_len, int num_values, int encoding) {
+    ThriftOut t;
+    t.elem();
+    t.i32(1, kind == KIND_DICT ? 2 : 0);
+    t.i32(2, raw_len);
+    t.i32(3, comp_len);
+    if (kind == KIND_DICT) {
+        t.begin(7);
+        t.i32(1, num_values);
+        t.i32(2, encoding);
+        t.end();
+    } else {
+        t.begin(5);
+        t.i32(1, num_values);
+        t.i32(2, encoding);
+        t.i32(3, ENC_RLE);
+        t.i32(4, ENC_RLE);
+        t.end();
+    }
+    t.end();
+    return t.b;
+}
+
+std::string file_metadata(const std::vector<WColumn>& cols, const std::vector<long long>& rg_rows, const std::vector<std::vector<WChunkMeta>>& chunks,
+                          const std::string& arrow_schema_b64) {
+    ThriftOut t;
+    t.elem();
+    t.i32(1, 1);
+    t.list(2, TC_STRUCT, (uint32_t)cols.size() + 1);
+    t.elem();
+    t.binary(4, "schema");
+    t.i32(5, (int32_t)cols.size());
+    t.end();
+    for (const WColumn& c : cols) {
+        t.elem();
+        t.i32(1, c.phys);
+        t.i32(3, 1);   // OPTIONAL
+        t.binary(4, c.name);
+        if (c.converted >= 0) t.i32(6, c.converted);
+        if (c.logical) {
+            t.begin(10);
+            t.begin((int16_t)c.logical);
+            if (c.logical == 10) { t.byte(1, (int8_t)c.int_bits); t.boolean(2, c.int_signed != 0); }
+            if (c.logical == 7 || c.logical == 8) {
+                t.boolean(1, c.utc);
+                t.begin(2);
+                t.begin((int16_t)c.time_unit);
+                t.end();
+                t.end();
+            }
+            t.end();
+            t.end();
+        }
+        t.end();
+    }
+    long long rows = 0;
+    for (long long r : rg_rows) rows += r;
+    t.i64(3, rows);
+    t.list(4, TC_STRUCT, (uint32_t)rg_rows.size());
+    for (size_t g = 0; g < rg_rows.size(); g++) {
+        t.elem();
+        t.list(1, TC_STRUCT, (uint32_t)cols.size());
+        long long bytes = 0;
+        for (size_t k = 0; k < cols.size(); k++) {
+            const WChunkMeta& m = chunks[g][k];
+            bytes += m.total_uncompressed;
+            t.elem();
+            t.i64(2, m.dict_page_offset >= 0 ? m.dict_page_offset : m.data_page_offset);
+            t.begin(3);
+            t.i32(1, m.phys);
+            t.list(2, TC_I32, (uint32_t)m.encodings.size());
+            for (int e : m.encodings) t.varint(ThriftOut::zz(e));
+            t.list(3, TC_BINARY, 1);
+            t.varint(cols[k].name.size());
+            t.b += cols[k].name;
+            t.i32(4, m.codec);
+            t.i64(5, m.num_values);
+            t.i64(6, m.total_uncompressed);
+            t.i64(7, m.total_compressed);
+            t.i64(9, m.data_page_offset);
+            if (m.dict_page_offset >= 0) t.i64(11, m.dict_page_offset);
+            if (m.has_stats) {
+                t.begin(12);
+                t.i64(3, m.null_count);
+                if (m.has_minmax) { t.binary(5, m.max_value); t.binary(6, m.min_value); }
+                t.end();
+            }
+            t.end();
+            t.end();
+        }
+        t.i64(2, bytes);
+        t.i64(3, rg_rows[g]);
+        t.end();
+    }
+    t.list(5, TC_STRUCT, 1);
+    t.elem();
+    t.binary(1, "ARROW:schema");
+    t.binary(2, arrow_schema_b64);
+    t.end();
+    t.binary(6, "b200df parquet writer");
+    t.list(7, TC_STRUCT, (uint32_t)cols.size());
+    for (size_t k = 0; k < cols.size(); k++) {
+        t.elem();
+        t.begin(1);   // TYPE_ORDER: TypeDefinedOrder
+        t.end();
+        t.end();
+    }
+    t.end();
+    return t.b;
+}
+
+std::string base64(const std::string& s) {
+    static const char* a = "ABCDEFGHIJKLMNOPQRSTUVWXYZabcdefghijklmnopqrstuvwxyz0123456789+/";
+    std::string o;
+    size_t i = 0;
+    for (; i + 2 < s.size(); i += 3) {
+        const uint32_t v = (uint8_t)s[i] << 16 | (uint8_t)s[i + 1] << 8 | (uint8_t)s[i + 2];
+        o += a[v >> 18]; o += a[(v >> 12) & 63]; o += a[(v >> 6) & 63]; o += a[v & 63];
+    }
+    if (i + 1 == s.size()) {
+        const uint32_t v = (uint8_t)s[i] << 16;
+        o += a[v >> 18]; o += a[(v >> 12) & 63]; o += "==";
+    } else if (i + 2 == s.size()) {
+        const uint32_t v = (uint8_t)s[i] << 16 | (uint8_t)s[i + 1] << 8;
+        o += a[v >> 18]; o += a[(v >> 12) & 63]; o += a[(v >> 6) & 63]; o += '=';
+    }
+    return o;
+}
+
 }  // namespace pq

@@ -38,6 +38,9 @@
 #include "json_parse.cuh"
 #define PQ_HOST_PLAN
 #include "parquet_decode.cuh"
+#define PQ_HOST_WRITE
+#include "parquet_encode.cuh"
+#include "ipc_schema.cuh"
 
 using namespace bdf;
 
@@ -3242,6 +3245,530 @@ static int csv_write(bdf_ctx* c, const char* path, int n_cols, const char* const
 }
 
 // ---------------------------------------------------------------------------------------------------
+// Parquet writer (k_parquet_write.cu; DataFrame::to_parquet, src/dataframe.rs:545-560; the rules are in include/b200df.h).  The
+// dictionary of every column is found first (sorted_runs over (row group, value bits): a fixed number of launches per column).  Then
+// the pages go in blocks of consecutive pages in file order, as the CSV writer's text does: while block k is encoded (and
+// compressed) into one of two fixed device buffers, block k-1's page results come back in one small copy, the host serialises its
+// page headers, and the headers and bodies cross to the file through the pinned staging slots, pwrite by the CopyPool threads.
+
+static constexpr int64_t kPqwPageRows = (int64_t)1 << 17;
+static constexpr size_t kPqwRaw = (size_t)64 << 20;     // bytes of each of the two page-body buffers
+static constexpr size_t kPqwFrag = (size_t)80 << 20;    // bytes of the snappy fragment buffer
+static constexpr int64_t kPqwDictLimit = (int64_t)1 << 20;
+static constexpr int64_t kPqwMaxChunks = (int64_t)1 << 20;   // column chunks (row groups x columns) per file: the host's per-chunk tables
+
+namespace {
+struct PqwCol {
+    int dtype = 0, phys = 0, width = 0, in_width = 0, conv = pq::CONV_NONE, ord = pq::ORD_SIGNED;
+    pq::WColumn meta;
+    // per row group, for a column with a dictionary: whether the chunk keeps it, its entries, their first index in the kept
+    // entries, and the index in the kept ids of the row group's first row
+    std::vector<char> keep;
+    std::vector<unsigned int> dcount;
+    std::vector<int64_t> dfirst, id0;
+};
+}  // namespace
+
+// The Parquet type of a column (b200df.h's table).
+static int pqw_type(const bdf_col* col, const bdf_temporal_type* tt, const char* name, PqwCol* o) {
+    const int dt = col->dtype;
+    o->dtype = dt;
+    o->meta.name = name;
+    pq::WColumn& m = o->meta;
+    const bool tagged = tt && tt->kind;
+    if (tagged) {   // the tag is checked as bdf_ipc_write_typed checks it: the temporal functions' validation, then the physical dtype
+        int32_t rd = 0;
+        int st = bdf_temporal_result(BDF_TEMPORAL_UNIX_TIMESTAMP, tt, 0, &rd, nullptr);
+        if (st == BDF_UNSUPPORTED) st = bdf_temporal_result(BDF_TEMPORAL_HOUR, tt, 0, &rd, nullptr);   // time kinds
+        if (st != BDF_OK) return st;
+        const int phys = (tt->kind == BDF_DATE32 || tt->kind == BDF_TIME32) ? BDF_I32 : BDF_I64;
+        if (dt != phys) return fail(BDF_INVALID, "column '%s' of dtype %d does not hold temporal kind %d", name, dt, tt->kind);
+    }
+    if (dt == kBool) { o->phys = pq::PHYS_BOOLEAN; o->width = 0; o->in_width = 0; o->ord = pq::ORD_UNSIGNED; return BDF_OK; }
+    if (dt < 0 || dt >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "column '%s': dtype %d is not written to Parquet", name, dt);
+    o->in_width = dtype_width(dt);
+    if (dt == BDF_F32 || dt == BDF_F64) {
+        o->phys = dt == BDF_F32 ? pq::PHYS_FLOAT : pq::PHYS_DOUBLE;
+        o->width = o->in_width;
+        o->ord = dt == BDF_F32 ? pq::ORD_FLOAT : pq::ORD_DOUBLE;
+    } else {
+        const bool sg = dtype_is_signed_int(dt);
+        const int bits = 8 * o->in_width;
+        o->phys = bits == 64 ? pq::PHYS_INT64 : pq::PHYS_INT32;
+        o->width = bits == 64 ? 8 : 4;
+        o->conv = sg && bits < 32 ? pq::CONV_SEXT : pq::CONV_NONE;
+        o->ord = sg ? pq::ORD_SIGNED : pq::ORD_UNSIGNED;
+        m.logical = 10; m.int_bits = bits; m.int_signed = sg ? 1 : 0;
+        static const int conv_sg[4] = {15, 16, 17, 18}, conv_us[4] = {11, 12, 13, 14};   // INT_8 .. INT_64, UINT_8 .. UINT_64
+        const int k = bits == 8 ? 0 : bits == 16 ? 1 : bits == 32 ? 2 : 3;
+        m.converted = sg ? conv_sg[k] : conv_us[k];
+    }
+    m.phys = o->phys;
+    if (!tagged) return BDF_OK;
+    const int kind = tt->kind, unit = tt->unit;
+    o->ord = pq::ORD_SIGNED;
+    o->conv = pq::CONV_NONE;
+    m.int_bits = 0;
+    switch (kind) {
+        case BDF_DATE32: case BDF_DATE64:
+            o->phys = pq::PHYS_INT32; o->width = 4; m.logical = 6; m.converted = 6;
+            if (kind == BDF_DATE64) o->conv = pq::CONV_DAYS;
+            break;
+        case BDF_TIME32:
+            o->phys = pq::PHYS_INT32; o->width = 4; m.logical = 7; m.converted = 7; m.time_unit = 1; m.utc = true;
+            if (unit == BDF_SECOND) o->conv = pq::CONV_MUL1000;
+            break;
+        case BDF_TIME64:
+            o->phys = pq::PHYS_INT64; o->width = 8; m.logical = 7; m.time_unit = unit; m.utc = true;
+            m.converted = unit == BDF_MICROSECOND ? 8 : -1;
+            break;
+        default:   // BDF_TIMESTAMP
+            o->phys = pq::PHYS_INT64; o->width = 8; m.logical = 8; m.utc = tt->tz != nullptr;
+            m.time_unit = unit == BDF_SECOND ? 1 : unit;
+            if (unit == BDF_SECOND) o->conv = pq::CONV_MUL1000;
+            m.converted = m.utc && m.time_unit == 1 ? 9 : m.utc && m.time_unit == 2 ? 10 : -1;   // TIMESTAMP_MILLIS / _MICROS mean UTC
+            break;
+    }
+    m.phys = o->phys;
+    return BDF_OK;
+}
+
+// Device-to-device copies of the ranges [from, from + len) of src to consecutive places of dst (elements of `w` bytes).
+static cudaError_t pqw_gather(bdf_ctx* c, const char* src, char* dst, const std::vector<std::pair<int64_t, int64_t>>& ranges, int w) {
+    int64_t at = 0;
+    for (const auto& r : ranges) {
+        cudaError_t e = cudaMemcpyAsync(dst + at * w, src + r.first * w, (size_t)(r.second * w), cudaMemcpyDeviceToDevice, c->s_compute);
+        if (e != cudaSuccess) return e;
+        at += r.second;
+    }
+    return cudaSuccess;
+}
+
+// The dictionary of every row group of one column.  Found over the whole column: ids (one per row, its entry in its row group's
+// dictionary) and the distinct values (every row group's valid runs, ascending bits).  Kept: only what the chunks that keep a
+// dictionary read -- their rows' ids and their entries (at most kPqwDictLimit bytes each) -- in *ids and *dvals; both stay empty when
+// no chunk keeps one.
+static int pqw_dictionary(bdf_ctx* c, const bdf_col* col, const bdf_col* rg_col, const std::vector<int64_t>& rg_start, PqwCol* pc, ColOwner* ids,
+                          ColOwner* dvals) {
+    const int64_t n = col->total_len;
+    const int n_rg = (int)rg_start.size() - 1;
+    static const int as_unsigned[4] = {BDF_U8, BDF_U16, BDF_U32, BDF_U64};
+    const int w = dtype_width(col->dtype);
+    ColOwner view(c);
+    {
+        bdf_col* v = new (std::nothrow) bdf_col();   // the column's chunks read as unsigned integers of its width: no arenas of its own
+        if (!v) return fail(BDF_OOM, "host allocation failed");
+        v->dtype = as_unsigned[w == 1 ? 0 : w == 2 ? 1 : w == 4 ? 2 : 3];
+        v->total_len = n;
+        v->chunks = col->chunks;
+        v->null_counts = col->null_counts;
+        *view.out() = v;
+    }
+    wait_groups(c->s_compute, col, 0, (int64_t)col->chunks.size());
+    const bdf_col* keys[2] = {rg_col, view.get()};
+    ColOwner all_ids(c);
+    std::vector<unsigned int> first((size_t)n_rg, 0);
+    pc->dcount.assign((size_t)n_rg, 0);
+    SortedRuns r(c);
+    TRY(sorted_runs(c, 2, keys, "Parquet dictionary iota", &r));
+    {
+        TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, all_ids.out()));
+        const int64_t words = (n + 31) / 32;
+        const int64_t blocks = (words + window_count_tile() - 1) / window_count_tile();
+        Scratch<unsigned int> cf;
+        Scratch<unsigned long long> prefix, block_sums;
+        cudaError_t e = cf.alloc(c, (size_t)2 * n_rg * sizeof(unsigned int));
+        if (e == cudaSuccess) e = prefix.alloc(c, (size_t)(words + 1) * sizeof(unsigned long long));
+        if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long));
+        if (e == cudaSuccess) e = cudaMemsetAsync(cf, 0, (size_t)n_rg * sizeof(unsigned int), c->s_compute);
+        if (e == cudaSuccess) e = cudaMemsetAsync(cf + n_rg, 0xff, (size_t)n_rg * sizeof(unsigned int), c->s_compute);
+        const int64_t n_runs = r.n_runs;
+        const uint32_t* head = (const uint32_t*)r.head->chunks[0].values;
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_PARQUET_WRITE, BDF_U32, n, words * (4 + 8 + 16) + n * 16 + n_runs * 8);   // head prefix; perm, ids; runs
+            c->launches += 4;                                                                                // count, scan (2), runs, ids
+            e = launch_window_count(head, words, prefix, block_sums, c->s_compute);
+            if (e == cudaSuccess) e = launch_join_scan(prefix, words, block_sums, c->s_compute);
+            if (e == cudaSuccess)
+                e = launch_pqw_dict((const uint32_t*)r.distinct[0]->chunks[0].values, r.distinct[1]->chunks[0].validity, n_runs, head, prefix,
+                                    (const uint32_t*)r.perm->chunks[0].values, n, cf, cf + n_rg, (uint32_t*)all_ids->chunks[0].values, c->sm_count,
+                                    c->s_compute);
+        }
+        if (e == cudaSuccess) e = cudaMemcpyAsync(pc->dcount.data(), cf, (size_t)n_rg * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(first.data(), cf + n_rg, (size_t)n_rg * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->s_compute);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);
+        if (e != cudaSuccess) return fail_cuda(e, "Parquet dictionary");
+    }
+    // which chunks keep a dictionary, and the ranges of ids and entries they read (adjacent row groups merged)
+    pc->keep.assign((size_t)n_rg, 0);
+    pc->dfirst.assign((size_t)n_rg, 0);
+    pc->id0.assign((size_t)n_rg, 0);
+    std::vector<std::pair<int64_t, int64_t>> id_ranges, entry_ranges;
+    int64_t kept_ids = 0, kept_entries = 0;
+    for (int g = 0; g < n_rg; g++) {
+        const int64_t cnt = pc->dcount[(size_t)g];
+        if (cnt == 0 || cnt * pc->width > kPqwDictLimit) continue;   // the limit counts physical bytes
+        pc->keep[(size_t)g] = 1;
+        const int64_t rows = rg_start[g + 1] - rg_start[g];
+        pc->id0[(size_t)g] = kept_ids;
+        pc->dfirst[(size_t)g] = kept_entries;
+        if (!id_ranges.empty() && id_ranges.back().first + id_ranges.back().second == rg_start[g]) id_ranges.back().second += rows;
+        else id_ranges.push_back({rg_start[g], rows});
+        if (!entry_ranges.empty() && entry_ranges.back().first + entry_ranges.back().second == (int64_t)first[(size_t)g]) entry_ranges.back().second += cnt;
+        else entry_ranges.push_back({(int64_t)first[(size_t)g], cnt});
+        kept_ids += rows;
+        kept_entries += cnt;
+    }
+    if (kept_ids == 0) return BDF_OK;   // every chunk is written PLAIN: nothing is kept
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{kept_ids, false}}, nullptr, 0, ids->out()));
+    TRY(col_alloc(c, view->dtype, {ChunkPlan{kept_entries, false}}, nullptr, 0, dvals->out()));
+    cudaError_t e = pqw_gather(c, all_ids->chunks[0].values, (*ids)->chunks[0].values, id_ranges, 4);
+    if (e == cudaSuccess) e = pqw_gather(c, r.distinct[1]->chunks[0].values, (*dvals)->chunks[0].values, entry_ranges, w);
+    if (e == cudaSuccess) e = finish_single_group(c, ids->get());
+    if (e == cudaSuccess) e = finish_single_group(c, dvals->get());
+    if (e != cudaSuccess) return fail_cuda(e, "Parquet dictionary (kept entries)");
+    return BDF_OK;
+}
+
+static int parquet_write(bdf_ctx* c, const char* path, int n_cols, const char* const* names, const bdf_col* const* cols, const bdf_temporal_type* types,
+                         const bdf_parquet_write_options* opt) {
+    if (!path || !names || !cols) return fail(BDF_INVALID, "null argument");
+    if (n_cols <= 0) return fail(BDF_INVALID, "no columns to write");
+    const int compression = opt ? opt->compression : 0, use_dict = opt ? opt->dictionary : 1;
+    const int64_t rg_rows_opt = opt ? opt->row_group_rows : 0;
+    if (compression != 0 && compression != 1) return fail(BDF_INVALID, "compression must be 0 (UNCOMPRESSED) or 1 (SNAPPY), not %d", compression);
+    if (use_dict != 0 && use_dict != 1) return fail(BDF_INVALID, "dictionary must be 0 or 1, not %d", use_dict);
+    if (rg_rows_opt < 0) return fail(BDF_INVALID, "row_group_rows must be at least 0");
+    std::vector<PqwCol> pc((size_t)n_cols);
+    std::vector<int32_t> dtypes((size_t)n_cols);
+    int64_t n_chunks = -1;
+    for (int j = 0; j < n_cols; j++) {
+        const bdf_col* col = cols[j];
+        if (!col || !names[j]) return fail(BDF_INVALID, "null column or name");
+        if (!col->fparts.empty()) return fail(BDF_INVALID, "a column of a multi-GPU context was passed to a one-GPU context");
+        TRY(pqw_type(col, types ? &types[j] : nullptr, names[j], &pc[(size_t)j]));
+        dtypes[(size_t)j] = col->dtype;
+        const int64_t nc = (int64_t)col->chunks.size();
+        if (n_chunks < 0) n_chunks = nc;
+        if (nc != n_chunks)
+            return fail(BDF_LENGTH_MISMATCH, "columns have different numbers of chunks (%lld, %lld)", (long long)nc, (long long)n_chunks);
+        for (int64_t b = 0; b < nc; b++)
+            if (col->chunks[b].len != cols[0]->chunks[b].len)
+                return fail(BDF_LENGTH_MISMATCH, "chunk %lld: column '%s' has %lld rows, column '%s' has %lld", (long long)b, names[j],
+                            (long long)col->chunks[b].len, names[0], (long long)cols[0]->chunks[b].len);
+    }
+    std::vector<int64_t> starts((size_t)n_chunks + 1, 0);
+    for (int64_t b = 0; b < n_chunks; b++) starts[b + 1] = starts[b] + cols[0]->chunks[b].len;
+    const int64_t rows = starts[n_chunks];
+    if (rows > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "at most 2^32-1 rows per file (the dictionary's UInt32 row numbers)");
+    // row groups: one per non-empty chunk, or row_group_rows rows each across the chunks
+    int64_t n_rg64 = 0;
+    if (rg_rows_opt == 0) { for (int64_t b = 0; b < n_chunks; b++) n_rg64 += starts[b + 1] > starts[b]; }
+    else n_rg64 = (rows + rg_rows_opt - 1) / rg_rows_opt;
+    if (n_rg64 * n_cols > kPqwMaxChunks)
+        return fail(BDF_INVALID, "%lld row groups x %d columns: at most %lld column chunks per file (use larger row groups)", (long long)n_rg64, n_cols,
+                    (long long)kPqwMaxChunks);
+    const int n_rg = (int)n_rg64;
+    std::vector<int64_t> rg_start;
+    if (rg_rows_opt == 0) { for (int64_t b = 0; b < n_chunks; b++) if (starts[b + 1] > starts[b]) rg_start.push_back(starts[b]); }
+    else for (int64_t r = 0; r < rows; r += rg_rows_opt) rg_start.push_back(r);
+    rg_start.push_back(rows);
+    std::string arrow_schema;
+    {
+        std::vector<bdf_temporal_type> tts((size_t)n_cols, bdf_temporal_type{0, 0, nullptr});
+        if (types) for (int j = 0; j < n_cols; j++) tts[(size_t)j] = types[j];
+        arrow_schema = pq::base64(bdf::arrow_schema_message(n_cols, names, dtypes.data(), tts.data()));
+    }
+    std::vector<pq::WColumn> wcols;
+    for (auto& p : pc) wcols.push_back(p.meta);
+
+    // dictionaries (every non-Boolean column when dictionary = 1)
+    std::vector<ColOwner> ids, dvals;
+    for (int j = 0; j < n_cols; j++) { ids.emplace_back(c); dvals.emplace_back(c); }
+    if (use_dict && rows > 0) {
+        ColOwner rg_col(c);
+        TRY(col_alloc(c, BDF_U32, {ChunkPlan{rows, false}}, nullptr, 0, rg_col.out()));
+        Scratch<long long> d_rg;
+        cudaError_t e = d_rg.alloc(c, (size_t)n_rg * sizeof(long long));
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_rg, rg_start.data(), (size_t)n_rg * sizeof(long long), cudaMemcpyHostToDevice, c->s_compute);
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_PARQUET_WRITE, BDF_U32, rows, rows * 4);
+            e = launch_pqw_rgid(d_rg, n_rg, rows, (uint32_t*)rg_col->chunks[0].values, c->sm_count, c->s_compute);
+        }
+        if (e == cudaSuccess) e = finish_single_group(c, rg_col.get());
+        if (e != cudaSuccess) return fail_cuda(e, "Parquet row-group ids");
+        for (int j = 0; j < n_cols; j++)
+            if (cols[j]->dtype != kBool) TRY(pqw_dictionary(c, cols[j], rg_col.get(), rg_start, &pc[(size_t)j], &ids[(size_t)j], &dvals[(size_t)j]));
+    }
+
+    // the page, tile and fragment tables of every block, in file order
+    const bool snappy = compression == 1;
+    const uint32_t frag_cap = pq::snappy_bound(pq::kFragment);
+    struct Blk { size_t p0, p1, t0, t1, f0, f1; size_t raw; };
+    struct PageRef { int rg, col; };
+    std::vector<pq::WPage> pages;
+    std::vector<pq::WTile> tiles;
+    std::vector<int> frag_page;
+    std::vector<PageRef> pref;
+    std::vector<Blk> blocks;
+    std::vector<std::vector<int>> chunk_dict((size_t)n_rg, std::vector<int>((size_t)n_cols, 0));   // the chunk is dictionary-encoded
+    Blk cur{0, 0, 0, 0, 0, 0, 0};
+    size_t frag_used = 0;
+    auto add_page = [&](pq::WPage pg, size_t raw_worst, int rg, int j, const std::function<void(int)>& make_tiles) {
+        pg.n_frags = snappy ? (int)((raw_worst + pq::kFragment - 1) / pq::kFragment) : 0;
+        size_t slot = raw_worst;
+        if (snappy) slot = raw_worst + raw_worst / 6 + 32 * (size_t)pg.n_frags + 8;
+        slot = align_up(slot, 16);
+        const size_t frags = (size_t)pg.n_frags * frag_cap;
+        if (pages.size() > cur.p0 && (cur.raw + slot > kPqwRaw || frag_used + frags > kPqwFrag)) {
+            cur.p1 = pages.size(); cur.t1 = tiles.size(); cur.f1 = frag_page.size();
+            blocks.push_back(cur);
+            cur = Blk{pages.size(), 0, tiles.size(), 0, frag_page.size(), 0, 0};
+            frag_used = 0;
+        }
+        pg.slot = (long long)cur.raw;
+        pg.frag0 = (long long)(frag_page.size() - cur.f0);
+        pg.tile0 = (int)(tiles.size() - cur.t0);
+        for (int f = 0; f < pg.n_frags; f++) frag_page.push_back((int)(pages.size() - cur.p0));
+        make_tiles((int)(pages.size() - cur.p0));
+        pg.n_tiles = (int)(tiles.size() - cur.t0) - pg.tile0;
+        cur.raw += slot;
+        frag_used += frags;
+        pages.push_back(pg);
+        pref.push_back(PageRef{rg, j});
+    };
+    for (int g = 0; g < n_rg; g++)
+        for (int j = 0; j < n_cols; j++) {
+            const PqwCol& p = pc[(size_t)j];
+            const bdf_col* col = cols[j];
+            pq::WPage base{};
+            base.width = p.width; base.in_width = p.in_width; base.conv = p.conv; base.ord = p.ord;
+            const bool dict = dvals[(size_t)j].get() && p.keep[(size_t)g];
+            chunk_dict[(size_t)g][(size_t)j] = dict;
+            if (dict) {
+                pq::WPage pg = base;
+                pg.kind = pq::KIND_DICT;
+                pg.rows = (int)p.dcount[(size_t)g];
+                const DevChunk& dv = dvals[(size_t)j]->chunks[0];
+                const long long first = p.dfirst[(size_t)g];
+                add_page(pg, (size_t)pg.rows * p.width, g, j, [&](int page) {
+                    for (int e0 = 0; e0 < pg.rows; e0 += pq::kWTileRows)
+                        tiles.push_back(pq::WTile{dv.values, nullptr, nullptr, first + e0, 0, 0, page, e0, std::min(pq::kWTileRows, pg.rows - e0), 0});
+                });
+                base.id_bw = pq::id_bit_width(p.dcount[(size_t)g]);
+            }
+            for (int64_t r0 = rg_start[g]; r0 < rg_start[g + 1]; r0 += kPqwPageRows) {
+                const int64_t r1 = std::min(rg_start[g + 1], r0 + kPqwPageRows);
+                pq::WPage pg = base;
+                pg.kind = pq::KIND_V1;
+                pg.rows = (int)(r1 - r0);
+                const size_t nr = (size_t)pg.rows, bits = (nr + 7) / 8;
+                const size_t values = pg.id_bw ? 1 + 5 + bits * (size_t)pg.id_bw : p.width ? nr * (size_t)p.width : bits;
+                add_page(pg, 4 + 5 + bits + values, g, j, [&](int page) {
+                    int64_t b = std::upper_bound(starts.begin(), starts.end(), r0) - starts.begin() - 1;
+                    for (int64_t r = r0; r < r1;) {
+                        while (starts[b + 1] <= r) b++;
+                        const DevChunk& ch = col->chunks[(size_t)b];
+                        const int64_t end = std::min({r1, starts[b + 1], r + (int64_t)pq::kWTileRows});
+                        const uint32_t* idp = dict ? (const uint32_t*)ids[(size_t)j]->chunks[0].values + p.id0[(size_t)g] + (r - rg_start[g]) : nullptr;
+                        tiles.push_back(pq::WTile{ch.values, ch.validity, idp, r - starts[b], ch.bit_off, ch.val_bit_off, page, (int)(r - r0), (int)(end - r), 0});
+                        r = end;
+                    }
+                });
+            }
+        }
+    if (pages.size() > cur.p0) { cur.p1 = pages.size(); cur.t1 = tiles.size(); cur.f1 = frag_page.size(); blocks.push_back(cur); }
+    if (tiles.size() > (size_t)0x7fffffff) return fail(BDF_UNSUPPORTED, "the file has more tiles than one launch covers");
+
+    // device buffers, then the file
+    for (int j = 0; j < n_cols; j++) wait_groups(c->s_compute, cols[j], 0, n_chunks);
+    const size_t np = std::max<size_t>(pages.size(), 1), nt = std::max<size_t>(tiles.size(), 1), nf = std::max<size_t>(frag_page.size(), 1);
+    Scratch<char> d_pages, d_tiles, d_out, d_lay;
+    Scratch<unsigned int> d_tvalid, d_tbase, d_flen;
+    Scratch<int> d_fpage;
+    Scratch<uint8_t> raw[2], frag;
+    struct Pinned { pq::WPageOut* p = nullptr; ~Pinned() { if (p) cudaFreeHost(p); } } h_out;
+    cudaError_t e = d_pages.alloc(c, np * sizeof(pq::WPage));
+    if (e == cudaSuccess) e = d_tiles.alloc(c, nt * sizeof(pq::WTile));
+    if (e == cudaSuccess) e = d_out.alloc(c, np * sizeof(pq::WPageOut));
+    if (e == cudaSuccess) e = d_lay.alloc(c, np * sizeof(uint2));
+    if (e == cudaSuccess) e = d_tvalid.alloc(c, nt * sizeof(unsigned int));
+    if (e == cudaSuccess) e = d_tbase.alloc(c, nt * sizeof(unsigned int));
+    if (e == cudaSuccess) e = d_fpage.alloc(c, nf * sizeof(int));
+    if (e == cudaSuccess) e = d_flen.alloc(c, nf * sizeof(unsigned int));
+    if (e == cudaSuccess && !blocks.empty()) e = raw[0].alloc(c, kPqwRaw);
+    if (e == cudaSuccess && blocks.size() > 1) e = raw[1].alloc(c, kPqwRaw);
+    if (e == cudaSuccess && snappy && !blocks.empty()) e = frag.alloc(c, kPqwFrag);
+    if (e == cudaSuccess && !pages.empty()) e = cudaMemcpyAsync(d_pages, pages.data(), pages.size() * sizeof(pq::WPage), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess && !tiles.empty()) e = cudaMemcpyAsync(d_tiles, tiles.data(), tiles.size() * sizeof(pq::WTile), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess && !frag_page.empty()) e = cudaMemcpyAsync(d_fpage, frag_page.data(), frag_page.size() * sizeof(int), cudaMemcpyHostToDevice, c->s_compute);
+    if (e == cudaSuccess) e = cudaHostAlloc((void**)&h_out.p, np * sizeof(pq::WPageOut), cudaHostAllocDefault);
+    if (e != cudaSuccess) return fail_cuda(e, "Parquet write setup");
+    TRY(ensure_stage(c));
+    struct Events { bdf_ctx* c; cudaEvent_t ev[4] = {}; ~Events() { for (auto x : ev) ev_put(c, x); } } evs{c};
+    for (auto& x : evs.ev) CK(ev_get(c, &x));
+    cudaEvent_t* ev_done = evs.ev;       // block k's page results are on the host and its bodies complete in raw[k & 1]
+    cudaEvent_t* ev_d2h = evs.ev + 2;    // block k's bodies have left raw[k & 1]
+
+    const int fd = open(path, O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0644);
+    if (fd < 0) return fail(BDF_INVALID, "cannot create %s: %s", path, strerror(errno));
+    struct FdGuard { int fd; ~FdGuard() { if (fd >= 0) close(fd); } } fdg{fd};
+    // Declared after the buffers, so it runs first on every exit: no copy may still read a body buffer when it is freed.
+    struct DrainD2H { cudaStream_t s; ~DrainD2H() { cudaStreamSynchronize(s); } } drain_guard{c->s_d2h};
+    off_t file_off = 0;
+
+    size_t rec_enc[2] = {0, 0}, rec_snappy[2] = {0, 0};
+    auto enqueue = [&](size_t k) -> int {
+        const Blk& B = blocks[k];
+        const int b = (int)(k & 1);
+        cudaError_t e2 = k >= 2 ? cudaStreamWaitEvent(c->s_compute, ev_d2h[b], 0) : cudaSuccess;
+        if (e2 == cudaSuccess) e2 = cudaMemsetAsync(raw[b], 0, B.raw, c->s_compute);
+        const int n_p = (int)(B.p1 - B.p0), n_t = (int)(B.t1 - B.t0), n_f = (int)(B.f1 - B.f0);
+        if (e2 == cudaSuccess) {
+            int64_t in_rows = 0, in_bytes = 0;
+            for (size_t t = B.t0; t < B.t1; t++) {
+                const pq::WPage& pg = pages[B.p0 + (size_t)tiles[t].page];
+                in_rows += tiles[t].rows;
+                in_bytes += pg.in_width ? (int64_t)tiles[t].rows * pg.in_width : tiles[t].rows / 8;
+            }
+            LaunchTimer t(c, BDF_K_PARQUET_WRITE, -1, in_rows, in_bytes);   // + the bodies, once their sizes are known
+            c->launches += 2;                                                // count, layout, encode
+            e2 = launch_pqw_encode(d_pages + B.p0 * sizeof(pq::WPage), n_p, d_tiles + B.t0 * sizeof(pq::WTile), n_t, d_tvalid + B.t0, d_tbase + B.t0,
+                                   d_lay + B.p0 * sizeof(uint2), raw[b], d_out + B.p0 * sizeof(pq::WPageOut), c->s_compute);
+        }
+        if (c->profiling) rec_enc[b] = c->prof.size() - 1;
+        if (e2 == cudaSuccess && snappy) {
+            LaunchTimer t(c, BDF_K_PARQUET_WRITE, BDF_U8, n_p, 0);   // bytes: the bodies read and written, once known
+            c->launches++;                                           // snappy, compaction
+            e2 = launch_pqw_snappy(d_pages + B.p0 * sizeof(pq::WPage), d_fpage + B.f0, n_f, raw[b], d_out + B.p0 * sizeof(pq::WPageOut), frag,
+                                   d_flen + B.f0, c->s_compute);
+            if (c->profiling) rec_snappy[b] = c->prof.size() - 1;
+        }
+        if (e2 == cudaSuccess)
+            e2 = cudaMemcpyAsync(h_out.p + B.p0, d_out + B.p0 * sizeof(pq::WPageOut), (size_t)n_p * sizeof(pq::WPageOut), cudaMemcpyDeviceToHost, c->s_compute);
+        if (e2 == cudaSuccess) e2 = cudaEventRecord(ev_done[b], c->s_compute);
+        return e2 == cudaSuccess ? BDF_OK : fail_cuda(e2, "Parquet write kernels");
+    };
+    struct Pending { bdf_ctx::StageSlot* sl; off_t off; size_t n; };
+    std::deque<Pending> pending;
+    auto retire = [&]() -> int {
+        const Pending p = pending.front();
+        pending.pop_front();
+        CK(cudaEventSynchronize(p.sl->ev));
+        p.sl->busy = false;
+        constexpr size_t kJob = (size_t)512 << 10;
+        std::atomic<int> werr{0};
+        c->pool->run((p.n + kJob - 1) / kJob, [&](size_t j) {
+            const int we = pwrite_all(fd, p.sl->p + j * kJob, std::min(kJob, p.n - j * kJob), p.off + (off_t)(j * kJob));
+            if (we) werr = we;
+        });
+        if (werr) return fail(BDF_INVALID, "writing %s failed: %s", path, strerror(werr));
+        return BDF_OK;
+    };
+    // The file's bytes go through the staging slots in order: a header is copied in by the host, a body by a D2H copy.
+    bdf_ctx::StageSlot* sl = nullptr;
+    size_t fill = 0;
+    off_t slot_off = 0;
+    auto close_slot = [&]() -> int {
+        if (!sl) return BDF_OK;
+        CK(cudaEventRecord(sl->ev, c->s_d2h));
+        sl->busy = true;
+        pending.push_back(Pending{sl, slot_off, fill});
+        sl = nullptr;
+        return BDF_OK;
+    };
+    auto put = [&](const char* src, size_t n, bool device) -> int {
+        while (n) {
+            if (!sl || fill == kStageBytes) {
+                TRY(close_slot());
+                if ((int)pending.size() >= kStageSlots - 1) TRY(retire());
+                sl = &c->stage[c->stage_next++ % kStageSlots];
+                if (sl->busy) CK(cudaEventSynchronize(sl->ev));   // an upload's slot
+                fill = 0;
+                slot_off = file_off;
+            }
+            const size_t m = std::min(n, kStageBytes - fill);
+            if (device) CK(cudaMemcpyAsync(sl->p + fill, src, m, cudaMemcpyDeviceToHost, c->s_d2h));
+            else memcpy(sl->p + fill, src, m);
+            fill += m; src += m; n -= m; file_off += (off_t)m;
+        }
+        return BDF_OK;
+    };
+    TRY(put("PAR1", 4, false));
+    std::vector<std::vector<pq::WChunkMeta>> meta((size_t)n_rg, std::vector<pq::WChunkMeta>((size_t)n_cols));
+    std::vector<std::vector<pq::Stats>> cst((size_t)n_rg, std::vector<pq::Stats>((size_t)n_cols, pq::stats_empty()));
+    auto drain = [&](size_t k) -> int {
+        const Blk& B = blocks[k];
+        const int b = (int)(k & 1);
+        CK(cudaEventSynchronize(ev_done[b]));
+        CK(cudaStreamWaitEvent(c->s_d2h, ev_done[b], 0));
+        int64_t raw_sum = 0, comp_sum = 0;
+        for (size_t i = B.p0; i < B.p1; i++) {
+            const pq::WPage& pg = pages[i];
+            const pq::WPageOut& o = h_out.p[i];
+            if (o.err) return fail(BDF_INVALID, "a snappy fragment outgrew its worst-case bound");
+            const PageRef& pr = pref[i];
+            pq::WChunkMeta& m = meta[(size_t)pr.rg][(size_t)pr.col];
+            const bool dict = chunk_dict[(size_t)pr.rg][(size_t)pr.col] != 0;
+            const int enc = pg.kind == pq::KIND_DICT || pg.id_bw ? pq::ENC_PLAIN_DICTIONARY : pq::ENC_PLAIN;
+            const std::string h = pq::page_header(pg.kind, (int)o.raw_len, (int)o.comp_len, pg.rows, enc);
+            if (pg.kind == pq::KIND_DICT) m.dict_page_offset = file_off;
+            else if (m.num_values == 0) m.data_page_offset = file_off;
+            if (pg.kind != pq::KIND_DICT) { m.num_values += pg.rows; pq::stats_merge(&cst[(size_t)pr.rg][(size_t)pr.col], o.st); }
+            m.total_uncompressed += (long long)(h.size() + o.raw_len);
+            m.total_compressed += (long long)(h.size() + o.comp_len);
+            m.phys = pc[(size_t)pr.col].phys;
+            m.codec = snappy ? 1 : 0;
+            m.encodings = dict ? std::vector<int>{pq::ENC_PLAIN_DICTIONARY, pq::ENC_RLE} : std::vector<int>{pq::ENC_PLAIN, pq::ENC_RLE};
+            raw_sum += o.raw_len;
+            comp_sum += o.comp_len;
+            TRY(put(h.data(), h.size(), false));
+            TRY(put((const char*)raw[b].get() + pg.slot, o.comp_len, true));
+        }
+        if (c->profiling) {
+            c->prof[rec_enc[b]].rec.bytes += raw_sum;
+            if (snappy) c->prof[rec_snappy[b]].rec.bytes += raw_sum + comp_sum;
+        }
+        CK(cudaEventRecord(ev_d2h[b], c->s_d2h));
+        return BDF_OK;
+    };
+    if (!blocks.empty()) TRY(enqueue(0));
+    for (size_t k = 0; k < blocks.size(); k++) {
+        if (k + 1 < blocks.size()) TRY(enqueue(k + 1));
+        TRY(drain(k));
+    }
+    // the footer: chunk statistics in the stored physical values
+    for (int g = 0; g < n_rg; g++)
+        for (int j = 0; j < n_cols; j++) {
+            pq::WChunkMeta& m = meta[(size_t)g][(size_t)j];
+            const pq::Stats& s = cst[(size_t)g][(size_t)j];
+            const PqwCol& p = pc[(size_t)j];
+            const int w = p.width ? p.width : 1;
+            m.has_stats = true;
+            m.null_count = (long long)s.nulls;
+            m.has_minmax = s.count > 0;
+            if (m.has_minmax) {
+                const uint64_t lo = pq::stat_value(p.ord, w, s.kmin, false), hi = pq::stat_value(p.ord, w, s.kmax, true);
+                m.min_value.assign((const char*)&lo, (size_t)w);   // little-endian
+                m.max_value.assign((const char*)&hi, (size_t)w);
+            }
+        }
+    std::vector<long long> rg_rows((size_t)n_rg);
+    for (int g = 0; g < n_rg; g++) rg_rows[(size_t)g] = rg_start[g + 1] - rg_start[g];
+    std::string tail = pq::file_metadata(wcols, rg_rows, meta, arrow_schema);
+    const uint32_t flen = (uint32_t)tail.size();
+    tail.append((const char*)&flen, 4);
+    tail += "PAR1";
+    TRY(put(tail.data(), tail.size(), false));
+    TRY(close_slot());
+    while (!pending.empty()) TRY(retire());
+    const int fdv = fdg.fd;
+    fdg.fd = -1;
+    if (close(fdv) != 0) return fail(BDF_INVALID, "closing %s failed: %s", path, strerror(errno));
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // Multi-GPU context (bdf_init_multi): ONE process, every GPU of the box.  The library owns the sharding that the
 // reference leaves to rayon (par_iter over chunks, src/functions/scalar.rs:28-31,99-102): the rows of a call are cut into
 // one contiguous range per GPU (cuts on 64-row boundaries inside a chunk, so a piece is a zero-copy Arrow slice whose
@@ -5735,6 +6262,13 @@ int bdf_csv_write(bdf_ctx* c, const char* path, int32_t n_cols, const char* cons
     if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the CSV writer writes from one GPU: use a one-GPU context (bdf_init) for it");
     ENTER(c);
     return csv_write(c, path, n_cols, names, cols, options);
+}
+
+int bdf_parquet_write(bdf_ctx* c, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols, const bdf_temporal_type* types,
+                      const bdf_parquet_write_options* options) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the Parquet writer writes from one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return parquet_write(c, path, n_cols, names, cols, types, options);
 }
 
 int bdf_take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, bdf_col** out) {

@@ -39,7 +39,7 @@ from .arrays import F32, F64, I8, I64, U8, U32, U64, PrimitiveArray, is_float
 from .functions import Column, _expr_nodes, eval_expr, sort_indices, window as _window
 from .csv_reader import CsvFile, write_csv
 from .json_reader import JsonFile
-from .parquet_reader import ParquetFile
+from .parquet_reader import ParquetFile, write_parquet
 from .ipc import BOOL, IpcFile, write_ipc
 
 ARITH = {"add": N.ADD, "subtract": N.SUB, "multiply": N.MUL, "divide": N.DIV}
@@ -449,6 +449,11 @@ class DeviceFrame:
             if getattr(c, "temporal", None) is not None:
                 raise N.UnsupportedType(f"column {n!r} is {c.temporal!r}: temporal text is not written by the CSV writer")
         write_csv(path, self.columns, has_header=has_header, delimiter=delimiter)
+
+    def to_parquet(self, path: str, compression: str = "none", dictionary: bool = True, row_group_rows: int = 0) -> None:
+        """DataFrame::to_parquet: the frame's pages are encoded (and compressed) on the device and streamed to the file
+        (write_parquet); temporal columns are written as Date / Time / Timestamp columns."""
+        write_parquet(path, self.columns, compression=compression, dictionary=dictionary, row_group_rows=row_group_rows)
 
     def to_host(self) -> Dict[str, list]:
         return {n: c.download() for n, c in self.columns.items()}

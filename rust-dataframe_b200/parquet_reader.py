@@ -8,11 +8,12 @@ include/b200df.h):
         f.schema                             # [(name, dtype or -1, nullable)]; temporal columns report their physical dtype
         f.temporal_columns                   # {name: TemporalType}
         cols = f.read(["id", "ts"])          # -> {name: Column}, one chunk per RecordBatch; temporal columns come back tagged
+    write_parquet("out.parquet", cols, compression="snappy")   # encoded and compressed on the device (csrc/k_parquet_write.cu)
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional, Sequence, Union
+from typing import Dict, Mapping, Optional, Sequence, Union
 
 from . import _native as N
 from .arrays import TemporalType
@@ -97,3 +98,30 @@ class ParquetFile:
             name = self.schema[i][0]
             res[name] = Column(ctx, C.c_void_p(outs[j]), self.temporal_columns.get(name))
         return res
+
+
+_CODECS = {"none": 0, "uncompressed": 0, "snappy": 1}
+
+
+def write_parquet(path: str, columns: Mapping[str, "object"], compression: str = "none", dictionary: bool = True,
+                  row_group_rows: int = 0) -> None:
+    """Device Columns (chunk b of every column has the same length) -> a Parquet file, encoded and compressed on the device
+    (bdf_parquet_write; the rules are in include/b200df.h).  One row group per chunk (row_group_rows = 0) or row_group_rows rows per
+    row group; Date / Time / Timestamp columns are written as such from ``Column.temporal``."""
+    if compression not in _CODECS:
+        raise ValueError(f"compression is one of {sorted(_CODECS)}, not {compression!r}")
+    from .functions import Column
+
+    names = list(columns)
+    for s in names:
+        if not isinstance(columns[s], Column):
+            raise N.UnsupportedType(f"column {s!r} is a {type(columns[s]).__name__}: only numeric, Boolean and temporal columns are written to Parquet")
+    k = len(names)
+    ctx = columns[names[0]].ctx if k else N.default_context()
+    cnames = (C.c_char_p * max(k, 1))(*[s.encode() for s in names])
+    handles = (C.c_void_p * max(k, 1))(*[columns[s].handle for s in names])
+    tags = [getattr(columns[s], "temporal", None) for s in names]
+    types = (N.TemporalTypeC * max(k, 1))(*[N.TemporalTypeC(t.kind, t.unit, t.tz.encode() if t.tz is not None else None) if t is not None
+                                             else N.TemporalTypeC(0, 0, None) for t in tags])
+    opts = N.ParquetWriteOptions(_CODECS[compression], 1 if dictionary else 0, int(row_group_rows))
+    N.raise_for_status(N.lib().bdf_parquet_write(ctx.handle, str(path).encode(), k, cnames, handles, types, C.byref(opts)))
