@@ -14,6 +14,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --ndjson [--csv-rows 50000000]                   # the line-delimited JSON reader rows (a 4.85 GB temporary file)
     python benchmarks/kernels_bench.py --parquet [--csv-rows 50000000]                  # the Parquet reader rows (two temporary files: snappy, none)
     python benchmarks/kernels_bench.py --parquet-write [--csv-rows 50000000]            # the Parquet writer rows (none/PLAIN, none/dictionary, snappy/dictionary)
+    python benchmarks/kernels_bench.py --distribution [--rows 100000000]                # median, hist, uniques, mode next to k_reduce and the sort
 """
 from __future__ import annotations
 
@@ -586,6 +587,65 @@ def stats_bench(ctx, lens, report, rows_out):
         col.free()
 
 
+def _wall3(ctx, fn):
+    """The median of three timed calls after one warm-up call (each call ends in a device synchronise), in ms."""
+    def once():
+        out = fn()
+        ctx.synchronize()
+        for o in out if isinstance(out, (list, tuple)) else [out]:
+            if isinstance(o, rdf.Column):
+                o.free()
+    once()
+    t = []
+    for _ in range(3):
+        t0 = time.perf_counter()
+        once()
+        t.append((time.perf_counter() - t0) * 1e3)
+    return float(np.median(t))
+
+
+def distribution_bench(ctx, lens, rows_out):
+    """The column distributions: whole-column median (radix select), hist, uniques and mode, each next to k_reduce and
+    bdf_sort_indices_dev on the same column in the same session; per-group median and mode next to avg.  Times are the median of three
+    calls after a warm-up call, host clock around calls that end in a synchronise."""
+    G = rdf.Column.generate
+    card = _card()
+    print("card:", card, flush=True)
+
+    def row(case, col, fn):
+        ms = _wall3(ctx, fn)
+        red = _wall3(ctx, lambda: col.aggregate_all())
+        srt = _wall3(ctx, lambda: rdf.sort_indices([(col, False)]))
+        rows_out.append({"case": case, "ms": ms, "k_reduce_ms": red, "sort_indices_ms": srt, "card": card})
+        print(f"{case:44s} {ms:9.3f} ms   k_reduce {red:8.3f} ms   sort_indices {srt:9.3f} ms   {'faster' if ms < srt else 'SLOWER'} than the sort",
+              flush=True)
+
+    f64 = G(rdf.F64, lens, 0, -1e3, 1e3, col_id=60)
+    f64n = G(rdf.F64, lens, 0, -1e3, 1e3, col_id=61, null_mod=10)
+    eq = G(rdf.F64, lens, 0, 5.0, 5.0, col_id=62)
+    i32 = G(rdf.I32, lens, 2, col_id=63)
+    i32n = G(rdf.I32, lens, 2, col_id=64, null_mod=10)
+    kf = G(rdf.F64, lens, 0, -100.0, 100.0, col_id=65)
+    i8 = kf.cast(rdf.I8)
+    kf.free()
+    eq_i32 = eq.cast(rdf.I32)
+    for what, col in (("f64", f64), ("f64 10% nulls", f64n), ("f64 all equal", eq), ("i32", i32), ("i32 10% nulls", i32n),
+                      ("i32 all equal", eq_i32)):
+        row(f"median {what}", col, lambda: col.median())
+    row("hist f64, 10 bins", f64, lambda: f64.hist(10))
+    row("hist f64, 2^20 bins", f64, lambda: f64.hist(2 ** 20))
+    row("uniques i8 (200 values)", i8, lambda: i8.uniques())
+    row("mode i8 (200 values)", i8, lambda: i8.mode())
+    row("uniques i32 (~1e8 values)", i32, lambda: i32.uniques())
+    row("mode i32 (~1e8 values)", i32, lambda: i32.mode())
+    for fn in ("avg", "exact_median", "mode"):
+        ms = _wall3(ctx, lambda: [c for part in rdf.group_by([i32n, i8], [(f64, fn)]) for c in part])
+        rows_out.append({"case": f"group-by i32 (nulls) x i8 keys, {fn} f64", "ms": ms, "card": card})
+        print(f"{'group-by i32 (nulls) x i8 keys, ' + fn + ' f64':44s} {ms:9.3f} ms", flush=True)
+    for col in (f64, f64n, eq, i32, i32n, i8, eq_i32):
+        col.free()
+
+
 def _stream_rates(rows):
     """The HBM rates of benchmarks/tune_stream.cu (best of each class), built into a temporary directory and run here:
     {"read": read-only sum, "copy": copy 1 read + 1 write} in GB/s."""
@@ -739,6 +799,7 @@ def main():
     ap.add_argument("--ndjson", action="store_true", help="run the line-delimited JSON reader rows (--csv-rows records)")
     ap.add_argument("--parquet", action="store_true", help="run the Parquet reader rows (--csv-rows rows, snappy and uncompressed)")
     ap.add_argument("--parquet-write", action="store_true", help="run the Parquet writer rows (--csv-rows rows, three encodings)")
+    ap.add_argument("--distribution", action="store_true", help="run only the distribution rows (median, hist, uniques, mode)")
     args = ap.parse_args()
     ctx = rdf.default_context()
     if args.parquet_write:
@@ -822,6 +883,12 @@ def main():
                          "GBs": gbs, "frac_of_peak": gbs / pk, "rows_per_s": rows / ms * 1e3})
         print(f"{name:44s} {ms:8.4f} ms  {nbytes / rows:7.3f} B/row  {gbs:8.1f} GB/s  {gbs / pk:5.3f} of peak  {rows / ms * 1e3:10.3e} rows/s", flush=True)
 
+    if args.distribution:
+        distribution_bench(ctx, lens, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"results": rows_out}, f, indent=1)
+        return
     if args.math or args.stats:
         (math_bench(ctx, lens, report) if args.math else stats_bench(ctx, lens, report, rows_out))
         if args.json:

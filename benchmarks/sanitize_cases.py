@@ -150,6 +150,14 @@ with tempfile.TemporaryDirectory() as td:
     for kw in ({}, {"compression": "snappy"}, {"dictionary": False}, {"row_group_rows": 700, "compression": "snappy"}):
         rdf.write_parquet(os.path.join(td, "w.parquet"), pw, **kw)
     rdf.write_parquet(os.path.join(td, "e.parquet"), {"x": rdf.Column.upload([P.from_numpy(np.zeros(0, dtype=np.int32))])})
+# the distributions: select levels from the column and from compacted scratch (many prefixes), the all-equal column, the histogram on
+# both bin paths over ragged, offset chunks with nulls, uniques with counts and mode
+for npdt in (np.int8, np.int64, np.float32, np.float64):
+    dc = rdf.Column.upload([P.from_numpy(rng.integers(-1000, 1000, n + 3).astype(npdt), rng.random(n + 3) > 0.2).slice(3, n) for n in lens])
+    dc.percentile(list(np.linspace(0, 1, 300))); dc.median(); dc.mode(); dc.hist(10); dc.hist(5000, range=(-10.0, 10.0))
+    vals, cnts = dc.value_counts()
+    vals.download(); cnts.download()
+rdf.Column.upload([P.from_numpy(np.full(70000, 2.5))]).median()
 # round 2: the fleet code path on one GPU, and a single-rank communicator (pack -> combine -> unpack on the stream)
 fleet = rdf.Context.multi(1)
 fa = [P.from_numpy(rng.integers(-100, 100, n).astype(np.int64), rng.random(n) > 0.3) for n in (1000, 0, 77)]

@@ -322,7 +322,12 @@ int  bdf_group_aggregate_dev(bdf_ctx* ctx, const bdf_col* key, int32_t n_values,
  *                   once).  Never NULL: a group without a valid value sums to 0.  A NaN among them makes the sum NaN. */
 typedef enum { BDF_GROUP_SUM = 0, BDF_GROUP_MAX, BDF_GROUP_MIN, BDF_GROUP_AVG, BDF_GROUP_COUNT, BDF_GROUP_COUNT_DISTINCT, BDF_GROUP_FIRST,
                BDF_GROUP_LAST, BDF_GROUP_KURTOSIS, BDF_GROUP_SKEWNESS, BDF_GROUP_STDDEV, BDF_GROUP_SUM_DISTINCT, BDF_GROUP_VARIANCE,
-               BDF_GROUP_STDDEV_POP, BDF_GROUP_VAR_POP } bdf_group_fn;   /* AggregateFunction order, then the population forms */
+               BDF_GROUP_STDDEV_POP, BDF_GROUP_VAR_POP,
+               BDF_GROUP_MEDIAN = 32, BDF_GROUP_MODE } bdf_group_fn;   /* AggregateFunction order and the population forms; 32..: the distributions */
+/* The distribution functions (section "distributions" below) per group, after the second sort of COUNT_DISTINCT.  They are not members of
+ * AggregateFunction, so they start a block of their own at 32 and 15..31 stay unknown function ids (BDF_UNSUPPORTED):
+ *   MEDIAN  Float64: the percentile at p = 0.5 of the group's valid values, by the whole-column rule; NULL without a valid value.
+ *   MODE    dtype of x: the group's most frequent valid value by the whole-column rule; NULL without a valid value. */
 typedef struct { const bdf_col* column; int32_t function; } bdf_group_agg;
 int  bdf_group_by_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_col* const* keys, int32_t n_aggs, const bdf_group_agg* aggs,
                       bdf_col** out_keys /* n_keys */, bdf_col** out /* n_aggs */, int64_t* n_groups);
@@ -446,6 +451,54 @@ int  bdf_moments_stat(const bdf_moment_rec* m, int stat, double* out, int32_t* i
 int  bdf_moments_merge(const bdf_moment_rec* a, const bdf_moment_rec* b, bdf_moment_rec* out);
 int  bdf_distinct(bdf_ctx* ctx, int dtype, int64_t n_chunks, const bdf_view* in, bdf_distinct_rec* out);   /* host in */
 int  bdf_distinct_dev(bdf_ctx* ctx, const bdf_col* in, bdf_distinct_rec* out);
+
+/* ---- distributions (Column::hist and Column::uniques, src/table.rs:244-345; Spark's percentile, median and mode for the
+ * "mode, median" of the reference's README) -------------------------------------------------------------------------------------
+ * Input.  A column of any of the ten numeric types; nulls are skipped.  Keys are the sort's (all NaNs are one value, greater than every
+ *   number; -0.0 == 0.0).
+ * Percentile (Spark's exact percentile): n = the valid values, pos = (double)(n - 1) * p, lo = floor(pos), hi = ceil(pos); a and b are
+ *   the lo-th and hi-th valid values in key order, read `as f64` (Int64 / UInt64 beyond 2^53 round to nearest).  The result is a when
+ *   lo == hi or a == b, else (hi - pos) * a + (pos - lo) * b -- exactly these IEEE operations, no FMA.  A selected -0.0 is +0.0, and
+ *   every NaN result (a selected NaN, or -inf and +inf interpolated) is the positive quiet NaN: the result is a function of the keys,
+ *   whichever rows held them.  median is p = 0.5.  is_some[i] = 0 (out[i] = 0) when the column has no valid value.
+ *   Whole columns are selected, not sorted: an MSD radix select over the keys (a digit histogram of the column read in place, then
+ *   only the keys of the chosen buckets, compacted into a scratch of at most the valid values).
+ * Mode: the valid value with the most rows; ties go to the smallest in key order (Spark 4's mode(col, deterministic => true)).  bits
+ *   is the value of the class's first row in the caller's row order (chunk order, then row), T::Native in the low bytes as bdf_agg4
+ *   (so a class of -0.0 and 0.0 returns whichever came first, as sum_distinct's representative); freq is the class's row count.
+ *   is_some = 0 (bits = freq = 0) without a valid value.
+ * Uniques: the distinct valid values in ascending key order, each class represented as mode represents it, as one chunk without
+ *   nulls; counts[i] (Int64) is the number of rows of class i.  Departures from Column::uniques: (1) the order is ascending, not
+ *   HashSet order; (2) nulls are skipped (the reference reads the bytes of null slots); (3) NaN is one value (the reference panics in
+ *   noisy_float::r64); (4) all ten numeric types, not only Int64 / Float64; (5) Utf8 is not supported (no string columns on the device).
+ * Histogram: numpy.histogram's uniform bins, which are the definition (histo_fp's bucket rule is a departure not followed).  Every
+ *   value is read `as f64`.  Range: the explicit {lo, hi}, else [min, max] of the valid non-NaN values (a -0.0 bound is +0.0), else
+ *   [0, 1] when there is none; lo == hi becomes [lo - 0.5, hi + 0.5].  edges[i] = (double)i * ((hi - lo) / nbins) + lo, two
+ *   roundings (np.linspace; when the step rounds to 0: ((double)i / nbins) * (hi - lo) + lo), edges[nbins] = hi.  A value x with
+ *   lo <= x <= hi goes to bin i = min((int)((x - lo) / (hi - lo) * nbins), nbins - 1), then numpy's one-step correction: i - 1 when
+ *   x < edges[i], else i + 1 when x >= edges[i + 1] and i != nbins - 1.  NaN and values outside an explicit range are not counted.
+ *   Departure: numpy refuses a NaN in an automatic range; here NaN is skipped.  Up to 2048 bins are counted per CTA in shared memory,
+ *   more with global atomics; either way the counts are exact.
+ * bdf_hist_density (no context, no GPU): numpy's density=True, out[i] = ((double)counts[i] / (edges[i + 1] - edges[i])) /
+ *   (double)sum(counts) -- NaN everywhere when no value was counted, as numpy.  Column::hist accepts density and ignores it.
+ * Deterministic: every result is exact (selected keys, integer counts, one interpolation), so the same rows give the same bits on
+ *   every call and under any chunking; atomics only add integers.
+ * Errors (nothing is written, nothing leaks): a null pointer, n_p outside 1..1024, a p outside [0, 1] or NaN, nbins outside 1..2^24
+ *   -> BDF_INVALID; an explicit range with lo > hi -> BDF_INVALID "max must be larger than min in range parameter.", one that is not
+ *   finite -> BDF_INVALID "supplied range of [lo, hi] is not finite"; an automatic range with an infinity -> BDF_INVALID "autodetected
+ *   range of [lo, hi] is not finite"; a non-numeric or Boolean column -> BDF_UNSUPPORTED; more than 2^32-1 rows -> the sort's
+ *   BDF_UNSUPPORTED; a multi-GPU context of either kind -> BDF_UNSUPPORTED (every row of the column must be on one GPU); a scratch
+ *   that does not fit -> BDF_OOM.
+ * Launch records: BDF_K_SELECT for the select passes, BDF_K_HIST for the range and count passes. */
+int  bdf_percentile(bdf_ctx* ctx, int dtype, int64_t n_chunks, const bdf_view* in, int32_t n_p, const double* p, double* out,
+                    int32_t* is_some);   /* host in */
+int  bdf_percentile_dev(bdf_ctx* ctx, const bdf_col* in, int32_t n_p, const double* p, double* out, int32_t* is_some);
+int  bdf_mode(bdf_ctx* ctx, int dtype, int64_t n_chunks, const bdf_view* in, uint64_t* bits, int64_t* freq, int32_t* is_some);   /* host in */
+int  bdf_mode_dev(bdf_ctx* ctx, const bdf_col* in, uint64_t* bits, int64_t* freq, int32_t* is_some);
+int  bdf_uniques_dev(bdf_ctx* ctx, const bdf_col* in, bdf_col** values, bdf_col** counts /* may be NULL */);
+int  bdf_hist_dev(bdf_ctx* ctx, const bdf_col* in, int32_t nbins, const double* range /* NULL or {lo, hi} */, double* edges /* nbins + 1 */,
+                  int64_t* counts /* nbins */);
+int  bdf_hist_density(int32_t nbins, const double* edges, const int64_t* counts, double* out);
 
 /* ---- N4: Arrow IPC files either side of the path ---------------------------------------------------------------
  * DataFrame::from_arrow (src/dataframe.rs:391-407: arrow::ipc::reader::FileReader, every RecordBatch -> one chunk per
@@ -951,7 +1004,7 @@ typedef struct {
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
-typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL, BDF_K_JSON, BDF_K_PARQUET, BDF_K_PARQUET_WRITE } bdf_kernel_id;
+typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL, BDF_K_JSON, BDF_K_PARQUET, BDF_K_PARQUET_WRITE, BDF_K_SELECT, BDF_K_HIST } bdf_kernel_id;
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

@@ -52,6 +52,25 @@ pub fn gpu_distinct<T: ArrowNumericType>(arrays: &[&PrimitiveArray<T>]) -> (i64,
     (r.count, sum)
 }
 
+/// Spark's exact percentile of the valid values at p in [0, 1] (include/b200df.h "distributions"); None without a valid value.
+pub fn gpu_percentile<T: ArrowNumericType>(arrays: &[&PrimitiveArray<T>], p: f64) -> Option<f64> {
+    let v: Vec<BdfView> = arrays.iter().map(|a| view(*a)).collect();
+    let (mut out, mut some) = (0f64, 0i32);
+    let st = unsafe { bdf_percentile(ctx(), dtype_id(&T::get_data_type()), v.len() as i64, v.as_ptr(), 1, &p, &mut out, &mut some) };
+    assert_eq!(st, BDF_OK, "{}", last_error());
+    if some != 0 { Some(out) } else { None }
+}
+
+/// The most frequent valid value (ties: the smallest in the sort's order) and its row count; None without a valid value.
+pub fn gpu_mode<T: ArrowNumericType>(arrays: &[&PrimitiveArray<T>]) -> Option<(T::Native, i64)> {
+    let v: Vec<BdfView> = arrays.iter().map(|a| view(*a)).collect();
+    let (mut bits, mut freq, mut some) = (0u64, 0i64, 0i32);
+    let st = unsafe { bdf_mode(ctx(), dtype_id(&T::get_data_type()), v.len() as i64, v.as_ptr(), &mut bits, &mut freq, &mut some) };
+    assert_eq!(st, BDF_OK, "{}", last_error());
+    if some == 0 { return None; }
+    Some((unsafe { std::ptr::read_unaligned(&bits as *const u64 as *const T::Native) }, freq))
+}
+
 // In src/functions/aggregate.rs:
 //   pub fn sum<T>(arrays)   -> gpu_agg::<T, T::Native>(0, &arrays)
 //   pub fn min<T>(arrays)   -> gpu_agg::<T, T::Native>(1, &arrays)   // the intended minimum; the current body is a copy of max (aggregate.rs:22-31)
@@ -66,3 +85,6 @@ pub fn gpu_distinct<T: ArrowNumericType>(arrays: &[&PrimitiveArray<T>]) -> (i64,
 //   pub fn kurtosis<T: ArrowNumericType>(arrays: Vec<&PrimitiveArray<T>>) -> Option<f64>     -> gpu_stat(BDF_STAT_KURTOSIS, &arrays)   // excess
 //   pub fn count_distinct<T: ArrowNumericType>(arrays: Vec<&PrimitiveArray<T>>) -> i64       -> gpu_distinct(&arrays).0
 //   pub fn sum_distinct<T: ArrowNumericType>(arrays: Vec<&PrimitiveArray<T>>) -> T::Native   -> gpu_distinct(&arrays).1    // 0, not None, like sum
+//   pub fn percentile<T: ArrowNumericType>(arrays: Vec<&PrimitiveArray<T>>, p: f64) -> Option<f64> -> gpu_percentile(&arrays, p)
+//   pub fn median<T: ArrowNumericType>(arrays: Vec<&PrimitiveArray<T>>) -> Option<f64>       -> gpu_percentile(&arrays, 0.5)
+//   pub fn mode<T: ArrowNumericType>(arrays: Vec<&PrimitiveArray<T>>) -> Option<T::Native>   -> gpu_mode(&arrays).map(|m| m.0)

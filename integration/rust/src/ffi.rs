@@ -97,6 +97,8 @@ pub const BDF_GROUP_SUM_DISTINCT: i32 = 11;
 pub const BDF_GROUP_VARIANCE: i32 = 12;
 pub const BDF_GROUP_STDDEV_POP: i32 = 13;
 pub const BDF_GROUP_VAR_POP: i32 = 14;
+pub const BDF_GROUP_MEDIAN: i32 = 32;   // the distributions start a block of their own
+pub const BDF_GROUP_MODE: i32 = 33;
 /// bdf_moment_rec: count, mean and the central sums m2, m3, m4 of the valid values (read `as f64`).
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
@@ -180,6 +182,13 @@ extern "C" {
     pub fn bdf_moments_stat(m: *const BdfMomentRec, stat: c_int, out: *mut f64, is_some: *mut i32) -> c_int;
     pub fn bdf_moments_merge(a: *const BdfMomentRec, b: *const BdfMomentRec, out: *mut BdfMomentRec) -> c_int;
     pub fn bdf_distinct(ctx: *mut BdfCtx, dtype: c_int, n: i64, input: *const BdfView, out: *mut BdfDistinctRec) -> c_int;
+    // distributions: Spark's exact percentile and mode (host in), uniques and numpy's histogram (device in), numpy's density
+    pub fn bdf_percentile(ctx: *mut BdfCtx, dtype: c_int, n: i64, input: *const BdfView, n_p: i32, p: *const f64, out: *mut f64,
+                          is_some: *mut i32) -> c_int;
+    pub fn bdf_mode(ctx: *mut BdfCtx, dtype: c_int, n: i64, input: *const BdfView, bits: *mut u64, freq: *mut i64, is_some: *mut i32) -> c_int;
+    pub fn bdf_uniques_dev(ctx: *mut BdfCtx, input: *const BdfCol, values: *mut *mut BdfCol, counts: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_hist_dev(ctx: *mut BdfCtx, input: *const BdfCol, nbins: i32, range: *const f64, edges: *mut f64, counts: *mut i64) -> c_int;
+    pub fn bdf_hist_density(nbins: i32, edges: *const f64, counts: *const i64, out: *mut f64) -> c_int;
     // device-resident columns (the lazy evaluator keeps a frame's numeric columns in HBM between Calculations)
     pub fn bdf_upload_many(ctx: *mut BdfCtx, n_cols: i64, dtypes: *const i32, n_chunks: *const i64, input: *const *const BdfView, flags: c_int,
                            out: *mut *mut BdfCol) -> c_int;

@@ -261,6 +261,28 @@ pub fn to_parquet_device(frame: &DeviceColumns, path: &str, types: Option<&[BdfT
     check(unsafe { bdf_parquet_write(dev(), c_path.as_ptr(), cols.len() as i32, name_ptrs.as_ptr(), cols.as_ptr(), t, p) })
 }
 
+/// `Column::hist(nbins, density)` on the device (include/b200df.h "distributions"): numpy.histogram's equal-width bins over the
+/// valid non-NaN values; `range` None is their [min, max].  Returns (edges, counts or numpy's density).
+pub fn hist_device(frame: &DeviceColumns, col: usize, nbins: i32, density: bool, range: Option<(f64, f64)>) -> Result<(Vec<f64>, Vec<f64>), String> {
+    let n = nbins.max(0) as usize;
+    let (mut edges, mut counts) = (vec![0f64; n + 1], vec![0i64; n]);
+    let r = range.map(|(lo, hi)| [lo, hi]);
+    let rp = r.as_ref().map_or(std::ptr::null(), |r| r.as_ptr());
+    check(unsafe { bdf_hist_dev(dev(), frame.cols[col], nbins, rp, edges.as_mut_ptr(), counts.as_mut_ptr()) })?;
+    if !density { return Ok((edges, counts.iter().map(|c| *c as f64).collect())); }
+    let mut d = vec![0f64; n];
+    check(unsafe { bdf_hist_density(nbins, edges.as_ptr(), counts.as_ptr(), d.as_mut_ptr()) })?;
+    Ok((edges, d))
+}
+
+/// `Column::uniques()` on the device: the distinct valid values in ascending order as a one-chunk column (and their row counts).
+pub fn uniques_device(frame: &DeviceColumns, col: usize, with_counts: bool) -> Result<(*mut BdfCol, Option<*mut BdfCol>), String> {
+    let (mut values, mut counts): (*mut BdfCol, *mut BdfCol) = (std::ptr::null_mut(), std::ptr::null_mut());
+    let cp = if with_counts { &mut counts as *mut *mut BdfCol } else { std::ptr::null_mut() };
+    check(unsafe { bdf_uniques_dev(dev(), frame.cols[col], &mut values, cp) })?;
+    Ok((values, if with_counts { Some(counts) } else { None }))
+}
+
 /// A run of Float64 Calculations whose intermediates are not kept (config 2: h = sin(((a+b)*c)/d)) as one pass.
 /// `inputs` are column indices; node k writes slot inputs.len() + k (see include/b200df.h, bdf_eval_expr_dev).
 pub fn fused_chain(frame: &DeviceColumns, inputs: &[usize], nodes: &[BdfExprNode]) -> Result<*mut BdfCol, String> {

@@ -23,7 +23,8 @@ ASYNC = 1
 (K_BINARY, K_UNARY, K_CAST, K_REDUCE, K_GENERATE, K_AVG, K_COMPARE, K_FILTER, K_EXPR, K_SORT, K_TAKE, K_GROUP, K_JOIN, K_CSV, K_WINDOW,
  K_MOMENTS, K_CSV_WRITE, K_LIST, K_TEMPORAL, K_JSON, K_PARQUET) = range(21)
 KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
-                "window", "moments", "csv_write", "list", "temporal", "json", "parquet", "parquet_write"]
+                "window", "moments", "csv_write", "list", "temporal", "json", "parquet", "parquet_write", "select", "hist"]
+K_SELECT, K_HIST = 22, 23
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -32,10 +33,12 @@ UTF8 = 11   # CSV schema entry only: a string column the device skips
 # bdf_group_fn (AggregateFunction order)
 (GROUP_SUM, GROUP_MAX, GROUP_MIN, GROUP_AVG, GROUP_COUNT, GROUP_COUNT_DISTINCT, GROUP_FIRST, GROUP_LAST, GROUP_KURTOSIS, GROUP_SKEWNESS,
  GROUP_STDDEV, GROUP_SUM_DISTINCT, GROUP_VARIANCE, GROUP_STDDEV_POP, GROUP_VAR_POP) = range(15)
+GROUP_MEDIAN, GROUP_MODE = 32, 33   # the distributions: a block of their own (not AggregateFunction members)
 GROUP_FNS = {"sum": GROUP_SUM, "max": GROUP_MAX, "min": GROUP_MIN, "avg": GROUP_AVG, "count": GROUP_COUNT,
              "count_distinct": GROUP_COUNT_DISTINCT, "first": GROUP_FIRST, "last": GROUP_LAST, "kurtosis": GROUP_KURTOSIS,
              "skewness": GROUP_SKEWNESS, "stddev": GROUP_STDDEV, "sum_distinct": GROUP_SUM_DISTINCT, "variance": GROUP_VARIANCE,
-             "stddev_pop": GROUP_STDDEV_POP, "var_pop": GROUP_VAR_POP}
+             "stddev_pop": GROUP_STDDEV_POP, "var_pop": GROUP_VAR_POP, "exact_median": GROUP_MEDIAN,
+             "mode": GROUP_MODE}
 # bdf_stat
 STAT_VARIANCE, STAT_VAR_POP, STAT_STDDEV, STAT_STDDEV_POP, STAT_SKEWNESS, STAT_KURTOSIS = range(6)
 STATS = {"variance": STAT_VARIANCE, "var_pop": STAT_VAR_POP, "stddev": STAT_STDDEV, "stddev_pop": STAT_STDDEV_POP,
@@ -241,6 +244,13 @@ def lib() -> C.CDLL:
         "bdf_moments_merge": ([P(MomentRec), P(MomentRec), P(MomentRec)], C.c_int),
         "bdf_distinct": ([vp, C.c_int, i64, P(View), P(DistinctRec)], C.c_int),
         "bdf_distinct_dev": ([vp, vp, P(DistinctRec)], C.c_int),
+        "bdf_percentile": ([vp, C.c_int, i64, P(View), i32, P(C.c_double), P(C.c_double), P(i32)], C.c_int),
+        "bdf_percentile_dev": ([vp, vp, i32, P(C.c_double), P(C.c_double), P(i32)], C.c_int),
+        "bdf_mode": ([vp, C.c_int, i64, P(View), P(u64), P(i64), P(i32)], C.c_int),
+        "bdf_mode_dev": ([vp, vp, P(u64), P(i64), P(i32)], C.c_int),
+        "bdf_uniques_dev": ([vp, vp, P(vp), P(vp)], C.c_int),
+        "bdf_hist_dev": ([vp, vp, i32, P(C.c_double), P(C.c_double), P(i64)], C.c_int),
+        "bdf_hist_density": ([i32, P(C.c_double), P(i64), P(C.c_double)], C.c_int),
         "bdf_expr_check": ([i32, P(i32), i32, P(ExprNode), P(i32), P(i32)], C.c_int),
         "bdf_eval_expr_dev": ([vp, i32, P(vp), i32, P(ExprNode), P(vp)], C.c_int),
         "bdf_eval_expr_agg_dev": ([vp, i32, P(vp), i32, P(ExprNode), P(vp), P(Agg4)], C.c_int),
@@ -356,6 +366,7 @@ EXPORTED_SYMBOLS = [
     "bdf_ipc_write_typed",
     "bdf_parquet_open", "bdf_parquet_describe", "bdf_parquet_column", "bdf_parquet_temporal_column", "bdf_parquet_check", "bdf_parquet_read",
     "bdf_parquet_stats", "bdf_parquet_close", "bdf_parquet_write",
+    "bdf_percentile", "bdf_percentile_dev", "bdf_mode", "bdf_mode_dev", "bdf_uniques_dev", "bdf_hist_dev", "bdf_hist_density",
 ]
 
 

@@ -401,6 +401,22 @@ size_t group_big_scratch_bytes(long long n_rows);
 cudaError_t launch_moments(int dtype, const RedDesc* d, int n, int64_t tiles, Moments* partials, Moments* result, cudaStream_t s);
 int64_t moments_partials(int64_t tiles);
 
+// Column distributions (k_dist.cu).
+int dist_tile_elems(int dtype);
+cudaError_t launch_select_pass(int dtype, int key_bytes, bool compact, const RedDesc* d, int n, int64_t tiles, const unsigned long long* prefixes,
+                               int m, unsigned long long pmask, int shift, unsigned long long* hist, unsigned long long* and_or,
+                               const uint32_t* chosen, void* out, unsigned long long* cursor, int sm_count, cudaStream_t s);
+cudaError_t launch_hist(int dtype, bool range, const RedDesc* d, int n, int64_t tiles, const double* edges, double lo, double hi, int nbins,
+                        unsigned long long* out, int sm_count, cudaStream_t s);
+cudaError_t launch_dist_groups(const uint32_t* starts, long long n_groups, long long n_rows, const uint32_t* pos, long long n_pos, const uint32_t* valid,
+                               uint32_t* first_run, uint32_t* vend, cudaStream_t s);
+cudaError_t launch_dist_runs(const uint32_t* pos, long long n_pos, const uint32_t* starts, long long n_groups, long long n_rows, const uint32_t* first_run,
+                             const uint32_t* vend, long long* counts, unsigned long long* best, cudaStream_t s);
+cudaError_t launch_dist_mode(const unsigned long long* best, long long n_groups, const uint32_t* first_run, const uint32_t* pos, uint32_t* row,
+                             uint32_t* row_valid, long long* freq, cudaStream_t s);
+cudaError_t launch_dist_median(int dtype, const void* sval, const uint32_t* starts, long long n_groups, const uint32_t* vend, double* out,
+                               uint32_t* out_valid, cudaStream_t s);
+
 // Joins (k_join.cu).
 int join_tile_rows();
 cudaError_t launch_join_count(int n_keys, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,

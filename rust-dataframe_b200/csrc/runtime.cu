@@ -35,6 +35,7 @@
 #include "common.cuh"
 #include "comm.cuh"
 #include "moments.cuh"
+#include "dist.cuh"
 #include "json_parse.cuh"
 #define PQ_HOST_PLAN
 #include "parquet_decode.cuh"
@@ -2025,6 +2026,69 @@ static int distinct_sum(bdf_ctx* c, const DistinctRuns& dr, const uint32_t* d_fi
     return BDF_OK;
 }
 
+// Median / mode per group (k_dist.cu) over distinct_runs: in the second sort each group's valid values come first, in key order.
+// vend: the end of every group's valid prefix; first_run: the first distinct run of every group (mode only).
+static int dist_group_bounds(bdf_ctx* c, const DistinctRuns& dr, const uint32_t* d_starts, int64_t n_groups, int64_t n, bool runs,
+                             Scratch<uint32_t>* first_run, Scratch<uint32_t>* vend) {
+    const size_t bytes = (size_t)std::max<int64_t>(n_groups, 1) * sizeof(uint32_t);
+    cudaError_t e = vend->alloc(c, bytes);
+    if (e == cudaSuccess && runs) e = first_run->alloc(c, bytes);
+    const int64_t n_pos = dr.pos->chunks.empty() ? 0 : dr.pos->chunks[0].len;
+    if (n_pos) wait_groups(c->s_compute, dr.pos.get(), 0, 1);
+    wait_groups(c->s_compute, dr.sval.get(), 0, 1);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_GROUP, BDF_U32, n_groups, n_groups * 12);
+        e = launch_dist_groups(d_starts, n_groups, n, runs && n_pos ? (const uint32_t*)dr.pos->chunks[0].values : nullptr, n_pos,
+                               dr.sval->chunks[0].validity, runs ? first_run->get() : nullptr, vend->get(), c->s_compute);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "distribution group bounds");
+    return BDF_OK;
+}
+
+static int group_median(bdf_ctx* c, const DistinctRuns& dr, const uint32_t* d_starts, int64_t n_groups, int64_t n, bdf_col** out) {
+    ColOwner res(c);
+    TRY(col_alloc(c, BDF_F64, {ChunkPlan{n_groups, true}}, nullptr, 0, res.out()));
+    Scratch<uint32_t> first_run, vend;
+    TRY(dist_group_bounds(c, dr, d_starts, n_groups, n, false, &first_run, &vend));
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_GROUP, BDF_F64, n_groups, n_groups * (4 + 4 + 2 * dtype_width(dr.sval->dtype) + 8));
+        e = launch_dist_median(dr.sval->dtype, dr.sval->chunks[0].values, d_starts, n_groups, vend, (double*)res->chunks[0].values,
+                               res->chunks[0].validity, c->s_compute);
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, res.get());
+    if (e != cudaSuccess) return fail_cuda(e, "group median");
+    res->null_counts[0] = -1;   // learnt on demand (ensure_null_counts)
+    *out = res.release();
+    return BDF_OK;
+}
+
+// The mode of every group: the sorted row of its most frequent (then smallest) distinct run, gathered from the sorted values; d_freq
+// (may be null): the run's row count per group, 0 without a valid value.
+static int group_mode(bdf_ctx* c, const DistinctRuns& dr, const uint32_t* d_starts, int64_t n_groups, int64_t n, bdf_col** out, long long* d_freq) {
+    Scratch<uint32_t> first_run, vend;
+    TRY(dist_group_bounds(c, dr, d_starts, n_groups, n, true, &first_run, &vend));
+    const int64_t n_pos = dr.pos->chunks.empty() ? 0 : dr.pos->chunks[0].len;
+    const uint32_t* pos = n_pos ? (const uint32_t*)dr.pos->chunks[0].values : nullptr;
+    ColOwner rows(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n_groups, true}}, nullptr, 0, rows.out()));
+    Scratch<unsigned long long> best;
+    cudaError_t e = best.alloc(c, (size_t)std::max<int64_t>(n_groups, 1) * 8);
+    if (e == cudaSuccess) e = cudaMemsetAsync(best, 0, (size_t)std::max<int64_t>(n_groups, 1) * 8, c->s_compute);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_GROUP, BDF_I64, n_pos, n_pos * 8 + n_groups * 16);
+        e = launch_dist_runs(pos, n_pos, d_starts, n_groups, n, first_run, vend, nullptr, best, c->s_compute);
+    }
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_GROUP, BDF_U32, n_groups, n_groups * 20);
+        e = launch_dist_mode(best, n_groups, first_run, pos, (uint32_t*)rows->chunks[0].values, rows->chunks[0].validity, d_freq, c->s_compute);
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, rows.get());
+    if (e != cudaSuccess) return fail_cuda(e, "group mode");
+    rows->null_counts[0] = -1;
+    return take_dev(c, dr.sval.get(), rows.get(), out);
+}
+
 static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int n_aggs, const bdf_group_agg* aggs, bdf_col** out_keys, bdf_col** out,
                         int64_t* n_groups_out) {
     if (n_keys < 1 || n_keys > 16) return fail(BDF_INVALID, "1..16 group key columns");
@@ -2037,7 +2101,9 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
         const bdf_col* v = aggs[j].column;
         if (!v) return fail(BDF_INVALID, "null value column");
         if (v->dtype < 0 || v->dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "aggregated columns must be numeric");
-        if (aggs[j].function < BDF_GROUP_SUM || aggs[j].function > BDF_GROUP_VAR_POP) return fail(BDF_UNSUPPORTED, "unknown group function %d", aggs[j].function);
+        const int fn = aggs[j].function;
+        if (!((fn >= BDF_GROUP_SUM && fn <= BDF_GROUP_VAR_POP) || fn == BDF_GROUP_MEDIAN || fn == BDF_GROUP_MODE))
+            return fail(BDF_UNSUPPORTED, "unknown group function %d", fn);
         if (aggs[j].function == BDF_GROUP_AVG && (v->dtype == BDF_I64 || v->dtype == BDF_U64)) return fail(BDF_UNSUPPORTED, "avg needs f64: From<T::Native>");
         if (v->total_len != keys[0]->total_len) return fail(BDF_LENGTH_MISMATCH, "key and value columns have different lengths");
     }
@@ -2205,6 +2271,19 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
             TRY(distinct_sum(c, dr, (const uint32_t*)dstarts->chunks[0].values, n_groups, res[j].out()));
         }
     }
+
+    // median / mode: the same second sort; the median reads the two middle valid values of every group, the mode counts the distinct
+    // runs (k_dist.cu)
+    for (int j = 0; j < n_aggs; j++) {
+        const int fn = aggs[j].function;
+        if (fn != BDF_GROUP_MEDIAN && fn != BDF_GROUP_MODE) continue;
+        std::vector<const bdf_col*> sorted_keys;
+        for (const ColOwner& s : runs.sorted) sorted_keys.push_back(s.get());
+        DistinctRuns dr(c);
+        TRY(distinct_runs(c, n_keys, keys, sorted_keys, aggs[j].column, runs.iota.get(), n, &dr));
+        if (fn == BDF_GROUP_MEDIAN) TRY(group_median(c, dr, d_starts, n_groups, n, res[j].out()));
+        else TRY(group_mode(c, dr, d_starts, n_groups, n, res[j].out(), nullptr));
+    }
     for (int k = 0; k < n_keys; k++) out_keys[k] = runs.distinct[k].release();
     for (int j = 0; j < n_aggs; j++) out[j] = res[j].release();
     if (n_groups_out) *n_groups_out = n_groups;
@@ -2291,6 +2370,21 @@ static int moments_dev(bdf_ctx* c, const bdf_col* col, Moments* out) {
     return BDF_OK;
 }
 
+// The distinct runs of a whole column of n > 0 rows, handled as one group (starts: that group's start, 0).
+static int column_runs(bdf_ctx* c, const bdf_col* x, DistinctRuns* dr, ColOwner* starts) {
+    const int64_t n = x->total_len;
+    ColOwner iota(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, iota.out()));
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{1, false}}, nullptr, 0, starts->out()));
+    c->launches++;
+    cudaError_t e = launch_iota((uint32_t*)iota->chunks[0].values, n, c->sm_count, c->s_compute);
+    if (e == cudaSuccess) e = cudaMemsetAsync((*starts)->chunks[0].values, 0, sizeof(uint32_t), c->s_compute);   // the one group starts at 0
+    if (e == cudaSuccess) e = finish_single_group(c, iota.get());
+    if (e == cudaSuccess) e = finish_single_group(c, starts->get());
+    if (e != cudaSuccess) return fail_cuda(e, "distinct iota");
+    return distinct_runs(c, 0, nullptr, {}, x, iota.get(), n, dr);
+}
+
 // count_distinct / sum_distinct of a whole column: the group-by's distinct machinery with the column as one group.
 static int distinct_dev(bdf_ctx* c, const bdf_col* x, bdf_distinct_rec* out) {
     if (x->dtype < 0 || x->dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "count_distinct / sum_distinct need a numeric column");
@@ -2298,23 +2392,318 @@ static int distinct_dev(bdf_ctx* c, const bdf_col* x, bdf_distinct_rec* out) {
         return fail(BDF_UNSUPPORTED, "distinct values need every row of the column on one GPU (as sort / group-by / join): use a one-GPU context");
     const int64_t n = x->total_len;
     if (n == 0) { *out = bdf_distinct_rec{0, 0}; return BDF_OK; }
-    ColOwner iota(c), first(c), sum(c);
-    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, iota.out()));
-    TRY(col_alloc(c, BDF_U32, {ChunkPlan{1, false}}, nullptr, 0, first.out()));
-    c->launches++;
-    cudaError_t e = launch_iota((uint32_t*)iota->chunks[0].values, n, c->sm_count, c->s_compute);
-    if (e == cudaSuccess) e = cudaMemsetAsync(first->chunks[0].values, 0, sizeof(uint32_t), c->s_compute);   // the one group starts at 0
-    if (e == cudaSuccess) e = finish_single_group(c, iota.get());
-    if (e == cudaSuccess) e = finish_single_group(c, first.get());
-    if (e != cudaSuccess) return fail_cuda(e, "distinct iota");
+    ColOwner first(c), sum(c);
     DistinctRuns dr(c);
-    TRY(distinct_runs(c, 0, nullptr, {}, x, iota.get(), n, &dr));
+    TRY(column_runs(c, x, &dr, &first));
     const int64_t count = dr.pos->chunks.empty() ? 0 : dr.pos->chunks[0].len;
     TRY(distinct_sum(c, dr, (const uint32_t*)first->chunks[0].values, 1, sum.out()));
     uint64_t bits = 0;
     CK(cudaMemcpyAsync(&bits, sum->chunks[0].values, (size_t)dtype_width(x->dtype), cudaMemcpyDeviceToHost, c->s_compute));
     CK(cudaStreamSynchronize(c->s_compute));
     *out = bdf_distinct_rec{count, bits};
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// distributions (k_dist.cu, dist.cuh): exact percentiles by an MSD radix select, the histogram, mode and uniques
+
+static int dist_check(bdf_ctx* c, const bdf_col* x) {
+    if (x->dtype < 0 || x->dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "the distributions need a numeric column");
+    if (is_global(c)) return fail(BDF_UNSUPPORTED, "the distributions need every row of the column on one GPU: use a one-GPU context");
+    if (x->total_len > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
+    return BDF_OK;
+}
+
+// The chunks of col as k_reduce descriptors with tiles of dist_tile_elems(dtype) elements.
+static int dist_descs(bdf_ctx* c, const bdf_col* col, const RedDesc** d, int64_t* tiles) {
+    const int64_t n = (int64_t)col->chunks.size();
+    wait_groups(c->s_compute, col, 0, n);
+    const int tile = dist_tile_elems(col->dtype);
+    void *hp = nullptr, *dp = nullptr;
+    TRY(ring_alloc(c, (size_t)std::max<int64_t>(n, 1) * sizeof(RedDesc), &hp, &dp));
+    RedDesc* hd = (RedDesc*)hp;
+    int64_t t = 0;
+    for (int64_t i = 0; i < n; i++) {
+        const DevChunk& ch = col->chunks[i];
+        hd[i].in = ch.values; hd[i].vin = ch.validity; hd[i].len = ch.len; hd[i].tile0 = t; hd[i].off = ch.bit_off; hd[i].pad = 0;
+        t += (ch.len + tile - 1) / tile;
+    }
+    CK(desc_upload(c, dp, hd, (size_t)n * sizeof(RedDesc)));
+    *d = (const RedDesc*)dp;
+    *tiles = t;
+    return BDF_OK;
+}
+
+// The value a sort key stands for, read as f64 (+0.0 for a zero, the positive quiet NaN for NaN).
+static double key_value(int dtype, uint64_t k) {
+    switch (dtype) {
+        case BDF_I8: return (double)(int8_t)(uint8_t)(k ^ 0x80u);
+        case BDF_I16: return (double)(int16_t)(uint16_t)(k ^ 0x8000u);
+        case BDF_I32: return (double)(int32_t)(uint32_t)(k ^ 0x80000000u);
+        case BDF_I64: return (double)(int64_t)(k ^ (1ull << 63));
+        case BDF_F32: {
+            const uint32_t b = (k >> 31) ? (uint32_t)k ^ 0x80000000u : ~(uint32_t)k;
+            float f;
+            memcpy(&f, &b, sizeof f);
+            return dist_canonical((double)f);
+        }
+        case BDF_F64: {
+            const uint64_t b = (k >> 63) ? k ^ (1ull << 63) : ~k;
+            double f;
+            memcpy(&f, &b, sizeof f);
+            return dist_canonical(f);
+        }
+        default: return (double)k;
+    }
+}
+
+constexpr int kMaxPercentiles = 1024;
+
+// MSD radix select: the keys of the valid values at the given ranks (0-based in key order).  ranks_of(n_valid) gives the wanted ranks,
+// ascending and distinct, once the first pass has counted the valid values; n_valid = 0 selects nothing.
+//   A level histograms one 8-bit digit of every candidate (a key whose decided high bits equal a target's prefix), then every target
+//   takes the bucket holding its rank.  Bits below the digit on which every candidate agrees (their AND equals their OR there) are
+//   decided at once.  When the chosen buckets hold fewer keys than the candidates, those keys are compacted into a scratch that the
+//   next level reads instead; otherwise (a column of one value, or every bucket chosen) the next level reads the same source again.
+static int select_keys(bdf_ctx* c, const bdf_col* col, const std::function<std::vector<int64_t>(int64_t)>& ranks_of, int max_targets,
+                       std::vector<uint64_t>* keys, int64_t* n_valid) {
+    const int dt = col->dtype, w = dtype_width(dt), kb = w <= 4 ? 4 : 8;
+    const RedDesc* cd = nullptr;
+    int64_t col_tiles = 0;
+    TRY(dist_descs(c, col, &cd, &col_tiles));
+    const int64_t col_bytes = reduce_bytes(col, 0, (int64_t)col->chunks.size());
+    const size_t max_bins = (size_t)max_targets * 256;
+    Scratch<unsigned long long> hist, small, d_pre;   // small: AND, OR, cursor
+    Scratch<uint32_t> chosen;
+    CK(hist.alloc(c, max_bins * 8));
+    CK(small.alloc(c, 3 * 8));
+    CK(d_pre.alloc(c, (size_t)max_targets * 8));
+    CK(chosen.alloc(c, max_bins / 8));
+    std::unique_ptr<Scratch<void>> cur;   // the candidates of the current source when it is a scratch
+    const RedDesc* src = cd;              // the current source: the column (key_bytes 0) or the scratch (raw keys)
+    int src_n = (int)col->chunks.size(), src_kb = 0;
+    int64_t src_tiles = col_tiles, src_bytes = col_bytes, cand = 0;
+    struct Target { uint64_t prefix; int64_t rank; };
+    std::vector<Target> tg;
+    std::vector<uint64_t> pre{0}, hh(max_bins), ao(2);
+    uint64_t pmask = 0;
+    int s_top = 8 * w;   // bits at and above s_top are decided (zero above the type's width)
+    for (int level = 0; s_top > 0; level++) {
+        const int shift = std::max(0, s_top - 8), m = (int)pre.size();
+        const uint64_t ao0[3] = {~0ull, 0ull, 0ull};
+        CK(cudaMemcpyAsync(d_pre, pre.data(), (size_t)m * 8, cudaMemcpyHostToDevice, c->s_compute));
+        CK(cudaMemcpyAsync(small, ao0, sizeof ao0, cudaMemcpyHostToDevice, c->s_compute));
+        CK(cudaMemsetAsync(hist, 0, (size_t)m * 256 * 8, c->s_compute));
+        {
+            LaunchTimer t(c, BDF_K_SELECT, dt, src_kb ? cand : col->total_len, src_bytes);
+            CK(launch_select_pass(dt, src_kb, false, src, src_n, src_tiles, d_pre, m, pmask, shift, hist, small, nullptr, nullptr, nullptr,
+                                  c->sm_count, c->s_compute));
+        }
+        CK(cudaMemcpyAsync(hh.data(), hist, (size_t)m * 256 * 8, cudaMemcpyDeviceToHost, c->s_compute));
+        CK(cudaMemcpyAsync(ao.data(), small, 2 * 8, cudaMemcpyDeviceToHost, c->s_compute));
+        CK(cudaStreamSynchronize(c->s_compute));
+        if (level == 0) {
+            cand = 0;
+            for (int d = 0; d < 256; d++) cand += (int64_t)hh[d];
+            *n_valid = cand;
+            if (!cand) return BDF_OK;
+            for (int64_t r : ranks_of(cand)) tg.push_back(Target{0, r});
+        }
+        // every target takes the bucket of its rank inside its class (targets ascend, so do their prefixes)
+        std::vector<uint32_t> chosen_bits((size_t)m * 8, 0u);
+        int64_t kept = 0;
+        size_t ci = 0;
+        for (Target& t : tg) {
+            while (pre[ci] != t.prefix) ci++;
+            const uint64_t* h = &hh[ci * 256];
+            int64_t cum = 0;
+            int d = 0;
+            while (cum + (int64_t)h[d] <= t.rank) cum += (int64_t)h[d++];
+            t.rank -= cum;
+            t.prefix |= (uint64_t)d << shift;
+            const size_t bin = ci * 256 + (size_t)d;
+            if (!((chosen_bits[bin >> 5] >> (bin & 31)) & 1u)) {
+                chosen_bits[bin >> 5] |= 1u << (bin & 31);
+                kept += (int64_t)h[d];
+            }
+        }
+        // bits below the digit on which every candidate agrees are decided too
+        const uint64_t low = shift ? (1ull << shift) - 1 : 0ull, diff = (ao[0] ^ ao[1]) & low;
+        const int new_top = diff ? 64 - __builtin_clzll(diff) : 0;
+        const uint64_t agreed = low & ~(new_top ? (new_top == 64 ? ~0ull : (1ull << new_top) - 1) : 0ull);
+        for (Target& t : tg) t.prefix |= ao[0] & agreed;
+        if (new_top == 0) break;
+        if (kept < cand) {   // compact the chosen buckets (this level's prefixes and digit)
+            std::unique_ptr<Scratch<void>> next(new Scratch<void>());
+            CK(next->alloc(c, (size_t)kept * kb));
+            CK(cudaMemcpyAsync(chosen, chosen_bits.data(), chosen_bits.size() * 4, cudaMemcpyHostToDevice, c->s_compute));
+            CK(cudaMemsetAsync(small.get() + 2, 0, 8, c->s_compute));
+            {
+                LaunchTimer t(c, BDF_K_SELECT, dt, src_kb ? cand : col->total_len, src_bytes + kept * kb);
+                CK(launch_select_pass(dt, src_kb, true, src, src_n, src_tiles, d_pre, m, pmask, shift, nullptr, nullptr, chosen, next->get(),
+                                      small.get() + 2, c->sm_count, c->s_compute));
+            }
+            void *hp = nullptr, *dp = nullptr;
+            TRY(ring_alloc(c, sizeof(RedDesc), &hp, &dp));
+            RedDesc* hd = (RedDesc*)hp;
+            const int tile = kThreads * kUnroll * (16 / kb);
+            hd->in = next->get(); hd->vin = nullptr; hd->len = kept; hd->tile0 = 0; hd->off = 0; hd->pad = 0;
+            CK(desc_upload(c, dp, hd, sizeof(RedDesc)));
+            cur = std::move(next);   // the previous scratch is freed in stream order, after the compaction that read it
+            src = (const RedDesc*)dp; src_n = 1; src_kb = kb;
+            src_tiles = (kept + tile - 1) / tile;
+            src_bytes = kept * kb;
+            cand = kept;
+        }
+        pre.clear();
+        for (const Target& t : tg)
+            if (pre.empty() || pre.back() != t.prefix) pre.push_back(t.prefix);
+        s_top = new_top;
+        pmask = ~((1ull << s_top) - 1) & (kb == 4 ? 0xffffffffull : ~0ull);
+    }
+    keys->clear();
+    for (const Target& t : tg) keys->push_back(t.prefix);
+    return BDF_OK;
+}
+
+static int percentile_dev(bdf_ctx* c, const bdf_col* col, int n_p, const double* p, double* out, int32_t* is_some) {
+    TRY(dist_check(c, col));
+    std::vector<double> pos((size_t)n_p);
+    std::vector<int64_t> ranks;
+    auto ranks_of = [&](int64_t n) {
+        for (int i = 0; i < n_p; i++) {
+            pos[i] = dist_mul((double)(n - 1), p[i]);
+            ranks.push_back((int64_t)floor(pos[i]));
+            ranks.push_back((int64_t)ceil(pos[i]));
+        }
+        std::sort(ranks.begin(), ranks.end());
+        ranks.erase(std::unique(ranks.begin(), ranks.end()), ranks.end());
+        return ranks;
+    };
+    std::vector<uint64_t> keys;
+    int64_t n_valid = 0;
+    TRY(select_keys(c, col, ranks_of, 2 * n_p, &keys, &n_valid));
+    for (int i = 0; i < n_p; i++) {
+        if (!n_valid) { out[i] = 0.0; is_some[i] = 0; continue; }
+        const double lo = floor(pos[i]), hi = ceil(pos[i]);
+        const size_t a = std::lower_bound(ranks.begin(), ranks.end(), (int64_t)lo) - ranks.begin();
+        const size_t b = std::lower_bound(ranks.begin(), ranks.end(), (int64_t)hi) - ranks.begin();
+        out[i] = dist_interp(key_value(col->dtype, keys[a]), key_value(col->dtype, keys[b]), pos[i], lo, hi);
+        is_some[i] = 1;
+    }
+    return BDF_OK;
+}
+
+static int mode_dev(bdf_ctx* c, const bdf_col* x, uint64_t* bits, int64_t* freq, int32_t* is_some) {
+    TRY(dist_check(c, x));
+    const int64_t n = x->total_len;
+    if (n == 0) { *bits = 0; *freq = 0; *is_some = 0; return BDF_OK; }
+    ColOwner first(c), val(c);
+    DistinctRuns dr(c);
+    TRY(column_runs(c, x, &dr, &first));
+    Scratch<long long> d_freq;
+    CK(d_freq.alloc(c, sizeof(long long)));
+    TRY(group_mode(c, dr, (const uint32_t*)first->chunks[0].values, 1, n, val.out(), d_freq));
+    uint64_t b = 0;
+    long long f = 0;
+    wait_groups(c->s_compute, val.get(), 0, 1);
+    CK(cudaMemcpyAsync(&b, val->chunks[0].values, (size_t)dtype_width(x->dtype), cudaMemcpyDeviceToHost, c->s_compute));
+    CK(cudaMemcpyAsync(&f, d_freq, sizeof f, cudaMemcpyDeviceToHost, c->s_compute));
+    CK(cudaStreamSynchronize(c->s_compute));
+    *bits = f ? b : 0;
+    *freq = f;
+    *is_some = f ? 1 : 0;
+    return BDF_OK;
+}
+
+static int uniques_dev(bdf_ctx* c, const bdf_col* x, bdf_col** values, bdf_col** counts) {
+    TRY(dist_check(c, x));
+    const int64_t n = x->total_len;
+    ColOwner v(c), cnt(c);
+    if (n == 0) {
+        TRY(col_alloc(c, x->dtype, {ChunkPlan{0, false}}, nullptr, 0, v.out()));
+        if (counts) TRY(col_alloc(c, BDF_I64, {ChunkPlan{0, false}}, nullptr, 0, cnt.out()));
+    } else {
+        ColOwner first(c);
+        DistinctRuns dr(c);
+        TRY(column_runs(c, x, &dr, &first));
+        TRY(filter_dev(c, dr.sval.get(), dr.dhead.get(), v.out()));
+        if (counts) {
+            const int64_t n_pos = dr.pos->chunks.empty() ? 0 : dr.pos->chunks[0].len;
+            const uint32_t* d_starts = (const uint32_t*)first->chunks[0].values;
+            Scratch<uint32_t> first_run, vend;
+            TRY(dist_group_bounds(c, dr, d_starts, 1, n, true, &first_run, &vend));
+            TRY(col_alloc(c, BDF_I64, {ChunkPlan{n_pos, false}}, nullptr, 0, cnt.out()));
+            cudaError_t e;
+            {
+                LaunchTimer t(c, BDF_K_GROUP, BDF_I64, n_pos, n_pos * 12);
+                e = launch_dist_runs(n_pos ? (const uint32_t*)dr.pos->chunks[0].values : nullptr, n_pos, d_starts, 1, n, first_run, vend,
+                                     n_pos ? (long long*)cnt->chunks[0].values : nullptr, nullptr, c->s_compute);
+            }
+            if (e == cudaSuccess) e = finish_single_group(c, cnt.get());
+            if (e != cudaSuccess) return fail_cuda(e, "uniques counts");
+        }
+    }
+    *values = v.release();
+    if (counts) *counts = cnt.release();
+    return BDF_OK;
+}
+
+// numpy's linspace of the bin edges (dist.cuh's operations: one rounding each).
+static void hist_edges(double lo, double hi, int nbins, double* edges) {
+    const double delta = dist_sub(hi, lo), step = delta / (double)nbins;
+    for (int i = 0; i < nbins; i++)
+        edges[i] = step == 0.0 ? dist_add(dist_mul((double)i / (double)nbins, delta), lo) : dist_add(dist_mul((double)i, step), lo);
+    edges[nbins] = hi;
+}
+
+static int hist_dev(bdf_ctx* c, const bdf_col* x, int nbins, const double* range, double* edges_out, int64_t* counts_out) {
+    TRY(dist_check(c, x));
+    double lo = 0.0, hi = 1.0;
+    if (range) {
+        lo = range[0];
+        hi = range[1];
+        if (lo > hi) return fail(BDF_INVALID, "max must be larger than min in range parameter.");
+        if (!std::isfinite(lo) || !std::isfinite(hi)) return fail(BDF_INVALID, "supplied range of [%.17g, %.17g] is not finite", lo, hi);
+    }
+    const RedDesc* d = nullptr;
+    int64_t tiles = 0;
+    TRY(dist_descs(c, x, &d, &tiles));
+    const int64_t bytes = reduce_bytes(x, 0, (int64_t)x->chunks.size());
+    Scratch<unsigned long long> dev;
+    Scratch<double> d_edges;
+    CK(dev.alloc(c, (size_t)std::max(nbins, 2) * 8));   // the range pass writes two keys
+    CK(d_edges.alloc(c, (size_t)(nbins + 1) * 8));
+    if (!range) {   // [min, max] of the valid non-NaN values
+        const unsigned long long init[2] = {~0ull, 0ull};
+        unsigned long long mm[2];
+        CK(cudaMemcpyAsync(dev, init, sizeof init, cudaMemcpyHostToDevice, c->s_compute));
+        {
+            LaunchTimer t(c, BDF_K_HIST, x->dtype, x->total_len, bytes);
+            CK(launch_hist(x->dtype, true, d, (int)x->chunks.size(), tiles, nullptr, 0.0, 0.0, 0, dev, c->sm_count, c->s_compute));
+        }
+        CK(cudaMemcpyAsync(mm, dev, sizeof mm, cudaMemcpyDeviceToHost, c->s_compute));
+        CK(cudaStreamSynchronize(c->s_compute));
+        if (mm[0] <= mm[1]) {
+            lo = key_value(x->dtype, mm[0]);
+            hi = key_value(x->dtype, mm[1]);
+            if (!std::isfinite(lo) || !std::isfinite(hi)) return fail(BDF_INVALID, "autodetected range of [%.17g, %.17g] is not finite", lo, hi);
+        }
+    }
+    if (lo == hi) { lo = dist_sub(lo, 0.5); hi = dist_add(hi, 0.5); }
+    std::vector<double> edges((size_t)nbins + 1);
+    std::vector<int64_t> counts((size_t)nbins);
+    hist_edges(lo, hi, nbins, edges.data());
+    CK(cudaMemcpyAsync(d_edges, edges.data(), edges.size() * 8, cudaMemcpyHostToDevice, c->s_compute));
+    CK(cudaMemsetAsync(dev, 0, (size_t)nbins * 8, c->s_compute));
+    {
+        LaunchTimer t(c, BDF_K_HIST, x->dtype, x->total_len, bytes);
+        CK(launch_hist(x->dtype, false, d, (int)x->chunks.size(), tiles, d_edges, lo, hi, nbins, dev, c->sm_count, c->s_compute));
+    }
+    CK(cudaMemcpyAsync(counts.data(), dev, (size_t)nbins * 8, cudaMemcpyDeviceToHost, c->s_compute));
+    CK(cudaStreamSynchronize(c->s_compute));
+    memcpy(edges_out, edges.data(), edges.size() * 8);
+    memcpy(counts_out, counts.data(), counts.size() * 8);
     return BDF_OK;
 }
 
@@ -5988,6 +6377,71 @@ int bdf_distinct_dev(bdf_ctx* c, const bdf_col* in, bdf_distinct_rec* out) {
     return distinct_dev(c, in, out);
 }
 
+static const char* kDistFleet = "the distributions need every row of the column on one GPU: use a one-GPU context";
+
+static int check_percentiles(int32_t n_p, const double* p, const double* out, const int32_t* is_some) {
+    if (!p || !out || !is_some) return fail(BDF_INVALID, "null argument");
+    if (n_p < 1 || n_p > kMaxPercentiles) return fail(BDF_INVALID, "1..%d percentiles per call", kMaxPercentiles);
+    for (int32_t i = 0; i < n_p; i++)
+        if (!(p[i] >= 0.0 && p[i] <= 1.0)) return fail(BDF_INVALID, "percentile %d is %g: it must be in [0, 1]", i, p[i]);
+    return BDF_OK;
+}
+
+static int check_hist(int32_t nbins, const double* edges, const int64_t* counts) {
+    if (!edges || !counts) return fail(BDF_INVALID, "null argument");
+    if (nbins < 1 || nbins > (1 << 24)) return fail(BDF_INVALID, "nbins must be in 1..2^24, not %d", nbins);
+    return BDF_OK;
+}
+
+int bdf_percentile_dev(bdf_ctx* c, const bdf_col* in, int32_t n_p, const double* p, double* out, int32_t* is_some) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "%s", kDistFleet);
+    ENTER(c);
+    if (!in) return fail(BDF_INVALID, "null argument");
+    TRY(check_percentiles(n_p, p, out, is_some));
+    std::vector<double> o((size_t)n_p);
+    std::vector<int32_t> some((size_t)n_p);
+    TRY(percentile_dev(c, in, n_p, p, o.data(), some.data()));
+    memcpy(out, o.data(), o.size() * sizeof(double));
+    memcpy(is_some, some.data(), some.size() * sizeof(int32_t));
+    return BDF_OK;
+}
+
+int bdf_mode_dev(bdf_ctx* c, const bdf_col* in, uint64_t* bits, int64_t* freq, int32_t* is_some) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "%s", kDistFleet);
+    ENTER(c);
+    if (!in || !bits || !freq || !is_some) return fail(BDF_INVALID, "null argument");
+    uint64_t b = 0;
+    int64_t f = 0;
+    int32_t some = 0;
+    TRY(mode_dev(c, in, &b, &f, &some));
+    *bits = b; *freq = f; *is_some = some;
+    return BDF_OK;
+}
+
+int bdf_uniques_dev(bdf_ctx* c, const bdf_col* in, bdf_col** values, bdf_col** counts) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "%s", kDistFleet);
+    ENTER(c);
+    if (!in || !values) return fail(BDF_INVALID, "null argument");
+    return uniques_dev(c, in, values, counts);
+}
+
+int bdf_hist_dev(bdf_ctx* c, const bdf_col* in, int32_t nbins, const double* range, double* edges, int64_t* counts) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "%s", kDistFleet);
+    ENTER(c);
+    if (!in) return fail(BDF_INVALID, "null argument");
+    TRY(check_hist(nbins, edges, counts));
+    return hist_dev(c, in, nbins, range, edges, counts);
+}
+
+int bdf_hist_density(int32_t nbins, const double* edges, const int64_t* counts, double* out) {
+    TRY(check_hist(nbins, edges, counts));
+    if (!out) return fail(BDF_INVALID, "null argument");
+    int64_t total = 0;
+    for (int32_t i = 0; i < nbins; i++) total += counts[i];
+    for (int32_t i = 0; i < nbins; i++) out[i] = ((double)counts[i] / dist_sub(edges[i + 1], edges[i])) / (double)total;
+    return BDF_OK;
+}
+
 int bdf_moments_stat(const bdf_moment_rec* m, int stat, double* out, int32_t* is_some) {
     if (!m || !out || !is_some) return fail(BDF_INVALID, "null argument");
     if (stat < BDF_STAT_VARIANCE || stat > BDF_STAT_KURTOSIS) return fail(BDF_INVALID, "unknown statistic %d", stat);
@@ -6462,6 +6916,35 @@ int bdf_distinct(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, bdf_disti
     if (is_global(c))
         return fail(BDF_UNSUPPORTED, "distinct values need every row of the column on one GPU (as sort / group-by / join): use a one-GPU context");
     return host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) { return distinct_dev(c, cols[0], out); });
+}
+
+int bdf_percentile(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, int32_t n_p, const double* p, double* out, int32_t* is_some) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "%s", kDistFleet);
+    ENTER(c);
+    TRY(check_stat_dtype(dtype));
+    if (n < 0 || (n && !in)) return fail(BDF_INVALID, "bad arguments");
+    TRY(check_percentiles(n_p, p, out, is_some));
+    if (is_global(c)) return fail(BDF_UNSUPPORTED, "%s", kDistFleet);
+    std::vector<double> o((size_t)n_p);
+    std::vector<int32_t> some((size_t)n_p);
+    TRY(host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) { return percentile_dev(c, cols[0], n_p, p, o.data(), some.data()); }));
+    memcpy(out, o.data(), o.size() * sizeof(double));
+    memcpy(is_some, some.data(), some.size() * sizeof(int32_t));
+    return BDF_OK;
+}
+
+int bdf_mode(bdf_ctx* c, int dtype, int64_t n, const bdf_view* in, uint64_t* bits, int64_t* freq, int32_t* is_some) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "%s", kDistFleet);
+    ENTER(c);
+    TRY(check_stat_dtype(dtype));
+    if (n < 0 || (n && !in) || !bits || !freq || !is_some) return fail(BDF_INVALID, "bad arguments");
+    if (is_global(c)) return fail(BDF_UNSUPPORTED, "%s", kDistFleet);
+    uint64_t b = 0;
+    int64_t f = 0;
+    int32_t some = 0;
+    TRY(host_call(c, {UploadSpec{dtype, n, in}}, [&](bdf_col* const* cols) { return mode_dev(c, cols[0], &b, &f, &some); }));
+    *bits = b; *freq = f; *is_some = some;
+    return BDF_OK;
 }
 
 // ---- measurement support -------------------------------------------------------------------------

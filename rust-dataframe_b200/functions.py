@@ -361,8 +361,55 @@ class AggregateFunctions:
         dtype, r = AggregateFunctions._distinct(arrays, dtype, ctx)
         return _scalar_from_bits(dtype, r.sum)
 
+    # -- distributions (include/b200df.h "distributions") --
+    @staticmethod
+    def percentile(arrays: Chunks, p, dtype: Optional[int] = None, ctx=None):
+        """Spark's exact percentile of the valid values at p in [0, 1] (a float, or a sequence of up to 1024 of them): a float, or
+        ``None`` without a valid value; a list for a sequence."""
+        ctx = ctx or N.default_context()
+        if dtype is None:
+            dtype = _dtype_of(arrays) if len(arrays) else N_I64_FALLBACK
+        ps, out, some = _percentile_args(p)
+        N.raise_for_status(N.lib().bdf_percentile(ctx.handle, dtype, len(arrays), N.make_views(arrays), len(np.atleast_1d(p)), ps, out, some))
+        return _percentile_result(p, out, some)
+
+    @staticmethod
+    def median(arrays: Chunks, dtype: Optional[int] = None, ctx=None) -> Optional[float]:
+        return AggregateFunctions.percentile(arrays, 0.5, dtype, ctx)
+
+    @staticmethod
+    def mode(arrays: Chunks, dtype: Optional[int] = None, ctx=None):
+        """The most frequent valid value (ties: the smallest), in the dtype of the column; ``None`` without a valid value."""
+        ctx = ctx or N.default_context()
+        if dtype is None:
+            dtype = _dtype_of(arrays) if len(arrays) else N_I64_FALLBACK
+        bits, freq, some = C.c_uint64(0), C.c_int64(0), C.c_int32(0)
+        N.raise_for_status(N.lib().bdf_mode(ctx.handle, dtype, len(arrays), N.make_views(arrays), C.byref(bits), C.byref(freq), C.byref(some)))
+        return _scalar_from_bits(dtype, bits.value) if some.value else None
+
 
 N_I64_FALLBACK = 3  # Int64: only used to type an empty Vec (results do not depend on it)
+
+
+def _percentile_args(p):
+    ps = np.ascontiguousarray(np.atleast_1d(np.asarray(p, dtype=np.float64)))
+    n = len(ps)
+    return ps.ctypes.data_as(C.POINTER(C.c_double)), (C.c_double * max(n, 1))(), (C.c_int32 * max(n, 1))()
+
+
+def _percentile_result(p, out, some):
+    vals = [out[i] if some[i] else None for i in range(len(np.atleast_1d(p)))]
+    return vals if np.ndim(p) else vals[0]
+
+
+def hist_density(edges, counts) -> np.ndarray:
+    """bdf_hist_density: numpy's ``density=True`` from the edges and counts of a histogram (no context and no GPU needed)."""
+    e = np.ascontiguousarray(edges, dtype=np.float64)
+    c = np.ascontiguousarray(counts, dtype=np.int64)
+    out = np.zeros(len(c), dtype=np.float64)
+    N.raise_for_status(N.lib().bdf_hist_density(len(c), e.ctypes.data_as(C.POINTER(C.c_double)), c.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                out.ctypes.data_as(C.POINTER(C.c_double))))
+    return out
 
 
 def _moments_to_dict(r: "N.MomentRec") -> dict:
@@ -637,6 +684,47 @@ class Column:
         _refuse_temporal("sum_distinct", self)
         return _scalar_from_bits(self.dtype, self._distinct().sum)
 
+    # -- distributions (include/b200df.h "distributions"): Column::hist and Column::uniques of src/table.rs, Spark's percentile and mode --
+    def percentile(self, p):
+        """Spark's exact percentile at p (a float, or a sequence of up to 1024): a float or None, or a list of them."""
+        _refuse_temporal("a percentile", self)
+        ps, out, some = _percentile_args(p)
+        N.raise_for_status(N.lib().bdf_percentile_dev(self.ctx.handle, self.handle, len(np.atleast_1d(p)), ps, out, some))
+        return _percentile_result(p, out, some)
+
+    def median(self) -> Optional[float]: return self.percentile(0.5)
+
+    def _mode(self):
+        bits, freq, some = C.c_uint64(0), C.c_int64(0), C.c_int32(0)
+        N.raise_for_status(N.lib().bdf_mode_dev(self.ctx.handle, self.handle, C.byref(bits), C.byref(freq), C.byref(some)))
+        return (_scalar_from_bits(self.dtype, bits.value), int(freq.value)) if some.value else (None, 0)
+
+    def mode(self):
+        """The most frequent valid value (ties: the smallest in key order), or None."""
+        return self._mode()[0]
+
+    def uniques(self) -> "Column":
+        """The distinct valid values, ascending, as a one-chunk column (all NaNs are one value, -0.0 == 0.0)."""
+        h = C.c_void_p()
+        N.raise_for_status(N.lib().bdf_uniques_dev(self.ctx.handle, self.handle, C.byref(h), None))
+        return Column(self.ctx, h, self.temporal)
+
+    def value_counts(self):
+        """``(values, counts)``: the distinct valid values ascending (as ``uniques``) and the Int64 number of rows of each."""
+        h, hc = C.c_void_p(), C.c_void_p()
+        N.raise_for_status(N.lib().bdf_uniques_dev(self.ctx.handle, self.handle, C.byref(h), C.byref(hc)))
+        return Column(self.ctx, h, self.temporal), Column(self.ctx, hc)
+
+    def hist(self, nbins: int, density: bool = False, range=None):
+        """numpy.histogram's equal-width bins: ``(edges, counts)`` as numpy arrays (Float64 densities when ``density``); NaN is skipped."""
+        _refuse_temporal("a histogram", self)
+        edges = np.zeros(max(int(nbins), 0) + 1, dtype=np.float64)
+        counts = np.zeros(max(int(nbins), 0), dtype=np.int64)
+        rng = None if range is None else (C.c_double * 2)(float(range[0]), float(range[1]))
+        N.raise_for_status(N.lib().bdf_hist_dev(self.ctx.handle, self.handle, int(nbins), rng, edges.ctypes.data_as(C.POINTER(C.c_double)),
+                                                counts.ctypes.data_as(C.POINTER(C.c_int64))))
+        return edges, (hist_density(edges, counts) if density else counts)
+
     # -- dates and timestamps (include/b200df.h "dates and timestamps"); the column must carry a temporal tag --
     def _temporal_fn(self, fn: int, arg=0) -> "Column":
         t = _temporal_of([self], None) if self.temporal is None else self.temporal
@@ -785,8 +873,8 @@ def group_aggregate(key: "Column", values: Sequence["Column"]):
 def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
     """Group-by over 1..16 key columns (bdf_group_by_dev).  ``aggregations``: ``[(Column, function)]`` with function one of
     "sum", "max", "min", "avg", "count", "count_distinct", "first", "last", "kurtosis", "skewness", "stddev", "sum_distinct",
-    "variance", "stddev_pop", "var_pop".  Returns ``([key Column per key], [result Column per aggregation])``; groups in the order
-    DataFrame::sort gives (ascending, nulls last per key).  Counts are Int64, avg and the statistics are Float64, everything else
+    "variance", "stddev_pop", "var_pop", "exact_median", "mode".  Returns ``([key Column per key], [result Column per aggregation])``; groups in the order
+    DataFrame::sort gives (ascending, nulls last per key).  Counts are Int64, avg, median and the statistics are Float64, everything else
     has the value column's type; see include/b200df.h for the NULL rules."""
     fns = []
     for col, fn in aggregations:
@@ -810,7 +898,7 @@ def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
             [Column(ctx, C.c_void_p(out[j]), carry(*aggregations[j])) for j in range(na)])
 
 
-_CARRY_GROUP = ("min", "max", "first", "last")   # aggregations whose results are values of the column: a temporal tag carries
+_CARRY_GROUP = ("min", "max", "first", "last", "mode")   # aggregations whose results are values of the column: a temporal tag carries
 
 
 def join_indices(left_keys: Sequence["Column"], right_keys: Sequence["Column"], how: str):

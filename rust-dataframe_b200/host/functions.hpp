@@ -233,6 +233,23 @@ struct AggregateFunctions {
         std::memcpy(&out, &r.sum, sizeof(T));
         return out;
     }
+    // The distributions (include/b200df.h "distributions"): Spark's exact percentile (p in [0, 1]), median and mode.
+    template <typename T> static std::optional<double> percentile(const Arrays<T>& a, double p) {
+        auto v = detail::views(a);
+        double out = 0; int32_t some = 0;
+        check(bdf_percentile(context(), ArrowType<T>::id, (int64_t)v.size(), v.data(), 1, &p, &out, &some));
+        return some ? std::optional<double>(out) : std::nullopt;
+    }
+    template <typename T> static std::optional<double> median(const Arrays<T>& a) { return percentile<T>(a, 0.5); }
+    template <typename T> static std::optional<T> mode(const Arrays<T>& a) {   // ties: the smallest value
+        auto v = detail::views(a);
+        uint64_t bits = 0; int64_t freq = 0; int32_t some = 0;
+        check(bdf_mode(context(), ArrowType<T>::id, (int64_t)v.size(), v.data(), &bits, &freq, &some));
+        if (!some) return std::nullopt;
+        T out{};
+        std::memcpy(&out, &bits, sizeof(T));
+        return out;
+    }
 
    private:
     template <typename T> static std::optional<double> stat(int which, const Arrays<T>& a) {
