@@ -399,16 +399,50 @@ int  bdf_join_indices_dev(bdf_ctx* ctx, int32_t join_type, int32_t n_keys, const
  *   keys and only ranking functions: no rows to number) -> BDF_INVALID; an unknown function or frame, a non-numeric column, AVG of
  *   Int64 / UInt64 ("avg needs f64: From<T::Native>"), more than 2^32-1 rows (the sort's message), a multi-GPU context ->
  *   BDF_UNSUPPORTED; columns of different lengths -> BDF_LENGTH_MISMATCH. */
+/* Bounded frames (WindowSpec's rows_between / range_between).  A zero-initialised call's new fields change nothing above.
+ * Frame resolution.  Every frame is a range of sorted positions [s, e] inside the current row's partition [ps, pe]; s > e is empty.
+ *   ROWS_BETWEEN   s = max(ps, i + start), e = min(pe, i + end) in saturating arithmetic; an UNBOUNDED start is ps, an UNBOUNDED end pe.
+ *   RANGE_BETWEEN  exactly one order column.  With v the current row's key, an ascending key gives the rows whose key k is valid, not
+ *                  NaN and v + start <= k <= v + end; a descending key v - end <= k <= v - start (PRECEDING always points towards the
+ *                  start of the sorted order).  As positions: s is the first row of the partition's valid non-NaN keys that meets the
+ *                  start bound (the row after them when none does), e the last that meets the end bound (the row before them when
+ *                  none does).  Integer (and temporal) keys use start / end and compare exactly, with no wrap: a bound outside the
+ *                  type's range takes in every row on that side, and an unsigned key accepts a negative start.  Float keys use
+ *                  start_f / end_f and compare with (double)v + start_f rounded once; -0.0 == 0.0 and +-inf keys follow IEEE
+ *                  arithmetic.  When the current key is null or NaN, an offset bound is the first (start) or last (end) row of the
+ *                  row's own peer run.  An UNBOUNDED bound is always the partition's edge, so UNBOUNDED FOLLOWING includes the null
+ *                  and NaN keys where they sort.
+ *   Offsets follow Spark's rowsBetween / rangeBetween: negative = PRECEDING, 0 = CURRENT ROW, positive = FOLLOWING; INT64_MIN /
+ *   INT64_MAX (-inf / +inf for start_f / end_f) = UNBOUNDED.
+ *   Equivalent specifications run the existing frame and give its bits: ROWS_BETWEEN(UNBOUNDED, 0) = ROWS, ROWS_BETWEEN(UNBOUNDED,
+ *   UNBOUNDED) = PARTITION, RANGE_BETWEEN(UNBOUNDED, 0) = RANGE, RANGE_BETWEEN(UNBOUNDED, UNBOUNDED) = PARTITION.
+ * Aggregates over a bounded frame keep the types and null rules above: an empty frame gives SUM 0, COUNT 0 and NULL for MIN, MAX and
+ *   AVG.  COUNT, integer SUM (wrapping) and MIN / MAX (totalOrder for floats) are exact.  Float SUM and every AVG stay within
+ *   16 * log2(max(k, 2)) * 2^-53 * sum(|x|) over the frame's k rows, plus the final f32 rounding, and are the same bits on every run
+ *   and under any chunking: each frame is combined from a radix-32 hierarchy of block prefixes and suffixes, every term a sum over part
+ *   of the frame, in an order fixed by (s, e); the cost per row does not grow with the frame's width.  A float prefix-sum difference
+ *   does not meet this bar, and neither does a sliding add / subtract: their error grows with the magnitudes of the partition, not of
+ *   the frame.  (Integer sums could use prefix differences: wrapping arithmetic makes them exact.)
+ * FIRST_VALUE / LAST_VALUE / NTH_VALUE (column x of any numeric type; the output has x's dtype; any frame, the three above included).
+ *   RESPECT NULLS (ignore_nulls = 0): x at s, at e, or at s + n - 1 when that is at most e (n = offset); NULL when that row's x is null
+ *   or the frame is empty.  IGNORE NULLS: the first, last or n-th valid x in [s, e]; NULL when the frame holds fewer valid values.
+ * Errors of bounded frames (BDF_INVALID; nothing is returned and nothing leaks): start > end; a start of UNBOUNDED FOLLOWING or an end
+ *   of UNBOUNDED PRECEDING; a NaN float offset; RANGE_BETWEEN without exactly one order column; NTH_VALUE with n < 1; ignore_nulls on a
+ *   function other than the three value functions. */
 typedef enum { BDF_WIN_ROW_NUMBER = 0, BDF_WIN_RANK, BDF_WIN_DENSE_RANK, BDF_WIN_PERCENT_RANK, BDF_WIN_CUME_DIST,
-               BDF_WIN_LAG, BDF_WIN_LEAD, BDF_WIN_SUM, BDF_WIN_COUNT, BDF_WIN_MIN, BDF_WIN_MAX, BDF_WIN_AVG } bdf_window_fn;
-typedef enum { BDF_FRAME_ROWS = 0, BDF_FRAME_RANGE, BDF_FRAME_PARTITION } bdf_window_frame;
+               BDF_WIN_LAG, BDF_WIN_LEAD, BDF_WIN_SUM, BDF_WIN_COUNT, BDF_WIN_MIN, BDF_WIN_MAX, BDF_WIN_AVG,
+               BDF_WIN_FIRST_VALUE, BDF_WIN_LAST_VALUE, BDF_WIN_NTH_VALUE } bdf_window_fn;
+typedef enum { BDF_FRAME_ROWS = 0, BDF_FRAME_RANGE, BDF_FRAME_PARTITION, BDF_FRAME_ROWS_BETWEEN, BDF_FRAME_RANGE_BETWEEN } bdf_window_frame;
 typedef struct {
     int32_t function;        /* bdf_window_fn */
-    int32_t frame;           /* bdf_window_frame; aggregates only */
-    const bdf_col* column;   /* LAG / LEAD / aggregates; NULL for the five ranking functions */
-    int64_t offset;          /* LAG / LEAD, >= 0 */
+    int32_t frame;           /* bdf_window_frame; aggregates and value functions */
+    const bdf_col* column;   /* LAG / LEAD / aggregates / value functions; NULL for the five ranking functions */
+    int64_t offset;          /* LAG / LEAD, >= 0; NTH_VALUE's n, >= 1 */
     uint64_t default_bits;   /* LAG / LEAD: T::Native of `column` in the low bytes (as bdf_agg4) */
     int32_t has_default;
+    int32_t ignore_nulls;    /* FIRST_VALUE / LAST_VALUE / NTH_VALUE: IGNORE NULLS */
+    int64_t start, end;      /* ROWS_BETWEEN, and RANGE_BETWEEN over an integer or temporal order key: signed offsets */
+    double start_f, end_f;   /* RANGE_BETWEEN over a Float32 / Float64 order key; -inf / +inf = UNBOUNDED */
 } bdf_window_call;
 int  bdf_window_dev(bdf_ctx* ctx, int32_t n_partition, const bdf_col* const* partition_by, int32_t n_order, const bdf_sort_key* order_by,
                     int32_t n_calls, const bdf_window_call* calls, bdf_col** out /* n_calls */);

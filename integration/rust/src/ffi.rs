@@ -119,10 +119,15 @@ pub const BDF_GROUP_LAST: i32 = 7;
 #[repr(C)]
 pub struct BdfSortKey { pub column: *const BdfCol, pub descending: i32 }
 /// bdf_window_call (include/b200df.h): one window function over the shared WindowSpec.  `column` is null for the five ranking
-/// functions; `offset` / `default_bits` / `has_default` are LAG / LEAD's, `frame` (bdf_window_frame) the aggregates'.
+/// functions; `offset` / `default_bits` / `has_default` are LAG / LEAD's (`offset` is also NTH_VALUE's n), `frame` (bdf_window_frame) the
+/// aggregates' and value functions'.  `start` / `end` are ROWS_BETWEEN's and an integer RANGE_BETWEEN's offsets (i64::MIN / i64::MAX =
+/// UNBOUNDED), `start_f` / `end_f` a float RANGE_BETWEEN's (-inf / +inf); `ignore_nulls` is the value functions'.
 #[repr(C)]
 #[derive(Clone, Copy)]
-pub struct BdfWindowCall { pub function: i32, pub frame: i32, pub column: *const BdfCol, pub offset: i64, pub default_bits: u64, pub has_default: i32 }
+pub struct BdfWindowCall {
+    pub function: i32, pub frame: i32, pub column: *const BdfCol, pub offset: i64, pub default_bits: u64, pub has_default: i32,
+    pub ignore_nulls: i32, pub start: i64, pub end: i64, pub start_f: f64, pub end_f: f64,
+}
 /// bdf_window_fn, in WindowFunctions order, then the aggregates.
 pub const BDF_WIN_ROW_NUMBER: i32 = 0;
 pub const BDF_WIN_RANK: i32 = 1;
@@ -136,10 +141,16 @@ pub const BDF_WIN_COUNT: i32 = 8;
 pub const BDF_WIN_MIN: i32 = 9;
 pub const BDF_WIN_MAX: i32 = 10;
 pub const BDF_WIN_AVG: i32 = 11;
-/// bdf_window_frame: ROWS = partition start .. current row, RANGE = .. the current row's last peer, PARTITION = the whole partition.
+pub const BDF_WIN_FIRST_VALUE: i32 = 12;
+pub const BDF_WIN_LAST_VALUE: i32 = 13;
+pub const BDF_WIN_NTH_VALUE: i32 = 14;
+/// bdf_window_frame: ROWS = partition start .. current row, RANGE = .. the current row's last peer, PARTITION = the whole partition;
+/// ROWS_BETWEEN / RANGE_BETWEEN = WindowSpec's rows_between / range_between with signed offsets.
 pub const BDF_FRAME_ROWS: i32 = 0;
 pub const BDF_FRAME_RANGE: i32 = 1;
 pub const BDF_FRAME_PARTITION: i32 = 2;
+pub const BDF_FRAME_ROWS_BETWEEN: i32 = 3;
+pub const BDF_FRAME_RANGE_BETWEEN: i32 = 4;
 pub const BDF_ASYNC: c_int = 1;
 
 /// All four aggregates of one pass (include/b200df.h `bdf_agg4`, ABI version 2: `n_chunks` added).

@@ -202,6 +202,20 @@ pub fn window_device(frame: &DeviceColumns, partition: &[usize], order: &[(usize
     Ok(DeviceColumns { names: calls.iter().map(|(n, _)| n.clone()).collect(), cols: out })
 }
 
+/// `WindowSpec::rows_between(start, end)` for one aggregate or value function over `column` (Spark's offsets: negative = PRECEDING,
+/// 0 = CURRENT ROW, positive = FOLLOWING, `None` = UNBOUNDED), as a call for `window_device`; e.g. a moving average
+/// `rows_between(BDF_WIN_AVG, x, Some(-99), Some(0))` or a forward fill with `ignore_nulls = 1` on `BDF_WIN_LAST_VALUE, None, Some(0)`.
+pub fn rows_between(function: i32, column: *const BdfCol, start: Option<i64>, end: Option<i64>) -> BdfWindowCall {
+    BdfWindowCall { function, frame: BDF_FRAME_ROWS_BETWEEN, column, offset: if function == BDF_WIN_NTH_VALUE { 1 } else { 0 }, default_bits: 0,
+                    has_default: 0, ignore_nulls: 0, start: start.unwrap_or(i64::MIN), end: end.unwrap_or(i64::MAX), start_f: 0.0, end_f: 0.0 }
+}
+
+/// `WindowSpec::range_between(start, end)` over the single order key: integer / temporal keys take `start` / `end` in the key's unit,
+/// Float32 / Float64 keys `start_f` / `end_f` (set them on the returned call; `None` = UNBOUNDED).
+pub fn range_between(function: i32, column: *const BdfCol, start: Option<i64>, end: Option<i64>) -> BdfWindowCall {
+    BdfWindowCall { frame: BDF_FRAME_RANGE_BETWEEN, start_f: f64::NEG_INFINITY, end_f: f64::INFINITY, ..rows_between(function, column, start, end) }
+}
+
 /// `DataFrame::from_csv(path, None)` on the device: a header, ',', the schema inferred from every record, 1024 rows per
 /// RecordBatch (`schema`: one dtype per column instead, BDF_UTF8 for a string column).  Utf8 columns are not on the device path and
 /// are left out; a caller that needs them reads just those with arrow's CPU reader and a projection

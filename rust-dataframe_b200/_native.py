@@ -48,11 +48,12 @@ JOIN_LEFT, JOIN_RIGHT, JOIN_INNER, JOIN_FULL = range(4)
 JOIN_TYPES = {"left": JOIN_LEFT, "right": JOIN_RIGHT, "inner": JOIN_INNER, "full": JOIN_FULL}
 # bdf_window_fn / bdf_window_frame
 (WIN_ROW_NUMBER, WIN_RANK, WIN_DENSE_RANK, WIN_PERCENT_RANK, WIN_CUME_DIST, WIN_LAG, WIN_LEAD, WIN_SUM, WIN_COUNT, WIN_MIN, WIN_MAX,
- WIN_AVG) = range(12)
+ WIN_AVG, WIN_FIRST_VALUE, WIN_LAST_VALUE, WIN_NTH_VALUE) = range(15)
 WINDOW_FNS = {"row_number": WIN_ROW_NUMBER, "rank": WIN_RANK, "dense_rank": WIN_DENSE_RANK, "percent_rank": WIN_PERCENT_RANK,
               "cume_dist": WIN_CUME_DIST, "lag": WIN_LAG, "lead": WIN_LEAD, "sum": WIN_SUM, "count": WIN_COUNT, "min": WIN_MIN,
-              "max": WIN_MAX, "avg": WIN_AVG}
-FRAME_ROWS, FRAME_RANGE, FRAME_PARTITION = range(3)
+              "max": WIN_MAX, "avg": WIN_AVG, "first_value": WIN_FIRST_VALUE, "last_value": WIN_LAST_VALUE, "nth_value": WIN_NTH_VALUE}
+FRAME_ROWS, FRAME_RANGE, FRAME_PARTITION, FRAME_ROWS_BETWEEN, FRAME_RANGE_BETWEEN = range(5)
+BOUNDED_FRAMES = {"rows": FRAME_ROWS_BETWEEN, "range": FRAME_RANGE_BETWEEN}   # ("rows" | "range", start, end) frames
 WINDOW_FRAMES = {"rows": FRAME_ROWS, "range": FRAME_RANGE, "partition": FRAME_PARTITION}
 # list columns (bdf_list_*)
 LIST_BASE = 32
@@ -115,7 +116,8 @@ class GroupAggC(C.Structure):
 
 class WindowCall(C.Structure):
     _fields_ = [("function", C.c_int32), ("frame", C.c_int32), ("column", C.c_void_p), ("offset", C.c_int64), ("default_bits", C.c_uint64),
-                ("has_default", C.c_int32)]
+                ("has_default", C.c_int32), ("ignore_nulls", C.c_int32), ("start", C.c_int64), ("end", C.c_int64), ("start_f", C.c_double),
+                ("end_f", C.c_double)]
 
 
 class TemporalTypeC(C.Structure):

@@ -440,6 +440,24 @@ cudaError_t launch_window_shift(int dtype, const void* const* p, long long n_p, 
 size_t window_scan_scratch_bytes(long long n);
 cudaError_t launch_window_scan(int dtype, int fn, const void* x, int nx, const uint32_t* heads, long long n, void* scratch, void* out, uint32_t* vout,
                                cudaStream_t s);
+// Bounded frames: how every sorted position finds its frame [s, e] inside its partition (the rules are in include/b200df.h).
+enum : int { WIN_FR_ROWS = 0, WIN_FR_PEERS, WIN_FR_RANGE };
+struct WinFrameDesc {
+    int kind;                 // ROWS: offsets from the position; PEERS: partition start .. last peer; RANGE: offsets of the order key
+    int key_dtype, key_desc, key_chunks;
+    long long start, end;     // ROWS and integer RANGE; LLONG_MIN / LLONG_MAX = UNBOUNDED
+    double start_f, end_f;    // float RANGE; -inf / +inf = UNBOUNDED
+    const void* key;          // RANGE: the order key in sorted order, as a chunk table (sort_table)
+};
+int window_frame_levels(long long n);
+size_t window_frame_scratch_bytes(int dtype, long long n);
+cudaError_t launch_window_frame_build(int dtype, const void* x, int nx, long long n, void* scratch, cudaStream_t s);
+cudaError_t launch_window_frame_agg(int dtype, int fn, const void* const* p, long long n_p, const void* const* q, long long n_q, const WinFrameDesc& f,
+                                    const void* x, int nx, long long n, void* scratch, void* out, uint32_t* vout, cudaStream_t s);
+cudaError_t launch_window_valid_words(const void* x, int nx, long long n, uint32_t* words, cudaStream_t s);
+cudaError_t launch_window_frame_value(int dtype, int which, long long nth, const void* const* p, long long n_p, const void* const* q, long long n_q,
+                                      const WinFrameDesc& f, const void* x, int nx, long long n, const uint32_t* vwords,
+                                      const unsigned long long* vprefix, void* out, uint32_t* vout, cudaStream_t s);
 
 // CSV reader (k_csv.cu).
 int csv_tile_bytes();

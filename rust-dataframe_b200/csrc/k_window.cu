@@ -17,6 +17,16 @@
 //                    start), (2) k_window_carry, one CTA, scans those tile records into every tile's carry-in, (3) every tile
 //                    rescans its rows from its carry.  The order in which values are combined depends only on n, so float sums
 //                    are the same bits on every run; a decoupled look-back would combine predecessors in a timing-dependent order.
+//   k_window_level   bounded frames: one level of a radix-32 prefix / suffix hierarchy of the scan's accumulator.  Level 0 holds,
+//                    for every position, the inclusive prefix and suffix of its aligned block of 32 values; level L + 1 does the
+//                    same over the block totals of level L, up to the first level of at most 32 items (~2.07 n records in all).
+//   k_window_frame_agg   per position: the frame [s, e] (frame_bounds: ROWS arithmetic, or a binary search of the order key for
+//                    RANGE), then a fixed sequence of terms: while s and e lie in different blocks, suffix(s) on the left and
+//                    prefix(e) on the right, one level up; then a fold of at most 32 items.  Every term is an aggregate of rows
+//                    inside the frame, so float sums stay accurate relative to the frame, and the order of the terms depends only on
+//                    (s, e): the same bits on every run and under any chunking.  The cost does not grow with the frame's width.
+//   k_window_frame_value first_value / last_value / nth_value: a read at s, e or s + n - 1, or with IGNORE NULLS the rank of the valid
+//                    slots (the popcount prefix of the validity words) and a search for the wanted rank inside [s, e].
 // Values are read through a chunk table (SortChunk), so the call without keys reads the caller's chunks in place and writes row
 // order directly.
 #include "group_acc.cuh"
@@ -423,5 +433,369 @@ cudaError_t launch_window_scan(int dtype, int fn, const void* x, int nx, const u
         default: return cudaErrorInvalidValue;
     }
 }
+
+// ---- bounded frames: [s, e] of every position -----------------------------------------------------------------------------
+// The order key at sorted position j: its class (the numeric run is class 0 ascending, 1 descending; NaN sorts above every number,
+// so it is class 1 ascending and 0 descending; null is class 2 both ways) and its value, exact in __int128 or as a double.
+struct WinKey { int cls; __int128 i; double f; };
+
+__device__ __forceinline__ WinKey win_key(const WinFrameDesc& f, long long j) {
+    const void* p;
+    long long local;
+    const bool ok = read_chunked((const SortChunk*)f.key, f.key_chunks, j, &p, &local);
+    WinKey k;
+    k.i = 0;
+    k.f = 0.0;
+    int raw = 0;   // 0 number, 1 NaN, 2 null
+    if (!ok) raw = 2;
+    else switch (f.key_dtype) {
+        case T_I8: k.i = ((const int8_t*)p)[local]; break;
+        case T_I16: k.i = ((const int16_t*)p)[local]; break;
+        case T_I32: k.i = ((const int32_t*)p)[local]; break;
+        case T_I64: k.i = ((const long long*)p)[local]; break;
+        case T_U8: k.i = ((const uint8_t*)p)[local]; break;
+        case T_U16: k.i = ((const uint16_t*)p)[local]; break;
+        case T_U32: k.i = ((const uint32_t*)p)[local]; break;
+        case T_U64: k.i = (__int128)((const unsigned long long*)p)[local]; break;
+        case T_F32: k.f = (double)((const float*)p)[local]; raw = k.f != k.f; break;
+        default: k.f = ((const double*)p)[local]; raw = k.f != k.f; break;
+    }
+    k.cls = raw == 2 ? 2 : (f.key_desc ? 1 - raw : raw);
+    return k;
+}
+
+// The first position j in [lo, hi) for which pred(j) holds (pred is false, then true, over the range); hi when there is none.
+template <typename P>
+__device__ __forceinline__ long long win_search(long long lo, long long hi, P pred) {
+    while (lo < hi) {
+        const long long mid = lo + ((hi - lo) >> 1);
+        if (pred(mid)) hi = mid;
+        else lo = mid + 1;
+    }
+    return lo;
+}
+
+__device__ __forceinline__ long long win_clamp(long long o) {   // offsets beyond any partition act alike; no overflow below
+    const long long lim = 1ll << 34;
+    return o < -lim ? -lim : (o > lim ? lim : o);
+}
+
+__device__ __forceinline__ void frame_bounds(const WinRuns& r, const WinFrameDesc& f, long long i, long long* s, long long* e) {
+    const WinPos p = win_pos(r, i, f.kind == WIN_FR_PEERS);
+    *s = p.ps;
+    *e = p.pe;
+    if (f.kind == WIN_FR_ROWS) {
+        if (f.start != LLONG_MIN) *s = max(p.ps, i + win_clamp(f.start));
+        if (f.end != LLONG_MAX) *e = min(p.pe, i + win_clamp(f.end));
+        return;
+    }
+    if (f.kind == WIN_FR_PEERS) { *e = p.qe; return; }
+    const bool is_f = f.key_dtype == T_F32 || f.key_dtype == T_F64;
+    const bool s_unb = is_f ? f.start_f == -INFINITY : f.start == LLONG_MIN;
+    const bool e_unb = is_f ? f.end_f == INFINITY : f.end == LLONG_MAX;
+    if (s_unb && e_unb) return;
+    const WinKey v = win_key(f, i);
+    const int num = f.key_desc ? 1 : 0;
+    const long long end = p.pe + 1;
+    if (v.cls != num) {   // a null or NaN key: an offset bound is the edge of the row's own peer run
+        if (!s_unb) *s = win_search(p.ps, end, [=](long long j) { return win_key(f, j).cls >= v.cls; });
+        if (!e_unb) *e = win_search(p.ps, end, [=](long long j) { return win_key(f, j).cls > v.cls; }) - 1;
+        return;
+    }
+    const long long a = win_search(p.ps, end, [=](long long j) { return win_key(f, j).cls >= num; });
+    const long long b = win_search(a, end, [=](long long j) { return win_key(f, j).cls > num; });   // numbers: [a, b)
+    // The keys of [a, b) run in the sort's direction.  Ascending: v + start <= k <= v + end; descending: v - end <= k <= v - start.
+    if (!s_unb) {
+        if (is_f) {
+            const double t = f.key_desc ? __dsub_rn(v.f, f.start_f) : __dadd_rn(v.f, f.start_f);
+            *s = win_search(a, b, [=](long long j) { const double k = win_key(f, j).f; return f.key_desc ? k <= t : k >= t; });
+        } else {
+            const __int128 t = f.key_desc ? v.i - (__int128)f.start : v.i + (__int128)f.start;
+            *s = win_search(a, b, [=](long long j) { const __int128 k = win_key(f, j).i; return f.key_desc ? k <= t : k >= t; });
+        }
+    }
+    if (!e_unb) {
+        if (is_f) {
+            const double t = f.key_desc ? __dsub_rn(v.f, f.end_f) : __dadd_rn(v.f, f.end_f);
+            *e = win_search(a, b, [=](long long j) { const double k = win_key(f, j).f; return f.key_desc ? k < t : k > t; }) - 1;
+        } else {
+            const __int128 t = f.key_desc ? v.i - (__int128)f.end : v.i + (__int128)f.end;
+            *e = win_search(a, b, [=](long long j) { const __int128 k = win_key(f, j).i; return f.key_desc ? k < t : k > t; }) - 1;
+        }
+    }
+}
+
+// ---- bounded frames: the prefix / suffix hierarchy --------------------------------------------------------------------------
+constexpr int kWinMaxLevels = 8;   // 32^7 > 2^32 rows
+template <typename T> struct WinLevels {
+    WinAcc<T>* pre[kWinMaxLevels];
+    WinAcc<T>* suf[kWinMaxLevels];
+    long long cnt[kWinMaxLevels + 1];   // items of every level; cnt[levels] <= 32
+    int levels;                         // levels with stored records
+};
+
+template <typename A>
+__device__ __forceinline__ A shfl_down_rec(const A& a, int o) {
+    static_assert(sizeof(A) % 8 == 0, "record of 64-bit words");
+    A r;
+    unsigned long long w[sizeof(A) / 8];
+    memcpy(w, &a, sizeof(A));
+#pragma unroll
+    for (int k = 0; k < (int)(sizeof(A) / 8); k++) w[k] = __shfl_down_sync(0xffffffffu, w[k], o);
+    memcpy(&r, w, sizeof(A));
+    return r;
+}
+
+// Item j of level lvl: x at j on level 0, else the total of block j of the level below (its last prefix).
+template <typename T>
+__device__ __forceinline__ WinAcc<T> win_item(const WinLevels<T>& h, const SortChunk* __restrict__ x, int nx, int lvl, long long j) {
+    WinAcc<T> a;
+    if (lvl == 0) {
+        const void* p;
+        long long local;
+        const bool ok = read_chunked(x, nx, j, &p, &local);
+        a.init();
+        a.add(ok ? ((const T*)p)[local] : (T)0, ok);
+    } else {
+        a = h.pre[lvl - 1][min(32 * j + 31, h.cnt[lvl - 1] - 1)];
+    }
+    return a;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads)
+k_window_level(const SortChunk* __restrict__ x, int nx, const WinLevels<T> h, int lvl) {
+    const long long j = (long long)blockIdx.x * kThreads + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    WinAcc<T> pre;
+    pre.init();
+    if (j < h.cnt[lvl]) pre = win_item(h, x, nx, lvl, j);
+    WinAcc<T> suf = pre;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {   // a fixed-order warp scan each way over one aligned block of 32 items
+        WinAcc<T> up = shfl_up_rec(pre, o);
+        const WinAcc<T> dn = shfl_down_rec(suf, o);
+        if (lane >= o) { up.merge(pre); pre = up; }
+        if (lane + o < 32) suf.merge(dn);
+    }
+    if (j < h.cnt[lvl]) {
+        h.pre[lvl][j] = pre;
+        h.suf[lvl][j] = suf;
+    }
+}
+
+// The aggregate of positions [s, e]: suffix / prefix terms level by level, then a fold of at most 32 items, in an order fixed by (s, e).
+template <typename T>
+__device__ __forceinline__ WinAcc<T> frame_fold(const WinLevels<T>& h, const SortChunk* __restrict__ x, int nx, long long s, long long e) {
+    WinAcc<T> l, r;
+    l.init();
+    r.init();
+    int lvl = 0;
+    while (s <= e) {
+        if ((s >> 5) == (e >> 5)) {
+            for (long long j = s; j <= e; j++) l.merge(win_item(h, x, nx, lvl, j));
+            break;
+        }
+        l.merge(h.suf[lvl][s]);
+        WinAcc<T> t = h.pre[lvl][e];
+        t.merge(r);
+        r = t;
+        s = (s >> 5) + 1;
+        e = (e >> 5) - 1;
+        lvl++;
+    }
+    l.merge(r);
+    return l;
+}
+
+// __launch_bounds__(kThreads, 4) on the two frame kernels: without the occupancy hint ptxas held them to 32 registers and spilled.
+template <typename T, int FN>
+__global__ void __launch_bounds__(kThreads, 4)
+k_window_frame_agg(const WinRuns runs, const WinFrameDesc f, const SortChunk* __restrict__ x, int nx, const WinLevels<T> h,
+                   typename WinOutT<T, FN>::type* __restrict__ out, uint32_t* __restrict__ vout) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    bool valid = false;
+    if (i < runs.n) {
+        long long s, e;
+        frame_bounds(runs, f, i, &s, &e);
+        out[i] = win_result<T, FN>(frame_fold(h, x, nx, s, e), &valid);
+    }
+    const unsigned word = __ballot_sync(0xffffffffu, valid);
+    if (vout && (threadIdx.x & 31) == 0 && i < runs.n) vout[i >> 5] = word;
+}
+
+// ---- bounded frames: first_value / last_value / nth_value ------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads)
+k_window_valid_words(const SortChunk* __restrict__ x, int nx, long long n, uint32_t* __restrict__ words) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    bool ok = false;
+    if (i < n) {
+        const void* p;
+        long long local;
+        ok = read_chunked(x, nx, i, &p, &local);
+    }
+    const unsigned word = __ballot_sync(0xffffffffu, ok);
+    if ((threadIdx.x & 31) == 0 && i < n) words[i >> 5] = word;
+}
+
+// Valid slots in [0, p] (p may be -1).
+__device__ __forceinline__ long long valid_upto(const uint32_t* __restrict__ w, const unsigned long long* __restrict__ pre, long long p) {
+    if (p < 0) return 0;
+    const uint32_t below = (2u << (p & 31)) - 1u;
+    return (long long)__ldg(pre + (p >> 5)) + __popc(__ldg(w + (p >> 5)) & below);
+}
+
+// The position of the r-th valid slot (1-based), known to lie in words [w0, w1].
+__device__ __forceinline__ long long valid_select(const uint32_t* __restrict__ w, const unsigned long long* __restrict__ pre, long long r, long long w0,
+                                                  long long w1) {
+    const long long wd = win_search(w0, w1 + 1, [=](long long k) { return (long long)__ldg(pre + k) >= r; }) - 1;   // last word with prefix < r
+    uint32_t bits = __ldg(w + wd);
+    for (long long k = r - (long long)__ldg(pre + wd); k > 1; k--) bits &= bits - 1u;
+    return 32 * wd + __ffs(bits) - 1;
+}
+
+// which: 0 first_value, 1 last_value, 2 nth_value (nth >= 1).  vwords / vprefix: the sorted validity and its popcount prefix for
+// IGNORE NULLS, null for RESPECT NULLS.
+template <typename T>
+__global__ void __launch_bounds__(kThreads, 4)
+k_window_frame_value(const WinRuns runs, const WinFrameDesc f, const SortChunk* __restrict__ x, int nx, int which, long long nth,
+                     const uint32_t* __restrict__ vwords, const unsigned long long* __restrict__ vprefix, T* __restrict__ out,
+                     uint32_t* __restrict__ vout) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    bool valid = false;
+    if (i < runs.n) {
+        long long s, e, j = -1;
+        frame_bounds(runs, f, i, &s, &e);
+        if (s <= e) {
+            if (!vwords) {
+                j = which == 0 ? s : which == 1 ? e : (nth - 1 <= e - s ? s + nth - 1 : -1);
+            } else {
+                const long long before = valid_upto(vwords, vprefix, s - 1), upto = valid_upto(vwords, vprefix, e);
+                const long long have = upto - before;
+                const long long k = which == 0 ? 1 : which == 1 ? have : nth;   // the k-th valid slot of the frame
+                if (k >= 1 && k <= have) j = valid_select(vwords, vprefix, before + k, s >> 5, e >> 5);
+            }
+        }
+        T v = (T)0;
+        if (j >= 0) {
+            const void* p;
+            long long local;
+            valid = read_chunked(x, nx, j, &p, &local);
+            if (valid) v = ((const T*)p)[local];
+        }
+        out[i] = v;
+    }
+    const unsigned word = __ballot_sync(0xffffffffu, valid);
+    if ((threadIdx.x & 31) == 0 && i < runs.n) vout[i >> 5] = word;
+}
+
+// ---- bounded frame launchers ------------------------------------------------------------------------------------------------
+int window_frame_levels(long long n) {
+    int l = 0;
+    for (long long c = n; c > 32; c = (c + 31) / 32) l++;
+    return l;
+}
+
+static size_t acc_bytes(int dtype) { return dtype_is_float(dtype) ? sizeof(WinAcc<double>) : sizeof(WinAcc<long long>); }
+static size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+size_t window_frame_scratch_bytes(int dtype, long long n) {
+    size_t b = 256;
+    for (long long c = n; c > 32; c = (c + 31) / 32) b += 2 * round256((size_t)c * acc_bytes(dtype));
+    return b;
+}
+
+template <typename T>
+static WinLevels<T> levels_in(void* scratch, long long n) {
+    WinLevels<T> h{};
+    char* p = (char*)scratch;
+    long long c = n;
+    int l = 0;
+    for (; c > 32; c = (c + 31) / 32, l++) {
+        h.cnt[l] = c;
+        h.pre[l] = (WinAcc<T>*)p;
+        p += round256((size_t)c * sizeof(WinAcc<T>));
+        h.suf[l] = (WinAcc<T>*)p;
+        p += round256((size_t)c * sizeof(WinAcc<T>));
+    }
+    h.cnt[l] = c;
+    h.levels = l;
+    return h;
+}
+
+#define BDF_WIN_DTYPES(X) X(T_I8, int8_t) X(T_I16, int16_t) X(T_I32, int32_t) X(T_I64, int64_t) X(T_U8, uint8_t) X(T_U16, uint16_t) \
+    X(T_U32, uint32_t) X(T_U64, uint64_t) X(T_F32, float) X(T_F64, double)
+
+template <typename T>
+static cudaError_t frame_build(const SortChunk* x, int nx, long long n, void* scratch, cudaStream_t s) {
+    const WinLevels<T> h = levels_in<T>(scratch, n);
+    for (int l = 0; l < h.levels; l++)
+        k_window_level<T><<<(unsigned)((h.cnt[l] + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, nx, h, l);
+    return cudaGetLastError();
+}
+
+// Every level of x's hierarchy (window_frame_levels(n) launches) into scratch (window_frame_scratch_bytes).
+cudaError_t launch_window_frame_build(int dtype, const void* x, int nx, long long n, void* scratch, cudaStream_t s) {
+    const SortChunk* xc = (const SortChunk*)x;
+    switch (dtype) {
+#define BDF_BUILD_CASE(ID, T) case ID: return frame_build<T>(xc, nx, n, scratch, s);
+        BDF_WIN_DTYPES(BDF_BUILD_CASE)
+#undef BDF_BUILD_CASE
+        default: return cudaErrorInvalidValue;
+    }
+}
+
+template <typename T>
+static cudaError_t frame_agg(int fn, const WinRuns& r, const WinFrameDesc& f, const SortChunk* x, int nx, long long n, void* scratch, void* out,
+                             uint32_t* vout, cudaStream_t s) {
+    const WinLevels<T> h = levels_in<T>(scratch, n);
+    const unsigned g = (unsigned)((n + kThreads - 1) / kThreads);
+    switch (fn) {
+#define BDF_AGG_CASE(FN) \
+    case FN: k_window_frame_agg<T, FN><<<g, kThreads, 0, s>>>(r, f, x, nx, h, (typename WinOutT<T, FN>::type*)out, vout); break;
+        BDF_AGG_CASE(WIN_SUM) BDF_AGG_CASE(WIN_COUNT) BDF_AGG_CASE(WIN_MIN) BDF_AGG_CASE(WIN_MAX) BDF_AGG_CASE(WIN_AVG)
+#undef BDF_AGG_CASE
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+
+// fn: 0 sum, 1 count, 2 min, 3 max, 4 avg over the frames of f; scratch: x's hierarchy from launch_window_frame_build.
+cudaError_t launch_window_frame_agg(int dtype, int fn, const void* const* p, long long n_p, const void* const* q, long long n_q, const WinFrameDesc& f,
+                                    const void* x, int nx, long long n, void* scratch, void* out, uint32_t* vout, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    const WinRuns r = make_runs(p, n_p, q, n_q, n);
+    const SortChunk* xc = (const SortChunk*)x;
+    switch (dtype) {
+#define BDF_FAGG_CASE(ID, T) case ID: return frame_agg<T>(fn, r, f, xc, nx, n, scratch, out, vout, s);
+        BDF_WIN_DTYPES(BDF_FAGG_CASE)
+#undef BDF_FAGG_CASE
+        default: return cudaErrorInvalidValue;
+    }
+}
+
+cudaError_t launch_window_valid_words(const void* x, int nx, long long n, uint32_t* words, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    k_window_valid_words<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, s>>>((const SortChunk*)x, nx, n, words);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_window_frame_value(int dtype, int which, long long nth, const void* const* p, long long n_p, const void* const* q, long long n_q,
+                                      const WinFrameDesc& f, const void* x, int nx, long long n, const uint32_t* vwords,
+                                      const unsigned long long* vprefix, void* out, uint32_t* vout, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    const WinRuns r = make_runs(p, n_p, q, n_q, n);
+    const unsigned g = (unsigned)((n + kThreads - 1) / kThreads);
+    const SortChunk* xc = (const SortChunk*)x;
+    switch (dtype) {
+#define BDF_VALUE_CASE(ID, T)                                                                                              \
+    case ID: k_window_frame_value<T><<<g, kThreads, 0, s>>>(r, f, xc, nx, which, nth, vwords, vprefix, (T*)out, vout); break;
+        BDF_WIN_DTYPES(BDF_VALUE_CASE)
+#undef BDF_VALUE_CASE
+        default: return cudaErrorInvalidValue;
+    }
+    return cudaGetLastError();
+}
+#undef BDF_WIN_DTYPES
 
 }  // namespace bdf

@@ -2862,6 +2862,48 @@ static int window_runs(bdf_ctx* c, const bdf_col* iota, int64_t n, WinHeadsHost*
 
 static bool win_is_rank(int f) { return f >= BDF_WIN_ROW_NUMBER && f <= BDF_WIN_CUME_DIST; }
 static bool win_is_shift(int f) { return f == BDF_WIN_LAG || f == BDF_WIN_LEAD; }
+static bool win_is_value(int f) { return f >= BDF_WIN_FIRST_VALUE && f <= BDF_WIN_NTH_VALUE; }
+static bool win_bounded(int fr) { return fr == BDF_FRAME_ROWS_BETWEEN || fr == BDF_FRAME_RANGE_BETWEEN; }
+
+// The bounded frame of a call as the kernels resolve it: an equivalent specification becomes the existing frame (same bits), and a
+// value function's existing frame becomes bounds (ROWS and PARTITION as row offsets, RANGE as partition start .. last peer).
+static bdf_window_call win_normalise(bdf_window_call k, bool float_key) {
+    if (k.frame == BDF_FRAME_ROWS_BETWEEN && k.start == INT64_MIN && (k.end == 0 || k.end == INT64_MAX))
+        k.frame = k.end == 0 ? BDF_FRAME_ROWS : BDF_FRAME_PARTITION;
+    if (k.frame == BDF_FRAME_RANGE_BETWEEN) {
+        const bool s_unb = float_key ? k.start_f == -INFINITY : k.start == INT64_MIN;
+        const bool e_zero = float_key ? k.end_f == 0.0 : k.end == 0, e_unb = float_key ? k.end_f == INFINITY : k.end == INT64_MAX;
+        if (s_unb && (e_zero || e_unb)) k.frame = e_zero ? BDF_FRAME_RANGE : BDF_FRAME_PARTITION;
+    }
+    return k;
+}
+
+static WinFrameDesc win_frame_desc(const bdf_window_call& k) {
+    WinFrameDesc f{};
+    f.kind = WIN_FR_ROWS;
+    f.start = k.start;
+    f.end = k.end;
+    f.start_f = k.start_f;
+    f.end_f = k.end_f;
+    if (k.frame == BDF_FRAME_ROWS) { f.start = INT64_MIN; f.end = 0; }
+    else if (k.frame == BDF_FRAME_PARTITION) { f.start = INT64_MIN; f.end = INT64_MAX; }
+    else if (k.frame == BDF_FRAME_RANGE) f.kind = WIN_FR_PEERS;
+    else if (k.frame == BDF_FRAME_RANGE_BETWEEN) f.kind = WIN_FR_RANGE;
+    return f;
+}
+
+// The checks of a bounded frame's offsets (the key type decides which pair is read for RANGE).
+static int win_check_bounds(const bdf_window_call& k, bool float_key) {
+    if (k.frame == BDF_FRAME_RANGE_BETWEEN && float_key) {
+        if (k.start_f != k.start_f || k.end_f != k.end_f) return fail(BDF_INVALID, "a RANGE offset is NaN");
+        if (k.start_f > k.end_f) return fail(BDF_INVALID, "the frame starts after it ends");
+        if (k.start_f == INFINITY || k.end_f == -INFINITY) return fail(BDF_INVALID, "a frame cannot start at UNBOUNDED FOLLOWING or end at UNBOUNDED PRECEDING");
+        return BDF_OK;
+    }
+    if (k.start > k.end) return fail(BDF_INVALID, "the frame starts after it ends");
+    if (k.start == INT64_MAX || k.end == INT64_MIN) return fail(BDF_INVALID, "a frame cannot start at UNBOUNDED FOLLOWING or end at UNBOUNDED PRECEDING");
+    return BDF_OK;
+}
 
 static int win_out_dtype(const bdf_window_call& k) {
     switch (k.function) {
@@ -2870,6 +2912,85 @@ static int win_out_dtype(const bdf_window_call& k) {
         case BDF_WIN_COUNT: return BDF_I64;
         default: return k.column->dtype;
     }
+}
+
+// The prefix / suffix hierarchy of the last column a bounded aggregate read: the aggregates of one column share it.
+struct WinHierarchy {
+    std::unique_ptr<Scratch<void>> bytes;
+    const bdf_col* of = nullptr;
+};
+
+// One bounded-frame aggregate or value function, in sorted order, into *out (one chunk).  src / table: x in sorted order; key: the
+// single order key (RANGE BETWEEN), which source() brings into sorted order (null source: nothing is sorted).
+static int window_frame_call(bdf_ctx* c, const bdf_window_call& k, const void* const* p, int64_t n_p, const void* const* q, int64_t n_q,
+                             const bdf_col* src, void* table, int n_chunks, bool nullable, bdf_sort_key key,
+                             const std::function<int(const bdf_col*, const bdf_col**)>* source, int64_t n, WinHierarchy* hier, bdf_col** out) {
+    WinFrameDesc f = win_frame_desc(k);
+    if (f.kind == WIN_FR_RANGE) {
+        const bdf_col* ks = key.column;
+        if (source) TRY((*source)(key.column, &ks));
+        bool key_nullable = false;
+        TRY(sort_table(c, ks, (void**)&f.key, &f.key_chunks, &key_nullable));
+        f.key_dtype = key.column->dtype;
+        f.key_desc = key.descending ? 1 : 0;
+    }
+    const int dt = k.column->dtype, w = dtype_width(dt);
+    const int64_t run_bytes = (p ? 16 : 0) + (q ? 16 : 0) + (f.kind == WIN_FR_RANGE ? 2 * dtype_width(f.key_dtype) : 0);
+    ColOwner tmp(c);
+    cudaError_t e = cudaSuccess;
+    if (win_is_value(k.function)) {
+        TRY(col_alloc(c, dt, {ChunkPlan{n, true}}, nullptr, 0, tmp.out()));
+        const int64_t words = (n + 31) / 32;
+        Scratch<uint32_t> vwords;
+        Scratch<unsigned long long> vprefix, block_sums;
+        const bool ranks = k.ignore_nulls && nullable;   // IGNORE NULLS over a column with nulls: the popcount prefix of its validity
+        if (ranks) {
+            const int64_t blocks = (words + window_count_tile() - 1) / window_count_tile();
+            e = vwords.alloc(c, (size_t)words * sizeof(uint32_t));
+            if (e == cudaSuccess) e = vprefix.alloc(c, (size_t)(words + 1) * sizeof(unsigned long long));
+            if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long));
+            if (e == cudaSuccess) {
+                LaunchTimer t(c, BDF_K_WINDOW, BDF_U32, n, bitmap_bytes(n) * 2 + words * (8 + 16));   // validity words, popcounts, scan
+                c->launches += 2;                                                                      // the scan's two kernels
+                e = launch_window_valid_words(table, n_chunks, n, vwords, c->s_compute);
+                if (e == cudaSuccess) e = launch_window_count(vwords, words, vprefix, block_sums, c->s_compute);
+                if (e == cudaSuccess) e = launch_join_scan(vprefix, words, block_sums, c->s_compute);
+            }
+        }
+        if (e == cudaSuccess) {
+            LaunchTimer t(c, BDF_K_WINDOW, dt, n, n * (2 * w + run_bytes) + (nullable ? bitmap_bytes(n) : 0) + bitmap_bytes(n) + (ranks ? words * 12 : 0));
+            const int which = k.function - BDF_WIN_FIRST_VALUE;   // 0 first, 1 last, 2 nth
+            e = launch_window_frame_value(dt, which, k.offset, p, n_p, q, n_q, f, table, n_chunks, n, ranks ? vwords.get() : nullptr,
+                                          ranks ? vprefix.get() : nullptr, tmp->chunks[0].values, tmp->chunks[0].validity, c->s_compute);
+        }
+    } else {
+        const int fn = k.function - BDF_WIN_SUM;   // SUM, COUNT, MIN, MAX, AVG: the order of k_window.cu's scans
+        const int od = win_out_dtype(k);
+        const bool out_nullable = k.function == BDF_WIN_MIN || k.function == BDF_WIN_MAX || k.function == BDF_WIN_AVG;
+        TRY(col_alloc(c, od, {ChunkPlan{n, out_nullable}}, nullptr, 0, tmp.out()));
+        const int levels = window_frame_levels(n);
+        if (hier->of != src) {
+            hier->of = nullptr;
+            hier->bytes.reset(new Scratch<void>());
+            e = hier->bytes->alloc(c, window_frame_scratch_bytes(dt, n));
+            if (e == cudaSuccess && levels > 0) {
+                const int64_t rec = dtype_is_float(dt) ? 32 : 40;   // sizeof(WinAcc<T>)
+                LaunchTimer t(c, BDF_K_WINDOW, dt, n, n * w + (nullable ? bitmap_bytes(n) : 0) + (int64_t)((double)n * 2.07 * rec));
+                c->launches += levels - 1;
+                e = launch_window_frame_build(dt, table, n_chunks, n, hier->bytes->get(), c->s_compute);
+            }
+            if (e == cudaSuccess) hier->of = src;
+        }
+        if (e == cudaSuccess) {
+            const int64_t rec = dtype_is_float(dt) ? 32 : 40;
+            LaunchTimer t(c, BDF_K_WINDOW, od, n, n * (dtype_width(od) + run_bytes + 2 * (levels + 1) * rec) + (out_nullable ? bitmap_bytes(n) : 0));
+            e = launch_window_frame_agg(dt, fn, p, n_p, q, n_q, f, table, n_chunks, n, hier->bytes->get(), tmp->chunks[0].values,
+                                        out_nullable ? tmp->chunks[0].validity : nullptr, c->s_compute);
+        }
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "window frame");
+    *out = tmp.release();
+    return BDF_OK;
 }
 
 static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_order, const bdf_sort_key* order, int n_calls,
@@ -2884,12 +3005,16 @@ static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_
         if (!x) return fail(BDF_INVALID, "null partition or order column");
     for (int j = 0; j < n_calls; j++) {
         const bdf_window_call& k = calls[j];
-        if (k.function < BDF_WIN_ROW_NUMBER || k.function > BDF_WIN_AVG) return fail(BDF_UNSUPPORTED, "unknown window function %d", k.function);
+        if (k.function < BDF_WIN_ROW_NUMBER || k.function > BDF_WIN_NTH_VALUE) return fail(BDF_UNSUPPORTED, "unknown window function %d", k.function);
         if (win_is_rank(k.function) && k.column) return fail(BDF_INVALID, "a ranking function takes no column");
         if (!win_is_rank(k.function) && !k.column) return fail(BDF_INVALID, "lag, lead and the aggregates need a column");
         if (win_is_shift(k.function) && k.offset < 0) return fail(BDF_INVALID, "lag / lead offset must be >= 0");
-        if (!win_is_rank(k.function) && !win_is_shift(k.function) && (k.frame < BDF_FRAME_ROWS || k.frame > BDF_FRAME_PARTITION))
+        if (!win_is_rank(k.function) && !win_is_shift(k.function) && (k.frame < BDF_FRAME_ROWS || k.frame > BDF_FRAME_RANGE_BETWEEN))
             return fail(BDF_UNSUPPORTED, "unknown window frame %d", k.frame);
+        if (k.ignore_nulls && !win_is_value(k.function)) return fail(BDF_INVALID, "IGNORE NULLS is for first_value, last_value and nth_value");
+        if (k.function == BDF_WIN_NTH_VALUE && k.offset < 1) return fail(BDF_INVALID, "nth_value needs n >= 1");
+        if (k.frame == BDF_FRAME_RANGE_BETWEEN && !win_is_rank(k.function) && !win_is_shift(k.function) && n_order != 1)
+            return fail(BDF_INVALID, "RANGE BETWEEN needs exactly one order column");
         if (k.column) cols.push_back(k.column);
     }
     for (const bdf_col* x : cols)
@@ -2897,6 +3022,14 @@ static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_
     for (int j = 0; j < n_calls; j++)
         if (calls[j].function == BDF_WIN_AVG && (calls[j].column->dtype == BDF_I64 || calls[j].column->dtype == BDF_U64))
             return fail(BDF_UNSUPPORTED, "avg needs f64: From<T::Native>");
+    const bool float_key = n_order == 1 && (order[0].column->dtype == BDF_F32 || order[0].column->dtype == BDF_F64);
+    std::vector<bdf_window_call> norm(calls, calls + n_calls);   // the calls with their frames resolved (win_normalise)
+    for (auto& k : norm) {
+        if (win_is_rank(k.function) || win_is_shift(k.function)) continue;
+        if (win_bounded(k.frame)) TRY(win_check_bounds(k, float_key));
+        k = win_normalise(k, float_key);
+    }
+    calls = norm.data();
     if (cols.empty()) {
         if (n_calls == 0) return BDF_OK;
         return fail(BDF_INVALID, "a window without partition, order or value columns has no rows to number");
@@ -2927,7 +3060,10 @@ static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_
         const int f = calls[j].function;
         if (f == BDF_WIN_RANK || f == BDF_WIN_DENSE_RANK || f == BDF_WIN_PERCENT_RANK || f == BDF_WIN_CUME_DIST) need_q = true;
         else if (win_is_shift(f)) need_inv = need_inv || sorted;
-        else if (!win_is_rank(f)) {
+        else if (win_is_value(f) || win_bounded(calls[j].frame)) {   // bounded frames: computed in sorted order, one take back
+            need_inv = need_inv || sorted;
+            if (calls[j].frame == BDF_FRAME_RANGE) need_q = true;
+        } else if (!win_is_rank(f)) {
             const int fr = calls[j].frame;
             if (fr == BDF_FRAME_ROWS) need_inv = need_inv || sorted;
             else if (fr == BDF_FRAME_RANGE && sorted) { need_q = true; need_range = true; }
@@ -3018,6 +3154,8 @@ static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_
         *src = gathered.back().second.get();
         return BDF_OK;
     };
+    const std::function<int(const bdf_col*, const bdf_col**)> source_fn = source;
+    WinHierarchy hier;
     for (int j = 0; j < n_calls; j++) {
         const bdf_window_call& k = calls[j];
         if (win_is_rank(k.function)) continue;
@@ -3030,7 +3168,11 @@ static int window_dev(bdf_ctx* c, int n_part, const bdf_col* const* part, int n_
         const int dt = k.column->dtype, w = dtype_width(dt);
         ColOwner tmp(c);
         const bdf_col* idx = nullptr;   // sorted order back to row order; null: tmp already is in row order
-        if (win_is_shift(k.function)) {
+        if (win_is_value(k.function) || win_bounded(k.frame)) {
+            TRY(window_frame_call(c, k, has_p ? P.arrays : nullptr, P.n_runs, has_q ? Q.arrays : nullptr, Q.n_runs, src, table, n_chunks, nullable,
+                                  n_order == 1 && sorted ? order[0] : bdf_sort_key{nullptr, 0}, sorted ? &source_fn : nullptr, n, &hier, tmp.out()));
+            idx = sorted ? inv.get() : nullptr;
+        } else if (win_is_shift(k.function)) {
             TRY(col_alloc(c, dt, {ChunkPlan{n, true}}, nullptr, 0, tmp.out()));
             LaunchTimer t(c, BDF_K_WINDOW, dt, n, n * (2 * w + (has_p ? 8 : 0)) + (nullable ? bitmap_bytes(n) : 0) + bitmap_bytes(n));
             e = launch_window_shift(dt, p_arrays, P.n_runs, n, table, n_chunks, k.offset, k.function == BDF_WIN_LEAD ? 1 : 0, k.default_bits,

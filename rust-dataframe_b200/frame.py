@@ -166,7 +166,8 @@ def plan_join(schema_a: Dict[str, int], schema_b: Dict[str, int], criteria: Sequ
 
 def window(partition_by: Sequence[str], order_by: Sequence[Tuple[str, bool]], calls: Sequence[tuple]):
     """Window functions over one WindowSpec: ``calls`` are ``(output, function, *arguments)`` with column arguments by name, e.g.
-    ``("r", "rank")``, ``("prev", "lag", "x", 1, 0.0)`` or ``("s", "sum", "x", "range")`` (see functions.window)."""
+    ``("r", "rank")``, ``("prev", "lag", "x", 1, 0.0)``, ``("s", "sum", "x", "range")``, a moving average ``("ma", "avg", "x", ("rows", -99, 0))``
+    or a forward fill ``("x", "last_value", "x", ("rows", None, 0), True)`` (see functions.window)."""
     return ("window", (list(partition_by), [(c, bool(d)) for c, d in order_by], [tuple(c) for c in calls]))
 
 
@@ -181,7 +182,8 @@ def plan_window(schema: Dict[str, int], partition_by: Sequence[str], order_by: S
     """The frame after a window step, as [(name, dtype)]: the frame's columns, then every call's output in call order; an output
     whose name exists replaces that column in place of the old one at the end, as with_column does.  A missing column is a
     ComputeError; an unknown function, a non-numeric column and avg of Int64 / UInt64 are UnsupportedType.  Output types: UInt32
-    for row_number / rank / dense_rank, Float64 for percent_rank / cume_dist / avg, Int64 for count, the column's type otherwise."""
+    for row_number / rank / dense_rank, Float64 for percent_rank / cume_dist / avg, Int64 for count, the column's type otherwise
+    (lag / lead, sum / min / max, first_value / last_value / nth_value)."""
     for name in _window_columns(partition_by, order_by, calls):
         if name not in schema:
             raise N.ComputeError(f"Window column {json.dumps(name)} does not exist")

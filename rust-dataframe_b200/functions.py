@@ -13,12 +13,14 @@ Every function makes exactly one call into libb200df.so (CUDA); nothing here com
 from __future__ import annotations
 
 import ctypes as C
+import datetime
+import math
 from typing import List, Optional, Sequence
 
 import numpy as np
 
 from . import _native as N
-from .arrays import F64, I64, NP_DTYPES, PrimitiveArray, TemporalType, is_float, width_of
+from .arrays import DATE32, DATE64, F32, F64, I64, NP_DTYPES, TIMESTAMP, PrimitiveArray, TemporalType, is_float, width_of
 
 Chunks = Sequence[PrimitiveArray]
 
@@ -922,10 +924,67 @@ def join_indices(left_keys: Sequence["Column"], right_keys: Sequence["Column"], 
     return Column(ctx, hl), Column(ctx, hr)
 
 
-def _window_call(call: tuple, ordered: bool) -> "N.WindowCall":
+_INT64_MIN, _INT64_MAX = -2 ** 63, 2 ** 63 - 1
+_TIMESTAMP_UNIT_US = (10 ** 6, 1000, 1)   # microseconds per arrow TimeUnit s, ms, us (ns: x 1000)
+
+
+def _frame_offset(v, key, upper: bool):
+    """One bound of a ("rows" | "range", start, end) frame as the C call takes it: None is UNBOUNDED (PRECEDING for the start, FOLLOWING
+    for the end).  A RANGE offset is typed by the order key: a float offset for a Float32 / Float64 key, an integer otherwise, and a
+    datetime.timedelta for a Date or Timestamp key, converted to the key's unit (days for Date32, ms for Date64)."""
+    is_float = key is not None and key[0] in (F32, F64)
+    if v is None:
+        return (math.inf if upper else -math.inf) if is_float else (_INT64_MAX if upper else _INT64_MIN)
+    if isinstance(v, datetime.timedelta):
+        t = key[1] if key is not None else None
+        if t is None or t.kind not in (DATE32, DATE64, TIMESTAMP):
+            raise N.ComputeError("a timedelta frame offset needs a Date or Timestamp order key")
+        us = (v.days * 86_400 + v.seconds) * 10 ** 6 + v.microseconds
+        if t.kind == TIMESTAMP and t.unit == 3:
+            return us * 1000
+        per = {DATE32: 86_400 * 10 ** 6, DATE64: 1000}.get(t.kind) or _TIMESTAMP_UNIT_US[t.unit]
+        if us % per:
+            raise N.ComputeError(f"frame offset {v!r} is not a whole number of the order key's unit")
+        return us // per
+    if is_float:
+        return float(v)
+    if isinstance(v, float) and not v.is_integer():
+        raise N.ComputeError(f"frame offset {v!r} over an integer order key must be an integer")
+    return int(v)
+
+
+def _window_frame(k: "N.WindowCall", frame, ordered: bool, key) -> None:
+    if frame is None:
+        frame = "range" if ordered else "partition"
+    if isinstance(frame, tuple):
+        if len(frame) != 3 or frame[0] not in N.BOUNDED_FRAMES:
+            raise N.UnsupportedType(f"window frame {frame!r} is not (\"rows\" | \"range\", start, end)")
+        k.frame = N.BOUNDED_FRAMES[frame[0]]
+        rng = frame[0] == "range"
+        s, e = (_frame_offset(frame[1], key if rng else None, False), _frame_offset(frame[2], key if rng else None, True))
+        if rng and key is not None and key[0] in (F32, F64):
+            k.start_f, k.end_f = s, e
+        else:
+            for v in (s, e):
+                if not _INT64_MIN <= v <= _INT64_MAX:
+                    raise N.ComputeError(f"frame offset {v} does not fit Int64")
+            k.start, k.end = s, e
+        return
+    if frame not in N.WINDOW_FRAMES:
+        raise N.UnsupportedType(f"window frame {frame!r} is not one of {sorted(N.WINDOW_FRAMES)}")
+    k.frame = N.WINDOW_FRAMES[frame]
+
+
+_WINDOW_VALUES = ("first_value", "last_value", "nth_value")
+
+
+def _window_call(call: tuple, ordered: bool, key=None) -> "N.WindowCall":
     """One call tuple -> bdf_window_call.  ``("row_number",)`` .. ``("cume_dist",)``; ``("lag" | "lead", x, offset=1, default=None)``;
-    ``("sum" | "count" | "min" | "max" | "avg", x, frame=None)`` with frame "rows", "range" or "partition" (None: SQL's default, "range"
-    with an ORDER BY and "partition" without)."""
+    ``("sum" | "count" | "min" | "max" | "avg", x, frame=None)``; ``("first_value" | "last_value", x, frame=None, ignore_nulls=False)``
+    and ``("nth_value", x, n, frame=None, ignore_nulls=False)``.  A frame is "rows", "range" or "partition" (None: SQL's default,
+    "range" with an ORDER BY and "partition" without), or a bounded ``("rows" | "range", start, end)`` with signed offsets (negative =
+    PRECEDING, 0 = CURRENT ROW, positive = FOLLOWING, None = UNBOUNDED).  ``key``: (dtype, TemporalType or None) of the single order
+    column, which types RANGE offsets."""
     name = call[0]
     if name not in N.WINDOW_FNS:
         raise N.UnsupportedType(f"window function {name!r} is not one of {sorted(N.WINDOW_FNS)}")
@@ -939,7 +998,7 @@ def _window_call(call: tuple, ordered: bool) -> "N.WindowCall":
     if len(call) < 2:
         raise N.ComputeError(f"{name} needs a column")
     x = call[1]
-    if name not in ("lag", "lead", "min", "max", "count"):
+    if name not in ("lag", "lead", "min", "max", "count") + _WINDOW_VALUES:
         _refuse_temporal(name, x)
     k.column = x.handle.value if isinstance(x.handle, C.c_void_p) else x.handle
     if fn in (N.WIN_LAG, N.WIN_LEAD):
@@ -950,23 +1009,31 @@ def _window_call(call: tuple, ordered: bool) -> "N.WindowCall":
             k.default_bits = int.from_bytes(raw.ljust(8, b"\0"), "little")
             k.has_default = 1
         return k
-    frame = call[2] if len(call) > 2 and call[2] is not None else ("range" if ordered else "partition")
-    if frame not in N.WINDOW_FRAMES:
-        raise N.UnsupportedType(f"window frame {frame!r} is not one of {sorted(N.WINDOW_FRAMES)}")
-    k.frame = N.WINDOW_FRAMES[frame]
+    rest = list(call[2:])
+    if name == "nth_value":
+        if not rest:
+            raise N.ComputeError("nth_value needs n")
+        k.offset = int(rest.pop(0))
+    _window_frame(k, rest[0] if rest else None, ordered, key)
+    if name in _WINDOW_VALUES:
+        k.ignore_nulls = 1 if len(rest) > 1 and rest[1] else 0
+    elif len(rest) > 1:
+        raise N.ComputeError(f"{name} takes a column and a frame")
     return k
 
 
 def window(partition_by: Sequence["Column"], order_by: Sequence[tuple], calls: Sequence[tuple]) -> List["Column"]:
     """Window functions over one specification (bdf_window_dev): rows are partitioned by the tuple of ``partition_by`` columns
     and ordered inside a partition by ``order_by`` (``[(Column, descending)]``; nulls last in both directions, ties in row order).
-    ``calls`` are tuples as ``_window_call`` describes, e.g. ``("row_number",)``, ``("lag", x, 1, 0.0)`` or ``("sum", x, "range")``.
-    Returns one one-chunk Column per call, in the caller's row order: row r of each belongs to input row r."""
+    ``calls`` are tuples as ``_window_call`` describes, e.g. ``("row_number",)``, ``("lag", x, 1, 0.0)``, ``("sum", x, "range")``,
+    ``("avg", x, ("rows", -99, 0))`` or ``("last_value", x, ("rows", None, 0), True)`` (forward fill).  Returns one one-chunk Column
+    per call, in the caller's row order: row r of each belongs to input row r."""
     cols = list(partition_by) + [c for c, _ in order_by] + [c[1] for c in calls if len(c) > 1]
     ctx = cols[0].ctx if cols else N.default_context()
+    key = (order_by[0][0].dtype, getattr(order_by[0][0], "temporal", None)) if len(order_by) == 1 else None
     arr = (N.WindowCall * max(len(calls), 1))()
     for j, call in enumerate(calls):
-        arr[j] = _window_call(call, bool(order_by))
+        arr[j] = _window_call(call, bool(order_by), key)
     handle = lambda c: c.handle.value if isinstance(c.handle, C.c_void_p) else c.handle
     pk = (C.c_void_p * max(len(partition_by), 1))(*[handle(c) for c in partition_by])
     ok = (N.SortKeyC * max(len(order_by), 1))()
@@ -974,7 +1041,7 @@ def window(partition_by: Sequence["Column"], order_by: Sequence[tuple], calls: S
         ok[i].column, ok[i].descending = handle(c), 1 if desc else 0
     out = (C.c_void_p * max(len(calls), 1))()
     N.raise_for_status(N.lib().bdf_window_dev(ctx.handle, len(partition_by), pk, len(order_by), ok, len(calls), arr, out))
-    carry = lambda c: getattr(c[1], "temporal", None) if c[0] in ("lag", "lead", "min", "max") else None
+    carry = lambda c: getattr(c[1], "temporal", None) if c[0] in ("lag", "lead", "min", "max") + _WINDOW_VALUES else None
     return [Column(ctx, C.c_void_p(out[j]), carry(calls[j])) for j in range(len(calls))]
 
 
