@@ -689,7 +689,9 @@ def _timed_calls(ctx, fn, reps=3):
 def lists_bench(ctx, rows, rows_out):
     """ArrayFunctions over rows elements of Int64 and Float64 in 25 chunks at mean list lengths 4, 32 and 1000 (lengths uniform in
     [1, 2 * mean - 1]: no empty list, so max / min are defined), plus one hot list of rows / 10 elements among about rows one-element lists.
-    Algorithmic bytes: offsets and elements read once, plus what is written."""
+    Algorithmic bytes: offsets and elements read once, plus what is written.  Then list take by a random permutation of the lists beside
+    the flat take of the elements by a random permutation of the same count, list filter keeping 50 %, and collect_list / collect_set
+    of rows Float64 values by an Int32 key of about 1e6 groups beside group-by count of the same columns."""
     card = _card()
     stream = _stream_rates(rows)["read"]
     print(f"card: {card}; tune_stream read-only rate {stream:.1f} GB/s", flush=True)
@@ -727,6 +729,14 @@ def lists_bench(ctx, rows, rows_out):
                      ("array_repeat(2)", lambda: c.array_repeat(2), lambda o: E * w + off_b + 2 * E * w + 4 * (N_ + 1), False),
                      ("array_union(self)", lambda: c.array_union(c), lambda o: 2 * (E * w + off_b) + len(o.values()) * w + 4 * (N_ + 1), False),
                      ("explode", lambda: c.explode(), lambda o: E * w + off_b + E * (w + 4), False)]
+            # whole lists moved between rows (frames: sort / join / filter), beside the flat take of the same element count
+            perm = rdf.Column.upload([rdf.PrimitiveArray.from_numpy(rng.permutation(N_).astype(np.uint32))], ctx)
+            eperm = rdf.Column.upload([rdf.PrimitiveArray.from_numpy(rng.permutation(E).astype(np.uint32))], ctx)
+            flat = c.values()
+            mask = rdf.Column.upload([rdf.BooleanArray.from_numpy(rng.random(c.chunk_info(k)["len"]) < 0.5) for k in range(n_chunks)], ctx)
+            cases += [("take, flat elements (yardstick)", lambda: flat.take(eperm), lambda o: E * (4 + 2 * w), False),
+                      ("list take (random permutation)", lambda: c.take(perm), lambda o: E * (4 + 2 * w) + 4 * N_ + 2 * off_b + 20 * N_, False),
+                      ("list filter 50 %", lambda: c.filter(mask), lambda o: len(o) * 24 + len(o.values()) * (4 + 2 * w) + N_ / 8, False)]
             for name, fn, nbytes, single in cases:
                 ms, out = _timed_calls(ctx, fn)
                 b = nbytes(out)
@@ -737,6 +747,14 @@ def lists_bench(ctx, rows, rows_out):
                 print(f"{name:28s} {rdf.DTYPE_NAMES[dt]:8s} {label:10s} {ms:9.3f} ms {gbs:8.1f} GB/s{frac}", flush=True)
                 del out
             c.free()
+    # lists built per group, beside group-by count of the same shape: Float64 values by an Int32 key of about 1e6 groups
+    keys = rdf.Column.upload([rdf.PrimitiveArray.from_numpy(rng.integers(0, 1_000_000, per).astype(np.int32)) for _ in range(n_chunks)], ctx)
+    x = rdf.Column.upload([rdf.PrimitiveArray.from_numpy(rng.normal(size=per), rng.random(per) > 0.1) for _ in range(n_chunks)], ctx)
+    for fn in ("count", "collect_list", "collect_set"):
+        ms, out = _timed_calls(ctx, lambda: rdf.group_by([keys], [(x, fn)]))
+        rows_out.append({"case": f"group-by {fn} Float64 by Int32, 1e6 groups", "ms": ms, "rows": per * n_chunks, "card": card})
+        print(f"group-by {fn:26s} Float64 1e6 groups {ms:9.3f} ms", flush=True)
+        del out
 
 
 def temporal_bench(ctx, rows, rows_out):

@@ -139,6 +139,19 @@ for dtype in (rdf.I8, rdf.U16, rdf.I64, rdf.F32, rdf.F64):
         col.download()
     nonempty = rdf.ListColumn.upload([rdf.ListArray.from_pylist(dtype, [[1, None], [None], None, [k % 100 for k in range(70000)]])])
     nonempty.array_max().download(); nonempty.array_min().download()
+    # whole lists between rows: take with null and repeated indices (the hot 20000-element lists several times), filter per chunk
+    n_l = len(la)
+    idx = rng.integers(0, n_l, 3 * n_l).astype(np.uint32)
+    idx[:40] = (np.arange(40) * 7) % n_l
+    la.take(rdf.Column.upload([P.from_numpy(idx, rng.random(idx.shape[0]) > 0.1)])).download()
+    lens_la = [la.chunk_info(k)["len"] for k in range(la.n_chunks)]
+    la.filter(rdf.Column.upload([rdf.BooleanArray.from_numpy(rng.random(n) < 0.5, rng.random(n) > 0.1) for n in lens_la])).download()
+# collect_list / collect_set over groups whose values are all null, a null key group, one-row groups
+ck = rdf.Column.upload([P.from_numpy(rng.integers(0, 50, n).astype(np.int32), rng.random(n) > 0.05) for n in lens])
+cx = rdf.Column.upload([P.from_numpy(rng.integers(0, 9, n).astype(np.float64), rng.random(n) > 0.5) for n in lens])
+cn = rdf.Column.upload([P.from_numpy(np.zeros(n), np.zeros(n, dtype=bool)) for n in lens])
+for r in rdf.group_by([ck], [(cx, "collect_list"), (cx, "collect_set"), (cn, "collect_list"), (cn, "collect_set")])[1]:
+    r.download()
 # the Parquet writer: ragged and offset chunks, nulls, every encoding path (PLAIN, dictionary, Boolean bits), snappy fragments, row
 # groups cut across chunks, and a frame without rows
 import tempfile

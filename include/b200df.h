@@ -331,6 +331,22 @@ typedef enum { BDF_GROUP_SUM = 0, BDF_GROUP_MAX, BDF_GROUP_MIN, BDF_GROUP_AVG, B
 typedef struct { const bdf_col* column; int32_t function; } bdf_group_agg;
 int  bdf_group_by_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_col* const* keys, int32_t n_aggs, const bdf_group_agg* aggs,
                       bdf_col** out_keys /* n_keys */, bdf_col** out /* n_aggs */, int64_t* n_groups);
+/* Lists per group (ArrayFunction::CollectList / CollectSet, src/expression.rs; Spark's collect_list / collect_set, made deterministic).
+ * bdf_group_by_lists_dev is bdf_group_by_dev that also takes the two list builders, all in one call over ONE sort of the keys.  A
+ * collect aggregation writes out_lists[j] and sets out[j] = NULL; every other aggregation writes out[j] and sets out_lists[j] = NULL.
+ * bdf_group_by_dev keeps refusing ids 48 and 49 (BDF_UNSUPPORTED): its outputs cannot hold a list.  Keys, value columns, group order
+ * and errors are those of bdf_group_by_dev.  Every list result has ONE chunk of n_groups lists, no NULL list and no null element:
+ *   COLLECT_LIST  The valid values of the group in row order (chunk order, then row).  Null values are skipped; a group without a
+ *                 valid value gives a valid EMPTY list.
+ *   COLLECT_SET   The distinct valid values of the group, ascending in DataFrame::sort's order (NaN greatest).  Equality is that of
+ *                 COUNT_DISTINCT: all NaNs are one value, -0.0 == 0.0; the bits kept are those of the value's first occurrence in
+ *                 row order.  Empty and null rules as COLLECT_LIST.  Costs the second sort of COUNT_DISTINCT, once per value column
+ *                 however many COLLECT_SET aggregations name it.
+ * More than 2^31 - 1 elements in one result -> BDF_UNSUPPORTED (Int32 offsets).  On failure nothing is returned and nothing leaks. */
+typedef enum { BDF_GROUP_COLLECT_LIST = 48, BDF_GROUP_COLLECT_SET } bdf_group_list_fn;   /* function ids of bdf_group_agg: a block of their own */
+typedef struct bdf_list bdf_list;
+int  bdf_group_by_lists_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_col* const* keys, int32_t n_aggs, const bdf_group_agg* aggs,
+                            bdf_col** out_keys /* n_keys */, bdf_col** out /* n_aggs */, bdf_list** out_lists /* n_aggs */, int64_t* n_groups);
 
 /* ---- equi-join (Transformation::Join -> DataFrame::join, src/dataframe.rs:626-719; the body of calc_equijoin_indices,
  * src/functions/join.rs:19-137) ------------------------------------------------------------------------------------------------
@@ -697,7 +713,6 @@ int  bdf_csv_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* c
  * Errors (nothing is returned and nothing leaks): a null pointer or an unknown function -> BDF_INVALID; a non-numeric child, the limits
  *   above, a multi-GPU context -> BDF_UNSUPPORTED; children of different dtypes in a set function -> BDF_UNSUPPORTED. */
 #define BDF_LIST_BASE 32   /* bdf_ipc_list_column reports a List<T> column as BDF_LIST_BASE + T */
-typedef struct bdf_list bdf_list;
 typedef struct {
     const int32_t* offsets;   /* base of the offsets buffer, NOT offset-adjusted: entries offset .. offset + len are read    */
     const uint8_t* validity;  /* list validity, LSB-first, 1 = valid; NULL when every list is valid                          */
@@ -733,6 +748,18 @@ int  bdf_list_transform_dev(bdf_ctx* ctx, int fn, const bdf_list* list, uint64_t
                             bdf_list** out);
 int  bdf_list_set_dev(bdf_ctx* ctx, int fn, const bdf_list* a, const bdf_list* b, bdf_list** out);
 int  bdf_list_explode_dev(bdf_ctx* ctx, const bdf_list* list, bdf_col** rows, bdf_col** values);
+/* Whole lists moved between rows: the list columns of a frame through take (DataFrame::sort, join, limit) and filter.
+ *   bdf_list_take_dev    out[i] = list[indices[i]] (Column::take), indices a UInt32 column whose row numbers count through the list's
+ *                        chunks.  ONE chunk.  A null index gives a null list, a null list stays null, null elements stay null with
+ *                        their bits.  Offsets start at 0 and only the elements of valid lists are copied.  An index past the end ->
+ *                        BDF_INVALID.
+ *   bdf_list_filter_dev  The lists where the Boolean mask is valid and true (ChunkedArray::filter).  The chunks of the input are kept:
+ *                        chunk i holds the kept lists of chunk i, so list columns stay RecordBatch-aligned with the numeric columns
+ *                        bdf_filter_dev filters.  Mask chunk lengths that differ from the list's -> BDF_LENGTH_MISMATCH.
+ *   Both: exact null counts (bdf_list_chunk_info); more than 2^31 - 1 result elements in one chunk -> BDF_UNSUPPORTED (Int32 offsets);
+ *   a multi-GPU context -> BDF_UNSUPPORTED.  On failure nothing is returned and nothing leaks. */
+int  bdf_list_take_dev(bdf_ctx* ctx, const bdf_list* list, const bdf_col* indices /* UInt32 */, bdf_list** out);
+int  bdf_list_filter_dev(bdf_ctx* ctx, const bdf_list* list, const bdf_col* mask /* Boolean */, bdf_list** out);
 /* List<T> columns of an IPC file.  bdf_ipc_column keeps reporting them with dtype -1 (outside the column path: bdf_ipc_read and
  * bdf_ipc_view refuse them, and readers that take every column of dtype >= 0 are unaffected); bdf_ipc_list_column gives
  * BDF_LIST_BASE + T for a List of one numeric T and -1 for every other column (LargeList, nested lists, List<bool> ...);
@@ -896,6 +923,13 @@ int  bdf_ipc_temporal_column(const bdf_ipc* file, int32_t col, bdf_temporal_type
 int  bdf_ipc_read_temporal(bdf_ctx* ctx, const bdf_ipc* file, int32_t col, int flags, bdf_col** out);
 int  bdf_ipc_write_typed(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
                          const bdf_temporal_type* types /* n_cols entries, or NULL */);
+/* bdf_ipc_write_typed with list columns: column j is lists[j] when that is non-NULL (then cols[j] must be NULL and types[j].kind 0),
+ * otherwise cols[j] as in bdf_ipc_write_typed.  A list is written as List<item: T>, field and child both nullable, the child named
+ * "item" as pyarrow names it; its FieldNodes are the list's and then the child's, its buffers the list validity, the Int32 offsets
+ * (from 0), the child validity and the child values, each on a 64-byte file offset.  List chunk b is RecordBatch b: any other chunk
+ * structure -> BDF_LENGTH_MISMATCH.  bdf_ipc_read_list reads such a column back. */
+int  bdf_ipc_write_lists(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
+                         const bdf_temporal_type* types /* or NULL */, const bdf_list* const* lists /* n_cols entries, or NULL */);
 
 /* ---- Parquet files straight to the device (DataFrame::from_parquet, src/dataframe.rs) ----------------------------------------------
  * The reference reads a file, or every file of a directory, with parquet's ParquetFileArrowReader in batches of 1024 rows.  Rules

@@ -155,6 +155,46 @@ pub fn explode<T: ArrowNumericType>(a: &ListArray) -> Result<(UInt32Array, Primi
     Ok((download_col(DataType::UInt32, rows)?, download_col(T::get_data_type(), vals)?))
 }
 
+/// Column::take of a ListArray column (DataFrame::sort / join / limit dispatch here for DataType::List): out[i] = a[indices[i]], a
+/// null index gives a null list; an index past the end is an error.  `indices` is a device UInt32 column (the sort's or the join's).
+pub fn take<T: ArrowNumericType>(a: &ListArray, indices: *const BdfCol) -> Result<ListArray, ArrowError> {
+    let l = upload::<T>(a)?;
+    let mut out = std::ptr::null_mut();
+    let st = unsafe { bdf_list_take_dev(ctx_one_gpu(), l, indices, &mut out) };
+    unsafe { bdf_list_free(ctx_one_gpu(), l) };
+    check(st)?;
+    download_list::<T>(out)
+}
+
+/// ChunkedArray::filter of a ListArray chunk: the lists where the device Boolean mask is valid and true.
+pub fn filter<T: ArrowNumericType>(a: &ListArray, mask: *const BdfCol) -> Result<ListArray, ArrowError> {
+    let l = upload::<T>(a)?;
+    let mut out = std::ptr::null_mut();
+    let st = unsafe { bdf_list_filter_dev(ctx_one_gpu(), l, mask, &mut out) };
+    unsafe { bdf_list_free(ctx_one_gpu(), l) };
+    check(st)?;
+    download_list::<T>(out)
+}
+
+/// ArrayFunction::CollectList / CollectSet per group of the device key columns: (key columns, one list per group).  collect_list: the
+/// valid values in row order; collect_set: the distinct valid values ascending (NaN greatest, -0.0 == 0.0).  Never a null list.
+fn collect<T: ArrowNumericType>(f: i32, keys: &[*const BdfCol], x: *const BdfCol) -> Result<(Vec<*mut BdfCol>, ListArray), ArrowError> {
+    let agg = BdfGroupAgg { column: x, function: f };
+    let mut out_keys = vec![std::ptr::null_mut(); keys.len()];
+    let (mut out, mut list, mut n_groups) = (std::ptr::null_mut(), std::ptr::null_mut(), 0i64);
+    check(unsafe { bdf_group_by_lists_dev(ctx_one_gpu(), keys.len() as i32, keys.as_ptr(), 1, &agg, out_keys.as_mut_ptr(), &mut out, &mut list,
+                                          &mut n_groups) })?;
+    Ok((out_keys, download_list::<T>(list)?))
+}
+
+pub fn collect_list<T: ArrowNumericType>(keys: &[*const BdfCol], x: *const BdfCol) -> Result<(Vec<*mut BdfCol>, ListArray), ArrowError> {
+    collect::<T>(BDF_GROUP_COLLECT_LIST, keys, x)
+}
+
+pub fn collect_set<T: ArrowNumericType>(keys: &[*const BdfCol], x: *const BdfCol) -> Result<(Vec<*mut BdfCol>, ListArray), ArrowError> {
+    collect::<T>(BDF_GROUP_COLLECT_SET, keys, x)
+}
+
 // In src/functions/array.rs (ArrayFunctions):
 //   pub fn array_contains<T>(array, val)  -> array_gpu::array_contains::<T>(array, val)
 //   pub fn array_position<T>(array, val)  -> array_gpu::array_position::<T>(array, val)

@@ -99,6 +99,8 @@ pub const BDF_GROUP_STDDEV_POP: i32 = 13;
 pub const BDF_GROUP_VAR_POP: i32 = 14;
 pub const BDF_GROUP_MEDIAN: i32 = 32;   // the distributions start a block of their own
 pub const BDF_GROUP_MODE: i32 = 33;
+pub const BDF_GROUP_COLLECT_LIST: i32 = 48;   // the list builders: bdf_group_by_lists_dev only
+pub const BDF_GROUP_COLLECT_SET: i32 = 49;
 /// bdf_moment_rec: count, mean and the central sums m2, m3, m4 of the valid values (read `as f64`).
 #[repr(C)]
 #[derive(Clone, Copy, Default)]
@@ -219,6 +221,9 @@ extern "C" {
     // group-by over 1..16 key columns with a flat list of (column, function) pairs; every returned column is the caller's to free
     pub fn bdf_group_by_dev(ctx: *mut BdfCtx, n_keys: i32, keys: *const *const BdfCol, n_aggs: i32, aggs: *const BdfGroupAgg,
                             out_keys: *mut *mut BdfCol, out: *mut *mut BdfCol, n_groups: *mut i64) -> c_int;
+    // the same with collect_list / collect_set: a collect aggregation writes out_lists[j] (one chunk) and sets out[j] = NULL
+    pub fn bdf_group_by_lists_dev(ctx: *mut BdfCtx, n_keys: i32, keys: *const *const BdfCol, n_aggs: i32, aggs: *const BdfGroupAgg,
+                                  out_keys: *mut *mut BdfCol, out: *mut *mut BdfCol, out_lists: *mut *mut BdfList, n_groups: *mut i64) -> c_int;
     // equi-join (calc_equijoin_indices): join_type in JoinType order (LeftJoin, RightJoin, InnerJoin, FullJoin); two UInt32 index
     // columns, NULL = no partner, to take every column of each side with
     pub fn bdf_join_indices_dev(ctx: *mut BdfCtx, join_type: i32, n_keys: i32, left_keys: *const *const BdfCol, right_keys: *const *const BdfCol,
@@ -258,6 +263,9 @@ extern "C" {
     pub fn bdf_list_transform_dev(ctx: *mut BdfCtx, func: c_int, list: *const BdfList, value_bits: u64, count: i64, out: *mut *mut BdfList) -> c_int;
     pub fn bdf_list_set_dev(ctx: *mut BdfCtx, func: c_int, a: *const BdfList, b: *const BdfList, out: *mut *mut BdfList) -> c_int;
     pub fn bdf_list_explode_dev(ctx: *mut BdfCtx, list: *const BdfList, rows: *mut *mut BdfCol, values: *mut *mut BdfCol) -> c_int;
+    // whole lists between rows: take gives one chunk, filter keeps the chunks (RecordBatch-aligned with bdf_filter_dev)
+    pub fn bdf_list_take_dev(ctx: *mut BdfCtx, list: *const BdfList, indices: *const BdfCol, out: *mut *mut BdfList) -> c_int;
+    pub fn bdf_list_filter_dev(ctx: *mut BdfCtx, list: *const BdfList, mask: *const BdfCol, out: *mut *mut BdfList) -> c_int;
     pub fn bdf_ipc_list_column(file: *const BdfIpc, col: i32, dtype: *mut i32) -> c_int;
     pub fn bdf_ipc_read_list(ctx: *mut BdfCtx, file: *const BdfIpc, col: i32, flags: c_int, out: *mut *mut BdfList) -> c_int;
     pub fn bdf_ipc_write(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol) -> c_int;
@@ -271,6 +279,9 @@ extern "C" {
     pub fn bdf_ipc_read_temporal(ctx: *mut BdfCtx, file: *const BdfIpc, col: i32, flags: c_int, out: *mut *mut BdfCol) -> c_int;
     pub fn bdf_ipc_write_typed(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol,
                                types: *const BdfTemporalType) -> c_int;
+    // column j is lists[j] (List<item: T>) when that is non-null, cols[j] otherwise
+    pub fn bdf_ipc_write_lists(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol,
+                               types: *const BdfTemporalType, lists: *const *const BdfList) -> c_int;
     // Parquet files straight to the device (include/b200df.h "Parquet files straight to the device")
     pub fn bdf_parquet_open(path: *const c_char, options: *const BdfParquetOptions, out: *mut *mut BdfParquet) -> c_int;
     pub fn bdf_parquet_describe(file: *const BdfParquet, n_columns: *mut i32, n_batches: *mut i64, n_rows: *mut i64) -> c_int;

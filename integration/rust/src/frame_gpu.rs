@@ -81,6 +81,41 @@ pub fn sort_device(frame: &DeviceColumns, criteria: &[(usize, bool)]) -> Result<
     Ok(out)
 }
 
+/// Column::take of one column of a frame, as sort / join / limit call it: a DataType::List column goes through bdf_list_take_dev (whole
+/// lists, one chunk; a null index gives a null list), every other column through bdf_take_dev.  ChunkedArray::filter dispatches the same
+/// way to bdf_list_filter_dev, which keeps the chunks, so list chunk b stays RecordBatch b for to_arrow (bdf_ipc_write_lists).
+pub enum DeviceColumn { Flat(*mut BdfCol), List(*mut BdfList) }
+
+pub fn take_column(c: &DeviceColumn, indices: *const BdfCol) -> Result<DeviceColumn, String> {
+    match c {
+        DeviceColumn::Flat(col) => {
+            let mut out: *mut BdfCol = std::ptr::null_mut();
+            check(unsafe { bdf_take_dev(dev(), *col, indices, &mut out) })?;
+            Ok(DeviceColumn::Flat(out))
+        }
+        DeviceColumn::List(list) => {
+            let mut out: *mut BdfList = std::ptr::null_mut();
+            check(unsafe { bdf_list_take_dev(dev(), *list, indices, &mut out) })?;
+            Ok(DeviceColumn::List(out))
+        }
+    }
+}
+
+pub fn filter_column(c: &DeviceColumn, mask: *const BdfCol) -> Result<DeviceColumn, String> {
+    match c {
+        DeviceColumn::Flat(col) => {
+            let mut out: *mut BdfCol = std::ptr::null_mut();
+            check(unsafe { bdf_filter_dev(dev(), *col, mask, &mut out) })?;
+            Ok(DeviceColumn::Flat(out))
+        }
+        DeviceColumn::List(list) => {
+            let mut out: *mut BdfList = std::ptr::null_mut();
+            check(unsafe { bdf_list_filter_dev(dev(), *list, mask, &mut out) })?;
+            Ok(DeviceColumn::List(out))
+        }
+    }
+}
+
 /// One aggregate of the plan `Dataset::try_aggregate` makes (src/expression.rs:114-221): the ones on this path.
 #[derive(Clone, Copy, PartialEq)]
 pub enum GroupFn { Sum, Count, Min, Max }

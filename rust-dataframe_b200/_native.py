@@ -39,6 +39,8 @@ GROUP_FNS = {"sum": GROUP_SUM, "max": GROUP_MAX, "min": GROUP_MIN, "avg": GROUP_
              "skewness": GROUP_SKEWNESS, "stddev": GROUP_STDDEV, "sum_distinct": GROUP_SUM_DISTINCT, "variance": GROUP_VARIANCE,
              "stddev_pop": GROUP_STDDEV_POP, "var_pop": GROUP_VAR_POP, "exact_median": GROUP_MEDIAN,
              "mode": GROUP_MODE}
+GROUP_COLLECT_LIST, GROUP_COLLECT_SET = 48, 49   # the list builders: bdf_group_by_lists_dev only
+COLLECT_FNS = {"collect_list": GROUP_COLLECT_LIST, "collect_set": GROUP_COLLECT_SET}
 # bdf_stat
 STAT_VARIANCE, STAT_VAR_POP, STAT_STDDEV, STAT_STDDEV_POP, STAT_SKEWNESS, STAT_KURTOSIS = range(6)
 STATS = {"variance": STAT_VARIANCE, "var_pop": STAT_VAR_POP, "stddev": STAT_STDDEV, "stddev_pop": STAT_STDDEV_POP,
@@ -261,6 +263,7 @@ def lib() -> C.CDLL:
         "bdf_take_dev": ([vp, vp, vp, P(vp)], C.c_int),
         "bdf_group_aggregate_dev": ([vp, vp, i32, P(vp), P(vp), P(GroupOut), P(i64)], C.c_int),
         "bdf_group_by_dev": ([vp, i32, P(vp), i32, P(GroupAggC), P(vp), P(vp), P(i64)], C.c_int),
+        "bdf_group_by_lists_dev": ([vp, i32, P(vp), i32, P(GroupAggC), P(vp), P(vp), P(vp), P(i64)], C.c_int),
         "bdf_join_indices_dev": ([vp, i32, i32, P(vp), P(vp), P(vp), P(vp), P(i64)], C.c_int),
         "bdf_window_dev": ([vp, i32, P(vp), i32, P(SortKeyC), i32, P(WindowCall), P(vp)], C.c_int),
         "bdf_compare_dev": ([vp, C.c_int, vp, vp, C.c_double, P(vp)], C.c_int),
@@ -326,6 +329,8 @@ def lib() -> C.CDLL:
         "bdf_list_transform_dev": ([vp, C.c_int, vp, u64, i64, P(vp)], C.c_int),
         "bdf_list_set_dev": ([vp, C.c_int, vp, vp, P(vp)], C.c_int),
         "bdf_list_explode_dev": ([vp, vp, P(vp), P(vp)], C.c_int),
+        "bdf_list_take_dev": ([vp, vp, vp, P(vp)], C.c_int),
+        "bdf_list_filter_dev": ([vp, vp, vp, P(vp)], C.c_int),
         "bdf_ipc_list_column": ([vp, i32, P(i32)], C.c_int),
         "bdf_ipc_read_list": ([vp, vp, i32, C.c_int, P(vp)], C.c_int),
         "bdf_temporal": ([vp, C.c_int, P(TemporalTypeC), i64, i64, P(View), P(Out)], C.c_int),
@@ -335,6 +340,7 @@ def lib() -> C.CDLL:
         "bdf_ipc_temporal_column": ([vp, i32, P(TemporalTypeC)], C.c_int),
         "bdf_ipc_read_temporal": ([vp, vp, i32, C.c_int, P(vp)], C.c_int),
         "bdf_ipc_write_typed": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(TemporalTypeC)], C.c_int),
+        "bdf_ipc_write_lists": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(TemporalTypeC), P(vp)], C.c_int),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError if the library does not export a declared symbol
@@ -353,7 +359,7 @@ EXPORTED_SYMBOLS = [
     "bdf_host_alloc", "bdf_host_free", "bdf_host_register", "bdf_host_unregister", "bdf_binary", "bdf_unary", "bdf_cast",
     "bdf_aggregate", "bdf_aggregate_all", "bdf_avg", "bdf_upload", "bdf_upload_many", "bdf_col_wait", "bdf_col_describe",
     "bdf_col_chunk_info", "bdf_binary_dev", "bdf_unary_dev", "bdf_cast_dev", "bdf_aggregate_dev",
-    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_join_indices_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
+    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_group_by_lists_dev", "bdf_join_indices_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
     "bdf_binary_agg_dev", "bdf_binary_agg_dev_async", "bdf_aggregate_all_dev_async", "bdf_future_wait", "bdf_col_free", "bdf_profile_enable", "bdf_profile_read",
     "bdf_launch_count", "bdf_timer_start", "bdf_timer_stop", "bdf_flush_l2", "bdf_generate",
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",
@@ -363,9 +369,10 @@ EXPORTED_SYMBOLS = [
     "bdf_moments", "bdf_moments_dev", "bdf_moments_stat", "bdf_moments_merge", "bdf_distinct", "bdf_distinct_dev",
     "bdf_list_upload", "bdf_list_describe", "bdf_list_chunk_info", "bdf_list_download", "bdf_list_values", "bdf_list_free",
     "bdf_list_find_dev", "bdf_list_reduce_dev", "bdf_list_transform_dev", "bdf_list_set_dev", "bdf_list_explode_dev",
+    "bdf_list_take_dev", "bdf_list_filter_dev",
     "bdf_ipc_list_column", "bdf_ipc_read_list",
     "bdf_temporal", "bdf_temporal_dev", "bdf_temporal_binary_dev", "bdf_temporal_result", "bdf_ipc_temporal_column", "bdf_ipc_read_temporal",
-    "bdf_ipc_write_typed",
+    "bdf_ipc_write_typed", "bdf_ipc_write_lists",
     "bdf_parquet_open", "bdf_parquet_describe", "bdf_parquet_column", "bdf_parquet_temporal_column", "bdf_parquet_check", "bdf_parquet_read",
     "bdf_parquet_stats", "bdf_parquet_close", "bdf_parquet_write",
     "bdf_percentile", "bdf_percentile_dev", "bdf_mode", "bdf_mode_dev", "bdf_uniques_dev", "bdf_hist_dev", "bdf_hist_density",

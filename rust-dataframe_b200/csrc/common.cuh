@@ -555,5 +555,16 @@ cudaError_t launch_list_repeat(const int32_t* base, long long n_lists, long long
 cudaError_t launch_list_size(const int32_t* off, const uint32_t* lvalid, long long len, int32_t* out, cudaStream_t s);
 cudaError_t launch_list_minmax_valid(const int32_t* off, const uint32_t* lvalid, const uint32_t* nonempty, long long len, uint32_t* valid, int* empty,
                                      cudaStream_t s);
+struct ListChunkDesc {         // one list chunk in the concatenated list rows and elements of a take / filter
+    const int32_t* off;        // len + 1 offsets from 0
+    const uint32_t* valid;     // list validity at bit 0, or nullptr
+    long long start, elem0;    // first global list row and first global element of the chunk
+};
+cudaError_t launch_list_take_sizes(const void* idx_table, int n_idx, long long n, const void* list_table, int n_lists, long long total, int local,
+                                   uint32_t* const* vout, unsigned long long* sizes, uint32_t* first, unsigned long long* nulls, int* flags,
+                                   cudaStream_t s);
+cudaError_t launch_list_take_rows(const unsigned long long* off, long long n, const uint32_t* first, long long n_out, uint32_t* src, cudaStream_t s);
+cudaError_t launch_list_rebase(const unsigned long long* off, long long len, int32_t* out, cudaStream_t s);
+cudaError_t launch_list_ranks(const uint32_t* kept, long long n_kept, const uint32_t* starts, long long n_groups, int32_t* out, cudaStream_t s);
 
 }  // namespace bdf

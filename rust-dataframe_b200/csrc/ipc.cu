@@ -576,7 +576,9 @@ size_t fb_struct_vec(FbOut& o, const void* data, uint32_t count, size_t elem) { 
     return p;
 }
 
-// Schema table (fields of primitive / boolean type) at the current end of `o`; returns its position.
+size_t fb_field(FbOut& o, const char* name, int dt, const bdf_temporal_type* type);
+
+// Schema table (fields of primitive, boolean, temporal or List<numeric> type) at the current end of `o`; returns its position.
 size_t fb_schema(FbOut& o, int n_cols, const char* const* names, const int32_t* dtypes, const bdf_temporal_type* types) {
     std::vector<size_t> refs;
     const size_t schema = fb_table(o, {{1, 0, 0}}, &refs);
@@ -587,39 +589,51 @@ size_t fb_schema(FbOut& o, int n_cols, const char* const* names, const int32_t* 
     const size_t slots = o.b.size();
     o.b.resize(slots + 4 * (size_t)n_cols, 0);
     for (int c = 0; c < n_cols; c++) {
-        const int dt = dtypes[c];
-        const int kind = types ? types[c].kind : 0;
-        uint8_t tt = dt == BDF_BOOL ? T_Bool : (dt == BDF_F32 || dt == BDF_F64) ? T_FloatingPoint : T_Int;
-        if (kind == BDF_DATE32 || kind == BDF_DATE64) tt = T_Date;
-        if (kind == BDF_TIME32 || kind == BDF_TIME64) tt = T_Time;
-        if (kind == BDF_TIMESTAMP) tt = T_Timestamp;
-        std::vector<size_t> fr;
-        // Field: name(0) nullable(1) type_type(2) type(3) children(5)
-        const size_t field = fb_table(o, {{0, 0, 0}, {1, 1, 1}, {2, 1, tt}, {3, 0, 0}, {5, 0, 0}}, &fr);
+        const size_t field = fb_field(o, names[c], dtypes[c], types ? &types[c] : nullptr);
         o.link(slots + 4 * (size_t)c, field);
-        o.link(fr[0], fb_string(o, names[c]));
-        size_t ty;
-        if (tt == T_Bool) ty = fb_table(o, {}, nullptr);
-        else if (tt == T_Date) ty = fb_table(o, {{0, 2, (uint64_t)(kind == BDF_DATE32 ? 0 : 1)}}, nullptr);
-        else if (tt == T_Time) ty = fb_table(o, {{0, 2, (uint64_t)types[c].unit}, {1, 4, (uint64_t)(kind == BDF_TIME32 ? 32 : 64)}}, nullptr);
-        else if (tt == T_Timestamp) {
-            std::vector<size_t> tr;
-            if (types[c].tz) {
-                ty = fb_table(o, {{0, 2, (uint64_t)types[c].unit}, {1, 0, 0}}, &tr);
-                o.link(tr[0], fb_string(o, types[c].tz));
-            } else ty = fb_table(o, {{0, 2, (uint64_t)types[c].unit}}, nullptr);
-        }
-        else if (tt == T_FloatingPoint) ty = fb_table(o, {{0, 2, (uint64_t)(dt == BDF_F32 ? 1 : 2)}}, nullptr);
-        else {
-            static const int bw[8] = {8, 16, 32, 64, 8, 16, 32, 64};
-            ty = fb_table(o, {{0, 4, (uint64_t)bw[dt]}, {1, 1, (uint64_t)(dt <= BDF_I64 ? 1 : 0)}}, nullptr);
-        }
-        o.link(fr[1], ty);
-        o.pad_to(4);
-        o.link(fr[2], o.b.size());
-        o.put<uint32_t>(0);   // children: empty vector
     }
     return schema;
+}
+
+// One nullable Field; a List<T> (dtype BDF_LIST_BASE + T) has one child field, pyarrow's "item" of type T.
+size_t fb_field(FbOut& o, const char* name, int dt, const bdf_temporal_type* type) {
+    const int kind = type ? type->kind : 0;
+    const bool list = dt >= BDF_LIST_BASE;
+    uint8_t tt = list ? T_List : dt == BDF_BOOL ? T_Bool : (dt == BDF_F32 || dt == BDF_F64) ? T_FloatingPoint : T_Int;
+    if (kind == BDF_DATE32 || kind == BDF_DATE64) tt = T_Date;
+    if (kind == BDF_TIME32 || kind == BDF_TIME64) tt = T_Time;
+    if (kind == BDF_TIMESTAMP) tt = T_Timestamp;
+    std::vector<size_t> fr;
+    // Field: name(0) nullable(1) type_type(2) type(3) children(5)
+    const size_t field = fb_table(o, {{0, 0, 0}, {1, 1, 1}, {2, 1, tt}, {3, 0, 0}, {5, 0, 0}}, &fr);
+    o.link(fr[0], fb_string(o, name));
+    size_t ty;
+    if (tt == T_Bool) ty = fb_table(o, {}, nullptr);
+    else if (tt == T_Date) ty = fb_table(o, {{0, 2, (uint64_t)(kind == BDF_DATE32 ? 0 : 1)}}, nullptr);
+    else if (tt == T_Time) ty = fb_table(o, {{0, 2, (uint64_t)type->unit}, {1, 4, (uint64_t)(kind == BDF_TIME32 ? 32 : 64)}}, nullptr);
+    else if (tt == T_Timestamp) {
+        std::vector<size_t> tr;
+        if (type->tz) {
+            ty = fb_table(o, {{0, 2, (uint64_t)type->unit}, {1, 0, 0}}, &tr);
+            o.link(tr[0], fb_string(o, type->tz));
+        } else ty = fb_table(o, {{0, 2, (uint64_t)type->unit}}, nullptr);
+    }
+    else if (tt == T_FloatingPoint) ty = fb_table(o, {{0, 2, (uint64_t)(dt == BDF_F32 ? 1 : 2)}}, nullptr);
+    else if (tt == T_List) ty = fb_table(o, {}, nullptr);
+    else {
+        static const int bw[8] = {8, 16, 32, 64, 8, 16, 32, 64};
+        ty = fb_table(o, {{0, 4, (uint64_t)bw[dt]}, {1, 1, (uint64_t)(dt <= BDF_I64 ? 1 : 0)}}, nullptr);
+    }
+    o.link(fr[1], ty);
+    o.pad_to(4);
+    o.link(fr[2], o.b.size());
+    o.put<uint32_t>(list ? 1 : 0);   // children
+    if (list) {
+        const size_t slot = o.b.size();
+        o.put<uint32_t>(0);
+        o.link(slot, fb_field(o, "item", dt - BDF_LIST_BASE, nullptr));
+    }
+    return field;
 }
 
 struct Block { int64_t offset; int32_t meta_len; int32_t pad; int64_t body_len; };
@@ -648,6 +662,11 @@ struct ChunkSpec {
     bool has_validity = false;            // a validity buffer is written (always when nulls > 0)
     int64_t validity_pos = 0, values_pos = 0;   // absolute file offsets (filled by plan_file)
     int64_t validity_len = 0, values_len = 0;
+    // a List<T> column: the offsets, then the child's node and buffers
+    int64_t offsets_pos = 0, offsets_len = 0;
+    int64_t child_rows = 0, child_nulls = 0;
+    bool child_has_validity = false;
+    int64_t child_validity_pos = 0, child_values_pos = 0, child_validity_len = 0, child_values_len = 0;
 };
 
 // The whole file is laid out before a byte of data moves: metadata is small and known up front, so the file can be
@@ -699,20 +718,32 @@ void plan_file(int n_cols, const char* const* names, const int32_t* dtypes, cons
         const int64_t rows = spec[0][b].rows;
         struct Node { int64_t len, nulls; };
         struct Buf { int64_t off, len; };
-        std::vector<Node> nodes((size_t)n_cols);
-        std::vector<Buf> bufs(2 * (size_t)n_cols);
+        std::vector<Node> nodes;
+        std::vector<Buf> bufs;
         int64_t body = 0;
+        auto buffer = [&](int64_t len, int64_t* pos) {   // positions are relative for now
+            bufs.push_back({body, len});
+            *pos = body;
+            body += (len + 63) / 64 * 64;
+        };
         for (int c = 0; c < n_cols; c++) {
             ChunkSpec& cs = spec[c][b];
-            nodes[c] = {rows, cs.nulls};
+            const bool list = dtypes[c] >= BDF_LIST_BASE;
+            nodes.push_back({rows, cs.nulls});
             cs.validity_len = cs.has_validity ? (rows + 7) / 8 : 0;
-            dtype_bytes(dtypes[c], rows, &cs.values_len);
-            bufs[2 * c] = {body, cs.validity_len};
-            cs.validity_pos = body;                      // relative for now
-            body += (cs.validity_len + 63) / 64 * 64;
-            bufs[2 * c + 1] = {body, cs.values_len};
-            cs.values_pos = body;
-            body += (cs.values_len + 63) / 64 * 64;
+            buffer(cs.validity_len, &cs.validity_pos);
+            if (list) {   // List<T>: validity, offsets; then the child node with its validity and values
+                cs.offsets_len = 4 * (rows + 1);
+                buffer(cs.offsets_len, &cs.offsets_pos);
+                nodes.push_back({cs.child_rows, cs.child_nulls});
+                cs.child_validity_len = cs.child_has_validity ? (cs.child_rows + 7) / 8 : 0;
+                buffer(cs.child_validity_len, &cs.child_validity_pos);
+                dtype_bytes(dtypes[c] - BDF_LIST_BASE, cs.child_rows, &cs.child_values_len);
+                buffer(cs.child_values_len, &cs.child_values_pos);
+            } else {
+                dtype_bytes(dtypes[c], rows, &cs.values_len);
+                buffer(cs.values_len, &cs.values_pos);
+            }
         }
         FbOut fb;
         fb.put<uint32_t>(0);
@@ -721,12 +752,15 @@ void plan_file(int n_cols, const char* const* names, const int32_t* dtypes, cons
         fb.link(0, msg);
         const size_t rb = fb_table(fb, {{0, 8, (uint64_t)rows}, {1, 0, 0}, {2, 0, 0}}, &rr);
         fb.link(mr[0], rb);
-        fb.link(rr[0], fb_struct_vec(fb, nodes.data(), (uint32_t)n_cols, 16));
-        fb.link(rr[1], fb_struct_vec(fb, bufs.data(), 2 * (uint32_t)n_cols, 16));
+        fb.link(rr[0], fb_struct_vec(fb, nodes.data(), (uint32_t)nodes.size(), 16));
+        fb.link(rr[1], fb_struct_vec(fb, bufs.data(), (uint32_t)bufs.size(), 16));
         fb.pad_to(8);
         Block blk{pos, 0, 0, body};
         frame_message(plan, &pos, fb, &blk.meta_len);
-        for (int c = 0; c < n_cols; c++) { spec[c][b].validity_pos += pos; spec[c][b].values_pos += pos; }
+        for (int c = 0; c < n_cols; c++)
+            for (int64_t* p : {&spec[c][b].validity_pos, &spec[c][b].values_pos, &spec[c][b].offsets_pos, &spec[c][b].child_validity_pos,
+                               &spec[c][b].child_values_pos})
+                *p += pos;
         pos += body;
         blocks.push_back(blk);
     }
@@ -853,15 +887,24 @@ int bdf_ipc_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* co
 
 int bdf_ipc_write_typed(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
                         const bdf_temporal_type* types) {
+    if (!cols) return ipc_fail(BDF_INVALID, "null argument");
+    return bdf_ipc_write_lists(ctx, path, n_cols, names, cols, types, nullptr);
+}
+
+int bdf_ipc_write_lists(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
+                        const bdf_temporal_type* types, const bdf_list* const* lists) {
     if (!ctx || !path || !names || !cols || n_cols <= 0) return ipc_fail(BDF_INVALID, "null argument");
     std::vector<int32_t> dtypes((size_t)n_cols);
     std::vector<std::vector<ChunkSpec>> spec((size_t)n_cols);
     int64_t n_batches = -1;
     for (int c = 0; c < n_cols; c++) {
         int64_t nch = 0, total = 0;
-        if (!cols[c] || !names[c]) return ipc_fail(BDF_INVALID, "null column or name");
-        int st = bdf_col_describe(cols[c], &dtypes[c], &nch, &total);
+        const bdf_list* l = lists ? lists[c] : nullptr;
+        if (!(l ? !cols[c] : cols[c] != nullptr) || !names[c]) return ipc_fail(BDF_INVALID, "column %d: null column or name, or both a column and a list", c);
+        if (l && types && types[c].kind) return ipc_fail(BDF_INVALID, "list column '%s' cannot carry a temporal type", names[c]);
+        int st = l ? bdf_list_describe(l, &dtypes[c], &nch, &total) : bdf_col_describe(cols[c], &dtypes[c], &nch, &total);
         if (st != BDF_OK) return st;
+        if (l) dtypes[c] += BDF_LIST_BASE;
         if (types && types[c].kind) {   // the same validation as the temporal functions' (bdf_temporal_result)
             int32_t rd = 0;
             st = bdf_temporal_result(BDF_TEMPORAL_UNIX_TIMESTAMP, &types[c], 0, &rd, nullptr);
@@ -875,12 +918,22 @@ int bdf_ipc_write_typed(bdf_ctx* ctx, const char* path, int32_t n_cols, const ch
         spec[c].resize((size_t)nch);
         for (int64_t b = 0; b < nch; b++) {
             int64_t len = 0, nulls = 0; int32_t hv = 0;
-            st = bdf_col_chunk_info(ctx, cols[c], b, &len, &nulls, &hv);
-            if (st != BDF_OK) return st;
+            ChunkSpec& cs = spec[c][b];
+            if (l) {
+                int64_t ne = 0, cl = 0, cn = 0; int32_t chv = 0;
+                st = bdf_list_chunk_info(ctx, l, b, &len, &nulls, &ne);
+                if (st == BDF_OK) st = bdf_col_chunk_info(ctx, bdf_list_values(l), b, &cl, &cn, &chv);
+                if (st != BDF_OK) return st;
+                hv = nulls > 0;
+                cs.child_rows = cl; cs.child_nulls = chv ? cn : 0; cs.child_has_validity = chv != 0;
+            } else {
+                st = bdf_col_chunk_info(ctx, cols[c], b, &len, &nulls, &hv);
+                if (st != BDF_OK) return st;
+            }
             if (len != spec[0][b].rows && c > 0)
                 return ipc_fail(BDF_LENGTH_MISMATCH, "chunk %lld: column '%s' has %lld rows, column '%s' has %lld", (long long)b, names[c], (long long)len,
                                 names[0], (long long)spec[0][b].rows);
-            spec[c][b].rows = len; spec[c][b].nulls = hv ? nulls : 0; spec[c][b].has_validity = hv != 0;
+            cs.rows = len; cs.nulls = hv ? nulls : 0; cs.has_validity = hv != 0;
         }
     }
     FilePlan plan;
@@ -890,18 +943,33 @@ int bdf_ipc_write_typed(bdf_ctx* ctx, const char* path, int32_t n_cols, const ch
     if (st != BDF_OK) return st;
     // device -> host copies land in the mapping: every column's chunks go to their final place in the file
     std::vector<std::vector<bdf_out>> outs((size_t)n_cols);
+    std::vector<std::vector<bdf_list_out>> louts((size_t)n_cols);
+    std::vector<std::vector<uint8_t>> unused_bits;   // the bitmap of a list chunk without a null list is downloaded, not written
     for (int c = 0; c < n_cols; c++) {
-        outs[c].resize((size_t)std::max<int64_t>(n_batches, 1));
+        const size_t nb = (size_t)std::max<int64_t>(n_batches, 1);
+        if (lists && lists[c]) louts[c].resize(nb);
+        else outs[c].resize(nb);
         for (int64_t b = 0; b < n_batches; b++) {
             const ChunkSpec& cs = spec[c][b];
-            outs[c][b] = bdf_out{of.map + cs.values_pos, cs.has_validity ? of.map + cs.validity_pos : nullptr, cs.rows, 0, 0};
+            if (lists && lists[c]) {
+                uint8_t* lv = of.map + cs.validity_pos;
+                if (!cs.has_validity) {
+                    unused_bits.emplace_back((size_t)(cs.rows + 7) / 8 + 8);
+                    lv = unused_bits.back().data();
+                }
+                louts[c][b] = bdf_list_out{(int32_t*)(of.map + cs.offsets_pos), lv, of.map + cs.child_values_pos,
+                                           cs.child_has_validity ? of.map + cs.child_validity_pos : nullptr, 0, 0, 0, 0};
+            } else {
+                outs[c][b] = bdf_out{of.map + cs.values_pos, cs.has_validity ? of.map + cs.validity_pos : nullptr, cs.rows, 0, 0};
+            }
         }
     }
     int begun = 0;
-    for (; begun < n_cols && st == BDF_OK; begun++) st = bdf_download_begin(ctx, cols[begun], outs[begun].data());
+    for (; begun < n_cols && st == BDF_OK; begun++)
+        if (!(lists && lists[begun])) st = bdf_download_begin(ctx, cols[begun], outs[begun].data());
     if (st != BDF_OK) begun--;   // the failing column never started
     for (int c = 0; c < begun; c++) {
-        const int s2 = bdf_download_end(ctx, cols[c], outs[c].data());
+        const int s2 = lists && lists[c] ? bdf_list_download(ctx, lists[c], louts[c].data()) : bdf_download_end(ctx, cols[c], outs[c].data());
         if (st == BDF_OK) st = s2;
     }
     return of.commit(path, st);

@@ -16,6 +16,13 @@
 //   k_list_offsets   the offsets of a result from the list numbers of its kept elements (in list order): one binary search per list.
 //   k_list_repeat    array_repeat's gather indices, one thread per OUTPUT element (binary search of the output offsets).
 //   k_list_size / k_list_minmax_valid  size, and the validity / empty-list check of max and min (folded by k_group_reduce).
+//   k_list_take_sizes  take / filter of whole lists, one thread per OUTPUT list: the size and first element of its source list (0 for
+//                    a null index or a null list), and its validity bit (warp-aggregated atomicOr: an output chunk may start
+//                    inside a word).  k_list_take_rows then gives every output element its source element, one thread per OUTPUT
+//                    element (binary search of the scanned sizes, as k_list_repeat), so one hot list is spread over the GPU;
+//                    take_dev gathers the elements.
+//   k_list_rebase    Int32 offsets of one output chunk from the 64-bit scan of all output sizes.
+//   k_list_ranks     collect_list / collect_set offsets: the rank of every group start among the sorted rows that are kept.
 #include "sort_keys.cuh"
 
 namespace bdf {
@@ -391,6 +398,119 @@ cudaError_t launch_list_minmax_valid(const int32_t* off, const uint32_t* lvalid,
                                      cudaStream_t s) {
     if (len <= 0) return cudaSuccess;
     k_list_minmax_valid<<<(unsigned)((len + kThreads - 1) / kThreads), kThreads, 0, s>>>(off, lvalid, nonempty, len, valid, empty);
+    return cudaGetLastError();
+}
+
+// ---- take / filter of whole lists -----------------------------------------------------------------------------------------------
+// The list chunk of global list row r: the last chunk whose start is <= r (empty chunks share their start with the next one).
+__device__ __forceinline__ int list_chunk_of(const ListChunkDesc* __restrict__ t, int n, long long r) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (t[mid].start <= r) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// Output list i is source list idx[i] (take: a global row; local: a row of list chunk ic, where ic is the index chunk of i).
+// sizes[i] = its element count, first[i] = its first element in the concatenated children; its validity bit goes to bit
+// (i - chunk start) of vout[ic] (local) or bit i of vout[0]; nulls[ic or 0] counts the null outputs.
+__global__ void __launch_bounds__(kThreads)
+k_list_take_sizes(const SortChunk* __restrict__ idx, int n_idx, long long n, const ListChunkDesc* __restrict__ lists, int n_lists, long long total,
+                  int local, uint32_t* const* __restrict__ vout, unsigned long long* __restrict__ sizes, uint32_t* __restrict__ first,
+                  unsigned long long* __restrict__ nulls, int* __restrict__ flags) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    bool valid = false;
+    int ic = 0;
+    long long il = i;
+    if (i < n) {
+        ic = n_idx == 1 ? 0 : chunk_of(idx, n_idx, i);
+        const SortChunk ich = idx[ic];
+        il = i - ich.start;
+        unsigned long long size = 0;
+        uint32_t f = 0;
+        if (!ich.validity || chunk_bit(ich.validity, ich.bit_off + il)) {
+            const long long r0 = (long long)((const uint32_t*)ich.values)[il];
+            const long long r = local ? lists[ic].start + r0 : r0;
+            if (r >= total) atomicOr(flags, 1);   // arrow take: index out of bounds is an error
+            else {
+                const int lc = local ? ic : (n_lists == 1 ? 0 : list_chunk_of(lists, n_lists, r));
+                const ListChunkDesc d = lists[lc];
+                const long long j = r - d.start;
+                if (!d.valid || bit_at(d.valid, j)) {
+                    valid = true;
+                    const int32_t b = __ldg(d.off + j);
+                    size = (unsigned long long)(__ldg(d.off + j + 1) - b);
+                    f = (uint32_t)(d.elem0 + b);
+                }
+            }
+        }
+        sizes[i] = size;
+        first[i] = f;
+    }
+    const int key = i < n ? (local ? ic : 0) : -1;
+    // validity: lanes that write the same word of the same chunk OR their bits together; one atomic per word
+    const long long bit = local ? il : i;
+    const unsigned long long word = i < n && valid ? (unsigned long long)(uintptr_t)(vout[key] + (bit >> 5)) : 0ull;
+    const unsigned same = __match_any_sync(0xffffffffu, word);
+    const unsigned bits = __reduce_or_sync(same, valid ? 1u << (bit & 31) : 0u);
+    if (word && (threadIdx.x & 31) == __ffs(same) - 1) atomicOr((uint32_t*)(uintptr_t)word, bits);
+    // null outputs per chunk, one atomic per chunk a warp touches
+    const unsigned same_chunk = __match_any_sync(0xffffffffu, key);
+    const unsigned n_null = __popc(__ballot_sync(0xffffffffu, i < n && !valid) & same_chunk);
+    if (key >= 0 && n_null && (threadIdx.x & 31) == __ffs(same_chunk) - 1) atomicAdd(nulls + key, (unsigned long long)n_null);
+}
+
+cudaError_t launch_list_take_sizes(const void* idx_table, int n_idx, long long n, const void* list_table, int n_lists, long long total, int local,
+                                   uint32_t* const* vout, unsigned long long* sizes, uint32_t* first, unsigned long long* nulls, int* flags,
+                                   cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    k_list_take_sizes<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, s>>>((const SortChunk*)idx_table, n_idx, n,
+                                                                                     (const ListChunkDesc*)list_table, n_lists, total, local, vout,
+                                                                                     sizes, first, nulls, flags);
+    return cudaGetLastError();
+}
+
+// Output element o belongs to output list p (the last p with off[p] <= o) and is element o - off[p] of its source list.
+__global__ void __launch_bounds__(kThreads)
+k_list_take_rows(const unsigned long long* __restrict__ off, long long n, const uint32_t* __restrict__ first, long long n_out, uint32_t* __restrict__ src) {
+    const long long o = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (o >= n_out) return;
+    long long lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const long long mid = (lo + hi + 1) >> 1;
+        if ((long long)__ldg(off + mid) <= o) lo = mid; else hi = mid - 1;
+    }
+    src[o] = __ldg(first + lo) + (uint32_t)(o - (long long)__ldg(off + lo));
+}
+
+cudaError_t launch_list_take_rows(const unsigned long long* off, long long n, const uint32_t* first, long long n_out, uint32_t* src, cudaStream_t s) {
+    if (n_out <= 0) return cudaSuccess;
+    k_list_take_rows<<<(unsigned)((n_out + kThreads - 1) / kThreads), kThreads, 0, s>>>(off, n, first, n_out, src);
+    return cudaGetLastError();
+}
+
+__global__ void __launch_bounds__(kThreads)
+k_list_rebase(const unsigned long long* __restrict__ off, long long len, int32_t* __restrict__ out) {
+    const long long j = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (j <= len) out[j] = (int32_t)(off[j] - off[0]);
+}
+
+cudaError_t launch_list_rebase(const unsigned long long* off, long long len, int32_t* out, cudaStream_t s) {
+    k_list_rebase<<<(unsigned)((len + 1 + kThreads - 1) / kThreads), kThreads, 0, s>>>(off, len, out);
+    return cudaGetLastError();
+}
+
+// out[g] = the number of kept sorted rows before starts[g] (kept: ascending), g < n_groups; out[n_groups] = n_kept.
+__global__ void __launch_bounds__(kThreads)
+k_list_ranks(const uint32_t* __restrict__ kept, long long n_kept, const uint32_t* __restrict__ starts, long long n_groups, int32_t* __restrict__ out) {
+    const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (g > n_groups) return;
+    out[g] = (int32_t)(g == n_groups ? n_kept : lower_bound_u32_list(kept, n_kept, __ldg(starts + g)));
+}
+
+cudaError_t launch_list_ranks(const uint32_t* kept, long long n_kept, const uint32_t* starts, long long n_groups, int32_t* out, cudaStream_t s) {
+    k_list_ranks<<<(unsigned)((n_groups + 1 + kThreads - 1) / kThreads), kThreads, 0, s>>>(kept, n_kept, starts, n_groups, out);
     return cudaGetLastError();
 }
 

@@ -1843,7 +1843,10 @@ static int sort_indices_dev(bdf_ctx* c, int n_keys, const bdf_sort_key* keys, bd
     return BDF_OK;
 }
 
-static int take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, bdf_col** out) {
+static int col_borrow(int dtype, const std::vector<DevChunk>& chunks, bdf_col** out);
+
+// keep_chunks: chunk k of the result is the take of index chunk k (one launch per chunk) instead of one chunk for all indices.
+static int take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, bdf_col** out, bool keep_chunks = false) {
     if (indices->dtype != BDF_U32) return fail(BDF_UNSUPPORTED, "take indices must be a UInt32 column");
     const int64_t n = indices->total_len;
     void *vt = nullptr, *it = nullptr;
@@ -1852,13 +1855,30 @@ static int take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, b
     TRY(sort_table(c, values, &vt, &nv, &vnull));
     TRY(sort_table(c, indices, &it, &ni, &inull));
     ColOwner o(c);
-    TRY(col_alloc(c, values->dtype, {ChunkPlan{n, vnull || inull}}, nullptr, take_tile_elems(), o.out()));
+    std::vector<ChunkPlan> plan;
+    if (keep_chunks) for (const DevChunk& ch : indices->chunks) plan.push_back(ChunkPlan{ch.len, vnull || inull});
+    else plan.push_back(ChunkPlan{n, vnull || inull});
+    TRY(col_alloc(c, values->dtype, plan, nullptr, take_tile_elems(), o.out()));
     o->counts_on_device = o->d_warp_counts != nullptr;
     cudaError_t e = cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute);
     if (e == cudaSuccess) {
         const int w = values->dtype == kBool ? 1 : dtype_width(values->dtype);
         LaunchTimer t(c, BDF_K_TAKE, values->dtype, n, n * (4 + 2 * (int64_t)w));
-        e = launch_take(values->dtype, vt, nv, it, ni, n, values->total_len, o->chunks[0].values, o->chunks[0].validity, o->d_warp_counts, c->d_flag, c->s_compute);
+        if (!keep_chunks)
+            e = launch_take(values->dtype, vt, nv, it, ni, n, values->total_len, o->chunks[0].values, o->chunks[0].validity, o->d_warp_counts, c->d_flag,
+                            c->s_compute);
+        for (size_t k = 0; keep_chunks && k < plan.size() && e == cudaSuccess; k++) {
+            if (!plan[k].len) continue;
+            ColOwner one(c);
+            void* kt = nullptr;
+            int nk = 0;
+            int st = col_borrow(BDF_U32, {indices->chunks[k]}, one.out());
+            if (st == BDF_OK) st = sort_table(c, one.get(), &kt, &nk, nullptr);
+            if (st != BDF_OK) return st;
+            const DevChunk& oc = o->chunks[k];
+            e = launch_take(values->dtype, vt, nv, kt, nk, plan[k].len, values->total_len, oc.values, oc.validity,
+                            o->d_warp_counts ? o->d_warp_counts + o->tile0[k] * kWarpsPerCta : nullptr, c->d_flag, c->s_compute);
+        }
     }
     if (e == cudaSuccess) e = finish_single_group(c, o.get());
     int flag = 0;
@@ -2089,8 +2109,13 @@ static int group_mode(bdf_ctx* c, const DistinctRuns& dr, const uint32_t* d_star
     return take_dev(c, dr.sval.get(), rows.get(), out);
 }
 
+static bool group_is_collect(int fn) { return fn == BDF_GROUP_COLLECT_LIST || fn == BDF_GROUP_COLLECT_SET; }
+static void drop(bdf_ctx* c, bdf_list* l);
+static int group_collect(bdf_ctx* c, const SortedRuns& runs, const bdf_col* x, int fn, const DistinctRuns* dr, bdf_list** out);
+
+// out_lists == nullptr: the entry without list outputs (bdf_group_by_dev), which does not know the collect functions.
 static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int n_aggs, const bdf_group_agg* aggs, bdf_col** out_keys, bdf_col** out,
-                        int64_t* n_groups_out) {
+                        bdf_list** out_lists, int64_t* n_groups_out) {
     if (n_keys < 1 || n_keys > 16) return fail(BDF_INVALID, "1..16 group key columns");
     for (int k = 0; k < n_keys; k++) {
         if (!keys[k]) return fail(BDF_INVALID, "null key column");
@@ -2102,7 +2127,7 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
         if (!v) return fail(BDF_INVALID, "null value column");
         if (v->dtype < 0 || v->dtype >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "aggregated columns must be numeric");
         const int fn = aggs[j].function;
-        if (!((fn >= BDF_GROUP_SUM && fn <= BDF_GROUP_VAR_POP) || fn == BDF_GROUP_MEDIAN || fn == BDF_GROUP_MODE))
+        if (!((fn >= BDF_GROUP_SUM && fn <= BDF_GROUP_VAR_POP) || fn == BDF_GROUP_MEDIAN || fn == BDF_GROUP_MODE || (out_lists && group_is_collect(fn))))
             return fail(BDF_UNSUPPORTED, "unknown group function %d", fn);
         if (aggs[j].function == BDF_GROUP_AVG && (v->dtype == BDF_I64 || v->dtype == BDF_U64)) return fail(BDF_UNSUPPORTED, "avg needs f64: From<T::Native>");
         if (v->total_len != keys[0]->total_len) return fail(BDF_LENGTH_MISMATCH, "key and value columns have different lengths");
@@ -2284,8 +2309,26 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
         if (fn == BDF_GROUP_MEDIAN) TRY(group_median(c, dr, d_starts, n_groups, n, res[j].out()));
         else TRY(group_mode(c, dr, d_starts, n_groups, n, res[j].out(), nullptr));
     }
+
+    // collect_list / collect_set: lists of n_groups rows; collect_set shares one second sort per value column
+    std::vector<Owned<bdf_list>> lists;
+    for (int j = 0; j < n_aggs; j++) lists.emplace_back(c);
+    for (int j = 0; j < n_aggs; j++) {
+        const int fn = aggs[j].function;
+        if (!group_is_collect(fn)) continue;
+        if (fn == BDF_GROUP_COLLECT_LIST) { TRY(group_collect(c, runs, aggs[j].column, fn, nullptr, lists[j].out())); continue; }
+        if (lists[j].get()) continue;   // made with an earlier collect_set of the same column
+        std::vector<const bdf_col*> sorted_keys;
+        for (const ColOwner& s : runs.sorted) sorted_keys.push_back(s.get());
+        DistinctRuns dr(c);
+        TRY(distinct_runs(c, n_keys, keys, sorted_keys, aggs[j].column, runs.iota.get(), n, &dr));
+        for (int j2 = j; j2 < n_aggs; j2++)
+            if (aggs[j2].function == BDF_GROUP_COLLECT_SET && aggs[j2].column == aggs[j].column)
+                TRY(group_collect(c, runs, aggs[j].column, fn, &dr, lists[j2].out()));
+    }
     for (int k = 0; k < n_keys; k++) out_keys[k] = runs.distinct[k].release();
     for (int j = 0; j < n_aggs; j++) out[j] = res[j].release();
+    for (int j = 0; out_lists && j < n_aggs; j++) out_lists[j] = lists[j].release();
     if (n_groups_out) *n_groups_out = n_groups;
     return BDF_OK;
 }
@@ -2307,7 +2350,7 @@ static int group_aggregate_dev(bdf_ctx* c, const bdf_col* key, int n_values, con
         }
     }
     std::vector<bdf_col*> res(aggs.size(), nullptr);
-    const int st = group_by_dev(c, 1, &key, (int)aggs.size(), aggs.data(), out_keys, res.data(), n_groups_out);
+    const int st = group_by_dev(c, 1, &key, (int)aggs.size(), aggs.data(), out_keys, res.data(), nullptr, n_groups_out);
     if (st != BDF_OK) {
         for (int j = 0; j < n_values; j++) outs[j] = bdf_group_out{nullptr, nullptr, nullptr, nullptr};
         return st;
@@ -5355,6 +5398,168 @@ static int list_explode(bdf_ctx* c, const bdf_list* l, bdf_col** rows_out, bdf_c
     return BDF_OK;
 }
 
+// Take / filter of whole lists: output list i is source list rows[i].  local (filter): rows chunk k holds rows of list chunk k and
+// becomes output chunk k; otherwise rows count through the chunks and the result is one chunk.  A null row or a null list gives a
+// null list of no element; only the elements of valid lists are copied.
+static int list_gather(bdf_ctx* c, const bdf_list* l, const bdf_col* rows, bool local, bdf_list** out) {
+    const int64_t n = rows->total_len, n_lc = (int64_t)l->lens.size();
+    const size_t n_out = local ? rows->chunks.size() : 1;
+    std::vector<int64_t> out_lens;
+    if (local) for (const DevChunk& ch : rows->chunks) out_lens.push_back(ch.len);
+    else out_lens.push_back(n);
+    ListOwner res(c);
+    TRY(list_alloc(c, l->dtype, out_lens, std::vector<bool>(n_out, true), res.out()));
+    // the list chunk table and the output validity pointers, uploaded together
+    std::vector<ListChunkDesc> lt((size_t)std::max<int64_t>(n_lc, 1), ListChunkDesc{nullptr, nullptr, 0, 0});
+    int64_t start = 0, elem0 = 0;
+    for (int64_t i = 0; i < n_lc; i++) {
+        lt[i] = ListChunkDesc{l->off[i], l->valid[i], (long long)start, (long long)elem0};
+        start += l->lens[i];
+        elem0 += l->values->chunks[i].len;
+    }
+    void* it = nullptr;
+    int ni = 0;
+    TRY(sort_table(c, rows, &it, &ni, nullptr));
+    wait_groups(c->s_compute, l->values, 0, n_lc);
+    Scratch<char> tables;
+    Scratch<unsigned long long> sizes, scan_sums, nulls;
+    Scratch<uint32_t> first;
+    const size_t lt_bytes = lt.size() * sizeof(ListChunkDesc);
+    CK(tables.alloc(c, lt_bytes + n_out * sizeof(uint32_t*)));
+    CK(sizes.alloc(c, (size_t)(n + 1) * 8));
+    CK(scan_sums.alloc(c, (size_t)json_scan_sums(n) * 8));
+    CK(nulls.alloc(c, n_out * 8));
+    CK(first.alloc(c, (size_t)std::max<int64_t>(n, 1) * 4));
+    std::vector<char> host(lt_bytes + n_out * sizeof(uint32_t*));
+    memcpy(host.data(), lt.data(), lt_bytes);
+    memcpy(host.data() + lt_bytes, res->valid.data(), n_out * sizeof(uint32_t*));
+    CK(cudaMemcpyAsync(tables.get(), host.data(), host.size(), cudaMemcpyHostToDevice, c->s_compute));
+    CK(cudaMemsetAsync(nulls, 0, n_out * 8, c->s_compute));
+    for (size_t k = 0; k < n_out; k++)
+        if (out_lens[k]) CK(cudaMemsetAsync(res->valid[k], 0, align_up((size_t)bitmap_bytes(out_lens[k]), 4), c->s_compute));
+    CK(cudaMemsetAsync(c->d_flag, 0, sizeof(int), c->s_compute));
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_LIST, BDF_U64, n, n * (4 + 8 + 8 + 4) + n / 8);   // index, two offsets, size and first element
+        c->launches += 3;   // the scan's three kernels
+        e = launch_list_take_sizes(it, ni, n, tables.get(), (int)std::max<int64_t>(n_lc, 1), l->total_len, local ? 1 : 0,
+                                   (uint32_t* const*)(tables.get() + lt_bytes), sizes, first, nulls, c->d_flag, c->s_compute);
+        if (e == cudaSuccess) e = launch_json_scan(sizes, n, scan_sums, c->s_compute);
+    }
+    // the host needs the element count of every output chunk (scan entries at the chunk bounds), the null counts and the flag
+    std::vector<unsigned long long> bounds(n_out + 1), h_nulls(n_out);
+    int64_t p = 0;
+    for (size_t k = 0; k <= n_out && e == cudaSuccess; k++) {
+        e = cudaMemcpyAsync(&bounds[k], sizes + p, 8, cudaMemcpyDeviceToHost, c->s_compute);
+        if (k < n_out) p += out_lens[k];
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_nulls.data(), nulls, n_out * 8, cudaMemcpyDeviceToHost, c->s_compute);
+    int flag = 0;
+    if (e == cudaSuccess) e = flag_read(c, false, &flag);   // synchronises the compute stream
+    if (e != cudaSuccess) return fail_cuda(e, "list take (sizes)");
+    if (flag) return fail(BDF_INVALID, "take: index out of bounds");
+    const int64_t n_elem = (int64_t)bounds[n_out];
+    if (n_elem > kListMaxChunkElems) return fail(BDF_UNSUPPORTED, "a list result of 2^31 or more elements (Int32 offsets)");
+    ColOwner src(c), src_view(c), values(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n_elem, false}}, nullptr, 0, src.out()));
+    {
+        LaunchTimer t(c, BDF_K_LIST, BDF_U32, n_elem, n_elem * 4 + 4 * (int64_t)n_out + 4 * (n + (int64_t)n_out));
+        e = launch_list_take_rows(sizes, n, first, n_elem, (uint32_t*)src->chunks[0].values, c->s_compute);
+        p = 0;
+        for (size_t k = 0; k < n_out && e == cudaSuccess; k++) {
+            e = launch_list_rebase(sizes + p, out_lens[k], res->off[k], c->s_compute);
+            p += out_lens[k];
+        }
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, src.get());
+    if (e != cudaSuccess) return fail_cuda(e, "list take (rows)");
+    if (local) {   // one view of src per output chunk: the element gather keeps the chunks
+        std::vector<DevChunk> views(n_out);
+        for (size_t k = 0; k < n_out; k++)
+            views[k] = DevChunk{src->chunks[0].values + 4 * bounds[k], nullptr, (int64_t)(bounds[k + 1] - bounds[k]), 0, 0};
+        TRY(col_borrow(BDF_U32, views, src_view.out()));
+    }
+    TRY(take_dev(c, l->values, local ? src_view.get() : src.get(), values.out(), local));
+    for (size_t k = 0; k < n_out; k++) {
+        res->null_counts[k] = (int64_t)h_nulls[k];
+        res->valid_elems[k] = (int64_t)(bounds[k + 1] - bounds[k]);
+        if (!h_nulls[k]) res->valid[k] = nullptr;   // every list is valid: no bitmap (its bytes stay in the arena)
+    }
+    res->values = values.release();
+    *out = res.release();
+    return BDF_OK;
+}
+
+static int list_take(bdf_ctx* c, const bdf_list* l, const bdf_col* indices, bdf_list** out) {
+    if (indices->dtype != BDF_U32) return fail(BDF_UNSUPPORTED, "take indices must be a UInt32 column");
+    return list_gather(c, l, indices, false, out);
+}
+
+// collect_list: the valid values of x in sorted-row order (row order inside a group: the sort is stable).  collect_set: the heads
+// of the distinct runs of dr (the first occurrence in row order of every distinct valid value, ascending inside a group).  Either
+// way the groups keep their sorted row ranges, so list g starts at the rank of the group's first sorted row among the kept rows.
+static int group_collect(bdf_ctx* c, const SortedRuns& runs, const bdf_col* x, int fn, const DistinctRuns* dr, bdf_list** out) {
+    const int64_t n = runs.perm->total_len, n_groups = runs.n_runs;
+    ColOwner sval(c), valid(c), vals(c), kept(c);
+    const bdf_col* kv = nullptr;   // the kept values in sorted order
+    const bdf_col* kr = nullptr;   // their sorted rows
+    if (fn == BDF_GROUP_COLLECT_SET) {
+        TRY(filter_dev(c, dr->sval.get(), dr->dhead.get(), vals.out()));
+        kv = vals.get();
+        kr = dr->pos.get();
+    } else {
+        TRY(take_dev(c, x, runs.perm.get(), sval.out()));
+        if (sval->chunks[0].validity) {   // the validity of x in sorted order is the mask of the kept rows
+            TRY(col_borrow(kBool, {DevChunk{(char*)sval->chunks[0].validity, nullptr, n, 0, 0}}, valid.out()));
+            TRY(filter_dev(c, sval.get(), valid.get(), vals.out()));
+            TRY(filter_dev(c, runs.iota.get(), valid.get(), kept.out()));
+            kv = vals.get();
+            kr = kept.get();
+        } else {
+            kv = sval.get();
+            kr = runs.iota.get();
+        }
+    }
+    const int64_t n_elem = kv->total_len;
+    if (n_elem > kListMaxChunkElems) return fail(BDF_UNSUPPORTED, "a list result of 2^31 or more elements (Int32 offsets)");
+    ListOwner l(c);
+    TRY(list_alloc(c, x->dtype, {n_groups}, {false}, l.out()));
+    wait_groups(c->s_compute, kr, 0, 1);
+    wait_groups(c->s_compute, runs.starts.get(), 0, 1);
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_LIST, BDF_I32, n_groups, n_groups * 8 + 4);
+        e = launch_list_ranks(n_elem ? (const uint32_t*)kr->chunks[0].values : nullptr, n_elem, (const uint32_t*)runs.starts->chunks[0].values, n_groups,
+                              l->off[0], c->s_compute);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "collect offsets");
+    l->valid_elems[0] = n_elem;
+    l->values = kv == sval.get() ? sval.release() : vals.release();
+    *out = l.release();
+    return BDF_OK;
+}
+
+// The kept row numbers of every list chunk (a filter of 0 .. len-1 per chunk), then the gather with the chunks kept.
+static int list_filter(bdf_ctx* c, const bdf_list* l, const bdf_col* mask, bdf_list** out) {
+    if (mask->dtype != kBool) return fail(BDF_INVALID, "the filter mask must be a boolean column");
+    if (mask->chunks.size() != l->lens.size()) return fail(BDF_LENGTH_MISMATCH, "Filter array must have the same length as the data");
+    int64_t max_len = 0;
+    for (size_t i = 0; i < l->lens.size(); i++) {
+        if (mask->chunks[i].len != l->lens[i]) return fail(BDF_LENGTH_MISMATCH, "Filter array must have the same length as the data");
+        max_len = std::max(max_len, l->lens[i]);
+    }
+    ColOwner iota(c), rows_of(c), kept(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{max_len, false}}, nullptr, 0, iota.out()));
+    c->launches++;
+    cudaError_t e = max_len ? launch_iota((uint32_t*)iota->chunks[0].values, max_len, c->sm_count, c->s_compute) : cudaSuccess;
+    if (e != cudaSuccess) return fail_cuda(e, "list filter rows");
+    std::vector<DevChunk> views;
+    for (int64_t len : l->lens) views.push_back(DevChunk{iota->chunks[0].values, nullptr, len, 0, 0});
+    TRY(col_borrow(BDF_U32, views, rows_of.out()));
+    TRY(filter_dev(c, rows_of.get(), mask, kept.out()));
+    return list_gather(c, l, kept.get(), true, out);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // line-delimited JSON reader (k_json.cu; the rules are in include/b200df.h): the file goes to HBM as for the CSV reader; the lines
 // are found, checked and walked on the device, which lists every member of every record's object.  The host decodes the distinct
@@ -6734,7 +6939,16 @@ int bdf_group_by_dev(bdf_ctx* c, int32_t n_keys, const bdf_col* const* keys, int
     ENTER(c);
     if (!keys || !out_keys || (n_aggs && (!aggs || !out))) return fail(BDF_INVALID, "null argument");
     if (n_aggs < 0 || n_aggs > 64) return fail(BDF_INVALID, "0..64 aggregations");
-    return group_by_dev(c, n_keys, keys, n_aggs, aggs, out_keys, out, n_groups);
+    return group_by_dev(c, n_keys, keys, n_aggs, aggs, out_keys, out, nullptr, n_groups);
+}
+
+int bdf_group_by_lists_dev(bdf_ctx* c, int32_t n_keys, const bdf_col* const* keys, int32_t n_aggs, const bdf_group_agg* aggs, bdf_col** out_keys,
+                           bdf_col** out, bdf_list** out_lists, int64_t* n_groups) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "group-by moves rows between chunks: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    if (!keys || !out_keys || (n_aggs && (!aggs || !out || !out_lists))) return fail(BDF_INVALID, "null argument");
+    if (n_aggs < 0 || n_aggs > 64) return fail(BDF_INVALID, "0..64 aggregations");
+    return group_by_dev(c, n_keys, keys, n_aggs, aggs, out_keys, out, out_lists, n_groups);
 }
 
 int bdf_join_indices_dev(bdf_ctx* c, int32_t join_type, int32_t n_keys, const bdf_col* const* left_keys, const bdf_col* const* right_keys,
@@ -7262,6 +7476,18 @@ int bdf_list_explode_dev(bdf_ctx* c, const bdf_list* l, bdf_col** rows, bdf_col*
     LIST_ENTER(c);
     if (!l || !rows || !values) return fail(BDF_INVALID, "null argument");
     return list_explode(c, l, rows, values);
+}
+
+int bdf_list_take_dev(bdf_ctx* c, const bdf_list* l, const bdf_col* indices, bdf_list** out) {
+    LIST_ENTER(c);
+    if (!l || !indices || !out) return fail(BDF_INVALID, "null argument");
+    return list_take(c, l, indices, out);
+}
+
+int bdf_list_filter_dev(bdf_ctx* c, const bdf_list* l, const bdf_col* mask, bdf_list** out) {
+    LIST_ENTER(c);
+    if (!l || !mask || !out) return fail(BDF_INVALID, "null argument");
+    return list_filter(c, l, mask, out);
 }
 
 }  // extern "C"

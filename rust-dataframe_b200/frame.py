@@ -36,7 +36,7 @@ import numpy as np
 
 from . import _native as N
 from .arrays import F32, F64, I8, I64, U8, U32, U64, PrimitiveArray, is_float
-from .functions import Column, _expr_nodes, eval_expr, sort_indices, window as _window
+from .functions import Column, ListColumn, _expr_nodes, eval_expr, sort_indices, window as _window
 from .csv_reader import CsvFile, write_csv
 from .json_reader import JsonFile
 from .parquet_reader import ParquetFile, write_parquet
@@ -387,7 +387,10 @@ def _try_fuse(run: List[Calculation], needed_after_run: set, max_inputs: int, ma
 # ---------------------------------------------------------------------------------------------------------
 
 class DeviceFrame:
-    """Ordered name -> Column; every column has the same chunk lengths (the frame's RecordBatches)."""
+    """Ordered name -> Column or ListColumn; every column has the same chunk lengths (the frame's RecordBatches).  A ListColumn is
+    carried through filter, sort, limit, join, select, drop, with_column and window; it is reported in the schema as
+    ``BDF_LIST_BASE + T``, so the planners refuse it as a key or an aggregated column, and it cannot be computed on, compared or
+    sorted by."""
 
     def __init__(self, columns: "OrderedDict[str, Column]"):
         self.columns: "OrderedDict[str, Column]" = OrderedDict(columns)
@@ -417,8 +420,8 @@ class DeviceFrame:
     def from_json(cls, path: str, schema: Optional[Sequence[Tuple[str, int]]] = None, max_records: Optional[int] = None, batch_size: int = 1024,
                   ctx: Optional[N.Context] = None) -> "DeviceFrame":
         """DataFrame::from_json over a line-delimited file: one object per line, the schema inferred from every record (or the given
-        (name, dtype) pairs), 1024 rows per RecordBatch.  The numeric and Boolean columns are taken; List columns (frames do not carry
-        lists yet; read them with JsonFile.read_list) and columns off the device path are left out."""
+        (name, dtype) pairs), 1024 rows per RecordBatch.  The numeric and Boolean columns are taken; List columns (read them with
+        JsonFile.read_list and add them with with_column) and columns off the device path are left out."""
         with JsonFile(path, schema=schema, max_records=max_records, batch_size=batch_size, ctx=ctx) as f:
             names = [n for n, dt, _ in f.schema if 0 <= dt <= N.BOOL]
             cols = f.read(names)
@@ -444,9 +447,15 @@ class DeviceFrame:
     def to_arrow(self, path: str) -> None:
         write_ipc(path, dict(self.columns))
 
+    def _refuse_lists(self, what: str) -> None:
+        for n, c in self.columns.items():
+            if isinstance(c, ListColumn):
+                raise N.UnsupportedType(f"column {n!r} is a list column: {what} does not write lists (to_arrow does)")
+
     def to_csv(self, path: str, has_header: bool = True, delimiter: str = ",") -> None:
         """DataFrame::to_csv: the frame's text is formatted on the device and streamed to the file (write_csv).  A frame with a
-        temporal column is refused: its raw Int32 / Int64 values are not the text a reader would expect."""
+        temporal or a list column is refused: its raw Int32 / Int64 values are not the text a reader would expect."""
+        self._refuse_lists("the CSV writer")
         for n, c in self.columns.items():
             if getattr(c, "temporal", None) is not None:
                 raise N.UnsupportedType(f"column {n!r} is {c.temporal!r}: temporal text is not written by the CSV writer")
@@ -454,7 +463,8 @@ class DeviceFrame:
 
     def to_parquet(self, path: str, compression: str = "none", dictionary: bool = True, row_group_rows: int = 0) -> None:
         """DataFrame::to_parquet: the frame's pages are encoded (and compressed) on the device and streamed to the file
-        (write_parquet); temporal columns are written as Date / Time / Timestamp columns."""
+        (write_parquet); temporal columns are written as Date / Time / Timestamp columns.  A frame with a list column is refused."""
+        self._refuse_lists("the Parquet writer")
         write_parquet(path, self.columns, compression=compression, dictionary=dictionary, row_group_rows=row_group_rows)
 
     def to_host(self) -> Dict[str, list]:
@@ -462,12 +472,18 @@ class DeviceFrame:
 
     @property
     def schema(self) -> "OrderedDict[str, int]":
-        return OrderedDict((n, c.dtype) for n, c in self.columns.items())
+        return OrderedDict((n, N.LIST_BASE + c.dtype if isinstance(c, ListColumn) else c.dtype) for n, c in self.columns.items())
 
     def column(self, name: str) -> Column:
         if name not in self.columns:
             raise N.ReferencePanic(f"column {name!r} not found (column_by_name panics)")
         return self.columns[name]
+
+    def _numeric(self, name: str, what: str) -> Column:
+        c = self.column(name)
+        if isinstance(c, ListColumn):
+            raise N.UnsupportedType(f"column {name!r} is a list column: {what} needs a numeric column")
+        return c
 
     # -- DataFrame methods --
     def with_column(self, name: str, column: Column) -> "DeviceFrame":
@@ -482,13 +498,16 @@ class DeviceFrame:
         return DeviceFrame(OrderedDict((n, c) for n, c in self.columns.items() if n not in names))
 
     def filter(self, cond) -> "DeviceFrame":
+        for name in _filter_columns(cond):
+            if name in self.columns:
+                self._numeric(name, "a filter condition")
         mask = self._boolean(cond)
         return DeviceFrame(OrderedDict((n, c.filter(mask)) for n, c in self.columns.items()))
 
     def sort(self, criteria: Sequence[Tuple[str, bool]]) -> "DeviceFrame":
         if not criteria:
             raise N.ComputeError("Sort criteria cannot be empty")
-        idx = sort_indices([(self.column(c), d) for c, d in criteria])
+        idx = sort_indices([(self._numeric(c, "a sort key"), d) for c, d in criteria])
         return DeviceFrame(OrderedDict((n, c.take(idx)) for n, c in self.columns.items()))
 
     def group_aggregate(self, groups, aggregates: Sequence[Tuple[str, str]]) -> "DeviceFrame":
@@ -508,11 +527,13 @@ class DeviceFrame:
             groups = groups[0]
         if groups not in self.columns:
             raise N.ComputeError(f"Grouping column {groups!r} does not exist")
+        self._numeric(groups, "a group key")
         for cname, fn in aggregates:
             if cname not in self.columns:
                 raise N.ComputeError(f"Aggregating column {cname!r} does not exist")
             if fn not in ("sum", "count", "min", "max"):
                 raise N.UnsupportedType(f"aggregate {fn!r} is not on the path")
+            self._numeric(cname, "an aggregate")
             if fn == "sum" and getattr(self.columns[cname], "temporal", None) is not None:
                 raise N.UnsupportedType(f"sum of {cname!r} ({self.columns[cname].temporal!r}): temporal values are not summed")
         names = list(OrderedDict.fromkeys(c for c, _ in aggregates))
@@ -626,7 +647,7 @@ class DeviceFrame:
         fn = calc.function
         if fn == "rename":
             return DeviceFrame(OrderedDict(((calc.output if n == calc.inputs[0] else n), c) for n, c in self.columns.items()))
-        cols = [self.column(n) for n in calc.inputs]
+        cols = [self._numeric(n, "a Calculation") for n in calc.inputs]
         if fn in ARITH:
             if cols[0].dtype in (I8, U8) or cols[0].dtype == BOOL:
                 raise N.ReferencePanic("Unsupported operation")          # evaluation.rs:116-244 has no Int8/UInt8 arm
@@ -649,7 +670,7 @@ class DeviceFrame:
                 frame = frame.calculate(arg)
             elif kind == "fused":
                 try:
-                    frame = frame.with_column(arg.output, eval_expr([frame.column(n) for n in arg.inputs], arg.nodes))
+                    frame = frame.with_column(arg.output, eval_expr([frame._numeric(n, "a Calculation") for n in arg.inputs], arg.nodes))
                 except N.UnsupportedType:      # e.g. more than two live intermediates: run the Calculations one by one
                     for calc in arg.replaced:
                         frame = frame.calculate(calc)

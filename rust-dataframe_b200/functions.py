@@ -875,16 +875,22 @@ def group_aggregate(key: "Column", values: Sequence["Column"]):
 def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
     """Group-by over 1..16 key columns (bdf_group_by_dev).  ``aggregations``: ``[(Column, function)]`` with function one of
     "sum", "max", "min", "avg", "count", "count_distinct", "first", "last", "kurtosis", "skewness", "stddev", "sum_distinct",
-    "variance", "stddev_pop", "var_pop", "exact_median", "mode".  Returns ``([key Column per key], [result Column per aggregation])``; groups in the order
-    DataFrame::sort gives (ascending, nulls last per key).  Counts are Int64, avg, median and the statistics are Float64, everything else
-    has the value column's type; see include/b200df.h for the NULL rules."""
+    "variance", "stddev_pop", "var_pop", "exact_median", "mode", "collect_list", "collect_set".  Returns ``([key Column per key],
+    [result per aggregation])``; groups in the order DataFrame::sort gives (ascending, nulls last per key).  Counts are Int64, avg,
+    median and the statistics are Float64, collect_list / collect_set are ListColumns of one chunk (bdf_group_by_lists_dev, called
+    only when one of them is asked for), everything else has the value column's type; see include/b200df.h for the NULL rules.  A
+    temporal column is refused for collect: a ListColumn carries no temporal tag."""
     fns = []
     for col, fn in aggregations:
-        if fn not in N.GROUP_FNS:
+        if fn not in N.GROUP_FNS and fn not in N.COLLECT_FNS:
             raise N.UnsupportedType(f"group function {fn!r} is not on the path")
+        if isinstance(col, ListColumn):
+            raise N.UnsupportedType(f"{fn} of a list column: aggregated columns must be numeric")
         if fn not in _CARRY_GROUP and fn not in ("count", "count_distinct"):
-            _refuse_temporal(fn, col)
-        fns.append(N.GROUP_FNS[fn])
+            _refuse_temporal(fn, col)   # collect too: a ListColumn carries no temporal tag
+        fns.append(N.GROUP_FNS.get(fn, N.COLLECT_FNS.get(fn)))
+    if any(isinstance(k, ListColumn) for k in keys):
+        raise N.UnsupportedType("a list column is not a group key: group-by keys must be numeric")
     ctx = keys[0].ctx if keys else (aggregations[0][0].ctx if aggregations else N.default_context())
     nk, na = len(keys), len(aggregations)
     kcols = (C.c_void_p * max(nk, 1))(*[k.handle for k in keys])
@@ -894,10 +900,16 @@ def group_by(keys: Sequence["Column"], aggregations: Sequence[tuple]):
     hk = (C.c_void_p * max(nk, 1))()
     out = (C.c_void_p * max(na, 1))()
     ng = C.c_int64(0)
-    N.raise_for_status(N.lib().bdf_group_by_dev(ctx.handle, nk, kcols, na, aggs, hk, out, C.byref(ng)))
+    if any(fn in N.COLLECT_FNS for _, fn in aggregations):   # list outputs: the entry that can return them
+        lists = (C.c_void_p * max(na, 1))()
+        N.raise_for_status(N.lib().bdf_group_by_lists_dev(ctx.handle, nk, kcols, na, aggs, hk, out, lists, C.byref(ng)))
+    else:
+        lists = None
+        N.raise_for_status(N.lib().bdf_group_by_dev(ctx.handle, nk, kcols, na, aggs, hk, out, C.byref(ng)))
     carry = lambda col, fn: getattr(col, "temporal", None) if fn in _CARRY_GROUP else None
-    return ([Column(ctx, C.c_void_p(hk[k]), keys[k].temporal) for k in range(nk)],
-            [Column(ctx, C.c_void_p(out[j]), carry(*aggregations[j])) for j in range(na)])
+    result = lambda j: (ListColumn(ctx, C.c_void_p(lists[j])) if lists is not None and lists[j]
+                        else Column(ctx, C.c_void_p(out[j]), carry(*aggregations[j])))
+    return ([Column(ctx, C.c_void_p(hk[k]), keys[k].temporal) for k in range(nk)], [result(j) for j in range(na)])
 
 
 _CARRY_GROUP = ("min", "max", "first", "last", "mode")   # aggregations whose results are values of the column: a temporal tag carries
@@ -1254,6 +1266,15 @@ class ListColumn:
 
     def array_union(self, other: "ListColumn") -> "ListColumn":
         return self._list(N.lib().bdf_list_set_dev, N.LIST_UNION, self.handle, other.handle)
+
+    def take(self, indices: "Column") -> "ListColumn":
+        """Column::take of whole lists: out[i] = self[indices[i]] (UInt32 row numbers through the chunks), one chunk; a null
+        index gives a null list."""
+        return self._list(N.lib().bdf_list_take_dev, self.handle, indices.handle)
+
+    def filter(self, mask: "Column") -> "ListColumn":
+        """ChunkedArray::filter of whole lists: the lists where the Boolean mask is valid and true, chunk by chunk."""
+        return self._list(N.lib().bdf_list_filter_dev, self.handle, mask.handle)
 
     def explode(self):
         """(UInt32 parent row numbers, values): one row per element of every valid list; null and empty lists give none."""

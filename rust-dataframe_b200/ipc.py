@@ -176,13 +176,22 @@ def write_ipc_host(path: str, columns: Dict[str, List]) -> None:
 
 def write_ipc(path: str, columns: Dict[str, "object"]) -> None:
     """Device Columns -> IPC file (DataFrame::to_arrow).  Columns tagged with a TemporalType are written as Date / Time / Timestamp
-    fields (bdf_ipc_write_typed)."""
+    fields (bdf_ipc_write_typed); ListColumns as List<item: T> fields (bdf_ipc_write_lists)."""
+    from .functions import ListColumn
+
     names = list(columns)
     k = len(names)
     ctx = columns[names[0]].ctx
     cnames = (C.c_char_p * k)(*[s.encode() for s in names])
-    handles = (C.c_void_p * k)(*[columns[s].handle for s in names])
+    is_list = [isinstance(columns[s], ListColumn) for s in names]
+    handles = (C.c_void_p * k)(*[None if l else columns[s].handle for s, l in zip(names, is_list)])
     tags = [getattr(columns[s], "temporal", None) for s in names]
+    if any(is_list):
+        lists = (C.c_void_p * k)(*[columns[s].handle if l else None for s, l in zip(names, is_list)])
+        types = (N.TemporalTypeC * k)(*[N.TemporalTypeC(t.kind, t.unit, t.tz.encode() if t.tz is not None else None) if t is not None
+                                         else N.TemporalTypeC(0, 0, None) for t in tags])
+        N.raise_for_status(N.lib().bdf_ipc_write_lists(ctx.handle, str(path).encode(), k, cnames, handles, types, lists))
+        return
     if any(t is not None for t in tags):
         types = (N.TemporalTypeC * k)(*[N.TemporalTypeC(t.kind, t.unit, t.tz.encode() if t.tz is not None else None) if t is not None
                                          else N.TemporalTypeC(0, 0, None) for t in tags])
