@@ -15,10 +15,12 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --parquet [--csv-rows 50000000]                  # the Parquet reader rows (two temporary files: snappy, none)
     python benchmarks/kernels_bench.py --parquet-write [--csv-rows 50000000]            # the Parquet writer rows (none/PLAIN, none/dictionary, snappy/dictionary)
     python benchmarks/kernels_bench.py --distribution [--rows 100000000]                # median, hist, uniques, mode next to k_reduce and the sort
+    python benchmarks/kernels_bench.py --nulls [--rows 100000000]                       # coalesce, case_when, greatest, nanvl, is_null ... against ADD, then bench.py
 """
 from __future__ import annotations
 
 import argparse
+from collections import OrderedDict
 import json
 import os
 import sys
@@ -802,6 +804,77 @@ def temporal_bench(ctx, rows, rows_out):
         del out
 
 
+def nulls_bench(ctx, rows, rows_out):
+    """Null handling and conditional selection over rows values in 25 chunks, Float64 and Int32, 10 % nulls.  Each row: the median of
+    three calls (after a warm-up) of the summed per-launch CUDA-event records, its GB/s at the bytes a two-argument selection
+    moves (two value columns read, one written, and their bitmaps), and its time over the time of bdf_binary_dev ADD of the same two
+    columns -- the yardstick: the same rows and the same bytes."""
+    card = _card()
+    print(f"card: {card}", flush=True)
+    n_chunks = 25
+    per = rows // n_chunks
+    rng = np.random.default_rng(20261017)
+
+    def column(npdt, null_frac, nan_frac=0.0):
+        chunks = []
+        for _ in range(n_chunks):
+            v = rng.uniform(-1e3, 1e3, per).astype(npdt) if np.dtype(npdt).kind == "f" else rng.integers(-10 ** 6, 10 ** 6, per).astype(npdt)
+            if nan_frac:
+                v[rng.random(per) < nan_frac] = np.nan
+            chunks.append(rdf.PrimitiveArray.from_numpy(v, rng.random(per) >= null_frac) if null_frac else rdf.PrimitiveArray.from_numpy(v, np.ones(per, bool)))
+        return rdf.Column.upload(chunks, ctx)
+
+    def bools(p_true):
+        return rdf.Column.upload([rdf.BooleanArray.from_numpy(rng.random(per) < p_true, rng.random(per) >= 0.1) for _ in range(n_chunks)], ctx,
+                                 dtype=rdf.native.BOOL)
+
+    for name, npdt in (("Float64", np.float64), ("Int32", np.int32)):
+        w = np.dtype(npdt).itemsize
+        a, b, a0 = column(npdt, 0.1, 0.05 if w == 8 else 0.0), column(npdt, 0.1), column(npdt, 0.0)
+        c, d = column(npdt, 0.1), column(npdt, 0.1)
+        conds = [bools(0.25) for _ in range(4)]
+        n = len(a)
+        two = n * 3 * w + 3 * n / 8
+        cases = [("ADD (yardstick)", lambda: a.add(b), two),
+                 ("coalesce(a, b), 10 % nulls in a", lambda: rdf.coalesce(a, b), two),
+                 ("coalesce(a, b), 0 % nulls in a", lambda: rdf.coalesce(a0, b), two),
+                 ("coalesce(a, 0)", lambda: rdf.coalesce(a, 0), n * 2 * w + 2 * n / 8),
+                 ("case_when 1 branch", lambda: rdf.when(conds[0], a).otherwise(b), two + 2 * n / 8),
+                 ("case_when 4 branches", lambda: rdf.when(conds[0], a).when(conds[1], b).when(conds[2], c).when(conds[3], d).otherwise(a0),
+                  two + 8 * n / 8 + 3 * n / 8),
+                 ("greatest of 2", lambda: rdf.greatest(a, b), two),
+                 ("greatest of 4", lambda: rdf.greatest(a, b, c, d), n * 5 * w + 5 * n / 8)]
+        if w == 8:
+            cases.append(("nanvl(a, b)", lambda: a.nanvl(b), two))
+        # is_nan of an integer column reads no values (it is all false): only the result bitmap is written
+        cases += [("is_null(a)", lambda: a.is_null(), 2 * n / 8),
+                  ("is_nan(a)", lambda: a.is_nan(), n * w + 2 * n / 8 if w == 8 else n / 8)]
+        base = None
+        for case, fn, b_ in cases:
+            ms, out = _timed_calls(ctx, fn)
+            base = base or ms
+            gbs = b_ / ms / 1e6
+            rows_out.append({"case": f"{name} {case}", "ms": ms, "rows": n, "bytes": b_, "GBs": gbs, "vs_add": ms / base, "card": card})
+            print(f"{name} {case:36s} {ms:9.3f} ms {gbs:8.1f} GB/s  {ms / base:5.2f} x ADD", flush=True)
+            del out
+        frame = rdf.DeviceFrame(OrderedDict([("a", a), ("b", b), ("c", c), ("d", d)]))
+        ms, out = _timed_calls(ctx, lambda: frame.drop_nulls())
+        rows_out.append({"case": f"{name} drop_nulls over 4 columns", "ms": ms, "rows": n, "card": card})
+        print(f"{name} {'drop_nulls over 4 columns':36s} {ms:9.3f} ms", flush=True)
+        del out, frame
+        for col in (a, b, a0, c, d, *conds):
+            col.free()
+    # the headline step in the same call, to show it unchanged
+    import subprocess
+
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--gpus", "1", "--steps", "50", "--warmup", "10"],
+                       capture_output=True, text=True, check=True)
+    head = json.loads([ln for ln in r.stdout.splitlines() if ln.startswith("{")][-1])
+    rows_out.append({"case": "bench.py --gpus 1 (headline add+sum)", "ms": head["ms_per_step"], "rows_per_s": head["value"], "card": card})
+    print(f"bench.py --gpus 1: {head['ms_per_step']:.3f} ms per step, {head['value']:.4g} rows/s", flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
@@ -818,8 +891,16 @@ def main():
     ap.add_argument("--parquet", action="store_true", help="run the Parquet reader rows (--csv-rows rows, snappy and uncompressed)")
     ap.add_argument("--parquet-write", action="store_true", help="run the Parquet writer rows (--csv-rows rows, three encodings)")
     ap.add_argument("--distribution", action="store_true", help="run only the distribution rows (median, hist, uniques, mode)")
+    ap.add_argument("--nulls", action="store_true", help="run only the null-handling and conditional rows (coalesce, case_when, ...)")
     args = ap.parse_args()
     ctx = rdf.default_context()
+    if args.nulls:
+        rows_out = []
+        nulls_bench(ctx, args.rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"results": rows_out}, f, indent=1)
+        return
     if args.parquet_write:
         import subprocess
 

@@ -171,6 +171,19 @@ for npdt in (np.int8, np.int64, np.float32, np.float64):
     vals, cnts = dc.value_counts()
     vals.download(); cnts.download()
 rdf.Column.upload([P.from_numpy(np.full(70000, 2.5))]).median()
+# null handling and conditional selection: every kernel of k_cond.cu over ragged, offset chunks with nulls, scalars and NULL literals
+for npdt in (np.int8, np.uint16, np.int32, np.float32, np.float64, np.uint64):
+    nc = [rdf.Column.upload([P.from_numpy(rng.integers(-9, 9, n + 5).astype(npdt), rng.random(n + 5) > 0.3).slice(2 + j, n) for n in lens])
+          for j in range(3)]
+    conds = [rdf.Column.upload([rdf.BooleanArray.from_numpy(rng.random(n + 5) < 0.5, rng.random(n + 5) > 0.2).slice(1 + j, n) for n in lens], dtype=10)
+             for j in range(2)]
+    rdf.coalesce(nc[0], nc[1], 1).download(); rdf.greatest(*nc).download(); rdf.least(nc[0], None, nc[2]).download()
+    rdf.when(conds[0], nc[0]).when(conds[1], 2).end().download()
+    nc[0].is_null().download(); nc[1].is_not_null().download(); nc[2].is_nan().download()
+    if npdt in (np.float32, np.float64):
+        nc[0].nanvl(nc[1]).download()
+rdf.coalesce(conds[0], conds[1], False).download()
+rdf.when(conds[0], conds[1]).otherwise(True).download()
 # round 2: the fleet code path on one GPU, and a single-rank communicator (pack -> combine -> unpack on the stream)
 fleet = rdf.Context.multi(1)
 fa = [P.from_numpy(rng.integers(-100, 100, n).astype(np.int64), rng.random(n) > 0.3) for n in (1000, 0, 77)]

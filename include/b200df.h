@@ -208,6 +208,42 @@ int  bdf_download(bdf_ctx* ctx, const bdf_col* col, bdf_out* out /* n_chunks ent
 int  bdf_compare_dev(bdf_ctx* ctx, int op, const bdf_col* left, const bdf_col* right, double scalar, bdf_col** out);
 int  bdf_boolean_dev(bdf_ctx* ctx, int op, const bdf_col* a, const bdf_col* b, bdf_col** out);
 int  bdf_filter_dev(bdf_ctx* ctx, const bdf_col* values, const bdf_col* mask, bdf_col** out);
+/* ---- null handling and conditional selection (Spark's coalesce / greatest / least / nanvl / isnull / isnan / CASE WHEN) --------
+ * The functions the reference names in src/functions/scalar.rs with empty bodies (coalesce, greatest, least, nanv1), with
+ * Spark's definitions, and the null tests and the conditional that make them usable.
+ *   coalesce(a1..an)        1..64 arguments: per row, the first argument valid there; NULL where every argument is NULL.  NaN
+ *                           is a value, not a null.  fill_null(x, v) is coalesce(x, v); nvl / ifnull are two-argument coalesce.
+ *   greatest / least(a1..an) 2..64 arguments: nulls are skipped, NULL only where every argument is NULL.  Values are ordered as
+ *                           DataFrame::sort orders them (every NaN equal and greater than +inf, -0.0 == 0.0); among equal values
+ *                           the earliest argument wins, so greatest(-0.0, 0.0) returns the bits of -0.0.
+ *   nanvl(a, b)             Float32 / Float64: a where a is valid and not NaN, b where a is NaN (even a NULL b), NULL where a is.
+ *   case_when               1..64 branches: a row takes the value of the first branch whose condition is valid and true there
+ *                           (a NULL condition counts as false, as in SQL), else values[n_branches]; a NULL literal there is the
+ *                           missing ELSE.
+ *   is_null / is_not_null / is_nan  a Boolean column with no bitmap; is_nan of a NULL slot, of an integer or of a Boolean column
+ *                           is false.
+ * Every value of a result is copied bit for bit from the argument that supplied it (NaN payloads and the sign of zero survive):
+ * no arithmetic, so results are identical under any chunking and on any number of GPUs.
+ * Types: the value columns of a call share one dtype (else BDF_INVALID; a temporal column is its storage type here) and at least
+ * one value is a column, which gives the result type.  Boolean values are allowed in coalesce and case_when, not in greatest,
+ * least or nanvl (BDF_UNSUPPORTED); nanvl of an integer type is BDF_UNSUPPORTED.  A condition must be a Boolean column
+ * (BDF_INVALID).  A scalar holds T::Native bits (Boolean: 0 or 1).
+ * Chunks: zipped as the element-wise operators zip them -- n = the smallest chunk count among the column arguments, conditions
+ * included; chunk i of every column must have the same length (BDF_LENGTH_MISMATCH).  Chunk i of the result is RecordBatch i;
+ * it has a bitmap when some value argument can be NULL in that chunk (a bitmap there, or a NULL scalar in the call), and null
+ * counts are exact.  Chunk groups are those of the other element-wise operators: work on a chunk starts once that chunk of every
+ * column argument has landed.  Launch records: BDF_K_BINARY for value results, BDF_K_COMPARE for the null tests.
+ * Limit: a call's per-chunk descriptor takes 48 + 32 x (conditions + values) bytes of the context's 32 MiB descriptor ring, so a
+ * call of c chunks needs c x that many bytes: about 8,000 chunks with 64 branches, about 16,000 with 64 coalesce arguments, about
+ * 300,000 with two.  A larger call returns BDF_OOM; split it by chunks. */
+typedef struct { const bdf_col* column; uint64_t bits; int32_t valid; } bdf_arg;   /* column == NULL: a scalar, T::Native bits
+                                                                                      (Boolean 0/1); valid == 0: a NULL literal */
+typedef enum { BDF_ROW_COALESCE = 0, BDF_ROW_GREATEST, BDF_ROW_LEAST, BDF_ROW_NANVL } bdf_row_fn;
+typedef enum { BDF_IS_NULL = 0, BDF_IS_NOT_NULL, BDF_IS_NAN } bdf_null_test;
+int  bdf_rowwise_dev(bdf_ctx* ctx, int fn, int32_t n_args, const bdf_arg* args, bdf_col** out);
+int  bdf_case_when_dev(bdf_ctx* ctx, int32_t n_branches, const bdf_col* const* conditions,
+                       const bdf_arg* values /* n_branches + 1, last = else */, bdf_col** out);
+int  bdf_null_test_dev(bdf_ctx* ctx, int fn, const bdf_col* in, bdf_col** out);
 /* ---- N3: consecutive Calculations fused into one pass -----------------------------------------------------------
  * Evaluate::evaluate (src/evaluation.rs:66-96) materialises every Calculation; when the intermediates are not kept, the
  * chain can be evaluated per element in ONE kernel: inputs are read once, only the final column is written

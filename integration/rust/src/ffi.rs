@@ -31,6 +31,19 @@ pub enum BdfParquet {}   // the mapped files of a Parquet read, footers and page
 pub enum BdfCsv {}
 pub const BDF_PARSE: i32 = 9;   // -> ArrowError::ParseError(last_error())
 pub const BDF_UTF8: i32 = 11;   // CSV schema entry: a string column the device skips
+// include/b200df.h "null handling and conditional selection": column == null is a scalar (T::Native bits, Boolean 0 / 1);
+// valid == 0 is a NULL literal.
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct BdfArg { pub column: *const BdfCol, pub bits: u64, pub valid: i32 }
+pub const BDF_ROW_COALESCE: c_int = 0;
+pub const BDF_ROW_GREATEST: c_int = 1;
+pub const BDF_ROW_LEAST: c_int = 2;
+pub const BDF_ROW_NANVL: c_int = 3;
+pub const BDF_IS_NULL: c_int = 0;
+pub const BDF_IS_NOT_NULL: c_int = 1;
+pub const BDF_IS_NAN: c_int = 2;
+
 #[repr(C)]
 pub struct BdfCsvOptions { pub has_header: i32, pub delimiter: u8, pub max_records: i64 /* <0: all */, pub batch_size: i64 }
 #[repr(C)]
@@ -166,6 +179,11 @@ pub const BDF_DIVIDE_BY_ZERO: c_int = 2;
 pub const BDF_WOULD_PANIC: c_int = 7;
 
 extern "C" {
+    pub fn bdf_upload(ctx: *mut BdfCtx, dtype: c_int, n_chunks: i64, input: *const BdfView, flags: c_int, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_rowwise_dev(ctx: *mut BdfCtx, func: c_int, n_args: i32, args: *const BdfArg, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_case_when_dev(ctx: *mut BdfCtx, n_branches: i32, conditions: *const *const BdfCol, values: *const BdfArg /* n_branches + 1 */,
+                             out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_null_test_dev(ctx: *mut BdfCtx, func: c_int, input: *const BdfCol, out: *mut *mut BdfCol) -> c_int;
     pub fn bdf_init(device: c_int, out: *mut *mut BdfCtx) -> c_int;
     /// ONE context over `n_gpus` GPUs of the box (0 = all visible): the library shards every call by row range, each GPU
     /// moves its pieces over its own PCIe link, aggregates are combined over NVLink (grouped ncclAllReduce / peer-memory

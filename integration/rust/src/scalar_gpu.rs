@@ -56,6 +56,32 @@ fn finish<T: ArrowNumericType>(vals: Vec<MutableBuffer>, bits: Vec<MutableBuffer
     }).collect()
 }
 
+/// coalesce / greatest / least / nanvl (bdf_row_fn 0..3) over columns given as their chunks: scalar.rs's empty stubs with Spark's
+/// definitions.  Every column is uploaded, bdf_rowwise_dev runs on them, the result comes back (zip(): the smallest chunk count).
+pub fn gpu_rowwise<T: ArrowNumericType>(func: c_int, columns: Vec<Vec<&PrimitiveArray<T>>>) -> Result<Vec<PrimitiveArray<T>>, ArrowError> {
+    let dtype = dtype_id(&T::get_data_type());
+    let mut cols: Vec<*mut BdfCol> = Vec::new();
+    let free = |cols: &Vec<*mut BdfCol>| for c in cols { unsafe { bdf_col_free(ctx(), *c) } };
+    for chunks in &columns {
+        let v: Vec<BdfView> = chunks.iter().map(|a| view(*a)).collect();
+        let mut col: *mut BdfCol = std::ptr::null_mut();
+        let st = unsafe { bdf_upload(ctx(), dtype, v.len() as i64, v.as_ptr(), 0, &mut col) };
+        if st != BDF_OK { free(&cols); return Err(to_arrow_error(st)); }
+        cols.push(col);
+    }
+    let args: Vec<BdfArg> = cols.iter().map(|c| BdfArg { column: *c as *const BdfCol, bits: 0, valid: 1 }).collect();
+    let mut res: *mut BdfCol = std::ptr::null_mut();
+    let st = unsafe { bdf_rowwise_dev(ctx(), func, args.len() as i32, args.as_ptr(), &mut res) };
+    if st != BDF_OK { free(&cols); return Err(to_arrow_error(st)); }
+    let n = columns.iter().map(|c| c.len()).min().unwrap_or(0);
+    let (vals, bits, mut outs) = alloc_outputs::<T>(&columns[0][..n].iter().map(|a| a.len()).collect::<Vec<_>>());
+    let st = unsafe { bdf_download(ctx(), res, outs.as_mut_ptr()) };
+    unsafe { bdf_col_free(ctx(), res) };
+    free(&cols);
+    if st != BDF_OK { return Err(to_arrow_error(st)); }
+    Ok(finish::<T>(vals, bits, &outs))
+}
+
 /// Dates and timestamps: the temporal function `func` (bdf_temporal_fn: 0 year .. 6 hour .. 17 to_timestamp) over every chunk of a column
 /// whose DataType is Date32 / Date64 / Timestamp / Time32 / Time64; R is the result type bdf_temporal_result reports: Int32Type for the
 /// fields, Date32Type for to_date .. next_day, T for date_trunc, Int64Type for unix_timestamp, the Timestamp*Type of the target unit for
@@ -128,6 +154,8 @@ fn finish_as<R: ArrowPrimitiveType>(vals: Vec<MutableBuffer>, bits: Vec<MutableB
 //   pub fn divide<T>(left, right)       -> gpu_binary(3, left, right)     // Err(ArrowError::DivideByZero) preserved (scalar.rs:51-68)
 //   pub fn multiply / par_multiply<T>   -> gpu_binary(2, left, right)     // (scalar.rs:69-103)
 //   pub fn abs/sin/cos/tan/acos/...<T>  -> gpu_unary(op, array)           // was: scalar_op(a, |a| Ok(num::Float::sin(a)))      (scalar.rs:106-457)
+//   pub fn coalesce / greatest / least<T>(arrays: Vec<Vec<&PrimitiveArray<T>>>) -> gpu_rowwise(0 | 1 | 2, arrays)   // stubs (scalar.rs:180,264,286)
+//   pub fn nanv1<T>(a, b)               -> gpu_rowwise(3, vec![a, b])     // Spark's nanvl (stub, scalar.rs:343)
 //   pub fn hour<T>(array) -> Result<Vec<Int32Array>>  -> gpu_temporal::<T, Int32Type>(6, 0, array)   // was: compute::hour per chunk (scalar.rs:267-273)
 //   the stubs: year 0, quarter 1, month 2, day_of_month 3, day_of_year 4, day_of_week 5, minute 7, second 8  -> gpu_temporal::<T, Int32Type>
 //              to_date 9, date_add 10 (arg days), date_sub 11, add_months 12 (arg months), last_day 13, next_day 14 (arg 1..7)

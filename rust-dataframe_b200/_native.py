@@ -28,6 +28,9 @@ K_SELECT, K_HIST = 22, 23
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
+# null handling and conditional selection (bdf_row_fn, bdf_null_test)
+ROW_COALESCE, ROW_GREATEST, ROW_LEAST, ROW_NANVL = range(4)
+IS_NULL, IS_NOT_NULL, IS_NAN = range(3)
 BOOL = 10
 UTF8 = 11   # CSV schema entry only: a string column the device skips
 # bdf_group_fn (AggregateFunction order)
@@ -102,6 +105,11 @@ class DistinctRec(C.Structure):
 
 class ExprNode(C.Structure):
     _fields_ = [("op", C.c_int32), ("a", C.c_int32), ("b", C.c_int32)]
+
+
+class Arg(C.Structure):
+    """bdf_arg: a column (column != NULL) or a scalar's T::Native bits; valid == 0 is a NULL literal."""
+    _fields_ = [("column", C.c_void_p), ("bits", C.c_uint64), ("valid", C.c_int32)]
 
 
 class SortKeyC(C.Structure):
@@ -269,6 +277,9 @@ def lib() -> C.CDLL:
         "bdf_compare_dev": ([vp, C.c_int, vp, vp, C.c_double, P(vp)], C.c_int),
         "bdf_boolean_dev": ([vp, C.c_int, vp, vp, P(vp)], C.c_int),
         "bdf_filter_dev": ([vp, vp, vp, P(vp)], C.c_int),
+        "bdf_rowwise_dev": ([vp, C.c_int, i32, P(Arg), P(vp)], C.c_int),
+        "bdf_case_when_dev": ([vp, i32, P(vp), P(Arg), P(vp)], C.c_int),
+        "bdf_null_test_dev": ([vp, C.c_int, vp, P(vp)], C.c_int),
         "bdf_download": ([vp, vp, P(Out)], C.c_int),
         "bdf_download_begin": ([vp, vp, P(Out)], C.c_int),
         "bdf_download_end": ([vp, vp, P(Out)], C.c_int),
@@ -359,7 +370,7 @@ EXPORTED_SYMBOLS = [
     "bdf_host_alloc", "bdf_host_free", "bdf_host_register", "bdf_host_unregister", "bdf_binary", "bdf_unary", "bdf_cast",
     "bdf_aggregate", "bdf_aggregate_all", "bdf_avg", "bdf_upload", "bdf_upload_many", "bdf_col_wait", "bdf_col_describe",
     "bdf_col_chunk_info", "bdf_binary_dev", "bdf_unary_dev", "bdf_cast_dev", "bdf_aggregate_dev",
-    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_group_by_lists_dev", "bdf_join_indices_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
+    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_group_by_lists_dev", "bdf_join_indices_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_rowwise_dev", "bdf_case_when_dev", "bdf_null_test_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
     "bdf_binary_agg_dev", "bdf_binary_agg_dev_async", "bdf_aggregate_all_dev_async", "bdf_future_wait", "bdf_col_free", "bdf_profile_enable", "bdf_profile_read",
     "bdf_launch_count", "bdf_timer_start", "bdf_timer_stop", "bdf_flush_l2", "bdf_generate",
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",

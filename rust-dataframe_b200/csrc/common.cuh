@@ -231,6 +231,26 @@ struct CsvwDesc {
     int32_t dtype; int32_t pad;
 };
 
+// Null handling and conditional selection (k_cond.cu): one header per chunk followed by its arguments, so the stride of the
+// descriptor array is cond_desc_bytes(n_conds + n_vals).  Arguments [0, n_conds) are the Boolean conditions of a case_when,
+// [n_conds, n_conds + n_vals) the values (for a case_when the last one is the else).
+enum : int { COND_COLUMN = 0, COND_SCALAR, COND_NULL };
+struct CondArg {
+    const void* values;         // COND_COLUMN: the chunk's values (a bitmap for Boolean columns)
+    const uint32_t* validity;   // nullptr: every slot valid
+    unsigned long long bits;    // COND_SCALAR: T::Native bits (Boolean 0 / 1)
+    int16_t bit_off;            // validity bit offset
+    int16_t val_bit_off;        // Boolean values bit offset
+    int32_t kind;               // COND_COLUMN, COND_SCALAR or COND_NULL (a NULL literal)
+};
+struct CondHead {
+    void* out; uint32_t* vout;  // vout nullptr: the result chunk has no bitmap
+    int64_t len; int64_t tile0;
+    int32_t n_conds, n_vals;
+    int64_t pad;
+};
+__host__ __device__ inline size_t cond_desc_bytes(int n_args) { return sizeof(CondHead) + (size_t)n_args * sizeof(CondArg); }
+
 // Partial / final aggregate as the kernels produce it.
 struct AggDev {
     unsigned long long sum_bits;  // ints: 64-bit wrapping sum; floats: double bit pattern
@@ -367,6 +387,13 @@ void expr_prog_stats(const void* prog, int* n_instructions, int* n_temporaries);
 int expr_compile(int n_inputs, const int* in_dtypes, int n_nodes, const int* op, const int* a, const int* b, void* prog);
 cudaError_t launch_expr(const void* descs, int n_chunks, int64_t tiles, const void* prog, uint32_t* warp_counts, int* flags, AggDev* tile_partials,
                         cudaStream_t s);
+
+// Null handling and conditional selection (k_cond.cu).  fn: bdf_row_fn (case_when is a COALESCE launch with n_conds > 0);
+// test: bdf_null_test.  `descs` is the CondHead array of stride cond_desc_bytes(n_args).
+int cond_tile_elems(int dtype);
+int null_test_tile_elems(int dtype, int test);
+cudaError_t launch_cond(int fn, int dtype, const void* descs, int n_args, int n_chunks, int64_t tiles, uint32_t* warp_counts, cudaStream_t s);
+cudaError_t launch_null_test(int test, int dtype, const void* descs, int n_chunks, int64_t tiles, cudaStream_t s);
 
 // Sort indices and take (k_sort.cu).
 size_t sort_chunk_size();

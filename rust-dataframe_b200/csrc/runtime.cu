@@ -515,18 +515,22 @@ static void wait_groups(cudaStream_t s, const bdf_col* col, int64_t begin, int64
 // Group boundaries for an operator over `n` chunks: a single group when the inputs are resident, else
 // the union of the inputs' group ends (so work starts as soon as its own inputs have landed).  A context made with
 // BDF_PIPELINE_SPLIT=1 always splits at the group ends, so that the grouped launches run whether or not the copies have landed.
-static std::vector<int64_t> plan_groups(const bdf_ctx* c, int64_t n, std::initializer_list<const bdf_col*> inputs) {
+static std::vector<int64_t> plan_groups(const bdf_ctx* c, int64_t n, const bdf_col* const* inputs, size_t n_inputs) {
     bool all_done = !c->pipeline_split;
-    for (auto* col : inputs) all_done = all_done && col_complete(col);
+    for (size_t j = 0; j < n_inputs; j++) all_done = all_done && (!inputs[j] || col_complete(inputs[j]));
     std::vector<int64_t> ends;
     if (!all_done)
-        for (auto* col : inputs)
-            for (auto& g : col->groups)
-                if (g.end < n) ends.push_back(g.end);
+        for (size_t j = 0; j < n_inputs; j++)
+            if (inputs[j])
+                for (auto& g : inputs[j]->groups)
+                    if (g.end < n) ends.push_back(g.end);
     ends.push_back(n);
     std::sort(ends.begin(), ends.end());
     ends.erase(std::unique(ends.begin(), ends.end()), ends.end());
     return ends;
+}
+static std::vector<int64_t> plan_groups(const bdf_ctx* c, int64_t n, std::initializer_list<const bdf_col*> inputs) {
+    return plan_groups(c, n, inputs.begin(), inputs.size());
 }
 
 static int64_t bitmap_bytes(int64_t len) { return (len + 7) / 8; }
@@ -947,7 +951,7 @@ static cudaError_t fused_finish(bdf_ctx* c, bdf_future* f, bdf_ctx::PartBuf* pb,
 //   fill(host descriptors, chunk i, tile0 of i within its group, output chunk i) -> the chunk's bytes for the launch record
 //   launch(device descriptors of the group, begin, end, tiles, tile_base = tiles of the groups before, warp counts) -> cudaError_t
 template <class Fill, class Launch>
-static int launch_groups(bdf_ctx* c, std::initializer_list<const bdf_col*> inputs, const std::vector<int64_t>& ends, int dtype,
+static int launch_groups(bdf_ctx* c, const bdf_col* const* inputs, size_t n_inputs, const std::vector<int64_t>& ends, int dtype,
                          const std::vector<ChunkPlan>& plan, int tile, size_t desc_bytes, int kernel, const char* what, Fill fill,
                          Launch launch, bdf_col** out) {
     ColOwner o(c);
@@ -966,8 +970,8 @@ static int launch_groups(bdf_ctx* c, std::initializer_list<const bdf_col*> input
             tiles += (plan[i].len + tile - 1) / tile;
             rows += plan[i].len;
         }
-        for (const bdf_col* in : inputs)
-            if (in) wait_groups(c->s_compute, in, begin, end);
+        for (size_t j = 0; j < n_inputs; j++)
+            if (inputs[j]) wait_groups(c->s_compute, inputs[j], begin, end);
         if (end > begin) {
             e = desc_upload(c, dd + begin * desc_bytes, hd + begin * desc_bytes, (size_t)(end - begin) * desc_bytes);
             if (e == cudaSuccess) {
@@ -983,6 +987,12 @@ static int launch_groups(bdf_ctx* c, std::initializer_list<const bdf_col*> input
     if (e != cudaSuccess) return fail_cuda(e, what);
     *out = o.release();
     return BDF_OK;
+}
+template <class Fill, class Launch>
+static int launch_groups(bdf_ctx* c, std::initializer_list<const bdf_col*> inputs, const std::vector<int64_t>& ends, int dtype,
+                         const std::vector<ChunkPlan>& plan, int tile, size_t desc_bytes, int kernel, const char* what, Fill fill,
+                         Launch launch, bdf_col** out) {
+    return launch_groups(c, inputs.begin(), inputs.size(), ends, dtype, plan, tile, desc_bytes, kernel, what, fill, launch, out);
 }
 
 static int binary_dev(bdf_ctx* c, int op, const bdf_col* l, const bdf_col* r, bdf_col** out, bdf_future** fut = nullptr) {
@@ -1573,6 +1583,117 @@ static int boolean_dev(bdf_ctx* c, int op, const bdf_col* a, const bdf_col* b, b
         },
         [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t* wc) {
             return launch_boolean(op, dd, (int)(end - begin), tiles, wc, c->s_compute);
+        },
+        out);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Null handling and conditional selection (k_cond.cu): coalesce, greatest, least, nanvl, case_when, is_null / is_nan
+
+static constexpr int kCondMaxArgs = 64;
+
+// The checks of a row-wise call, shared by the one-GPU and multi-GPU forms and made before any device work.  *dtype: the type of
+// the value columns (they give the result type, so at least one value must be a column).
+static int cond_check(int fn, int32_t n_conds, const bdf_col* const* conds, int32_t n_vals, const bdf_arg* vals, int* dtype) {
+    *dtype = -1;
+    for (int32_t k = 0; k < n_conds; k++) {
+        if (!conds[k]) return fail(BDF_INVALID, "null condition %d", (int)k);
+        if (conds[k]->dtype != kBool) return fail(BDF_INVALID, "condition %d is not a Boolean column", (int)k);
+    }
+    for (int32_t k = 0; k < n_vals; k++) {
+        const bdf_col* col = vals[k].column;
+        if (!col) continue;
+        if (*dtype < 0) *dtype = col->dtype;
+        else if (col->dtype != *dtype) return fail(BDF_INVALID, "arguments of different types (%d, %d): cast them first", *dtype, col->dtype);
+    }
+    if (*dtype < 0) return fail(BDF_INVALID, "no value argument is a column, so nothing gives the result type");
+    if (*dtype == kBool && fn != BDF_ROW_COALESCE) return fail(BDF_UNSUPPORTED, "greatest / least / nanvl of Boolean columns");
+    if (fn == BDF_ROW_NANVL && !dtype_is_float(*dtype)) return fail(BDF_UNSUPPORTED, "nanvl needs Float32 or Float64 arguments");
+    for (int32_t k = 0; k < n_vals; k++)
+        if (*dtype == kBool && !vals[k].column && vals[k].valid && vals[k].bits > 1)
+            return fail(BDF_INVALID, "a Boolean scalar is 0 or 1, not %llu", (unsigned long long)vals[k].bits);
+    return BDF_OK;
+}
+
+// Every column of the call: the conditions, then the value columns in argument order.
+static std::vector<const bdf_col*> cond_columns(int32_t n_conds, const bdf_col* const* conds, int32_t n_vals, const bdf_arg* vals) {
+    std::vector<const bdf_col*> cols(conds, conds + n_conds);
+    for (int32_t k = 0; k < n_vals; k++)
+        if (vals[k].column) cols.push_back(vals[k].column);
+    return cols;
+}
+
+static CondArg cond_arg(const DevChunk* ch, const bdf_arg& v) {
+    if (ch) return CondArg{ch->values, ch->validity, 0ull, (int16_t)ch->bit_off, (int16_t)ch->val_bit_off, COND_COLUMN};
+    return CondArg{nullptr, nullptr, v.valid ? (unsigned long long)v.bits : 0ull, 0, 0, v.valid ? COND_SCALAR : COND_NULL};
+}
+
+// fn: bdf_row_fn; a case_when is a COALESCE with n_conds = n_vals - 1 conditions (the last value is the else).
+static int cond_dev(bdf_ctx* c, int fn, int32_t n_conds, const bdf_col* const* conds, int32_t n_vals, const bdf_arg* vals, bdf_col** out) {
+    int dtype = 0;
+    TRY(cond_check(fn, n_conds, conds, n_vals, vals, &dtype));
+    const std::vector<const bdf_col*> cols = cond_columns(n_conds, conds, n_vals, vals);
+    int64_t n = 0;
+    TRY(zip_chunks(cols.data(), (int)cols.size(), &n));
+    bool null_literal = false;
+    for (int32_t k = 0; k < n_vals; k++) null_literal = null_literal || (!vals[k].column && !vals[k].valid);
+    std::vector<ChunkPlan> plan((size_t)n);
+    for (int64_t i = 0; i < n; i++) {
+        bool nullable = null_literal;
+        for (int32_t k = 0; k < n_vals; k++) nullable = nullable || (vals[k].column && vals[k].column->chunks[i].validity);
+        plan[i] = {cols[0]->chunks[i].len, nullable};
+    }
+    const int n_args = n_conds + n_vals;
+    const size_t stride = cond_desc_bytes(n_args);
+    const int64_t w = dtype == kBool ? 0 : dtype_width(dtype);
+    int64_t value_cols = 0;
+    for (int32_t k = 0; k < n_vals; k++) value_cols += vals[k].column ? 1 : 0;
+    // the launch record's bytes: one value read per row for a selection (every value column for greatest / least), the write, and
+    // every bitmap read and written
+    const int64_t reads = (fn == BDF_ROW_GREATEST || fn == BDF_ROW_LEAST) ? value_cols : 1;
+    // grouped as the other element-wise operators: a group starts once its own chunks of every input have landed
+    return launch_groups(c, cols.data(), cols.size(), plan_groups(c, n, cols.data(), cols.size()), dtype, plan, cond_tile_elems(dtype), stride, BDF_K_BINARY, "row-wise selection",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            const int64_t len = plan[i].len;
+            CondHead* h = (CondHead*)((char*)hd + i * stride);
+            *h = CondHead{oc.values, oc.validity, len, tile0, n_conds, n_vals, 0};
+            CondArg* a = (CondArg*)(h + 1);
+            int64_t bitmaps = (oc.validity ? 1 : 0) + (dtype == kBool ? 1 + reads : 0);
+            for (int32_t k = 0; k < n_conds; k++) {
+                const DevChunk& ch = conds[k]->chunks[i];
+                a[k] = cond_arg(&ch, bdf_arg{});
+                bitmaps += 1 + (ch.validity ? 1 : 0);
+            }
+            for (int32_t k = 0; k < n_vals; k++) {
+                const DevChunk* ch = vals[k].column ? &vals[k].column->chunks[i] : nullptr;
+                a[n_conds + k] = cond_arg(ch, vals[k]);
+                bitmaps += ch && ch->validity ? 1 : 0;
+            }
+            return (reads + 1) * w * len + bitmaps * bitmap_bytes(len);
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t* wc) {
+            return launch_cond(fn, dtype, dd, n_args, (int)(end - begin), tiles, wc, c->s_compute);
+        },
+        out);
+}
+
+static int null_test_dev(bdf_ctx* c, int test, const bdf_col* in, bdf_col** out) {
+    const int64_t n = (int64_t)in->chunks.size();
+    std::vector<ChunkPlan> plan((size_t)n);
+    for (int64_t i = 0; i < n; i++) plan[i] = {in->chunks[i].len, false};
+    const size_t stride = cond_desc_bytes(1);
+    const bool reads_values = test == BDF_IS_NAN && dtype_is_float(in->dtype);
+    const int64_t w = reads_values ? dtype_width(in->dtype) : 0;
+    return launch_groups(c, {in}, plan_groups(c, n, {in}), kBool, plan, null_test_tile_elems(in->dtype, test), stride, BDF_K_COMPARE, "null test",
+        [&](void* hd, int64_t i, int64_t tile0, const DevChunk& oc) {
+            const DevChunk& ch = in->chunks[i];
+            CondHead* h = (CondHead*)((char*)hd + i * stride);
+            *h = CondHead{oc.values, nullptr, ch.len, tile0, 0, 1, 0};
+            *(CondArg*)(h + 1) = cond_arg(&ch, bdf_arg{});
+            return w * ch.len + (1 + (ch.validity ? 1 : 0)) * bitmap_bytes(ch.len);
+        },
+        [&](const void* dd, int64_t begin, int64_t end, int64_t tiles, int64_t, uint32_t*) {
+            return launch_null_test(test, in->dtype, dd, (int)(end - begin), tiles, c->s_compute);
         },
         out);
 }
@@ -4641,18 +4762,22 @@ static int fleet_zip(const bdf_col* const* cols, size_t n_cols, int mismatch, in
 }
 
 // One elementwise operator over fleet columns: `call(k, parts of the inputs on kid k, &result part)`.
-static int fleet_map(bdf_ctx* c, int out_dtype, std::initializer_list<const bdf_col*> inputs, bdf_col** out,
+static int fleet_map(bdf_ctx* c, int out_dtype, const bdf_col* const* inputs, size_t n_inputs, bdf_col** out,
                      const std::function<int(int, bdf_col**)>& call) {
     Fleet* f = c->fleet;
     const int nk = (int)f->kids.size();
     int64_t n = 0;
-    TRY(fleet_zip(inputs.begin(), inputs.size(), BDF_LENGTH_MISMATCH, BDF_UNSUPPORTED, &n));
-    bdf_col* o = fleet_col_like(*inputs.begin(), out_dtype, nk, n);
+    TRY(fleet_zip(inputs, n_inputs, BDF_LENGTH_MISMATCH, BDF_UNSUPPORTED, &n));
+    bdf_col* o = fleet_col_like(inputs[0], out_dtype, nk, n);
     if (!o) return fail(BDF_OOM, "host allocation failed");
     int st = fleet_run(f, [&](int k) { return call(k, &o->fparts[k]); });
     if (st != BDF_OK) { const std::string keep = g_err; fleet_col_free(f, o); g_err = keep; return st; }
     *out = o;
     return BDF_OK;
+}
+static int fleet_map(bdf_ctx* c, int out_dtype, std::initializer_list<const bdf_col*> inputs, bdf_col** out,
+                     const std::function<int(int, bdf_col**)>& call) {
+    return fleet_map(c, out_dtype, inputs.begin(), inputs.size(), out, call);
 }
 
 static bdf_future* fleet_future_new(int n_kids) {
@@ -7110,6 +7235,52 @@ int bdf_boolean_dev(bdf_ctx* c, int op, const bdf_col* a, const bdf_col* b, bdf_
     ENTER(c);
     if (!a || !out) return fail(BDF_INVALID, "null argument");
     return boolean_dev(c, op, a, b, out);
+}
+
+// A row-wise call on a multi-GPU context: the checks once, then the same call on every GPU's parts.
+static int fleet_cond(bdf_ctx* c, int fn, int32_t n_conds, const bdf_col* const* conds, int32_t n_vals, const bdf_arg* vals, bdf_col** out) {
+    int dtype = 0;
+    TRY(cond_check(fn, n_conds, conds, n_vals, vals, &dtype));
+    const std::vector<const bdf_col*> cols = cond_columns(n_conds, conds, n_vals, vals);
+    Fleet* f = c->fleet;
+    return fleet_map(c, dtype, cols.data(), cols.size(), out, [&](int k, bdf_col** o) {
+        std::vector<const bdf_col*> kc((size_t)n_conds);
+        std::vector<bdf_arg> kv(vals, vals + n_vals);
+        for (int32_t j = 0; j < n_conds; j++) kc[j] = conds[j]->fparts[k];
+        for (auto& v : kv)
+            if (v.column) v.column = v.column->fparts[k];
+        return n_conds ? bdf_case_when_dev(f->kids[k], n_conds, kc.data(), kv.data(), o) : bdf_rowwise_dev(f->kids[k], fn, n_vals, kv.data(), o);
+    });
+}
+
+int bdf_rowwise_dev(bdf_ctx* c, int fn, int32_t n_args, const bdf_arg* args, bdf_col** out) {
+    NEED_CTX(c);
+    if (!args || !out) return fail(BDF_INVALID, "null argument");
+    if (fn < BDF_ROW_COALESCE || fn > BDF_ROW_NANVL) return fail(BDF_INVALID, "invalid row-wise function %d", fn);
+    const int lo = fn == BDF_ROW_COALESCE ? 1 : 2, hi = fn == BDF_ROW_NANVL ? 2 : kCondMaxArgs;
+    if (n_args < lo || n_args > hi) return fail(BDF_INVALID, "this function takes %d..%d arguments, not %d", lo, hi, (int)n_args);
+    if (c->fleet) return fleet_cond(c, fn, 0, nullptr, n_args, args, out);
+    ENTER(c);
+    return cond_dev(c, fn, 0, nullptr, n_args, args, out);
+}
+
+int bdf_case_when_dev(bdf_ctx* c, int32_t n_branches, const bdf_col* const* conditions, const bdf_arg* values, bdf_col** out) {
+    NEED_CTX(c);
+    if (!conditions || !values || !out) return fail(BDF_INVALID, "null argument");
+    if (n_branches < 1 || n_branches > kCondMaxArgs) return fail(BDF_INVALID, "case_when takes 1..%d branches, not %d", kCondMaxArgs, (int)n_branches);
+    if (c->fleet) return fleet_cond(c, BDF_ROW_COALESCE, n_branches, conditions, n_branches + 1, values, out);
+    ENTER(c);
+    return cond_dev(c, BDF_ROW_COALESCE, n_branches, conditions, n_branches + 1, values, out);
+}
+
+int bdf_null_test_dev(bdf_ctx* c, int fn, const bdf_col* in, bdf_col** out) {
+    NEED_CTX(c);
+    if (!in || !out) return fail(BDF_INVALID, "null argument");
+    if (fn < BDF_IS_NULL || fn > BDF_IS_NAN) return fail(BDF_INVALID, "invalid null test %d", fn);
+    if (Fleet* f = c->fleet)
+        return fleet_map(c, kBool, {in}, out, [=](int k, bdf_col** o) { return bdf_null_test_dev(f->kids[k], fn, in->fparts[k], o); });
+    ENTER(c);
+    return null_test_dev(c, fn, in, out);
 }
 
 int bdf_filter_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* mask, bdf_col** out) {

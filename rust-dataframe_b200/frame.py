@@ -35,7 +35,7 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 import numpy as np
 
 from . import _native as N
-from .arrays import F32, F64, I8, I64, U8, U32, U64, PrimitiveArray, is_float
+from .arrays import F32, F64, I8, I64, NP_DTYPES, U8, U32, U64, PrimitiveArray, is_float
 from .functions import Column, ListColumn, _expr_nodes, eval_expr, sort_indices, window as _window
 from .csv_reader import CsvFile, write_csv
 from .json_reader import JsonFile
@@ -216,6 +216,22 @@ def lit(v: float):
     return ("scalar", float(v))
 
 
+# null tests as condition nodes: ("is_null", x) | ("is_not_null", x) | ("is_nan", x), x a ("col", name) node
+NULL_TESTS = {"is_null": N.IS_NULL, "is_not_null": N.IS_NOT_NULL, "is_nan": N.IS_NAN}
+
+
+def is_null(x):
+    return ("is_null", col(x) if isinstance(x, str) else x)
+
+
+def is_not_null(x):
+    return ("is_not_null", col(x) if isinstance(x, str) else x)
+
+
+def is_nan(x):
+    return ("is_nan", col(x) if isinstance(x, str) else x)
+
+
 def _filter_columns(cond) -> set:
     if cond[0] == "col":
         return {cond[1]}
@@ -386,6 +402,29 @@ def _try_fuse(run: List[Calculation], needed_after_run: set, max_inputs: int, ma
 
 # ---------------------------------------------------------------------------------------------------------
 
+def fill_value_fits(dtype: int, value) -> bool:
+    """Can a column of `dtype` hold `value` exactly?  A bool only a Boolean column; an int an integer column whose range holds it
+    or a float column that represents it exactly; a float a float column that represents it exactly (NaN and the infinities
+    included)."""
+    if isinstance(value, (bool, np.bool_)):
+        return dtype == BOOL
+    if dtype == BOOL or not 0 <= dtype < len(NP_DTYPES):
+        return False
+    npt = NP_DTYPES[dtype]
+    if isinstance(value, (int, np.integer)):
+        if is_float(dtype):
+            x = npt.type(value)
+            return bool(np.isfinite(x)) and int(x) == int(value)
+        info = np.iinfo(npt)
+        return info.min <= int(value) <= info.max
+    if isinstance(value, (float, np.floating)):
+        if not is_float(dtype):
+            return False
+        x = npt.type(value)
+        return float(x) == float(value) or (x != x and value != value)
+    return False
+
+
 class DeviceFrame:
     """Ordered name -> Column or ListColumn; every column has the same chunk lengths (the frame's RecordBatches).  A ListColumn is
     carried through filter, sort, limit, join, select, drop, with_column and window; it is reported in the schema as
@@ -502,6 +541,39 @@ class DeviceFrame:
             if name in self.columns:
                 self._numeric(name, "a filter condition")
         mask = self._boolean(cond)
+        return DeviceFrame(OrderedDict((n, c.filter(mask)) for n, c in self.columns.items()))
+
+    def fill_null(self, value, subset: Optional[Sequence[str]] = None) -> "DeviceFrame":
+        """pandas' fillna / Spark's na.fill: the NULL slots of columns replaced by coalesce(column, value).  `value` is a scalar or a
+        {column: value} dict.  With a scalar and no subset, every column that can hold the value exactly is filled: an int fills the
+        integer columns whose range holds it and the float columns that hold it exactly, a float fills the float columns that hold
+        it, a bool fills the Boolean columns; temporal and list columns are never filled by default.  A named column that cannot
+        hold its value raises UnsupportedType before any device work."""
+        if isinstance(value, dict):
+            plan = dict(value)
+        elif subset is None:
+            plan = {n: value for n, c in self.columns.items()
+                    if not isinstance(c, ListColumn) and getattr(c, "temporal", None) is None and fill_value_fits(c.dtype, value)}
+        else:
+            plan = {n: value for n in subset}
+        for n, v in plan.items():
+            c = self._numeric(n, "fill_null")
+            if not fill_value_fits(c.dtype, v):
+                raise N.UnsupportedType(f"column {n!r} (dtype {c.dtype}) cannot hold {v!r} exactly")
+        return DeviceFrame(OrderedDict((n, c.fill_null(plan[n]) if n in plan else c) for n, c in self.columns.items()))
+
+    def drop_nulls(self, subset: Optional[Sequence[str]] = None, how: str = "any") -> "DeviceFrame":
+        """pandas' dropna / Spark's na.drop: the rows where any (how="any") or every (how="all") column of `subset` (default: all)
+        is NULL are removed -- the AND / OR of is_not_null masks, then the frame's filter."""
+        if how not in ("any", "all"):
+            raise N.ComputeError(f"how must be 'any' or 'all', not {how!r}")
+        names = list(self.columns) if subset is None else list(subset)
+        if not names:
+            return self
+        masks = [self._numeric(n, "drop_nulls").is_not_null() for n in names]
+        mask = masks[0]
+        for m in masks[1:]:
+            mask = mask.logical_and(m) if how == "any" else mask.logical_or(m)
         return DeviceFrame(OrderedDict((n, c.filter(mask)) for n, c in self.columns.items()))
 
     def sort(self, criteria: Sequence[Tuple[str, bool]]) -> "DeviceFrame":
@@ -630,6 +702,10 @@ class DeviceFrame:
         if kind in ("and", "or"):
             a, b = self._boolean(cond[1]), self._boolean(cond[2])
             return a.logical_and(b) if kind == "and" else a.logical_or(b)
+        if kind in NULL_TESTS:
+            if cond[1][0] != "col":
+                raise N.UnsupportedType(f"{kind} needs a column operand")
+            return self._numeric(cond[1][1], f"{kind}")._null_test(NULL_TESTS[kind])
         if kind in CMP:
             l, r = cond[1], cond[2]
             if l[0] == "scalar" and r[0] == "col":

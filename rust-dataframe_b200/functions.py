@@ -620,6 +620,24 @@ class Column:
         N.raise_for_status(N.lib().bdf_filter_dev(self.ctx.handle, self.handle, mask.handle, C.byref(h)))
         return Column(self.ctx, h, self.temporal)
 
+    # -- null handling and conditional selection (include/b200df.h "null handling and conditional selection") --
+    def _null_test(self, fn: int) -> "Column":
+        h = C.c_void_p()
+        N.raise_for_status(N.lib().bdf_null_test_dev(self.ctx.handle, fn, self.handle, C.byref(h)))
+        return Column(self.ctx, h)
+
+    def is_null(self) -> "Column": return self._null_test(N.IS_NULL)
+    def is_not_null(self) -> "Column": return self._null_test(N.IS_NOT_NULL)
+    def is_nan(self) -> "Column": return self._null_test(N.IS_NAN)
+
+    def fill_null(self, value) -> "Column":
+        """coalesce(self, value): the NULL slots replaced by a scalar (or by the slots of another column)."""
+        return coalesce(self, value)
+
+    def nanvl(self, other) -> "Column":
+        """Spark's nanvl: self where it is not NaN, `other` where it is NaN, NULL where self is NULL (Float32 / Float64)."""
+        return _rowwise(N.ROW_NANVL, (self, other))
+
     def unary(self, op: int) -> "Column":
         _refuse_temporal("a math function", self)
         h = C.c_void_p()
@@ -827,6 +845,155 @@ class Column:
             self.free()
         except Exception:
             pass
+
+
+# ---- null handling and conditional selection ---------------------------------------------------------------------------
+def _scalar_bits(dtype: int, v) -> int:
+    """T::Native bits of the Python scalar v in a column of `dtype` (the column arguments type the scalars); a value the type
+    cannot hold exactly is refused, as the casts the caller would otherwise write."""
+    if dtype == N.BOOL:
+        if not isinstance(v, (bool, np.bool_)):
+            raise N.UnsupportedType(f"{v!r} is not a Boolean scalar")
+        return int(bool(v))
+    if isinstance(v, (bool, np.bool_)):
+        raise N.UnsupportedType(f"a Boolean scalar in a {dtype} argument list")
+    npt = NP_DTYPES[dtype]
+    if is_float(dtype):
+        x = npt.type(v)
+        if not (float(x) == float(v) or (x != x and v != v)):
+            raise N.UnsupportedType(f"{v!r} is not exactly a {npt} value")
+    else:
+        if isinstance(v, (float, np.floating)):
+            if not float(v).is_integer():
+                raise N.UnsupportedType(f"{v!r} is not an integer")
+            v = int(v)
+        info = np.iinfo(npt)
+        if not info.min <= int(v) <= info.max:
+            raise N.UnsupportedType(f"{v!r} is out of range for {npt}")
+        x = npt.type(int(v))
+    return int(np.array([x], dtype=npt).view(np.dtype(f"u{npt.itemsize}"))[0])
+
+
+def _args_type(columns, what: str):
+    """(dtype, temporal tag) of the column arguments; mismatched temporal types are refused here, before any device work."""
+    if not columns:
+        raise N.ComputeError(f"{what} needs at least one column argument: the columns give the result type")
+    tags = {repr(getattr(c, "temporal", None)) for c in columns}
+    if len(tags) > 1:
+        raise N.UnsupportedType(f"{what} of columns of different temporal types ({', '.join(sorted(tags))}): cast them first")
+    for c in columns:
+        if isinstance(c, ListColumn):
+            raise N.UnsupportedType(f"{what} of a list column")
+    return columns[0].dtype, getattr(columns[0], "temporal", None)
+
+
+def _make_args(values, dtype: int):
+    args = (N.Arg * max(len(values), 1))()
+    for i, v in enumerate(values):
+        if isinstance(v, Column):
+            args[i].column, args[i].valid = v.handle, 1
+        elif v is None:
+            args[i].column, args[i].valid = None, 0
+        else:
+            args[i].column, args[i].bits, args[i].valid = None, _scalar_bits(dtype, v), 1
+    return args
+
+
+def _rowwise(fn: int, values, what: str = "a row-wise function") -> "Column":
+    cols = [v for v in values if isinstance(v, (Column, ListColumn))]
+    dtype, tag = _args_type(cols, what)
+    args = _make_args(values, dtype)
+    h = C.c_void_p()
+    N.raise_for_status(N.lib().bdf_rowwise_dev(cols[0].ctx.handle, fn, len(values), args, C.byref(h)))
+    return Column(cols[0].ctx, h, tag)
+
+
+def coalesce(*args) -> "Column":
+    """Spark's coalesce: per row the first argument valid there, NULL where every argument is NULL (1..64 arguments, Columns or
+    scalars of the columns' type; None is a NULL literal)."""
+    return _rowwise(N.ROW_COALESCE, args, "coalesce")
+
+
+def greatest(*args) -> "Column":
+    """Spark's greatest: the largest valid argument per row in DataFrame::sort's order (NaN above +inf); NULL only where every
+    argument is NULL; among equal values the earliest argument's bits (2..64 arguments)."""
+    return _rowwise(N.ROW_GREATEST, args, "greatest")
+
+
+def least(*args) -> "Column":
+    """Spark's least: greatest with the order reversed."""
+    return _rowwise(N.ROW_LEAST, args, "least")
+
+
+def nanvl(a, b) -> "Column":
+    return _rowwise(N.ROW_NANVL, (a, b), "nanvl")
+
+
+class CaseWhen:
+    """``when(c1, v1).when(c2, v2).otherwise(v)``: SQL's CASE WHEN.  Each row takes the value of the first branch whose Boolean
+    condition is valid and true there (a NULL condition counts as false); rows no branch takes get the ``otherwise`` value
+    (None, or no ``otherwise`` call at all through ``end()``, means NULL)."""
+
+    def __init__(self, branches):
+        self.branches = list(branches)
+
+    def when(self, cond: "Column", value) -> "CaseWhen":
+        return CaseWhen(self.branches + [(cond, value)])
+
+    def otherwise(self, value=None) -> "Column":
+        conds = [c for c, _ in self.branches]
+        values = [v for _, v in self.branches] + [value]
+        for c in conds:
+            if not isinstance(c, Column):
+                raise N.UnsupportedType("a case_when condition must be a Boolean Column")
+        dtype, tag = _args_type([v for v in values if isinstance(v, (Column, ListColumn))], "case_when")
+        args = _make_args(values, dtype)
+        ca = (C.c_void_p * len(conds))(*[c.handle for c in conds])
+        h = C.c_void_p()
+        N.raise_for_status(N.lib().bdf_case_when_dev(conds[0].ctx.handle, len(conds), ca, args, C.byref(h)))
+        return Column(conds[0].ctx, h, tag)
+
+    def end(self) -> "Column":
+        return self.otherwise(None)
+
+
+def when(cond: "Column", value) -> CaseWhen:
+    return CaseWhen([(cond, value)])
+
+
+def _rowwise_host(fn: int, args, ctx) -> List[PrimitiveArray]:
+    """A row-wise function over host chunks: every chunk list is uploaded, the device entry runs, the result comes back."""
+    ctx = ctx or N.default_context()
+    cols = []
+    try:
+        vals = []
+        for a in args:
+            if a is None or not isinstance(a, (list, tuple)):
+                vals.append(a)
+            else:
+                cols.append(Column.upload(a, ctx, dtype=_dtype_of(a) if len(a) else None))
+                vals.append(cols[-1])
+        out = _rowwise(fn, vals)
+        try:
+            return out.download()
+        finally:
+            out.free()
+    finally:
+        for c in cols:
+            c.free()
+
+
+def _scalar_fn(fn: int, doc: str):
+    def f(*args, ctx=None) -> List[PrimitiveArray]:
+        return _rowwise_host(fn, args, ctx)
+    f.__doc__ = doc
+    return staticmethod(f)
+
+
+ScalarFunctions.coalesce = _scalar_fn(N.ROW_COALESCE, "coalesce over columns given as lists of chunks (or scalars): scalar.rs's empty stub, Spark's definition.")
+ScalarFunctions.greatest = _scalar_fn(N.ROW_GREATEST, "greatest over columns given as lists of chunks (or scalars): scalar.rs's empty stub, Spark's definition.")
+ScalarFunctions.least = _scalar_fn(N.ROW_LEAST, "least over columns given as lists of chunks (or scalars): scalar.rs's empty stub, Spark's definition.")
+ScalarFunctions.nanvl = _scalar_fn(N.ROW_NANVL, "nanvl(a, b) over columns given as lists of chunks: scalar.rs's nanv1 stub, Spark's definition.")
 
 
 def sort_indices(criteria: Sequence[tuple]) -> "Column":

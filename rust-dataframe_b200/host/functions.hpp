@@ -148,6 +148,38 @@ Result<std::vector<PrimitiveArray<R>>> temporal(int fn, const bdf_temporal_type&
     return out.finish();
 }
 
+// Null handling and conditional selection over host chunks: every column is uploaded, the device entry runs on them, the result
+// comes back.  zip() semantics as the device entry has them: the smallest chunk count of the columns.
+template <typename T>
+Result<std::vector<PrimitiveArray<T>>> rowwise(int fn, const std::vector<std::vector<const PrimitiveArray<T>*>>& columns) {
+    std::vector<bdf_col*> cols;
+    std::vector<bdf_arg> args;
+    auto release = [&] { for (auto* c : cols) bdf_col_free(context(), c); };
+    size_t n = columns.empty() ? 0 : columns[0].size();
+    for (auto& c : columns) n = std::min(n, c.size());
+    int st = BDF_OK;
+    for (auto& c : columns) {
+        auto v = views(c);
+        bdf_col* col = nullptr;
+        st = bdf_upload(context(), ArrowType<T>::id, (int64_t)v.size(), v.data(), 0, &col);
+        if (st != BDF_OK) break;
+        cols.push_back(col);
+        args.push_back(bdf_arg{col, 0, 1});
+    }
+    bdf_col* res = nullptr;
+    if (st == BDF_OK) st = bdf_rowwise_dev(context(), fn, (int32_t)args.size(), args.data(), &res);
+    if (st == BDF_UNSUPPORTED) { release(); throw std::logic_error(std::string("trait bound not satisfied: ") + bdf_last_error()); }
+    if (st != BDF_OK) { release(); return to_error(st); }
+    std::vector<int64_t> lens;
+    for (size_t i = 0; i < n; i++) lens.push_back(columns[0][i]->len());
+    Outputs<T> out(lens);
+    st = bdf_download(context(), res, out.outs.data());
+    bdf_col_free(context(), res);
+    release();
+    if (st != BDF_OK) return to_error(st);
+    return out.finish();
+}
+
 }  // namespace detail
 
 struct ScalarFunctions {
@@ -186,6 +218,12 @@ struct ScalarFunctions {
     RDF_TEMPORAL_ARG(to_timestamp, BDF_TEMPORAL_TO_TIMESTAMP, int64_t)
 #undef RDF_TEMPORAL
 #undef RDF_TEMPORAL_ARG
+    // coalesce / greatest / least / nanv1: scalar.rs's empty stubs with Spark's definitions (include/b200df.h "null handling and
+    // conditional selection"); every argument is a column given as its chunks.
+    template <typename T> static Out<T> coalesce(const std::vector<Arrays<T>>& a) { return detail::rowwise<T>(BDF_ROW_COALESCE, a); }
+    template <typename T> static Out<T> greatest(const std::vector<Arrays<T>>& a) { return detail::rowwise<T>(BDF_ROW_GREATEST, a); }
+    template <typename T> static Out<T> least(const std::vector<Arrays<T>>& a) { return detail::rowwise<T>(BDF_ROW_LEAST, a); }
+    template <typename T> static Out<T> nanvl(const Arrays<T>& a, const Arrays<T>& b) { return detail::rowwise<T>(BDF_ROW_NANVL, {a, b}); }
     // date_trunc keeps the input's type: the result has the column's physical type T
     template <typename T> static Out<T> date_trunc(const bdf_temporal_type& t, int64_t unit, const Arrays<T>& a) {
         return detail::temporal<T, T>(BDF_TEMPORAL_DATE_TRUNC, t, unit, a);
