@@ -408,10 +408,52 @@ int  bdf_group_by_lists_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_col* const* 
  *   -> BDF_INVALID; an unknown join type or a non-numeric key -> BDF_UNSUPPORTED; a criterion whose two columns have different
  *   dtypes -> BDF_UNSUPPORTED "Join columns must have compatible types" (the text of try_join); key columns of one side with
  *   different lengths -> BDF_LENGTH_MISMATCH; a side of more than 2^32-1 rows -> the sort's BDF_UNSUPPORTED; a multi-GPU context
- *   -> BDF_UNSUPPORTED (as sort / take / filter / group-by); an output that does not fit in device memory -> BDF_OOM. */
-typedef enum { BDF_JOIN_LEFT = 0, BDF_JOIN_RIGHT, BDF_JOIN_INNER, BDF_JOIN_FULL } bdf_join_type;   /* JoinType order */
+ *   -> BDF_UNSUPPORTED (as sort / take / filter / group-by); an output that does not fit in device memory -> BDF_OOM.
+ * Existence joins (Spark's left_semi / left_anti; not in the reference, whose JoinType has the first four):
+ *   LEFT_SEMI    every left row that has at least one match, once, however many partners it has;
+ *   LEFT_ANTI    every other left row, rows with a null in any criterion included (a null key matches nothing: Spark's left_anti
+ *                for an equi-join, not SQL's NOT IN).
+ *   *left_indices is one UInt32 chunk without nulls: left row numbers in ascending order, *n_rows of them.  No right indices are
+ *   made: right_indices may be NULL, and if it is not, *right_indices is set to NULL.  Match rules and errors are those above. */
+typedef enum { BDF_JOIN_LEFT = 0, BDF_JOIN_RIGHT, BDF_JOIN_INNER, BDF_JOIN_FULL, BDF_JOIN_LEFT_SEMI, BDF_JOIN_LEFT_ANTI } bdf_join_type;   /* JoinType order, then the existence joins */
 int  bdf_join_indices_dev(bdf_ctx* ctx, int32_t join_type, int32_t n_keys, const bdf_col* const* left_keys, const bdf_col* const* right_keys,
                           bdf_col** left_indices, bdf_col** right_indices, int64_t* n_rows);
+
+/* ---- as-of join (pandas' merge_asof, polars' join_asof, DuckDB's ASOF JOIN; not in the reference) ----------------------------------
+ * For every left row, one right row: the last one at or before its `on` key (BACKWARD), the first one at or after it (FORWARD), or the
+ * nearer of those two (NEAREST), among the right rows whose 0..16 `by` keys equal the left row's.
+ * Output.  *right_indices: one UInt32 chunk of as many rows as the left side; row i belongs to left row i (left order is kept, so the
+ *   left columns need no take) and holds a right row number counting through the chunks, NULL when the row has no partner.  Take the
+ *   right columns with bdf_take_dev / bdf_list_take_dev.
+ * Candidates of left row i: the right rows j whose every `by` pair is valid on both sides and equal under the join's key equality (all
+ *   NaNs equal, -0.0 == 0.0), and whose right_on[j] is valid and not NaN.  A left row whose `on` is null or NaN, or one of whose `by`
+ *   keys is null, gets NULL.
+ * Choice.  Keys compare in the sort's order, -0.0 == 0.0.  With l the left key and r the right keys:
+ *   BACKWARD  among the candidates with r <= l (r < l without exact matches) the greatest r; of equal r the LAST in right row order;
+ *   FORWARD   among the candidates with r >= l (r > l) the least r; of equal r the FIRST in right row order;
+ *   NEAREST   b = the BACKWARD pick, f = the FORWARD pick: the one that exists, else b when l - r_b <= r_f - l (ties go backward), else f.
+ * Tolerance (has_tolerance != 0): the pick becomes NULL when its distance is greater than the tolerance.  Integer and temporal keys:
+ *   `tolerance`, in the key's own units; the distance is exact (INT64_MAX against INT64_MIN is 2^64 - 1).  Float32 / Float64 keys:
+ *   `tolerance_f` (may be +inf); the distance is (double)l - (double)r or the reverse, rounded once, Float32 widened exactly; equal keys,
+ *   infinities included, are at distance 0.
+ * Departures from pandas, on purpose: neither side needs to be sorted; left order is kept; null and NaN keys simply match nothing
+ *   (pandas refuses them).
+ * Errors (nothing is returned and nothing leaks): n_by outside 0..16, a null pointer, a negative or NaN tolerance -> BDF_INVALID; an
+ *   unknown direction, a non-numeric or Boolean key -> BDF_UNSUPPORTED; an `on` or `by` pair of different dtypes -> BDF_UNSUPPORTED
+ *   "Join columns must have compatible types"; key columns of one side with different lengths -> BDF_LENGTH_MISMATCH; more than
+ *   2^32-1 right rows -> the sort's BDF_UNSUPPORTED; a multi-GPU context -> BDF_UNSUPPORTED.
+ * The right side is sorted once by (by..., on), stably; every left row then binary-searches its `by` run and, inside it, its `on` key,
+ *   reading the left chunks in place.  The result does not depend on timing (no atomics on results). */
+typedef enum { BDF_ASOF_BACKWARD = 0, BDF_ASOF_FORWARD, BDF_ASOF_NEAREST } bdf_asof_direction;
+typedef struct {
+    int32_t direction;            /* bdf_asof_direction */
+    int32_t allow_exact_matches;  /* 1: <= / >= ; 0: < / > */
+    int32_t has_tolerance;
+    int64_t tolerance;            /* integer and temporal on-keys, in the key's own units, >= 0 */
+    double  tolerance_f;          /* Float32 / Float64 on-keys, >= 0, may be +inf */
+} bdf_asof_spec;
+int  bdf_join_asof_dev(bdf_ctx* ctx, const bdf_col* left_on, const bdf_col* right_on, int32_t n_by, const bdf_col* const* left_by,
+                       const bdf_col* const* right_by, const bdf_asof_spec* spec, bdf_col** right_indices);
 
 /* ---- window functions (WindowFunctions, src/functions/window.rs:1-11; WindowSpec, src/window.rs:8-22: stubs in the reference) ----
  * One call computes n_calls window columns that share one specification, so the rows are sorted once.

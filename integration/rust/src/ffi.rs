@@ -143,6 +143,18 @@ pub struct BdfWindowCall {
     pub function: i32, pub frame: i32, pub column: *const BdfCol, pub offset: i64, pub default_bits: u64, pub has_default: i32,
     pub ignore_nulls: i32, pub start: i64, pub end: i64, pub start_f: f64, pub end_f: f64,
 }
+/// bdf_asof_spec: the rules of one as-of join (include/b200df.h "as-of join").  `tolerance` bounds an integer or temporal key's distance in
+/// its own units, `tolerance_f` a Float32 / Float64 key's (+inf allowed); both only when `has_tolerance` is 1.
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct BdfAsofSpec { pub direction: i32, pub allow_exact_matches: i32, pub has_tolerance: i32, pub tolerance: i64, pub tolerance_f: f64 }
+/// bdf_asof_direction.
+pub const BDF_ASOF_BACKWARD: i32 = 0;
+pub const BDF_ASOF_FORWARD: i32 = 1;
+pub const BDF_ASOF_NEAREST: i32 = 2;
+/// bdf_join_type: JoinType's four, then the existence joins.
+pub const BDF_JOIN_LEFT_SEMI: i32 = 4;
+pub const BDF_JOIN_LEFT_ANTI: i32 = 5;
 /// bdf_window_fn, in WindowFunctions order, then the aggregates.
 pub const BDF_WIN_ROW_NUMBER: i32 = 0;
 pub const BDF_WIN_RANK: i32 = 1;
@@ -243,9 +255,13 @@ extern "C" {
     pub fn bdf_group_by_lists_dev(ctx: *mut BdfCtx, n_keys: i32, keys: *const *const BdfCol, n_aggs: i32, aggs: *const BdfGroupAgg,
                                   out_keys: *mut *mut BdfCol, out: *mut *mut BdfCol, out_lists: *mut *mut BdfList, n_groups: *mut i64) -> c_int;
     // equi-join (calc_equijoin_indices): join_type in JoinType order (LeftJoin, RightJoin, InnerJoin, FullJoin); two UInt32 index
-    // columns, NULL = no partner, to take every column of each side with
+    // columns, NULL = no partner, to take every column of each side with.  BDF_JOIN_LEFT_SEMI / _ANTI: only left_indices (the left
+    // rows with / without a partner, ascending); right_indices may be null and is set to null
     pub fn bdf_join_indices_dev(ctx: *mut BdfCtx, join_type: i32, n_keys: i32, left_keys: *const *const BdfCol, right_keys: *const *const BdfCol,
                                 left_indices: *mut *mut BdfCol, right_indices: *mut *mut BdfCol, n_rows: *mut i64) -> c_int;
+    // as-of join (pandas' merge_asof): one UInt32 column, a right row number per left row in left order, NULL = no partner
+    pub fn bdf_join_asof_dev(ctx: *mut BdfCtx, left_on: *const BdfCol, right_on: *const BdfCol, n_by: i32, left_by: *const *const BdfCol,
+                             right_by: *const *const BdfCol, spec: *const BdfAsofSpec, right_indices: *mut *mut BdfCol) -> c_int;
     // window functions over one WindowSpec (src/window.rs:8-22; WindowFunctions, src/functions/window.rs:1-11): n_calls one-chunk columns
     // in the caller's row order, every one the caller's to free
     pub fn bdf_window_dev(ctx: *mut BdfCtx, n_partition: i32, partition_by: *const *const BdfCol, n_order: i32, order_by: *const BdfSortKey,

@@ -204,12 +204,22 @@ pub fn group_by_device(frame: &DeviceColumns, keys: &[usize], aggr: &[(usize, Gr
 /// right column) pairs; `join_type`: JoinType's discriminant (Left, Right, Inner, Full -- bdf_join_type).  Output = every column of
 /// `left`, then every column of `right`, taken by the index pairs (NULL index -> NULL slot); a name present on both sides becomes
 /// `a.<name>` / `b.<name>`, the schema `Dataset::try_join` plans.  Pair order and the departures from the reference: include/b200df.h.
+/// BDF_JOIN_LEFT_SEMI / BDF_JOIN_LEFT_ANTI: the columns of `left` only, names unchanged, at the left rows that have (lack) a partner.
 pub fn join_device(left: &DeviceColumns, right: &DeviceColumns, criteria: &[(usize, usize)], join_type: i32) -> Result<DeviceColumns, String> {
     let lk: Vec<*const BdfCol> = criteria.iter().map(|(l, _)| left.cols[*l] as *const BdfCol).collect();
     let rk: Vec<*const BdfCol> = criteria.iter().map(|(_, r)| right.cols[*r] as *const BdfCol).collect();
     let (mut li, mut ri, mut n_rows) = (std::ptr::null_mut(), std::ptr::null_mut(), 0i64);
     check(unsafe { bdf_join_indices_dev(dev(), join_type, lk.len() as i32, lk.as_ptr(), rk.as_ptr(), &mut li, &mut ri, &mut n_rows) })?;
     let idx = DeviceColumns { names: vec![], cols: vec![li, ri] };   // freed when this function returns, early or not
+    if join_type == BDF_JOIN_LEFT_SEMI || join_type == BDF_JOIN_LEFT_ANTI {
+        let mut out = DeviceColumns { names: left.names.clone(), cols: Vec::with_capacity(left.cols.len()) };
+        for col in &left.cols {
+            let mut taken: *mut BdfCol = std::ptr::null_mut();
+            check(unsafe { bdf_take_dev(dev(), *col, idx.cols[0], &mut taken) })?;
+            out.cols.push(taken);
+        }
+        return Ok(out);
+    }
     let mut out = DeviceColumns { names: vec![], cols: vec![] };
     for (side, other, prefix, indices) in [(left, right, "a", idx.cols[0]), (right, left, "b", idx.cols[1])] {
         for (name, col) in side.names.iter().zip(&side.cols) {
@@ -218,6 +228,28 @@ pub fn join_device(left: &DeviceColumns, right: &DeviceColumns, criteria: &[(usi
             out.names.push(if other.names.contains(name) { format!("{}.{}", prefix, name) } else { name.clone() });
             out.cols.push(taken);
         }
+    }
+    Ok(out)
+}
+
+/// An as-of join (pandas' merge_asof; include/b200df.h "as-of join"): for every row of `left`, in its order, the row of `right` whose
+/// `on.1` key is the last at or before its `on.0` key (BDF_ASOF_BACKWARD), the first at or after it (FORWARD) or the nearer (NEAREST),
+/// among the rows whose `by` pairs are equal.  Returns the columns of `right` only, taken by that row (NULL where there is none), one
+/// chunk each in `left`'s row order; a name `left` also has becomes `b.<name>` (the caller renames its own column to `a.<name>`, the
+/// schema `Dataset::try_join` plans), so the left columns are never copied.
+pub fn join_asof_device(left: &DeviceColumns, right: &DeviceColumns, on: (usize, usize), by: &[(usize, usize)], spec: &BdfAsofSpec)
+                        -> Result<DeviceColumns, String> {
+    let lb: Vec<*const BdfCol> = by.iter().map(|(l, _)| left.cols[*l] as *const BdfCol).collect();
+    let rb: Vec<*const BdfCol> = by.iter().map(|(_, r)| right.cols[*r] as *const BdfCol).collect();
+    let mut ri: *mut BdfCol = std::ptr::null_mut();
+    check(unsafe { bdf_join_asof_dev(dev(), left.cols[on.0], right.cols[on.1], lb.len() as i32, lb.as_ptr(), rb.as_ptr(), spec, &mut ri) })?;
+    let idx = DeviceColumns { names: vec![], cols: vec![ri] };   // freed when this function returns, early or not
+    let mut out = DeviceColumns { names: vec![], cols: Vec::with_capacity(right.cols.len()) };
+    for (name, col) in right.names.iter().zip(&right.cols) {
+        let mut taken: *mut BdfCol = std::ptr::null_mut();
+        check(unsafe { bdf_take_dev(dev(), *col, idx.cols[0], &mut taken) })?;
+        out.names.push(if left.names.contains(name) { format!("b.{}", name) } else { name.clone() });
+        out.cols.push(taken);
     }
     Ok(out)
 }

@@ -456,6 +456,13 @@ cudaError_t launch_join_emit(const unsigned long long* offs, long long n_probe, 
                              uint32_t* build_valid, cudaStream_t s);
 cudaError_t launch_join_unmatched(const uint32_t* perm, long long n_build, const uint32_t* run_starts, long long n_runs, const unsigned char* hit,
                                   uint32_t* mask, int sm_count, cudaStream_t s);
+cudaError_t launch_join_exists(int n_keys, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,
+                               const uint32_t* const* build_valid, long long n_probe, long long n_runs, int anti, uint32_t* mask, cudaStream_t s);
+cudaError_t launch_join_asof(int n_by, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,
+                             const uint32_t* const* build_valid, int on_dtype, const void* on_table, int on_chunks, const void* on_build,
+                             const uint32_t* on_build_valid, int direction, int exact, int has_tol, unsigned long long tol, double tol_f,
+                             long long n_probe, const uint32_t* run_starts, long long n_runs, long long n_build, const uint32_t* perm, uint32_t* out,
+                             uint32_t* out_valid, cudaStream_t s);
 
 // Window functions (k_window.cu).
 int window_count_tile();

@@ -2087,9 +2087,10 @@ struct SortedRuns {
     int64_t n_runs = 0;
 };
 
-// Sort the keys, gather them in sorted order, mark the heads, compact the distinct key tuples and the run starts.  `what` names
-// the caller's iota in a CUDA failure.
-static int sorted_runs(bdf_ctx* c, int n_keys, const bdf_col* const* keys, const char* what, SortedRuns* r) {
+// Sort the keys, gather them in sorted order, mark the heads, compact the distinct key tuples and the run starts.  Only the first
+// n_cut keys cut runs; the keys after them order the rows inside a run (the as-of join's `on` key).  n_cut == 0: the whole side is one
+// run (none when it is empty), and no heads, distinct tuples or starts are made.  `what` names the caller's iota in a CUDA failure.
+static int sorted_runs(bdf_ctx* c, int n_keys, int n_cut, const bdf_col* const* keys, const char* what, SortedRuns* r) {
     const int64_t n = keys[0]->total_len;
     std::vector<bdf_sort_key> sk((size_t)n_keys);
     for (int k = 0; k < n_keys; k++) sk[k] = bdf_sort_key{keys[k], 0};
@@ -2100,8 +2101,13 @@ static int sorted_runs(bdf_ctx* c, int n_keys, const bdf_col* const* keys, const
         TRY(take_dev(c, keys[k], r->perm.get(), r->sorted[k].out()));
         sorted.push_back(r->sorted[k].get());
     }
+    if (n_cut == 0) {
+        r->n_runs = n > 0 ? 1 : 0;
+        return BDF_OK;
+    }
+    sorted.resize((size_t)n_cut);
     TRY(group_heads(c, sorted, false, n, r->head.out()));
-    for (int k = 0; k < n_keys; k++) {
+    for (int k = 0; k < n_cut; k++) {
         r->distinct.emplace_back(c);
         TRY(filter_dev(c, sorted[k], r->head.get(), r->distinct[k].out()));
     }
@@ -2255,7 +2261,7 @@ static int group_by_dev(bdf_ctx* c, int n_keys, const bdf_col* const* keys, int 
     }
     const int64_t n = keys[0]->total_len;
     SortedRuns runs(c);
-    TRY(sorted_runs(c, n_keys, keys, "group iota", &runs));
+    TRY(sorted_runs(c, n_keys, n_keys, keys, "group iota", &runs));
     const bdf_col* idx = runs.perm.get();
     const int64_t n_groups = runs.n_runs;
     const uint32_t* d_starts = (const uint32_t*)runs.starts->chunks[0].values;
@@ -2875,7 +2881,61 @@ static int hist_dev(bdf_ctx* c, const bdf_col* x, int nbins, const double* range
 // equi-join (k_join.cu): the build side (the right side; the left side for RIGHT) is sorted, gathered and cut into runs of equal
 // key tuples by sorted_runs, as group-by's groups are; every probe row binary-searches the distinct tuples, the counts are scanned into
 // output offsets (one host wait for the total), and the emit writes the index pairs by output position.  FULL appends the build
-// rows of the runs no probe row hit, listed in row order by a compaction of an iota.
+// rows of the runs no probe row hit, listed in row order by a compaction of an iota.  LEFT SEMI / ANTI write one bit per left row
+// instead and compact an iota of the left rows with it.
+
+// What the probe kernels read of every criterion: the probe column's chunk table and the build side's distinct keys.
+struct JoinProbe {
+    std::vector<const void*> tables, build;
+    std::vector<const uint32_t*> build_valid;
+    std::vector<int> chunks, dtypes;
+    int64_t key_bytes = 0;
+};
+
+static int join_probe(bdf_ctx* c, int n_keys, const bdf_col* const* probe, const SortedRuns& runs, JoinProbe* p) {
+    for (int k = 0; k < n_keys; k++) {
+        void* t = nullptr;
+        int n_chunks = 0;
+        TRY(sort_table(c, probe[k], &t, &n_chunks, nullptr));
+        p->tables.push_back(t);
+        p->chunks.push_back(n_chunks);
+        p->build.push_back(runs.distinct[k]->chunks[0].values);
+        p->build_valid.push_back(runs.distinct[k]->chunks[0].validity);
+        p->dtypes.push_back(probe[k]->dtype);
+        p->key_bytes += dtype_width(probe[k]->dtype);
+    }
+    return BDF_OK;
+}
+
+// LEFT SEMI / ANTI: the left rows with (without) a partner, ascending.  No counts and no host wait for a total: a bit per left row
+// compacts an iota, as FULL lists its unmatched rows.
+static int join_exists_dev(bdf_ctx* c, bool anti, int n_keys, const bdf_col* const* lk, const bdf_col* const* rk, bdf_col** out_l, bdf_col** out_r,
+                           int64_t* n_rows_out) {
+    const int64_t np = lk[0]->total_len;
+    SortedRuns runs(c);
+    TRY(sorted_runs(c, n_keys, n_keys, rk, "join iota", &runs));
+    JoinProbe p;
+    TRY(join_probe(c, n_keys, lk, runs, &p));
+    ColOwner mask(c), iota(c), rows(c);
+    TRY(col_alloc(c, kBool, {ChunkPlan{np, false}}, nullptr, 0, mask.out()));
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{np, false}}, nullptr, 0, iota.out()));
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_JOIN, kBool, np, np * p.key_bytes + bitmap_bytes(np));
+        e = launch_join_exists(n_keys, p.dtypes.data(), p.tables.data(), p.chunks.data(), p.build.data(), p.build_valid.data(), np, runs.n_runs,
+                               anti ? 1 : 0, (uint32_t*)mask->chunks[0].values, c->s_compute);
+    }
+    c->launches++;
+    if (e == cudaSuccess && np > 0) e = launch_iota((uint32_t*)iota->chunks[0].values, np, c->sm_count, c->s_compute);
+    if (e == cudaSuccess) e = finish_single_group(c, mask.get());
+    if (e == cudaSuccess) e = finish_single_group(c, iota.get());
+    if (e != cudaSuccess) return fail_cuda(e, "join existence mask");
+    TRY(filter_dev(c, iota.get(), mask.get(), rows.out()));
+    if (n_rows_out) *n_rows_out = rows->chunks[0].len;
+    *out_l = rows.release();
+    if (out_r) *out_r = nullptr;
+    return BDF_OK;
+}
 
 static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, const bdf_col* const* rk, bdf_col** out_l, bdf_col** out_r,
                     int64_t* n_rows_out) {
@@ -2884,7 +2944,7 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
     if (!lk || !rk) return fail(BDF_INVALID, "null argument");
     for (int k = 0; k < n_keys; k++)
         if (!lk[k] || !rk[k]) return fail(BDF_INVALID, "null join column");
-    if (how < BDF_JOIN_LEFT || how > BDF_JOIN_FULL) return fail(BDF_UNSUPPORTED, "unknown join type %d", how);
+    if (how < BDF_JOIN_LEFT || how > BDF_JOIN_LEFT_ANTI) return fail(BDF_UNSUPPORTED, "unknown join type %d", how);
     for (int k = 0; k < n_keys; k++)
         if (lk[k]->dtype < 0 || lk[k]->dtype >= BDF_NTYPES || rk[k]->dtype < 0 || rk[k]->dtype >= BDF_NTYPES)
             return fail(BDF_UNSUPPORTED, "join columns must be numeric");
@@ -2894,6 +2954,7 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
         if (lk[k]->total_len != lk[0]->total_len || rk[k]->total_len != rk[0]->total_len)
             return fail(BDF_LENGTH_MISMATCH, "join columns of one side have different lengths");
     if (lk[0]->total_len > 0xffffffffLL || rk[0]->total_len > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
+    if (how == BDF_JOIN_LEFT_SEMI || how == BDF_JOIN_LEFT_ANTI) return join_exists_dev(c, how == BDF_JOIN_LEFT_ANTI, n_keys, lk, rk, out_l, out_r, n_rows_out);
     const bool swap = how == BDF_JOIN_RIGHT, full = how == BDF_JOIN_FULL, outer = how != BDF_JOIN_INNER;
     const bdf_col* const* probe = swap ? rk : lk;
     const bdf_col* const* build = swap ? lk : rk;
@@ -2901,25 +2962,14 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
 
     // the build side: sorted row numbers, the distinct key tuples, the first sorted row of every run
     SortedRuns runs(c);
-    TRY(sorted_runs(c, n_keys, build, "join iota", &runs));
+    TRY(sorted_runs(c, n_keys, n_keys, build, "join iota", &runs));
     const int64_t n_runs = runs.n_runs;
     const uint32_t* perm = (const uint32_t*)runs.perm->chunks[0].values;
     const uint32_t* starts = (const uint32_t*)runs.starts->chunks[0].values;
 
     // the probe side is read in place, through the chunk tables of its key columns
-    std::vector<const void*> ptables((size_t)n_keys), bkeys((size_t)n_keys);
-    std::vector<const uint32_t*> bvalid((size_t)n_keys);
-    std::vector<int> pchunks((size_t)n_keys), dtypes((size_t)n_keys);
-    int64_t key_bytes = 0;
-    for (int k = 0; k < n_keys; k++) {
-        void* t = nullptr;
-        TRY(sort_table(c, probe[k], &t, &pchunks[k], nullptr));
-        ptables[k] = t;
-        bkeys[k] = runs.distinct[k]->chunks[0].values;
-        bvalid[k] = runs.distinct[k]->chunks[0].validity;
-        dtypes[k] = probe[k]->dtype;
-        key_bytes += dtype_width(probe[k]->dtype);
-    }
+    JoinProbe jp;
+    TRY(join_probe(c, n_keys, probe, runs, &jp));
     const int64_t blocks = (np + join_tile_rows() - 1) / join_tile_rows();
     Scratch<unsigned long long> counts, block_sums;
     Scratch<uint32_t> mstart;
@@ -2932,9 +2982,9 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
     if (e != cudaSuccess) return fail_cuda(e, "join scratch allocation");
     unsigned long long total = 0;   // output rows of the probe part
     {
-        LaunchTimer t(c, BDF_K_JOIN, BDF_U32, np, np * (key_bytes + 8 + 4));
-        e = launch_join_count(n_keys, dtypes.data(), ptables.data(), pchunks.data(), bkeys.data(), bvalid.data(), np, starts, n_runs, nb, outer ? 1 : 0,
-                              counts, mstart, hit, block_sums, c->s_compute);
+        LaunchTimer t(c, BDF_K_JOIN, BDF_U32, np, np * (jp.key_bytes + 8 + 4));
+        e = launch_join_count(n_keys, jp.dtypes.data(), jp.tables.data(), jp.chunks.data(), jp.build.data(), jp.build_valid.data(), np, starts, n_runs, nb,
+                              outer ? 1 : 0, counts, mstart, hit, block_sums, c->s_compute);
     }
     if (e == cudaSuccess) {
         LaunchTimer t(c, BDF_K_JOIN, BDF_U64, np, np * 16 + blocks * 16);
@@ -2983,6 +3033,63 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
     *out_l = swap ? b : p;
     *out_r = swap ? p : b;
     if (n_rows_out) *n_rows_out = (int64_t)n_out;
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// as-of join (k_join.cu k_join_asof): the right side is sorted once by (by..., on), stably, and cut into runs on the `by` keys only;
+// every left row finds its run with the equi-join's search and its `on` key inside the run, reading the left chunks in place.
+
+static int join_asof_dev(bdf_ctx* c, const bdf_col* lon, const bdf_col* ron, int n_by, const bdf_col* const* lby, const bdf_col* const* rby,
+                         const bdf_asof_spec* spec, bdf_col** out) {
+    if (n_by < 0 || n_by > 16) return fail(BDF_INVALID, "0..16 as-of by keys");
+    if (!lon || !ron || !spec || !out || (n_by && (!lby || !rby))) return fail(BDF_INVALID, "null argument");
+    std::vector<const bdf_col*> lk, rk;   // by..., on
+    for (int k = 0; k < n_by; k++) {
+        if (!lby[k] || !rby[k]) return fail(BDF_INVALID, "null join column");
+        lk.push_back(lby[k]);
+        rk.push_back(rby[k]);
+    }
+    lk.push_back(lon);
+    rk.push_back(ron);
+    const int nk = n_by + 1;
+    if (spec->direction < BDF_ASOF_BACKWARD || spec->direction > BDF_ASOF_NEAREST) return fail(BDF_UNSUPPORTED, "unknown as-of direction %d", spec->direction);
+    for (int k = 0; k < nk; k++)
+        if (lk[k]->dtype < 0 || lk[k]->dtype >= BDF_NTYPES || rk[k]->dtype < 0 || rk[k]->dtype >= BDF_NTYPES)
+            return fail(BDF_UNSUPPORTED, "join columns must be numeric");
+    for (int k = 0; k < nk; k++)
+        if (lk[k]->dtype != rk[k]->dtype) return fail(BDF_UNSUPPORTED, "Join columns must have compatible types");
+    if (spec->has_tolerance && (dtype_is_float(lon->dtype) ? !(spec->tolerance_f >= 0.0) : spec->tolerance < 0))
+        return fail(BDF_INVALID, "the as-of tolerance must be >= 0");
+    for (int k = 0; k < nk; k++)
+        if (lk[k]->total_len != lon->total_len || rk[k]->total_len != ron->total_len)
+            return fail(BDF_LENGTH_MISMATCH, "join columns of one side have different lengths");
+    if (ron->total_len > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
+    const int64_t nl = lon->total_len, nr = ron->total_len;
+
+    SortedRuns runs(c);
+    TRY(sorted_runs(c, nk, n_by, rk.data(), "as-of join iota", &runs));
+    JoinProbe p;
+    TRY(join_probe(c, n_by, lk.data(), runs, &p));
+    void* on_table = nullptr;
+    int on_chunks = 0;
+    TRY(sort_table(c, lon, &on_table, &on_chunks, nullptr));
+    const DevChunk& son = runs.sorted[n_by]->chunks[0];   // the right `on` key in sorted order
+    ColOwner o(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{nl, true}}, nullptr, 0, o.out()));
+    cudaError_t e;
+    {
+        LaunchTimer t(c, BDF_K_JOIN, lon->dtype, nl, nl * (p.key_bytes + dtype_width(lon->dtype) + 4) + bitmap_bytes(nl));
+        e = launch_join_asof(n_by, p.dtypes.data(), p.tables.data(), p.chunks.data(), p.build.data(), p.build_valid.data(), lon->dtype, on_table,
+                             on_chunks, son.values, son.validity, spec->direction, spec->allow_exact_matches ? 1 : 0, spec->has_tolerance ? 1 : 0,
+                             (unsigned long long)spec->tolerance, spec->tolerance_f, nl,
+                             n_by ? (const uint32_t*)runs.starts->chunks[0].values : nullptr, runs.n_runs, nr,
+                             (const uint32_t*)runs.perm->chunks[0].values, (uint32_t*)o->chunks[0].values, o->chunks[0].validity, c->s_compute);
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "as-of join");
+    o->null_counts[0] = -1;   // the rows without a partner: counted on demand
+    *out = o.release();
     return BDF_OK;
 }
 
@@ -4065,7 +4172,7 @@ static int pqw_dictionary(bdf_ctx* c, const bdf_col* col, const bdf_col* rg_col,
     std::vector<unsigned int> first((size_t)n_rg, 0);
     pc->dcount.assign((size_t)n_rg, 0);
     SortedRuns r(c);
-    TRY(sorted_runs(c, 2, keys, "Parquet dictionary iota", &r));
+    TRY(sorted_runs(c, 2, 2, keys, "Parquet dictionary iota", &r));
     {
         TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, all_ids.out()));
         const int64_t words = (n + 31) / 32;
@@ -7080,8 +7187,15 @@ int bdf_join_indices_dev(bdf_ctx* c, int32_t join_type, int32_t n_keys, const bd
                          bdf_col** left_indices, bdf_col** right_indices, int64_t* n_rows) {
     if (c && c->fleet) return fail(BDF_UNSUPPORTED, "a join moves rows between chunks: use a one-GPU context (bdf_init) for it");
     ENTER(c);
-    if (!left_indices || !right_indices) return fail(BDF_INVALID, "null argument");
+    if (!left_indices || (!right_indices && join_type != BDF_JOIN_LEFT_SEMI && join_type != BDF_JOIN_LEFT_ANTI)) return fail(BDF_INVALID, "null argument");
     return join_dev(c, join_type, n_keys, left_keys, right_keys, left_indices, right_indices, n_rows);
+}
+
+int bdf_join_asof_dev(bdf_ctx* c, const bdf_col* left_on, const bdf_col* right_on, int32_t n_by, const bdf_col* const* left_by,
+                      const bdf_col* const* right_by, const bdf_asof_spec* spec, bdf_col** right_indices) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "a join moves rows between chunks: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return join_asof_dev(c, left_on, right_on, n_by, left_by, right_by, spec, right_indices);
 }
 
 int bdf_window_dev(bdf_ctx* c, int32_t n_partition, const bdf_col* const* partition_by, int32_t n_order, const bdf_sort_key* order_by,

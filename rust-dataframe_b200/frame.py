@@ -137,15 +137,27 @@ def plan_aggregate(schema: Dict[str, int], groups: Sequence[str], aggregations: 
 
 
 def join(other: "DeviceFrame", criteria: Sequence[Tuple[str, str]], how: str):
-    """Transformation::Join against `other`: criteria [(column of this frame, column of other)], how in left | right | inner | full."""
+    """Transformation::Join against `other`: criteria [(column of this frame, column of other)], how in left | right | inner | full |
+    left_semi | left_anti."""
     return ("join", (other, [(a, b) for a, b in criteria], how))
 
 
-def plan_join(schema_a: Dict[str, int], schema_b: Dict[str, int], criteria: Sequence[Tuple[str, str]]) -> List[Tuple[str, int]]:
+def join_asof(other: "DeviceFrame", left_on: str, right_on: Optional[str] = None, by: Sequence[Tuple[str, str]] = (), direction: str = "backward",
+              allow_exact_matches: bool = True, tolerance=None):
+    """An as-of join against `other` (DeviceFrame.join_asof): `by` is [(column of this frame, column of other)]."""
+    return ("join_asof", (other, left_on, left_on if right_on is None else right_on, [(a, b) for a, b in by], direction, allow_exact_matches,
+                          tolerance))
+
+
+EXISTENCE_JOINS = ("left_semi", "left_anti")
+
+
+def plan_join(schema_a: Dict[str, int], schema_b: Dict[str, int], criteria: Sequence[Tuple[str, str]], how: Optional[str] = None) -> List[Tuple[str, int]]:
     """The joined schema `Dataset::try_join` (expression.rs:223-287) plans for `criteria` ([(column of a, column of b)]), as
     [(name, dtype)]: a's columns, then b's; a name present on both sides becomes `a.<name>` / `b.<name>`.  Its checks in its
     order, per criterion: both missing, a missing, b missing, different types -- ComputeError with its texts.  Then what the
-    device path adds: non-numeric keys are UnsupportedType, and zero criteria (a cross join in the reference) are refused."""
+    device path adds: non-numeric keys are UnsupportedType, and zero criteria (a cross join in the reference) are refused.
+    how = "left_semi" | "left_anti": the same checks, and a's columns only, names unchanged."""
     for a, b in criteria:
         if a not in schema_a and b not in schema_b:
             raise N.ComputeError("Join columns do not exist in tables")
@@ -160,6 +172,8 @@ def plan_join(schema_a: Dict[str, int], schema_b: Dict[str, int], criteria: Sequ
             raise N.UnsupportedType(f"join column {a!r} is not numeric: join keys must be")
     if not criteria:
         raise N.ComputeError("Join criteria cannot be empty")
+    if how in EXISTENCE_JOINS:
+        return list(schema_a.items())
     out = [(f"a.{n}" if n in schema_b else n, t) for n, t in schema_a.items()]
     return out + [(f"b.{n}" if n in schema_a else n, t) for n, t in schema_b.items()]
 
@@ -258,6 +272,8 @@ def _columns_read(t) -> set:
         return {c for c, _ in arg}
     if kind == "window":
         return set(_window_columns(*arg))
+    if kind == "join_asof":
+        return {arg[1]} | {a for a, _ in arg[3]}
     return set()
 
 
@@ -301,9 +317,12 @@ def _schema_walk(schema: "OrderedDict[str, int]", transformations: Sequence[tupl
                 t = arg.dtype if arg.function == "cast" else cur.get(arg.inputs[0], F64)
                 cur.pop(arg.output, None)
                 cur[arg.output] = t
-        elif kind == "join":
+        elif kind in ("join", "join_asof"):
             try:
-                cur = OrderedDict(plan_join(cur, arg[0].schema, arg[1]))
+                if kind == "join":
+                    cur = OrderedDict(plan_join(cur, arg[0].schema, arg[1], arg[2]))
+                else:
+                    cur = OrderedDict(plan_join(cur, arg[0].schema, list(arg[3]) + [(arg[1], arg[2])]))
             except N.ArrowError:       # the step itself raises when it is evaluated; nothing after it is fused
                 cur = OrderedDict()
         elif kind == "window":
@@ -332,7 +351,7 @@ def plan_fusion(schema: "OrderedDict[str, int]", transformations: Sequence[tuple
     schemas = _schema_walk(schema, steps)
     needed = _needed_after(steps, list(schemas[-1].keys()))
     for i, (kind, _) in enumerate(steps):
-        if kind == "join":   # every column of the frame reaches the joined frame (perhaps renamed): all are observable
+        if kind in ("join", "join_asof"):   # every column of the frame reaches the joined frame (perhaps renamed): all are observable
             for j in range(i):
                 needed[j] |= set(schemas[i])
     out: List[tuple] = []
@@ -657,12 +676,40 @@ class DeviceFrame:
         pairs of `join_indices` (one chunk each; a NULL index gives a NULL slot)."""
         from .functions import join_indices
 
-        plan = plan_join(self.schema, other.schema, criteria)
+        plan = plan_join(self.schema, other.schema, criteria, how)
         li, ri = join_indices([self.column(a) for a, _ in criteria], [other.column(b) for _, b in criteria], how)
+        if how in EXISTENCE_JOINS:   # the left rows that have (lack) a partner, in left order: this frame's columns only
+            try:
+                return DeviceFrame(OrderedDict((name, c.take(li)) for name, c in self.columns.items()))
+            finally:
+                li.free()
         try:
             cols = [c.take(li) for c in self.columns.values()] + [c.take(ri) for c in other.columns.values()]
         finally:
             li.free()
+            ri.free()
+        return DeviceFrame(OrderedDict((name, c) for (name, _), c in zip(plan, cols)))
+
+    def join_asof(self, other: "DeviceFrame", left_on: str, right_on: Optional[str] = None, by: Sequence[Tuple[str, str]] = (),
+                  direction: str = "backward", allow_exact_matches: bool = True, tolerance=None) -> "DeviceFrame":
+        """pandas' merge_asof (join_asof_indices): every row of this frame, in its order, with the columns of the `other` row whose
+        `right_on` key is the last at or before its `left_on` key ("backward"), the first at or after it ("forward") or the nearer
+        ("nearest"), among the rows whose `by` pairs [(column of this frame, column of other)] are equal.  The schema is plan_join's
+        (this frame's columns, then other's, `a.` / `b.` on a name clash); other's columns are NULL where there is no partner.  The
+        two `on` columns must have the same temporal type; for a Date / Timestamp / Time key `tolerance` may be a datetime.timedelta,
+        which must be a whole number of the key's unit."""
+        from .functions import join_asof_indices
+
+        right_on = left_on if right_on is None else right_on
+        plan = plan_join(self.schema, other.schema, list(by) + [(left_on, right_on)])
+        lon, ron = self.column(left_on), other.column(right_on)
+        if lon.temporal != ron.temporal:
+            raise N.UnsupportedType(f"as-of keys {left_on!r} ({lon.temporal!r}) and {right_on!r} ({ron.temporal!r}) have different temporal types")
+        ri = join_asof_indices(lon, ron, [self.column(a) for a, _ in by], [other.column(b) for _, b in by], direction, allow_exact_matches,
+                               tolerance)
+        try:
+            cols = list(self.columns.values()) + [c.take(ri) for c in other.columns.values()]
+        finally:
             ri.free()
         return DeviceFrame(OrderedDict((name, c) for (name, _), c in zip(plan, cols)))
 
@@ -762,6 +809,8 @@ class DeviceFrame:
                 frame = frame.sort(arg)
             elif kind == "join":
                 frame = frame.join(*arg)
+            elif kind == "join_asof":
+                frame = frame.join_asof(*arg)
             elif kind == "window":
                 frame = frame.window(*arg)
             elif kind == "group_aggregate":

@@ -1084,10 +1084,11 @@ _CARRY_GROUP = ("min", "max", "first", "last", "mode")   # aggregations whose re
 
 def join_indices(left_keys: Sequence["Column"], right_keys: Sequence["Column"], how: str):
     """calc_equijoin_indices (src/functions/join.rs:19-137) on the device (bdf_join_indices_dev): criterion k is
-    ``(left_keys[k], right_keys[k])``; ``how`` is "left", "right", "inner" or "full".  Returns ``(left_idx, right_idx)``, two
-    one-chunk UInt32 Columns of row numbers (NULL = no partner) to ``take`` each side's columns with.  The order of the pairs is
-    fixed (left rows in row order, each one's partners in right row order; see include/b200df.h), a null key matches nothing,
-    NaN == NaN and -0.0 == 0.0."""
+    ``(left_keys[k], right_keys[k])``; ``how`` is "left", "right", "inner", "full", "left_semi" or "left_anti".  Returns
+    ``(left_idx, right_idx)``, two one-chunk UInt32 Columns of row numbers (NULL = no partner) to ``take`` each side's columns with.
+    The order of the pairs is fixed (left rows in row order, each one's partners in right row order; see include/b200df.h), a null
+    key matches nothing, NaN == NaN and -0.0 == 0.0.  "left_semi" / "left_anti" return ``(left_idx, None)``: the left rows that have
+    (lack) a partner, each once, ascending, without nulls."""
     if how not in N.JOIN_TYPES:
         raise N.UnsupportedType(f"join type {how!r} is not one of {sorted(N.JOIN_TYPES)}")
     if len(left_keys) != len(right_keys):
@@ -1100,7 +1101,68 @@ def join_indices(left_keys: Sequence["Column"], right_keys: Sequence["Column"], 
     rk = (C.c_void_p * n)(*[k.handle for k in right_keys])
     hl, hr, rows = C.c_void_p(), C.c_void_p(), C.c_int64(0)
     N.raise_for_status(N.lib().bdf_join_indices_dev(ctx.handle, N.JOIN_TYPES[how], n, lk, rk, C.byref(hl), C.byref(hr), C.byref(rows)))
+    if how in ("left_semi", "left_anti"):
+        return Column(ctx, hl), None
     return Column(ctx, hl), Column(ctx, hr)
+
+
+_TIME_UNIT_NS = (10 ** 9, 10 ** 6, 1000, 1)   # nanoseconds per arrow TimeUnit s, ms, us, ns
+
+
+def _asof_tolerance(tolerance, on: "Column"):
+    """(has_tolerance, tolerance, tolerance_f) of bdf_asof_spec: a float for a Float32 / Float64 key (+inf allowed), an integer in the
+    key's own units otherwise, or a datetime.timedelta for a Date / Timestamp / Time key, converted exactly to its unit."""
+    if tolerance is None:
+        return 0, 0, 0.0
+    if isinstance(tolerance, datetime.timedelta):
+        t = getattr(on, "temporal", None)
+        if t is None:
+            raise N.ComputeError("a timedelta tolerance needs a Date, Timestamp or Time key")
+        us = (tolerance.days * 86_400 + tolerance.seconds) * 10 ** 6 + tolerance.microseconds
+        per = 86_400 * 10 ** 9 if t.kind == DATE32 else 10 ** 6 if t.kind == DATE64 else _TIME_UNIT_NS[t.unit]
+        if (us * 1000) % per:
+            raise N.ComputeError(f"tolerance {tolerance!r} is not a whole number of the key's unit")
+        tolerance = us * 1000 // per
+    elif is_float(on.dtype):
+        v = float(tolerance)
+        if not v >= 0:
+            raise N.ComputeError(f"the as-of tolerance must be >= 0, not {tolerance!r}")
+        return 1, 0, v
+    if isinstance(tolerance, float) and not tolerance.is_integer():
+        raise N.ComputeError(f"tolerance {tolerance!r} over an integer key must be an integer")
+    v = int(tolerance)
+    if not 0 <= v <= _INT64_MAX:
+        raise N.ComputeError(f"the as-of tolerance must be in 0..2^63-1, not {tolerance!r}")
+    return 1, v, 0.0
+
+
+def join_asof_indices(left_on: "Column", right_on: "Column", left_by: Sequence["Column"] = (), right_by: Sequence["Column"] = (),
+                      direction: str = "backward", allow_exact_matches: bool = True, tolerance=None) -> "Column":
+    """pandas' merge_asof on the device (bdf_join_asof_dev): for every left row, the right row whose ``on`` key is the last at or before
+    its own ("backward"), the first at or after it ("forward") or the nearer of the two ("nearest", ties backward), among the right rows
+    whose ``by`` keys equal the left row's.  Of equal keys, backward takes the last right row and forward the first.  Returns one
+    one-chunk UInt32 Column with a right row number per left row (NULL = no partner) to ``take`` the right columns with; left order
+    is kept.  ``allow_exact_matches=False`` makes the bounds strict; ``tolerance`` (see _asof_tolerance) nulls a pick farther away.
+    Neither side needs to be sorted; null and NaN keys match nothing (include/b200df.h)."""
+    if direction not in N.ASOF_DIRECTIONS:
+        raise N.UnsupportedType(f"as-of direction {direction!r} is not one of {sorted(N.ASOF_DIRECTIONS)}")
+    if len(left_by) != len(right_by):
+        raise N.ComputeError("every as-of by key needs a left and a right column")
+    if len(left_by) > 16:
+        raise N.ComputeError("0..16 as-of by keys")
+    cols = [left_on, right_on, *left_by, *right_by]
+    if any(isinstance(c, ListColumn) for c in cols):
+        raise N.UnsupportedType("a list column is not a join key: as-of keys must be numeric")
+    if getattr(left_on, "temporal", None) != getattr(right_on, "temporal", None):
+        raise N.UnsupportedType(f"as-of keys of different temporal types ({left_on.temporal!r}, {right_on.temporal!r}): cast them first")
+    spec = N.AsofSpec(N.ASOF_DIRECTIONS[direction], 1 if allow_exact_matches else 0, *_asof_tolerance(tolerance, left_on))
+    ctx = left_on.ctx
+    n = len(left_by)
+    lb = (C.c_void_p * max(n, 1))(*[k.handle for k in left_by])
+    rb = (C.c_void_p * max(n, 1))(*[k.handle for k in right_by])
+    h = C.c_void_p()
+    N.raise_for_status(N.lib().bdf_join_asof_dev(ctx.handle, left_on.handle, right_on.handle, n, lb, rb, C.byref(spec), C.byref(h)))
+    return Column(ctx, h)
 
 
 _INT64_MIN, _INT64_MAX = -2 ** 63, 2 ** 63 - 1
