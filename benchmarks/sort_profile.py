@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One 1e8-row Float64 sort (k_sort_keys, 8 x [k_radix_hist, k_radix_scan, k_radix_scatter]) and one take, for ncu:
+"""One 1e8-row Float64 sort (k_sort_keys, 8 x [k_radix_hist, k_scan_one, k_radix_scatter]) and one take, for ncu:
    ncu --set full -k regex:"k_sort_keys|k_radix_hist|k_radix_scatter|k_take" --launch-skip 15 -c 3 python benchmarks/sort_profile.py"""
 import os
 import sys

@@ -395,6 +395,19 @@ int null_test_tile_elems(int dtype, int test);
 cudaError_t launch_cond(int fn, int dtype, const void* descs, int n_args, int n_chunks, int64_t tiles, uint32_t* warp_counts, cudaStream_t s);
 cudaError_t launch_null_test(int test, int dtype, const void* descs, int n_chunks, int64_t tiles, cudaStream_t s);
 
+// Exclusive prefix scans (k_scan.cu).  launch_scan_one scans `count` entries in place in one CTA; *total = their sum unless total is
+// null.  The others scan n 64-bit entries in place in a buffer of n + 1: afterwards data[i] = the sum of the entries before i and
+// data[n] = the total; sums is scratch of scan_tile_sums(n) entries.  k...Launches: the kernels each launcher counts for.
+template <typename T>
+cudaError_t launch_scan_one(T* data, long long count, T* total, cudaStream_t s);
+long long scan_tile_sums(long long n);
+constexpr int kScanSumsLaunches = 2;   // sums already holds the tile sums (kScanTile entries per CTA, scan.cuh)
+cudaError_t launch_scan_sums(unsigned long long* data, long long n, unsigned long long* sums, cudaStream_t s);
+constexpr int kScanLaunches = 3;
+cudaError_t launch_scan(unsigned long long* data, long long n, unsigned long long* sums, cudaStream_t s);
+constexpr int kScanPopcountLaunches = 3;   // the entries are the popcounts of words[0, n_words): counts[w] = the set bits before word w
+cudaError_t launch_scan_popcount(const uint32_t* words, long long n_words, unsigned long long* counts, unsigned long long* sums, cudaStream_t s);
+
 // Sort indices and take (k_sort.cu).
 size_t sort_chunk_size();
 void fill_sort_chunk(void* base, int64_t i, const void* values, const uint32_t* validity, int64_t start, int32_t bit_off, int32_t val_bit_off);
@@ -445,12 +458,10 @@ cudaError_t launch_dist_median(int dtype, const void* sval, const uint32_t* star
                                uint32_t* out_valid, cudaStream_t s);
 
 // Joins (k_join.cu).
-int join_tile_rows();
 cudaError_t launch_join_count(int n_keys, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,
                               const uint32_t* const* build_valid, long long n_probe, const uint32_t* run_starts, long long n_runs, long long n_build,
                               int outer, unsigned long long* counts, uint32_t* match_start, unsigned char* hit, unsigned long long* block_sums,
                               cudaStream_t s);
-cudaError_t launch_join_scan(unsigned long long* counts, long long n_probe, unsigned long long* block_sums, cudaStream_t s);
 cudaError_t launch_join_emit(const unsigned long long* offs, long long n_probe, const uint32_t* match_start, const uint32_t* perm, unsigned long long probe_rows,
                              const uint32_t* unmatched, unsigned long long n_out, uint32_t* probe_out, uint32_t* probe_valid, uint32_t* build_out,
                              uint32_t* build_valid, cudaStream_t s);
@@ -465,8 +476,6 @@ cudaError_t launch_join_asof(int n_by, const int* dtypes, const void* const* pro
                              uint32_t* out_valid, cudaStream_t s);
 
 // Window functions (k_window.cu).
-int window_count_tile();
-cudaError_t launch_window_count(const uint32_t* words, long long n_words, unsigned long long* counts, unsigned long long* block_sums, cudaStream_t s);
 cudaError_t launch_window_rank(const void* const* p, long long n_p, const void* const* q, long long n_q, long long n, const uint32_t* perm,
                                void* const* outs, cudaStream_t s);
 cudaError_t launch_window_shift(int dtype, const void* const* p, long long n_p, long long n, const void* x, int nx, long long k, int lead,
@@ -532,10 +541,8 @@ size_t json_key_bytes();
 size_t json_desc_bytes();
 size_t json_slow_bytes();
 size_t json_list_chunk_bytes();
-long long json_scan_sums(long long n);
 cudaError_t launch_json_nl_count(const uint8_t* text, long long n, unsigned long long* counts, cudaStream_t s);
 cudaError_t launch_json_nl_index(const uint8_t* text, long long n, const unsigned long long* offsets, unsigned long long* nl, cudaStream_t s);
-cudaError_t launch_json_scan(unsigned long long* data, long long n, unsigned long long* sums, cudaStream_t s);
 cudaError_t launch_json_lex(const uint8_t* text, long long n, const unsigned long long* nl, long long n_nl, unsigned long long* members,
                             unsigned long long* is_rec, unsigned long long* bad, int sm_count, cudaStream_t s);
 cudaError_t launch_json_members(const uint8_t* text, long long n, const unsigned long long* nl, long long n_nl, const unsigned long long* first_member,
@@ -555,7 +562,6 @@ cudaError_t launch_json_list_fill(const uint8_t* text, const void* members, cons
                                   void* slow, unsigned long long* n_slow, long long slow_cap, cudaStream_t s);
 
 // CSV writer (k_csv_write.cu).
-int csvw_tile();
 cudaError_t launch_csvw_measure(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows,
                                 unsigned long long* lens, unsigned long long* block_sums, cudaStream_t s);
 cudaError_t launch_csvw_emit(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows, int delim,

@@ -8,8 +8,7 @@
 //   k_csv_dfa_scan     one CTA: the true state at the first byte of every CTA, and the state at the end of the file;
 //   k_csv_mark         the exclusive scan inside the CTA gives every thread its start state; it walks its 16 bytes and writes
 //                      two 16-bit masks: the bytes that end a field (delimiter or terminator) and those that end a record, and
-//                      the CTA's count of field ends;
-//   k_csv_scan_counts  one CTA: exclusive 64-bit scan of the CTA counts, and the total;
+//                      the CTA's count of field ends, whose exclusive scan (k_scan_one of k_scan.cu) ends with the total;
 //   k_csv_index        the masks -> the field index: one int64 per field, the byte where it ends, bit 63 set when the field
 //                      ends its record; the first such field gives the first record's field count.
 // A field starts one byte after the end of the previous one; after a record end, csv-core skips every '\r' / '\n' first (blank
@@ -25,6 +24,7 @@
 //   k_csv_scatter      writes the host's exact values.
 #include "common.cuh"
 #include "csv_parse.cuh"
+#include "scan.cuh"
 
 #include <algorithm>
 
@@ -125,7 +125,6 @@ __global__ void __launch_bounds__(kThreads)
 k_csv_mark(const uint8_t* __restrict__ text, long long n, uint8_t delim, const uint8_t* __restrict__ start, uint16_t* __restrict__ fe,
            uint16_t* __restrict__ re, unsigned long long* __restrict__ block_counts) {
     __shared__ uint32_t s_warp[kWarpsPerCta];
-    __shared__ int s_cnt[kWarpsPerCta];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
     uint8_t b[kCsvBytes];
@@ -151,53 +150,16 @@ k_csv_mark(const uint8_t* __restrict__ text, long long n, uint8_t delim, const u
     }
     fe[g] = (uint16_t)fbits;
     re[g] = (uint16_t)rbits;
-    int c = __popc(fbits);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-    if (lane == 0) s_cnt[warp] = c;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long t = 0;
-#pragma unroll
-        for (int w = 0; w < kWarpsPerCta; w++) t += (unsigned long long)s_cnt[w];
-        block_counts[blockIdx.x] = t;
-    }
-}
-
-// Exclusive scan of the CTA counts in place (one CTA of 1024 threads, each owning a contiguous run); *total = the sum.
-__global__ void __launch_bounds__(1024) k_csv_scan_counts(unsigned long long* __restrict__ data, long long count, unsigned long long* __restrict__ total) {
-    __shared__ unsigned long long s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long per = (count + 1023) / 1024;
-    const long long begin = min(count, (long long)threadIdx.x * per), end = min(count, begin + per);
-    unsigned long long sum = 0;
-    for (long long i = begin; i < end; i++) sum += data[i];
-    unsigned long long x = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    unsigned long long run = x - sum;
-    for (int w = 0; w < warp; w++) run += s_warp[w];
-    for (long long i = begin; i < end; i++) { const unsigned long long v = data[i]; data[i] = run; run += v; }
-    if (threadIdx.x == 1023) *total = run;
+    const int c = cta_sum(__popc(fbits));
+    if (threadIdx.x == 0) block_counts[blockIdx.x] = (unsigned long long)c;
 }
 
 __global__ void __launch_bounds__(kThreads)
 k_csv_index(const uint16_t* __restrict__ fe, const uint16_t* __restrict__ re, long long n16, const unsigned long long* __restrict__ block_offsets,
             unsigned long long* __restrict__ ends, unsigned long long* __restrict__ first_rec) {
-    __shared__ int s_warp[kWarpsPerCta];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
     const uint32_t fbits = g < n16 ? fe[g] : 0u, rbits = g < n16 ? re[g] : 0u;
-    const int c = __popc(fbits);
-    int x = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    unsigned long long off = block_offsets[blockIdx.x] + (unsigned long long)(x - c);
-    for (int w = 0; w < warp; w++) off += (unsigned long long)s_warp[w];
+    unsigned long long off = block_offsets[blockIdx.x] + (unsigned long long)cta_exclusive_sum(__popc(fbits));
     uint32_t m = fbits;
     while (m) {
         const int k = __ffs(m) - 1;
@@ -344,8 +306,7 @@ cudaError_t launch_csv_tokenize(const uint8_t* text, long long n, uint8_t delim,
     k_csv_dfa_reduce<<<(unsigned)tiles, kThreads, 0, s>>>(text, n, delim, agg);
     k_csv_dfa_scan<<<1, 1024, 0, s>>>(agg, tiles, start, final_state);
     k_csv_mark<<<(unsigned)tiles, kThreads, 0, s>>>(text, n, delim, start, fe, re, block_counts);
-    k_csv_scan_counts<<<1, 1024, 0, s>>>(block_counts, tiles, block_counts + tiles);
-    return cudaGetLastError();
+    return launch_scan_one(block_counts, tiles, block_counts + tiles, s);   // its error check covers the launches above
 }
 
 cudaError_t launch_csv_index(const uint16_t* fe, const uint16_t* re, long long n, const unsigned long long* block_offsets, unsigned long long* ends,

@@ -3,9 +3,8 @@
 //
 // The rows are written in blocks of at most a few million rows, so the text of one block fits a fixed device buffer; per block:
 //   k_csvw_measure  one thread per row walks the column table and computes the row's byte length from every value, validity bit and
-//                   dtype (floats: their shortest digits); the CTA's total goes to block_sums, in the tile layout of k_join.cu's
-//                   64-bit scan (256 threads x 8 rows), which then turns the lengths into byte offsets and puts the block's total
-//                   behind its last row.
+//                   dtype (floats: their shortest digits); the CTA's total goes to block_sums, the tile sums of launch_scan_sums
+//                   (k_scan.cu), which then turns the lengths into byte offsets and puts the block's total behind its last row.
 //   k_csvw_emit     one row per thread: formats it again (the digits are recomputed rather than stored: a few hundred integer
 //                   instructions per float against the 8+ bytes per field a stored form would move) into a shared-memory window
 //                   at its offset, then the CTA stores its contiguous byte range with aligned 16-byte stores, single bytes only at
@@ -15,11 +14,11 @@
 // the chunk of a row is found once per CTA by binary search and then by a forward walk.
 #include "common.cuh"
 #include "csv_format.cuh"
+#include "scan.cuh"
 
 namespace bdf {
 
-constexpr int kCsvwItems = 8;
-constexpr int kCsvwTile = kThreads * kCsvwItems;   // rows per measure CTA: the tile of launch_join_scan
+constexpr int kCsvwTile = kScanTile;              // rows per measure CTA
 constexpr int kCsvwWindow = 24576;                 // bytes of text a CTA of the emit step stages in shared memory
 
 struct CsvwArgs {
@@ -89,13 +88,12 @@ __device__ int csvw_row(const CsvwArgs& a, int ch, long long local, char* p) {
 
 __global__ void __launch_bounds__(kThreads) k_csvw_measure(const CsvwArgs a, unsigned long long* __restrict__ lens, unsigned long long* __restrict__ block_sums) {
     __shared__ int s_chunk;
-    __shared__ unsigned long long s_warp[kWarpsPerCta];
     const long long base = (long long)blockIdx.x * kCsvwTile;
     if (threadIdx.x == 0) s_chunk = csvw_chunk_of(a, a.row0 + base);
     __syncthreads();
     int ch = s_chunk;
     unsigned long long sum = 0;
-    for (int it = 0; it < kCsvwItems; it++) {
+    for (int it = 0; it < kScanItems; it++) {
         const long long i = base + it * kThreads + threadIdx.x;
         if (i >= a.rows) break;
         const long long g = a.row0 + i;
@@ -104,16 +102,8 @@ __global__ void __launch_bounds__(kThreads) k_csvw_measure(const CsvwArgs a, uns
         lens[i] = len;
         sum += len;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = sum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long t = 0;
-#pragma unroll
-        for (int w = 0; w < kWarpsPerCta; w++) t += s_warp[w];
-        block_sums[blockIdx.x] = t;
-    }
+    sum = cta_sum(sum);
+    if (threadIdx.x == 0) block_sums[blockIdx.x] = sum;
 }
 
 __global__ void __launch_bounds__(kThreads) k_csvw_emit(const CsvwArgs a, const unsigned long long* __restrict__ offs, char* __restrict__ out) {
@@ -160,9 +150,7 @@ static CsvwArgs csvw_args(const CsvwDesc* cols, const long long* chunk_start, in
     return a;
 }
 
-int csvw_tile() { return kCsvwTile; }
-
-// lens: rows + 1 entries; block_sums: ceil(rows / csvw_tile()) entries.
+// lens: rows + 1 entries; block_sums: scan_tile_sums(rows) entries.
 cudaError_t launch_csvw_measure(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows,
                                 unsigned long long* lens, unsigned long long* block_sums, cudaStream_t s) {
     if (rows <= 0) return cudaSuccess;

@@ -7,9 +7,9 @@
 //   k_join_count        one thread per probe row, reading the probe side's chunks in place: a binary search of the distinct
 //                       build tuples in the sort's total order (sort_keys.cuh: the very key transform the sort used, null last)
 //                       gives the run of equal build rows; writes the run's first sorted row and the row's output count
-//                       (outer joins: at least 1), marks the run as hit (full join), and the CTA's total.
-//   k_join_scan_blocks  one CTA: exclusive scan of the CTA totals; the grand total lands behind the last row's count.
-//   k_join_scan_rows    the counts of every CTA become 64-bit exclusive output offsets.
+//                       (outer joins: at least 1), marks the run as hit (full join), and the CTA's total: the tile sums of
+//                       launch_scan_sums (k_scan.cu), which turns the counts into 64-bit output offsets and puts the total behind
+//                       the last one.
 //   k_join_emit         load-balanced by OUTPUT position: every CTA owns kJoinTile output rows, finds the probe rows that produce
 //                       them with a binary search of the offsets, and writes (probe row, perm[run start + j]) and both validity
 //                       bitmaps as whole words.  A hot key with 10^5 x 10^3 partners is spread over the whole GPU.  Rows past
@@ -22,6 +22,7 @@
 //                       valid, non-NaN prefix (the build side is sorted by (by..., on)); direction, exactness and tolerance pick
 //                       one sorted row, whose original row number is written with the validity word by ballot.
 // All three probe kernels find the build run through join_find_run, so they cannot disagree on key equality.
+#include "scan.cuh"
 #include "sort_keys.cuh"
 
 #include <algorithm>
@@ -29,8 +30,7 @@
 namespace bdf {
 
 constexpr int kMaxJoinKeys = 16;
-constexpr int kJoinItems = 8;
-constexpr int kJoinTile = kThreads * kJoinItems;   // rows per CTA of the count, scan and emit kernels
+constexpr int kJoinTile = kScanTile;              // rows per CTA of the count and emit kernels
 constexpr uint32_t kNoMatch = 0xffffffffu;         // match start of a probe row without partners (build rows are < 2^32 - 1)
 
 struct JoinKey {
@@ -85,9 +85,8 @@ __global__ void __launch_bounds__(kThreads)
 k_join_count(const __grid_constant__ JoinKeys keys, long long n_probe, const uint32_t* __restrict__ run_starts, long long n_runs, long long n_build,
              int outer, unsigned long long* __restrict__ counts, uint32_t* __restrict__ match_start, unsigned char* __restrict__ hit,
              unsigned long long* __restrict__ block_sums) {
-    __shared__ unsigned long long s_warp[kWarpsPerCta];
     unsigned long long total = 0;
-    for (int it = 0; it < kJoinItems; it++) {
+    for (int it = 0; it < kScanItems; it++) {
         const long long i = (long long)blockIdx.x * kJoinTile + it * kThreads + threadIdx.x;
         if (i >= n_probe) break;
         unsigned long long cnt = 0;
@@ -103,65 +102,8 @@ k_join_count(const __grid_constant__ JoinKeys keys, long long n_probe, const uin
         match_start[i] = start;
         total += cnt;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = total;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long t = 0;
-#pragma unroll
-        for (int w = 0; w < kWarpsPerCta; w++) t += s_warp[w];
-        block_sums[blockIdx.x] = t;
-    }
-}
-
-// Exclusive scan of the CTA totals in place (one CTA of 1024 threads, each owning a contiguous run); *total = the sum.
-__global__ void __launch_bounds__(1024) k_join_scan_blocks(unsigned long long* __restrict__ data, long long count, unsigned long long* __restrict__ total) {
-    __shared__ unsigned long long s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long per = (count + 1023) / 1024;
-    const long long begin = min(count, (long long)threadIdx.x * per), end = min(count, begin + per);
-    unsigned long long sum = 0;
-    for (long long i = begin; i < end; i++) sum += data[i];
-    unsigned long long x = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        unsigned long long w = s_warp[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-        s_warp[lane] = w;   // inclusive over warps
-    }
-    __syncthreads();
-    unsigned long long run = (warp ? s_warp[warp - 1] : 0ull) + x - sum;
-    for (long long i = begin; i < end; i++) { const unsigned long long v = data[i]; data[i] = run; run += v; }
-    if (threadIdx.x == 1023) *total = run;
-}
-
-// The counts of CTA b (rows [b * kJoinTile, ...), thread t owning kJoinItems consecutive rows) -> exclusive offsets.
-__global__ void __launch_bounds__(kThreads)
-k_join_scan_rows(unsigned long long* __restrict__ counts, long long n, const unsigned long long* __restrict__ block_offsets) {
-    __shared__ unsigned long long s_warp[kWarpsPerCta];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long base = (long long)blockIdx.x * kJoinTile + (long long)threadIdx.x * kJoinItems;
-    unsigned long long v[kJoinItems], sum = 0;
-#pragma unroll
-    for (int k = 0; k < kJoinItems; k++) { v[k] = base + k < n ? counts[base + k] : 0ull; sum += v[k]; }
-    unsigned long long x = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    unsigned long long run = block_offsets[blockIdx.x] + x - sum;
-#pragma unroll
-    for (int w = 0; w < kWarpsPerCta; w++) run += w < warp ? s_warp[w] : 0ull;
-#pragma unroll
-    for (int k = 0; k < kJoinItems; k++) {
-        if (base + k < n) counts[base + k] = run;
-        run += v[k];
-    }
+    total = cta_sum(total);
+    if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
 }
 
 // The last probe row i in [lo, hi] with offs[i] <= o (offs is non-decreasing; probe rows of an inner join may produce nothing).
@@ -189,7 +131,7 @@ k_join_emit(const unsigned long long* __restrict__ offs, long long n_probe, cons
     }
     __syncthreads();
     const long long lo = s_range[0], hi = s_range[1];
-    for (int it = 0; it < kJoinItems; it++) {
+    for (int it = 0; it < kScanItems; it++) {
         const unsigned long long o = o0 + (unsigned long long)(it * kThreads + threadIdx.x);
         bool pv = false, bv = false;
         uint32_t p = 0, b = 0;
@@ -331,8 +273,6 @@ k_join_asof(const __grid_constant__ JoinKeys by, const __grid_constant__ AsofOn 
 }
 
 // ---- launchers ------------------------------------------------------------------------------------------------------
-int join_tile_rows() { return kJoinTile; }
-
 static JoinKeys join_keys(int n_keys, const int* dtypes, const void* const* probe_tables, const int* probe_chunks, const void* const* build_keys,
                           const uint32_t* const* build_valid) {
     JoinKeys jk{};
@@ -352,15 +292,6 @@ cudaError_t launch_join_count(int n_keys, const int* dtypes, const void* const* 
     const JoinKeys jk = join_keys(n_keys, dtypes, probe_tables, probe_chunks, build_keys, build_valid);
     const long long blocks = (n_probe + kJoinTile - 1) / kJoinTile;
     k_join_count<<<(unsigned)blocks, kThreads, 0, s>>>(jk, n_probe, run_starts, n_runs, n_build, outer, counts, match_start, hit, block_sums);
-    return cudaGetLastError();
-}
-
-// counts: n_probe + 1 entries; afterwards counts[i] = the first output row of probe row i, counts[n_probe] = the total.
-cudaError_t launch_join_scan(unsigned long long* counts, long long n_probe, unsigned long long* block_sums, cudaStream_t s) {
-    if (n_probe <= 0) return cudaMemsetAsync(counts, 0, sizeof(unsigned long long), s);
-    const long long blocks = (n_probe + kJoinTile - 1) / kJoinTile;
-    k_join_scan_blocks<<<1, 1024, 0, s>>>(block_sums, blocks, counts + n_probe);
-    k_join_scan_rows<<<(unsigned)blocks, kThreads, 0, s>>>(counts, n_probe, block_sums);
     return cudaGetLastError();
 }
 

@@ -6,9 +6,9 @@
 // state: the newline positions are compacted (count / scan / scatter, as the CSV field index), and every record is then walked by
 // one thread.  Records of event and log data are short (tens to hundreds of bytes), so a warp walks 32 neighbouring lines and
 // their bytes come through L1 together.
-//   k_json_nl_count / k_json_nl_index   the '\n' positions: per-CTA counts, their scan (k_json_scan_one), the positions
-//   k_json_lex          per line: blank, a record, or malformed (the first bad line by atomicMin); the members of its object
-//   k_json_scan_*       exclusive 64-bit scans of the per-line counts: the first member of every line, the record of every line
+//   k_json_nl_count / k_json_nl_index   the '\n' positions: per-CTA counts, their scan (k_scan_one of k_scan.cu), the positions
+//   k_json_lex          per line: blank, a record, or malformed (the first bad line by atomicMin); the members of its object; the
+//                       exclusive 64-bit scans of these per-line counts (launch_scan) give the first member and the record of every line
 //   k_json_members      per line again: one 32-byte entry per member (record, key bytes, value bytes, value class)
 //   k_json_keys         the distinct keys: an open-addressing table on (hash, length) with the first member of each (atomicMin)
 //   k_json_resolve      every member's key checked byte for byte against its table entry (a hash collision is reported, never
@@ -21,6 +21,7 @@
 //                       counts) the offsets of every chunk from 0 and the elements converted into the child column
 #include "common.cuh"
 #include "json_parse.cuh"
+#include "scan.cuh"
 
 #include <algorithm>
 
@@ -28,8 +29,6 @@ namespace bdf {
 
 constexpr int kJsonBytes = 16;                     // bytes per thread of the newline pass
 constexpr int kJsonTile = kThreads * kJsonBytes;   // bytes per CTA
-constexpr int kJsonScanItems = 16;                 // items per thread of the scans
-constexpr int kJsonScanTile = kThreads * kJsonScanItems;
 constexpr int kJsonRows = kThreads;                // rows per CTA of the parser
 
 struct JsonMember {
@@ -89,92 +88,21 @@ __device__ __forceinline__ uint32_t nl_mask(const uint8_t* __restrict__ text, lo
     return m;
 }
 
-// CTA-wide exclusive scan of one value per thread; *total = the CTA's sum.
-__device__ __forceinline__ unsigned long long cta_scan(unsigned long long x, unsigned long long* total) {
-    __shared__ unsigned long long s_warp[kWarpsPerCta];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned long long inc = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long y = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += y;
-    }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    unsigned long long before = 0, all = 0;
-#pragma unroll
-    for (int w = 0; w < kWarpsPerCta; w++) {
-        if (w < warp) before += s_warp[w];
-        all += s_warp[w];
-    }
-    __syncthreads();
-    *total = all;
-    return before + inc - x;
-}
-
 __global__ void __launch_bounds__(kThreads) k_json_nl_count(const uint8_t* __restrict__ text, long long n, unsigned long long* __restrict__ counts) {
-    unsigned long long total;
-    cta_scan((unsigned long long)__popc(nl_mask(text, n, (long long)blockIdx.x * kThreads + threadIdx.x)), &total);
-    if (threadIdx.x == 0) counts[blockIdx.x] = total;
+    const int total = cta_sum(__popc(nl_mask(text, n, (long long)blockIdx.x * kThreads + threadIdx.x)));
+    if (threadIdx.x == 0) counts[blockIdx.x] = (unsigned long long)total;
 }
 
 __global__ void __launch_bounds__(kThreads)
 k_json_nl_index(const uint8_t* __restrict__ text, long long n, const unsigned long long* __restrict__ offsets, unsigned long long* __restrict__ nl) {
     const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
     uint32_t m = nl_mask(text, n, g);
-    unsigned long long total;
-    unsigned long long off = offsets[blockIdx.x] + cta_scan((unsigned long long)__popc(m), &total);
+    unsigned long long off = offsets[blockIdx.x] + (unsigned long long)cta_exclusive_sum(__popc(m));
     while (m) {
         const int k = __ffs(m) - 1;
         m &= m - 1;
         nl[off++] = (unsigned long long)(g * kJsonBytes + k);
     }
-}
-
-// One CTA of 1024 threads, each owning a contiguous run: exclusive scan in place; *total = the sum.
-__global__ void __launch_bounds__(1024) k_json_scan_one(unsigned long long* __restrict__ data, long long count, unsigned long long* __restrict__ total) {
-    __shared__ unsigned long long s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long per = (count + 1023) / 1024;
-    const long long begin = min(count, (long long)threadIdx.x * per), end = min(count, begin + per);
-    unsigned long long sum = 0;
-    for (long long i = begin; i < end; i++) sum += data[i];
-    unsigned long long x = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    unsigned long long run = x - sum;
-    for (int w = 0; w < warp; w++) run += s_warp[w];
-    for (long long i = begin; i < end; i++) { const unsigned long long v = data[i]; data[i] = run; run += v; }
-    if (threadIdx.x == 1023) *total = run;
-}
-
-// The scan of n values: the sums of tiles of kJsonScanTile, their scan, then every tile in place from its offset.
-__global__ void __launch_bounds__(kThreads) k_json_scan_tiles(const unsigned long long* __restrict__ data, long long n, unsigned long long* __restrict__ sums) {
-    const long long base = (long long)blockIdx.x * kJsonScanTile + (long long)threadIdx.x * kJsonScanItems;
-    unsigned long long s = 0;
-#pragma unroll
-    for (int k = 0; k < kJsonScanItems; k++)
-        if (base + k < n) s += data[base + k];
-    unsigned long long total;
-    cta_scan(s, &total);
-    if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(kThreads) k_json_scan_apply(unsigned long long* __restrict__ data, long long n, const unsigned long long* __restrict__ sums) {
-    const long long base = (long long)blockIdx.x * kJsonScanTile + (long long)threadIdx.x * kJsonScanItems;
-    unsigned long long v[kJsonScanItems], s = 0;
-#pragma unroll
-    for (int k = 0; k < kJsonScanItems; k++) {
-        v[k] = base + k < n ? data[base + k] : 0;
-        s += v[k];
-    }
-    unsigned long long total;
-    unsigned long long run = sums[blockIdx.x] + cta_scan(s, &total);
-#pragma unroll
-    for (int k = 0; k < kJsonScanItems; k++)
-        if (base + k < n) { data[base + k] = run; run += v[k]; }
 }
 
 struct CountMembers {
@@ -447,24 +375,12 @@ cudaError_t launch_json_nl_count(const uint8_t* text, long long n, unsigned long
     const long long tiles = std::max<long long>((n + kJsonTile - 1) / kJsonTile, 1);
     if (tiles > 0x7fffffffLL) return cudaErrorInvalidValue;
     k_json_nl_count<<<(unsigned)tiles, kThreads, 0, s>>>(text, n, counts);
-    k_json_scan_one<<<1, 1024, 0, s>>>(counts, tiles, counts + tiles);
-    return cudaGetLastError();
+    return launch_scan_one(counts, tiles, counts + tiles, s);   // its error check covers the launch above
 }
 
 cudaError_t launch_json_nl_index(const uint8_t* text, long long n, const unsigned long long* offsets, unsigned long long* nl, cudaStream_t s) {
     const long long tiles = std::max<long long>((n + kJsonTile - 1) / kJsonTile, 1);
     k_json_nl_index<<<(unsigned)tiles, kThreads, 0, s>>>(text, n, offsets, nl);
-    return cudaGetLastError();
-}
-
-// data: n + 1 entries; the exclusive scan in place, the total in data[n].  sums: json_scan_sums(n) entries.
-long long json_scan_sums(long long n) { return std::max<long long>((n + kJsonScanTile - 1) / kJsonScanTile, 1) + 1; }
-cudaError_t launch_json_scan(unsigned long long* data, long long n, unsigned long long* sums, cudaStream_t s) {
-    const long long tiles = json_scan_sums(n) - 1;
-    if (tiles > 0x7fffffffLL) return cudaErrorInvalidValue;
-    k_json_scan_tiles<<<(unsigned)tiles, kThreads, 0, s>>>(data, n, sums);
-    k_json_scan_one<<<1, 1024, 0, s>>>(sums, tiles, data + n);
-    k_json_scan_apply<<<(unsigned)tiles, kThreads, 0, s>>>(data, n, sums);
     return cudaGetLastError();
 }
 

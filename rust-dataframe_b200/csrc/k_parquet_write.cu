@@ -47,7 +47,7 @@ __global__ void k_pqw_dict_runs(const uint32_t* __restrict__ run_rg, const uint3
     }
 }
 
-// head: bit i set when sorted row i starts a run; prefix[w]: the runs that start before row 32w (k_window_count + the join scan), so
+// head: bit i set when sorted row i starts a run; prefix[w]: the runs that start before row 32w (launch_scan_popcount), so
 // the run of a row costs one word and one popcount.
 __global__ void k_pqw_dict_ids(const uint32_t* __restrict__ head, const unsigned long long* __restrict__ prefix, const uint32_t* __restrict__ perm,
                                const uint32_t* __restrict__ run_rg, const unsigned int* __restrict__ first, long long n, uint32_t* __restrict__ ids) {

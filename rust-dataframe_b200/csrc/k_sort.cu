@@ -11,7 +11,7 @@
 // null flag moves the nulls behind the valid rows without disturbing either group.
 //
 // Pass structure (per 8-bit digit): k_radix_hist (per-CTA digit counts over the CTA's contiguous range of tiles) ->
-// k_radix_scan (one CTA, exclusive scan in digit-major order) -> k_radix_scatter (per tile: warp-level peer masks from per-bit ballots -> ranks,
+// k_scan_one (k_scan.cu: one CTA, exclusive scan in digit-major order) -> k_radix_scatter (per tile: warp-level peer masks from per-bit ballots -> ranks,
 // reorder through shared memory, write each digit's run contiguously).  A digit on which every key agrees is skipped:
 // k_sort_keys also folds the OR and the AND of the keys it builds.
 // HBM traffic per executed pass: 8 (hist) + 12 + 12 B/row with 64-bit keys, 4 + 8 + 8 with 32-bit keys (criteria of at most
@@ -93,32 +93,6 @@ k_radix_hist(const K* __restrict__ keys, int64_t n, int shift, int64_t tiles_per
     for (int64_t i = begin + threadIdx.x; i < end; i += kThreads) atomicAdd(&s_hist[(keys[i] >> shift) & 0xff], 1u);
     __syncthreads();
     block_hist[(int64_t)threadIdx.x * gridDim.x + blockIdx.x] = s_hist[threadIdx.x];
-}
-
-// Exclusive scan of `count` entries in place, one CTA of 1024 threads: every thread owns a contiguous run (its loads are
-// independent of each other), one block scan of the 1024 run totals, then the runs are rewritten.  (A first version
-// walked the array 1024 entries at a time with a carried total: one dependent iteration per 1024 entries.)
-__global__ void __launch_bounds__(1024) k_radix_scan(unsigned int* __restrict__ data, int64_t count) {
-    __shared__ unsigned int s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t per = (count + 1023) / 1024;
-    const int64_t begin = min(count, (int64_t)threadIdx.x * per), end = min(count, begin + per);
-    unsigned int sum = 0;
-    for (int64_t i = begin; i < end; i++) sum += data[i];
-    unsigned int x = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        unsigned int w = s_warp[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-        s_warp[lane] = w;   // inclusive over warps
-    }
-    __syncthreads();
-    unsigned int run = (warp ? s_warp[warp - 1] : 0u) + x - sum;
-    for (int64_t i = begin; i < end; i++) { const unsigned int v = data[i]; data[i] = run; run += v; }
 }
 
 // Lanes of the warp holding the same 9-bit value (digit, or 256 for "not a key"): one ballot per bit instead of MATCH.ANY.  A
@@ -358,7 +332,8 @@ static cudaError_t radix_pass(const K* keys_in, const uint32_t* idx_in, int64_t 
     static const cudaError_t attr = cudaFuncSetAttribute(k_radix_scatter<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem<K>());
     if (attr != cudaSuccess) return attr;
     k_radix_hist<K><<<g, kThreads, 0, s>>>(keys_in, n, shift, per, block_hist);
-    k_radix_scan<<<1, 1024, 0, s>>>(block_hist, (int64_t)256 * g);
+    const cudaError_t e = launch_scan_one<unsigned int>(block_hist, (long long)256 * g, nullptr, s);
+    if (e != cudaSuccess) return e;
     k_radix_scatter<K><<<g, kSortThreads, scatter_smem<K>(), s>>>(keys_in, idx_in, n, shift, per, block_hist, keys_out, idx_out);
     return cudaGetLastError();
 }

@@ -4,10 +4,9 @@
 // The host (runtime.cu window_dev) sorts the rows by (partition keys ascending, order keys with their directions) with the stable
 // radix lexsort, gathers the keys, marks the first row of every partition (P heads) and of every peer group (Q heads, a superset
 // of P) with k_group_heads, and compacts the head positions with filter(iota, heads).  The kernels work in that sorted space,
-// positions i = 0..n-1:
-//   k_window_count   popcount of every head word and the total of every CTA, for the 64-bit scan of k_join.cu: afterwards
-//                    prefix[w] is the number of runs starting before position 32w, so the run of position i -- and through the
-//                    compacted starts its first and last position -- costs O(1) (no binary search per row).
+// positions i = 0..n-1.  The host scans the popcounts of the head words first (launch_scan_popcount, k_scan.cu): prefix[w] is the
+// number of runs starting before position 32w, so the run of position i -- and through the compacted starts its first and last
+// position -- costs O(1) (no binary search per row).
 //   k_window_rank    per position: partition and peer bounds -> row_number, rank, dense_rank, percent_rank, cume_dist, written
 //                    to out[perm[i]] (the caller's row order), and the gather indices that bring a sorted-order column back to
 //                    row order: i itself (the inverse permutation), the last peer of i, the last row of i's partition.
@@ -71,26 +70,6 @@ __device__ __forceinline__ WinPos win_pos(const WinRuns& r, long long i, bool ne
         o.dense = q - run_of(r.q, o.ps) + 1;   // a partition start is always a peer start
     }
     return o;
-}
-
-// counts[w] = popcount(words[w]); block_sums[b] = the total of CTA b (kJoinTile words: 256 threads x 8) -- the input of launch_join_scan.
-__global__ void __launch_bounds__(kThreads)
-k_window_count(const uint32_t* __restrict__ words, long long n_words, unsigned long long* __restrict__ counts, unsigned long long* __restrict__ block_sums) {
-    __shared__ unsigned long long s_warp[kWarpsPerCta];
-    const long long base = (long long)blockIdx.x * kWinTile + (long long)threadIdx.x * kWinItems;
-    unsigned long long sum = 0;
-#pragma unroll
-    for (int k = 0; k < kWinItems; k++)
-        if (base + k < n_words) { const unsigned long long c = __popc(words[base + k]); counts[base + k] = c; sum += c; }
-    sum = __reduce_add_sync(0xffffffffu, (unsigned)sum);
-    if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = sum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long t = 0;
-#pragma unroll
-        for (int w = 0; w < kWarpsPerCta; w++) t += s_warp[w];
-        block_sums[blockIdx.x] = t;
-    }
 }
 
 // ---- ranking functions and gather indices -------------------------------------------------------------------------------
@@ -330,21 +309,13 @@ k_window_carry(const WinSeg<T>* __restrict__ tiles, long long n_tiles, WinAcc<T>
 }
 
 // ---- launchers ----------------------------------------------------------------------------------------------------------
-// The three head arrays of one head bitmap (words, prefix from launch_join_scan, compacted starts) and the number of runs.
+// The three head arrays of one head bitmap (words, prefix from launch_scan_popcount, compacted starts) and the number of runs.
 static WinRuns make_runs(const void* const* p, long long n_p, const void* const* q, long long n_q, long long n) {
     WinRuns r{};
     if (p) r.p = WinHeads{(const uint32_t*)p[0], (const unsigned long long*)p[1], (const uint32_t*)p[2], n_p};
     if (q) r.q = WinHeads{(const uint32_t*)q[0], (const unsigned long long*)q[1], (const uint32_t*)q[2], n_q};
     r.n = n;
     return r;
-}
-
-int window_count_tile() { return kWinTile; }
-
-cudaError_t launch_window_count(const uint32_t* words, long long n_words, unsigned long long* counts, unsigned long long* block_sums, cudaStream_t s) {
-    if (n_words <= 0) return cudaSuccess;
-    k_window_count<<<(unsigned)((n_words + kWinTile - 1) / kWinTile), kThreads, 0, s>>>(words, n_words, counts, block_sums);
-    return cudaGetLastError();
 }
 
 // p / q: {head words, prefix, starts} or null (one partition / peers = partition); outs: the 8 WinRankOut pointers in order, each

@@ -2970,13 +2970,13 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
     // the probe side is read in place, through the chunk tables of its key columns
     JoinProbe jp;
     TRY(join_probe(c, n_keys, probe, runs, &jp));
-    const int64_t blocks = (np + join_tile_rows() - 1) / join_tile_rows();
+    const int64_t blocks = scan_tile_sums(np);
     Scratch<unsigned long long> counts, block_sums;
     Scratch<uint32_t> mstart;
     Scratch<unsigned char> hit;
     cudaError_t e = counts.alloc(c, (size_t)(np + 1) * sizeof(unsigned long long));
     if (e == cudaSuccess) e = mstart.alloc(c, (size_t)std::max<int64_t>(np, 1) * sizeof(uint32_t));
-    if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)blocks * sizeof(unsigned long long));
     if (e == cudaSuccess && full) e = hit.alloc(c, (size_t)std::max<int64_t>(n_runs, 1));
     if (e == cudaSuccess && full) e = cudaMemsetAsync(hit, 0, (size_t)std::max<int64_t>(n_runs, 1), c->s_compute);
     if (e != cudaSuccess) return fail_cuda(e, "join scratch allocation");
@@ -2987,9 +2987,9 @@ static int join_dev(bdf_ctx* c, int how, int n_keys, const bdf_col* const* lk, c
                               outer ? 1 : 0, counts, mstart, hit, block_sums, c->s_compute);
     }
     if (e == cudaSuccess) {
-        LaunchTimer t(c, BDF_K_JOIN, BDF_U64, np, np * 16 + blocks * 16);
-        c->launches++;   // two kernels: the CTA totals, then the rows
-        e = launch_join_scan(counts, np, block_sums, c->s_compute);
+        LaunchTimer t(c, BDF_K_JOIN, BDF_U64, np, np > 0 ? np * 16 + blocks * 16 : 0);   // no probe rows: a memset of the total
+        c->launches += kScanSumsLaunches - 1;   // the timer counts one
+        e = launch_scan_sums(counts, np, block_sums, c->s_compute);
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(&total, counts + np, sizeof(total), cudaMemcpyDeviceToHost, c->s_compute);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->s_compute);   // the output length sizes the result
@@ -3112,15 +3112,13 @@ struct WinHeadsHost {
 
 static int window_runs(bdf_ctx* c, const bdf_col* iota, int64_t n, WinHeadsHost* h) {
     const int64_t words = (n + 31) / 32;
-    const int64_t blocks = (words + window_count_tile() - 1) / window_count_tile();
     Scratch<unsigned long long> block_sums;
     cudaError_t e = h->prefix.alloc(c, (size_t)(words + 1) * sizeof(unsigned long long));
-    if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)scan_tile_sums(words) * sizeof(unsigned long long));
     if (e == cudaSuccess) {
         LaunchTimer t(c, BDF_K_WINDOW, BDF_U64, n, words * (4 + 8 + 16));   // popcounts written, then read and written by the scan
-        c->launches += 2;                                                       // the scan's two kernels
-        e = launch_window_count((const uint32_t*)h->bits->chunks[0].values, words, h->prefix, block_sums, c->s_compute);
-        if (e == cudaSuccess) e = launch_join_scan(h->prefix, words, block_sums, c->s_compute);
+        c->launches += kScanPopcountLaunches - 1;                              // the timer counts one
+        e = launch_scan_popcount((const uint32_t*)h->bits->chunks[0].values, words, h->prefix, block_sums, c->s_compute);
     }
     if (e != cudaSuccess) return fail_cuda(e, "window run prefix");
     TRY(filter_dev(c, iota, h->bits.get(), h->starts.out()));
@@ -3216,16 +3214,14 @@ static int window_frame_call(bdf_ctx* c, const bdf_window_call& k, const void* c
         Scratch<unsigned long long> vprefix, block_sums;
         const bool ranks = k.ignore_nulls && nullable;   // IGNORE NULLS over a column with nulls: the popcount prefix of its validity
         if (ranks) {
-            const int64_t blocks = (words + window_count_tile() - 1) / window_count_tile();
             e = vwords.alloc(c, (size_t)words * sizeof(uint32_t));
             if (e == cudaSuccess) e = vprefix.alloc(c, (size_t)(words + 1) * sizeof(unsigned long long));
-            if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long));
+            if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)scan_tile_sums(words) * sizeof(unsigned long long));
             if (e == cudaSuccess) {
                 LaunchTimer t(c, BDF_K_WINDOW, BDF_U32, n, bitmap_bytes(n) * 2 + words * (8 + 16));   // validity words, popcounts, scan
-                c->launches += 2;                                                                      // the scan's two kernels
+                c->launches += kScanPopcountLaunches;                                                  // the timer counts the first
                 e = launch_window_valid_words(table, n_chunks, n, vwords, c->s_compute);
-                if (e == cudaSuccess) e = launch_window_count(vwords, words, vprefix, block_sums, c->s_compute);
-                if (e == cudaSuccess) e = launch_join_scan(vprefix, words, block_sums, c->s_compute);
+                if (e == cudaSuccess) e = launch_scan_popcount(vwords, words, vprefix, block_sums, c->s_compute);
             }
         }
         if (e == cudaSuccess) {
@@ -3960,13 +3956,12 @@ static int csv_write(bdf_ctx* c, const char* path, int n_cols, const char* const
     Scratch<long long> d_starts;
     Scratch<char> text[2];
     Scratch<unsigned long long> lens, sums;
-    const int64_t max_tiles = (block_rows + csvw_tile() - 1) / csvw_tile();
     cudaError_t e = d_desc.alloc(c, descs.size() * sizeof(CsvwDesc));
     if (e == cudaSuccess) e = d_starts.alloc(c, starts.size() * sizeof(long long));
     if (e == cudaSuccess) e = text[0].alloc(c, text_cap);
     if (e == cudaSuccess) e = text[1].alloc(c, text_cap);
     if (e == cudaSuccess) e = lens.alloc(c, (size_t)(block_rows + 1) * sizeof(unsigned long long));
-    if (e == cudaSuccess) e = sums.alloc(c, (size_t)max_tiles * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = sums.alloc(c, (size_t)scan_tile_sums(block_rows) * sizeof(unsigned long long));
     // pageable sources: the copies have read them when they return
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_desc, descs.data(), descs.size() * sizeof(CsvwDesc), cudaMemcpyHostToDevice, c->s_compute);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_starts, starts.data(), starts.size() * sizeof(long long), cudaMemcpyHostToDevice, c->s_compute);
@@ -3988,9 +3983,9 @@ static int csv_write(bdf_ctx* c, const char* path, int n_cols, const char* const
         cudaError_t e2 = k >= 2 ? cudaStreamWaitEvent(c->s_compute, ev_d2h[b], 0) : cudaSuccess;
         if (e2 == cudaSuccess) {
             LaunchTimer t(c, BDF_K_CSV_WRITE, BDF_U64, n, n * (8 + 16));   // lengths written, then read and written by the scan
-            c->launches += 2;                                                // the scan's two kernels
+            c->launches += kScanSumsLaunches;                                // the timer counts the measure
             e2 = launch_csvw_measure(d_desc, d_starts, n_cols, (int)n_chunks, row0, n, lens, sums, c->s_compute);
-            if (e2 == cudaSuccess) e2 = launch_join_scan(lens, n, sums, c->s_compute);
+            if (e2 == cudaSuccess) e2 = launch_scan_sums(lens, n, sums, c->s_compute);
         }
         if (e2 == cudaSuccess) e2 = cudaMemcpyAsync(tot.p + b, lens + n, sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->s_compute);
         if (e2 == cudaSuccess) {
@@ -4176,21 +4171,19 @@ static int pqw_dictionary(bdf_ctx* c, const bdf_col* col, const bdf_col* rg_col,
     {
         TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, all_ids.out()));
         const int64_t words = (n + 31) / 32;
-        const int64_t blocks = (words + window_count_tile() - 1) / window_count_tile();
         Scratch<unsigned int> cf;
         Scratch<unsigned long long> prefix, block_sums;
         cudaError_t e = cf.alloc(c, (size_t)2 * n_rg * sizeof(unsigned int));
         if (e == cudaSuccess) e = prefix.alloc(c, (size_t)(words + 1) * sizeof(unsigned long long));
-        if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)std::max<int64_t>(blocks, 1) * sizeof(unsigned long long));
+        if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)scan_tile_sums(words) * sizeof(unsigned long long));
         if (e == cudaSuccess) e = cudaMemsetAsync(cf, 0, (size_t)n_rg * sizeof(unsigned int), c->s_compute);
         if (e == cudaSuccess) e = cudaMemsetAsync(cf + n_rg, 0xff, (size_t)n_rg * sizeof(unsigned int), c->s_compute);
         const int64_t n_runs = r.n_runs;
         const uint32_t* head = (const uint32_t*)r.head->chunks[0].values;
         if (e == cudaSuccess) {
             LaunchTimer t(c, BDF_K_PARQUET_WRITE, BDF_U32, n, words * (4 + 8 + 16) + n * 16 + n_runs * 8);   // head prefix; perm, ids; runs
-            c->launches += 4;                                                                                // count, scan (2), runs, ids
-            e = launch_window_count(head, words, prefix, block_sums, c->s_compute);
-            if (e == cudaSuccess) e = launch_join_scan(prefix, words, block_sums, c->s_compute);
+            c->launches += kScanPopcountLaunches + 1;                                                        // and runs, ids
+            e = launch_scan_popcount(head, words, prefix, block_sums, c->s_compute);
             if (e == cudaSuccess)
                 e = launch_pqw_dict((const uint32_t*)r.distinct[0]->chunks[0].values, r.distinct[1]->chunks[0].validity, n_runs, head, prefix,
                                     (const uint32_t*)r.perm->chunks[0].values, n, cf, cf + n_rg, (uint32_t*)all_ids->chunks[0].values, c->sm_count,
@@ -5659,7 +5652,7 @@ static int list_gather(bdf_ctx* c, const bdf_list* l, const bdf_col* rows, bool 
     const size_t lt_bytes = lt.size() * sizeof(ListChunkDesc);
     CK(tables.alloc(c, lt_bytes + n_out * sizeof(uint32_t*)));
     CK(sizes.alloc(c, (size_t)(n + 1) * 8));
-    CK(scan_sums.alloc(c, (size_t)json_scan_sums(n) * 8));
+    CK(scan_sums.alloc(c, (size_t)scan_tile_sums(n) * 8));
     CK(nulls.alloc(c, n_out * 8));
     CK(first.alloc(c, (size_t)std::max<int64_t>(n, 1) * 4));
     std::vector<char> host(lt_bytes + n_out * sizeof(uint32_t*));
@@ -5673,10 +5666,10 @@ static int list_gather(bdf_ctx* c, const bdf_list* l, const bdf_col* rows, bool 
     cudaError_t e;
     {
         LaunchTimer t(c, BDF_K_LIST, BDF_U64, n, n * (4 + 8 + 8 + 4) + n / 8);   // index, two offsets, size and first element
-        c->launches += 3;   // the scan's three kernels
+        c->launches += kScanLaunches;   // the timer counts the sizes
         e = launch_list_take_sizes(it, ni, n, tables.get(), (int)std::max<int64_t>(n_lc, 1), l->total_len, local ? 1 : 0,
                                    (uint32_t* const*)(tables.get() + lt_bytes), sizes, first, nulls, c->d_flag, c->s_compute);
-        if (e == cudaSuccess) e = launch_json_scan(sizes, n, scan_sums, c->s_compute);
+        if (e == cudaSuccess) e = launch_scan(sizes, n, scan_sums, c->s_compute);
     }
     // the host needs the element count of every output chunk (scan entries at the chunk bounds), the null counts and the flag
     std::vector<unsigned long long> bounds(n_out + 1), h_nulls(n_out);
@@ -5949,7 +5942,7 @@ static int json_open(bdf_ctx* c, const char* path, const bdf_json_options* o, in
     const int64_t lines = (int64_t)n_nl + 1;
     e = members.alloc(c, (size_t)(lines + 1) * 8);
     if (e == cudaSuccess) e = is_rec.alloc(c, (size_t)(lines + 1) * 8);
-    if (e == cudaSuccess) e = sums.alloc(c, (size_t)json_scan_sums(lines) * 8);
+    if (e == cudaSuccess) e = sums.alloc(c, (size_t)scan_tile_sums(lines) * 8);
     if (e == cudaSuccess) {
         LaunchTimer t(c, BDF_K_JSON, BDF_U64, lines, f->n + lines * 16);
         e = launch_json_lex(f->d_text, f->n, nl, (long long)n_nl, members, is_rec, small, c->sm_count, c->s_compute);
@@ -5961,9 +5954,9 @@ static int json_open(bdf_ctx* c, const char* path, const bdf_json_options* o, in
     if (bad != ~0ull) return json_bad_line(c, f.get(), nl, (int64_t)n_nl, (int64_t)bad);
     {
         LaunchTimer t(c, BDF_K_JSON, BDF_U64, lines, lines * 32);
-        c->launches += 5;   // two scans of three kernels each
-        e = launch_json_scan(members, lines, sums, c->s_compute);
-        if (e == cudaSuccess) e = launch_json_scan(is_rec, lines, sums, c->s_compute);
+        c->launches += 2 * kScanLaunches - 1;   // two scans; the timer counts one
+        e = launch_scan(members, lines, sums, c->s_compute);
+        if (e == cudaSuccess) e = launch_scan(is_rec, lines, sums, c->s_compute);
     }
     unsigned long long tot[2] = {0, 0};
     if (e == cudaSuccess) e = cudaMemcpyAsync(&tot[0], members + lines, 8, cudaMemcpyDeviceToHost, c->s_compute);
@@ -6211,7 +6204,7 @@ static int json_read_list(bdf_ctx* c, const bdf_json* f, int col, bdf_list** out
     Scratch<uint32_t> vwords;
     Scratch<void> descs, slow;
     cudaError_t e = counts.alloc(c, (size_t)(n_rows + 1) * 8);
-    if (e == cudaSuccess) e = sums.alloc(c, (size_t)json_scan_sums(n_rows) * 8);
+    if (e == cudaSuccess) e = sums.alloc(c, (size_t)scan_tile_sums(n_rows) * 8);
     if (e == cudaSuccess) e = bounds.alloc(c, (size_t)(n_chunks + 1) * 8);
     if (e == cudaSuccess) e = nulls.alloc(c, (size_t)n_chunks * 16);
     if (e == cudaSuccess) e = cudaMemsetAsync(nulls, 0, (size_t)n_chunks * 16, c->s_compute);
@@ -6219,9 +6212,9 @@ static int json_read_list(bdf_ctx* c, const bdf_json* f, int col, bdf_list** out
     if (e != cudaSuccess) return fail_cuda(e, "JSON list scratch allocation");
     {
         LaunchTimer t(c, BDF_K_JSON, ldt, n_rows, n_rows * 16);
-        c->launches += 4;   // count, the scan's three kernels, bounds
+        c->launches += kScanLaunches + 1;   // the timer counts the count; and bounds
         e = launch_json_list_count(f->d_text, f->d_members, f->d_slots, n_file_cols, col, n_rows, batch, counts, vwords, nulls, c->s_compute);
-        if (e == cudaSuccess) e = launch_json_scan(counts, n_rows, sums, c->s_compute);
+        if (e == cudaSuccess) e = launch_scan(counts, n_rows, sums, c->s_compute);
         if (e == cudaSuccess) e = launch_json_bounds(counts, n_rows, batch, n_chunks, bounds, c->s_compute);
     }
     std::vector<unsigned long long> hb((size_t)n_chunks + 1), hn((size_t)n_chunks * 2);

@@ -7,7 +7,7 @@ switch points instead of leaving them to random sizes:
   * radix sort (k_sort.cu): SORT_TILE-key tiles, and the first lengths where a CTA of the capped grid (SORT_CTAS_PER_SM x SMs)
     walks two tiles and carries its digit bases; 32- and 64-bit keys; key sets built for the skipped-digit rule, whose pass
     count is read back from the sort's launch record;
-  * the one-CTA scans of 1024 threads (k_join_scan_blocks, k_window_carry): 1023, 1024, 1025 and 2049 totals;
+  * the one-CTA scans of 1024 threads (k_scan_one, k_window_carry): 1023, 1024, 1025 and 2049 totals;
   * the group fold (k_group.cu): each lane count, groups of LANE_ROWS x LANES (+1) rows and of one and two BIG_GROUP segments (+1),
     extremes planted on segment and group ends, an all-null long group, a cancelling float column held to the stated sum bar;
   * list find (k_list.cu): each lane count, lists on the long-path threshold and on LONG_LIST segment ends, first matches
@@ -40,13 +40,13 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(os.path.dirname(HERE), "rust-dataframe_b200", "csrc")
 
 # ---------------------------------------------------------------------------------------------------------
-# the constants; test_constants_match_csrc re-reads every one of them from the sources
+# the constants; test_switch_points_match_csrc re-reads every one of them from the sources
 
 THREADS = 256                  # common.cuh kThreads
 SORT_TILE = 512 * 8            # k_sort.cu kSortTile = kSortThreads * kSortItems: keys per scatter tile
 SORT_CTAS_PER_SM = 4           # k_sort.cu sort_pass_ctas: the grid of a pass is at most 4 x SMs CTAs
-SCAN_THREADS = 1024            # k_join_scan_blocks / k_window_carry: one CTA, each thread owns ceil(count / 1024) totals
-JOIN_TILE = THREADS * 8        # k_join.cu kJoinTile: probe rows per CTA total
+SCAN_THREADS = 1024            # k_scan_one / k_window_carry: one CTA, each thread owns ceil(count / 1024) totals
+JOIN_TILE = THREADS * 8        # k_join.cu kJoinTile = scan.cuh kScanTile: probe rows per CTA total
 WIN_TILE = THREADS * 8         # k_window.cu kWinTile: rows per scan tile
 LANE_RULE = (64, 4)            # k_group.cu / k_list.cu: lanes = avg > 64 ? 32 : avg > 4 ? 8 : 1
 LANE_ROWS = 512                # k_group.cu kLaneRows: a 1- or 8-lane group longer than LANE_ROWS x LANES goes to k_group_medium
@@ -66,9 +66,10 @@ def _read(name):
         return f.read()
 
 
-def test_constants_match_csrc():
+def test_switch_points_match_csrc():
     """Every switch point above, read back from the kernel sources (the SM count comes from the device at run time)."""
     common, srt, runtime = _read("common.cuh"), _read("k_sort.cu"), _read("runtime.cu")
+    scan_h, scan, csvw = _read("scan.cuh"), _read("k_scan.cu"), _read("k_csv_write.cu")
     join, win, grp, lst, dist = _read("k_join.cu"), _read("k_window.cu"), _read("k_group.cu"), _read("k_list.cu"), _read("k_dist.cu")
 
     def num(src, pat):
@@ -91,12 +92,14 @@ def test_constants_match_csrc():
     assert re.search(r"pass_bytes \+= \(int64_t\)\(3 \* kb \+ 8\) \* n;", runtime)
     assert re.search(r"rec\.bytes = 8 \* n \+ pass_bytes \+ 4 \* n;", runtime)
     # the 1024-thread scans
-    for src, pat in ((srt, r"k_radix_scan\(unsigned int\* __restrict__ data, int64_t count\)"),
-                     (join, r"k_join_scan_blocks<<<1, 1024, 0, s>>>"), (win, r"constexpr int kWinCarryThreads = (\d+);")):
+    for src, pat in ((srt, r"launch_scan_one<unsigned int>\(block_hist, "), (scan, r"__launch_bounds__\(1024\) k_scan_one\("),
+                     (scan, r"k_scan_one<T><<<1, 1024, 0, s>>>"), (scan, r"k_scan_one<unsigned long long><<<1, 1024, 0, s>>>\(sums, tiles, data \+ n\)"),
+                     (win, r"constexpr int kWinCarryThreads = (\d+);")):
         assert re.search(pat, src), pat
     assert num(win, r"constexpr int kWinCarryThreads = (\d+);") == SCAN_THREADS
-    assert re.search(r"per = \(count \+ 1023\) / 1024;", join) and re.search(r"per = \(n_tiles \+ kWinCarryThreads - 1\) / kWinCarryThreads;", win)
-    assert re.search(r"constexpr int kJoinTile = kThreads \* kJoinItems;", join) and THREADS * num(join, r"constexpr int kJoinItems = (\d+);") == JOIN_TILE
+    assert re.search(r"per = \(count \+ 1023\) / 1024;", scan) and re.search(r"per = \(n_tiles \+ kWinCarryThreads - 1\) / kWinCarryThreads;", win)
+    assert re.search(r"constexpr int kScanTile = kThreads \* kScanItems;", scan_h) and THREADS * num(scan_h, r"constexpr int kScanItems = (\d+);") == JOIN_TILE
+    assert re.search(r"constexpr int kJoinTile = kScanTile;", join) and re.search(r"constexpr int kCsvwTile = kScanTile;", csvw)
     assert re.search(r"constexpr int kWinTile = kThreads \* kWinItems;", win) and THREADS * num(win, r"constexpr int kWinItems = (\d+);") == WIN_TILE
     # group fold and list find: the lane rule in both, the thresholds of the second paths
     for src in (grp, lst):
@@ -349,7 +352,7 @@ SCAN_COUNTS = [SCAN_THREADS - 1, SCAN_THREADS, SCAN_THREADS + 1, 2 * SCAN_THREAD
 @gpu
 @pytest.mark.parametrize("count", SCAN_COUNTS)
 def test_join_scan_block_counts(rdf, ctx, count):
-    """count CTA totals in k_join_scan_blocks: probe rows (the left side of inner and left joins) filling count - 1 tiles and part
+    """count CTA totals in k_scan_one: probe rows (the left side of inner and left joins) filling count - 1 tiles and part
     of one more.  Partner counts run 0..3 from key to key, so output offsets grow unevenly."""
     rng = np.random.default_rng(count)
     n_probe = (count - 1) * JOIN_TILE + 1 + (count * 37) % (JOIN_TILE - 1)
