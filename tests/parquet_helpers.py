@@ -1,10 +1,12 @@
-"""Parquet fixtures shared by tests/test_parquet.py (CPU) and tests/test_parquet_gpu.py: pyarrow-written files, a small Thrift
-compact-protocol reader for page headers, and byte patches that make the device-detected errors.  The CPU tests run the patched bytes
-through the sanitized host build of the decoders before the GPU tests read them on the device."""
+"""Parquet fixtures shared by tests/test_parquet.py (CPU), tests/test_parquet_gpu.py and tests/test_parquet_geometry_gpu.py: pyarrow-written
+files, a small Thrift compact-protocol reader for page headers, byte patches that make the device-detected errors, hand-built files with
+the page shapes pyarrow does not write, snappy streams of chosen elements, and the check of a device read against pyarrow.  The CPU
+tests run the patched bytes through the sanitized host build of the decoders before the GPU tests read them on the device."""
 from __future__ import annotations
 
 import numpy as np
 import pyarrow as pa
+import pyarrow.compute as pc
 import pyarrow.parquet as pq
 
 
@@ -395,9 +397,9 @@ def _read_value(b, i, t):
     return _skip(b, i, t) and None, _skip(b, i, t)
 
 
-def chunk_pages(path: str, column: int = 0):
-    """[(page header as a dict, page bytes after the header)] of a column chunk of row group 0."""
-    md = pq.ParquetFile(path).metadata.row_group(0).column(column)
+def chunk_pages(path: str, column: int = 0, row_group: int = 0):
+    """[(page header as a dict, page bytes after the header)] of a column chunk."""
+    md = pq.ParquetFile(path).metadata.row_group(row_group).column(column)
     b = open(path, "rb").read()
     pos = md.dictionary_page_offset if md.has_dictionary_page else md.data_page_offset
     end = pos + md.total_compressed_size
@@ -407,3 +409,244 @@ def chunk_pages(path: str, column: int = 0):
         pages.append((h, b[data:data + h[3]]))
         pos = data + h[3]
     return pages
+
+
+# ---- what a page holds: its kind, rows and encoding, its level and value sections, the runs of a hybrid stream ----------------------
+ENC_PLAIN, ENC_PLAIN_DICTIONARY, ENC_RLE, ENC_RLE_DICTIONARY, ENC_BSS = 0, 2, 3, 8, 9
+
+
+def page_info(h: dict):
+    """(kind, values, encoding) of a page header: kind "dict", "v1" or "v2"."""
+    if h[1] == 2:
+        return "dict", h[7][1], h[7][2]
+    if h[1] == 0:
+        return "v1", h[5][1], h[5][2]
+    assert h[1] == 3, h[1]
+    return "v2", h[8][1], h[8][4]
+
+
+def data_page_rows(pages) -> list:
+    return [page_info(h)[1] for h, _ in pages if h[1] != 2]
+
+
+def page_sections(h: dict, body: bytes, optional: bool, snappy: bool):
+    """(definition-level stream or None, values section) of a data page, decompressed."""
+    kind = page_info(h)[0]
+    if kind == "v2":
+        rep, dl = h[8].get(6, 0), h[8].get(5, 0)
+        levels = body[rep:rep + dl] if dl else None
+        vals = body[rep + dl:]
+        if snappy and h[8].get(7, True):
+            vals = pa.decompress(vals, h[2] - rep - dl, codec="snappy").to_pybytes()
+        return levels, vals
+    if snappy:
+        body = pa.decompress(body, h[2], codec="snappy").to_pybytes()
+    if not optional:
+        return None, body
+    n = int.from_bytes(body[:4], "little")
+    return body[4:4 + n], body[4 + n:]
+
+
+def hybrid_runs(s: bytes, bw: int, need: int) -> list:
+    """The runs of an RLE / bit-packed hybrid stream until `need` values are covered: ("rle", count, value) or ("bp", count)."""
+    runs, p, cov = [], 0, 0
+    while cov < need:
+        h, p = _varint(s, p)
+        if h & 1:
+            count = (h >> 1) * 8
+            runs.append(("bp", count))
+            p += (h >> 1) * bw
+        else:
+            count = h >> 1
+            vb = (bw + 7) // 8
+            runs.append(("rle", count, int.from_bytes(s[p:p + vb], "little")))
+            p += vb
+        cov += count
+    return runs
+
+
+def hybrid_decode(s: bytes, bw: int, n: int) -> np.ndarray:
+    """The first n values of an RLE / bit-packed hybrid stream."""
+    out, p = [], 0
+    while len(out) < n:
+        h, p = _varint(s, p)
+        if h & 1:
+            groups = h >> 1
+            bits = int.from_bytes(s[p:p + groups * bw], "little")
+            out += [(bits >> (j * bw)) & ((1 << bw) - 1) for j in range(groups * 8)]
+            p += groups * bw
+        else:
+            vb = (bw + 7) // 8
+            out += [int.from_bytes(s[p:p + vb], "little")] * (h >> 1)
+            p += vb
+    return np.array(out[:n], dtype=np.int64)
+
+
+# ---- snappy streams of chosen elements --------------------------------------------------------------------------------------------
+def snappy_encode(elements) -> tuple:
+    """(uncompressed bytes, snappy stream) of elements ("lit", bytes) and ("copy", offset, length, tag) with tag 1 (copy with a 1-byte
+    offset, length 4..11, offset < 2048), 2 (2-byte offset, length 1..64) or 4 (4-byte offset, length 1..64)."""
+    out, tags = bytearray(), bytearray()
+    for e in elements:
+        if e[0] == "lit":
+            m = len(e[1]) - 1
+            if m < 60:
+                tags.append(m << 2)
+            else:
+                nb = (m.bit_length() + 7) // 8
+                tags.append((59 + nb) << 2)
+                tags += m.to_bytes(nb, "little")
+            tags += e[1]
+            out += e[1]
+            continue
+        _, off, ln, tag = e
+        assert 0 < off <= len(out)
+        if tag == 1:
+            assert 4 <= ln <= 11 and off < 2048
+            tags += bytes([1 | (ln - 4) << 2 | (off >> 8) << 5, off & 0xFF])
+        else:
+            assert 1 <= ln <= 64
+            tags.append((2 if tag == 2 else 3) | (ln - 1) << 2)
+            tags += off.to_bytes(2 if tag == 2 else 4, "little")
+        for j in range(ln):
+            out.append(out[len(out) - off])
+    return bytes(out), _varint_encode(len(out), None) + bytes(tags)
+
+
+def snappy_elements(stream: bytes) -> tuple:
+    """(uncompressed length, [(kind, length, offset, output position)]) of a snappy stream; kind "lit", "copy1", "copy2" or "copy4"."""
+    n, i = _varint(stream, 0)
+    els, op = [], 0
+    while i < len(stream):
+        t = stream[i]
+        i += 1
+        if t & 3 == 0:
+            ln = (t >> 2) + 1
+            if ln > 60:
+                nb = ln - 60
+                ln = int.from_bytes(stream[i:i + nb], "little") + 1
+                i += nb
+            els.append(("lit", ln, 0, op))
+            i += ln
+        elif t & 3 == 1:
+            ln, off = 4 + ((t >> 2) & 7), (t >> 5) << 8 | stream[i]
+            i += 1
+            els.append(("copy1", ln, off, op))
+        else:
+            nb = 2 if t & 3 == 2 else 4
+            ln, off = (t >> 2) + 1, int.from_bytes(stream[i:i + nb], "little")
+            i += nb
+            els.append((f"copy{nb}", ln, off, op))
+        op += ln
+    assert op == n
+    return n, els
+
+
+# ---- a hand-built file of one column chunk ----------------------------------------------------------------------------------------
+def rle_levels(runs) -> bytes:
+    """A definition-level stream (bit width 1) of RLE runs (value, count)."""
+    return b"".join(_varint_encode(c << 1, None) + bytes([v]) for v, c in runs)
+
+
+def hand_file(path: str, phys: int, pages, codec: int = 0) -> None:
+    """One optional column "x" (physical type phys, no logical type) in one row group, written by hand.  pages: (rows, encoding,
+    raw body, compressed body or None) of V1 data pages, the body being the 4-byte level length, the levels and the values.  codec 1
+    (SNAPPY): a page without its compressed body is compressed by pyarrow."""
+    body = bytearray(b"PAR1")
+    start = len(body)
+    encs = {3}
+    data_off = len(body)
+    n = 0
+    for rows, enc, raw, comp in pages:
+        if comp is None:
+            comp = pa.compress(raw, codec="snappy", asbytes=True) if codec else raw
+        body += _page_header(0, len(raw), len(comp), rows, enc) + comp
+        encs.add(enc)
+        n += rows
+    total = len(body) - start
+    w = ThriftWriter().i32(1, 1)
+    w.list(2, 12, 2)
+    w.begin().binary(4, b"schema").i32(5, 1).end()
+    w.begin().i32(1, phys).i32(3, 1).binary(4, b"x").end()
+    w.i64(3, n)
+    w.list(4, 12, 1).begin()
+    w.list(1, 12, 1)
+    w.begin().i64(2, start).begin(3)
+    w.i32(1, phys).list(2, 5, len(encs))
+    for e in sorted(encs):
+        w.b += _varint_encode(_zz(e), None)
+    w.list(3, 8, 1)
+    w.b += _varint_encode(1, None) + b"x"
+    w.i32(4, codec).i64(5, n).i64(6, total).i64(7, total).i64(9, data_off)
+    w.end().end()
+    w.i64(2, total).i64(3, n).end()
+    w.b.append(0)
+    footer = bytes(w.b)
+    body += footer + struct_pack_u32(len(footer)) + b"PAR1"
+    open(path, "wb").write(bytes(body))
+
+
+# ---- a device read against pyarrow.parquet ------------------------------------------------------------------------------------------
+def device_bits(col):
+    """(values as unsigned bits, validity, chunk lengths, bitmap presence per chunk) of a device column."""
+    vals, valid, lens, hv = [], [], [], []
+    for a in col.download():
+        m = np.asarray(a.valid_mask(), dtype=bool)
+        if hasattr(a, "value_bits"):
+            v = np.asarray(a.value_bits(), dtype=np.uint64)
+        else:
+            v = np.asarray(a.value_slice())
+            v = v.view(f"u{v.dtype.itemsize}").astype(np.uint64)
+        vals.append(v); valid.append(m); lens.append(a.length); hv.append(a.validity is not None)
+    return np.concatenate(vals), np.concatenate(valid), lens, hv
+
+
+def expected_bits(arr):
+    """(values as unsigned bits, nulls as 0; validity) of an Arrow array or chunked array; temporal values as their integers."""
+    if isinstance(arr, pa.ChunkedArray):
+        arr = arr.combine_chunks()
+    valid = np.asarray(arr.is_valid())
+    t = arr.type
+    if pa.types.is_boolean(t):
+        v = np.asarray(pc.fill_null(arr, False)).astype(np.uint64)
+    else:
+        if pa.types.is_temporal(t):
+            arr = arr.cast(pa.int32() if t.bit_width == 32 else pa.int64())
+        v = np.asarray(pc.fill_null(arr, pa.scalar(0).cast(arr.type)) if arr.null_count else arr)
+        v = v.view(f"u{v.dtype.itemsize}").astype(np.uint64)
+    return v, valid
+
+
+def check_read(rdf, ctx, paths, read_path, batch_size, names=None):
+    """DataFrame::from_parquet of read_path (the files `paths`, in order) against pyarrow.parquet.read_table of each: every value bit for
+    bit, the same null slots, 0 in a null slot, the output chunk lengths (every file cut into batches of batch_size), the bitmap
+    presence of each chunk, and the temporal tags."""
+    tables = [pq.read_table(p) for p in paths]
+    with rdf.ParquetFile(read_path, batch_size=batch_size) as f:
+        if names is None:
+            names = [n for n, dt, _ in f.schema if dt >= 0]
+        cols = f.read(names, ctx=ctx)
+        assert f.num_rows == sum(t.num_rows for t in tables)
+        for name in names:
+            got, gvalid, lens, hv = device_bits(cols[name])
+            want_lens, want_hv, wv, wvalid = [], [], [], []
+            for t in tables:
+                v, m = expected_bits(t.column(name))
+                wv.append(v); wvalid.append(m)
+                for s in range(0, t.num_rows, batch_size):
+                    want_lens.append(min(batch_size, t.num_rows - s))
+                    want_hv.append(not m[s:s + batch_size].all())
+            wv, wvalid = np.concatenate(wv), np.concatenate(wvalid)
+            assert lens == want_lens, name
+            assert hv == want_hv, name
+            assert np.array_equal(gvalid, wvalid), name
+            assert np.array_equal(got[wvalid], wv[wvalid]), name
+            assert not got[~wvalid].any(), name   # a null slot holds 0
+            tag = f.temporal_columns.get(name)
+            t = tables[0].schema.field(name).type
+            if pa.types.is_temporal(t):
+                assert tag is not None, name
+                if pa.types.is_timestamp(t):
+                    assert (tag.unit, tag.tz) == ({"ms": 1, "us": 2, "ns": 3}[t.unit], t.tz), name
+            else:
+                assert tag is None, name

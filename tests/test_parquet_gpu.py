@@ -5,7 +5,6 @@ import ctypes as C
 import os
 
 import numpy as np
-import pyarrow as pa
 import pyarrow.compute as pc
 import pyarrow.csv as pacsv
 import pyarrow.parquet as pq
@@ -19,78 +18,20 @@ pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "uk_cities_with_headers.csv")
 
 
-def _device(col):
-    vals, valid, lens, hv = [], [], [], []
-    for a in col.download():
-        m = np.asarray(a.valid_mask(), dtype=bool)
-        if hasattr(a, "value_bits"):
-            v = np.asarray(a.value_bits(), dtype=np.uint64)
-        else:
-            v = np.asarray(a.value_slice())
-            v = v.view(f"u{v.dtype.itemsize}").astype(np.uint64)
-        vals.append(v); valid.append(m); lens.append(a.length); hv.append(a.validity is not None)
-    return np.concatenate(vals), np.concatenate(valid), lens, hv
-
-
-def _expected(arr: pa.ChunkedArray):
-    arr = arr.combine_chunks()
-    valid = np.asarray(arr.is_valid())
-    t = arr.type
-    if pa.types.is_boolean(t):
-        v = np.asarray(pc.fill_null(arr, False)).astype(np.uint64)
-    else:
-        if pa.types.is_temporal(t):
-            arr = arr.cast(pa.int32() if t.bit_width == 32 else pa.int64())
-        v = np.asarray(pc.fill_null(arr, pa.scalar(0).cast(arr.type)) if arr.null_count else arr)
-        v = v.view(f"u{v.dtype.itemsize}").astype(np.uint64)
-    return v, valid
-
-
-def _check(rdf, ctx, paths, read_path, batch_size):
-    tables = [pq.read_table(p) for p in paths]
-    with rdf.ParquetFile(read_path, batch_size=batch_size) as f:
-        names = [n for n, dt, _ in f.schema if dt >= 0]
-        cols = f.read(names, ctx=ctx)
-        assert f.num_rows == sum(t.num_rows for t in tables)
-        for name in names:
-            got, gvalid, lens, hv = _device(cols[name])
-            want_lens, want_hv, wv, wvalid = [], [], [], []
-            for t in tables:
-                v, m = _expected(t.column(name))
-                wv.append(v); wvalid.append(m)
-                for s in range(0, t.num_rows, batch_size):
-                    want_lens.append(min(batch_size, t.num_rows - s))
-                    want_hv.append(not m[s:s + batch_size].all())
-            wv, wvalid = np.concatenate(wv), np.concatenate(wvalid)
-            assert lens == want_lens, name
-            assert hv == want_hv, name
-            assert np.array_equal(gvalid, wvalid), name
-            assert np.array_equal(got[wvalid], wv[wvalid]), name
-            assert not got[~wvalid].any(), name   # a null slot holds 0
-            tag = f.temporal_columns.get(name)
-            t = tables[0].schema.field(name).type
-            if pa.types.is_temporal(t):
-                assert tag is not None, name
-                if pa.types.is_timestamp(t):
-                    assert (tag.unit, tag.tz) == ({"ms": 1, "us": 2, "ns": 3}[t.unit], t.tz), name
-            else:
-                assert tag is None, name
-
-
 @pytest.mark.parametrize("wid,kw", H.MATRIX, ids=[m[0] for m in H.MATRIX])
 @pytest.mark.parametrize("null_frac", [0.0, 0.1])
 def test_matrix(rdf, ctx, tmp_path, wid, kw, null_frac):
     p = str(tmp_path / "t.parquet")
     pq.write_table(H.table(5000, seed=len(wid), null_frac=null_frac), p, **kw)
-    _check(rdf, ctx, [p], p, 1024)
+    H.check_read(rdf, ctx, [p], p, 1024)
 
 
 def test_all_null_and_required(rdf, ctx, tmp_path):
     p1, p2 = str(tmp_path / "n.parquet"), str(tmp_path / "r.parquet")
     pq.write_table(H.table(3000, seed=5, null_frac=1.0), p1)
     pq.write_table(H.required(H.table(3000, seed=6, null_frac=0.0)), p2, data_page_version="2.0")
-    _check(rdf, ctx, [p1], p1, 1024)
-    _check(rdf, ctx, [p2], p2, 1024)
+    H.check_read(rdf, ctx, [p1], p1, 1024)
+    H.check_read(rdf, ctx, [p2], p2, 1024)
 
 
 @pytest.mark.parametrize("batch_size", [7, 1024, 1 << 20])
@@ -106,7 +47,7 @@ def test_batch_sizes_and_directory(rdf, ctx, tmp_path, batch_size):
     (d / ".hidden").write_bytes(b"junk")
     pq.ParquetWriter(str(d / "zz-empty.parquet"), H.table(1, seed=1).schema).close()   # no row groups: skipped
     assert pq.ParquetFile(str(d / "zz-empty.parquet")).metadata.num_row_groups == 0
-    _check(rdf, ctx, paths, str(d), batch_size)
+    H.check_read(rdf, ctx, paths, str(d), batch_size)
 
 
 def test_projection_uploads_only_its_chunks(rdf, ctx, tmp_path):
@@ -147,15 +88,15 @@ def test_reference_csv_data(rdf, ctx, tmp_path):
     b = rdf.DeviceFrame.from_csv(GOLDEN, ctx=ctx)
     assert list(a.columns) == list(b.columns)
     for n in a.columns:
-        ga, va, la, _ = _device(a.columns[n])
-        gb, vb, lb, _ = _device(b.columns[n])
+        ga, va, la, _ = H.device_bits(a.columns[n])
+        gb, vb, lb, _ = H.device_bits(b.columns[n])
         assert la == lb and np.array_equal(va, vb) and np.array_equal(ga[va], gb[vb]), n
 
 
 def test_legacy_converted_types(rdf, ctx, tmp_path):
     p = str(tmp_path / "legacy.parquet")
     H.legacy_file(p, n=5000, seed=4)
-    _check(rdf, ctx, [p], p, 1024)
+    H.check_read(rdf, ctx, [p], p, 1024)
 
 
 def test_sort_on_parquet_frame(rdf, ctx, tmp_path):
