@@ -455,6 +455,44 @@ typedef struct {
 int  bdf_join_asof_dev(bdf_ctx* ctx, const bdf_col* left_on, const bdf_col* right_on, int32_t n_by, const bdf_col* const* left_by,
                        const bdf_col* const* right_by, const bdf_asof_spec* spec, bdf_col** right_indices);
 
+/* ---- distinct rows and set operations (pandas' duplicated / drop_duplicates / concat; Spark's distinct, dropDuplicates, union,
+ * intersect, intersectAll, subtract, exceptAll; not in the reference) --------------------------------------------------------------
+ * Every operation is a Boolean mask over the (left) rows, to be applied with bdf_filter_dev / bdf_list_filter_dev: the result keeps
+ * the caller's row order and needs no second sort.
+ * Equality.  Two rows are equal when every key is equal under group-by's equality: nulls equal each other, all NaNs are one value,
+ *   and -0.0 == 0.0.
+ * Keys.  1..16 key columns per side, each one of the ten numeric types or Boolean.  Boolean keys are accepted by these entries only:
+ *   inside them they are widened to one byte per row (bdf_bool_widen_dev); bdf_sort_indices_dev and bdf_group_by_dev still refuse them.
+ * bdf_duplicated_dev  *mask: one Boolean slot per row, no nulls, chunked like the keys; true for the rows pandas' duplicated(keep=...)
+ *   marks: KEEP_FIRST every row of a run of equal rows except its first in row order; KEEP_LAST every row except its last; KEEP_NONE
+ *   every row of a run longer than one.
+ * bdf_set_op_dev  *mask: one Boolean slot per LEFT row, no nulls, chunked like left[0]; true = kept.  In a run of equal rows with cl
+ *   left and cr right rows, the run keeps its first q left rows in row order:
+ *     INTERSECT       q = cl > 0 && cr > 0 ? 1 : 0
+ *     INTERSECT_ALL   q = min(cl, cr)
+ *     EXCEPT          q = cr == 0 ? 1 : 0          (Spark's subtract: distinct)
+ *     EXCEPT_ALL      q = max(cl - cr, 0)
+ *   Row counts and row order follow Spark; which copies are kept (the earliest) is this library's definition, so the result is
+ *   deterministic.  Kept rows keep their own bits: when the first occurrence is -0.0, the result holds -0.0.
+ * bdf_concat_dev / bdf_list_concat_dev  the chunks of cols[0], then those of cols[1], and so on, copied device to device; bitmaps
+ *   start at bit 0 of every result chunk.  All inputs must have one dtype (child dtype for lists), else BDF_UNSUPPORTED.
+ * bdf_bool_widen_dev  a Boolean column as UInt8 0 / 1, chunked like it, nulls kept: a Boolean payload column goes through
+ *   bdf_filter_dev this way, and bdf_compare_dev(NE, 0) turns it back.
+ * Errors (nothing is returned and nothing leaks): n_keys outside 1..16, n < 1, a null pointer, an unknown keep or op -> BDF_INVALID; a
+ *   non-numeric key -> BDF_UNSUPPORTED; a key position whose left and right dtypes differ -> BDF_UNSUPPORTED "Union can only be
+ *   performed on tables with compatible column types"; key columns of one side with different lengths -> BDF_LENGTH_MISMATCH; more
+ *   than 2^32-1 rows in the sort (left + right for the set operations) -> the sort's BDF_UNSUPPORTED; a multi-GPU context ->
+ *   BDF_UNSUPPORTED, as for sort / group-by / join.
+ * The keys are sorted stably once (a set operation sorts the left rows, then the right rows, as one column), so a run's left rows
+ *   come first and its left count is the distance from the run start to its first right row.  Launch records: BDF_K_GROUP. */
+typedef enum { BDF_KEEP_FIRST = 0, BDF_KEEP_LAST, BDF_KEEP_NONE } bdf_keep;
+typedef enum { BDF_SETOP_INTERSECT = 0, BDF_SETOP_INTERSECT_ALL, BDF_SETOP_EXCEPT, BDF_SETOP_EXCEPT_ALL } bdf_setop;
+int  bdf_duplicated_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_col* const* keys, int32_t keep, bdf_col** mask);
+int  bdf_set_op_dev(bdf_ctx* ctx, int32_t op, int32_t n_keys, const bdf_col* const* left, const bdf_col* const* right, bdf_col** mask);
+int  bdf_concat_dev(bdf_ctx* ctx, int32_t n, const bdf_col* const* cols, bdf_col** out);
+int  bdf_list_concat_dev(bdf_ctx* ctx, int32_t n, const bdf_list* const* lists, bdf_list** out);
+int  bdf_bool_widen_dev(bdf_ctx* ctx, const bdf_col* in, bdf_col** out);
+
 /* ---- window functions (WindowFunctions, src/functions/window.rs:1-11; WindowSpec, src/window.rs:8-22: stubs in the reference) ----
  * One call computes n_calls window columns that share one specification, so the rows are sorted once.
  * Rows and order.  Partitions are the runs of equal tuples of the 0..16 numeric partition_by columns; within a partition rows are

@@ -152,6 +152,14 @@ pub struct BdfAsofSpec { pub direction: i32, pub allow_exact_matches: i32, pub h
 pub const BDF_ASOF_BACKWARD: i32 = 0;
 pub const BDF_ASOF_FORWARD: i32 = 1;
 pub const BDF_ASOF_NEAREST: i32 = 2;
+// bdf_keep / bdf_setop
+pub const BDF_KEEP_FIRST: i32 = 0;
+pub const BDF_KEEP_LAST: i32 = 1;
+pub const BDF_KEEP_NONE: i32 = 2;
+pub const BDF_SETOP_INTERSECT: i32 = 0;
+pub const BDF_SETOP_INTERSECT_ALL: i32 = 1;
+pub const BDF_SETOP_EXCEPT: i32 = 2;
+pub const BDF_SETOP_EXCEPT_ALL: i32 = 3;
 /// bdf_join_type: JoinType's four, then the existence joins.
 pub const BDF_JOIN_LEFT_SEMI: i32 = 4;
 pub const BDF_JOIN_LEFT_ANTI: i32 = 5;
@@ -262,6 +270,15 @@ extern "C" {
     // as-of join (pandas' merge_asof): one UInt32 column, a right row number per left row in left order, NULL = no partner
     pub fn bdf_join_asof_dev(ctx: *mut BdfCtx, left_on: *const BdfCol, right_on: *const BdfCol, n_by: i32, left_by: *const *const BdfCol,
                              right_by: *const *const BdfCol, spec: *const BdfAsofSpec, right_indices: *mut *mut BdfCol) -> c_int;
+    // distinct rows and set operations: a Boolean mask over the (left) rows, chunked like the keys, no nulls (include/b200df.h)
+    pub fn bdf_duplicated_dev(ctx: *mut BdfCtx, n_keys: i32, keys: *const *const BdfCol, keep: i32, mask: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_set_op_dev(ctx: *mut BdfCtx, op: i32, n_keys: i32, left: *const *const BdfCol, right: *const *const BdfCol,
+                          mask: *mut *mut BdfCol) -> c_int;
+    // the chunks of cols[0], then those of cols[1], ... copied on the device; one dtype
+    pub fn bdf_concat_dev(ctx: *mut BdfCtx, n: i32, cols: *const *const BdfCol, out: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_list_concat_dev(ctx: *mut BdfCtx, n: i32, lists: *const *const BdfList, out: *mut *mut BdfList) -> c_int;
+    // a Boolean column as UInt8 0 / 1 (nulls kept), the form in which a Boolean payload goes through bdf_filter_dev
+    pub fn bdf_bool_widen_dev(ctx: *mut BdfCtx, input: *const BdfCol, out: *mut *mut BdfCol) -> c_int;
     // window functions over one WindowSpec (src/window.rs:8-22; WindowFunctions, src/functions/window.rs:1-11): n_calls one-chunk columns
     // in the caller's row order, every one the caller's to free
     pub fn bdf_window_dev(ctx: *mut BdfCtx, n_partition: i32, partition_by: *const *const BdfCol, n_order: i32, order_by: *const BdfSortKey,

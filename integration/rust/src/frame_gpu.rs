@@ -254,6 +254,45 @@ pub fn join_asof_device(left: &DeviceColumns, right: &DeviceColumns, on: (usize,
     Ok(out)
 }
 
+/// pandas' `duplicated` over the columns `keys` of `frame` (include/b200df.h "distinct rows and set operations"): a Boolean mask
+/// without nulls, chunked like the frame, true for the rows `keep` (BDF_KEEP_FIRST / _LAST / _NONE) marks.  Filter every column with
+/// its NOT for `drop_duplicates`.  Not in the reference.
+pub fn duplicated_device(frame: &DeviceColumns, keys: &[usize], keep: i32) -> Result<*mut BdfCol, String> {
+    let ks: Vec<*const BdfCol> = keys.iter().map(|k| frame.cols[*k] as *const BdfCol).collect();
+    let mut mask: *mut BdfCol = std::ptr::null_mut();
+    check(unsafe { bdf_duplicated_dev(dev(), ks.len() as i32, ks.as_ptr(), keep, &mut mask) })?;
+    Ok(mask)
+}
+
+/// Spark's `intersect` / `intersectAll` / `subtract` / `exceptAll` (`op`: BDF_SETOP_*), every column compared by position: the mask
+/// of the `left` rows kept, chunked like `left`, in its row order.  Not in the reference.
+pub fn set_op_device(left: &DeviceColumns, right: &DeviceColumns, op: i32) -> Result<*mut BdfCol, String> {
+    if left.cols.len() != right.cols.len() {
+        return Err("Union can only be performed on tables with compatible column types".to_string());
+    }
+    let lk: Vec<*const BdfCol> = left.cols.iter().map(|c| *c as *const BdfCol).collect();
+    let rk: Vec<*const BdfCol> = right.cols.iter().map(|c| *c as *const BdfCol).collect();
+    let mut mask: *mut BdfCol = std::ptr::null_mut();
+    check(unsafe { bdf_set_op_dev(dev(), op, lk.len() as i32, lk.as_ptr(), rk.as_ptr(), &mut mask) })?;
+    Ok(mask)
+}
+
+/// Spark's `union` (UNION ALL) of two frames by position: the chunks of `top`, then those of `bottom`, column by column, with the
+/// names of `top`.  The column types must be equal.  Not in the reference.
+pub fn concat_device(top: &DeviceColumns, bottom: &DeviceColumns) -> Result<DeviceColumns, String> {
+    if top.cols.len() != bottom.cols.len() {
+        return Err("Union can only be performed on tables with compatible column types".to_string());
+    }
+    let mut out = DeviceColumns { names: top.names.clone(), cols: Vec::with_capacity(top.cols.len()) };
+    for (a, b) in top.cols.iter().zip(&bottom.cols) {
+        let pair = [*a as *const BdfCol, *b as *const BdfCol];
+        let mut c: *mut BdfCol = std::ptr::null_mut();
+        check(unsafe { bdf_concat_dev(dev(), 2, pair.as_ptr(), &mut c) })?;
+        out.cols.push(c);
+    }
+    Ok(out)
+}
+
 /// Window functions over one `WindowSpec` (src/window.rs:8-22, not in lib.rs; `WindowFunctions`, src/functions/window.rs:1-11, empty
 /// bodies): `partition` are column indices of `frame`, `order` (column index, descending) pairs, `calls` (output name, call) with
 /// `call.column` a column pointer of `frame` or null for a ranking function.  The rows are sorted once for all calls.  Returns the new

@@ -55,6 +55,10 @@ JOIN_TYPES = {"left": JOIN_LEFT, "right": JOIN_RIGHT, "inner": JOIN_INNER, "full
 # bdf_asof_direction
 ASOF_BACKWARD, ASOF_FORWARD, ASOF_NEAREST = range(3)
 ASOF_DIRECTIONS = {"backward": ASOF_BACKWARD, "forward": ASOF_FORWARD, "nearest": ASOF_NEAREST}
+# bdf_keep / bdf_setop
+KEEP_FIRST, KEEP_LAST, KEEP_NONE = range(3)
+SETOP_INTERSECT, SETOP_INTERSECT_ALL, SETOP_EXCEPT, SETOP_EXCEPT_ALL = range(4)
+SET_OPS = {"intersect": SETOP_INTERSECT, "intersect_all": SETOP_INTERSECT_ALL, "except": SETOP_EXCEPT, "except_all": SETOP_EXCEPT_ALL}
 # bdf_window_fn / bdf_window_frame
 (WIN_ROW_NUMBER, WIN_RANK, WIN_DENSE_RANK, WIN_PERCENT_RANK, WIN_CUME_DIST, WIN_LAG, WIN_LEAD, WIN_SUM, WIN_COUNT, WIN_MIN, WIN_MAX,
  WIN_AVG, WIN_FIRST_VALUE, WIN_LAST_VALUE, WIN_NTH_VALUE) = range(15)
@@ -283,6 +287,11 @@ def lib() -> C.CDLL:
         "bdf_group_by_lists_dev": ([vp, i32, P(vp), i32, P(GroupAggC), P(vp), P(vp), P(vp), P(i64)], C.c_int),
         "bdf_join_indices_dev": ([vp, i32, i32, P(vp), P(vp), P(vp), P(vp), P(i64)], C.c_int),
         "bdf_join_asof_dev": ([vp, vp, vp, i32, P(vp), P(vp), P(AsofSpec), P(vp)], C.c_int),
+        "bdf_duplicated_dev": ([vp, i32, P(vp), i32, P(vp)], C.c_int),
+        "bdf_set_op_dev": ([vp, i32, i32, P(vp), P(vp), P(vp)], C.c_int),
+        "bdf_concat_dev": ([vp, i32, P(vp), P(vp)], C.c_int),
+        "bdf_list_concat_dev": ([vp, i32, P(vp), P(vp)], C.c_int),
+        "bdf_bool_widen_dev": ([vp, vp, P(vp)], C.c_int),
         "bdf_window_dev": ([vp, i32, P(vp), i32, P(SortKeyC), i32, P(WindowCall), P(vp)], C.c_int),
         "bdf_compare_dev": ([vp, C.c_int, vp, vp, C.c_double, P(vp)], C.c_int),
         "bdf_boolean_dev": ([vp, C.c_int, vp, vp, P(vp)], C.c_int),
@@ -380,7 +389,7 @@ EXPORTED_SYMBOLS = [
     "bdf_host_alloc", "bdf_host_free", "bdf_host_register", "bdf_host_unregister", "bdf_binary", "bdf_unary", "bdf_cast",
     "bdf_aggregate", "bdf_aggregate_all", "bdf_avg", "bdf_upload", "bdf_upload_many", "bdf_col_wait", "bdf_col_describe",
     "bdf_col_chunk_info", "bdf_binary_dev", "bdf_unary_dev", "bdf_cast_dev", "bdf_aggregate_dev",
-    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_group_by_lists_dev", "bdf_join_indices_dev", "bdf_join_asof_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_rowwise_dev", "bdf_case_when_dev", "bdf_null_test_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
+    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_group_by_lists_dev", "bdf_join_indices_dev", "bdf_join_asof_dev", "bdf_duplicated_dev", "bdf_set_op_dev", "bdf_concat_dev", "bdf_list_concat_dev", "bdf_bool_widen_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_rowwise_dev", "bdf_case_when_dev", "bdf_null_test_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
     "bdf_binary_agg_dev", "bdf_binary_agg_dev_async", "bdf_aggregate_all_dev_async", "bdf_future_wait", "bdf_col_free", "bdf_profile_enable", "bdf_profile_read",
     "bdf_launch_count", "bdf_timer_start", "bdf_timer_stop", "bdf_flush_l2", "bdf_generate",
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",

@@ -475,6 +475,15 @@ cudaError_t launch_join_asof(int n_by, const int* dtypes, const void* const* pro
                              long long n_probe, const uint32_t* run_starts, long long n_runs, long long n_build, const uint32_t* perm, uint32_t* out,
                              uint32_t* out_valid, cudaStream_t s);
 
+// Distinct rows and set operations (k_setop.cu).  heads: {head words, per-word run prefix, run starts} of the sorted positions.
+// mode: 0..2 bdf_keep (duplicated), 3 + bdf_setop.  words: one bit per output row at the row's original position, zeroed by the caller.
+cudaError_t launch_setop_left_count(const void* const* heads, long long n_runs, long long n, const uint32_t* perm, long long n_left,
+                                    uint32_t* run_left, cudaStream_t s);
+cudaError_t launch_setop_mark(const void* const* heads, long long n_runs, long long n, const uint32_t* perm, long long n_out, int mode,
+                              const uint32_t* run_left, uint32_t* words, cudaStream_t s);
+cudaError_t launch_setop_widen_bool(const void* bits, long long off, long long len, unsigned char* out, cudaStream_t s);
+cudaError_t launch_bitmap_rebase(const void* src, long long off, long long len, uint32_t* dst, cudaStream_t s);
+
 // Window functions (k_window.cu).
 cudaError_t launch_window_rank(const void* const* p, long long n_p, const void* const* q, long long n_q, long long n, const uint32_t* perm,
                                void* const* outs, cudaStream_t s);

@@ -2121,6 +2121,246 @@ static int sorted_runs(bdf_ctx* c, int n_keys, int n_cut, const bdf_col* const* 
     return BDF_OK;
 }
 
+// One head bitmap and what k_window and k_setop need to find the run of a position in O(1).
+struct WinHeadsHost {
+    explicit WinHeadsHost(bdf_ctx* c) : bits(c), starts(c) {}
+    ColOwner bits;                        // bit i: sorted position i starts a run
+    Scratch<unsigned long long> prefix;   // per head word: the runs that start before it
+    ColOwner starts;                      // the first position of every run
+    int64_t n_runs = 0;
+    const void* arrays[3] = {nullptr, nullptr, nullptr};   // {words, prefix, starts} as the kernels take them
+};
+
+// The per-word run prefix of h->bits and the compacted run starts; the scan's launches are recorded under `kernel`.
+static int window_runs(bdf_ctx* c, const bdf_col* iota, int64_t n, WinHeadsHost* h, int kernel = BDF_K_WINDOW) {
+    const int64_t words = (n + 31) / 32;
+    Scratch<unsigned long long> block_sums;
+    cudaError_t e = h->prefix.alloc(c, (size_t)(words + 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)scan_tile_sums(words) * sizeof(unsigned long long));
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, kernel, BDF_U64, n, words * (4 + 8 + 16));   // popcounts written, then read and written by the scan
+        c->launches += kScanPopcountLaunches - 1;                        // the timer counts one
+        e = launch_scan_popcount((const uint32_t*)h->bits->chunks[0].values, words, h->prefix, block_sums, c->s_compute);
+    }
+    if (e != cudaSuccess) return fail_cuda(e, "window run prefix");
+    TRY(filter_dev(c, iota, h->bits.get(), h->starts.out()));
+    h->n_runs = h->starts->chunks[0].len;
+    h->arrays[0] = h->bits->chunks[0].values;
+    h->arrays[1] = h->prefix.get();
+    h->arrays[2] = h->starts->chunks[0].values;
+    return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// distinct rows and set operations (k_setop.cu): the key tuples are sorted stably once -- a set operation sorts the left rows and then
+// the right rows as one column, borrowing both sides' chunks -- gathered, and cut into runs by the head kernel, whose equality is
+// group-by's.  One pass over the sorted positions decides every row from its run's bounds (and, for a set operation, the run's left
+// count, which the run's last left position writes) and stores a byte at the row's original position; a second pass packs the bytes
+// of every output chunk into its bitmap.  The result is a Boolean mask over the (left) rows, chunked like the keys, for the filter.
+
+// A Boolean column as one UInt8 per row (0 / 1), chunked like it, its validity copied to bit 0: the sort and the head kernel compare
+// Boolean keys as UInt8.
+static int bool_widen(bdf_ctx* c, const bdf_col* in, bdf_col** out) {
+    std::vector<ChunkPlan> plan;
+    for (const DevChunk& ch : in->chunks) plan.push_back(ChunkPlan{ch.len, ch.validity != nullptr});
+    ColOwner o(c);
+    TRY(col_alloc(c, BDF_U8, plan, nullptr, 0, o.out()));
+    TRY(fetch_counts(c, const_cast<bdf_col*>(in)));   // a computed column's null counts may still be on the device
+    wait_groups(c->s_compute, in, 0, (int64_t)in->chunks.size());
+    cudaError_t e = cudaSuccess;
+    {
+        LaunchTimer t(c, BDF_K_GROUP, BDF_U8, in->total_len, in->total_len + in->total_len / 4);
+        int launches = 0;
+        for (size_t i = 0; i < in->chunks.size() && e == cudaSuccess; i++) {
+            const DevChunk& s = in->chunks[i];
+            if (!s.len) continue;
+            e = launch_setop_widen_bool(s.values, s.val_bit_off, s.len, (unsigned char*)o->chunks[i].values, c->s_compute);
+            launches++;
+            if (e == cudaSuccess && s.validity) {
+                e = launch_bitmap_rebase(s.validity, s.bit_off, s.len, o->chunks[i].validity, c->s_compute);
+                launches++;
+            }
+        }
+        c->launches += std::max(launches - 1, 0);   // the timer counts one
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "Boolean widening");
+    o->null_counts = in->null_counts;
+    *out = o.release();
+    return BDF_OK;
+}
+
+// The chunks of cols[0], then those of cols[1], ...: values copied device to device, bitmaps copied to bit 0 of their new chunk.
+static int concat_dev(bdf_ctx* c, int n, const bdf_col* const* cols, bdf_col** out) {
+    if (n < 1) return fail(BDF_INVALID, "concat takes at least one column");
+    if (!cols || !out) return fail(BDF_INVALID, "null argument");
+    for (int k = 0; k < n; k++)
+        if (!cols[k]) return fail(BDF_INVALID, "null column");
+    const int dt = cols[0]->dtype;
+    if (!((dt >= 0 && dt < BDF_NTYPES) || dt == kBool)) return fail(BDF_UNSUPPORTED, "concat takes numeric or Boolean columns");
+    for (int k = 0; k < n; k++)
+        if (cols[k]->dtype != dt) return fail(BDF_UNSUPPORTED, "concatenated columns must have the same dtype");
+    std::vector<ChunkPlan> plan;
+    std::vector<const DevChunk*> src;
+    std::vector<int64_t> nulls;
+    for (int k = 0; k < n; k++) {
+        TRY(fetch_counts(c, const_cast<bdf_col*>(cols[k])));   // a computed column's null counts may still be on the device
+        for (size_t i = 0; i < cols[k]->chunks.size(); i++) {
+            const DevChunk& ch = cols[k]->chunks[i];
+            plan.push_back(ChunkPlan{ch.len, ch.validity != nullptr});
+            src.push_back(&ch);
+            nulls.push_back(cols[k]->null_counts[i]);
+        }
+        wait_groups(c->s_compute, cols[k], 0, (int64_t)cols[k]->chunks.size());
+    }
+    ColOwner o(c);
+    TRY(col_alloc(c, dt, plan, nullptr, 0, o.out()));
+    cudaError_t e = cudaSuccess;
+    int64_t rows = 0, bytes = 0;   // read and written
+    for (const DevChunk* s : src) {
+        rows += s->len;
+        bytes += 2 * ((dt == kBool ? bitmap_bytes(s->len) : s->len * dtype_width(dt)) + (s->validity ? bitmap_bytes(s->len) : 0));
+    }
+    {
+        LaunchTimer t(c, BDF_K_GROUP, dt, rows, bytes);
+        int launches = 0;
+        for (size_t i = 0; i < src.size() && e == cudaSuccess; i++) {
+            const DevChunk &s = *src[i], &d = o->chunks[i];
+            if (!s.len) continue;
+            if (dt == kBool) {
+                e = launch_bitmap_rebase(s.values, s.val_bit_off, s.len, (uint32_t*)d.values, c->s_compute);
+                launches++;
+            } else {
+                e = cudaMemcpyAsync(d.values, s.values, (size_t)s.len * dtype_width(dt), cudaMemcpyDeviceToDevice, c->s_compute);
+            }
+            if (e == cudaSuccess && s.validity) {
+                e = launch_bitmap_rebase(s.validity, s.bit_off, s.len, d.validity, c->s_compute);
+                launches++;
+            }
+        }
+        c->launches += launches - 1;   // the timer counts one
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, o.get());
+    if (e != cudaSuccess) return fail_cuda(e, "concat");
+    o->null_counts = nulls;
+    *out = o.release();
+    return BDF_OK;
+}
+
+// A mask over the rows of `left` (one bitmap of all left rows, then copied to every chunk's bitmap).  mode 0..2: duplicated with that bdf_keep, right == null;
+// mode 3 + bdf_setop: the set operation against `right`.  The arguments are checked by the entries.
+static int setop_mask(bdf_ctx* c, int mode, int n_keys, const bdf_col* const* left, const bdf_col* const* right, bdf_col** out) {
+    const int64_t nl = left[0]->total_len, nr = right ? right[0]->total_len : 0, n = nl + nr;
+    if (n > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
+    std::vector<ChunkPlan> plan;
+    for (const DevChunk& ch : left[0]->chunks) plan.push_back(ChunkPlan{ch.len, false});
+    ColOwner mask(c);
+    TRY(col_alloc(c, kBool, plan, nullptr, 0, mask.out()));
+    if (nl == 0) {
+        cudaError_t e = finish_single_group(c, mask.get());
+        if (e != cudaSuccess) return fail_cuda(e, "distinct rows");
+        *out = mask.release();
+        return BDF_OK;
+    }
+
+    // the keys: Boolean ones widened, the two sides of a set operation borrowed as one column
+    std::vector<ColOwner> owned;
+    owned.reserve((size_t)n_keys * 4);
+    std::vector<bdf_sort_key> sk;
+    for (int k = 0; k < n_keys; k++) {
+        const bdf_col* side[2] = {left[k], right ? right[k] : nullptr};
+        for (int j = 0; j < 2 && side[j]; j++)
+            if (side[j]->dtype == kBool) {
+                owned.emplace_back(c);
+                TRY(bool_widen(c, side[j], owned.back().out()));
+                side[j] = owned.back().get();
+            }
+        if (side[1]) {
+            std::vector<DevChunk> chunks(side[0]->chunks);
+            chunks.insert(chunks.end(), side[1]->chunks.begin(), side[1]->chunks.end());
+            wait_groups(c->s_compute, side[0], 0, (int64_t)side[0]->chunks.size());
+            wait_groups(c->s_compute, side[1], 0, (int64_t)side[1]->chunks.size());
+            owned.emplace_back(c);
+            TRY(col_borrow(side[0]->dtype, chunks, owned.back().out()));
+            side[0] = owned.back().get();
+        }
+        sk.push_back(bdf_sort_key{side[0], 0});
+    }
+
+    // sort, gather, heads, run prefix and starts
+    ColOwner perm(c), iota(c);
+    TRY(sort_indices_dev(c, n_keys, sk.data(), perm.out()));
+    std::vector<ColOwner> sorted;
+    std::vector<const bdf_col*> sorted_keys;
+    for (int k = 0; k < n_keys; k++) {
+        sorted.emplace_back(c);
+        TRY(take_dev(c, sk[k].column, perm.get(), sorted.back().out()));
+        sorted_keys.push_back(sorted.back().get());
+    }
+    WinHeadsHost H(c);
+    TRY(group_heads(c, sorted_keys, false, n, H.bits.out(), BDF_K_GROUP));
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, iota.out()));
+    c->launches++;
+    cudaError_t e = launch_iota((uint32_t*)iota->chunks[0].values, n, c->sm_count, c->s_compute);
+    if (e == cudaSuccess) e = finish_single_group(c, iota.get());
+    if (e != cudaSuccess) return fail_cuda(e, "distinct rows iota");
+    TRY(window_runs(c, iota.get(), n, &H, BDF_K_GROUP));
+
+    // the decisions at every left row's original position, then one bitmap per chunk
+    const uint32_t* perm_d = (const uint32_t*)perm->chunks[0].values;
+    Scratch<uint32_t> run_left;
+    if (mode >= 3) e = run_left.alloc(c, (size_t)std::max<int64_t>(H.n_runs, 1) * sizeof(uint32_t));
+    if (e != cudaSuccess) return fail_cuda(e, "distinct rows scratch allocation");
+    if (mode >= 3) {
+        LaunchTimer t(c, BDF_K_GROUP, BDF_U32, n, n * 4 + nl * 24 / 32 + H.n_runs * 4);   // perm; head words, prefix and starts of left rows
+        e = launch_setop_left_count(H.arrays, H.n_runs, n, perm_d, nl, run_left, c->s_compute);
+    }
+    Scratch<uint32_t> words;   // one bit per left row, the true ones OR-ed in
+    const int64_t n_words = (nl + 31) / 32;
+    if (e == cudaSuccess) e = words.alloc(c, (size_t)n_words * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaMemsetAsync(words, 0, (size_t)n_words * sizeof(uint32_t), c->s_compute);
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_GROUP, kBool, n, n * (4 + 4 + 8) + n_words * 4 + (mode >= 3 ? nl * 4 : 0));
+        e = launch_setop_mark(H.arrays, H.n_runs, n, perm_d, nl, mode, run_left.get(), words, c->s_compute);
+    }
+    if (e == cudaSuccess) {
+        LaunchTimer t(c, BDF_K_GROUP, kBool, nl, 2 * n_words * 4);
+        int64_t row0 = 0;
+        int launches = 0;
+        for (size_t i = 0; i < mask->chunks.size() && e == cudaSuccess; i++) {
+            const DevChunk& d = mask->chunks[i];
+            if (d.len) {
+                e = launch_bitmap_rebase(words.get(), row0, d.len, (uint32_t*)d.values, c->s_compute);
+                launches++;
+            }
+            row0 += d.len;
+        }
+        c->launches += launches - 1;   // the timer counts one
+    }
+    if (e == cudaSuccess) e = finish_single_group(c, mask.get());
+    if (e != cudaSuccess) return fail_cuda(e, "distinct rows");
+    *out = mask.release();
+    return BDF_OK;
+}
+
+// The checks of the two entries; right == null for duplicated.
+static int setop_check(int n_keys, const bdf_col* const* left, const bdf_col* const* right, bool two_sides) {
+    if (n_keys < 1 || n_keys > 16) return fail(BDF_INVALID, "1..16 key columns");
+    if (!left || (two_sides && !right)) return fail(BDF_INVALID, "null argument");
+    for (int k = 0; k < n_keys; k++)
+        if (!left[k] || (two_sides && !right[k])) return fail(BDF_INVALID, "null key column");
+    auto keyable = [](int dt) { return (dt >= 0 && dt < BDF_NTYPES) || dt == kBool; };
+    for (int k = 0; k < n_keys; k++)
+        if (!keyable(left[k]->dtype) || (two_sides && !keyable(right[k]->dtype)))
+            return fail(BDF_UNSUPPORTED, "distinct rows and set operations take numeric or Boolean key columns");
+    for (int k = 0; two_sides && k < n_keys; k++)
+        if (left[k]->dtype != right[k]->dtype) return fail(BDF_UNSUPPORTED, "Union can only be performed on tables with compatible column types");
+    for (int k = 0; k < n_keys; k++)
+        if (left[k]->total_len != left[0]->total_len || (two_sides && right[k]->total_len != right[0]->total_len))
+            return fail(BDF_LENGTH_MISMATCH, "key columns of one side have different lengths");
+    return BDF_OK;
+}
+
 // The distinct valid values of x inside every group: a second stable lexsort over (keys..., x) -- the groups occupy the same row
 // ranges in both sort orders -- and the heads of (keys..., x) on a valid x, each of which starts a distinct value of its group.
 // n_keys == 0: the whole column is one group.  sval: x in that order; pos: the sorted rows of the heads (ascending value order
@@ -3099,35 +3339,6 @@ static int join_asof_dev(bdf_ctx* c, const bdf_col* lon, const bdf_col* ron, int
 // compacted run starts, so a position finds its partition and peer bounds in O(1).  Ranking functions are written straight to row
 // order through the permutation; lag / lead and the scans work in sorted order and come back through one take each, whose index
 // is the frame's last sorted position of every row.  Without any key nothing is sorted: the kernels read the caller's chunks in place.
-
-// One head bitmap and what k_window needs to find the run of a position in O(1).
-struct WinHeadsHost {
-    explicit WinHeadsHost(bdf_ctx* c) : bits(c), starts(c) {}
-    ColOwner bits;                        // bit i: sorted position i starts a run
-    Scratch<unsigned long long> prefix;   // per head word: the runs that start before it
-    ColOwner starts;                      // the first position of every run
-    int64_t n_runs = 0;
-    const void* arrays[3] = {nullptr, nullptr, nullptr};   // {words, prefix, starts} as the kernels take them
-};
-
-static int window_runs(bdf_ctx* c, const bdf_col* iota, int64_t n, WinHeadsHost* h) {
-    const int64_t words = (n + 31) / 32;
-    Scratch<unsigned long long> block_sums;
-    cudaError_t e = h->prefix.alloc(c, (size_t)(words + 1) * sizeof(unsigned long long));
-    if (e == cudaSuccess) e = block_sums.alloc(c, (size_t)scan_tile_sums(words) * sizeof(unsigned long long));
-    if (e == cudaSuccess) {
-        LaunchTimer t(c, BDF_K_WINDOW, BDF_U64, n, words * (4 + 8 + 16));   // popcounts written, then read and written by the scan
-        c->launches += kScanPopcountLaunches - 1;                              // the timer counts one
-        e = launch_scan_popcount((const uint32_t*)h->bits->chunks[0].values, words, h->prefix, block_sums, c->s_compute);
-    }
-    if (e != cudaSuccess) return fail_cuda(e, "window run prefix");
-    TRY(filter_dev(c, iota, h->bits.get(), h->starts.out()));
-    h->n_runs = h->starts->chunks[0].len;
-    h->arrays[0] = h->bits->chunks[0].values;
-    h->arrays[1] = h->prefix.get();
-    h->arrays[2] = h->starts->chunks[0].values;
-    return BDF_OK;
-}
 
 static bool win_is_rank(int f) { return f >= BDF_WIN_ROW_NUMBER && f <= BDF_WIN_CUME_DIST; }
 static bool win_is_shift(int f) { return f == BDF_WIN_LAG || f == BDF_WIN_LEAD; }
@@ -5785,6 +5996,48 @@ static int list_filter(bdf_ctx* c, const bdf_list* l, const bdf_col* mask, bdf_l
     return list_gather(c, l, kept.get(), true, out);
 }
 
+// The lists of ls[0], then those of ls[1], ...: offsets and list validity copied device to device, the elements concatenated with
+// concat_dev (chunk i of the elements stays the elements of list chunk i).
+static int list_concat(bdf_ctx* c, int n, const bdf_list* const* ls, bdf_list** out) {
+    if (n < 1) return fail(BDF_INVALID, "concat takes at least one list column");
+    if (!ls || !out) return fail(BDF_INVALID, "null argument");
+    for (int k = 0; k < n; k++)
+        if (!ls[k]) return fail(BDF_INVALID, "null list column");
+    for (int k = 0; k < n; k++)
+        if (ls[k]->dtype != ls[0]->dtype) return fail(BDF_UNSUPPORTED, "concatenated list columns must have the same child dtype");
+    std::vector<int64_t> lens, nulls, valid_elems;
+    std::vector<bool> has_valid;
+    std::vector<const bdf_col*> values;
+    for (int k = 0; k < n; k++) {
+        const bdf_list* l = ls[k];
+        lens.insert(lens.end(), l->lens.begin(), l->lens.end());
+        nulls.insert(nulls.end(), l->null_counts.begin(), l->null_counts.end());
+        valid_elems.insert(valid_elems.end(), l->valid_elems.begin(), l->valid_elems.end());
+        for (uint32_t* v : l->valid) has_valid.push_back(v != nullptr);
+        values.push_back(l->values);
+    }
+    int64_t elems = 0;
+    for (int k = 0; k < n; k++) elems += ls[k]->values->total_len;
+    if (elems >= kListMaxCallElems) return fail(BDF_UNSUPPORTED, "a list call holds 2^32 or more elements (the sort's UInt32 row numbers)");
+    ListOwner o(c);
+    TRY(list_alloc(c, ls[0]->dtype, lens, has_valid, o.out()));
+    TRY(concat_dev(c, n, values.data(), &o->values));   // waits for every input's elements, whose groups cover the offsets too
+    cudaError_t e = cudaSuccess;
+    size_t j = 0;
+    for (int k = 0; k < n && e == cudaSuccess; k++)
+        for (size_t i = 0; i < ls[k]->lens.size() && e == cudaSuccess; i++, j++) {
+            const int64_t len = ls[k]->lens[i];
+            e = cudaMemcpyAsync(o->off[j], ls[k]->off[i], (size_t)(len + 1) * 4, cudaMemcpyDeviceToDevice, c->s_compute);
+            if (e == cudaSuccess && ls[k]->valid[i] && len)
+                e = cudaMemcpyAsync(o->valid[j], ls[k]->valid[i], (size_t)(len + 31) / 32 * 4, cudaMemcpyDeviceToDevice, c->s_compute);
+        }
+    if (e != cudaSuccess) return fail_cuda(e, "list concat");
+    o->null_counts = nulls;
+    o->valid_elems = valid_elems;
+    *out = o.release();
+    return BDF_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // line-delimited JSON reader (k_json.cu; the rules are in include/b200df.h): the file goes to HBM as for the CSV reader; the lines
 // are found, checked and walked on the device, which lists every member of every record's object.  The host decodes the distinct
@@ -7766,6 +8019,45 @@ int bdf_list_filter_dev(bdf_ctx* c, const bdf_list* l, const bdf_col* mask, bdf_
     LIST_ENTER(c);
     if (!l || !mask || !out) return fail(BDF_INVALID, "null argument");
     return list_filter(c, l, mask, out);
+}
+
+// ---- distinct rows and set operations ---------------------------------------------------------------------------------------
+
+int bdf_duplicated_dev(bdf_ctx* c, int32_t n_keys, const bdf_col* const* keys, int32_t keep, bdf_col** mask) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "distinct rows move rows between chunks: use a one-GPU context (bdf_init) for them");
+    ENTER(c);
+    if (!mask) return fail(BDF_INVALID, "null argument");
+    if (keep < BDF_KEEP_FIRST || keep > BDF_KEEP_NONE) return fail(BDF_INVALID, "unknown keep %d", keep);
+    TRY(setop_check(n_keys, keys, nullptr, false));
+    return setop_mask(c, keep, n_keys, keys, nullptr, mask);
+}
+
+int bdf_set_op_dev(bdf_ctx* c, int32_t op, int32_t n_keys, const bdf_col* const* left, const bdf_col* const* right, bdf_col** mask) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "set operations move rows between chunks: use a one-GPU context (bdf_init) for them");
+    ENTER(c);
+    if (!mask) return fail(BDF_INVALID, "null argument");
+    if (op < BDF_SETOP_INTERSECT || op > BDF_SETOP_EXCEPT_ALL) return fail(BDF_INVALID, "unknown set operation %d", op);
+    TRY(setop_check(n_keys, left, right, true));
+    return setop_mask(c, 3 + op, n_keys, left, right, mask);
+}
+
+int bdf_bool_widen_dev(bdf_ctx* c, const bdf_col* in, bdf_col** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "use a one-GPU context (bdf_init) for the Boolean widening");
+    ENTER(c);
+    if (!in || !out) return fail(BDF_INVALID, "null argument");
+    if (in->dtype != kBool) return fail(BDF_UNSUPPORTED, "the widening takes a Boolean column");
+    return bool_widen(c, in, out);
+}
+
+int bdf_concat_dev(bdf_ctx* c, int32_t n, const bdf_col* const* cols, bdf_col** out) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "concat moves chunks between columns: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return concat_dev(c, n, cols, out);
+}
+
+int bdf_list_concat_dev(bdf_ctx* c, int32_t n, const bdf_list* const* lists, bdf_list** out) {
+    LIST_ENTER(c);
+    return list_concat(c, n, lists, out);
 }
 
 }  // extern "C"

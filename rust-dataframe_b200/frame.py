@@ -152,6 +152,46 @@ def join_asof(other: "DeviceFrame", left_on: str, right_on: Optional[str] = None
 EXISTENCE_JOINS = ("left_semi", "left_anti")
 
 
+def distinct(subset: Optional[Sequence[str]] = None, keep="first"):
+    """DeviceFrame.drop_duplicates(subset, keep) as a step; distinct() is drop_duplicates() over every column."""
+    return ("distinct", (None if subset is None else list(subset), keep))
+
+
+SET_OPS = ("union", "union_by_name", "intersect", "intersect_all", "subtract", "except_all")
+
+
+def set_op(other: "DeviceFrame", op: str):
+    """One of SET_OPS against `other` as a step (the DeviceFrame method of that name)."""
+    return ("set_op", (other, op))
+
+
+def plan_set_op(schema_a: Dict[str, int], schema_b: Dict[str, int], op: str) -> List[Tuple[str, int]]:
+    """The schema of a union / set operation: a's names and types.  The columns pair up by position (by name for union_by_name,
+    whose name sets must be equal) and each pair must have one dtype: else UnsupportedType with Spark's text.  Every operation but
+    the unions compares all the columns, so a list column there, or more than 16 columns (the limit of group-by and join), is
+    UnsupportedType too."""
+    if op not in SET_OPS:
+        raise N.UnsupportedType(f"set operation {op!r} is not one of {list(SET_OPS)}")
+    if len(schema_a) != len(schema_b) or (op == "union_by_name" and set(schema_a) != set(schema_b)):
+        raise N.UnsupportedType("Union can only be performed on tables with compatible column types")
+    pairs = [(t, schema_b[n]) for n, t in schema_a.items()] if op == "union_by_name" else list(zip(schema_a.values(), schema_b.values()))
+    if any(a != b for a, b in pairs):
+        raise N.UnsupportedType("Union can only be performed on tables with compatible column types")
+    if op not in ("union", "union_by_name"):
+        _check_compared(schema_a, list(schema_a), op)
+    return list(schema_a.items())
+
+
+def _check_compared(schema: Dict[str, int], names: Sequence[str], what: str) -> None:
+    if not 1 <= len(names) <= 16:
+        raise N.UnsupportedType(f"{what} compares 1..16 columns (the limit of group-by and join), not {len(names)}")
+    for n in names:
+        if n not in schema:
+            raise N.ReferencePanic(f"column {n!r} not found (column_by_name panics)")
+        if schema[n] >= N.LIST_BASE:
+            raise N.UnsupportedType(f"column {n!r} is a list column: {what} compares numeric, Boolean and temporal columns only")
+
+
 def plan_join(schema_a: Dict[str, int], schema_b: Dict[str, int], criteria: Sequence[Tuple[str, str]], how: Optional[str] = None) -> List[Tuple[str, int]]:
     """The joined schema `Dataset::try_join` (expression.rs:223-287) plans for `criteria` ([(column of a, column of b)]), as
     [(name, dtype)]: a's columns, then b's; a name present on both sides becomes `a.<name>` / `b.<name>`.  Its checks in its
@@ -260,7 +300,8 @@ def _filter_columns(cond) -> set:
 # ---------------------------------------------------------------------------------------------------------
 # the optimiser pass: which Calculations can be evaluated in one fused step
 
-def _columns_read(t) -> set:
+def _columns_read(t, schema: Optional[Dict[str, int]] = None) -> set:
+    """The columns step t reads; `schema` (the frame's before the step) names them for the steps that read every column."""
     kind, arg = t
     if kind == "calculate":
         return set(arg.inputs)
@@ -274,11 +315,16 @@ def _columns_read(t) -> set:
         return set(_window_columns(*arg))
     if kind == "join_asof":
         return {arg[1]} | {a for a, _ in arg[3]}
+    if kind == "distinct":   # the compared columns: the subset, or every column of the frame
+        return set(schema or ()) if arg[0] is None else set(arg[0])
+    if kind == "set_op":     # the left frame's columns are compared (or, for the unions, carried) by position
+        return set(schema or ())
     return set()
 
 
-def _needed_after(transformations: Sequence[tuple], final_columns: Sequence[str]) -> List[set]:
-    """needed[i] = names whose VALUES can still be observed after step i (read by a later step or present at the end)."""
+def _needed_after(transformations: Sequence[tuple], final_columns: Sequence[str], schemas: Optional[Sequence[Dict[str, int]]] = None) -> List[set]:
+    """needed[i] = names whose VALUES can still be observed after step i (read by a later step or present at the end).  schemas[i]:
+    the schema before step i (_schema_walk), for the steps that read every column."""
     needed = [set() for _ in transformations]
     live = set(final_columns)
     for i in range(len(transformations) - 1, -1, -1):
@@ -296,7 +342,7 @@ def _needed_after(transformations: Sequence[tuple], final_columns: Sequence[str]
         elif kind == "window":                                  # its DivideByZero panic is observable
             live = (live - {c[0] for c in arg[2]}) | _columns_read(transformations[i])   # the outputs are new columns
         else:
-            live = live | _columns_read(transformations[i])
+            live = live | _columns_read(transformations[i], schemas[i] if schemas else None)
     return needed
 
 
@@ -330,6 +376,16 @@ def _schema_walk(schema: "OrderedDict[str, int]", transformations: Sequence[tupl
                 cur = OrderedDict(plan_window(cur, *arg))
             except N.ArrowError:
                 cur = OrderedDict()
+        elif kind == "set_op":
+            try:
+                cur = OrderedDict(plan_set_op(cur, arg[0].schema, arg[1]))
+            except N.ArrowError:
+                cur = OrderedDict()
+        elif kind == "distinct":   # the rows change, the schema does not
+            try:
+                _check_compared(cur, list(cur) if arg[0] is None else arg[0], "drop_duplicates")
+            except N.ArrowError:
+                cur = OrderedDict()
     out.append(cur)
     return out
 
@@ -349,9 +405,10 @@ def plan_fusion(schema: "OrderedDict[str, int]", transformations: Sequence[tuple
     ``fuse_casts`` also folds a cast TO Float64 into the fused load (one pass instead of a cast launch plus the chain)."""
     steps = list(transformations)
     schemas = _schema_walk(schema, steps)
-    needed = _needed_after(steps, list(schemas[-1].keys()))
+    needed = _needed_after(steps, list(schemas[-1].keys()), schemas)
     for i, (kind, _) in enumerate(steps):
-        if kind in ("join", "join_asof"):   # every column of the frame reaches the joined frame (perhaps renamed): all are observable
+        if kind in ("join", "join_asof", "set_op") or (kind == "distinct" and steps[i][1][0] is None):
+            # every column of the frame reaches the joined frame (perhaps renamed), or is compared: all are observable
             for j in range(i):
                 needed[j] |= set(schemas[i])
     out: List[tuple] = []
@@ -713,6 +770,103 @@ class DeviceFrame:
             ri.free()
         return DeviceFrame(OrderedDict((name, c) for (name, _), c in zip(plan, cols)))
 
+    # -- distinct rows and set operations (include/b200df.h "distinct rows and set operations") --
+    def _compared(self, subset: Optional[Sequence[str]], what: str) -> List[Column]:
+        names = list(self.columns) if subset is None else list(subset)
+        _check_compared(self.schema, names, what)
+        return [self.columns[n] for n in names]
+
+    def duplicated(self, subset: Optional[Sequence[str]] = None, keep="first") -> Column:
+        """pandas' duplicated: a Boolean Column without nulls, true for the rows that repeat an earlier row of `subset` (default:
+        every column) with keep="first", a later one with "last", or any other one with False.  Nulls equal each other, all NaNs
+        are one value and -0.0 == 0.0.  At most 16 compared columns (the limit of group-by and join); no list columns."""
+        from .functions import duplicated
+
+        return duplicated(self._compared(subset, "duplicated"), keep)
+
+    def drop_duplicates(self, subset: Optional[Sequence[str]] = None, keep="first") -> "DeviceFrame":
+        """pandas' drop_duplicates / Spark's dropDuplicates: the rows duplicated() does not mark, every column (list, Boolean and
+        temporal columns included) filtered, in row order."""
+        from .functions import duplicated
+
+        mask = duplicated(self._compared(subset, "drop_duplicates"), keep)
+        return self._keep(mask, invert=True)
+
+    def distinct(self) -> "DeviceFrame":
+        """Spark's distinct: drop_duplicates() over every column (at most 16, none of them a list column)."""
+        return self.drop_duplicates()
+
+    def _keep(self, mask: Column, invert: bool = False) -> "DeviceFrame":
+        from .functions import filter_any
+
+        out: "OrderedDict[str, Column]" = OrderedDict()
+        try:
+            m = mask.logical_not() if invert else mask
+            try:
+                for n, c in self.columns.items():
+                    out[n] = filter_any(c, m)
+            finally:
+                if invert:
+                    m.free()
+        except BaseException:
+            for c in out.values():   # the columns filtered before the failure
+                c.free()
+            raise
+        finally:
+            mask.free()
+        return DeviceFrame(out)
+
+    def _check_temporal(self, other: "DeviceFrame", pairs: Sequence[Tuple[str, str]]) -> None:
+        for a, b in pairs:
+            ta, tb = getattr(self.columns[a], "temporal", None), getattr(other.columns[b], "temporal", None)
+            if ta != tb:
+                raise N.UnsupportedType(f"Union can only be performed on tables with compatible column types ({a!r}: {ta!r}, {b!r}: {tb!r})")
+
+    def _pairs(self, other: "DeviceFrame", op: str) -> List[Tuple[str, str]]:
+        plan_set_op(self.schema, other.schema, op)
+        pairs = [(n, n) for n in self.columns] if op == "union_by_name" else list(zip(self.columns, other.columns))
+        self._check_temporal(other, pairs)
+        return pairs
+
+    def union(self, other: "DeviceFrame") -> "DeviceFrame":
+        """Spark's union (UNION ALL): this frame's chunks, then other's, column by column by position (bdf_concat_dev); the names
+        are this frame's.  The types at every position must be equal (no widening), temporal types included."""
+        return self._union(other, "union")
+
+    def union_by_name(self, other: "DeviceFrame") -> "DeviceFrame":
+        """Spark's unionByName: union with other's columns matched by name (both frames must have the same names)."""
+        return self._union(other, "union_by_name")
+
+    def _union(self, other: "DeviceFrame", op: str) -> "DeviceFrame":
+        from .functions import concat
+
+        pairs = self._pairs(other, op)
+        return DeviceFrame(OrderedDict((a, concat([self.columns[a], other.columns[b]])) for a, b in pairs))
+
+    def _set_op(self, other: "DeviceFrame", op: str, native: str) -> "DeviceFrame":
+        from .functions import set_op_mask
+
+        pairs = self._pairs(other, op)
+        mask = set_op_mask([self.columns[a] for a, _ in pairs], [other.columns[b] for _, b in pairs], native)
+        return self._keep(mask)
+
+    def intersect(self, other: "DeviceFrame") -> "DeviceFrame":
+        """Spark's intersect: the distinct rows of this frame that other also has (the first copy of each, in row order).  The
+        columns are compared by position; nulls equal each other, all NaNs are one value and -0.0 == 0.0.  At most 16 columns."""
+        return self._set_op(other, "intersect", "intersect")
+
+    def intersect_all(self, other: "DeviceFrame") -> "DeviceFrame":
+        """Spark's intersectAll: of every row value present l times here and r times in other, the first min(l, r) copies."""
+        return self._set_op(other, "intersect_all", "intersect_all")
+
+    def subtract(self, other: "DeviceFrame") -> "DeviceFrame":
+        """Spark's subtract (EXCEPT DISTINCT): the distinct rows of this frame that other does not have, the first copy of each."""
+        return self._set_op(other, "subtract", "except")
+
+    def except_all(self, other: "DeviceFrame") -> "DeviceFrame":
+        """Spark's exceptAll: of every row value present l times here and r times in other, the first max(l - r, 0) copies."""
+        return self._set_op(other, "except_all", "except_all")
+
     def window(self, partition_by: Sequence[str], order_by: Sequence[Tuple[str, bool]], calls: Sequence[tuple]) -> "DeviceFrame":
         """Window functions over one specification (bdf_window_dev, one sort for all calls): every call ``(output, function,
         *arguments)`` adds its column as with_column does (an existing name is replaced); the other columns are untouched."""
@@ -813,6 +967,10 @@ class DeviceFrame:
                 frame = frame.join_asof(*arg)
             elif kind == "window":
                 frame = frame.window(*arg)
+            elif kind == "distinct":
+                frame = frame.drop_duplicates(*arg)
+            elif kind == "set_op":
+                frame = getattr(frame, arg[1])(arg[0])
             elif kind == "group_aggregate":
                 raise N.ReferencePanic("aggregations not supported")       # evaluation.rs:73
             else:

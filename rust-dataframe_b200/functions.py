@@ -1165,6 +1165,93 @@ def join_asof_indices(left_on: "Column", right_on: "Column", left_by: Sequence["
     return Column(ctx, h)
 
 
+_KEEP = {"first": N.KEEP_FIRST, "last": N.KEEP_LAST, False: N.KEEP_NONE}
+MAX_SET_KEYS = 16   # the key limit of group-by and join
+
+
+def _set_keys(keys: Sequence["Column"], what: str) -> None:
+    if not 1 <= len(keys) <= MAX_SET_KEYS:
+        raise N.UnsupportedType(f"{what} compares 1..{MAX_SET_KEYS} columns (the limit of group-by and join), not {len(keys)}")
+    if any(isinstance(k, ListColumn) for k in keys):
+        raise N.UnsupportedType(f"a list column cannot be compared by {what}: the compared columns must be numeric or Boolean")
+
+
+def duplicated(keys: Sequence["Column"], keep="first") -> "Column":
+    """pandas' duplicated over the rows of `keys` (bdf_duplicated_dev): a Boolean Column without nulls, chunked like the keys, true
+    for every row of a run of equal rows except its first ("first"), except its last ("last"), or for every row of a run longer
+    than one (False).  Nulls equal each other, all NaNs are one value and -0.0 == 0.0 (group-by's equality); Boolean keys are
+    allowed."""
+    if not (keep is False or (isinstance(keep, str) and keep in ("first", "last"))):
+        raise N.UnsupportedType(f"keep must be 'first', 'last' or False, not {keep!r}")
+    _set_keys(keys, "duplicated")
+    ctx = keys[0].ctx
+    ks = (C.c_void_p * len(keys))(*[k.handle for k in keys])
+    h = C.c_void_p()
+    N.raise_for_status(N.lib().bdf_duplicated_dev(ctx.handle, len(keys), ks, _KEEP[keep], C.byref(h)))
+    return Column(ctx, h)
+
+
+def set_op_mask(left: Sequence["Column"], right: Sequence["Column"], op: str) -> "Column":
+    """The rows of `left` a set operation keeps (bdf_set_op_dev), as a Boolean Column over the left rows, chunked like left[0]:
+    op is "intersect", "intersect_all", "except" (Spark's subtract) or "except_all".  In a run of equal rows with cl left and cr
+    right rows, the run keeps its first min(cl, cr) ("intersect_all"), max(cl - cr, 0) ("except_all"), one if cr > 0
+    ("intersect") or one if cr == 0 ("except") left rows in row order.  Equality is duplicated's."""
+    if op not in N.SET_OPS:
+        raise N.UnsupportedType(f"set operation {op!r} is not one of {sorted(N.SET_OPS)}")
+    if len(left) != len(right):
+        raise N.UnsupportedType("Union can only be performed on tables with the same number of columns")
+    _set_keys(left, op)
+    _set_keys(right, op)
+    for a, b in zip(left, right):
+        if a.dtype != b.dtype or getattr(a, "temporal", None) != getattr(b, "temporal", None):
+            raise N.UnsupportedType("Union can only be performed on tables with compatible column types")
+    ctx = left[0].ctx
+    lk = (C.c_void_p * len(left))(*[k.handle for k in left])
+    rk = (C.c_void_p * len(right))(*[k.handle for k in right])
+    h = C.c_void_p()
+    N.raise_for_status(N.lib().bdf_set_op_dev(ctx.handle, N.SET_OPS[op], len(left), lk, rk, C.byref(h)))
+    return Column(ctx, h)
+
+
+def filter_any(column, mask: "Column"):
+    """column.filter(mask) for every kind of column: a Boolean column goes through the filter as UInt8 (bdf_bool_widen_dev) and comes
+    back through a != 0 comparison, nulls kept; a ListColumn uses its own filter."""
+    if isinstance(column, ListColumn) or column.dtype != N.BOOL:
+        return column.filter(mask)
+    h = C.c_void_p()
+    N.raise_for_status(N.lib().bdf_bool_widen_dev(column.ctx.handle, column.handle, C.byref(h)))
+    wide = Column(column.ctx, h)
+    try:
+        kept = wide.filter(mask)
+    finally:
+        wide.free()
+    try:
+        return kept.ne(0)
+    finally:
+        kept.free()
+
+
+def concat(columns: Sequence) -> "Column":
+    """pandas' concat of columns (bdf_concat_dev / bdf_list_concat_dev): the chunks of columns[0], then those of columns[1], and so
+    on, copied on the device.  The columns must have one dtype and one temporal type; ListColumns concatenate with ListColumns."""
+    columns = list(columns)
+    if not columns:
+        raise N.ComputeError("concat needs at least one column")
+    if any(isinstance(c, ListColumn) for c in columns):
+        if not all(isinstance(c, ListColumn) for c in columns):
+            raise N.UnsupportedType("a list column concatenates only with list columns")
+        return ListColumn.concat(columns)
+    dtypes = {c.dtype for c in columns}
+    tags = {getattr(c, "temporal", None) for c in columns}
+    if len(dtypes) != 1 or len(tags) != 1:
+        raise N.UnsupportedType("Union can only be performed on tables with compatible column types")
+    ctx = columns[0].ctx
+    cs = (C.c_void_p * len(columns))(*[c.handle for c in columns])
+    h = C.c_void_p()
+    N.raise_for_status(N.lib().bdf_concat_dev(ctx.handle, len(columns), cs, C.byref(h)))
+    return Column(ctx, h, tags.pop())
+
+
 _INT64_MIN, _INT64_MAX = -2 ** 63, 2 ** 63 - 1
 _TIMESTAMP_UNIT_US = (10 ** 6, 1000, 1)   # microseconds per arrow TimeUnit s, ms, us (ns: x 1000)
 
@@ -1504,6 +1591,20 @@ class ListColumn:
     def filter(self, mask: "Column") -> "ListColumn":
         """ChunkedArray::filter of whole lists: the lists where the Boolean mask is valid and true, chunk by chunk."""
         return self._list(N.lib().bdf_list_filter_dev, self.handle, mask.handle)
+
+    @staticmethod
+    def concat(lists: Sequence["ListColumn"]) -> "ListColumn":
+        """The chunks of lists[0], then those of lists[1], and so on, copied on the device (bdf_list_concat_dev); one element type."""
+        lists = list(lists)
+        if not lists:
+            raise N.ComputeError("concat needs at least one list column")
+        if len({l.dtype for l in lists}) != 1:
+            raise N.UnsupportedType("Union can only be performed on tables with compatible column types")
+        ctx = lists[0].ctx
+        ls = (C.c_void_p * len(lists))(*[l.handle for l in lists])
+        h = C.c_void_p()
+        N.raise_for_status(N.lib().bdf_list_concat_dev(ctx.handle, len(lists), ls, C.byref(h)))
+        return ListColumn(ctx, h)
 
     def explode(self):
         """(UInt32 parent row numbers, values): one row per element of every valid list; null and empty lists give none."""
