@@ -307,6 +307,23 @@ typedef struct { const bdf_col* column; int32_t descending; } bdf_sort_key;
 int  bdf_sort_indices_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_sort_key* keys, bdf_col** indices);
 int  bdf_take_dev(bdf_ctx* ctx, const bdf_col* values, const bdf_col* indices, bdf_col** out);
 
+/* ---- top-k: DataFrame::sort followed by limit (SQL's ORDER BY ... LIMIT k, pandas' nsmallest / nlargest) -------------------
+ * bdf_top_k_indices_dev  The first min(k, n) row numbers of bdf_sort_indices_dev(ctx, n_keys, keys), bit for bit, for every input:
+ *                        the same criteria, stability, directions, nulls last, NaN greatest and -0.0 == 0.0.  Result: one UInt32
+ *                        chunk without nulls.  The sort's errors, statuses and messages in the sort's order (a multi-GPU context,
+ *                        null arguments, "Sort criteria cannot be empty", non-numeric criteria, different lengths, more than
+ *                        2^32-1 rows); then k < 0 -> BDF_INVALID.  k == 0 gives an empty column; k >= n the whole sort.
+ * Path.  When k > 5n / 8 the call runs the full sort and keeps its first k entries.  Otherwise it chooses the k rows without sorting
+ *   all of them: one round per criterion finds the threshold key of the rows still to choose with the radix select of the exact
+ *   percentiles, marks the rows before it as chosen and the rows equal to it as the next round's tie set; the first ties in row order
+ *   fill the rest.  Only the k chosen rows are then gathered and sorted.  The crossover was measured on an H100 (DESIGN §8).
+ * Memory (k <= 5n / 8).  Two bitmaps over n rows and a UInt32 iota (4.25 B/row), the select's candidate scratch (at most the
+ *   criterion's key width per valid row, usually far less), and for a tie set of m rows its row ids and one gathered criterion
+ *   (at most 16 B per tie row); then the k-row gathers and sort.  The full sort takes 24 B/row of scratch.
+ * Launch records: BDF_K_SELECT (threshold passes, marks and the tie prefix), BDF_K_FILTER (compactions), BDF_K_TAKE (gathers),
+ *   BDF_K_SORT (the sort of the k chosen rows, or of all rows above the crossover). */
+int  bdf_top_k_indices_dev(bdf_ctx* ctx, int32_t n_keys, const bdf_sort_key* keys, int64_t k, bdf_col** indices);
+
 /* ---- group-by aggregate (the tail of SURVEY 8(f) N4: `Transformation::GroupAggregate`, a panic! in the reference,
  * src/evaluation.rs:73; its intended shape is src/expression.rs:114-221) ---------------------------------------------------
  * Rows are grouped by ONE numeric key column; every value column is folded per group with the aggregates of

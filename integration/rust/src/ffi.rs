@@ -252,6 +252,7 @@ extern "C" {
     pub fn bdf_col_free(ctx: *mut BdfCtx, col: *mut BdfCol);
     // DataFrame::sort
     pub fn bdf_sort_indices_dev(ctx: *mut BdfCtx, n_keys: i32, keys: *const BdfSortKey, indices: *mut *mut BdfCol) -> c_int;
+    pub fn bdf_top_k_indices_dev(ctx: *mut BdfCtx, n_keys: i32, keys: *const BdfSortKey, k: i64, indices: *mut *mut BdfCol) -> c_int;
     pub fn bdf_take_dev(ctx: *mut BdfCtx, values: *const BdfCol, indices: *const BdfCol, out: *mut *mut BdfCol) -> c_int;
     // group-by aggregate (Transformation::GroupAggregate, src/evaluation.rs:73; planned shape src/expression.rs:114-221)
     pub fn bdf_group_aggregate_dev(ctx: *mut BdfCtx, key: *const BdfCol, n_values: i32, values: *const *const BdfCol, out_keys: *mut *mut BdfCol,

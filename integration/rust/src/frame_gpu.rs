@@ -81,6 +81,25 @@ pub fn sort_device(frame: &DeviceColumns, criteria: &[(usize, bool)]) -> Result<
     Ok(out)
 }
 
+/// DataFrame::sort followed by DataFrame::limit(k) as one call: the first k rows of the sort, chosen on the device without sorting every
+/// row (bdf_top_k_indices_dev), then every column taken at them.  A negative k gives no rows, as limit does.
+pub fn top_k_device(frame: &DeviceColumns, criteria: &[(usize, bool)], k: i64) -> Result<DeviceColumns, String> {
+    if criteria.is_empty() {
+        return Err("Sort criteria cannot be empty".to_string());
+    }
+    let keys: Vec<BdfSortKey> = criteria.iter().map(|(c, d)| BdfSortKey { column: frame.cols[*c], descending: *d as i32 }).collect();
+    let mut indices: *mut BdfCol = std::ptr::null_mut();
+    check(unsafe { bdf_top_k_indices_dev(dev(), keys.len() as i32, keys.as_ptr(), k.max(0), &mut indices) })?;
+    let idx = DeviceColumns { names: vec![], cols: vec![indices] };
+    let mut out = DeviceColumns { names: frame.names.clone(), cols: Vec::with_capacity(frame.cols.len()) };
+    for c in &frame.cols {
+        let mut taken: *mut BdfCol = std::ptr::null_mut();
+        check(unsafe { bdf_take_dev(dev(), *c, idx.cols[0], &mut taken) })?;
+        out.cols.push(taken);
+    }
+    Ok(out)
+}
+
 /// Column::take of one column of a frame, as sort / join / limit call it: a DataType::List column goes through bdf_list_take_dev (whole
 /// lists, one chunk; a null index gives a null list), every other column through bdf_take_dev.  ChunkedArray::filter dispatches the same
 /// way to bdf_list_filter_dev, which keeps the chunks, so list chunk b stays RecordBatch b for to_arrow (bdf_ipc_write_lists).

@@ -18,11 +18,11 @@ from .parquet_reader import ParquetFile, write_parquet
 from . import frame
 from .frame import DeviceFrame, plan_aggregate, plan_fusion, plan_join, plan_set_op, plan_window
 from .functions import (AggFuture, AggregateFunctions, ArrayFunctions, Column, ListColumn, ScalarFunctions, CaseWhen, cast, coalesce, concat, duplicated, eval_expr, eval_expr_agg, group_aggregate, group_by, join_asof_indices, join_indices,
-                        greatest, hist_density, least, moments_merge, moments_stat, nanvl, sort_columns, set_op_mask, sort_indices, temporal_result, when, window)
+                        greatest, hist_density, least, moments_merge, moments_stat, nanvl, sort_columns, set_op_mask, sort_indices, temporal_result, top_k_indices, when, window)
 
 __all__ = [
     "native", "ArrowError", "ComputeError", "Context", "DivideByZero", "ParseError", "ReferencePanic", "UnsupportedType",
-    "default_context", "PrimitiveArray", "BooleanArray", "ListArray", "ScalarFunctions", "AggregateFunctions", "ArrayFunctions", "Column", "ListColumn", "AggFuture", "cast", "eval_expr", "eval_expr_agg", "group_aggregate", "group_by", "join_indices", "join_asof_indices", "sort_indices", "sort_columns", "IpcFile", "CsvFile", "JsonFile", "ParquetFile", "write_parquet", "write_csv", "write_ipc", "write_ipc_host", "frame", "DeviceFrame", "plan_aggregate", "plan_fusion", "plan_join", "plan_set_op", "plan_window", "concat", "duplicated", "set_op_mask", "window", "moments_stat", "moments_merge", "hist_density",
+    "default_context", "PrimitiveArray", "BooleanArray", "ListArray", "ScalarFunctions", "AggregateFunctions", "ArrayFunctions", "Column", "ListColumn", "AggFuture", "cast", "eval_expr", "eval_expr_agg", "group_aggregate", "group_by", "join_indices", "join_asof_indices", "sort_indices", "sort_columns", "top_k_indices", "IpcFile", "CsvFile", "JsonFile", "ParquetFile", "write_parquet", "write_csv", "write_ipc", "write_ipc_host", "frame", "DeviceFrame", "plan_aggregate", "plan_fusion", "plan_join", "plan_set_op", "plan_window", "concat", "duplicated", "set_op_mask", "window", "moments_stat", "moments_merge", "hist_density",
     "TemporalType", "temporal_result", "coalesce", "greatest", "least", "nanvl", "when", "CaseWhen",
     "I8", "I16", "I32", "I64", "U8", "U16", "U32", "U64", "F32", "F64", "NP_DTYPES", "DTYPE_NAMES", "dtype_of", "width_of",
 ]

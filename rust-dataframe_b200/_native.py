@@ -281,6 +281,7 @@ def lib() -> C.CDLL:
         "bdf_eval_expr_agg_dev": ([vp, i32, P(vp), i32, P(ExprNode), P(vp), P(Agg4)], C.c_int),
         "bdf_eval_expr_agg_dev_async": ([vp, i32, P(vp), i32, P(ExprNode), P(vp), P(vp)], C.c_int),
         "bdf_sort_indices_dev": ([vp, i32, P(SortKeyC), P(vp)], C.c_int),
+        "bdf_top_k_indices_dev": ([vp, i32, P(SortKeyC), i64, P(vp)], C.c_int),
         "bdf_take_dev": ([vp, vp, vp, P(vp)], C.c_int),
         "bdf_group_aggregate_dev": ([vp, vp, i32, P(vp), P(vp), P(GroupOut), P(i64)], C.c_int),
         "bdf_group_by_dev": ([vp, i32, P(vp), i32, P(GroupAggC), P(vp), P(vp), P(i64)], C.c_int),
@@ -389,7 +390,7 @@ EXPORTED_SYMBOLS = [
     "bdf_host_alloc", "bdf_host_free", "bdf_host_register", "bdf_host_unregister", "bdf_binary", "bdf_unary", "bdf_cast",
     "bdf_aggregate", "bdf_aggregate_all", "bdf_avg", "bdf_upload", "bdf_upload_many", "bdf_col_wait", "bdf_col_describe",
     "bdf_col_chunk_info", "bdf_binary_dev", "bdf_unary_dev", "bdf_cast_dev", "bdf_aggregate_dev",
-    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_group_by_lists_dev", "bdf_join_indices_dev", "bdf_join_asof_dev", "bdf_duplicated_dev", "bdf_set_op_dev", "bdf_concat_dev", "bdf_list_concat_dev", "bdf_bool_widen_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_rowwise_dev", "bdf_case_when_dev", "bdf_null_test_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
+    "bdf_aggregate_all_dev", "bdf_avg_dev", "bdf_expr_check", "bdf_eval_expr_dev", "bdf_eval_expr_agg_dev", "bdf_eval_expr_agg_dev_async", "bdf_sort_indices_dev", "bdf_top_k_indices_dev", "bdf_take_dev", "bdf_group_aggregate_dev", "bdf_group_by_dev", "bdf_group_by_lists_dev", "bdf_join_indices_dev", "bdf_join_asof_dev", "bdf_duplicated_dev", "bdf_set_op_dev", "bdf_concat_dev", "bdf_list_concat_dev", "bdf_bool_widen_dev", "bdf_window_dev", "bdf_compare_dev", "bdf_boolean_dev", "bdf_filter_dev", "bdf_rowwise_dev", "bdf_case_when_dev", "bdf_null_test_dev", "bdf_download", "bdf_download_begin", "bdf_download_end",
     "bdf_binary_agg_dev", "bdf_binary_agg_dev_async", "bdf_aggregate_all_dev_async", "bdf_future_wait", "bdf_col_free", "bdf_profile_enable", "bdf_profile_read",
     "bdf_launch_count", "bdf_timer_start", "bdf_timer_stop", "bdf_flush_l2", "bdf_generate",
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",

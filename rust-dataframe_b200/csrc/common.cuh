@@ -475,6 +475,16 @@ cudaError_t launch_join_asof(int n_by, const int* dtypes, const void* const* pro
                              long long n_probe, const uint32_t* run_starts, long long n_runs, long long n_build, const uint32_t* perm, uint32_t* out,
                              uint32_t* out_valid, cudaStream_t s);
 
+// Top-k (k_topk.cu).  chunks: topk_chunk_size() bytes each, filled by fill_topk_chunk, tiles of topk_tile_elems(dtype) elements.
+// ids: the row of every tie-set position (gathered rounds) or null (positional).  tie and counts[0..1] are zeroed by the caller.
+int topk_chunk_size();
+int topk_tile_elems(int dtype);
+void fill_topk_chunk(void* descs, int64_t i, const void* values, const uint32_t* validity, int64_t len, int64_t tile0, int64_t row0, int bit_off,
+                     bool owns_words);
+cudaError_t launch_topk_mark(int dtype, const void* chunks, int n_chunks, int64_t tiles, unsigned long long t, bool all_valid, bool descending,
+                             const uint32_t* ids, uint32_t* chosen, uint32_t* tie, unsigned long long* counts, int sm_count, cudaStream_t s);
+cudaError_t launch_topk_choose(const uint32_t* ids, long long count, uint32_t* chosen, cudaStream_t s);
+
 // Distinct rows and set operations (k_setop.cu).  heads: {head words, per-word run prefix, run starts} of the sorted positions.
 // mode: 0..2 bdf_keep (duplicated), 3 + bdf_setop.  words: one bit per output row at the row's original position, zeroed by the caller.
 cudaError_t launch_setop_left_count(const void* const* heads, long long n_runs, long long n, const uint32_t* perm, long long n_left,

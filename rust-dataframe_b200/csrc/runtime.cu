@@ -1898,7 +1898,8 @@ static int sort_table(bdf_ctx* c, const bdf_col* col, void** dev, int* n_chunks,
     return BDF_OK;
 }
 
-static int sort_indices_dev(bdf_ctx* c, int n_keys, const bdf_sort_key* keys, bdf_col** out) {
+// The checks of the sort's criteria, shared with top-k.
+static int sort_check(int n_keys, const bdf_sort_key* keys) {
     if (n_keys < 1) return fail(BDF_INVALID, "Sort criteria cannot be empty");
     for (int k = 0; k < n_keys; k++) {
         if (!keys[k].column) return fail(BDF_INVALID, "null sort column");
@@ -1906,8 +1907,13 @@ static int sort_indices_dev(bdf_ctx* c, int n_keys, const bdf_sort_key* keys, bd
         if (dt < 0 || dt >= BDF_NTYPES) return fail(BDF_UNSUPPORTED, "sort criteria must be numeric columns");
         if (keys[k].column->total_len != keys[0].column->total_len) return fail(BDF_LENGTH_MISMATCH, "sort columns have different lengths");
     }
+    if (keys[0].column->total_len > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
+    return BDF_OK;
+}
+
+static int sort_indices_dev(bdf_ctx* c, int n_keys, const bdf_sort_key* keys, bdf_col** out) {
+    TRY(sort_check(n_keys, keys));
     const int64_t n = keys[0].column->total_len;
-    if (n > 0xffffffffLL) return fail(BDF_UNSUPPORTED, "sort indices are UInt32: at most 2^32-1 rows");
     ColOwner o(c);
     TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, sort_tile_elems(), o.out()));
     cudaError_t e = cudaSuccess;
@@ -2008,6 +2014,139 @@ static int take_dev(bdf_ctx* c, const bdf_col* values, const bdf_col* indices, b
     if (flag) return fail(BDF_INVALID, "take: index out of bounds");
     *out = o.release();
     return BDF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// top-k = the first k rows of DataFrame::sort, chosen by a radix select of the sort keys (k_topk.cu)
+//   Rounds, one per criterion, over a tie set (round 0: every row; later: the ascending row ids that tie on every earlier criterion)
+//   and `need`, the rows still to choose.  select_keys finds the key t of rank need - 1 (ascending) or v - need (descending) among
+//   the v valid keys of the tie set; k_topk_mark ORs the rows before t into the chosen bitmap and marks the rows equal to t.  When
+//   need > v every valid row is chosen and the nulls are the ties.  Once the ties hold exactly the rows still needed, or the last
+//   criterion is reached, the first `need` ties in row order are chosen: rows equal on every criterion keep row order, as in the
+//   stable sort.  The chosen rows (ascending) are then sorted on their gathered criteria and mapped back.
+
+static int select_keys(bdf_ctx* c, const bdf_col* col, const std::function<std::vector<int64_t>(int64_t)>& ranks_of, int max_targets,
+                       std::vector<uint64_t>* keys, int64_t* n_valid);
+
+// k above this share of the rows: one sort of all rows costs less than the rounds plus a sort of k rows (DESIGN §8).
+constexpr int64_t kTopkSortNum = 5, kTopkSortDen = 8;
+
+// A Boolean column over a bitmap the caller owns (bit 0 is row 0).
+static int bits_borrow(uint32_t* words, int64_t n, bdf_col** out) { return col_borrow(kBool, {DevChunk{(char*)words, nullptr, n, 0, 0}}, out); }
+
+// One mark pass over col: positional (ids null: the tie set is every row, chunk by chunk) or over one gathered chunk whose position i
+// is row ids[i].  tie: a bitmap over col's positions.  counts: BEFORE, TIE.
+static int topk_mark(bdf_ctx* c, const bdf_col* col, const uint32_t* ids, uint64_t t, bool all_valid, bool descending, uint32_t* chosen, uint32_t* tie,
+                     unsigned long long* d_counts, int64_t counts[2]) {
+    const int64_t nch = (int64_t)col->chunks.size(), n = col->total_len;
+    const int tile = topk_tile_elems(col->dtype);
+    void *hp = nullptr, *dp = nullptr;
+    TRY(ring_alloc(c, (size_t)std::max<int64_t>(nch, 1) * topk_chunk_size(), &hp, &dp));
+    int64_t tiles = 0, row0 = 0;
+    for (int64_t i = 0; i < nch; i++) {
+        const DevChunk& ch = col->chunks[i];
+        const int64_t end = row0 + ch.len;
+        fill_topk_chunk(hp, i, ch.values, ch.validity, ch.len, tiles, row0, ch.bit_off, row0 % 32 == 0 && (end % 32 == 0 || end == n));
+        tiles += (ch.len + tile - 1) / tile;
+        row0 = end;
+    }
+    wait_groups(c->s_compute, col, 0, nch);
+    CK(desc_upload(c, dp, hp, (size_t)std::max<int64_t>(nch, 1) * topk_chunk_size()));
+    const int64_t n_words = (n + 31) / 32;
+    CK(cudaMemsetAsync(tie, 0, (size_t)n_words * 4, c->s_compute));
+    CK(cudaMemsetAsync(d_counts, 0, 2 * sizeof(unsigned long long), c->s_compute));
+    {
+        LaunchTimer lt(c, BDF_K_SELECT, col->dtype, n, reduce_bytes(col, 0, nch) + 2 * n_words * 4);
+        CK(launch_topk_mark(col->dtype, dp, (int)std::max<int64_t>(nch, 1), tiles, t, all_valid, descending, ids, chosen, tie, d_counts, c->sm_count,
+                            c->s_compute));
+    }
+    unsigned long long h[2] = {0, 0};
+    CK(cudaMemcpyAsync(h, d_counts, sizeof h, cudaMemcpyDeviceToHost, c->s_compute));
+    CK(cudaStreamSynchronize(c->s_compute));
+    counts[0] = (int64_t)h[0];
+    counts[1] = (int64_t)h[1];
+    return BDF_OK;
+}
+
+static int top_k_indices_dev(bdf_ctx* c, int n_keys, const bdf_sort_key* keys, int64_t k, bdf_col** out) {
+    TRY(sort_check(n_keys, keys));
+    if (k < 0) return fail(BDF_INVALID, "top-k needs k >= 0");
+    const int64_t n = keys[0].column->total_len, k_out = std::min(k, n);
+    ColOwner o(c);
+    if (k_out == 0 || k_out * kTopkSortDen > n * kTopkSortNum) {   // no rows, or the whole sort and its first k entries
+        ColOwner full(c);
+        if (k_out) TRY(sort_indices_dev(c, n_keys, keys, full.out()));
+        TRY(col_alloc(c, BDF_U32, {ChunkPlan{k_out, false}}, nullptr, 0, o.out()));
+        cudaError_t e = cudaSuccess;
+        if (k_out) e = cudaMemcpyAsync(o->chunks[0].values, full->chunks[0].values, (size_t)k_out * 4, cudaMemcpyDeviceToDevice, c->s_compute);
+        if (e == cudaSuccess) e = finish_single_group(c, o.get());
+        if (e != cudaSuccess) return fail_cuda(e, "top-k");
+        *out = o.release();
+        return BDF_OK;
+    }
+
+    const int64_t n_words = (n + 31) / 32;
+    Scratch<uint32_t> chosen, tie;
+    Scratch<unsigned long long> d_counts;
+    CK(chosen.alloc(c, (size_t)n_words * 4));
+    CK(tie.alloc(c, (size_t)n_words * 4));
+    CK(d_counts.alloc(c, 2 * sizeof(unsigned long long)));
+    CK(cudaMemsetAsync(chosen, 0, (size_t)n_words * 4, c->s_compute));
+    ColOwner iota(c);
+    TRY(col_alloc(c, BDF_U32, {ChunkPlan{n, false}}, nullptr, 0, iota.out()));
+    c->launches++;
+    CK(launch_iota((uint32_t*)iota->chunks[0].values, n, c->sm_count, c->s_compute));
+    CK(finish_single_group(c, iota.get()));
+
+    ColOwner ids(c);   // the tie set's rows once it is not every row
+    bool all_rows = true;
+    int64_t need = k_out;
+    for (int j = 0; j < n_keys && need > 0; j++) {
+        const bool desc = keys[j].descending != 0;
+        ColOwner gathered(c);
+        const bdf_col* col = keys[j].column;
+        if (!all_rows) {
+            TRY(take_dev(c, col, ids.get(), gathered.out()));
+            col = gathered.get();
+        }
+        std::vector<uint64_t> t;
+        int64_t v = 0;
+        auto rank = [&](int64_t nv) { return std::vector<int64_t>{need > nv ? 0 : desc ? nv - need : need - 1}; };
+        TRY(select_keys(c, col, rank, 1, &t, &v));
+        const bool all_valid = need > v;
+        int64_t counts[2];
+        TRY(topk_mark(c, col, all_rows ? nullptr : (const uint32_t*)ids->chunks[0].values, all_valid ? 0 : t[0], all_valid, desc, chosen, tie,
+                      d_counts, counts));
+        need -= counts[0];
+        if (need == 0) break;
+        const bool last = counts[1] == need || j + 1 == n_keys;
+        if (all_rows && counts[1] == n && !last) continue;   // every row ties: the next criterion is read in place
+        ColOwner mask(c), tie_ids(c);
+        TRY(bits_borrow(tie, col->total_len, mask.out()));
+        TRY(filter_dev(c, all_rows ? iota.get() : ids.get(), mask.get(), tie_ids.out()));
+        if (last) {   // the first `need` ties in row order
+            LaunchTimer lt(c, BDF_K_SELECT, BDF_U32, need, need * 4);
+            CK(launch_topk_choose((const uint32_t*)tie_ids->chunks[0].values, need, chosen, c->s_compute));
+            break;
+        }
+        ids = std::move(tie_ids);
+        all_rows = false;
+    }
+
+    // the chosen rows in ascending order, sorted on their gathered criteria, mapped back to row numbers
+    ColOwner mask(c), rows(c), perm(c);
+    TRY(bits_borrow(chosen, n, mask.out()));
+    TRY(filter_dev(c, iota.get(), mask.get(), rows.out()));
+    if (rows->total_len != k_out) return fail(BDF_INVALID, "internal: top-k chose a wrong number of rows");
+    std::vector<ColOwner> gathered;
+    std::vector<bdf_sort_key> gk;
+    for (int j = 0; j < n_keys; j++) {
+        gathered.emplace_back(c);
+        TRY(take_dev(c, keys[j].column, rows.get(), gathered.back().out()));
+        gk.push_back(bdf_sort_key{gathered.back().get(), keys[j].descending});
+    }
+    TRY(sort_indices_dev(c, n_keys, gk.data(), perm.out()));
+    return take_dev(c, rows.get(), perm.get(), out);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -7401,6 +7540,13 @@ int bdf_sort_indices_dev(bdf_ctx* c, int32_t n_keys, const bdf_sort_key* keys, b
     ENTER(c);
     if (!keys || !indices) return fail(BDF_INVALID, "null argument");
     return sort_indices_dev(c, n_keys, keys, indices);
+}
+
+int bdf_top_k_indices_dev(bdf_ctx* c, int32_t n_keys, const bdf_sort_key* keys, int64_t k, bdf_col** indices) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "sort / take / filter move rows between chunks: use a one-GPU context (bdf_init) for them");
+    ENTER(c);
+    if (!keys || !indices) return fail(BDF_INVALID, "null argument");
+    return top_k_indices_dev(c, n_keys, keys, k, indices);
 }
 
 int bdf_group_aggregate_dev(bdf_ctx* c, const bdf_col* key, int32_t n_values, const bdf_col* const* values, bdf_col** out_keys, bdf_group_out* out,

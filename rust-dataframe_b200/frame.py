@@ -36,7 +36,7 @@ import numpy as np
 
 from . import _native as N
 from .arrays import F32, F64, I8, I64, NP_DTYPES, U8, U32, U64, PrimitiveArray, is_float
-from .functions import Column, ListColumn, _expr_nodes, eval_expr, sort_indices, window as _window
+from .functions import Column, ListColumn, _expr_nodes, eval_expr, sort_indices, top_k_indices, window as _window
 from .csv_reader import CsvFile, write_csv
 from .json_reader import JsonFile
 from .parquet_reader import ParquetFile, write_parquet
@@ -402,7 +402,8 @@ def plan_fusion(schema: "OrderedDict[str, int]", transformations: Sequence[tuple
                 fuse_casts: bool = True) -> List[tuple]:
     """Rewrite ``transformations``: runs of fusable Calculations whose intermediates nobody can observe become one
     ("fused", Fused) step.  The result evaluates to the same frame (same columns, same order, same values).
-    ``fuse_casts`` also folds a cast TO Float64 into the fused load (one pass instead of a cast launch plus the chain)."""
+    ``fuse_casts`` also folds a cast TO Float64 into the fused load (one pass instead of a cast launch plus the chain).
+    A sort followed by a limit becomes one ("top_k", (criteria, n)) step (_plan_top_k)."""
     steps = list(transformations)
     schemas = _schema_walk(schema, steps)
     needed = _needed_after(steps, list(schemas[-1].keys()), schemas)
@@ -430,6 +431,25 @@ def plan_fusion(schema: "OrderedDict[str, int]", transformations: Sequence[tuple
             out.append(steps[i]); i += 1
         else:
             out.append(("fused", fused)); i = j + 1
+    return _plan_top_k(out)
+
+
+def _plan_top_k(steps: List[tuple]) -> List[tuple]:
+    """A sort followed by a limit, with only select / drop steps (which keep the rows) between them, becomes one
+    ("top_k", (criteria, n)) step at the sort's place; the limit moves up."""
+    out: List[tuple] = []
+    i = 0
+    while i < len(steps):
+        if steps[i][0] == "sort":
+            j = i + 1
+            while j < len(steps) and steps[j][0] in ("select", "drop"):
+                j += 1
+            if j < len(steps) and steps[j][0] == "limit":
+                out.append(("top_k", (steps[i][1], steps[j][1])))
+                out.extend(steps[i + 1:j])
+                i = j + 1
+                continue
+        out.append(steps[i]); i += 1
     return out
 
 
@@ -656,6 +676,14 @@ class DeviceFrame:
         if not criteria:
             raise N.ComputeError("Sort criteria cannot be empty")
         idx = sort_indices([(self._numeric(c, "a sort key"), d) for c, d in criteria])
+        return DeviceFrame(OrderedDict((n, c.take(idx)) for n, c in self.columns.items()))
+
+    def top_k(self, criteria: Sequence[Tuple[str, bool]], k: int) -> "DeviceFrame":
+        """self.sort(criteria).limit(k) without sorting every row: the k rows are chosen by a radix select of the sort keys, then
+        only they are sorted and every column is taken at them.  A negative k gives no rows, as limit does."""
+        if not criteria:
+            raise N.ComputeError("Sort criteria cannot be empty")
+        idx = top_k_indices([(self._numeric(c, "a sort key"), d) for c, d in criteria], max(int(k), 0))
         return DeviceFrame(OrderedDict((n, c.take(idx)) for n, c in self.columns.items()))
 
     def group_aggregate(self, groups, aggregates: Sequence[Tuple[str, str]]) -> "DeviceFrame":
@@ -961,6 +989,8 @@ class DeviceFrame:
                 frame = frame.limit(arg)
             elif kind == "sort":
                 frame = frame.sort(arg)
+            elif kind == "top_k":
+                frame = frame.top_k(*arg)
             elif kind == "join":
                 frame = frame.join(*arg)
             elif kind == "join_asof":

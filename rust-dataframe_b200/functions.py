@@ -1010,6 +1010,21 @@ def sort_indices(criteria: Sequence[tuple]) -> "Column":
     return Column(ctx, h)
 
 
+def top_k_indices(criteria: Sequence[tuple], k: int) -> "Column":
+    """The first min(k, n) entries of sort_indices(criteria), chosen without sorting every row (SQL's ORDER BY ... LIMIT k).
+    criteria: [(Column, descending)]; the same order and errors as sort_indices, and k < 0 is refused.  Returns a one-chunk
+    UInt32 Column of row numbers."""
+    if not criteria:
+        raise N.ComputeError("Sort criteria cannot be empty")
+    ctx = criteria[0][0].ctx
+    arr = (N.SortKeyC * len(criteria))()
+    for i, (col, desc) in enumerate(criteria):
+        arr[i].column, arr[i].descending = col.handle.value if isinstance(col.handle, C.c_void_p) else col.handle, 1 if desc else 0
+    h = C.c_void_p()
+    N.raise_for_status(N.lib().bdf_top_k_indices_dev(ctx.handle, len(criteria), arr, int(k), C.byref(h)))
+    return Column(ctx, h)
+
+
 def sort_columns(criteria: Sequence[tuple], columns: Sequence["Column"]) -> List["Column"]:
     """DataFrame::sort: the index sort, then DataFrame::sort_by_indices (Column::take of every column, one chunk each)."""
     idx = sort_indices(criteria)
