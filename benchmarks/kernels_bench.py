@@ -9,6 +9,7 @@ is the evidence that every kernel of the path, not only f64 add, runs near the H
     python benchmarks/kernels_bench.py --math [--rows 100000000]                        # only the float-function rows
     python benchmarks/kernels_bench.py --stats [--rows 100000000]                       # only the statistical-aggregate rows
     python benchmarks/kernels_bench.py --csv-write [--csv-rows 50000000]                # the CSV writer rows (the reader's table written back)
+    python benchmarks/kernels_bench.py --json-write [--csv-rows 50000000]               # the JSON writer rows (that table and a List<Float64>)
     python benchmarks/kernels_bench.py --lists [--rows 100000000]                       # the list-function rows (ArrayFunctions)
     python benchmarks/kernels_bench.py --temporal [--rows 100000000]                    # the date / timestamp function rows
     python benchmarks/kernels_bench.py --ndjson [--csv-rows 50000000]                   # the line-delimited JSON reader rows (a 4.85 GB temporary file)
@@ -443,6 +444,81 @@ def csv_write_bench(ctx, rows, rows_out, reps=3):
         print(f"{name:44s} {ms:9.2f} ms  {os.path.getsize(out) / ms / 1e6:7.2f} GB/s of its text", flush=True)
         for c in cols.values():
             c.free()
+
+
+def json_write_bench(ctx, rows, rows_out, reps=3, pandas_rows=1_000_000):
+    """The CSV writer benchmark's table (Int64, two Float64, Boolean) plus a List<Float64> of mean length 4 (0..8 elements per row),
+    written as line-delimited JSON: the measure, scan and emit launches (launch records) in GB/s of text, end to end to /dev/null and
+    to a file, the CSV writer on the same numeric columns in the same session, and pandas' to_json(orient="records", lines=True) on
+    the host over the first `pandas_rows` rows.  Medians of `reps` runs after a warm-up."""
+    print("card:", _card(), flush=True)
+    with tempfile.TemporaryDirectory() as td:
+        src = os.path.join(td, "bench.csv")
+        write_csv(src, rows)
+        with rdf.CsvFile(src, schema=[rdf.I64, rdf.F64, rdf.F64, N.BOOL, N.UTF8], batch_size=1 << 20, ctx=ctx) as f:
+            cols = f.read(["id", "lat", "lng", "flag"])
+        os.unlink(src)
+        rng = np.random.default_rng(20261019)
+        chunks = []
+        for a in cols["id"].download():
+            offs = np.concatenate([[0], np.cumsum(rng.integers(0, 9, a.length))]).astype(np.int32)
+            chunks.append(rdf.ListArray(rdf.F64, offs, None, 0, a.length, 0, rdf.PrimitiveArray.from_numpy(rng.normal(size=int(offs[-1])) * 100.0)))
+        tags = rdf.ListColumn.upload(chunks, ctx=ctx, dtype=rdf.F64)
+        del chunks
+        frame = OrderedDict(list(cols.items()) + [("tags", tags)])
+        out = os.path.join(td, "out.json")
+        rdf.write_json(out, frame)
+        text = os.path.getsize(out)
+        rdf.write_csv(out, cols)
+        csv_text = os.path.getsize(out)
+        res = {"measure": [], "scan": [], "emit": [], "plan": [], "end to end, /dev/null": [], "end to end, file": [], "csv, /dev/null": []}
+        for i in range(reps + 1):
+            for target, key in (("/dev/null", "end to end, /dev/null"), (out, "end to end, file"), ("/dev/null", "csv, /dev/null")):
+                ctx.synchronize()
+                ctx.profile_read()
+                ctx.profile_enable(True)
+                t0 = time.perf_counter()
+                if key.startswith("csv"):
+                    rdf.write_csv(target, cols)
+                else:
+                    rdf.write_json(target, frame)
+                t1 = time.perf_counter()
+                ctx.profile_enable(False)
+                recs = [r for r in ctx.profile_read() if r["kernel"] == "json_write"]
+                if i == 0:
+                    continue
+                res[key].append((t1 - t0) * 1e3)
+                if key == "end to end, /dev/null":
+                    for part, dt in (("measure", rdf.U64), ("scan", rdf.U32), ("emit", rdf.U8), ("plan", -1)):
+                        res[part].append(sum(r["ms"] for r in recs if r["dtype"] == dt))
+        for key, v in res.items():
+            ms = float(np.median(v))
+            nb = csv_text if key.startswith("csv") else text
+            name = "csv write (same numeric columns) /dev/null" if key.startswith("csv") else f"json write {key}"
+            rows_out.append({"case": name, "config": "json-write", "kernel": "csv_write" if key.startswith("csv") else "json_write", "ms": ms,
+                             "rows": rows, "text_bytes": nb, "GBs_of_text": nb / ms / 1e6})
+            print(f"{name:44s} {ms:9.2f} ms  {nb / ms / 1e6:7.2f} GB/s of text ({nb / 1e9:.2f} GB, {rows:.1e} rows)", flush=True)
+        try:
+            import pandas as pd
+        except ImportError:
+            return
+        m = min(pandas_rows, rows)
+        host = {n: np.concatenate([a.value_bits() if n == "flag" else a.value_slice() for a in c.download()])[:m] for n, c in cols.items()}
+        lists = [x for a in tags.download() for x in a.to_pylist()][:m] if m <= 2_000_000 else None
+        df = pd.DataFrame(dict(host, tags=lists))
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            df.to_json(out, orient="records", lines=True)
+            ts.append((time.perf_counter() - t0) * 1e3)
+        ms = float(np.median(ts))
+        nb = os.path.getsize(out)
+        name = f"pandas to_json lines (not the reference), {m:.0e} rows"
+        rows_out.append({"case": name, "config": "json-write", "kernel": "host", "ms": ms, "rows": m, "text_bytes": nb, "GBs_of_text": nb / ms / 1e6})
+        print(f"{name:44s} {ms:9.2f} ms  {nb / ms / 1e6:7.2f} GB/s of its text", flush=True)
+        for c in cols.values():
+            c.free()
+        tags.free()
 
 
 def window_parts(recs, value_calls):
@@ -885,6 +961,7 @@ def main():
     ap.add_argument("--math", action="store_true", help="run only the float-function rows (unary, atan2/hypot/log, fused)")
     ap.add_argument("--stats", action="store_true", help="run only the statistical-aggregate rows (moments, group variance, count_distinct)")
     ap.add_argument("--csv-write", action="store_true", help="run only the CSV writer rows")
+    ap.add_argument("--json-write", action="store_true", help="run only the JSON writer rows (--csv-rows rows)")
     ap.add_argument("--lists", action="store_true", help="run only the list-function rows (ArrayFunctions)")
     ap.add_argument("--temporal", action="store_true", help="run only the date / timestamp function rows")
     ap.add_argument("--ndjson", action="store_true", help="run the line-delimited JSON reader rows (--csv-rows records)")
@@ -947,6 +1024,13 @@ def main():
         if args.json:
             with open(args.json, "w") as f:
                 json.dump({"results": rows_out}, f, indent=1)
+        return
+    if args.json_write:
+        rows_out = []
+        json_write_bench(ctx, args.csv_rows, rows_out)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"card": _card(), "results": rows_out}, f, indent=1)
         return
     if args.csv_write:
         rows_out = []

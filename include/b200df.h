@@ -1196,16 +1196,76 @@ int  bdf_parquet_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const cha
                        const bdf_temporal_type* types /* n_cols entries or NULL, as bdf_ipc_write_typed */,
                        const bdf_parquet_write_options* options /* NULL: the defaults above */);
 
+/* ---- line-delimited JSON files straight from the device (DataFrame::to_json) -------------------------------------------------------
+ * The reference has no JSON writer (its README leaves "JSON: Write" unchecked).  The rules follow arrow-rs's json::LineDelimitedWriter
+ * over serde_json, the reference's own dependencies; they are RECALLED, parity unpinned.  Departures are marked as such.
+ * Records.  One JSON object per row in row order (chunk order, then row), each followed by "\n", the last one too; compact as serde_json
+ *   writes it (no spaces).  A frame without rows writes an empty file, which bdf_json_open refuses with BDF_WOULD_PANIC (the reference
+ *   panics on an empty file): such a file does not read back.
+ * Members.  In column order, "name":value.  Names are escaped as serde_json escapes a string: \" \\ \b \f \n \r \t, other bytes below
+ *   0x20 as \u00xx (lowercase hex), every other byte as it is.
+ * NULL.  A NULL member is left out (arrow-rs's default, Spark's ignoreNullFields), so an all-NULL row is {}.  explicit_nulls = 1
+ *   writes "name":null instead (pandas' habit).  A null element inside a list is always null.
+ * Values:
+ *   integers (the 8 types)  plain decimal (-9223372036854775808, 18446744073709551615); Boolean true / false.
+ *   Float32 / Float64       the SHORTEST digits that read back to the same value in the column's own type, the closest of them when
+ *                           several do (the CSV writer's digits).  Float32 is formatted as an f32, never widened: a departure, as
+ *                           serde_json's Value widens f32 to f64.  Layout: ryu's (RECALLED: the ryu crate's format64 / format32).  With
+ *                           kk the decimal exponent of the first digit plus one (10^(kk-1) <= |v| < 10^kk): integral values as digits
+ *                           and ".0" while kk <= 16 (Float32 13); the point inside the digits for 0 < kk <= 16 (13); 0.000ddd for
+ *                           -5 < kk <= 0 (Float32 -6 < kk); otherwise d.ddde and the exponent, '-' for a negative one, no '+', no
+ *                           padding.  1.0, -0.0, 0.001, 1e16, 1e-7, 5e-324, 3.4028235e38 (f32::MAX).  So an all-integral Float64 column
+ *                           reads back as Float64 under inference (unlike the CSV writer's 1).
+ *                           NaN, inf and -inf are not JSON numbers: they are written as null (serde_json does the same), so the member
+ *                           is left out unless explicit_nulls.  THEY DO NOT SURVIVE A ROUND TRIP: they come back NULL.
+ *   temporal (types[j])     JSON strings, as bdf_parquet_write takes the types.  Date32 / Date64: "YYYY-MM-DD", the floor day.
+ *                           Timestamp: "YYYY-MM-DDTHH:MM:SS" and a fraction of a fixed number of digits for its unit (none for s, 3 for
+ *                           ms, 6 for us, 9 for ns), split by floor division as the temporal functions split (-1 us is
+ *                           "1969-12-31T23:59:59.999999").  Time zones follow the temporal functions' rules: no tz, no suffix; "UTC",
+ *                           "Z" or "+00:00": UTC fields and the suffix Z; a fixed offset +-HH:MM: the local fields (instant + offset)
+ *                           and that offset as the suffix (RFC 3339); a named zone -> BDF_UNSUPPORTED.  Time32 / Time64: "HH:MM:SS"
+ *                           with the same fraction rule.  Years as chrono's %Y: 4 digits for 0000..9999, '+' and the digits above 9999
+ *                           (+10000), '-' and at least 4 digits below 0 (-0001).  A date outside chrono's range (years -262144 ..=
+ *                           262143) or a time of day outside [0, one day) -> BDF_INVALID naming the column and the value, found from
+ *                           the column's min and max before the file is opened: nothing becomes NULL silently.
+ *   List<T> (lists[j])      [e,e,...] with each element formatted as a scalar of T, [] for an empty list; a null list is a NULL member.
+ * Columns.  Column j is lists[j] when lists is given and lists[j] is non-NULL (then cols[j] must be NULL and types[j].kind 0, as in
+ *   bdf_ipc_write_lists), otherwise cols[j]: one of the ten numeric types or Boolean, tagged with types[j] when types is given and
+ *   types[j].kind != 0 (the physical dtype must match the kind).  Chunk b of every column (the lists' chunk b) has the same number of
+ *   rows, else BDF_LENGTH_MISMATCH; sliced chunks and bit offsets are taken as they are.  Any number of columns.
+ * Reading it back.  bdf_json_open with an explicit schema reads numeric, Boolean and List<T> columns back bit for bit (NaN and +-inf as
+ *   NULL); temporal strings are not read back as temporal columns.
+ * Memory.  The rows go in windows of at most 2^21 rows and 2^23 list elements, and each window's text in blocks cut at row boundaries
+ *   where it fills a 64 MiB text buffer.  In HBM: two 64 MiB text buffers, 16 MiB of row offsets, 64 MiB of element offsets (with
+ *   list columns), 16 MiB per list column for the list positions, 48 B per (chunk, column) plus 64 B per column of tables and a
+ *   block table of 64 KiB plus 32 KiB per list column (in HBM and pinned); the context's pinned staging slots (6 x 8 MiB, shared with
+ *   uploads) carry the text to the file, written with pwrite by the staging threads.  None of it grows with the file.  Only the longest single row can add more: a row with
+ *   more than 2^23 elements needs 8 B per element of it, and a row whose text is longer than 64 MiB a buffer of its own size (one
+ *   List<Float64> of 10^7 elements: about 80 MB and 250 MB).
+ * Errors (nothing leaks; a refused call writes no file): a null pointer, n_cols <= 0, both or neither of cols[j] and lists[j], a
+ *   temporal type on a list column, an invalid temporal type or a value outside its range -> BDF_INVALID; a named tz or an
+ *   unsupported dtype -> BDF_UNSUPPORTED; a path that cannot be created or written -> BDF_INVALID with the OS error text (the file is
+ *   then incomplete); a multi-GPU context -> BDF_UNSUPPORTED.
+ * Launch records (BDF_K_JSON_WRITE): dtype BDF_U64 for the measure passes (element and row lengths), BDF_U32 for their scans, BDF_U8
+ *   for the emit passes (rows and elements), -1 for the one-thread planning steps (window ends, block cuts). */
+typedef struct { int32_t explicit_nulls; } bdf_json_write_options;
+int  bdf_json_write(bdf_ctx* ctx, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
+                    const bdf_temporal_type* types /* n_cols or NULL */, const bdf_list* const* lists /* n_cols or NULL */,
+                    const bdf_json_write_options* options /* NULL: explicit_nulls = 0 */);
+
 /* ---- measurement support ------------------------------------------------------------------------ */
 /* Per-launch CUDA-event timing on the library's compute stream (the stream the kernels run on). */
 typedef struct {
-    int32_t kernel;   /* bdf_kernel_id */
+    int32_t kernel;   /* bdf_kernel_id, or an id that follows it (BDF_K_JSON_WRITE) */
     int32_t dtype;    /* output dtype   */
     int64_t rows;     /* elements processed by the launch */
     int64_t bytes;    /* algorithmic bytes of the launch (SURVEY 8(d) per-row figure x rows) */
     float   ms;       /* device time between the bracketing events */
 } bdf_launch_record;
 typedef enum { BDF_K_BINARY = 0, BDF_K_UNARY, BDF_K_CAST, BDF_K_REDUCE, BDF_K_GENERATE, BDF_K_AVG, BDF_K_COMPARE, BDF_K_FILTER, BDF_K_EXPR, BDF_K_SORT, BDF_K_TAKE, BDF_K_GROUP, BDF_K_JOIN, BDF_K_CSV, BDF_K_WINDOW, BDF_K_MOMENTS, BDF_K_CSV_WRITE, BDF_K_LIST, BDF_K_TEMPORAL, BDF_K_JSON, BDF_K_PARQUET, BDF_K_PARQUET_WRITE, BDF_K_SELECT, BDF_K_HIST } bdf_kernel_id;
+/* Kernel ids that follow the enum.  bdf_kernel_id stays as published, ending at BDF_K_HIST: callers size their tables of kernel
+ * names by its members, so a later id is a constant here instead.  bdf_launch_record.kernel may hold one of them. */
+enum { BDF_K_JSON_WRITE = BDF_K_HIST + 1 };
 int     bdf_profile_enable(bdf_ctx* ctx, int on);
 int     bdf_profile_read(bdf_ctx* ctx, bdf_launch_record* buf, int64_t cap, int64_t* n); /* syncs; drains */
 int64_t bdf_launch_count(bdf_ctx* ctx);           /* kernels launched since bdf_init */

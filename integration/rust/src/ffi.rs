@@ -54,6 +54,9 @@ pub struct BdfParquetOptions { pub batch_size: i64 }
 pub struct BdfCsvWriteOptions { pub has_header: i32, pub delimiter: u8 }
 #[repr(C)]
 #[derive(Clone, Copy)]
+pub struct BdfJsonWriteOptions { pub explicit_nulls: i32 }
+#[repr(C)]
+#[derive(Clone, Copy)]
 pub struct BdfParquetWriteOptions { pub compression: i32, pub dictionary: i32, pub row_group_rows: i64 }
 
 #[repr(C)]
@@ -295,6 +298,10 @@ extern "C" {
     // CSV files straight from the device (DataFrame::to_csv): chunk b of every column = RecordBatch b; options NULL: a header and ','
     pub fn bdf_csv_write(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol,
                          options: *const BdfCsvWriteOptions) -> c_int;
+    // line-delimited JSON straight from the device (DataFrame::to_json): column j is lists[j] when that is non-null (cols[j] then
+    // null); types / lists may be null; options NULL: explicit_nulls = 0
+    pub fn bdf_json_write(ctx: *mut BdfCtx, path: *const c_char, n_cols: i32, names: *const *const c_char, cols: *const *const BdfCol,
+                          types: *const BdfTemporalType, lists: *const *const BdfList, options: *const BdfJsonWriteOptions) -> c_int;
     // Arrow IPC files (DataFrame::from_arrow / to_arrow)
     pub fn bdf_ipc_open(path: *const c_char, out: *mut *mut BdfIpc) -> c_int;
     pub fn bdf_ipc_close(file: *mut BdfIpc);

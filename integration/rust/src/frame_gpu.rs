@@ -384,6 +384,24 @@ pub fn to_csv_device(frame: &DeviceColumns, path: &str, options: Option<(bool, u
     check(unsafe { bdf_csv_write(dev(), c_path.as_ptr(), cols.len() as i32, name_ptrs.as_ptr(), cols.as_ptr(), p) })
 }
 
+/// `DataFrame::to_json(path)` on the device, as line-delimited JSON: every column is formatted on the GPU (floats in their shortest
+/// round-trip digits, ryu's layout) and streamed to the file.  `types`: one per column (kind 0 for a plain column) or None; `lists`:
+/// one per column, non-null where the column is a List<T> (its entry in `frame.cols` is then ignored), or None; `explicit_nulls`
+/// writes `"name":null` for a NULL member instead of leaving it out.
+pub fn to_json_device(frame: &DeviceColumns, path: &str, types: Option<&[BdfTemporalType]>, lists: Option<&[*const BdfList]>,
+                      explicit_nulls: bool) -> Result<(), String> {
+    let c_path = CString::new(path).map_err(|e| e.to_string())?;
+    let names: Vec<CString> = frame.names.iter().map(|n| CString::new(n.as_str())).collect::<Result<_, _>>().map_err(|e| e.to_string())?;
+    let name_ptrs: Vec<*const c_char> = names.iter().map(|n| n.as_ptr()).collect();
+    let cols: Vec<*const BdfCol> = frame.cols.iter().enumerate()
+        .map(|(j, c)| if lists.map_or(false, |l| !l[j].is_null()) { std::ptr::null() } else { *c as *const BdfCol }).collect();
+    let opts = BdfJsonWriteOptions { explicit_nulls: explicit_nulls as i32 };
+    check(unsafe {
+        bdf_json_write(dev(), c_path.as_ptr(), cols.len() as i32, name_ptrs.as_ptr(), cols.as_ptr(), types.map_or(std::ptr::null(), |t| t.as_ptr()),
+                       lists.map_or(std::ptr::null(), |l| l.as_ptr()), &opts)
+    })
+}
+
 /// DataFrame::to_parquet on the device: every column's pages encoded (and snappy-compressed) on the GPU and streamed to the file.
 /// `types`: one per column (kind 0 for a plain column) or None; `options`: None for the defaults.
 pub fn to_parquet_device(frame: &DeviceColumns, path: &str, types: Option<&[BdfTemporalType]>,

@@ -13,7 +13,7 @@ from .arrays import (BooleanArray, DTYPE_NAMES, ListArray, F32, F64, I8, I16, I3
                      dtype_of, width_of)
 from .ipc import IpcFile, write_ipc, write_ipc_host
 from .csv_reader import CsvFile, write_csv
-from .json_reader import JsonFile
+from .json_reader import JsonFile, write_json
 from .parquet_reader import ParquetFile, write_parquet
 from . import frame
 from .frame import DeviceFrame, plan_aggregate, plan_fusion, plan_join, plan_set_op, plan_window
@@ -22,7 +22,7 @@ from .functions import (AggFuture, AggregateFunctions, ArrayFunctions, Column, L
 
 __all__ = [
     "native", "ArrowError", "ComputeError", "Context", "DivideByZero", "ParseError", "ReferencePanic", "UnsupportedType",
-    "default_context", "PrimitiveArray", "BooleanArray", "ListArray", "ScalarFunctions", "AggregateFunctions", "ArrayFunctions", "Column", "ListColumn", "AggFuture", "cast", "eval_expr", "eval_expr_agg", "group_aggregate", "group_by", "join_indices", "join_asof_indices", "sort_indices", "sort_columns", "top_k_indices", "IpcFile", "CsvFile", "JsonFile", "ParquetFile", "write_parquet", "write_csv", "write_ipc", "write_ipc_host", "frame", "DeviceFrame", "plan_aggregate", "plan_fusion", "plan_join", "plan_set_op", "plan_window", "concat", "duplicated", "set_op_mask", "window", "moments_stat", "moments_merge", "hist_density",
+    "default_context", "PrimitiveArray", "BooleanArray", "ListArray", "ScalarFunctions", "AggregateFunctions", "ArrayFunctions", "Column", "ListColumn", "AggFuture", "cast", "eval_expr", "eval_expr_agg", "group_aggregate", "group_by", "join_indices", "join_asof_indices", "sort_indices", "sort_columns", "top_k_indices", "IpcFile", "CsvFile", "JsonFile", "ParquetFile", "write_parquet", "write_csv", "write_json", "write_ipc", "write_ipc_host", "frame", "DeviceFrame", "plan_aggregate", "plan_fusion", "plan_join", "plan_set_op", "plan_window", "concat", "duplicated", "set_op_mask", "window", "moments_stat", "moments_merge", "hist_density",
     "TemporalType", "temporal_result", "coalesce", "greatest", "least", "nanvl", "when", "CaseWhen",
     "I8", "I16", "I32", "I64", "U8", "U16", "U32", "U64", "F32", "F64", "NP_DTYPES", "DTYPE_NAMES", "dtype_of", "width_of",
 ]

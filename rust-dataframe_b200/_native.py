@@ -25,6 +25,9 @@ ASYNC = 1
 KERNEL_NAMES = ["binary", "unary", "cast", "reduce", "generate", "avg", "compare", "filter", "expr", "sort", "take", "group", "join", "csv",
                 "window", "moments", "csv_write", "list", "temporal", "json", "parquet", "parquet_write", "select", "hist"]
 K_SELECT, K_HIST = 22, 23
+K_JSON_WRITE = 24   # BDF_K_JSON_WRITE, the id that follows the bdf_kernel_id enum
+# KERNEL_NAMES mirrors the bdf_kernel_id enum; the ids after it (include/b200df.h) extend it for the launch records
+LAUNCH_KERNEL_NAMES = KERNEL_NAMES + ["json_write"]
 EXPR_UNARY = 100
 GT, GE, EQ, NE, LT, LE = range(6)
 AND, OR, NOT = range(3)
@@ -175,6 +178,10 @@ class CsvOptions(C.Structure):
 
 class CsvWriteOptions(C.Structure):
     _fields_ = [("has_header", C.c_int32), ("delimiter", C.c_uint8)]
+
+
+class JsonWriteOptions(C.Structure):
+    _fields_ = [("explicit_nulls", C.c_int32)]
 
 
 class LaunchRecord(C.Structure):
@@ -372,6 +379,7 @@ def lib() -> C.CDLL:
         "bdf_ipc_read_temporal": ([vp, vp, i32, C.c_int, P(vp)], C.c_int),
         "bdf_ipc_write_typed": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(TemporalTypeC)], C.c_int),
         "bdf_ipc_write_lists": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(TemporalTypeC), P(vp)], C.c_int),
+        "bdf_json_write": ([vp, C.c_char_p, i32, P(C.c_char_p), P(vp), P(TemporalTypeC), P(vp), P(JsonWriteOptions)], C.c_int),
     }
     for name, (args, res) in sig.items():
         fn = getattr(L, name)  # AttributeError if the library does not export a declared symbol
@@ -396,7 +404,7 @@ EXPORTED_SYMBOLS = [
     "bdf_ipc_open", "bdf_ipc_close", "bdf_ipc_describe", "bdf_ipc_column", "bdf_ipc_batch_rows", "bdf_ipc_view", "bdf_ipc_read", "bdf_ipc_read_batches",
     "bdf_ipc_write_host", "bdf_ipc_write",
     "bdf_csv_open", "bdf_csv_describe", "bdf_csv_column", "bdf_csv_read", "bdf_csv_stats", "bdf_csv_close", "bdf_csv_write",
-    "bdf_json_open", "bdf_json_describe", "bdf_json_column", "bdf_json_read", "bdf_json_read_list", "bdf_json_stats", "bdf_json_close",
+    "bdf_json_open", "bdf_json_describe", "bdf_json_column", "bdf_json_read", "bdf_json_read_list", "bdf_json_stats", "bdf_json_close", "bdf_json_write",
     "bdf_moments", "bdf_moments_dev", "bdf_moments_stat", "bdf_moments_merge", "bdf_distinct", "bdf_distinct_dev",
     "bdf_list_upload", "bdf_list_describe", "bdf_list_chunk_info", "bdf_list_download", "bdf_list_values", "bdf_list_free",
     "bdf_list_find_dev", "bdf_list_reduce_dev", "bdf_list_transform_dev", "bdf_list_set_dev", "bdf_list_explode_dev",
@@ -580,7 +588,7 @@ class Context:
         buf = (LaunchRecord * cap)()
         n = C.c_int64(0)
         raise_for_status(lib().bdf_profile_read(self.handle, buf, cap, C.byref(n)))
-        return [{"kernel": KERNEL_NAMES[buf[i].kernel], "dtype": buf[i].dtype, "rows": buf[i].rows,
+        return [{"kernel": LAUNCH_KERNEL_NAMES[buf[i].kernel], "dtype": buf[i].dtype, "rows": buf[i].rows,
                  "bytes": buf[i].bytes, "ms": buf[i].ms} for i in range(n.value)]
 
     def launch_count(self) -> int:

@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "libb200df.so")
 OBJ_DIR = os.path.join(HERE, "build")
-SOURCES = ["k_binary.cu", "k_unary.cu", "k_cast.cu", "k_reduce.cu", "k_filter.cu", "k_expr.cu", "k_sort.cu", "k_group.cu", "k_scan.cu", "k_join.cu", "k_setop.cu", "k_topk.cu", "k_window.cu", "k_list.cu", "k_temporal.cu", "k_moments.cu", "k_dist.cu", "k_cond.cu", "k_csv.cu", "k_csv_write.cu", "k_json.cu", "k_parquet.cu", "k_parquet_write.cu", "k_generate.cu", "runtime.cu", "ipc.cu", "parquet.cu", "comm.cu"]
+SOURCES = ["k_binary.cu", "k_unary.cu", "k_cast.cu", "k_reduce.cu", "k_filter.cu", "k_expr.cu", "k_sort.cu", "k_group.cu", "k_scan.cu", "k_join.cu", "k_setop.cu", "k_topk.cu", "k_window.cu", "k_list.cu", "k_temporal.cu", "k_moments.cu", "k_dist.cu", "k_cond.cu", "k_csv.cu", "k_csv_write.cu", "k_json.cu", "k_json_write.cu", "k_parquet.cu", "k_parquet_write.cu", "k_generate.cu", "runtime.cu", "ipc.cu", "parquet.cu", "comm.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]

@@ -230,6 +230,31 @@ struct CsvwDesc {
     int32_t val_bit_off;   // Boolean values bit offset
     int32_t dtype; int32_t pad;
 };
+// JSON writer (k_json_write.cu): one JsonwDesc per (chunk, column), chunk-major; one JsonwCol per column.
+struct JsonwDesc {
+    const void* values; const uint32_t* validity;   // a scalar column's, or a list column's elements'
+    const int32_t* loffs;       // list: len + 1 offsets from 0; nullptr for a scalar column
+    const uint32_t* lvalid;     // list: the list validity at bit 0, or nullptr
+    long long estart;           // list: elements in the column's earlier chunks
+    int32_t bit_off;            // validity bit offset
+    int32_t val_bit_off;        // Boolean values bit offset
+};
+struct JsonwCol {
+    long long upd, ups, off;    // temporal text (json_format.cuh): units per day, per second, tz offset in units
+    int32_t tkind, frac, suffix_len;
+    int32_t dtype;              // a list's element dtype
+    int32_t name_at, name_len;  // the column's "name": in the names buffer
+    int32_t list;               // its index among the list columns; -1 for a scalar column
+    char suffix[8];
+};
+// The tables of one write.  plan is the current window's plan (k_json_write.cu): [0] its end row, [1] its elements,
+// [2 + L] the first element of list L in it, [2 + n_lists + L] where list L's elements start in the window's element scan.
+struct JsonwArgs {
+    const JsonwDesc* desc; const JsonwCol* cols; const char* names; const long long* chunk_start;
+    const int32_t* list_cols;   // the column of list L
+    long long* plan;
+    int n_cols, n_chunks, n_lists, explicit_nulls;
+};
 
 // Null handling and conditional selection (k_cond.cu): one header per chunk followed by its arguments, so the stride of the
 // descriptor array is cond_desc_bytes(n_conds + n_vals).  Arguments [0, n_conds) are the Boolean conditions of a case_when,
@@ -585,6 +610,18 @@ cudaError_t launch_csvw_measure(const CsvwDesc* cols, const long long* chunk_sta
                                 unsigned long long* lens, unsigned long long* block_sums, cudaStream_t s);
 cudaError_t launch_csvw_emit(const CsvwDesc* cols, const long long* chunk_start, int n_cols, int n_chunks, long long row0, long long rows, int delim,
                              const unsigned long long* offs, char* out, cudaStream_t s);
+
+// JSON writer (k_json_write.cu).
+cudaError_t launch_jsonw_window(const JsonwArgs& a, long long row0, long long rows, long long max_rows, long long elem_cap, cudaStream_t s);
+cudaError_t launch_jsonw_elem_len(const JsonwArgs& a, long long n_elems, unsigned long long* elens, unsigned long long* block_sums, cudaStream_t s);
+cudaError_t launch_jsonw_measure(const JsonwArgs& a, long long row0, long long rows, const unsigned long long* escan, unsigned long long* lens,
+                                 unsigned long long* block_sums, cudaStream_t s);
+cudaError_t launch_jsonw_cut(const JsonwArgs& a, long long row0, long long rows, const unsigned long long* offs, unsigned long long cap, int max_cuts,
+                             long long* cuts, cudaStream_t s);
+cudaError_t launch_jsonw_emit(const JsonwArgs& a, long long wrow0, long long r0, long long r1, const unsigned long long* offs, unsigned long long base,
+                              const unsigned long long* escan, long long* lpos, long long lpos_stride, char* out, cudaStream_t s);
+cudaError_t launch_jsonw_elem_emit(const JsonwArgs& a, int list, long long e0, long long e1, long long wrow0, const unsigned long long* escan,
+                                   const long long* lpos, long long lpos_stride, unsigned long long base, char* out, cudaStream_t s);
 
 // Parquet writer (k_parquet_write.cu; the page, tile and page-result records are parquet_encode.cuh's pq::WPage, WTile and WPageOut).
 size_t pqw_page_bytes();

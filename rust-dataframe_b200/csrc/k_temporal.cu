@@ -11,6 +11,7 @@
 //
 // Roofline: HBM, sizeof(In) + sizeof(Out) + 2/8 bytes/row (Timestamp -> Int32 field: 12 B/row plus validity); the two-column form
 // sizeof(A) + sizeof(B) + sizeof(Out) (MONTHS_BETWEEN of two timestamps: 24 B/row).
+#include "civil.cuh"
 #include "common.cuh"
 
 namespace bdf {
@@ -22,9 +23,6 @@ enum : int {
 enum : int { TR_YEAR = 0, TR_QUARTER, TR_MONTH, TR_WEEK, TR_DAY, TR_HOUR, TR_MINUTE, TR_SECOND };
 enum : int { TB_DATE_DIFF = 0, TB_MONTHS_BETWEEN };
 
-constexpr int32_t kMinDay = -96465658;   // -262144-01-01, chrono's NaiveDate::MIN
-constexpr int32_t kMaxDay = 95026601;    //  262143-12-31, chrono's NaiveDate::MAX
-
 template <int CFG> struct TUnit;
 template <> struct TUnit<TC_DAYS> { static constexpr int64_t per_day = 1, per_sec = 1; };
 template <> struct TUnit<TC_S> { static constexpr int64_t per_day = 86400LL, per_sec = 1; };
@@ -32,18 +30,6 @@ template <> struct TUnit<TC_MS> { static constexpr int64_t per_day = 86400000LL,
 template <> struct TUnit<TC_US> { static constexpr int64_t per_day = 86400000000LL, per_sec = 1000000LL; };
 template <> struct TUnit<TC_NS> { static constexpr int64_t per_day = 86400000000000LL, per_sec = 1000000000LL; };
 
-// Hinnant's civil_from_days on 32-bit integers (valid for every day of chrono's range).
-__device__ __forceinline__ void civil_from_days(int32_t z, int32_t& y, uint32_t& m, uint32_t& d) {
-    z += 719468;
-    const int32_t era = (z >= 0 ? z : z - 146096) / 146097;
-    const uint32_t doe = (uint32_t)(z - era * 146097);
-    const uint32_t yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
-    const uint32_t doy = doe - (365 * yoe + yoe / 4 - yoe / 100);
-    const uint32_t mp = (5 * doy + 2) / 153;
-    d = doy - (153 * mp + 2) / 5 + 1;
-    m = mp < 10 ? mp + 3 : mp - 9;
-    y = (int32_t)yoe + era * 400 + (m <= 2 ? 1 : 0);
-}
 __device__ __forceinline__ int32_t days_from_civil(int32_t y, uint32_t m, uint32_t d) {
     y -= m <= 2 ? 1 : 0;
     const int32_t era = (y >= 0 ? y : y - 399) / 400;

@@ -37,6 +37,7 @@
 #include "moments.cuh"
 #include "dist.cuh"
 #include "json_parse.cuh"
+#include "json_format.cuh"
 #define PQ_HOST_PLAN
 #include "parquet_decode.cuh"
 #define PQ_HOST_WRITE
@@ -4248,6 +4249,54 @@ static int pwrite_all(int fd, const char* p, size_t n, off_t off) {   // 0 or an
     return 0;
 }
 
+// Text blocks from device buffers to a file, in order: each block crosses PCIe through the context's pinned staging slots (at most
+// kStageSlots - 1 in flight) and the CopyPool threads pwrite every slot at its offset in the file.  The CSV and JSON writers share it.
+struct FileSink {
+    bdf_ctx* c;
+    int fd;
+    const char* path;
+    off_t file_off;
+    struct Pending { bdf_ctx::StageSlot* sl; off_t off; size_t n; };
+    std::deque<Pending> pending;
+
+    int retire() {
+        const Pending p = pending.front();
+        pending.pop_front();
+        CK(cudaEventSynchronize(p.sl->ev));
+        p.sl->busy = false;
+        constexpr size_t kJob = (size_t)512 << 10;
+        std::atomic<int> werr{0};
+        c->pool->run((p.n + kJob - 1) / kJob, [&](size_t j) {
+            const int we = pwrite_all(fd, p.sl->p + j * kJob, std::min(kJob, p.n - j * kJob), p.off + (off_t)(j * kJob));
+            if (we) werr = we;
+        });
+        if (werr) return fail(BDF_INVALID, "writing %s failed: %s", path, strerror(werr));
+        return BDF_OK;
+    }
+    // `bytes` of `text`, complete once `ready` has fired, go next in the file; `left` is recorded on the copy stream once they have
+    // left `text`.
+    int put(const char* text, size_t bytes, cudaEvent_t ready, cudaEvent_t left) {
+        CK(cudaStreamWaitEvent(c->s_d2h, ready, 0));
+        for (size_t off = 0; off < bytes; off += kStageBytes) {
+            const size_t n = std::min(kStageBytes, bytes - off);
+            if ((int)pending.size() >= kStageSlots - 1) TRY(retire());
+            bdf_ctx::StageSlot& sl = c->stage[c->stage_next++ % kStageSlots];
+            if (sl.busy) CK(cudaEventSynchronize(sl.ev));   // an upload's slot
+            CK(cudaMemcpyAsync(sl.p, text + off, n, cudaMemcpyDeviceToHost, c->s_d2h));
+            CK(cudaEventRecord(sl.ev, c->s_d2h));
+            sl.busy = true;
+            pending.push_back(Pending{&sl, file_off + (off_t)off, n});
+        }
+        CK(cudaEventRecord(left, c->s_d2h));
+        file_off += (off_t)bytes;
+        return BDF_OK;
+    }
+    int flush() {
+        while (!pending.empty()) TRY(retire());
+        return BDF_OK;
+    }
+};
+
 static int csv_write(bdf_ctx* c, const char* path, int n_cols, const char* const* names, const bdf_col* const* cols, const bdf_csv_write_options* opt) {
     if (!path || !names || !cols) return fail(BDF_INVALID, "null argument");
     if (n_cols <= 0) return fail(BDF_INVALID, "no columns to write");
@@ -4346,48 +4395,20 @@ static int csv_write(bdf_ctx* c, const char* path, int n_cols, const char* const
         if (e2 == cudaSuccess) e2 = cudaEventRecord(ev_emit[b], c->s_compute);
         return e2 == cudaSuccess ? BDF_OK : fail_cuda(e2, "CSV write kernels");
     };
-    struct Pending { bdf_ctx::StageSlot* sl; off_t off; size_t n; };
-    std::deque<Pending> pending;
-    auto retire = [&]() -> int {
-        const Pending p = pending.front();
-        pending.pop_front();
-        CK(cudaEventSynchronize(p.sl->ev));
-        p.sl->busy = false;
-        constexpr size_t kJob = (size_t)512 << 10;
-        std::atomic<int> werr{0};
-        c->pool->run((p.n + kJob - 1) / kJob, [&](size_t j) {
-            const int we = pwrite_all(fd, p.sl->p + j * kJob, std::min(kJob, p.n - j * kJob), p.off + (off_t)(j * kJob));
-            if (we) werr = we;
-        });
-        if (werr) return fail(BDF_INVALID, "writing %s failed: %s", path, strerror(werr));
-        return BDF_OK;
-    };
+    FileSink sink{c, fd, path, file_off, {}};
     auto drain = [&](int64_t k) -> int {
         const int b = (int)(k & 1);
         CK(cudaEventSynchronize(ev_emit[b]));
         const size_t bytes = (size_t)tot.p[b];
         if (c->profiling) c->prof[emit_rec[b]].rec.bytes += (int64_t)bytes;
-        CK(cudaStreamWaitEvent(c->s_d2h, ev_emit[b], 0));
-        for (size_t off = 0; off < bytes; off += kStageBytes) {
-            const size_t n = std::min(kStageBytes, bytes - off);
-            if ((int)pending.size() >= kStageSlots - 1) TRY(retire());
-            bdf_ctx::StageSlot& sl = c->stage[c->stage_next++ % kStageSlots];
-            if (sl.busy) CK(cudaEventSynchronize(sl.ev));   // an upload's slot
-            CK(cudaMemcpyAsync(sl.p, text[b] + off, n, cudaMemcpyDeviceToHost, c->s_d2h));
-            CK(cudaEventRecord(sl.ev, c->s_d2h));
-            sl.busy = true;
-            pending.push_back(Pending{&sl, file_off + (off_t)off, n});
-        }
-        CK(cudaEventRecord(ev_d2h[b], c->s_d2h));
-        file_off += (off_t)bytes;
-        return BDF_OK;
+        return sink.put(text[b], bytes, ev_emit[b], ev_d2h[b]);
     };
     TRY(enqueue(0));
     for (int64_t k = 0; k < n_blocks; k++) {
         if (k + 1 < n_blocks) TRY(enqueue(k + 1));
         TRY(drain(k));
     }
-    while (!pending.empty()) TRY(retire());
+    TRY(sink.flush());
     return finish();
 }
 
@@ -7698,11 +7719,339 @@ int bdf_parquet_read(bdf_ctx* c, const bdf_parquet* f, int32_t n_cols, const int
     return parquet_read(c, f, n_cols, cols, out);
 }
 
+// ---------------------------------------------------------------------------------------------------
+// JSON writer (k_json_write.cu; the rules are in include/b200df.h).  A list row has no longest text, so the rows go in WINDOWS of at
+// most kJsonwMaxRows rows and kJsonwElems list elements (one row at least): the window's elements and rows are measured and
+// scanned, and its text is cut into blocks that fill a text buffer (a row longer than the buffer is a block in a buffer of its own).
+// As in the CSV writer, block k is formatted into one of two fixed buffers while block k-1 crosses PCIe to the file (FileSink).
+
+static constexpr size_t kJsonwText = (size_t)64 << 20;        // bytes of each of the two device text buffers
+static constexpr int64_t kJsonwMaxRows = (int64_t)1 << 21;    // rows per window
+static constexpr int64_t kJsonwElems = (int64_t)1 << 23;      // list elements per window, unless one row has more
+static constexpr int kJsonwMaxCuts = 4096;                    // blocks per window (a window with more ends at the last one)
+
+// A column name as serde_json writes a string, and the ':' after it.
+static std::string jsonw_name(const char* s) {
+    std::string o = "\"";
+    for (; *s; s++) {
+        const unsigned char ch = (unsigned char)*s;
+        switch (ch) {
+            case '"': o += "\\\""; break;
+            case '\\': o += "\\\\"; break;
+            case '\b': o += "\\b"; break;
+            case '\f': o += "\\f"; break;
+            case '\n': o += "\\n"; break;
+            case '\r': o += "\\r"; break;
+            case '\t': o += "\\t"; break;
+            default:
+                if (ch < 0x20) {
+                    char buf[8];
+                    snprintf(buf, sizeof buf, "\\u%04x", ch);
+                    o += buf;
+                } else {
+                    o += (char)ch;
+                }
+        }
+    }
+    return o + "\":";
+}
+
+// The temporal text of column j (types[j]): its JsonwCol fields, or BDF_INVALID / BDF_UNSUPPORTED as the temporal functions refuse.
+static int jsonw_temporal(const bdf_temporal_type* t, const bdf_col* col, const char* name, JsonwCol* jc) {
+    int dtype = 0, cfg = 0;
+    TRY(temporal_storage(t, &dtype, &cfg));
+    if (col->dtype != dtype) return fail(BDF_INVALID, "column '%s' of dtype %d does not hold temporal kind %d", name, col->dtype, t->kind);
+    int64_t off_sec = 0;
+    if (t->kind == BDF_TIMESTAMP && !temporal_tz_offset(t->tz, &off_sec))
+        return fail(BDF_UNSUPPORTED, "column '%s': time zone '%s' is not a fixed offset: named zones need a tz database the device does not have", name, t->tz);
+    const int64_t ups = temporal_per_sec(cfg);
+    jc->ups = ups;
+    jc->upd = cfg == TC_DAYS ? 1 : 86400 * ups;
+    jc->off = off_sec * ups;
+    jc->frac = t->kind == BDF_DATE32 || t->kind == BDF_DATE64 ? 0 : 3 * t->unit;
+    jc->tkind = t->kind == BDF_DATE32 || t->kind == BDF_DATE64 ? JT_DATE : t->kind == BDF_TIMESTAMP ? JT_TIMESTAMP : JT_TIME;
+    if (t->kind == BDF_TIMESTAMP && t->tz) {
+        const bool utc = !strcmp(t->tz, "UTC") || !strcmp(t->tz, "Z") || !strcmp(t->tz, "+00:00");
+        const char* sfx = utc ? "Z" : t->tz;   // a fixed offset is 6 bytes (temporal_tz_offset)
+        jc->suffix_len = (int32_t)strlen(sfx);
+        memcpy(jc->suffix, sfx, (size_t)jc->suffix_len);
+    }
+    return BDF_OK;
+}
+
+// Every date of a temporal column must lie in chrono's range and every time of day in [0, one day): its min and max decide.
+static int jsonw_check_range(bdf_ctx* c, const bdf_col* col, const JsonwCol& jc, const char* name) {
+    const int64_t n = (int64_t)col->chunks.size();
+    if (col->total_len == 0) return BDF_OK;
+    wait_groups(c->s_compute, col, 0, n);
+    TRY(reduce_range(c, col, 0, n, c->h_agg_dev));
+    CK(cudaStreamSynchronize(c->s_compute));
+    const AggDev a = c->h_agg[0];
+    if (a.count == 0) return BDF_OK;
+    const int64_t lo = (int64_t)(a.min_bits ^ (1ull << 63)), hi = (int64_t)(a.max_bits ^ (1ull << 63));   // k_reduce's sign-flipped keys
+    if (jc.tkind == JT_TIME) {
+        if (lo < 0) return fail(BDF_INVALID, "column '%s': the time of day %lld is outside [0, %lld)", name, (long long)lo, (long long)jc.upd);
+        if (hi >= jc.upd) return fail(BDF_INVALID, "column '%s': the time of day %lld is outside [0, %lld)", name, (long long)hi, (long long)jc.upd);
+        return BDF_OK;
+    }
+    for (const int64_t v : {lo, hi}) {
+        int64_t days = 0, tod = 0;
+        jsonf_split(v, jc.tkind, jc.upd, jc.off, days, tod);
+        if (days < kMinDay || days > kMaxDay)
+            return fail(BDF_INVALID, "column '%s': the value %lld is a date outside chrono's range (years -262144 ..= 262143)", name, (long long)v);
+    }
+    return BDF_OK;
+}
+
+static int json_write(bdf_ctx* c, const char* path, int n_cols, const char* const* names, const bdf_col* const* cols, const bdf_temporal_type* types,
+                      const bdf_list* const* lists, const bdf_json_write_options* opt) {
+    if (!path || !names || !cols) return fail(BDF_INVALID, "null argument");
+    if (n_cols <= 0) return fail(BDF_INVALID, "no columns to write");
+    std::vector<JsonwCol> jcols((size_t)n_cols);
+    std::vector<int32_t> list_cols;
+    std::string name_text;
+    int64_t n_chunks = -1;
+    auto chunk_rows = [&](int j, int64_t b) { return lists && lists[j] ? lists[j]->lens[(size_t)b] : cols[j]->chunks[(size_t)b].len; };
+    for (int j = 0; j < n_cols; j++) {
+        const bdf_list* l = lists ? lists[j] : nullptr;
+        if (!names[j] || (l ? cols[j] != nullptr : cols[j] == nullptr))
+            return fail(BDF_INVALID, "column %d: null column or name, or both a column and a list", j);
+        const bdf_col* col = l ? l->values : cols[j];
+        if (!col->fparts.empty()) return fail(BDF_INVALID, "a column of a multi-GPU context was passed to a one-GPU context");
+        JsonwCol& jc = jcols[(size_t)j];
+        jc = JsonwCol{};
+        jc.list = -1;
+        jc.dtype = col->dtype;
+        if (l) {
+            if (types && types[j].kind) return fail(BDF_INVALID, "list column '%s' cannot carry a temporal type", names[j]);
+            jc.list = (int32_t)list_cols.size();
+            list_cols.push_back(j);
+        } else if (!((col->dtype >= 0 && col->dtype < BDF_NTYPES) || col->dtype == kBool)) {
+            return fail(BDF_UNSUPPORTED, "column '%s': dtype %d", names[j], col->dtype);
+        } else if (types && types[j].kind) {
+            TRY(jsonw_temporal(&types[j], col, names[j], &jc));
+        }
+        const int64_t nc = l ? (int64_t)l->lens.size() : (int64_t)col->chunks.size();
+        if (n_chunks < 0) n_chunks = nc;
+        if (nc != n_chunks)
+            return fail(BDF_LENGTH_MISMATCH, "columns have different numbers of chunks (%lld, %lld)", (long long)nc, (long long)n_chunks);
+        for (int64_t b = 0; b < nc; b++)
+            if (chunk_rows(j, b) != chunk_rows(0, b))
+                return fail(BDF_LENGTH_MISMATCH, "chunk %lld: column '%s' has %lld rows, column '%s' has %lld", (long long)b, names[j],
+                            (long long)chunk_rows(j, b), names[0], (long long)chunk_rows(0, b));
+        const std::string nm = jsonw_name(names[j]);
+        jc.name_at = (int32_t)name_text.size();
+        jc.name_len = (int32_t)nm.size();
+        name_text += nm;
+    }
+    const int n_lists = (int)list_cols.size();
+    std::vector<long long> starts((size_t)n_chunks + 1, 0);
+    std::vector<JsonwDesc> descs((size_t)n_chunks * n_cols);
+    std::vector<long long> estart((size_t)n_cols, 0);
+    for (int64_t b = 0; b < n_chunks; b++) {
+        starts[b + 1] = starts[b] + chunk_rows(0, b);
+        for (int j = 0; j < n_cols; j++) {
+            const bdf_list* l = lists ? lists[j] : nullptr;
+            const DevChunk& ch = l ? l->values->chunks[(size_t)b] : cols[j]->chunks[(size_t)b];
+            JsonwDesc& d = descs[b * n_cols + j];
+            d = JsonwDesc{ch.values, ch.validity, nullptr, nullptr, 0, ch.bit_off, ch.val_bit_off};
+            if (l) {
+                d.loffs = l->off[(size_t)b];
+                d.lvalid = l->valid[(size_t)b];
+                d.estart = estart[(size_t)j];
+                estart[(size_t)j] += ch.len;
+            }
+        }
+    }
+    const int64_t rows = starts[(size_t)n_chunks];
+    for (int j = 0; j < n_cols; j++) {   // before the file is touched: a refused value leaves it as it was
+        const bdf_col* col = lists && lists[j] ? lists[j]->values : cols[j];
+        wait_groups(c->s_compute, col, 0, (int64_t)col->chunks.size());
+        if (jcols[(size_t)j].tkind != JT_NONE) TRY(jsonw_check_range(c, col, jcols[(size_t)j], names[j]));
+    }
+
+    const int fd = open(path, O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0644);
+    if (fd < 0) return fail(BDF_INVALID, "cannot create %s: %s", path, strerror(errno));
+    struct FdGuard { int fd; ~FdGuard() { if (fd >= 0) close(fd); } } fdg{fd};
+    auto finish = [&]() {
+        const int fdv = fdg.fd;
+        fdg.fd = -1;
+        if (close(fdv) != 0) return fail(BDF_INVALID, "closing %s failed: %s", path, strerror(errno));
+        return (int)BDF_OK;
+    };
+    if (rows == 0) return finish();
+
+    TRY(ensure_stage(c));
+    // the column tables in one buffer: descriptors, columns, chunk starts, list columns, names, the window plan
+    const int cut_stride = 2 + n_lists;
+    const size_t plan_n = 2 + 2 * (size_t)n_lists, cuts_n = 1 + (size_t)(kJsonwMaxCuts + 1) * cut_stride;
+    auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t o_cols = al(descs.size() * sizeof(JsonwDesc)), o_starts = o_cols + al(jcols.size() * sizeof(JsonwCol));
+    const size_t o_lists = o_starts + al(starts.size() * sizeof(long long)), o_names = o_lists + al(list_cols.size() * sizeof(int32_t) + 4);
+    const size_t o_plan = o_names + al(name_text.size() + 1), o_cuts = o_plan + al(plan_n * sizeof(long long)), meta_bytes = o_cuts + cuts_n * sizeof(long long);
+    std::vector<char> hmeta(o_plan, 0);
+    memcpy(hmeta.data(), descs.data(), descs.size() * sizeof(JsonwDesc));
+    memcpy(hmeta.data() + o_cols, jcols.data(), jcols.size() * sizeof(JsonwCol));
+    memcpy(hmeta.data() + o_starts, starts.data(), starts.size() * sizeof(long long));
+    if (n_lists) memcpy(hmeta.data() + o_lists, list_cols.data(), list_cols.size() * sizeof(int32_t));
+    memcpy(hmeta.data() + o_names, name_text.data(), name_text.size());
+
+    Scratch<char> meta;
+    Scratch<char> text[2];
+    Scratch<unsigned long long> lens, sums, elens_fixed, esums_fixed;
+    Scratch<long long> lpos;
+    cudaError_t e = meta.alloc(c, meta_bytes);
+    if (e == cudaSuccess) e = text[0].alloc(c, kJsonwText);
+    if (e == cudaSuccess) e = text[1].alloc(c, kJsonwText);
+    if (e == cudaSuccess) e = lens.alloc(c, (size_t)(kJsonwMaxRows + 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = sums.alloc(c, (size_t)scan_tile_sums(kJsonwMaxRows) * sizeof(unsigned long long));
+    if (e == cudaSuccess && n_lists) e = elens_fixed.alloc(c, (size_t)(kJsonwElems + 1) * sizeof(unsigned long long));
+    if (e == cudaSuccess && n_lists) e = esums_fixed.alloc(c, (size_t)scan_tile_sums(kJsonwElems) * sizeof(unsigned long long));
+    if (e == cudaSuccess && n_lists) e = lpos.alloc(c, (size_t)n_lists * kJsonwMaxRows * sizeof(long long));
+    // pageable source: the copy has read it when it returns
+    if (e == cudaSuccess) e = cudaMemcpyAsync(meta.get(), hmeta.data(), hmeta.size(), cudaMemcpyHostToDevice, c->s_compute);
+    if (e != cudaSuccess) return fail_cuda(e, "JSON write setup");
+    std::unique_ptr<Scratch<unsigned long long>> elens_big, esums_big;   // the elements of a row longer than the window's cap
+    std::unique_ptr<Scratch<char>> text_big;                             // the text of a row longer than a text buffer
+    int64_t elem_cap = kJsonwElems;
+    size_t big_cap = 0;
+    unsigned long long* elens = elens_fixed.get();
+    unsigned long long* esums = esums_fixed.get();
+    struct Pinned { long long* p = nullptr; ~Pinned() { if (p) cudaFreeHost(p); } } hp;
+    struct Events { bdf_ctx* c; cudaEvent_t ev[4] = {}; ~Events() { for (auto x : ev) ev_put(c, x); } } evs{c};
+    CK(cudaHostAlloc((void**)&hp.p, (plan_n + cuts_n) * sizeof(long long), cudaHostAllocDefault));
+    for (auto& x : evs.ev) CK(ev_get(c, &x));
+    cudaEvent_t* ev_emit = evs.ev;       // block k's text is complete in its buffer
+    cudaEvent_t* ev_d2h = evs.ev + 2;    // block k's text has left its buffer
+    // Declared after the buffers, so it runs first on every exit: no copy may still read a text buffer when it is freed.
+    struct DrainD2H { cudaStream_t s; ~DrainD2H() { cudaStreamSynchronize(s); } } drain_guard{c->s_d2h};
+
+    JsonwArgs a;
+    a.desc = (const JsonwDesc*)meta.get();
+    a.cols = (const JsonwCol*)(meta.get() + o_cols);
+    a.chunk_start = (const long long*)(meta.get() + o_starts);
+    a.list_cols = (const int32_t*)(meta.get() + o_lists);
+    a.names = meta.get() + o_names;
+    a.plan = (long long*)(meta.get() + o_plan);
+    a.n_cols = n_cols; a.n_chunks = (int)n_chunks; a.n_lists = n_lists; a.explicit_nulls = opt && opt->explicit_nulls ? 1 : 0;
+    long long* d_cuts = (long long*)(meta.get() + o_cuts);
+    long long* h_plan = hp.p;
+    long long* h_cuts = hp.p + plan_n;
+
+    FileSink sink{c, fd, path, 0, {}};
+    struct Block { const char* text; size_t bytes; int b; };
+    Block prev{nullptr, 0, 0};
+    bool have_prev = false;
+    auto put_prev = [&]() -> int {
+        if (!have_prev) return BDF_OK;
+        have_prev = false;
+        return sink.put(prev.text, prev.bytes, ev_emit[prev.b], ev_d2h[prev.b]);
+    };
+    int64_t k = 0;   // blocks so far
+    for (int64_t w0 = 0; w0 < rows;) {
+        TRY(put_prev());
+        int64_t w1 = std::min<int64_t>(rows, w0 + kJsonwMaxRows), n_el = 0;
+        if (n_lists) {
+            {
+                LaunchTimer t(c, BDF_K_JSON_WRITE, -1, 1, 0);
+                CK(launch_jsonw_window(a, w0, rows, kJsonwMaxRows, kJsonwElems, c->s_compute));
+            }
+            CK(cudaMemcpyAsync(h_plan, a.plan, plan_n * sizeof(long long), cudaMemcpyDeviceToHost, c->s_compute));
+            CK(cudaStreamSynchronize(c->s_compute));
+            w1 = h_plan[0];
+            n_el = h_plan[1];
+            if (n_el > elem_cap) {   // one row with more elements than the cap: buffers of its size (freed in stream order)
+                elens_big.reset(new Scratch<unsigned long long>());
+                esums_big.reset(new Scratch<unsigned long long>());
+                e = elens_big->alloc(c, (size_t)(n_el + 1) * sizeof(unsigned long long));
+                if (e == cudaSuccess) e = esums_big->alloc(c, (size_t)scan_tile_sums(n_el) * sizeof(unsigned long long));
+                if (e != cudaSuccess) return fail_cuda(e, "JSON write: the elements of a long list");
+                elens = elens_big->get(); esums = esums_big->get(); elem_cap = n_el;
+            }
+            if (n_el > 0) {
+                {
+                    LaunchTimer t(c, BDF_K_JSON_WRITE, BDF_U64, n_el, n_el * 8);
+                    CK(launch_jsonw_elem_len(a, n_el, elens, esums, c->s_compute));
+                }
+                LaunchTimer t(c, BDF_K_JSON_WRITE, BDF_U32, n_el, n_el * 16);
+                c->launches += kScanSumsLaunches - 1;
+                CK(launch_scan_sums(elens, n_el, esums, c->s_compute));
+            }
+        }
+        const int64_t wn = w1 - w0;
+        {
+            LaunchTimer t(c, BDF_K_JSON_WRITE, BDF_U64, wn, wn * 8);
+            CK(launch_jsonw_measure(a, w0, wn, elens, lens, sums, c->s_compute));
+        }
+        {
+            LaunchTimer t(c, BDF_K_JSON_WRITE, BDF_U32, wn, wn * 16);
+            c->launches += kScanSumsLaunches - 1;
+            CK(launch_scan_sums(lens, wn, sums, c->s_compute));
+        }
+        {
+            LaunchTimer t(c, BDF_K_JSON_WRITE, -1, 1, 0);
+            CK(launch_jsonw_cut(a, w0, wn, lens, kJsonwText, kJsonwMaxCuts, d_cuts, c->s_compute));
+        }
+        CK(cudaMemcpyAsync(h_cuts, d_cuts, cuts_n * sizeof(long long), cudaMemcpyDeviceToHost, c->s_compute));
+        CK(cudaStreamSynchronize(c->s_compute));
+        const int64_t nb = h_cuts[0];
+        for (int64_t q = 0; q < nb; q++) {
+            const long long* ce = h_cuts + 1 + q * cut_stride;
+            const long long* cn = ce + cut_stride;
+            const int64_t r0 = w0 + ce[0], r1 = w0 + cn[0];
+            const unsigned long long base = (unsigned long long)ce[1];
+            const size_t bytes = (size_t)(cn[1] - ce[1]);
+            const int b = (int)(k & 1);
+            char* out = text[b].get();
+            if (bytes > kJsonwText) {   // one row longer than a text buffer
+                TRY(put_prev());
+                // An earlier long row's text may still be crossing out of text_big.  Every copy queued so far precedes block k-1's
+                // `left` event on the copy stream (its put is done: just above, or at the start of this window), so the emit waits on it.
+                if (k >= 1) CK(cudaStreamWaitEvent(c->s_compute, ev_d2h[prev.b], 0));
+                if (bytes > big_cap) {
+                    CK(cudaStreamSynchronize(c->s_d2h));   // the last long row's text has left its buffer
+                    text_big.reset(new Scratch<char>());
+                    e = text_big->alloc(c, bytes);
+                    if (e != cudaSuccess) return fail_cuda(e, "JSON write: the text of a long row");
+                    big_cap = bytes;
+                }
+                out = text_big->get();
+            }
+            if (k >= 2) CK(cudaStreamWaitEvent(c->s_compute, ev_d2h[b], 0));
+            {
+                LaunchTimer t(c, BDF_K_JSON_WRITE, BDF_U8, r1 - r0, (int64_t)bytes);
+                CK(launch_jsonw_emit(a, w0, r0, r1, lens, base, elens, lpos.get(), kJsonwMaxRows, out, c->s_compute));
+            }
+            for (int L = 0; L < n_lists; L++) {
+                if (cn[2 + L] <= ce[2 + L]) continue;
+                LaunchTimer t(c, BDF_K_JSON_WRITE, BDF_U8, cn[2 + L] - ce[2 + L], 0);
+                CK(launch_jsonw_elem_emit(a, L, ce[2 + L], cn[2 + L], w0, elens, lpos.get(), kJsonwMaxRows, base, out, c->s_compute));
+            }
+            CK(cudaEventRecord(ev_emit[b], c->s_compute));
+            TRY(put_prev());   // block k-1 crosses while block k is formatted
+            prev = Block{out, bytes, b};
+            have_prev = true;
+            k++;
+        }
+        w0 += h_cuts[1 + nb * cut_stride];
+    }
+    TRY(put_prev());
+    TRY(sink.flush());
+    return finish();
+}
+
 int bdf_csv_write(bdf_ctx* c, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols,
                   const bdf_csv_write_options* options) {
     if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the CSV writer writes from one GPU: use a one-GPU context (bdf_init) for it");
     ENTER(c);
     return csv_write(c, path, n_cols, names, cols, options);
+}
+
+int bdf_json_write(bdf_ctx* c, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols, const bdf_temporal_type* types,
+                   const bdf_list* const* lists, const bdf_json_write_options* options) {
+    if (c && c->fleet) return fail(BDF_UNSUPPORTED, "the JSON writer writes from one GPU: use a one-GPU context (bdf_init) for it");
+    ENTER(c);
+    return json_write(c, path, n_cols, names, cols, types, lists, options);
 }
 
 int bdf_parquet_write(bdf_ctx* c, const char* path, int32_t n_cols, const char* const* names, const bdf_col* const* cols, const bdf_temporal_type* types,

@@ -38,7 +38,7 @@ from . import _native as N
 from .arrays import F32, F64, I8, I64, NP_DTYPES, U8, U32, U64, PrimitiveArray, is_float
 from .functions import Column, ListColumn, _expr_nodes, eval_expr, sort_indices, top_k_indices, window as _window
 from .csv_reader import CsvFile, write_csv
-from .json_reader import JsonFile
+from .json_reader import JsonFile, write_json
 from .parquet_reader import ParquetFile, write_parquet
 from .ipc import BOOL, IpcFile, write_ipc
 
@@ -595,6 +595,12 @@ class DeviceFrame:
             if getattr(c, "temporal", None) is not None:
                 raise N.UnsupportedType(f"column {n!r} is {c.temporal!r}: temporal text is not written by the CSV writer")
         write_csv(path, self.columns, has_header=has_header, delimiter=delimiter)
+
+    def to_json(self, path: str, explicit_nulls: bool = False) -> None:
+        """DataFrame::to_json as line-delimited JSON: one object per row, formatted on the device and streamed to the file
+        (write_json).  Every column a device frame holds is written: numeric and Boolean values, temporal columns as date / time /
+        timestamp strings, list columns as arrays.  NULL members are left out unless ``explicit_nulls``."""
+        write_json(path, self.columns, explicit_nulls=explicit_nulls)
 
     def to_parquet(self, path: str, compression: str = "none", dictionary: bool = True, row_group_rows: int = 0) -> None:
         """DataFrame::to_parquet: the frame's pages are encoded (and compressed) on the device and streamed to the file

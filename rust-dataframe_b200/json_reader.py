@@ -8,11 +8,15 @@ the keys, infers the schema and converts the requested columns on the device (cs
         f.schema                             # [(name, dtype or -1, nullable)]; List<T> columns are LIST_BASE + T
         cols = f.read(["id", "price"])       # -> {name: Column}, one chunk per RecordBatch
         tags = f.read_list("tags")           # -> ListColumn
+
+and writes device columns back as line-delimited JSON, formatted on the device (csrc/k_json_write.cu):
+
+    write_json(path, {"id": ids, "when": stamps, "tags": tags}, explicit_nulls=False)
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional, Sequence, Tuple, Union
+from typing import Dict, Mapping, Optional, Sequence, Tuple, Union
 
 from . import _native as N
 
@@ -98,3 +102,24 @@ class JsonFile:
         h = C.c_void_p()
         N.raise_for_status(N.lib().bdf_json_read_list(self.ctx.handle, self.handle, self.column_index(column), C.byref(h)))
         return ListColumn(self.ctx, h)
+
+
+def write_json(path: str, columns: Mapping[str, "object"], explicit_nulls: bool = False) -> None:
+    """Device Columns and ListColumns (chunk b of every column has the same row count) -> a line-delimited JSON file, one object per
+    row, formatted on the device (bdf_json_write; the rules are in include/b200df.h).  Columns tagged with a TemporalType
+    (``Column.temporal``) are written as date / time / timestamp strings.  A NULL member is left out unless ``explicit_nulls``; NaN and
+    infinities are written as null."""
+    from .functions import ListColumn
+
+    names = list(columns)
+    k = len(names)
+    ctx = columns[names[0]].ctx if k else N.default_context()
+    cnames = (C.c_char_p * max(k, 1))(*[s.encode() for s in names])
+    is_list = [isinstance(columns[s], ListColumn) for s in names]
+    handles = (C.c_void_p * max(k, 1))(*[None if l else columns[s].handle for s, l in zip(names, is_list)])
+    lists = (C.c_void_p * max(k, 1))(*[columns[s].handle if l else None for s, l in zip(names, is_list)])
+    tags = [None if l else getattr(columns[s], "temporal", None) for s, l in zip(names, is_list)]
+    types = (N.TemporalTypeC * max(k, 1))(*[N.TemporalTypeC(t.kind, t.unit, t.tz.encode() if t.tz is not None else None) if t is not None
+                                             else N.TemporalTypeC(0, 0, None) for t in tags])
+    opts = N.JsonWriteOptions(1 if explicit_nulls else 0)
+    N.raise_for_status(N.lib().bdf_json_write(ctx.handle, str(path).encode(), k, cnames, handles, types, lists, C.byref(opts)))
