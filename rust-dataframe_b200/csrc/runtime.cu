@@ -29,6 +29,7 @@
 #include <unistd.h>
 #include <string>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/b200df.h"
@@ -6410,13 +6411,13 @@ static int json_open(bdf_ctx* c, const char* path, const bdf_json_options* o, in
     std::vector<std::string> names;
     std::vector<Name> seen;
     std::vector<int> name_of(kJsonKeyCap, -1);
+    std::unordered_map<std::string, size_t> index;   // up to kJsonKeyCap names: no linear search
     for (unsigned s = 0; s < kJsonKeyCap; s++) {
         const JsonKeyH& k = keys[s];
         if (k.hash == ~0ull) continue;
         const uint8_t* p = f->map + f->off + k.kstart;
         const std::string name = memchr(p, '\\', k.klen) ? json_unescape(p, p + k.klen) : std::string((const char*)p, k.klen);
-        size_t j = 0;
-        while (j < names.size() && names[j] != name) j++;   // names are few
+        const size_t j = index.emplace(name, names.size()).first->second;
         if (j == names.size()) { names.push_back(name); seen.push_back(Name{k.first, k.rec}); }
         else if (k.first < seen[j].first) seen[j] = Name{k.first, k.rec};
         name_of[s] = (int)j;

@@ -62,6 +62,27 @@ def records(data: bytes, delim: int = ord(",")) -> List[List[bytes]]:
     return out
 
 
+def states(data: bytes, delim: int = ord(","), start: int = SR) -> List[int]:
+    """The DFA state before every byte of data (records()' transitions, from `start`), and after the last one: len(data) + 1 entries."""
+    out, st = [start], start
+    for b in data:
+        t = b in (13, 10)
+        if st == IQ:
+            st = QQ if b == 34 else IQ
+        elif st == QQ and b == 34:
+            st = IQ
+        elif b == delim:
+            st = SF
+        elif t:
+            st = SR
+        elif b == 34 and st in (SR, SF):
+            st = IQ
+        else:
+            st = IF
+        out.append(st)
+    return out
+
+
 _BOOL = re.compile(rb"(?i)^(true)$|^(false)$")
 _DEC = re.compile(rb"^-?(\d+\.\d+)$", re.ASCII)
 _INT = re.compile(rb"^-?(\d+)$", re.ASCII)

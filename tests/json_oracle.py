@@ -151,13 +151,12 @@ def read(data: bytes, schema: Optional[Sequence[Tuple[str, int]]] = None, max_re
     if not recs:
         raise Panic("no records")
     rows = []
-    order = []   # keys in the order first seen
+    order = {}   # keys in the order first seen
     for r in recs:
         d = {}
         for k, v in r:
             d[k] = v   # the last value wins
-            if k not in order:
-                order.append(k)
+            order.setdefault(k)
         rows.append(d)
     if schema is not None:
         names = [n for n, _ in schema]
